@@ -51,6 +51,9 @@ def parse_args():
     ap.add_argument("--kernel-times", action="store_true", help="also print per-kernel device times (stderr)")
     ap.add_argument("--trace", default="", help="after the timed runs: CUPTI timeline (torch.profiler) of a few graph-replayed "
                                                 "steps -> <path>.json (chrome trace) + <path>.txt (one step, kernel start/end)")
+    ap.add_argument("--dump-outputs", default="", metavar="DIR",
+                    help="after the timed steps: write what the last timed step returned (loss and accuracy, every updated "
+                         "parameter tensor) as DIR/<name>.npy, float32, at most 64 MB in all")
     return ap.parse_args()
 
 
@@ -102,9 +105,9 @@ class ClockSampler:
 
 # ----------------------------------------------------------------------------------------------------
 def run_reference(args):
-    # The reference is Python-2 / TensorFlow<=1.0 / Twisted code with no setup.py; `pip install --no-index
-    # --target baseline/_ref /root/reference` fails ("Neither 'setup.py' nor 'pyproject.toml' found") and
-    # neither tensorflow nor twisted exists offline (DESIGN.md "Reference arm").
+    # The reference is Python-2 / TensorFlow<=1.0 / Twisted code with no setup.py; pip cannot install it
+    # ("Neither 'setup.py' nor 'pyproject.toml' found") and neither tensorflow nor twisted exists offline
+    # (DESIGN.md "Reference arm").
     print(json.dumps({"impl": "reference",
                       "unavailable": "reference is py2/TF<=1.0/Twisted with no setup.py; pip --no-index install fails "
                                      "and tensorflow/twisted are absent offline"}))
@@ -143,6 +146,34 @@ def write_timeline(path: str, step_fn, barrier, rank: int, steps: int = 6) -> No
             f.write("# no step boundary found; %d device events\n" % len(ev))
 
 
+DUMP_LIMIT_BYTES = 64 << 20
+
+
+def dump_outputs(out_dir: str, engine) -> None:
+    """The last timed step's results as .npy files: ``loss_acc`` (the step's (loss, accuracy)) and one file per model
+    parameter after the step's SGD update.  A tensor that would push the total past 64 MB is replaced by a fixed sample
+    (``<name>.sample.npy``, elements at the seeded indices of ``<name>.sample_index.npy``, float64)."""
+    import numpy as np
+    import torch
+    torch.cuda.synchronize()
+    os.makedirs(out_dir, exist_ok=True)
+    loss, acc = engine.loss_acc()
+    np.save(os.path.join(out_dir, "loss_acc.npy"), np.array([loss, acc], dtype=np.float32))
+    views = engine.spec.views(engine.params)
+    budget = DUMP_LIMIT_BYTES - 4096
+    per_tensor = budget // max(1, len(views))
+    for name, t in views.items():
+        fname = "".join(c if c.isalnum() or c in "-_" else "_" for c in name)
+        a = t.detach().float().cpu().numpy()
+        if a.nbytes <= per_tensor:
+            np.save(os.path.join(out_dir, fname + ".npy"), a)
+        else:
+            n = per_tensor // 12                     # float32 value + float64 index per sampled element
+            idx = np.sort(np.random.default_rng(12345).choice(a.size, size=n, replace=False))
+            np.save(os.path.join(out_dir, fname + ".sample.npy"), a.reshape(-1)[idx])
+            np.save(os.path.join(out_dir, fname + ".sample_index.npy"), idx.astype(np.float64))
+
+
 def maybe_self_spawn(args) -> bool:
     """`python bench.py --gpus N` without torchrun: spawn the N ranks ourselves."""
     if args.gpus > 1 and "RANK" not in os.environ:
@@ -154,6 +185,10 @@ def maybe_self_spawn(args) -> bool:
 
 def main():
     args = parse_args()
+    if args.dump_outputs and args.impl != "ours":
+        print("bench: --dump-outputs writes the results of this engine's timed path; it is not available with --impl %s"
+              % args.impl, file=sys.stderr)
+        return 2
     if args.impl == "reference":
         return run_reference(args)
     maybe_self_spawn(args)
@@ -192,7 +227,7 @@ def main():
     engine.attach_optimizer(opt)
 
     # ---- synthetic data ------------------------------------------------------------------------------------
-    # host pool (pinned) for the e2e path; device pool > L2 (126 MB) for the device-timed path
+    # host pool (pinned) for the e2e path; device pool > L2 (50 MB) for the device-timed path
     # every batch is one packed buffer (images then labels, the device slot's layout): a step's input is ONE copy
     g = torch.Generator().manual_seed(1234 + rank)
     pool_n = int(160e6 / (B * 784 * 4)) + 1
@@ -202,8 +237,9 @@ def main():
     d_pool = torch.empty(pool_n, h_pool[0].numel(), dtype=torch.uint8, device=ctx.device)
     for i in range(pool_n):
         d_pool[i].copy_(h_pool[i % n_host])
+    gd = torch.Generator(device=ctx.device).manual_seed(4321 + rank)
     d_pool[:, :B * 784 * 4].view(torch.float32).view(pool_n, -1).add_(   # distinct images per pool entry
-        (torch.rand(pool_n, 1, device=ctx.device) - 0.5) * 0.1)
+        (torch.rand(pool_n, 1, device=ctx.device, generator=gd) - 0.5) * 0.1)
 
     def barrier():
         torch.cuda.synchronize()
@@ -335,6 +371,8 @@ def main():
     ms2_total = float(ms2.item())
     backend.check_error()
     info = engine.step_info()
+    if args.dump_outputs and rank == 0:
+        dump_outputs(args.dump_outputs, engine)
     if args.kernel_times:
         kt = engine.time_kernels(20)
         if rank == 0:
@@ -363,7 +401,7 @@ def main():
                                       % (n, k, n, "NVLS multimem.ld_reduce/st" if backend.nvls_active else
                                          ("P2P ld/st" if n > 1 else "single replica")),
                        "optimizer": "SGD, staircase exp-decay LR evaluated on device",
-                       "l2": "inputs rotate through a %d MB device pool (> 126 MB L2)" % int(d_pool.numel() / 1e6),
+                       "l2": "inputs rotate through a %d MB device pool (> 50 MB L2)" % int(d_pool.numel() / 1e6),
                        "cuda_graph": not args.no_graph},
             "clocks": {"sm_mhz": clocks["sm_mhz"], "sm_max_mhz": clocks["sm_max_mhz"], "reasons": clocks["reasons"],
                        "samples": clocks["samples"]},

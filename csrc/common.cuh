@@ -1,9 +1,9 @@
-// Shared device-side building blocks for the sm_100a kernels: mbarrier, TMA,
-// tcgen05/TMEM wrappers, UMMA descriptor encoders, small math helpers.
+// Shared device-side building blocks for the sm_90a kernels: mbarrier, TMA, ldmatrix,
+// wgmma wrappers, wgmma descriptor encoder, small math helpers.
 //
-// Everything here is written directly against the PTX ISA for sm_100a (no CUTLASS
-// dependency); bit layouts of the UMMA shared-memory and instruction descriptors
-// follow the PTX "tcgen05 matrix descriptor" / "instruction descriptor" tables.
+// Everything here is written directly against the PTX ISA for sm_90a (no CUTLASS
+// dependency); the bit layout of the shared-memory matrix descriptor follows the PTX
+// "wgmma matrix descriptor" table.
 #pragma once
 
 #include <cuda.h>
@@ -125,66 +125,135 @@ DMNIST_DEVICE void tma_load_4d(void* smem_dst, const CUtensorMap* m, uint64_t* b
 }
 
 // ---------------------------------------------------------------------------------
-// tcgen05 / TMEM
+// ldmatrix: 8x8 b16 tiles from shared memory into the mma / wgmma register-fragment layout
 // ---------------------------------------------------------------------------------
-template <uint32_t kCols>
-DMNIST_DEVICE void tmem_alloc(uint32_t* smem_holder) {  // one full warp, .sync.aligned
-  static_assert(kCols >= 32 && kCols <= 512 && (kCols & (kCols - 1)) == 0, "TMEM columns: power of 2 in [32,512]");
-  asm volatile("tcgen05.alloc.cta_group::1.sync.aligned.shared::cta.b32 [%0], %1;" ::"r"(smem_u32(smem_holder)),
-               "n"(kCols)
+// Lane l supplies the row address of tile l / 8 (row l % 8).  Register i of every lane holds tile i:
+// without .trans lane l gets row l / 4, elements 2 (l % 4) and 2 (l % 4) + 1; with .trans the tile is read
+// column-wise (lane l gets column l / 4, rows 2 (l % 4) and 2 (l % 4) + 1).
+DMNIST_DEVICE void ldsm_x4(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
                : "memory");
-  asm volatile("tcgen05.relinquish_alloc_permit.cta_group::1.sync.aligned;" ::: "memory");
 }
-template <uint32_t kCols>
-DMNIST_DEVICE void tmem_dealloc(uint32_t taddr) {  // same warp that allocated
-  asm volatile("tcgen05.dealloc.cta_group::1.sync.aligned.b32 %0, %1;" ::"r"(taddr), "n"(kCols) : "memory");
+DMNIST_DEVICE void ldsm_x4_trans(uint32_t addr, uint32_t (&r)[4]) {
+  asm volatile("ldmatrix.sync.aligned.m8n8.x4.trans.shared.b16 {%0, %1, %2, %3}, [%4];"
+               : "=r"(r[0]), "=r"(r[1]), "=r"(r[2]), "=r"(r[3])
+               : "r"(addr)
+               : "memory");
 }
-DMNIST_DEVICE void tc_fence_before_sync() { asm volatile("tcgen05.fence::before_thread_sync;" ::: "memory"); }
-DMNIST_DEVICE void tc_fence_after_sync() { asm volatile("tcgen05.fence::after_thread_sync;" ::: "memory"); }
 
-// D[tmem] (+)= A[smem] * B[smem], bf16 x bf16 -> fp32, single CTA.
-DMNIST_DEVICE void umma_bf16(uint32_t tmem_d, uint64_t desc_a, uint64_t desc_b, uint32_t idesc, uint32_t accumulate) {
+// ---------------------------------------------------------------------------------
+// wgmma (sm_90a warpgroup MMA): D[64 x N] (+)= A[64 x 16] * B[16 x N], bf16 in, fp32 accumulate in registers
+// ---------------------------------------------------------------------------------
+// Accumulator layout (per warp w of the warpgroup, lane l, g = l / 4, t = l % 4):
+//   d[4 j + 0], d[4 j + 1] = row 16 w + g,     columns 8 j + 2 t, 8 j + 2 t + 1
+//   d[4 j + 2], d[4 j + 3] = row 16 w + g + 8, same columns
+// A from registers uses the m16n8k16 A-fragment layout for the warp's 16 rows (what ldsm_x4 delivers for
+// tiles {rows 0-7, k 0-7}, {rows 8-15, k 0-7}, {rows 0-7, k 8-15}, {rows 8-15, k 8-15}).
+DMNIST_DEVICE void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
+DMNIST_DEVICE void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
+template <int N>
+DMNIST_DEVICE void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
+// keeps the compiler from moving accumulator accesses across the asynchronous MMAs
+template <int R>
+DMNIST_DEVICE void fence_regs(float (&d)[R]) {
+#pragma unroll
+  for (int i = 0; i < R; ++i) asm volatile("" : "+f"(d[i])::"memory");
+}
+
+// A and B from shared-memory descriptors; TA / TB = 1: operand is MN-major.
+template <int TA, int TB>
+DMNIST_DEVICE void wgmma_m64n64_ss(float (&d)[32], uint64_t desc_a, uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
       "{\n\t.reg .pred p;\n\t"
-      "setp.ne.b32 p, %4, 0;\n\t"
-      "tcgen05.mma.cta_group::1.kind::f16 [%0], %1, %2, %3, p;\n\t}\n" ::"r"(tmem_d),
-      "l"(desc_a), "l"(desc_b), "r"(idesc), "r"(accumulate)
+      "setp.ne.b32 p, %34, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, %32, %33, p, 1, 1, %35, %36;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "l"(desc_a), "l"(desc_b), "r"(accumulate), "n"(TA), "n"(TB)
       : "memory");
 }
-// Arrive on an mbarrier once all previously issued tcgen05.mma of this thread retire
-// (implies tcgen05.fence::before_thread_sync).
-DMNIST_DEVICE void umma_commit(uint64_t* bar) {
-  asm volatile("tcgen05.commit.cta_group::1.mbarrier::arrive::one.shared::cluster.b64 [%0];" ::"r"(smem_u32(bar))
-               : "memory");
-}
-
-// TMEM -> registers: 32 lanes x 32 consecutive fp32 columns; thread t of the warp gets
-// row (lane base + t), v[j] = column (col base + j).  Warp w may only touch lanes
-// 32*(w%4) .. 32*(w%4)+31.
-DMNIST_DEVICE void tmem_ld_32x32(uint32_t taddr, uint32_t (&v)[32]) {
+// A from registers, B from a shared-memory descriptor.
+template <int TB>
+DMNIST_DEVICE void wgmma_m64n64_rs(float (&d)[32], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
   asm volatile(
-      "tcgen05.ld.sync.aligned.32x32b.x32.b32 "
-      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, "
-      "%16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, [%32];"
-      : "=r"(v[0]), "=r"(v[1]), "=r"(v[2]), "=r"(v[3]), "=r"(v[4]), "=r"(v[5]), "=r"(v[6]), "=r"(v[7]),
-        "=r"(v[8]), "=r"(v[9]), "=r"(v[10]), "=r"(v[11]), "=r"(v[12]), "=r"(v[13]), "=r"(v[14]), "=r"(v[15]),
-        "=r"(v[16]), "=r"(v[17]), "=r"(v[18]), "=r"(v[19]), "=r"(v[20]), "=r"(v[21]), "=r"(v[22]), "=r"(v[23]),
-        "=r"(v[24]), "=r"(v[25]), "=r"(v[26]), "=r"(v[27]), "=r"(v[28]), "=r"(v[29]), "=r"(v[30]), "=r"(v[31])
-      : "r"(taddr)
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %37, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n64k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31}, {%32, %33, %34, %35}, %36, p, 1, 1, %38;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate), "n"(TB)
       : "memory");
 }
-DMNIST_DEVICE void tmem_ld_wait() { asm volatile("tcgen05.wait::ld.sync.aligned;" ::: "memory"); }
+template <int TB>
+DMNIST_DEVICE void wgmma_m64n32_rs(float (&d)[16], const uint32_t (&a)[4], uint64_t desc_b, uint32_t accumulate) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "setp.ne.b32 p, %21, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n32k16.f32.bf16.bf16 "
+      "{%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15}, {%16, %17, %18, %19}, %20, p, 1, 1, %22;\n\t}\n"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(desc_b), "r"(accumulate), "n"(TB)
+      : "memory");
+}
+
+// Named barrier over the first `threads` threads of the CTA (id 0 is __syncthreads).
+DMNIST_DEVICE void named_bar_sync(uint32_t id, uint32_t threads) {
+  asm volatile("bar.sync %0, %1;" ::"r"(id), "r"(threads) : "memory");
+}
 
 // ---------------------------------------------------------------------------------
-// UMMA descriptors
+// deterministic cross-CTA reductions
 // ---------------------------------------------------------------------------------
-enum : uint32_t { SWZ_NONE = 0, SWZ_128B = 2, SWZ_64B = 4, SWZ_32B = 6 };
+// Every CTA stores its partial sums to its own slot of a global workspace and then takes a ticket; the CTA that draws
+// the last ticket (returns true in all its threads) adds the slots up in slot order.  Unlike atomics into the output,
+// the summation order -- and so the result, to the bit -- does not depend on which CTA finishes first.
+// The workspaces and tickets are static per device (one set per kernel), so each of these kernels may have only ONE
+// launch in flight per device: launches on the same stream (the training step) are fine, concurrent launches of the
+// same kernel on two streams would mix their partial sums.  `threads` =
+// the CTA threads taking part (they must include thread 0), `bar_id` a named barrier reserved for them.  The last CTA
+// resets the ticket for the next launch.
+DMNIST_DEVICE bool arrive_last_cta(unsigned int* ticket, unsigned int ctas, uint32_t bar_id, uint32_t threads,
+                                   volatile unsigned int* s_flag) {
+  __threadfence();                                  // this CTA's partial is visible before its ticket
+  named_bar_sync(bar_id, threads);
+  if (threadIdx.x == 0) {
+    const unsigned int t = atomicAdd(ticket, 1u);
+    *s_flag = (t == ctas - 1) ? 1u : 0u;
+    if (t == ctas - 1) *ticket = 0u;
+  }
+  named_bar_sync(bar_id, threads);
+  const bool last = *s_flag != 0u;
+  if (last) __threadfence();                        // acquire side: the other CTAs' partials (read with __ldcg)
+  return last;
+}
 
-// Shared-memory matrix descriptor (64 bit):
+// sum_{k < n} p[k * stride] in k order, float4-wide; 16 loads in flight (L2, bypassing L1) per round.
+DMNIST_DEVICE float4 ordered_sum4(const float4* p, int n, size_t stride) {
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int k0 = 0; k0 < n; k0 += 16) {
+    float4 v[16];
+#pragma unroll
+    for (int u = 0; u < 16; ++u) v[u] = k0 + u < n ? __ldcg(p + (size_t)(k0 + u) * stride) : make_float4(0.f, 0.f, 0.f, 0.f);
+#pragma unroll
+    for (int u = 0; u < 16; ++u)
+      if (k0 + u < n) { s.x += v[u].x; s.y += v[u].y; s.z += v[u].z; s.w += v[u].w; }
+  }
+  return s;
+}
+
+// ---------------------------------------------------------------------------------
+// wgmma shared-memory matrix descriptors
+// ---------------------------------------------------------------------------------
+enum : uint32_t { SWZ_NONE = 0, SWZ_128B = 1, SWZ_64B = 2, SWZ_32B = 3 };
+
+// Shared-memory matrix descriptor (64 bit, sm_90):
 //   [0,14)  start address >> 4        [16,30) leading-dim byte offset >> 4
-//   [32,46) stride-dim byte offset >> 4   [46,48) version = 1 (Blackwell)
-//   [49,52) base offset (0: tiles are aligned to the swizzle repeat)   [61,64) swizzle mode
-// K-major operand, swizzled:   rows of <swizzle width> bytes, 8-row groups SBO apart (LBO unused).
+//   [32,46) stride-dim byte offset >> 4   [49,52) base offset (0: tiles are aligned to the swizzle repeat)
+//   [62,64) swizzle mode
+// K-major operand, swizzled:   rows of <swizzle width> bytes, 8-row groups SBO apart (LBO unused); a K step
+//                              inside the swizzle width advances the start address.
 // MN-major operand, swizzled:  k-rows of <swizzle width> bytes; 8-k groups SBO apart; successive
 //                              <swizzle width> chunks along M/N are LBO apart.
 DMNIST_DEVICE uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, uint32_t sbo_bytes, uint32_t swizzle) {
@@ -192,20 +261,11 @@ DMNIST_DEVICE uint64_t make_smem_desc(uint32_t smem_addr, uint32_t lbo_bytes, ui
   d |= (uint64_t)((smem_addr & 0x3FFFF) >> 4);
   d |= (uint64_t)((lbo_bytes >> 4) & 0x3FFF) << 16;
   d |= (uint64_t)((sbo_bytes >> 4) & 0x3FFF) << 32;
-  d |= (uint64_t)1 << 46;
-  d |= (uint64_t)(swizzle & 7) << 61;
+  d |= (uint64_t)(swizzle & 3) << 62;
   return d;
 }
 // Advance the start address of a descriptor by `bytes` (stays inside the 14-bit field:
 // shared memory is < 256 KB so no carry into the LBO field can occur).
 DMNIST_DEVICE uint64_t desc_advance(uint64_t desc, uint32_t bytes) { return desc + (uint64_t)(bytes >> 4); }
-
-// Instruction descriptor for kind::f16 with BF16 inputs and FP32 accumulation:
-//   [4,6) D format (1 = F32)  [7,10) A format (1 = BF16)  [10,13) B format (1 = BF16)
-//   [15] A major (0 = K, 1 = MN)  [16] B major  [17,23) N >> 3  [24,29) M >> 4
-__host__ __device__ constexpr uint32_t make_idesc_bf16(uint32_t M, uint32_t N, bool a_mn_major, bool b_mn_major) {
-  return (1u << 4) | (1u << 7) | (1u << 10) | ((a_mn_major ? 1u : 0u) << 15) | ((b_mn_major ? 1u : 0u) << 16) |
-         ((N >> 3) << 17) | ((M >> 4) << 24);
-}
 
 }  // namespace dm

@@ -1,46 +1,57 @@
-// conv2 (5x5 SAME, 32 -> 64 channels, 14x14 feature maps) as tcgen05 implicit GEMMs.
+// conv2 (5x5 SAME, 32 -> 64 channels, 14x14 feature maps) as wgmma implicit GEMMs.
 // reference op K5 (tf.nn.conv2d #2, src/mnist.py:119-122) = 82 % of the model FLOPs, fused with
 // K2/K3/K4 (bias, ReLU, 2x2 max-pool, src/mnist.py:123-127) in the forward epilogue.
 //
-// No im2col buffer exists anywhere: activations stay NHWC bf16 and every filter tap is one 4-D TMA
-// box (channels, 16 pixels of a row, 8 rows, 1 image) fetched at a shifted coordinate; the SAME
-// padding halo and the 14 -> 16 row/column round-up are TMA out-of-bounds zero fill.  An M tile is
-// therefore 128 pixels (8 x 16, 112 or 84 of them real) of one image; two tiles cover an image.
+// No im2col buffer exists anywhere: activations stay NHWC bf16 and a tile's whole receptive field is
+// one 4-D TMA box (channels, 12 pixels of a row, 20 rows, 1 image); the SAME padding halo and the
+// 14 -> 16 row/column round-up are TMA out-of-bounds zero fill.  An M tile is 128 pixels (16 rows x
+// 8 columns, 112 or 84 of them real) of one image; two tiles cover an image.
 //
-//   fwd    D[pixel, co]  += X[pixel + tap, ci] (K-major, 64B swizzle)  * W[tap][ci][co] (MN-major, 128B)
-//   dgrad  D[pixel, ci]  += dY[pixel - tap, co] (K-major, 128B swizzle) * W[tap][ci][co] (K-major,  128B)
-//   wgrad  D[(tap,ci), co] += X[pixel + tap, ci] (MN-major, 64B)        * dY[pixel, co]   (MN-major, 128B),
-//          K = pixels, split over CTAs, fp32 atomics into the HWIO gradient tensor.
-// The HWIO bf16 weight image (800 x 64) is loaded once per CTA and stays resident in shared memory
-// (100 KB) while the persistent CTA walks its tiles; accumulators are double-buffered in TMEM so the
-// epilogue of tile i overlaps the MMAs of tile i+1.
+//   fwd    D[pixel, co]  += X[pixel + tap, ci] (A: registers)  * W[tap][ci][co] (B: MN-major smem, 128B swizzle)
+//   dgrad  D[pixel, ci]  += dY[pixel - tap, co] (A: registers) * W[tap][ci][co] (B: K-major smem,  128B swizzle)
+//   wgrad  D[(tap,ci), co] += X[pixel + tap, ci] (A: registers, transposed) * dY[pixel, co] (B: MN-major smem),
+//          K = pixels, split over CTAs whose partial sums are added up in a fixed order (bit-reproducible).
+// The A operand of every tap is the same patch shifted by (kh, kw): a window that starts at an arbitrary
+// pixel of the swizzled patch, so each warp gathers its 16 rows with ldmatrix (addresses computed with the
+// TMA swizzle) and hands them to wgmma in registers; B always starts on a swizzle-atom boundary and is
+// read by wgmma straight from shared memory.  The HWIO bf16 weight image (800 x 64) is loaded once per
+// CTA and stays resident in shared memory (100 KB) while the persistent CTA walks its tiles.
+//
+// Threads: warps 0-7 = two consumer warpgroups (rows 0-63 / 64-127 of a tile), warp 8 = TMA producer.
 #include "common.cuh"
 #include "host_utils.h"
 
 namespace dm {
 
-constexpr int CV_THREADS = 192;
+constexpr int CV_CONSUMERS = 256;
+constexpr int CV_THREADS = CV_CONSUMERS + 32;
 constexpr int W_BYTES = 800 * 64 * 2;   // 102400
+
+// ldmatrix row address inside a patch of `row_bytes`-wide pixels written by TMA with a swizzle of the same width
+// (64 B: 16-byte chunk bits [4,5] ^= address bits [7,8]; 128 B: bits [4,6] ^= bits [7,9]); patches start on a
+// 1024-byte boundary.
+template <int ROW_BYTES>
+DMNIST_DEVICE uint32_t patch_addr(uint32_t base, int pixel, int chunk) {
+  if (ROW_BYTES == 64) return base + pixel * 64 + ((chunk ^ ((pixel >> 1) & 3)) << 4);
+  return base + pixel * 128 + ((chunk ^ (pixel & 7)) << 4);
+}
 
 // ------------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------------
 constexpr int FW_STAGES = 4;
 constexpr int FW_A_BYTES = 20 * 12 * 32 * 2;   // ONE patch per tile: 20 rows x 12 pixels x 32 ch = 15 KB, all 25 taps inside
+constexpr int FW_ACC_LD = 64 + 4;              // fp32 accumulator staging row (padded)
 struct FwSmem {
   static constexpr int A_OFF = W_BYTES;
-  static constexpr int BAR_OFF = A_OFF + FW_STAGES * FW_A_BYTES;
-  static constexpr int SCR_OFF = BAR_OFF + 512;                 // epilogue transpose scratch: 4 warps x 32 rows x 128 B
-  static constexpr int BIAS_OFF = SCR_OFF + 4 * 4096;           // 64 floats
-  static constexpr int TOTAL = BIAS_OFF + 256 + 1024;
+  static constexpr int ACC_OFF = A_OFF + FW_STAGES * FW_A_BYTES;
+  static constexpr int BIAS_OFF = ACC_OFF + 128 * FW_ACC_LD * 4;   // 64 floats
+  static constexpr int BAR_OFF = BIAS_OFF + 256;
+  static constexpr int TOTAL = BAR_OFF + 256 + 1024;
 };
 
-// EPI = 1: the 2x2 max-pool is an in-thread max.  Each epilogue warp transposes its 32 pixels x 32 channels through a
-//   swizzled 4 KB shared-memory scratch so that a lane ends up with ALL FOUR window positions of the 8 channels it stores
-//   (8 STS.128 + 8 LDS.128 per chunk) -- ~200 instructions per 32-channel chunk.
-// EPI = 0: first version, 2 warp shuffles + selects per value (~560 instructions per chunk; with one warp per scheduler
-//   the epilogue, not the MMAs, set the kernel's pace: 1.8 us vs 1.25 us per tile).
-template <int EPI>
+// The pool epilogue stages the 128 x 64 accumulator tile in shared memory; thread = (pooled pixel, 8 channels) then
+// reads the four window positions of its channels and stores 16 B of activations and 8 B of pooling codes.
 __global__ void __launch_bounds__(CV_THREADS, 1)
 conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,32], box (32,12,20,1), 64B swizzle
                  const __grid_constant__ CUtensorMap tmW,   // W [800][64], box (64,200), 128B swizzle
@@ -52,31 +63,24 @@ conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + FwSmem::BAR_OFF);
   uint64_t* a_empty = a_full + FW_STAGES;
-  uint64_t* acc_full = a_empty + FW_STAGES;   // [2]
-  uint64_t* acc_empty = acc_full + 2;         // [2]
-  uint64_t* w_full = acc_empty + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(w_full + 1);
+  uint64_t* w_full = a_empty + FW_STAGES;
   float* s_bias = reinterpret_cast<float*>(smem + FwSmem::BIAS_OFF);
+  float* s_acc = reinterpret_cast<float*>(smem + FwSmem::ACC_OFF);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmW);
-    for (int s = 0; s < FW_STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 4); }
+    for (int s = 0; s < FW_STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], CV_CONSUMERS / 32); }
     mbar_init(w_full, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<128>(tmem_holder);
-  if (warp == 2) { s_bias[lane] = __ldg(bias + lane); s_bias[32 + lane] = __ldg(bias + 32 + lane); }
-  tc_fence_before_sync();
+  if (threadIdx.x < 64) s_bias[threadIdx.x] = __ldg(bias + threadIdx.x);
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_holder;
   pdl_wait();
   // (no early launch_dependents: resident-but-blocked CTAs of the next kernel steal SM resources from this one)
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(w_full, W_BYTES);
       for (int i = 0; i < 4; ++i) tma_load_2d(smem + i * 25600, &tmW, w_full, 0, 200 * i);
@@ -91,153 +95,90 @@ conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,
         tma_load_4d(smem + FwSmem::A_OFF + s * FW_A_BYTES, &tmX, &a_full[s], 0, w0 - 2, -2, img);
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc_bf16(128, 64, /*A MN*/ false, /*B MN*/ true);
-    mbar_wait(w_full, 0);
-    int it = 0, tl = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++tl) {
-      const int buf = tl & 1;
-      mbar_wait(&acc_empty[buf], ((tl >> 1) & 1) ^ 1);
-      tc_fence_after_sync();
-      {
-        const int s = it % FW_STAGES;
-        mbar_wait(&a_full[s], (it / FW_STAGES) & 1);
-        tc_fence_after_sync();
-        if (elect_one()) {
-          // output pixel (h, w) reads patch pixel (h + kh, w + kw): the window of tap (kh,kw) starts (kh*12 + kw)
-          // rows into the patch; 8-row groups (fixed h) are one patch row = 12 pixels = 768 B apart.  A descriptor
-          // may start at any row of the swizzled buffer (the hardware XORs absolute address bits:
-          // profiles/umma_row_shift_probe_r1.txt).  Descriptors = one base + compile-time offsets (>> 4).
-          const uint64_t da0 = make_smem_desc(smem_u32(smem + FwSmem::A_OFF + s * FW_A_BYTES), 16, 768, SWZ_64B);
-          const uint64_t db0 = make_smem_desc(smem_u32(smem), 8192, 1024, SWZ_128B);
-          const uint32_t tm = tmem_base + buf * 64;
+    return;
+  }
+
+  // ldmatrix rows of this lane: tile row r = h * 8 + w (tiles 0/1 of x4: rows +0 / +8, tiles 2/3: channel chunk + 1)
+  const int r = 16 * warp + (lane & 7) + ((lane >> 3) & 1) * 8;
+  const int hr = r >> 3, wr = r & 7, kc = lane >> 4;
+  // W (MN-major, 128B swizzle): k-row = tap * 32 + ci (128 B = 64 co), 8-row groups 1024 B apart; a tap is 4096 B,
+  // a K step of 16 ci 2048 B
+  const uint64_t db0 = make_smem_desc(smem_u32(smem), 8192, 1024, SWZ_128B);
+  mbar_wait(w_full, 0);
+  float acc[32];
 #pragma unroll
-          for (int tap = 0; tap < 25; ++tap) {
+  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+  int it = 0;
+  for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
+    const int img = t >> 1, w0 = (t & 1) * 8;
+    const int s = it % FW_STAGES;
+    mbar_wait(&a_full[s], (it / FW_STAGES) & 1);
+    const uint32_t patch = smem_u32(smem + FwSmem::A_OFF + s * FW_A_BYTES);
+    fence_regs(acc);
 #pragma unroll
-            for (int k = 0; k < 2; ++k) {
-              const uint64_t da = da0 + (uint64_t)((((tap / 5) * 12 + (tap % 5)) * 64 + 32 * k) >> 4);
-              const uint64_t db = db0 + (uint64_t)((tap * 4096 + 2048 * k) >> 4);     // 16 ci rows per step
-              umma_bf16(tm, da, db, idesc, (tap | k) != 0);
-            }
-          }
-          umma_commit(&a_empty[s]);
-          umma_commit(&acc_full[buf]);
-        }
-        __syncwarp();
-        ++it;
+    for (int tap = 0; tap < 25; ++tap) {
+      // output pixel (h, w) reads patch pixel (h + kh, w + kw)
+      const int pix = (hr + tap / 5) * 12 + wr + tap % 5;
+      uint32_t a0[4], a1[4];
+      ldsm_x4(patch_addr<64>(patch, pix, kc), a0);
+      ldsm_x4(patch_addr<64>(patch, pix, 2 + kc), a1);
+      wgmma_fence();
+      wgmma_m64n64_rs<1>(acc, a0, desc_advance(db0, tap * 4096), tap != 0);
+      wgmma_m64n64_rs<1>(acc, a1, desc_advance(db0, tap * 4096 + 2048), 1);
+    }
+    wgmma_commit();
+    wgmma_wait<0>();
+    fence_regs(acc);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&a_empty[s]);
+
+    named_bar_sync(1, CV_CONSUMERS);               // the previous tile's epilogue has read the staging tile
+    {
+      const int r0 = 16 * warp + (lane >> 2);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int col = 8 * j + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(s_acc + r0 * FW_ACC_LD + col) = make_float2(acc[4 * j], acc[4 * j + 1]);
+        *reinterpret_cast<float2*>(s_acc + (r0 + 8) * FW_ACC_LD + col) = make_float2(acc[4 * j + 2], acc[4 * j + 3]);
       }
     }
-  } else {
-    const int q = warp & 3;
-    int tl = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++tl) {
-      const int buf = tl & 1;
-      const int img = t >> 1, w0 = (t & 1) * 8;
-      mbar_wait(&acc_full[buf], (tl >> 1) & 1);
-      tc_fence_after_sync();
-      // accumulator row = h*8 + w: this warp holds rows h = 4q .. 4q+3; lane = (h & 3) * 8 + w
-      const int w = w0 + (lane & 7), h = 4 * q + (lane >> 3);
-      const int ph = h >> 1, pw = w >> 1;
-      const bool valid = (h < 14) && (w < 14);
-      const int qp = (((lane >> 3) & 1) << 1) | (lane & 1);   // position inside the 2x2 pooling window
-#pragma unroll 1
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * 64 + c * 32, v);
-        tmem_ld_wait();
-        if (EPI == 1) {
-          uint8_t* scr = smem + FwSmem::SCR_OFF + q * 4096;
-          __syncwarp();                                   // previous chunk's reads are done
+    named_bar_sync(1, CV_CONSUMERS);
+    {
+      // 32 pooled pixels (8 x 4) x 8 groups of 8 channels
+      const int pooled = threadIdx.x >> 3, cg = threadIdx.x & 7;
+      const int ph = pooled >> 2, pwl = pooled & 3;
+      const int pw = (w0 >> 1) + pwl;
+      if (ph < 7 && pw < 7) {
+        float val[4][8];
 #pragma unroll
-          for (int k = 0; k < 8; ++k)                     // row = lane (pixel), 16-byte chunk k at k ^ (lane & 7)
-            *reinterpret_cast<uint4*>(scr + lane * 128 + ((k ^ (lane & 7)) << 4)) = make_uint4(v[4 * k], v[4 * k + 1], v[4 * k + 2], v[4 * k + 3]);
-          __syncwarp();
-          const int l0 = lane & ~9;                       // lane of window position 0 (dy = 0, dx = 0)
-          float val[4][8];
-#pragma unroll
-          for (int p = 0; p < 4; ++p) {
-            const int rp = l0 + (p & 1) + 8 * (p >> 1);
-#pragma unroll
-            for (int e = 0; e < 2; ++e) {
-              const float4 t = *reinterpret_cast<const float4*>(scr + rp * 128 + (((2 * qp + e) ^ (rp & 7)) << 4));
-              val[p][4 * e] = t.x; val[p][4 * e + 1] = t.y; val[p][4 * e + 2] = t.z; val[p][4 * e + 3] = t.w;
-            }
-          }
-          if (valid) {
-            uint32_t pk[4];
-            uint32_t cd[2] = {0u, 0u};
-#pragma unroll
-            for (int jj = 0; jj < 8; ++jj) {
-              float m = val[0][jj];
-              uint32_t idx = 0;
-#pragma unroll
-              for (int p = 1; p < 4; ++p)
-                if (val[p][jj] > m) { m = val[p][jj]; idx = p; }
-              m += s_bias[c * 32 + qp * 8 + jj];
-              const bool active = m > 0.f;
-              cd[jj >> 2] |= (idx | (active ? 4u : 0u)) << ((jj & 3) * 8);
-              const float o = active ? m : 0.f;
-              if (jj & 1) pk[jj >> 1] = pack_bf16x2(__uint_as_float(pk[jj >> 1]), o);
-              else pk[jj >> 1] = __float_as_uint(o);
-            }
-            const size_t off = (((size_t)img * 7 + ph) * 7 + pw) * 64 + c * 32 + qp * 8;
-            *reinterpret_cast<uint4*>(out + off) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-            *reinterpret_cast<uint2*>(code + off) = make_uint2(cd[0], cd[1]);
-          }
-          continue;
+        for (int p = 0; p < 4; ++p) {                // window position p = dy * 2 + dx
+          const float* src = s_acc + ((2 * ph + (p >> 1)) * 8 + 2 * pwl + (p & 1)) * FW_ACC_LD + cg * 8;
+          const float4 lo = *reinterpret_cast<const float4*>(src), hi = *reinterpret_cast<const float4*>(src + 4);
+          val[p][0] = lo.x; val[p][1] = lo.y; val[p][2] = lo.z; val[p][3] = lo.w;
+          val[p][4] = hi.x; val[p][5] = hi.y; val[p][6] = hi.z; val[p][7] = hi.w;
         }
-        uint32_t bits0 = 0, bits1 = 0;
+        uint32_t pk[4];
+        uint32_t cd[2] = {0u, 0u};
 #pragma unroll
-        for (int j = 0; j < 32; ++j) {
-          const float a = __uint_as_float(v[j]);
-          const float b = __shfl_xor_sync(0xffffffffu, a, 1);
-          const float odd = (lane & 1) ? a : b, even = (lane & 1) ? b : a;
-          bits0 |= (odd > even ? 1u : 0u) << j;           // argmax column inside my row pair
-          const float m1 = fmaxf(a, b);
-          const float o = __shfl_xor_sync(0xffffffffu, m1, 8);
-          const float bot = (lane & 8) ? m1 : o, top = (lane & 8) ? o : m1;
-          bits1 |= (bot > top ? 1u : 0u) << j;            // argmax row
-          v[j] = __float_as_uint(fmaxf(m1, o));
+        for (int jj = 0; jj < 8; ++jj) {
+          float m = val[0][jj];
+          uint32_t idx = 0;
+#pragma unroll
+          for (int p = 1; p < 4; ++p)
+            if (val[p][jj] > m) { m = val[p][jj]; idx = p; }
+          m += s_bias[cg * 8 + jj];
+          const bool active = m > 0.f;
+          cd[jj >> 2] |= (idx | (active ? 4u : 0u)) << ((jj & 3) * 8);
+          const float o = active ? m : 0.f;
+          if (jj & 1) pk[jj >> 1] = pack_bf16x2(__uint_as_float(pk[jj >> 1]), o);
+          else pk[jj >> 1] = __float_as_uint(o);
         }
-        const uint32_t other = __shfl_xor_sync(0xffffffffu, bits0, 8);
-        const uint32_t bits_top = (lane & 8) ? other : bits0, bits_bot = (lane & 8) ? bits0 : other;
-        if (valid) {
-          // every lane of the 2x2 window now holds the pooled values of all 32 channels; each writes 8
-          uint32_t pk[4];
-          uint32_t cd[2] = {0u, 0u};
-#pragma unroll
-          for (int jj = 0; jj < 8; ++jj) {
-            // select channel (qp*8 + jj) with compile-time register indices
-            float m = 0.f;
-            uint32_t i0t = 0, i0b = 0, i1 = 0;
-#pragma unroll
-            for (int s = 0; s < 4; ++s)
-              if (qp == s) {
-                m = __uint_as_float(v[s * 8 + jj]);
-                i0t = (bits_top >> (s * 8 + jj)) & 1u;
-                i0b = (bits_bot >> (s * 8 + jj)) & 1u;
-                i1 = (bits1 >> (s * 8 + jj)) & 1u;
-              }
-            m += bias[c * 32 + qp * 8 + jj];
-            const bool active = m > 0.f;
-            const uint32_t idx = i1 ? (2u | i0b) : i0t;
-            cd[jj >> 2] |= (idx | (active ? 4u : 0u)) << ((jj & 3) * 8);
-            const float o = active ? m : 0.f;
-            if (jj & 1) pk[jj >> 1] = pack_bf16x2(__uint_as_float(pk[jj >> 1]), o);
-            else pk[jj >> 1] = __float_as_uint(o);
-          }
-          const size_t off = (((size_t)img * 7 + ph) * 7 + pw) * 64 + c * 32 + qp * 8;
-          *reinterpret_cast<uint4*>(out + off) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
-          *reinterpret_cast<uint2*>(code + off) = make_uint2(cd[0], cd[1]);
-        }
+        const size_t off = (((size_t)img * 7 + ph) * 7 + pw) * 64 + cg * 8;
+        *reinterpret_cast<uint4*>(out + off) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
+        *reinterpret_cast<uint2*>(code + off) = make_uint2(cd[0], cd[1]);
       }
-      tc_fence_before_sync();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<128>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -251,11 +192,7 @@ struct DgSmem {
   static constexpr int TOTAL = BAR_OFF + 512 + 1024;
 };
 
-// Register cap: the register file is per scheduler (4 x 16 K).  At 230 registers/thread the two schedulers that hold two
-// of this CTA's six warps had 1.5 K registers left, so no other kernel's CTA (which needs a warp on every scheduler) could
-// share the SM: fc2_wgrad and the early aggregation kernel only started as these CTAs exited (profiles/bench_r1_call30_1gpu.txt,
-// profiles/coresidency_probe_r1.txt).  128 registers leave 8 K per scheduler.
-__global__ void __maxnreg__(128)
+__global__ void __launch_bounds__(CV_THREADS, 1)
 conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,14,64], box (64,12,20,1), 128B swizzle
                    const __grid_constant__ CUtensorMap tmW,
                    __nv_bfloat16* __restrict__ dx,            // [B,14,14,32]
@@ -264,32 +201,24 @@ conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,1
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + DgSmem::BAR_OFF);
   uint64_t* a_empty = a_full + DG_STAGES;
-  uint64_t* acc_full = a_empty + DG_STAGES;
-  uint64_t* acc_empty = acc_full + 2;
-  uint64_t* w_full = acc_empty + 2;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(w_full + 1);
+  uint64_t* w_full = a_empty + DG_STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmDY);
     tma_prefetch_desc(&tmW);
-    for (int s = 0; s < DG_STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], 1); }
-    for (int b = 0; b < 2; ++b) { mbar_init(&acc_full[b], 1); mbar_init(&acc_empty[b], 4); }
+    for (int s = 0; s < DG_STAGES; ++s) { mbar_init(&a_full[s], 1); mbar_init(&a_empty[s], CV_CONSUMERS / 32); }
     mbar_init(w_full, 1);
     fence_mbar_init();
   }
   const bool dbg_on = dbg != nullptr && blockIdx.x == 0;
   if (dbg_on && threadIdx.x == 0) dbg[0] = globaltimer_ns();
-  if (warp == 1) tmem_alloc<64>(tmem_holder);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_holder;
   pdl_wait();
   // (no early launch_dependents: resident-but-blocked CTAs of the next kernel steal SM resources from this one)
   if (dbg_on && threadIdx.x == 0) dbg[1] = globaltimer_ns();
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       mbar_expect_tx(w_full, W_BYTES);
       for (int i = 0; i < 4; ++i) tma_load_2d(smem + i * 25600, &tmW, w_full, 0, 200 * i);
@@ -305,110 +234,98 @@ conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,1
         tma_load_4d(smem + DgSmem::A_OFF + s * DG_A_BYTES, &tmDY, &a_full[s], 0, w0 - 2, -2, img);
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc_bf16(128, 32, false, false);
-    mbar_wait(w_full, 0);
-    if (dbg_on && lane == 0) dbg[2] = globaltimer_ns();                       // weights resident
-    int it = 0, tl = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++tl) {
-      const int buf = tl & 1;
-      mbar_wait(&acc_empty[buf], ((tl >> 1) & 1) ^ 1);
-      tc_fence_after_sync();
-      {
-        const int s = it % DG_STAGES;
-        mbar_wait(&a_full[s], (it / DG_STAGES) & 1);
-        tc_fence_after_sync();
-        if (dbg_on && lane == 0 && it < 20) dbg[32 + it] = globaltimer_ns();   // MMA: data of load `it` landed
-        if (elect_one()) {
-          // tap (kh,kw) starts (4-kh) patch rows and (4-kw) pixels into the patch; 128 B per pixel, groups 12*128 B apart
-          const uint64_t da0 = make_smem_desc(smem_u32(smem + DgSmem::A_OFF + s * DG_A_BYTES), 16, 1536, SWZ_128B);
-          const uint64_t db0 = make_smem_desc(smem_u32(smem), 16, 1024, SWZ_128B);   // W[tap]: 32 ci rows x 64 co, K-major
-          const uint32_t tm = tmem_base + buf * 32;
-#pragma unroll
-          for (int tap = 0; tap < 25; ++tap) {
-#pragma unroll
-            for (int k = 0; k < 4; ++k) {
-              const uint64_t da = da0 + (uint64_t)((((4 - tap / 5) * 12 + (4 - tap % 5)) * 128 + 32 * k) >> 4);
-              const uint64_t db = db0 + (uint64_t)((tap * 4096 + 32 * k) >> 4);
-              umma_bf16(tm, da, db, idesc, (tap | k) != 0);
-            }
-          }
-          umma_commit(&a_empty[s]);
-          umma_commit(&acc_full[buf]);
-        }
-        __syncwarp();
-        ++it;
-      }
-    }
   } else {
-    const int q = warp & 3;
-    int tl = 0;
-    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++tl) {
-      const int buf = tl & 1;
-      const int img = t >> 1, w0 = (t & 1) * 8;
-      mbar_wait(&acc_full[buf], (tl >> 1) & 1);
-      tc_fence_after_sync();
-      if (dbg_on && q == 0 && lane == 0 && tl < 8) dbg[56 + tl] = globaltimer_ns();   // epilogue: accumulator of tile tl complete
-      uint32_t v[32];
-      tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + buf * 32, v);
-      tmem_ld_wait();
-      tc_fence_before_sync();
-      if (lane == 0) mbar_arrive(&acc_empty[buf]);
-      const int h = 4 * q + (lane >> 3), w = w0 + (lane & 7);
-      if (h < 14 && w < 14) {
-        __nv_bfloat16* o = dx + (((size_t)img * 14 + h) * 14 + w) * 32;
+    const int r = 16 * warp + (lane & 7) + ((lane >> 3) & 1) * 8;
+    const int hr = r >> 3, wr = r & 7, kc = lane >> 4;
+    // W[tap] as B: 32 ci rows x 64 co, K-major (128 B rows, 8-row groups 1024 B apart); a K step of 16 co = 32 B
+    const uint64_t db0 = make_smem_desc(smem_u32(smem), 16, 1024, SWZ_128B);
+    mbar_wait(w_full, 0);
+    if (dbg_on && threadIdx.x == 0) dbg[2] = globaltimer_ns();                       // weights resident
+    float acc[16];
 #pragma unroll
-        for (int j = 0; j < 32; j += 8)
-          *reinterpret_cast<uint4*>(o + j) =
-              make_uint4(pack_bf16x2(__uint_as_float(v[j]), __uint_as_float(v[j + 1])),
-                         pack_bf16x2(__uint_as_float(v[j + 2]), __uint_as_float(v[j + 3])),
-                         pack_bf16x2(__uint_as_float(v[j + 4]), __uint_as_float(v[j + 5])),
-                         pack_bf16x2(__uint_as_float(v[j + 6]), __uint_as_float(v[j + 7])));
+    for (int j = 0; j < 16; ++j) acc[j] = 0.f;
+    int it = 0;
+    for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
+      const int img = t >> 1, w0 = (t & 1) * 8;
+      const int s = it % DG_STAGES;
+      mbar_wait(&a_full[s], (it / DG_STAGES) & 1);
+      if (dbg_on && threadIdx.x == 0 && it < 20) dbg[32 + it] = globaltimer_ns();   // MMA: data of load `it` landed
+      const uint32_t patch = smem_u32(smem + DgSmem::A_OFF + s * DG_A_BYTES);
+      fence_regs(acc);
+#pragma unroll
+      for (int tap = 0; tap < 25; ++tap) {
+        const int pix = (hr + 4 - tap / 5) * 12 + wr + 4 - tap % 5;
+        uint32_t a[4][4];
+#pragma unroll
+        for (int k = 0; k < 4; ++k) ldsm_x4(patch_addr<128>(patch, pix, 2 * k + kc), a[k]);
+        wgmma_fence();
+#pragma unroll
+        for (int k = 0; k < 4; ++k) wgmma_m64n32_rs<0>(acc, a[k], desc_advance(db0, tap * 4096 + 32 * k), (tap | k) != 0);
+      }
+      wgmma_commit();
+      wgmma_wait<0>();
+      fence_regs(acc);
+      __syncwarp();
+      if (lane == 0) mbar_arrive(&a_empty[s]);
+      if (dbg_on && threadIdx.x == 0 && it < 8) dbg[56 + it] = globaltimer_ns();    // accumulator of tile `it` complete
+      const int r0 = 16 * warp + (lane >> 2);
+#pragma unroll
+      for (int half = 0; half < 2; ++half) {
+        const int rr = r0 + 8 * half;
+        const int h = rr >> 3, w = w0 + (rr & 7);
+        if (h < 14 && w < 14) {
+          __nv_bfloat16* o = dx + (((size_t)img * 14 + h) * 14 + w) * 32 + 2 * (lane & 3);
+#pragma unroll
+          for (int j = 0; j < 4; ++j)
+            *reinterpret_cast<uint32_t*>(o + 8 * j) = pack_bf16x2(acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
+        }
       }
     }
   }
-  tc_fence_before_sync();
   __syncthreads();
   if (dbg_on && threadIdx.x == 0) dbg[3] = globaltimer_ns();
-  if (warp == 1) tmem_dealloc<64>(tmem_base);
 }
 
 // ------------------------------------------------------------------------------------------------------
 // wgrad: CTA = (group of 4 taps, slice of the pixel tiles).  Per pixel tile (16 rows x 8 columns) a stage
 // holds the same 20 x 12 input patch as the forward pass (15 KB, A operand for every tap of the group) and
-// the 16 x 8 tile of dY (16 KB, B operand).  M = (tap, ci): the four taps of a group are M-chunks whose
-// windows start a uniform distance apart inside the patch:
-//     group g < 5 : taps (kh = 0..3, kw = g)   -> chunk stride = one patch row = 768 B
-//     group 5     : taps (kh = 4, kw = 0..3)   -> chunk stride = one pixel     =  64 B
-//     group 6     : tap  (kh = 4, kw = 4) + three padding chunks (computed, never stored)
+// the 16 x 8 tile of dY (16 KB, B operand).  M = (tap, ci): the four taps of a group are 32-row M-chunks
+// (warps 2q, 2q + 1 hold chunk q) whose windows start at
+//     group g < 5 : taps (kh = 0..3, kw = g)
+//     group 5     : taps (kh = 4, kw = 0..3)
+//     group 6     : tap  (kh = 4, kw = 4) + three padding chunks (zero operands, never stored)
 // ------------------------------------------------------------------------------------------------------
-constexpr int WG_STAGES = 4;   // 4 x 32 KB: leaves room for two conv1_wgrad CTAs (37 KB each) on the same SM
+constexpr int WG_STAGES = 4;
 constexpr int WG_A_BYTES = 20 * 12 * 32 * 2;   // 15 KB patch
 constexpr int WG_B_BYTES = 128 * 64 * 2;       // 16 KB dY tile
 constexpr int WG_STAGE_BYTES = WG_A_BYTES + WG_B_BYTES + 1024;   // keep the dY tile 1024-aligned (128B swizzle)
 constexpr int WG_GROUPS = 7;
 struct WgSmem {
   static constexpr int BAR_OFF = WG_STAGES * WG_STAGE_BYTES;
-  static constexpr int TOTAL = BAR_OFF + 256 + 1024 + 4096;     // + slack: group 6's padding chunks read past the patch
+  static constexpr int TOTAL = BAR_OFF + 256 + 1024;
 };
+// Partial sums of one tap group of one CTA ([4 M-chunks][32 ci][64 co]), reduced in pixel-slice order by the last CTA of
+// the group's set (see arrive_last_cta).
+constexpr int WG_PART_FLOATS = 4 * 32 * 64;
+constexpr int WG_MAX_PARTS = 160;
+// One launch of this kernel in flight per device: the workspace and ticket are static (see arrive_last_cta).
+__device__ float g_c2wg_part[WG_MAX_PARTS * WG_PART_FLOATS];
+__device__ unsigned int g_c2wg_ticket[WG_GROUPS];
 
 // GPC = tap groups per CTA.  Every group of a CTA reuses the stage's patch + dY tile, so the shared-memory fill traffic
-// (the bound of the first version: 7 groups x 21 pixel slices re-read X and dY seven times = 111 MB through L2 per step at
-// batch 256) drops to ceil(7 / GPC) passes, at the price of ceil(7 / GPC) x fewer pixel slices, i.e. more atomics per output.
+// (7 groups x the pixel slices re-read X and dY seven times) drops to ceil(7 / GPC) passes, at the price of
+// ceil(7 / GPC) x fewer pixel slices, i.e. more atomics per output.
 template <int GPC>
 __global__ void __launch_bounds__(CV_THREADS, 1)
 conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,12,20,1), 64B swizzle
                    const __grid_constant__ CUtensorMap tmDY,   // dY, box (64,8,16,1), 128B swizzle
-                   float* __restrict__ g_w,                    // [25][32][64] fp32, accumulated atomically
+                   float* __restrict__ g_w,                    // [25][32][64] fp32, the gradient is added to it
                    int num_tiles, int splits) {
   constexpr int SETS = (WG_GROUPS + GPC - 1) / GPC;
-  constexpr uint32_t TM_COLS = GPC * 64 <= 64 ? 64 : (GPC * 64 <= 128 ? 128 : (GPC * 64 <= 256 ? 256 : 512));
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + WgSmem::BAR_OFF);
   uint64_t* empty = full + WG_STAGES;
-  uint64_t* acc_full = empty + WG_STAGES;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(acc_full + 1);
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int set = blockIdx.x % SETS, split = blockIdx.x / SETS;
   const int g_first = set * GPC;
@@ -417,22 +334,17 @@ conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,12
   const int t_end = (int)(((long long)num_tiles * (split + 1)) / splits);
   const int nt = t_end - t_begin;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmX);
     tma_prefetch_desc(&tmDY);
-    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], 1); }
-    mbar_init(acc_full, 1);
+    for (int s = 0; s < WG_STAGES; ++s) { mbar_init(&full[s], 1); mbar_init(&empty[s], CV_CONSUMERS / 32); }
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<TM_COLS>(tmem_holder);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_holder;
   pdl_wait();
   // (no early launch_dependents: resident-but-blocked CTAs of the next kernel steal SM resources from this one)
 
-  if (warp == 0) {
+  if (warp == 8) {
     if (lane == 0) {
       for (int i = 0; i < nt; ++i) {
         const int t = t_begin + i, img = t >> 1, w0 = (t & 1) * 8;
@@ -444,62 +356,83 @@ conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,12
         tma_load_4d(sA + WG_A_BYTES + 1024, &tmDY, &full[s], 0, w0, 0, img);
       }
     }
-  } else if (warp == 1) {
-    constexpr uint32_t idesc = make_idesc_bf16(128, 64, true, true);
-    for (int i = 0; i < nt; ++i) {
-      const int s = i % WG_STAGES;
-      mbar_wait(&full[s], (i / WG_STAGES) & 1);
-      tc_fence_after_sync();
-      if (elect_one()) {
-        const uint32_t b_addr = smem_u32(smem + s * WG_STAGE_BYTES) + WG_A_BYTES + 1024;
-        // B (MN-major, 128B swizzle): [pixel][64 co], 8-pixel groups 1024 B apart; K step = 2048 B.
-        const uint64_t db0 = make_smem_desc(b_addr, 8192, 1024, SWZ_128B);
+    return;
+  }
+
+  // A^T via ldmatrix.trans: x4 tile i covers ci + 8 (i & 1) and pixels + 8 (i >> 1); K step ks = pixels 16 ks ..
+  // 16 ks + 15 = tile rows 2 ks, 2 ks + 1, so this lane's pixel is (h = 2 ks + (lane >> 4), w = lane & 7)
+  const int q = warp >> 1;                         // M-chunk (tap of the group) of this warp's 16 rows
+  const int chunk = 2 * (warp & 1) + ((lane >> 3) & 1);   // 16-byte channel chunk (8 ci)
+  const int lh = lane >> 4, lw = lane & 7;
+  float acc[GPC][32];
 #pragma unroll
-        for (int gi = 0; gi < GPC; ++gi) {
-          if (gi < ng) {
-            const int group = g_first + gi;
-            // first tap of the group (as a pixel offset into the patch) and the byte distance between its four M-chunks
-            const int base_px = group < 5 ? group : (group == 5 ? 4 * 12 : 4 * 12 + 4);
-            const uint32_t lbo = group < 5 ? 768u : 64u;
-            // A (MN-major, 64B swizzle): k = pixel; 8-pixel groups (one tile row) are one patch row = 768 B apart,
-            //   M-chunks (taps) `lbo` apart; a K step = 16 pixels = two tile rows = 1536 B.
-            const uint64_t da0 = make_smem_desc(smem_u32(smem + s * WG_STAGE_BYTES) + base_px * 64, lbo, 768, SWZ_64B);
+  for (int gi = 0; gi < GPC; ++gi)
 #pragma unroll
-            for (int k = 0; k < 8; ++k)
-              umma_bf16(tmem_base + gi * 64, da0 + (uint64_t)((1536 * k) >> 4), db0 + (uint64_t)((2048 * k) >> 4), idesc, (i | k) != 0);
-          }
+    for (int j = 0; j < 32; ++j) acc[gi][j] = 0.f;
+  for (int i = 0; i < nt; ++i) {
+    const int s = i % WG_STAGES;
+    mbar_wait(&full[s], (i / WG_STAGES) & 1);
+    const uint32_t patch = smem_u32(smem + s * WG_STAGE_BYTES);
+    // B (MN-major, 128B swizzle): [pixel][64 co], 8-pixel groups 1024 B apart; K step = 16 pixels = 2048 B.
+    const uint64_t db0 = make_smem_desc(patch + WG_A_BYTES + 1024, 8192, 1024, SWZ_128B);
+#pragma unroll
+    for (int gi = 0; gi < GPC; ++gi) fence_regs(acc[gi]);
+#pragma unroll
+    for (int ks = 0; ks < 8; ++ks) {
+      uint32_t a[GPC][4];
+#pragma unroll
+      for (int gi = 0; gi < GPC; ++gi) {
+        const int group = g_first + gi;
+        // first pixel of this chunk's tap window inside the patch; group 6 chunks 1-3 are padding
+        const int base_px = group < 5 ? q * 12 + group : (group == 5 ? 48 + q : 52);
+        if (gi < ng && (group < 6 || q == 0)) {
+          ldsm_x4_trans(patch_addr<64>(patch, base_px + (2 * ks + lh) * 12 + lw, chunk), a[gi]);
+        } else {
+          a[gi][0] = a[gi][1] = a[gi][2] = a[gi][3] = 0u;
         }
-        umma_commit(&empty[s]);
-        if (i == nt - 1) umma_commit(acc_full);
       }
-      __syncwarp();
+      wgmma_fence();
+#pragma unroll
+      for (int gi = 0; gi < GPC; ++gi)
+        if (gi < ng) wgmma_m64n64_rs<1>(acc[gi], a[gi], desc_advance(db0, 2048 * ks), 1);
     }
-  } else if (nt > 0) {
-    const int q = warp & 3;               // rows 32q .. 32q+31 = M-chunk q of the group, row = ci
-    mbar_wait(acc_full, 0);
-    tc_fence_after_sync();
-#pragma unroll 1
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int gi = 0; gi < GPC; ++gi) fence_regs(acc[gi]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty[s]);
+  }
+
+  const int ci0 = 16 * (warp & 1) + (lane >> 2);
+#pragma unroll
+  for (int gi = 0; gi < GPC; ++gi) {
+    float* part = g_c2wg_part + (size_t)(blockIdx.x * GPC + gi) * WG_PART_FLOATS;
+#pragma unroll
+    for (int half = 0; half < 2; ++half) {
+      float* o = part + (q * 32 + ci0 + 8 * half) * 64 + 2 * (lane & 3);
+#pragma unroll
+      for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[gi][4 * j + 2 * half], acc[gi][4 * j + 2 * half + 1]);
+    }
+  }
+  __shared__ unsigned int s_last;
+  if (arrive_last_cta(&g_c2wg_ticket[set], splits, 1, CV_CONSUMERS, &s_last)) {
     for (int gi = 0; gi < ng; ++gi) {
       const int group = g_first + gi;
-      const int tap = group < 5 ? q * 5 + group : (group == 5 ? 20 + q : (q == 0 ? 24 : 25));
-#pragma unroll 1
-      for (int c = 0; c < 2; ++c) {
-        uint32_t v[32];
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + gi * 64 + c * 32, v);
-        tmem_ld_wait();
-        if (tap < 25) {
-          float* o = g_w + ((size_t)tap * 32 + lane) * 64 + c * 32;
-#pragma unroll
-          for (int j = 0; j < 32; j += 4)
-            red_add_f32x4(o + j, __uint_as_float(v[j]), __uint_as_float(v[j + 1]), __uint_as_float(v[j + 2]),
-                          __uint_as_float(v[j + 3]));
-        }
+      for (int e4 = threadIdx.x; e4 < WG_PART_FLOATS / 4; e4 += CV_CONSUMERS) {
+        const int row = e4 >> 4, co = (e4 & 15) * 4;        // row = M-chunk * 32 + ci
+        const int qq = row >> 5, ci = row & 31;
+        const int tap = group < 5 ? qq * 5 + group : (group == 5 ? 20 + qq : (qq == 0 ? 24 : 25));
+        if (tap >= 25) continue;
+        const float4 sum = ordered_sum4(
+            reinterpret_cast<const float4*>(g_c2wg_part + (size_t)(set * GPC + gi) * WG_PART_FLOATS) + e4, splits,
+            (size_t)SETS * GPC * WG_PART_FLOATS / 4);
+        float4* o = reinterpret_cast<float4*>(g_w + ((size_t)tap * 32 + ci) * 64 + co);
+        const float4 cur = *o;
+        *o = make_float4(cur.x + sum.x, cur.y + sum.y, cur.z + sum.z, cur.w + sum.w);
       }
     }
   }
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<TM_COLS>(tmem_base);
 }
 
 }  // namespace dm
@@ -512,19 +445,15 @@ int dm_conv2_fwd(const void* a1, const void* w_bf16, const void* bias, void* out
   CUtensorMap tmX, tmW;
   if (make_tmap_nhwc_bf16(&tmX, a1, 32, 14, 14, B, 32, 12, 20, 64)) return 101;
   if (make_tmap_2d_bf16(&tmW, w_bf16, 64, 800, 64, 64, 200, 128)) return 102;
-  static const int epi = env_int("DMNIST_CONV2_EPI", 1);
   static bool configured = false;
   if (!configured) {
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_fwd_kernel<0>, cudaFuncAttributeMaxDynamicSharedMemorySize, FwSmem::TOTAL));
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_fwd_kernel<0>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_fwd_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, FwSmem::TOTAL));
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_fwd_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    DM_CUDA_OK(cudaFuncSetAttribute(conv2_fwd_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, FwSmem::TOTAL));
+    DM_CUDA_OK(cudaFuncSetAttribute(conv2_fwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }
   const int tiles = 2 * B;
-  const int grid = tiles < 148 ? tiles : 148;
-  auto kern = epi == 0 ? conv2_fwd_kernel<0> : conv2_fwd_kernel<1>;
-  return (int)launch_kernel(kern, dim3(grid), dim3(CV_THREADS), FwSmem::TOTAL,
+  const int grid = tiles < num_sms() ? tiles : num_sms();
+  return (int)launch_kernel(conv2_fwd_kernel, dim3(grid), dim3(CV_THREADS), FwSmem::TOTAL,
                             reinterpret_cast<cudaStream_t>(stream), tmX, tmW, reinterpret_cast<const float*>(bias),
                             reinterpret_cast<__nv_bfloat16*>(out), reinterpret_cast<uint8_t*>(code), tiles);
 }
@@ -546,13 +475,13 @@ int dm_conv2_dgrad_dbg(const void* dy, const void* w_bf16, void* dx, int B, void
     configured = true;
   }
   const int tiles = 2 * B;
-  const int grid = tiles < g_max_ctas ? tiles : g_max_ctas;
+  const int grid = tiles < max_ctas() ? tiles : max_ctas();
   return (int)launch_kernel(conv2_dgrad_kernel, dim3(grid), dim3(CV_THREADS), DgSmem::TOTAL,
                             reinterpret_cast<cudaStream_t>(stream), tmDY, tmW, reinterpret_cast<__nv_bfloat16*>(dx), tiles,
                             reinterpret_cast<unsigned long long*>(dbg));
 }
 
-// g_w ([25][32][64] fp32) must be zeroed by the caller; accumulated with atomics.
+// g_w ([25][32][64] fp32) must be zeroed by the caller; the gradient is added to it.
 int dm_conv2_wgrad(const void* a1, const void* dy, void* g_w, int B, void* stream) {
   using namespace dm;
   CUtensorMap tmX, tmDY;
@@ -561,7 +490,8 @@ int dm_conv2_wgrad(const void* a1, const void* dy, void* g_w, int B, void* strea
   const int tiles = 2 * B;
   static const int gpc = env_int("DMNIST_WGRAD_GPC", 1);      // tap groups per CTA: 1 (first version), 2, 4
   const int sets = gpc == 1 ? 7 : (gpc == 2 ? 4 : 2);
-  int splits = g_max_ctas / sets;
+  int splits = max_ctas() / sets;
+  if (splits * sets * gpc > WG_MAX_PARTS) splits = WG_MAX_PARTS / (sets * gpc);
   if (splits > tiles) splits = tiles;
   static bool configured = false;
   if (!configured) {

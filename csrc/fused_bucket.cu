@@ -68,7 +68,7 @@ DMNIST_DEVICE float bf16_hi(uint32_t w) { return __uint_as_float(w & 0xffff0000u
 // early bucket
 // ---------------------------------------------------------------------------------------------------------------------
 // CTAs are small (128 threads, no shared memory, <= 96 registers) and there is one per SM: they sit next to the
-// tensor-core CTAs of the backward pass and borrow their idle issue slots (profiles/coresidency_probe_r1.txt).
+// tensor-core CTAs of the backward pass and borrow their idle issue slots.
 constexpr int EARLY2_THREADS = 128;
 
 // parts: bit 0 = exchange (arrival flags, in-place reduce of my shard, "shard out" flags), bit 1 = apply (wait for every
@@ -318,7 +318,7 @@ __global__ void __launch_bounds__(LATE2_THREADS, 1) bucket_late_kernel(SyncPeers
 // so data and "it has arrived" travel in ONE store: no flag word, no fence.sys round trip before the flag, no grid-wide
 // barrier.  A thread multicasts its lines (multimem.st; peer stores without NVLS) and then polls the matching lines of the
 // other replicas in its own inbox until all four tags of a float4 are current.  Exposed communication = one NVLink store
-// latency (~1.5 us) instead of store + ack + flag (~7 us measured at N = 2).  The inbox is double-buffered on the step's parity
+// latency instead of store + ack + flag.  The inbox is double-buffered on the step's parity
 // (a replica can be at most one step ahead of a reader) and costs 2x the bytes of the small bucket -- 475 KB per replica.
 // ---------------------------------------------------------------------------------------------------------------------
 DMNIST_DEVICE uint4 ld_volatile_b128(const void* p) {
@@ -328,7 +328,7 @@ DMNIST_DEVICE uint4 ld_volatile_b128(const void* p) {
 }
 
 // BF16 = true (default): a line carries FOUR gradients as bf16 -- {bf16x2, tag, bf16x2, tag} -- i.e. one line per float4, half the
-// bytes: at N = 8 every GPU ingests 7 slots, and 7 x 475 KB of fp32 lines were ~4 us of pure NVLink ingress on the critical path.
+// bytes: at N = 8 every GPU ingests 7 slots, and that NVLink ingress sits on the critical path.
 // Every replica sums the SAME bf16-rounded contributions (its own included) in fp32, so the replicas stay bit-identical.
 template <bool BF16>
 __global__ void __launch_bounds__(LATE2_THREADS) bucket_late_ll_kernel(SyncPeers P, SyncArgs a, BucketV2 r) {
@@ -511,7 +511,7 @@ int dm_bucket_sync(void* const* ctrl, void* const* params, void* const* grads, v
     configured = true;
   }
   if (phase != 2) {
-    if (ctas < 1) ctas = 148;
+    if (ctas < 1) ctas = dm::num_sms();
     const dim3 g(ctas), b(EARLY2_THREADS);
     const int parts = phase == 1 ? 3 : (phase == 3 ? 1 : 2);
     if (nranks == 1) return (int)launch_kernel(bucket_early_kernel<1>, g, b, 0, stream, P, a, r, parts);
@@ -532,7 +532,7 @@ int dm_bucket_sync(void* const* ctrl, void* const* params, void* const* grads, v
     return (int)launch_kernel(bucket_late_ll_kernel<false>, dim3(grid), dim3(LATE2_THREADS), 0, stream, P, a, r);
   }
   if (ctas >= 1 && grid > ctas) grid = ctas;
-  if (grid > 148) grid = 148;                                     // all CTAs must be co-resident (in-kernel barrier)
+  if (grid > dm::num_sms()) grid = dm::num_sms();                 // all CTAs must be co-resident (in-kernel barrier)
   return (int)launch_kernel(bucket_late_kernel, dim3(grid), dim3(LATE2_THREADS), 0, stream, P, a, r);
 }
 

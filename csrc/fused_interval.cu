@@ -228,7 +228,7 @@ int dm_interval_begin(void* ctrl, const void* params, void* shadow_bf16, long lo
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
   cudaError_t e = launch_kernel(iv_adopt_kernel, dim3(1), dim3(32), 0, st, reinterpret_cast<SyncCtrl*>(ctrl));
   if (e != cudaSuccess) return (int)e;
-  return (int)launch_kernel(iv_shadow_kernel, dim3(148), dim3(IV_THREADS), 0, st, reinterpret_cast<const SyncCtrl*>(ctrl),
+  return (int)launch_kernel(iv_shadow_kernel, dim3(num_sms()), dim3(IV_THREADS), 0, st, reinterpret_cast<const SyncCtrl*>(ctrl),
                             reinterpret_cast<const float*>(params), reinterpret_cast<__nv_bfloat16*>(shadow_bf16),
                             (int)(numel / 4));
 }
@@ -256,7 +256,7 @@ int dm_interval_end(void* const* ctrl, void* const* params, void* const* grads, 
   a.shadow = nullptr; a.mc_grads = nullptr;
   a.mc_params = nranks > 1 ? reinterpret_cast<float*>(mc_params) : nullptr;
   cudaStream_t st = reinterpret_cast<cudaStream_t>(stream_);
-  if (ctas < 1 || ctas > 148) ctas = 148;
+  if (ctas < 1 || ctas > num_sms()) ctas = num_sms();
   SyncCtrl* me = P.ctrl[rank];
   cudaError_t e = launch_kernel(iv_gate_kernel, dim3(1), dim3(32), 0, st, me);
   if (e != cudaSuccess) return (int)e;

@@ -197,7 +197,7 @@ __global__ void __launch_bounds__(SYNC_THREADS, 1) fused_sync_sgd_kernel(SyncPee
         }
       }
     } else {
-    // Latency is the enemy here (a remote load is ~2 us): every thread issues the loads of ALL contributors
+    // Latency is the enemy here (a remote load is a full NVLink round trip): every thread issues the loads of ALL contributors
     // for U elements before it touches any of them, so one NVLink round trip covers the whole reduction of
     // its elements (at N = 8 a shard is so small that most threads make exactly one trip).
     constexpr int U = 2;
@@ -267,7 +267,7 @@ __global__ void __launch_bounds__(SYNC_THREADS, 1) fused_sync_sgd_kernel(SyncPee
   __syncthreads();
   if (blockIdx.x == 0 && threadIdx.x == 0) me->t_phase[4] = globaltimer_ns();
 
-  // ---- local bf16 shadow of the fresh weights (operand source for the tcgen05 kernels) --------------
+  // ---- local bf16 shadow of the fresh weights (operand source for the tensor-core kernels) --------------
   if (a.shadow != nullptr) {
     const float* w = P.params[a.rank];
     for (int i = blockIdx.x * SYNC_THREADS + threadIdx.x; i < a.numel4; i += gridDim.x * SYNC_THREADS) {
@@ -315,10 +315,8 @@ struct BucketArgs {
 // NR = number of replicas (compile time: the peer loop keeps 16 independent 16-byte loads in flight per thread).
 // CTAs are SMALL (128 threads = one warp per scheduler, <= 96 registers, no shared memory) and there is one per SM: they fit
 // next to the tensor-core CTAs of conv2 dgrad/wgrad and conv1 wgrad, whose six warps leave the schedulers mostly idle,
-// so the exchange borrows issue slots instead of whole SMs.  (A first version used 20 full-size CTAs on reserved SMs:
-// an SM sustains only ~10 GB/s of peer traffic -- its outstanding-request budget over a ~3 us round trip -- so 20 of
-// them needed 33 us for the 2 x 3.2 MB, longer than the backward pass they were hiding under; see
-// profiles/bench_r1_call26_2gpu_bucketed.txt.)
+// so the exchange borrows issue slots instead of whole SMs.  (Peer traffic per SM is bounded by its outstanding-request
+// budget over an NVLink round trip, so a few full-size CTAs on reserved SMs cannot move the bucket in time.)
 constexpr int EARLY_THREADS = 128;   // one warp per scheduler, 3 K registers each: fits next to conv2_dgrad / conv1_wgrad CTAs
 template <int NR>
 __global__ void __launch_bounds__(EARLY_THREADS) fused_sync_early_kernel(SyncPeers P, SyncArgs a, BucketArgs r) {
@@ -532,7 +530,7 @@ __global__ void straggler_delay_kernel(const SyncCtrl* ctrl, float prob, unsigne
   }
 }
 
-// Device-side barrier over NVLink flags: returns on every replica within a flag hop (~2 us) of the LAST replica entering it.
+// Device-side barrier over NVLink flags: returns on every replica within a flag hop of the LAST replica entering it.
 // Used to align the replicas' streams (e.g. right before a timed region: a host-side barrier leaves tens of microseconds of
 // start skew between the processes).
 __global__ void device_barrier_kernel(SyncPeers P, int rank, int nranks, unsigned long long timeout_ns) {
@@ -637,11 +635,11 @@ int dm_fused_sync_bucket(void* const* ctrl, void* const* params, void* const* gr
   r.begin4 = (int)(begin / 4); r.end4 = (int)(end / 4);
   r.early_begin4 = (int)(early_begin / 4); r.early_end4 = (int)(early_end / 4);
   cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
-  if (ctas < 1) ctas = 148;
+  if (ctas < 1) ctas = dm::num_sms();
   if (phase == 1) {
     // The early kernel must be CO-RESIDENT with the tensor-core kernels of the backward pass.  CTAs of kernels that run
-    // with different L1/shared splits cannot share an SM (observed: the early kernel only got SMs as conv2_dgrad CTAs
-    // exited, profiles/bench_r1_call27_2gpu.txt), so EVERY kernel of the step asks for the same split (max shared).
+    // with different L1/shared splits cannot share an SM (the early kernel would only get SMs as the conv2_dgrad CTAs
+    // exit), so EVERY kernel of the step asks for the same split (max shared).
     static bool configured = false;
     if (!configured) {
       DM_CUDA_OK(cudaFuncSetAttribute(fused_sync_early_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
@@ -668,7 +666,7 @@ int dm_sync_set_host_mirror(void* ctrl, void* host_ptr) {
 
 int dm_f32_to_bf16(const void* src, void* dst, long long numel, void* stream_) {
   if (numel & 3) return -1;
-  dm::f32_to_bf16_kernel<<<148, 512, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+  dm::f32_to_bf16_kernel<<<dm::num_sms(), 512, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       reinterpret_cast<const float*>(src), reinterpret_cast<__nv_bfloat16*>(dst), (int)(numel / 4));
   return (int)cudaGetLastError();
 }

@@ -65,7 +65,7 @@ struct SyncCtrl {
   uint32_t cta_counter_iv;
   // ---- host mirror of the status words: the kernel that closes a step writes (epoch, error, accepted, dropped, last_mask,
   // last_count, last_late, seq) into page-locked HOST memory (zero-copy store over PCIe) so the training loop learns a step's
-  // outcome without a device read or a memcpy node in the step graph (a D2H memcpy node costs the graph ~10 us) ------------------
+  // outcome without a device read or a memcpy node in the step graph (a D2H memcpy node adds a copy to the graph) ------------------
   uint32_t status_seq;                     // number of steps closed so far (ring index of the mirror slot = seq & 3)
   uint32_t* host_mirror;                   // 4 slots x 8 words in mapped pinned host memory, or null
   uint32_t decider_claim;                  // step+1 of the newest launch whose arrival/commit decision a CTA has claimed
@@ -179,7 +179,7 @@ DMNIST_DEVICE float device_lr(const SyncArgs& a, uint32_t step) {
 
 // Poll (RELAXED loads inside pred) until pred() or the watchdog fires, then ONE acquire load of the flag the wait was about
 // (`acq`: LDG.STRONG.SYS + a single CCTL.IVALL; a fence.acq_rel.sys here would be a MEMBAR.ALL.SYS, which also waits for every
-// outstanding store of the SM -- measured: +4 us per step at N = 2 -- and an acquire load on every poll invalidates the SM's
+// outstanding store of the SM -- and an acquire load on every poll invalidates the SM's
 // L1 thousands of times under the co-resident tensor-core kernels).
 template <class Pred>
 DMNIST_DEVICE bool spin_until(Pred pred, unsigned long long timeout_ns, const volatile uint32_t* acq) {

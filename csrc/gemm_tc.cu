@@ -1,4 +1,4 @@
-// tcgen05 GEMM for sm_100a:  D[M,N] (+)= A[M,K] * B[K,N],  bf16 in, fp32 accumulate in TMEM.
+// wgmma GEMM for sm_90a:  D[M,N] (+)= A[M,K] * B[K,N],  bf16 in, fp32 accumulate in registers.
 //
 // Covers every dense GEMM of the models (reference ops K6/K8: tf.matmul, src/mnist.py:136,145,
 // and their gradients) without a single transpose kernel: each operand may be K-major or
@@ -9,9 +9,11 @@
 //     fc wgrad  D[in,out] = X[b,in]   (A MN-major) * dY[b,out]  (B MN-major),  K = batch
 //
 // Structure (one 128 x BN output tile per CTA, optional split-K over gridDim.z):
-//     warp 0      TMA producer      cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx
-//     warp 1      MMA issuer        one elected lane issues tcgen05.mma; tcgen05.commit frees the stage
-//     warps 2-5   epilogue          tcgen05.ld (32 lanes x 32 columns) -> registers -> global
+//     warps 0-7   two consumer warpgroups: warpgroup g issues wgmma for rows 64 g .. 64 g + 63 of the tile
+//                 (BN / 64 m64n64k16 instructions per K step); afterwards all eight warps run the epilogue
+//     warp 8      TMA producer      cp.async.bulk.tensor -> 128B-swizzled smem ring, mbarrier tx
+// The accumulator is staged through the (then idle) operand ring as a [128][BN] fp32 tile, so the epilogue
+// keeps one thread per output row with 32 consecutive columns in registers.
 #include "common.cuh"
 #include "host_utils.h"
 
@@ -20,7 +22,8 @@ namespace dm {
 constexpr int GEMM_BM = 128;
 constexpr int GEMM_BK = 64;
 constexpr int GEMM_STAGES = 4;
-constexpr int GEMM_THREADS = 192;
+constexpr int GEMM_CONSUMERS = 256;                   // two warpgroups
+constexpr int GEMM_THREADS = GEMM_CONSUMERS + 32;      // + the TMA producer warp
 
 enum GemmEpilogue : int { EPI_STORE_F32 = 0, EPI_ATOMIC_F32 = 1, EPI_STORE_BF16 = 2, EPI_BIAS_RELU_BF16 = 3,
                           // fc1 dgrad fused with the backward of maxpool2 + ReLU2 (reference K4/K3 gradients): a 64-column
@@ -37,7 +40,7 @@ struct GemmParams {
   long long split_stride;   // EPI_STORE_F32 with split-K: split z writes its partial tile at out + z*split_stride
   const float* bias;        // EPI_BIAS_RELU_BF16: per-column bias (reference K2/K3 fused into the producer)
   const uint8_t* code;      // EPI_UNPOOL2_BF16: pooling codes [M][N] (bits 0-1 argmax position, bit 2 ReLU active)
-  float* g_bias;            // EPI_UNPOOL2_BF16: conv2 bias gradient [64], accumulated atomically (pre-zeroed)
+  float* g_bias;            // EPI_UNPOOL2_BF16: conv2 bias gradient [64], the CTAs' sum is added to it (pre-zeroed)
 };
 
 template <int BN>
@@ -45,20 +48,25 @@ struct GemmSmem {
   static constexpr int A_BYTES = GEMM_BM * GEMM_BK * 2;   // 16 KB
   static constexpr int B_BYTES = BN * GEMM_BK * 2;
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
-  // (a 3-deep ring for the 128-wide tiles would let fc1_wgrad share SMs with fc1_dgrad; measured: both then take 12 us
-  //  instead of 9.4 + 7.8 back to back and the critical path loses 3 us -- profiles/bench_r1_call35_1gpu.txt -- so 4 it is)
   static constexpr int STAGES = GEMM_STAGES;
   static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int TOTAL = BAR_OFFSET + 256 + 1024;   // barriers + alignment slack
+  static constexpr int BPART_OFFSET = BAR_OFFSET + 128;   // EPI_UNPOOL2_BF16: [4 row quarters][64] bias partials + flag
+  static constexpr int TOTAL = BAR_OFFSET + 2048 + 1024;  // barriers, bias partials + alignment slack
+  // epilogue staging (reuses the ring): rows padded by 4 floats so that 32 threads reading 16 B of 32 different rows
+  // hit distinct banks
+  static constexpr int ACC_LD = BN + 4;
+  static_assert(GEMM_BM * ACC_LD * 4 <= BAR_OFFSET, "accumulator staging must fit in the operand ring");
 };
 
-// The unpool epilogue is instruction-heavy: it gets eight epilogue warps (two per TMEM lane quarter, one 32-column
-// chunk each) instead of four, so two warps share every scheduler and hide each other's latencies.
-template <int EPI>
-constexpr int gemm_threads() { return EPI == EPI_UNPOOL2_BF16 ? GEMM_THREADS + 128 : GEMM_THREADS; }
+// EPI_UNPOOL2_BF16: per-CTA conv2 bias-gradient partials, added up in CTA order by the last CTA (arrive_last_cta), so the
+// result does not depend on the order in which the CTAs finish.
+constexpr int UNPOOL_MAX_CTAS = 4096;                  // batch <= 4096 / 49 row tiles x 128 = 10 624 rows
+// One launch of this kernel in flight per device: the workspace and ticket are static (see arrive_last_cta).
+__device__ float g_unpool_bias_part[UNPOOL_MAX_CTAS * 64];
+__device__ unsigned int g_unpool_ticket;
 
 template <int BN, bool A_MN, bool B_MN, int EPI>
-__global__ void __launch_bounds__(gemm_threads<EPI>(), 1)
+__global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams p) {
   using S = GemmSmem<BN>;
   extern __shared__ uint8_t smem_raw[];
@@ -66,8 +74,6 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full_bar = reinterpret_cast<uint64_t*>(smem + S::BAR_OFFSET);
   uint64_t* empty_bar = full_bar + S::STAGES;
-  uint64_t* tmem_full_bar = empty_bar + S::STAGES;
-  uint32_t* tmem_holder = reinterpret_cast<uint32_t*>(tmem_full_bar + 1);
 
   const int warp = threadIdx.x >> 5;
   const int lane = threadIdx.x & 31;
@@ -78,25 +84,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   const int kb_end = (int)(((long long)p.num_kb * (blockIdx.z + 1)) / gridDim.z);
   const int nkb = kb_end - kb_begin;
 
-  if (warp == 0 && lane == 0) {
+  if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmA);
     tma_prefetch_desc(&tmB);
     for (int s = 0; s < S::STAGES; ++s) {
       mbar_init(&full_bar[s], 1);
-      mbar_init(&empty_bar[s], 1);
+      mbar_init(&empty_bar[s], GEMM_CONSUMERS / 32);   // one arrival per consumer warp
     }
-    mbar_init(tmem_full_bar, 1);
     fence_mbar_init();
   }
-  if (warp == 1) tmem_alloc<BN>(tmem_holder);
-  tc_fence_before_sync();
   __syncthreads();
-  tc_fence_after_sync();
-  const uint32_t tmem_base = *tmem_holder;
   pdl_wait();      // everything above is private set-up; operands / outputs belong to earlier kernels until here
   // (no early launch_dependents: resident-but-blocked CTAs of the next kernel steal SM resources from this one)
 
-  if (warp == 0) {
+  if (warp == 8) {
     // ------------------------------ TMA producer ------------------------------
     if (lane == 0) {
       for (int i = 0; i < nkb; ++i) {
@@ -121,61 +122,91 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
     }
-  } else if (warp == 1) {
-    // ------------------------------ MMA issuer --------------------------------
-    constexpr uint32_t idesc = make_idesc_bf16(GEMM_BM, BN, A_MN, B_MN);
-    for (int i = 0; i < nkb; ++i) {
-      const int s = i % S::STAGES;
-      const uint32_t ph = (i / S::STAGES) & 1;
-      mbar_wait(&full_bar[s], ph);
-      tc_fence_after_sync();
-      if (elect_one()) {
-        const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES);
-        const uint32_t b_addr = a_addr + S::A_BYTES;
-        // K-major:  128 B rows (64 bf16 of K), 8-row groups 1024 B apart; K advances 32 B per UMMA_K.
-        // MN-major: 128 B k-rows (64 bf16 of M/N), 8-k groups 1024 B apart, 64-wide M/N chunks 8192 B
-        //           apart; K advances 16 k-rows = 2048 B per UMMA_K.
-        const uint64_t da0 = A_MN ? make_smem_desc(a_addr, 8192, 1024, SWZ_128B)
-                                  : make_smem_desc(a_addr, 16, 1024, SWZ_128B);
-        const uint64_t db0 = B_MN ? make_smem_desc(b_addr, 8192, 1024, SWZ_128B)
-                                  : make_smem_desc(b_addr, 16, 1024, SWZ_128B);
+    return;
+  }
+
+  // ------------------------------ consumers: wgmma main loop ------------------------------
+  const int wg = warp >> 2;                        // warpgroup = rows 64 wg .. 64 wg + 63 of the tile
+  constexpr int NC = BN / 64;                      // 64-column chunks
+  float acc[NC][32];
 #pragma unroll
-        for (int k = 0; k < GEMM_BK / 16; ++k) {
-          const uint64_t da = desc_advance(da0, (A_MN ? 2048u : 32u) * k);
-          const uint64_t db = desc_advance(db0, (B_MN ? 2048u : 32u) * k);
-          umma_bf16(tmem_base, da, db, idesc, (i | k) != 0);
-        }
-        umma_commit(&empty_bar[s]);                  // stage reusable once these MMAs retire
-        if (i == nkb - 1) umma_commit(tmem_full_bar);  // accumulator complete
+  for (int c = 0; c < NC; ++c)
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[c][j] = 0.f;
+  for (int i = 0; i < nkb; ++i) {
+    const int s = i % S::STAGES;
+    mbar_wait(&full_bar[s], (i / S::STAGES) & 1);
+    const uint32_t a_addr = smem_u32(smem + s * S::STAGE_BYTES);
+    const uint32_t b_addr = a_addr + S::A_BYTES;
+    // K-major:  128 B rows (64 bf16 of K), 8-row groups 1024 B apart; K advances 32 B per K step of 16.
+    // MN-major: 128 B k-rows (64 bf16 of M/N), 8-k groups 1024 B apart, 64-wide M/N chunks 8192 B
+    //           apart; K advances 16 k-rows = 2048 B per K step.
+    // Either way rows 64 .. 127 of A and columns 64 c .. 64 c + 63 of B start 8192 B further on.
+    const uint64_t da0 = A_MN ? make_smem_desc(a_addr + 8192 * wg, 8192, 1024, SWZ_128B)
+                              : make_smem_desc(a_addr + 8192 * wg, 16, 1024, SWZ_128B);
+    const uint64_t db0 = B_MN ? make_smem_desc(b_addr, 8192, 1024, SWZ_128B)
+                              : make_smem_desc(b_addr, 16, 1024, SWZ_128B);
+#pragma unroll
+    for (int c = 0; c < NC; ++c) fence_regs(acc[c]);
+    wgmma_fence();
+#pragma unroll
+    for (int k = 0; k < GEMM_BK / 16; ++k) {
+      const uint64_t da = desc_advance(da0, (A_MN ? 2048u : 32u) * k);
+#pragma unroll
+      for (int c = 0; c < NC; ++c) {
+        const uint64_t db = desc_advance(db0, (B_MN ? 2048u : 32u) * k + 8192u * c);
+        wgmma_m64n64_ss<A_MN ? 1 : 0, B_MN ? 1 : 0>(acc[c], da, db, (i | k) != 0);
       }
-      __syncwarp();
     }
-  } else {
-    // ------------------------------ epilogue -----------------------------------
-    const int q = warp & 3;                          // TMEM lane quarter this warp may access
-    const int row = m0 + q * 32 + lane;
-    const int c_begin = EPI == EPI_UNPOOL2_BF16 ? (warp - 2) >> 2 : 0;
+    wgmma_commit();
+    wgmma_wait<0>();
+#pragma unroll
+    for (int c = 0; c < NC; ++c) fence_regs(acc[c]);
+    __syncwarp();
+    if (lane == 0) mbar_arrive(&empty_bar[s]);     // stage reusable: this warp's MMAs have read it
+  }
+
+  // ------------------------------ accumulator -> shared staging tile ------------------------------
+  named_bar_sync(1, GEMM_CONSUMERS);               // both warpgroups are done with the ring
+  float* stage = reinterpret_cast<float*>(smem);
+  {
+    const int r = 16 * warp + (lane >> 2);         // tile row of d[4j], d[4j+1]; d[4j+2], d[4j+3] are 8 rows below
+#pragma unroll
+    for (int c = 0; c < NC; ++c)
+#pragma unroll
+      for (int j = 0; j < 8; ++j) {
+        const int col = 64 * c + 8 * j + 2 * (lane & 3);
+        *reinterpret_cast<float2*>(stage + r * S::ACC_LD + col) = make_float2(acc[c][4 * j], acc[c][4 * j + 1]);
+        *reinterpret_cast<float2*>(stage + (r + 8) * S::ACC_LD + col) = make_float2(acc[c][4 * j + 2], acc[c][4 * j + 3]);
+      }
+  }
+  named_bar_sync(1, GEMM_CONSUMERS);
+
+  // ------------------------------ epilogue: thread = tile row, 32-column chunks ------------------------------
+  {
+    const int lr = threadIdx.x & 127;                // tile row
+    const int half = threadIdx.x >> 7;               // chunks half, half + 2, ...
+    const int row = m0 + lr;
+    const int c_begin = half;
     const int c_end = EPI == EPI_UNPOOL2_BF16 ? c_begin + 1 : BN / 32;
     uint32_t cw[8] = {0u, 0u, 0u, 0u, 0u, 0u, 0u, 0u};
     if (EPI == EPI_UNPOOL2_BF16 && row < p.M) {
-      // pooling codes of this thread's 32 channels: an input of the forward pass, fetched while the MMAs run
+      // pooling codes of this thread's 32 channels
       const uint4* cp = reinterpret_cast<const uint4*>(p.code + (size_t)row * p.N + n0 + c_begin * 32);
       const uint4 c0 = __ldg(cp), c1 = __ldg(cp + 1);
       cw[0] = c0.x; cw[1] = c0.y; cw[2] = c0.z; cw[3] = c0.w; cw[4] = c1.x; cw[5] = c1.y; cw[6] = c1.z; cw[7] = c1.w;
     }
-    if (nkb > 0) {
-      mbar_wait(tmem_full_bar, 0);
-      tc_fence_after_sync();
-    }
 #pragma unroll 1
-    for (int c = c_begin; c < c_end; ++c) {
+    for (int c = c_begin; c < c_end; c += 2) {
       uint32_t v[32];
-      if (nkb > 0) {
-        tmem_ld_32x32(tmem_base + ((uint32_t)(q * 32) << 16) + c * 32, v);
-        tmem_ld_wait();
-      } else {
+      {
+        const float* src = stage + lr * S::ACC_LD + c * 32;
 #pragma unroll
-        for (int j = 0; j < 32; ++j) v[j] = 0;
+        for (int j = 0; j < 32; j += 4) {
+          const float4 t = *reinterpret_cast<const float4*>(src + j);
+          v[j] = __float_as_uint(t.x); v[j + 1] = __float_as_uint(t.y);
+          v[j + 2] = __float_as_uint(t.z); v[j + 3] = __float_as_uint(t.w);
+        }
       }
       const int col0 = n0 + c * 32;
       if (row < p.M) {
@@ -278,14 +309,26 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
             }
           }
         }
-        atomicAdd(p.g_bias + ch0 + lane, gs[0]);
+        reinterpret_cast<float*>(smem + S::BPART_OFFSET)[((threadIdx.x >> 5) & 3) * 64 + ch0 + lane] = gs[0];
       }
     }
   }
+  if (EPI == EPI_UNPOOL2_BF16) {
+    const float* s_bpart = reinterpret_cast<const float*>(smem + S::BPART_OFFSET);
+    named_bar_sync(1, GEMM_CONSUMERS);
+    const int cta = blockIdx.y * gridDim.x + blockIdx.x;
+    if (threadIdx.x < 64)
+      g_unpool_bias_part[cta * 64 + threadIdx.x] =
+          s_bpart[threadIdx.x] + s_bpart[64 + threadIdx.x] + s_bpart[128 + threadIdx.x] + s_bpart[192 + threadIdx.x];
+    volatile unsigned int* s_flag = reinterpret_cast<volatile unsigned int*>(smem + S::BPART_OFFSET + 1024);
+    if (arrive_last_cta(&g_unpool_ticket, gridDim.x * gridDim.y, 1, GEMM_CONSUMERS, s_flag) && threadIdx.x < 16) {
+      const float4 sum = ordered_sum4(reinterpret_cast<const float4*>(g_unpool_bias_part) + threadIdx.x,
+                                      gridDim.x * gridDim.y, 16);
+      float* o = p.g_bias + 4 * threadIdx.x;
+      o[0] += sum.x; o[1] += sum.y; o[2] += sum.z; o[3] += sum.w;
+    }
+  }
 
-  tc_fence_before_sync();
-  __syncthreads();
-  if (warp == 1) tmem_dealloc<BN>(tmem_base);
 }
 
 // ---------------------------------------------------------------------------------
@@ -303,7 +346,7 @@ static int launch_gemm(const CUtensorMap& tmA, const CUtensorMap& tmB, const Gem
     configured = true;
   }
   dim3 grid((p.M + GEMM_BM - 1) / GEMM_BM, (p.N + BN - 1) / BN, splits);
-  return (int)launch_kernel(kern, grid, dim3(gemm_threads<EPI>()), smem, stream, tmA, tmB, p);
+  return (int)launch_kernel(kern, grid, dim3(GEMM_THREADS), smem, stream, tmA, tmB, p);
 }
 
 template <int BN, int EPI>
@@ -356,7 +399,7 @@ extern "C" int dm_gemm_bf16(const void* A, const void* B, void* out, int M, int 
     DM_DISPATCH(128, 3);
   } else {
     // 128 x 256 tiles: twice the FLOPs per operand byte fetched from L2 (the large MLP GEMMs are L2->SM bandwidth bound with
-    // 128 x 128 tiles: 2048 CTAs x 2 MB of operands each), M128 N256 K16 instructions run at the tensor-pipe floor
+    // 128 x 128 tiles: 2048 CTAs x 2 MB of operands each)
     if (epi == 0) DM_DISPATCH(256, 0);
     if (epi == 2) DM_DISPATCH(256, 2);
     if (epi == 3) DM_DISPATCH(256, 3);
@@ -368,7 +411,7 @@ extern "C" int dm_gemm_bf16(const void* A, const void* B, void* out, int M, int 
 // fc1 dgrad fused with the maxpool2/ReLU2 backward and the conv2 bias gradient:
 //   dxfc[b, j] = sum_k dh[b, k] * W1[j, k]   (A = dh [B,512] K-major, B = W1 [3136,512] rows = j, K contiguous)
 //   dy2[b, 2ph+dy, 2pw+dx, c] = dxfc[b, (ph*7+pw)*64 + c] where code says (dy,dx) is the argmax and ReLU was active
-//   g_bias2[c] += sum of the scattered values.          dy2: [B,14,14,64] bf16, fully written (zeros included).
+//   g_bias2[c] += sum of the scattered values (summed in a fixed order: bit-reproducible).          dy2: [B,14,14,64] bf16, fully written (zeros included).
 extern "C" int dm_fc1_dgrad_unpool(const void* dh, const void* w1_bf16, const void* code2, void* dy2, void* g_bias2, int B,
                                    void* stream_) {
   using namespace dm;
@@ -377,6 +420,7 @@ extern "C" int dm_fc1_dgrad_unpool(const void* dh, const void* w1_bf16, const vo
   if (rc) return 100 + rc;
   rc = make_tmap_2d_bf16(&tmB, w1_bf16, 512, 3136, 512, 64, 64, 128);
   if (rc) return 200 + rc;
+  if (((B + GEMM_BM - 1) / GEMM_BM) * (3136 / 64) > UNPOOL_MAX_CTAS) return -6;
   GemmParams p{B, 3136, 512 / GEMM_BK, 0, dy2, 0, nullptr, reinterpret_cast<const uint8_t*>(code2),
                reinterpret_cast<float*>(g_bias2)};
   return launch_gemm<64, false, false, EPI_UNPOOL2_BF16>(tmA, tmB, p, 1, reinterpret_cast<cudaStream_t>(stream_));

@@ -7,7 +7,20 @@
 namespace dm {
 
 int g_pdl = 0;
-int g_max_ctas = 148;
+int g_max_ctas = 0;
+
+int num_sms() {
+  static int n = 0;
+  if (n == 0) {
+    int dev = 0, v = 0;
+    if (cudaGetDevice(&dev) == cudaSuccess && cudaDeviceGetAttribute(&v, cudaDevAttrMultiProcessorCount, dev) == cudaSuccess &&
+        v > 0)
+      n = v;
+    else
+      return 1;
+  }
+  return n;
+}
 
 int env_int(const char* name, int dflt) {
   const char* v = getenv(name);
@@ -89,17 +102,20 @@ int make_tmap_nhwc_bf16(CUtensorMap* out, const void* base, int C, int W, int H,
 
 extern "C" int dm_version() { return 2; }
 
+// n outside [8, SM count] (0 included) restores the default: one CTA per SM.
 extern "C" int dm_set_max_ctas(int n) {
-  dm::g_max_ctas = (n >= 8 && n <= 148) ? n : 148;
-  return dm::g_max_ctas;
+  dm::g_max_ctas = (n >= 8 && n <= dm::num_sms()) ? n : 0;
+  return dm::max_ctas();
 }
+
+extern "C" int dm_num_sms() { return dm::num_sms(); }
 
 extern "C" int dm_set_pdl(int on) {
   dm::g_pdl = on ? 1 : 0;
   return dm::g_pdl;
 }
 
-// Device query used by the Python side to fail loudly on non-Blackwell parts.
+// Device query used by the Python side to fail loudly on parts other than sm_90.
 extern "C" int dm_device_cc(int device) {
   cudaDeviceProp prop;
   if (cudaGetDeviceProperties(&prop, device) != cudaSuccess) return -1;

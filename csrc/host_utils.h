@@ -22,13 +22,18 @@ namespace dm {
 
 // Programmatic dependent launch (PDL): every kernel of the training step is launched with the
 // programmatic-stream-serialization attribute and executes `griddepcontrol.wait` after its private
-// prologue (barrier init, TMEM alloc, descriptor prefetch), so the next kernel's CTAs are resident and
-// set up while the previous kernel drains -- the ~2-3 us launch gap between the step's 11 dependent
+// prologue (barrier init, descriptor prefetch), so the next kernel's CTAs are resident and
+// set up while the previous kernel drains -- the launch gap between the step's 11 dependent
 // kernels disappears (also inside a captured CUDA graph: the edges become programmatic).
 extern int g_pdl;
-// Upper bound for the persistent kernels' grids (default 148 = one CTA per SM).  The bucketed aggregation lowers it
+// Upper bound for the persistent kernels' grids (0 = one CTA per SM).  The bucketed aggregation lowers it
 // for the backward kernels that run next to the early sync kernel, so those leave SMs free for it.
 extern int g_max_ctas;
+
+// Number of SMs of the current device (queried once per process).
+int num_sms();
+// Grid bound of the persistent kernels: g_max_ctas if set, else num_sms().
+inline int max_ctas() { return g_max_ctas > 0 ? g_max_ctas : num_sms(); }
 
 template <typename Kern, typename... Args>
 inline cudaError_t launch_kernel(Kern kern, dim3 grid, dim3 block, size_t smem, cudaStream_t st, Args... args) {

@@ -15,6 +15,12 @@
 
 namespace dm {
 
+// Two channels per call (the same rounding as one fmaf each): keeps the channel-pair register layout of the loops.
+DMNIST_DEVICE float2 fma2_rn(float2 a, float2 b, float2 c) {
+  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
+}
+
+
 // =====================================================================================================
 // conv1 forward, fused.  One CTA per (image, pair of pooled rows): 2 x 14 pooled positions x 32 channels.
 // Work item = (pooled position, group of 8 channels): 4 conv outputs x 8 channels x 25 taps = 800 FMA,
@@ -62,7 +68,7 @@ __global__ void __launch_bounds__(C1_THREADS) conv1_fwd_kernel(const float* __re
   const int cg = threadIdx.x & 3, pos = threadIdx.x >> 2;
   if (pos >= 28) return;
   const int pr = pos / 14, pc = pos - pr * 14;          // pooled row (local) / col
-  // packed fp32 FMA (FFMA2 on sm_100): two channels per instruction, input value broadcast to both halves
+  // channel pairs: input value broadcast to both halves
   float2 acc2[4][4];
 #pragma unroll
   for (int p = 0; p < 4; ++p)
@@ -86,10 +92,10 @@ __global__ void __launch_bounds__(C1_THREADS) conv1_fwd_kernel(const float* __re
       const float2 a10 = make_float2(r1[kw], r1[kw]), a11 = make_float2(r1[kw + 1], r1[kw + 1]);
 #pragma unroll
       for (int j = 0; j < 4; ++j) {
-        acc2[0][j] = __ffma2_rn(a00, wv[j], acc2[0][j]);
-        acc2[1][j] = __ffma2_rn(a01, wv[j], acc2[1][j]);
-        acc2[2][j] = __ffma2_rn(a10, wv[j], acc2[2][j]);
-        acc2[3][j] = __ffma2_rn(a11, wv[j], acc2[3][j]);
+        acc2[0][j] = fma2_rn(a00, wv[j], acc2[0][j]);
+        acc2[1][j] = fma2_rn(a01, wv[j], acc2[1][j]);
+        acc2[2][j] = fma2_rn(a10, wv[j], acc2[2][j]);
+        acc2[3][j] = fma2_rn(a11, wv[j], acc2[3][j]);
       }
     }
   }
@@ -122,8 +128,8 @@ __global__ void __launch_bounds__(C1_THREADS) conv1_fwd_kernel(const float* __re
 // conv1 forward, second generation.  Same CTA = (image, pair of pooled rows), but a thread owns TWO horizontally adjacent
 // pooled positions (2 x 4 conv outputs) x 8 channels: the ten 16-byte weight loads of a filter row now feed 160 packed
 // FMAs instead of 80 and the input window is four aligned 16-byte loads, so the loop is bound by the FMA pipe rather
-// than by shared-memory issue slots (ncu, profiles/ncu_lenet_step_r1_call18.txt: the first version sat at IPC 1.95 with
-// 22 % LSU + 23 % ALU instructions next to 28 % FMA).  64 threads: 56 work items = 2 rows x 7 column pairs x 4 groups.
+// than by shared-memory issue slots (the first version spent more instructions on loads and address arithmetic than
+// on FMAs).  64 threads: 56 work items = 2 rows x 7 column pairs x 4 groups.
 constexpr int C1B_THREADS = 64;
 
 __global__ void __launch_bounds__(C1B_THREADS) conv1_fwd2_kernel(const float* __restrict__ images,  // [B,28,28]
@@ -185,8 +191,8 @@ __global__ void __launch_bounds__(C1B_THREADS) conv1_fwd2_kernel(const float* __
         const float2 a0 = make_float2(r0[col + kw], r0[col + kw]), a1 = make_float2(r1[col + kw], r1[col + kw]);
 #pragma unroll
         for (int j = 0; j < 4; ++j) {
-          acc[col][j] = __ffma2_rn(a0, wv[j], acc[col][j]);
-          acc[4 + col][j] = __ffma2_rn(a1, wv[j], acc[4 + col][j]);
+          acc[col][j] = fma2_rn(a0, wv[j], acc[col][j]);
+          acc[4 + col][j] = fma2_rn(a1, wv[j], acc[4 + col][j]);
         }
       }
     }
@@ -258,6 +264,13 @@ struct Fc2Args {
   float keep_prob;
   float inv_batch;           // 1 / (rows that make up the mean)
 };
+
+// Per-row (loss, hit) terms, added up in row order by the last CTA (arrive_last_cta): the reported loss and accuracy do
+// not depend on the order in which the rows' CTAs finish.
+constexpr int F2_MAX_ROWS = 1 << 16;                      // batch limit of dm_fc2_fwd_bwd
+// One launch of this kernel in flight per device: the workspace and ticket are static (see arrive_last_cta).
+__device__ float g_f2_row_terms[F2_MAX_ROWS * 2];
+__device__ unsigned int g_f2_ticket;
 
 __global__ void __launch_bounds__(F2_THREADS) fc2_fwd_bwd_kernel(Fc2Args a) {
   __shared__ float s_part[F2_THREADS / 32][DL_LD];
@@ -331,11 +344,30 @@ __global__ void __launch_bounds__(F2_THREADS) fc2_fwd_bwd_kernel(Fc2Args a) {
     const unsigned hit = __ballot_sync(0xffffffffu, lane < NCLS && logit == m);
     const float l_label = __shfl_sync(0xffffffffu, logit, label);
     if (lane == 0) {
-      atomicAdd(a.loss_acc + 0, (__logf(ssum) - (l_label - m)) * a.inv_batch);
-      atomicAdd(a.loss_acc + 1, ((__ffs(hit) - 1) == label ? 1.f : 0.f) * a.inv_batch);
+      g_f2_row_terms[2 * row] = (__logf(ssum) - (l_label - m)) * a.inv_batch;
+      g_f2_row_terms[2 * row + 1] = ((__ffs(hit) - 1) == label ? 1.f : 0.f) * a.inv_batch;
     }
     if (a.logits_out && lane < NCLS) a.logits_out[(size_t)row * NCLS + lane] = logit;
     if (a.train && lane < DL_LD) a.dl_out[(size_t)row * DL_LD + lane] = dl_mine;
+  }
+  {
+    __shared__ unsigned int s_last;
+    if (arrive_last_cta(&g_f2_ticket, gridDim.x, 1, F2_THREADS, &s_last) && warp == 0) {
+      float l = 0.f, h = 0.f;
+      for (int r = lane; r < (int)gridDim.x; r += 32) {
+        l += __ldcg(g_f2_row_terms + 2 * r);
+        h += __ldcg(g_f2_row_terms + 2 * r + 1);
+      }
+#pragma unroll
+      for (int o = 16; o > 0; o >>= 1) {
+        l += __shfl_xor_sync(0xffffffffu, l, o);
+        h += __shfl_xor_sync(0xffffffffu, h, o);
+      }
+      if (lane == 0) {
+        a.loss_acc[0] += l;
+        a.loss_acc[1] += h;
+      }
+    }
   }
   if (!a.train) return;
   float d[4] = {0.f, 0.f, 0.f, 0.f};
@@ -584,7 +616,7 @@ int dm_conv1_fwd(const void* images, const void* w, const void* bias, void* out,
 int dm_fc2_fwd_bwd(const void* h_part, long long part_stride, int splits, const void* b1, const void* w2, const void* b2,
                    const void* labels, void* dh, void* scratch_h, void* scratch_dl, void* loss_acc, void* logits_out,
                    int B, int train, unsigned int seed_mix, const void* step_ptr, float keep_prob, void* stream) {
-  if (splits < 1 || splits > dm::F2_MAX_SPLITS || B < 1) return -1;
+  if (splits < 1 || splits > dm::F2_MAX_SPLITS || B < 1 || B > dm::F2_MAX_ROWS) return -1;
   dm::Fc2Args a;
   a.h_part = reinterpret_cast<const float*>(h_part);
   a.part_stride = part_stride;
@@ -629,7 +661,7 @@ int dm_fc2_wgrad(const void* scratch_h, const void* scratch_dl, const void* dh, 
 
 int dm_unpool2(const void* dpool, const void* code, void* dy, void* g_bias, int B, void* stream) {
   int grid = (B * 49 * 8 + 255) / 256;
-  if (grid > 148 * 2) grid = 148 * 2;
+  if (grid > dm::num_sms() * 2) grid = dm::num_sms() * 2;
   return (int)dm::launch_kernel(dm::unpool2_kernel, dim3(grid), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
       reinterpret_cast<const __nv_bfloat16*>(dpool), reinterpret_cast<const uint8_t*>(code),
       reinterpret_cast<__nv_bfloat16*>(dy), reinterpret_cast<float*>(g_bias), B);
@@ -638,7 +670,7 @@ int dm_unpool2(const void* dpool, const void* code, void* dy, void* g_bias, int 
 int dm_conv1_wgrad(const void* images, const void* dpool, const void* code, void* g_w, void* g_b, int B, void* stream) {
   // one image per CTA (37 KB smem, 57 regs: up to four CTAs share an SM): all B CTAs are resident at once, so the
   // staging latency of one overlaps the accumulation loop of its neighbours instead of serialising per image
-  int grid = B < 148 * 4 ? B : 148 * 4;
+  int grid = B < dm::num_sms() * 4 ? B : dm::num_sms() * 4;
   return (int)dm::launch_kernel(dm::conv1_wgrad_kernel, dim3(grid), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
       reinterpret_cast<const float*>(images), reinterpret_cast<const __nv_bfloat16*>(dpool),
       reinterpret_cast<const uint8_t*>(code), reinterpret_cast<float*>(g_w), reinterpret_cast<float*>(g_b), B);
@@ -646,7 +678,7 @@ int dm_conv1_wgrad(const void* images, const void* dpool, const void* code, void
 
 int dm_bias_relu_bf16(void* acc, const void* bias, void* out, int rows, int cols, int zero_acc, void* stream) {
   long long n = (long long)rows * cols;
-  int grid = (int)((n + 255) / 256 < 148 * 8 ? (n + 255) / 256 : 148 * 8);
+  int grid = (int)((n + 255) / 256 < dm::num_sms() * 8 ? (n + 255) / 256 : dm::num_sms() * 8);
   dm::bias_relu_bf16_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
       reinterpret_cast<float*>(acc), reinterpret_cast<const float*>(bias), reinterpret_cast<__nv_bfloat16*>(out), rows,
       cols, zero_acc);

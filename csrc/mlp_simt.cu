@@ -1,5 +1,5 @@
 // SIMT kernels of the MLP models (BASELINE.json configs: 2-layer plumbing MLP, 3-layer MLP at batch
-// 8192/replica).  Hidden layers run on the tcgen05 GEMM (csrc/gemm_tc.cu, bias+ReLU fused in its
+// 8192/replica).  Hidden layers run on the wgmma GEMM (csrc/gemm_tc.cu, bias+ReLU fused in its
 // epilogue); what is left for CUDA cores:
 //   dense10_xent     last layer (H -> 10, too narrow for a TMA/UMMA operand: 20-byte rows) + softmax-CE +
 //                    accuracy, and backward to d(hidden) with the ReLU mask applied; the output-layer
@@ -13,7 +13,7 @@ namespace dm {
 
 constexpr int XN = 10;            // classes
 constexpr int XN_PAD = 64;        // dl is also written as a zero-padded [B,64] bf16 matrix: the B operand
-                                  // of the tcgen05 GEMM that forms the output-layer weight gradient
+                                  // of the wgmma GEMM that forms the output-layer weight gradient
 constexpr int X_WARPS = 8;
 
 struct XentArgs {
@@ -168,7 +168,7 @@ int dm_dense10_xent(const void* h, const void* w, const void* b, const void* lab
   if (smem > 220 * 1024) return -2;
   DM_CUDA_OK(cudaFuncSetAttribute(dense10_xent_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, smem));
   int grid = (B + X_WARPS - 1) / X_WARPS;
-  if (grid > 148) grid = 148;
+  if (grid > dm::num_sms()) grid = dm::num_sms();
   dense10_xent_kernel<<<grid, X_WARPS * 32, smem, reinterpret_cast<cudaStream_t>(stream)>>>(a);
   return (int)cudaGetLastError();
 }

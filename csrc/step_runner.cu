@@ -1,6 +1,6 @@
 // Native step executor: the per-step host work of the training loop -- wait for the input slot, DMA the packed batch, chain
 // the events, launch the step's CUDA graph, record completion -- as ONE C call instead of ~8 Python-dispatched torch calls
-// (≈ 45 us of interpreter time per step, comparable to the 70 us step itself).  The reference's equivalent layer is the TF
+// (interpreter time per step comparable to the step itself).  The reference's equivalent layer is the TF
 // session runtime driving `sess.run(train_op, feed_dict)` (src/distributed_train.py:309-335); here the device work is a
 // pre-instantiated cudaGraphExec_t per input slot and the host's job is six driver calls.
 #include <stdint.h>

@@ -12,8 +12,8 @@ both live in NVLink-symmetric memory) and exposes four calls:
 
 :class:`TorchEngine` is the plain-PyTorch implementation: the execution path on
 CPU (gloo plumbing config) and the cuDNN/cuBLAS *baseline* on GPU.  The product
-path on B200 is ``CudaLeNetEngine`` / ``CudaMlpEngine`` in ``engine_cuda.py``
-(hand-written sm_100a kernels).  Unlike the reference, loss and accuracy come
+path on H100 is ``CudaLeNetEngine`` / ``CudaMlpEngine`` in ``engine_cuda.py``
+(hand-written sm_90a kernels).  Unlike the reference, loss and accuracy come
 from the training forward itself -- the reference runs a second forward per
 iteration only for logging (src/distributed_train.py:334; SURVEY §5.9 item 6).
 """
@@ -52,7 +52,7 @@ class ComputeEngine:
     # ---- packed batches: one contiguous buffer per step (fp32 images [B,784] then int64 labels [B]) -----------------
     def pack_batch(self, images, labels, pin: bool = True) -> torch.Tensor:
         """Input pipelines fill one (page-locked) buffer per batch; ``load_packed`` then moves it with a single copy
-        (the sm_100a engines keep images and labels of a slot in one device allocation for exactly this)."""
+        (the sm_90a engines keep images and labels of a slot in one device allocation for exactly this)."""
         B = self.batch_size
         buf = torch.empty(B * 784 * 4 + B * 8, dtype=torch.uint8)
         if pin and torch.cuda.is_available():
@@ -135,7 +135,7 @@ class TorchEngine(ComputeEngine):
 
 
 def make_engine(flags, ctx, backend, force_torch: bool = False) -> ComputeEngine:
-    """GPU -> hand-written sm_100a engine (fails loudly if the extension is absent);
+    """GPU -> hand-written sm_90a engine (fails loudly if the extension is absent);
     CPU -> torch engine."""
     if ctx.on_gpu and not force_torch and flags.backend in ("auto", "fused"):
         from .engine_cuda import make_cuda_engine

@@ -1,20 +1,20 @@
-"""sm_100a compute engine: the reference convnet's training step as 11 hand-written kernels
+"""sm_90a compute engine: the reference convnet's training step as 11 hand-written kernels
 replayed from one CUDA graph.
 
 Step = (reference src/distributed_train.py:332 ``sess.run(apply_gradients_op)``)::
 
     memset(small grads, loss)                              2 memset nodes
     conv1_fwd        conv+bias+ReLU+pool (SIMT, K=25)       csrc/lenet_simt.cu
-    conv2_fwd        tcgen05 implicit GEMM + bias/ReLU/pool csrc/conv2_tc.cu
-    fc1_fwd          tcgen05 GEMM, split-K into fp32        csrc/gemm_tc.cu
+    conv2_fwd        wgmma implicit GEMM + bias/ReLU/pool csrc/conv2_tc.cu
+    fc1_fwd          wgmma GEMM, split-K into fp32        csrc/gemm_tc.cu
     fc2_fwd_bwd      bias+ReLU+dropout, fc2, softmax-CE,
                      accuracy, dlogits, d(fc1)              csrc/lenet_simt.cu
     fc2_wgrad        fc2 weight/bias + fc1 bias gradients   (side branch)
-    fc1_wgrad        tcgen05 GEMM (MN-major x MN-major) -> gradient arena
-    fc1_dgrad        tcgen05 GEMM -> bf16
+    fc1_wgrad        wgmma GEMM (MN-major x MN-major) -> gradient arena
+    fc1_dgrad        wgmma GEMM -> bf16
     unpool2          maxpool2/ReLU2 backward + conv2 bias grad
-    conv2_wgrad      tcgen05, K = pixels, fp32 atomics -> gradient arena
-    conv2_dgrad      tcgen05
+    conv2_wgrad      wgmma, K = pixels, fp32 atomics -> gradient arena
+    conv2_dgrad      wgmma
     conv1_wgrad      maxpool1/ReLU1 backward + conv1 weight/bias grad
     fused_sync_sgd   arrival -> mask -> NVLink reduce -> 1/count -> SGD -> push -> bf16 shadow
 
@@ -110,7 +110,7 @@ class CudaLeNetEngine(ComputeEngine):
         self._wgrad_late = os.environ.get("DMNIST_WGRAD_LATE", "1") != "0"
         self._branches = os.environ.get("DMNIST_BRANCHES", "1") != "0"
         self._fuse_unpool = os.environ.get("DMNIST_FUSE_UNPOOL", "1") != "0"
-        self._conv1_tc = os.environ.get("DMNIST_CONV1_TC", "1") != "0"    # conv1 fwd / wgrad on tcgen05 (csrc/conv1_tc.cu)
+        self._conv1_tc = os.environ.get("DMNIST_CONV1_TC", "1") != "0"    # conv1 fwd / wgrad on wgmma (csrc/conv1_tc.cu)
         self._copy_done = [torch.cuda.Event() for _ in range(2)]
         self._slot_free = [torch.cuda.Event() for _ in range(2)]
         self._graphs = [None, None]
@@ -266,13 +266,13 @@ class CudaLeNetEngine(ComputeEngine):
             n_late = self.spec.arena_numel - (e1 - e0)
             self._inbox = self.backend.allocate_buffer(2 * n * n_late * 8) if n > 1 else None   # LL lines: 8 bytes per float
         # early-bucket grid: the CTAs share SMs with the tensor-core kernels of the backward pass and every one of them fences
-        # at system scope once; measured at N = 4 (profiles/r2/bench_call12_4gpu.txt): 296 CTAs 90.8, 148 CTAs 85.8, 74 CTAs
-        # 82.5 us/step -- half the SMs carry the exchange, the kernel still ends before the backward pass does
-        self._early_ctas = int(os.environ.get("DMNIST_EARLY_CTAS", "0")) or (74 if n > 1 else 148)
+        # at system scope once, so with several replicas half the SMs carry the exchange
+        sms = int(self.lib.dm_num_sms())
+        self._early_ctas = int(os.environ.get("DMNIST_EARLY_CTAS", "0")) or (sms // 2 if n > 1 else sms)
         torch.cuda.synchronize()
         self._seq0 = self.backend.status_seq       # steps closed on this control block before the engine's first one
         self._steps_launched = 0
-        self.lib.dm_set_max_ctas(int(os.environ.get("DMNIST_MAX_CTAS", "148")))
+        self.lib.dm_set_max_ctas(int(os.environ.get("DMNIST_MAX_CTAS", "0")))
 
     def params_updated(self) -> None:
         """Parameters were written from the host (init / restore): refresh the bf16 shadow."""
@@ -615,8 +615,8 @@ class CudaLeNetEngine(ComputeEngine):
 
 
 class CudaMlpEngine(ComputeEngine):
-    """2-/3-layer MLP on the sm_100a kernels: hidden layers = tcgen05 GEMM with bias+ReLU fused in the
-    epilogue, output layer + softmax-CE = SIMT (csrc/mlp_simt.cu), every weight gradient = tcgen05 GEMM
+    """2-/3-layer MLP on the sm_90a kernels: hidden layers = wgmma GEMM with bias+ReLU fused in the
+    epilogue, output layer + softmax-CE = SIMT (csrc/mlp_simt.cu), every weight gradient = wgmma GEMM
     with MN-major operands writing straight into the gradient arena."""
 
     def __init__(self, model: str, batch_size: int, backend: FusedBackend, hidden: int = 1024, seed: int = 66478,
@@ -835,7 +835,7 @@ class CudaMlpEngine(ComputeEngine):
 
 def make_cuda_engine(flags, ctx, backend) -> ComputeEngine:
     if not isinstance(backend, FusedBackend):
-        raise RuntimeError("the sm_100a engine needs the fused backend")
+        raise RuntimeError("the sm_90a engine needs the fused backend")
     if flags.model == "lenet":
         return CudaLeNetEngine(flags.batch_size, backend, seed=flags.seed, rank=ctx.rank,
                                keep_prob=flags.dropout_keep_prob, use_graph=flags.use_cuda_graph)

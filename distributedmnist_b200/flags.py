@@ -7,7 +7,7 @@ src/sync_replicas_optimizer_modified/sync_replicas_optimizer_modified.py:38).
 Here every flag lives in one registry with the *same names and defaults*, so
 command lines written for the reference keep working, plus a small set of new
 flags (model choice, synthetic data, straggler injection, backend selection)
-that the single-box B200 design needs.
+that the single-box H100 design needs.
 
 Accepted syntaxes (same as absl): ``--name=value``, ``--name value``,
 ``--flag`` / ``--noflag`` for booleans, and ``true/false/1/0/yes/no/t/f`` as
@@ -201,7 +201,7 @@ def define_reference_flags(F: FlagValues = FLAGS) -> FlagValues:
     # reference: src/distributed_train.py:40-48
     F.DEFINE_string("job_name", "", 'One of "ps", "worker"')
     F.DEFINE_string("ps_hosts", "", "Comma-separated hostname:port list of parameter servers (accepted for "
-                    "compatibility; the B200 engine has no parameter server)")
+                    "compatibility; the H100 engine has no parameter server)")
     F.DEFINE_string("worker_hosts", "", "Comma-separated hostname:port list of workers; its length is the "
                     "number of replicas when WORLD_SIZE is not set")
     # reference: src/distributed_train.py:50-63
@@ -216,7 +216,7 @@ def define_reference_flags(F: FlagValues = FLAGS) -> FlagValues:
     # reference: src/distributed_train.py:68-78
     F.DEFINE_integer("task_id", 0, "Replica index; replica 0 is the chief")
     F.DEFINE_integer("num_replicas_to_aggregate", -1, "Gradients to collect before updating (K of N); -1 = all")
-    F.DEFINE_float("save_interval_secs", 20, "Checkpoint interval in seconds (chief); fractions allowed: a B200 step is ~0.1 ms")
+    F.DEFINE_float("save_interval_secs", 20, "Checkpoint interval in seconds (chief); fractions allowed: an H100 step takes ~0.15 ms")
     F.DEFINE_integer("save_summaries_secs", 300, "Summary interval in seconds (chief)")
     # reference: src/distributed_train.py:92-98
     F.DEFINE_float("initial_learning_rate", 0.1, "Initial learning rate")
@@ -234,7 +234,7 @@ def define_reference_flags(F: FlagValues = FLAGS) -> FlagValues:
 
 
 def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
-    """New flags of the B200 engine (no analogue in the reference)."""
+    """New flags of the H100 engine (no analogue in the reference)."""
     F.DEFINE_string("model", "lenet", "lenet | mlp2 | mlp3")
     F.DEFINE_integer("mlp_hidden", 1024, "Hidden width of the MLP models")
     F.DEFINE_string("data_dir", "MNIST-data", "Directory with the four MNIST IDX .gz files (never downloaded)")
@@ -242,7 +242,7 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_boolean("fake_data", False, "Constant all-ones images / label 0 (reference mnist_data.py fake_data)")
     F.DEFINE_integer("seed", 66478, "Base RNG seed (per-replica streams are derived from it)")
     F.DEFINE_string("compute_dtype", "bf16", "bf16 | fp32 (activations / tensor-core operand type)")
-    F.DEFINE_string("backend", "auto", "auto | fused (sm_100a kernels + symmetric memory) | nccl | gloo")
+    F.DEFINE_string("backend", "auto", "auto | fused (sm_90a kernels + symmetric memory) | nccl | gloo")
     F.DEFINE_string("inject_straggler", "", "rank:prob:usec[,rank:prob:usec...] device-side delay injection")
     F.DEFINE_integer("sync_timeout_ms", 30000, "Watchdog for device-side arrival polling")
     F.DEFINE_boolean("use_cuda_graph", True, "Capture the training step in a CUDA graph")

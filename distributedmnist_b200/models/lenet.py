@@ -8,7 +8,7 @@ mean top-1 hit (:161-164).
 
 This module holds (a) the parameter inventory and (b) a plain-PyTorch fp32
 forward used as the CPU execution path and as the numerics reference for the
-sm_100a kernels (``emulate_bf16=True`` rounds weights/activations to bf16 at the
+sm_90a kernels (``emulate_bf16=True`` rounds weights/activations to bf16 at the
 points where the CUDA pipeline does, so comparisons can be tight).
 """
 from __future__ import annotations
@@ -84,7 +84,7 @@ def lenet_forward(p: Dict[str, torch.Tensor], images: torch.Tensor, train: bool 
     """Logits ``[B, 10]`` from NHWC fp32 images ``[B, 28, 28, 1]``.
 
     ``p`` maps parameter names to tensors in TF layout (HWIO / [in, out]).  ``conv1_bf16`` (default: same as
-    ``emulate_bf16``) rounds the conv1 operands too -- the tcgen05 conv1 (csrc/conv1_tc.cu) does, the SIMT one does not.
+    ``emulate_bf16``) rounds the conv1 operands too -- the wgmma conv1 (csrc/conv1_tc.cu) does, the SIMT one does not.
     """
     q = emulate_bf16
     q1 = q if conv1_bf16 is None else conv1_bf16

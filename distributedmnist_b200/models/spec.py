@@ -13,7 +13,7 @@ matters twice:
   differ, sync_replicas_optimizer_modified.py:289-306).
 
 Tensor layouts inside the arena are exactly the TF layouts (conv HWIO, fc
-``[in, out]``): the tcgen05 kernels consume them natively through K-major /
+``[in, out]``): the wgmma kernels consume them natively through K-major /
 MN-major shared-memory descriptors, so checkpoints need no transposition.
 """
 from __future__ import annotations

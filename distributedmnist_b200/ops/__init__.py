@@ -1,1 +1,1 @@
-"""Hand-written sm_100a operators (ctypes bindings over csrc/)."""
+"""Hand-written sm_90a operators (ctypes bindings over csrc/)."""

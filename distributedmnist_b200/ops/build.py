@@ -1,6 +1,6 @@
-"""In-tree build of the sm_100a kernel library (``distributedmnist_b200/lib/libdmnist_b200.so``).
+"""In-tree build of the sm_90a kernel library (``distributedmnist_b200/lib/libdmnist_b200.so``).
 
-``nvcc -gencode arch=compute_100a,code=sm_100a -lineinfo`` per ``csrc/*.cu`` (in
+``nvcc -gencode arch=compute_90a,code=sm_90a -lineinfo`` per ``csrc/*.cu`` (in
 parallel), then one link.  No torch headers are involved: the library exposes a
 plain C ABI that takes raw device pointers and a stream handle, and Python calls
 it through ``ctypes`` -- so each translation unit compiles in seconds and the
@@ -25,7 +25,7 @@ LIB_PATH = os.path.join(LIB_DIR, "libdmnist_b200.so")
 STAMP = os.path.join(LIB_DIR, "libdmnist_b200.stamp")
 
 NVCC = os.environ.get("NVCC", "/usr/local/cuda/bin/nvcc")
-ARCH_FLAGS = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH_FLAGS = ["-gencode", "arch=compute_90a,code=sm_90a"]
 NVCC_FLAGS = ["-O3", "-std=c++17", "-lineinfo", "--use_fast_math", "-Xcompiler", "-fPIC", "-Xcompiler", "-O3",
               "--expt-relaxed-constexpr", "-Xptxas", "-v"]
 
@@ -71,7 +71,7 @@ def build(force: bool = False, verbose: bool = True) -> str:
     os.makedirs(LIB_DIR, exist_ok=True)
     srcs = sources()
     if verbose:
-        print("[dmnist build] nvcc sm_100a: %d sources" % len(srcs), file=sys.stderr)
+        print("[dmnist build] nvcc sm_90a: %d sources" % len(srcs), file=sys.stderr)
     with ThreadPoolExecutor(max_workers=min(8, len(srcs))) as ex:
         objs = list(ex.map(_compile, srcs))
     cmd = [NVCC] + ARCH_FLAGS + ["-shared", "-o", LIB_PATH] + objs + ["-cudart", "static", "-lrt", "-lpthread", "-ldl"]
@@ -90,7 +90,7 @@ PROBE_LIB_PATH = os.path.join(LIB_DIR, "libdmnist_probes.so")
 
 
 def build_probes() -> str:
-    """Bring-up probes (csrc/probes/*.cu: UMMA descriptor row-shift probe, SM co-residency probe) as their OWN library --
+    """Bring-up probes (csrc/probes/*.cu: SM co-residency probe) as their OWN library --
     they are measurement tools, not part of the product ``libdmnist_b200.so``."""
     os.makedirs(OBJ_DIR, exist_ok=True)
     os.makedirs(LIB_DIR, exist_ok=True)

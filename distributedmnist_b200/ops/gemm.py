@@ -1,4 +1,4 @@
-"""tcgen05 GEMM (csrc/gemm_tc.cu) -- Python entry points.
+"""wgmma GEMM (csrc/gemm_tc.cu) -- Python entry points.
 
 ``gemm_bf16(a, b, a_major, b_major)`` multiplies without ever materialising a
 transpose: ``a_major="k"`` means ``a`` is ``[M, K]`` row-major, ``"mn"`` means it is

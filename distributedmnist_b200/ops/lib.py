@@ -1,9 +1,8 @@
-"""ctypes loader for the sm_100a kernel library.
+"""ctypes loader for the sm_90a kernel library.
 
 The library is built in-tree by ``ops/build.py``.  On a box with a GPU a missing
 or unloadable library is a hard error -- the CUDA path never silently falls back
-to PyTorch ops (the driver records which ``.so`` files the test/bench processes
-loaded).
+to PyTorch ops.
 """
 from __future__ import annotations
 
@@ -52,7 +51,8 @@ def stream_ptr(stream: Optional[torch.cuda.Stream] = None) -> ctypes.c_void_p:
     return ctypes.c_void_p(s.cuda_stream)
 
 
-def require_blackwell(device: torch.device) -> None:
+def require_hopper(device: torch.device) -> None:
+    """The library holds sm_90a code only (wgmma, TMA): it loads on nothing but a compute capability 9.0 device."""
     cc = load().dm_device_cc(device.index or 0)
-    if cc < 100:
-        raise KernelLibraryError("device %s has compute capability %d; this library is sm_100a-only" % (device, cc))
+    if cc != 90:
+        raise KernelLibraryError("device %s has compute capability %d; this library is sm_90a-only" % (device, cc))

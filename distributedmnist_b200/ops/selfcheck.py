@@ -1,4 +1,4 @@
-"""Numerics self-checks of the sm_100a LeNet kernels against plain PyTorch fp32 references.
+"""Numerics self-checks of the sm_90a LeNet kernels against plain PyTorch fp32 references.
 
 Each check returns ``(name, error, tolerance)``; ``tests/test_lenet_kernels_gpu.py``
 asserts on them and ``tools/gpu_diag_lenet.py`` prints them all (one GPU call gives the
@@ -69,7 +69,7 @@ def check_conv1_fwd_tc(B: int = 8, seed: int = 0) -> List[Result]:
 
 
 def check_conv1_wgrad(B: int = 8, seed: int = 7, tc: bool = True) -> List[Result]:
-    """conv1 weight/bias gradient fused with the maxpool1/ReLU1 backward (SIMT and tcgen05 versions)."""
+    """conv1 weight/bias gradient fused with the maxpool1/ReLU1 backward (SIMT and wgmma versions)."""
     lib, dev = load(), "cuda"
     g = torch.Generator(device="cpu").manual_seed(seed)
     x = (torch.rand(B, 28, 28, generator=g) - 0.5).to(dev)
@@ -214,9 +214,8 @@ def _engine(B: int, seed: int = 5):
 # Per-tensor L2 bound of (gradients of the bf16-operand tensor-core step) vs (gradients of a PLAIN fp32 model, TF32 off).
 # This is not a kernel-accuracy figure -- against the bf16-emulating reference every tensor agrees to <= 0.44 % (above) -- but
 # the distance between bf16 and fp32 *training arithmetic*: activations rounded to bf16 flip ReLU / max-pool decisions, and the
-# flips accumulate towards the input.  Measured on B200 (B = 64, seed 5; profiles/r2/): conv1_w 9.6 %, conv1_b 4.0 %,
-# conv2_w 4.9 %, conv2_b 3.8 %, fc1_w 3.5 %, fc1_b 3.5 %, fc2_w 0.47 %, fc2_b 0.36 %.  Bounds = ~3x those: a wrong tap, a
-# transposed tile or a dropped bias shows up as O(1).
+# flips accumulate towards the input, so the bounds grow towards conv1 (several percent there, well under 1 % at fc2).
+# A wrong tap, a transposed tile or a dropped bias shows up as O(1).
 FP32_GRAD_TOLS = {"conv1_weights": 0.30, "conv1_biases": 0.15, "conv2_weights": 0.15, "conv2_biases": 0.15,
                   "fc1_weights": 0.12, "fc1_biases": 0.12, "fc2_weights": 0.03, "fc2_biases": 0.03}
 
@@ -244,7 +243,7 @@ def check_end_to_end(B: int = 64, seed: int = 5) -> List[Result]:
     gv, rv = spec.views(eng.grads), spec.views(flat.grad)
     for name in rv:
         scale = rv[name].abs().max().item() + 1e-8
-        # measured on B200: <= 0.0044 for every tensor (profiles/r2); a wrong tap / transposed tile shows up as O(1)
+        # a wrong tap / transposed tile shows up as O(1)
         out.append(("e2e.grad.%s(rel)" % name, (gv[name] - rv[name]).abs().max().item() / scale, 0.02))
     # the same gradients against a PLAIN fp32 reference (no bf16 emulation anywhere): the remaining difference is the bf16
     # rounding of the tensor-core operands, bounded per tensor in the L2 norm

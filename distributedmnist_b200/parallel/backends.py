@@ -10,7 +10,7 @@ The *policy* (K-of-N / full barrier / interval, SURVEY §2.3) lives in
 * :class:`NcclBackend`   -- GPU, ``ncclAllReduce`` + separate scale + SGD
   kernels.  **Baseline only** (what a stock framework does); never the product
   path.
-* ``FusedBackend`` (``fused.py``) -- the product path: one sm_100a kernel that
+* ``FusedBackend`` (``fused.py``) -- the product path: one sm_90a kernel that
   publishes arrival, polls the commit word, reduces over NVLink peer/multicast
   memory, scales by 1/count and applies SGD (no NCCL call, no separate
   elementwise kernel).
@@ -180,7 +180,7 @@ def make_backend(ctx: ReplicaContext, choice: str = "auto", flags=None) -> Backe
     if choice == "nccl":
         return NcclBackend(ctx) if ctx.world_size > 1 else LocalBackend(ctx)
     if choice == "fused":
-        from .fused import FusedBackend  # imports the sm_100a extension; fails loudly if missing
+        from .fused import FusedBackend  # imports the sm_90a extension; fails loudly if missing
         kw = {}
         if flags is not None:
             kw = dict(timeout_ms=float(getattr(flags, "sync_timeout_ms", 30000)),

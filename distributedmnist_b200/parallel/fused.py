@@ -1,4 +1,4 @@
-"""FusedBackend: gradient aggregation by the single sm_100a kernel of ``csrc/fused_sync.cu``.
+"""FusedBackend: gradient aggregation by the single sm_90a kernel of ``csrc/fused_sync.cu``.
 
 The product path for SURVEY §2.5 X1-X8: the parameter arena, the gradient arena and a
 control block live in symmetric memory; one kernel per step publishes arrival, obtains
@@ -23,7 +23,7 @@ from typing import Dict, List, Optional
 
 import torch
 
-from ..ops.lib import check, load, require_blackwell, stream_ptr
+from ..ops.lib import check, load, require_hopper, stream_ptr
 from .backends import Backend, StepInfo
 from .context import ReplicaContext
 from .symm_mem import SymmetricBuffer, allocate_symmetric
@@ -38,14 +38,14 @@ class FusedBackend(Backend):
         super().__init__(ctx)
         assert ctx.on_gpu, "FusedBackend needs a GPU"
         self.lib = load()
-        require_blackwell(ctx.device)
+        require_hopper(ctx.device)
         check(self.lib.dm_set_device(ctx.device.index or 0), "dm_set_device")
         # programmatic dependent launch between the kernels of a step (DMNIST_PDL=0 disables)
         self.lib.dm_set_pdl(0 if os.environ.get("DMNIST_PDL", "1") == "0" else 1)
-        self.ctas = ctas or int(os.environ.get("DMNIST_SYNC_CTAS", "148"))
+        self.ctas = ctas or int(os.environ.get("DMNIST_SYNC_CTAS", "0")) or int(self.lib.dm_num_sms())
         # NVLS (in-switch reduction + multicast store) for the arenas when the fabric offers it; DMNIST_NVLS=0 -> P2P only
-        #   DMNIST_NVLS unset: allocate multicast-capable arenas, use multimem from 4 replicas up (at 2 the peer path is
-        #   faster: measured 106 vs 115 us/step, profiles/bench_r1_call23_2gpu.txt); =1 always; =0 never (CUDA-IPC arenas)
+        #   DMNIST_NVLS unset: allocate multicast-capable arenas, use multimem from 4 replicas up (at 2 the peer path
+        #   moves fewer bytes per replica); =1 always; =0 never (CUDA-IPC arenas)
         #   (--use_nvls=false forces the P2P kernels and CUDA-IPC arenas, like DMNIST_NVLS=0)
         nv = os.environ.get("DMNIST_NVLS", "") if use_nvls is None else ("1" if use_nvls else "0")
         self.want_nvls = nv != "0"

@@ -4,7 +4,7 @@ Command-line compatible with the reference's src/mnist_distributed_train.py:15-4
 (``--job_name --task_id --ps_hosts --worker_hosts --train_dir ...``).  Under
 ``torchrun`` the rank/world come from the environment; with the reference's own
 flags the replica count is ``len(worker_hosts)`` and the rank is ``--task_id``.
-A ``--job_name=ps`` process has nothing to serve (the B200 engine keeps weights
+A ``--job_name=ps`` process has nothing to serve (the H100 engine keeps weights
 replicated in HBM and aggregates over NVLink), so it logs that and exits 0.
 """
 import _bootstrap  # noqa: F401

@@ -1,4 +1,4 @@
-"""Helper process: a few LeNet training steps on the sm_100a engine, aggregation = bucketed (overlapped) or single kernel.
+"""Helper process: a few LeNet training steps on the sm_90a engine, aggregation = bucketed (overlapped) or single kernel.
 
 argv: <out json with RANK placeholder> <steps>.  DMNIST_BUCKET / DMNIST_NVLS select the path."""
 import hashlib

@@ -1,4 +1,4 @@
-"""tcgen05 GEMM vs a plain PyTorch fp32 reference of the same op (SURVEY §4 item 2)."""
+"""wgmma GEMM vs a plain PyTorch fp32 reference of the same op (SURVEY §4 item 2)."""
 import pytest
 import torch
 

@@ -1,4 +1,4 @@
-"""sm_100a LeNet kernels vs plain PyTorch fp32 references (SURVEY §4 item 2)."""
+"""sm_90a LeNet kernels vs plain PyTorch fp32 references (SURVEY §4 item 2)."""
 import pytest
 
 pytestmark = pytest.mark.gpu
@@ -19,7 +19,7 @@ def test_conv1_fwd_fused_bias_relu_pool():
 def test_conv1_fwd_tcgen05_software_im2col():
     _run("check_conv1_fwd_tc")
     _run("check_conv1_fwd_tc", B=3, seed=9)        # one partial tile
-    _run("check_conv1_fwd_tc", B=150, seed=19)     # 230 tiles > 148 CTAs: two-stage operand ring + TMEM double buffering
+    _run("check_conv1_fwd_tc", B=150, seed=19)     # 230 tiles > one CTA per SM: persistent loop over the two-stage operand ring
 
 
 def test_conv1_wgrad_tcgen05_and_simt():
@@ -30,7 +30,7 @@ def test_conv1_wgrad_tcgen05_and_simt():
 
 def test_conv2_fwd_tcgen05_implicit_gemm():
     _run("check_conv2_fwd")
-    _run("check_conv2_fwd", B=75, seed=10)     # 150 tiles > 148 CTAs: persistent loop + TMEM double buffering
+    _run("check_conv2_fwd", B=75, seed=10)     # 150 tiles > one CTA per SM: persistent loop over the TMA stage ring
 
 
 def test_conv2_dgrad_tcgen05():

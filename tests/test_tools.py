@@ -177,11 +177,11 @@ def test_ptxas_report_parses_resource_lines(tmp_path):
     log = tmp_path / "k.log"
     log.write_text(
         "nvcc ...\n"
-        "ptxas info    : Compiling entry function '_ZN2dm6kernelEv' for 'sm_100a'\n"
+        "ptxas info    : Compiling entry function '_ZN2dm6kernelEv' for 'sm_90a'\n"
         "ptxas info    : Function properties for _ZN2dm6kernelEv\n"
         "    24 bytes stack frame, 44 bytes spill stores, 48 bytes spill loads\n"
         "ptxas info    : Used 128 registers, used 1 barriers, 16 bytes smem\n"
-        "ptxas info    : Compiling entry function '_ZN2dm5otherEv' for 'sm_100a'\n"
+        "ptxas info    : Compiling entry function '_ZN2dm5otherEv' for 'sm_90a'\n"
         "    0 bytes stack frame, 0 bytes spill stores, 0 bytes spill loads\n"
         "ptxas info    : Used 40 registers\n")
     rows = mod.parse(str(log))

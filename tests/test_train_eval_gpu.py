@@ -1,4 +1,4 @@
-"""End-to-end on one GPU: reference-compatible entrypoints train the convnet with the sm_100a engine,
+"""End-to-end on one GPU: reference-compatible entrypoints train the convnet with the sm_90a engine,
 checkpoint in the reference's layout, and the evaluator scores it (SURVEY §4 item 5)."""
 import os
 import re

@@ -3,8 +3,8 @@
 
 BASELINE.json config 5 ("gradient-allreduce bandwidth sweep 4 KB-256 MB at 2/4/8 GPUs vs NCCL").  Run under
 torchrun (one rank per GPU).  Device-timed with CUDA events, max over ranks.  Bus bandwidth uses the standard
-allreduce convention 2*(N-1)/N * bytes / time so both arms are comparable with the 900 GB/s (nominal) /
-770 GB/s (measured peer copy) per-direction NVLink figures.
+allreduce convention 2*(N-1)/N * bytes / time so both arms are comparable with the nominal per-direction NVLink
+bandwidth of the box (H100 SXM, NVLink 4: 450 GB/s).
 """
 import json
 import os
@@ -69,8 +69,8 @@ def main():
     be.check_error()
     if ctx.rank == 0:
         print(json.dumps({"n_gpus": n, "rows": rows}))
-        os.makedirs("gpurun_out", exist_ok=True)
-        with open("gpurun_out/allreduce_sweep_n%d_nvls%s.json" % (n, os.environ.get("DMNIST_NVLS", "auto")), "w") as f:
+        os.makedirs("results", exist_ok=True)
+        with open("results/allreduce_sweep_n%d_nvls%s.json" % (n, os.environ.get("DMNIST_NVLS", "auto")), "w") as f:
             json.dump({"n_gpus": n, "rows": rows}, f, indent=1)
     be.close()
     shutdown_context(ctx)

@@ -8,7 +8,7 @@ reference: tools/benchmark.py --
 ``time_step.png``, ``time_precision.png``, ``step_losses.png``, ``time_cdfs.png`` and the percentile
 report (:60-111, 165-263), ``plot_figs`` (:265-279) and the ``use_dir`` / ``select_files`` CLI (:281-292).
 Differences: the fleet is one box (tools/cluster.py), polling is every second instead of every 60 s
-(a 300-step run takes seconds on B200, not minutes), figures are written by a dependency-free
+(a 300-step run takes seconds on H100, not minutes), figures are written by a dependency-free
 rasteriser when matplotlib is absent, and the time-CDF plot is enabled.
 """
 from __future__ import annotations

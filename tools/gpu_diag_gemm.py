@@ -1,5 +1,5 @@
-"""GPU diagnostic: run every GEMM layout combination and print error structure.
-Used while bringing up the UMMA descriptors (writes gpurun_out/gemm_diag.txt)."""
+"""GPU diagnostic: run every GEMM layout combination and print error structure (rows / columns with large errors point
+at a wrong shared-memory descriptor or swizzle).  Also writes results/gemm_diag.txt."""
 import os
 import sys
 
@@ -10,12 +10,12 @@ from distributedmnist_b200.ops.gemm import gemm_bf16  # noqa: E402
 
 
 def main():
-    os.makedirs("gpurun_out", exist_ok=True)
+    os.makedirs("results", exist_ok=True)
     lines = []
     torch.manual_seed(0)
     for a_major in ("k", "mn"):
         for b_major in ("k", "mn"):
-            for bn in (64, 128):
+            for bn in (64, 128, 256):
                 for (M, N, K) in [(128, 128, 64), (128, 128, 256), (256, 256, 128), (200, 72, 784)]:
                     a = (torch.randn((K, M) if a_major == "mn" else (M, K), device="cuda") * 0.5).to(torch.bfloat16)
                     b = (torch.randn((K, N) if b_major == "mn" else (N, K), device="cuda") * 0.5).to(torch.bfloat16)
@@ -37,7 +37,7 @@ def main():
                         int(torch.isnan(out).sum())))
     txt = "\n".join(lines)
     print(txt)
-    open("gpurun_out/gemm_diag.txt", "w").write(txt + "\n")
+    open("results/gemm_diag.txt", "w").write(txt + "\n")
 
 
 if __name__ == "__main__":

@@ -10,7 +10,7 @@ from distributedmnist_b200.ops import selfcheck  # noqa: E402
 
 
 def main():
-    os.makedirs("gpurun_out", exist_ok=True)
+    os.makedirs("results", exist_ok=True)
     lines = []
     only = sys.argv[1:]
     for fn in selfcheck.ALL_CHECKS:
@@ -25,7 +25,7 @@ def main():
         print(lines[-1] if lines else "", flush=True)
     txt = "\n".join(lines)
     print("=" * 80 + "\n" + txt)
-    open("gpurun_out/lenet_diag.txt", "w").write(txt + "\n")
+    open("results/lenet_diag.txt", "w").write(txt + "\n")
 
 
 if __name__ == "__main__":

@@ -2,10 +2,10 @@
 """Per-kernel resource table from the ``-Xptxas -v`` output of the in-tree build (``build/obj/*.log``, written by
 ``distributedmnist_b200/ops/build.py``): registers, static shared memory, stack / spill bytes, barriers.  No GPU needed.
 
-    python tools/ptxas_report.py [profiles/r2/ptxas_resources.txt]
+    python tools/ptxas_report.py [out.txt]
 
 Why it is tracked: co-residency of the step's kernels is a register / shared-memory budget (4 x 16 K registers per SM
-sub-partition, one shared-memory carve-out for all of them), and a spill in a tcgen05 epilogue is a silent 2x.
+sub-partition, one shared-memory carve-out for all of them), and a spill in a wgmma accumulator is a silent 2x.
 """
 from __future__ import annotations
 
@@ -52,7 +52,7 @@ def parse(path):
 
 def main():
     out_path = sys.argv[1] if len(sys.argv) > 1 else None
-    lines = ["# -Xptxas -v of the shipped library (sm_100a); dynamic shared memory is set at launch and not listed here",
+    lines = ["# -Xptxas -v of the shipped library (sm_90a); dynamic shared memory is set at launch and not listed here",
              "%-14s %-78s %5s %7s %6s %9s %4s" % ("file", "kernel", "regs", "smem_B", "stack", "spill_B", "bar")]
     spills = 0
     for log in sorted(glob.glob(os.path.join(ROOT, "build", "obj", "*.log"))):
