@@ -29,11 +29,13 @@ constexpr int W_BYTES = 800 * 64 * 2;   // 102400
 
 // ldmatrix row address inside a patch of `row_bytes`-wide pixels written by TMA with a swizzle of the same width
 // (64 B: 16-byte chunk bits [4,5] ^= address bits [7,8]; 128 B: bits [4,6] ^= bits [7,9]); patches start on a
-// 1024-byte boundary.
+// 1024-byte boundary.  Swizzling the full address (rather than adding a per-pixel swizzled offset to the base) leaves
+// no loop-invariant per-tap offsets for the compiler to keep live across tiles; that keeps the pipelined tap loops at
+// about 100 registers, so the fc1 update kernel's small CTAs still fit next to conv2_dgrad's in each SM sub-partition.
 template <int ROW_BYTES>
 DMNIST_DEVICE uint32_t patch_addr(uint32_t base, int pixel, int chunk) {
-  if (ROW_BYTES == 64) return base + pixel * 64 + ((chunk ^ ((pixel >> 1) & 3)) << 4);
-  return base + pixel * 128 + ((chunk ^ (pixel & 7)) << 4);
+  const uint32_t a = base + pixel * ROW_BYTES + chunk * 16;
+  return a ^ ((a >> 3) & (ROW_BYTES == 64 ? 0x30 : 0x70));
 }
 
 // ------------------------------------------------------------------------------------------------------
@@ -114,19 +116,29 @@ conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,
     const int s = it % FW_STAGES;
     mbar_wait(&a_full[s], (it / FW_STAGES) & 1);
     const uint32_t patch = smem_u32(smem + FwSmem::A_OFF + s * FW_A_BYTES);
+    // A fragments (two 16-channel K steps) of one tap; output pixel (h, w) reads patch pixel (h + kh, w + kw)
+    auto load_tap = [&](int tap, uint32_t (&a)[2][4]) {
+      const int pix = (hr + tap / 5) * 12 + wr + tap % 5;
+      ldsm_x4(patch_addr<64>(patch, pix, kc), a[0]);
+      ldsm_x4(patch_addr<64>(patch, pix, 2 + kc), a[1]);
+    };
+    // Two-deep register ring, one commit group per tap: tap + 1 is gathered while tap's wgmmas run.  A buffer is
+    // overwritten only after the wgmmas that read it (tap - 1's group) have completed; every wgmma must be able to
+    // keep its A registers until its own group retires, or ptxas serializes the whole loop.
+    uint32_t a[2][2][4];
     fence_regs(acc);
+    load_tap(0, a[0]);
 #pragma unroll
     for (int tap = 0; tap < 25; ++tap) {
-      // output pixel (h, w) reads patch pixel (h + kh, w + kw)
-      const int pix = (hr + tap / 5) * 12 + wr + tap % 5;
-      uint32_t a0[4], a1[4];
-      ldsm_x4(patch_addr<64>(patch, pix, kc), a0);
-      ldsm_x4(patch_addr<64>(patch, pix, 2 + kc), a1);
       wgmma_fence();
-      wgmma_m64n64_rs<1>(acc, a0, desc_advance(db0, tap * 4096), tap != 0);
-      wgmma_m64n64_rs<1>(acc, a1, desc_advance(db0, tap * 4096 + 2048), 1);
+      wgmma_m64n64_rs<1>(acc, a[tap & 1][0], desc_advance(db0, tap * 4096), tap != 0);
+      wgmma_m64n64_rs<1>(acc, a[tap & 1][1], desc_advance(db0, tap * 4096 + 2048), 1);
+      wgmma_commit();
+      if (tap + 1 < 25) {
+        wgmma_wait<1>();
+        load_tap(tap + 1, a[(tap + 1) & 1]);
+      }
     }
-    wgmma_commit();
     wgmma_wait<0>();
     fence_regs(acc);
     __syncwarp();
@@ -251,18 +263,28 @@ conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,1
       mbar_wait(&a_full[s], (it / DG_STAGES) & 1);
       if (dbg_on && threadIdx.x == 0 && it < 20) dbg[32 + it] = globaltimer_ns();   // MMA: data of load `it` landed
       const uint32_t patch = smem_u32(smem + DgSmem::A_OFF + s * DG_A_BYTES);
-      fence_regs(acc);
-#pragma unroll
-      for (int tap = 0; tap < 25; ++tap) {
+      // A fragments (four 16-channel K steps) of one tap; tap (kh, kw) reads patch pixel (h + 4 - kh, w + 4 - kw)
+      auto load_tap = [&](int tap, uint32_t (&a)[4][4]) {
         const int pix = (hr + 4 - tap / 5) * 12 + wr + 4 - tap % 5;
-        uint32_t a[4][4];
 #pragma unroll
         for (int k = 0; k < 4; ++k) ldsm_x4(patch_addr<128>(patch, pix, 2 * k + kc), a[k]);
+      };
+      // Same two-deep register ring as the forward tap loop.
+      uint32_t a[2][4][4];
+      fence_regs(acc);
+      load_tap(0, a[0]);
+#pragma unroll
+      for (int tap = 0; tap < 25; ++tap) {
         wgmma_fence();
 #pragma unroll
-        for (int k = 0; k < 4; ++k) wgmma_m64n32_rs<0>(acc, a[k], desc_advance(db0, tap * 4096 + 32 * k), (tap | k) != 0);
+        for (int k = 0; k < 4; ++k)
+          wgmma_m64n32_rs<0>(acc, a[tap & 1][k], desc_advance(db0, tap * 4096 + 32 * k), (tap | k) != 0);
+        wgmma_commit();
+        if (tap + 1 < 25) {
+          wgmma_wait<1>();
+          load_tap(tap + 1, a[(tap + 1) & 1]);
+        }
       }
-      wgmma_commit();
       wgmma_wait<0>();
       fence_regs(acc);
       __syncwarp();
@@ -312,24 +334,18 @@ constexpr int WG_MAX_PARTS = 160;
 __device__ float g_c2wg_part[WG_MAX_PARTS * WG_PART_FLOATS];
 __device__ unsigned int g_c2wg_ticket[WG_GROUPS];
 
-// GPC = tap groups per CTA.  Every group of a CTA reuses the stage's patch + dY tile, so the shared-memory fill traffic
-// (7 groups x the pixel slices re-read X and dY seven times) drops to ceil(7 / GPC) passes, at the price of
-// ceil(7 / GPC) x fewer pixel slices, i.e. more atomics per output.
-template <int GPC>
+// CTA = (tap group, pixel slice): blockIdx.x = split * WG_GROUPS + group.
 __global__ void __launch_bounds__(CV_THREADS, 1)
 conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,12,20,1), 64B swizzle
                    const __grid_constant__ CUtensorMap tmDY,   // dY, box (64,8,16,1), 128B swizzle
                    float* __restrict__ g_w,                    // [25][32][64] fp32, the gradient is added to it
                    int num_tiles, int splits) {
-  constexpr int SETS = (WG_GROUPS + GPC - 1) / GPC;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + WgSmem::BAR_OFF);
   uint64_t* empty = full + WG_STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  const int set = blockIdx.x % SETS, split = blockIdx.x / SETS;
-  const int g_first = set * GPC;
-  const int ng = (g_first + GPC <= WG_GROUPS) ? GPC : (WG_GROUPS - g_first);   // groups this CTA really owns
+  const int group = blockIdx.x % WG_GROUPS, split = blockIdx.x / WG_GROUPS;
   const int t_begin = (int)(((long long)num_tiles * split) / splits);
   const int t_end = (int)(((long long)num_tiles * (split + 1)) / splits);
   const int nt = t_end - t_begin;
@@ -364,73 +380,57 @@ conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,12
   const int q = warp >> 1;                         // M-chunk (tap of the group) of this warp's 16 rows
   const int chunk = 2 * (warp & 1) + ((lane >> 3) & 1);   // 16-byte channel chunk (8 ci)
   const int lh = lane >> 4, lw = lane & 7;
-  float acc[GPC][32];
+  // first pixel of this chunk's tap window inside the patch; group 6 chunks 1-3 are padding
+  const int base_px = group < 5 ? q * 12 + group : (group == 5 ? 48 + q : 52);
+  const bool real_chunk = group < 6 || q == 0;
+  float acc[32];
 #pragma unroll
-  for (int gi = 0; gi < GPC; ++gi)
-#pragma unroll
-    for (int j = 0; j < 32; ++j) acc[gi][j] = 0.f;
+  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
   for (int i = 0; i < nt; ++i) {
     const int s = i % WG_STAGES;
     mbar_wait(&full[s], (i / WG_STAGES) & 1);
     const uint32_t patch = smem_u32(smem + s * WG_STAGE_BYTES);
     // B (MN-major, 128B swizzle): [pixel][64 co], 8-pixel groups 1024 B apart; K step = 16 pixels = 2048 B.
     const uint64_t db0 = make_smem_desc(patch + WG_A_BYTES + 1024, 8192, 1024, SWZ_128B);
-#pragma unroll
-    for (int gi = 0; gi < GPC; ++gi) fence_regs(acc[gi]);
+    fence_regs(acc);
 #pragma unroll
     for (int ks = 0; ks < 8; ++ks) {
-      uint32_t a[GPC][4];
-#pragma unroll
-      for (int gi = 0; gi < GPC; ++gi) {
-        const int group = g_first + gi;
-        // first pixel of this chunk's tap window inside the patch; group 6 chunks 1-3 are padding
-        const int base_px = group < 5 ? q * 12 + group : (group == 5 ? 48 + q : 52);
-        if (gi < ng && (group < 6 || q == 0)) {
-          ldsm_x4_trans(patch_addr<64>(patch, base_px + (2 * ks + lh) * 12 + lw, chunk), a[gi]);
-        } else {
-          a[gi][0] = a[gi][1] = a[gi][2] = a[gi][3] = 0u;
-        }
+      uint32_t a[4];
+      if (real_chunk) {
+        ldsm_x4_trans(patch_addr<64>(patch, base_px + (2 * ks + lh) * 12 + lw, chunk), a);
+      } else {
+        a[0] = a[1] = a[2] = a[3] = 0u;
       }
       wgmma_fence();
-#pragma unroll
-      for (int gi = 0; gi < GPC; ++gi)
-        if (gi < ng) wgmma_m64n64_rs<1>(acc[gi], a[gi], desc_advance(db0, 2048 * ks), 1);
+      wgmma_m64n64_rs<1>(acc, a, desc_advance(db0, 2048 * ks), 1);
     }
     wgmma_commit();
     wgmma_wait<0>();
-#pragma unroll
-    for (int gi = 0; gi < GPC; ++gi) fence_regs(acc[gi]);
+    fence_regs(acc);
     __syncwarp();
     if (lane == 0) mbar_arrive(&empty[s]);
   }
 
   const int ci0 = 16 * (warp & 1) + (lane >> 2);
+  float* part = g_c2wg_part + (size_t)blockIdx.x * WG_PART_FLOATS;
 #pragma unroll
-  for (int gi = 0; gi < GPC; ++gi) {
-    float* part = g_c2wg_part + (size_t)(blockIdx.x * GPC + gi) * WG_PART_FLOATS;
+  for (int half = 0; half < 2; ++half) {
+    float* o = part + (q * 32 + ci0 + 8 * half) * 64 + 2 * (lane & 3);
 #pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      float* o = part + (q * 32 + ci0 + 8 * half) * 64 + 2 * (lane & 3);
-#pragma unroll
-      for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[gi][4 * j + 2 * half], acc[gi][4 * j + 2 * half + 1]);
-    }
+    for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
   }
   __shared__ unsigned int s_last;
-  if (arrive_last_cta(&g_c2wg_ticket[set], splits, 1, CV_CONSUMERS, &s_last)) {
-    for (int gi = 0; gi < ng; ++gi) {
-      const int group = g_first + gi;
-      for (int e4 = threadIdx.x; e4 < WG_PART_FLOATS / 4; e4 += CV_CONSUMERS) {
-        const int row = e4 >> 4, co = (e4 & 15) * 4;        // row = M-chunk * 32 + ci
-        const int qq = row >> 5, ci = row & 31;
-        const int tap = group < 5 ? qq * 5 + group : (group == 5 ? 20 + qq : (qq == 0 ? 24 : 25));
-        if (tap >= 25) continue;
-        const float4 sum = ordered_sum4(
-            reinterpret_cast<const float4*>(g_c2wg_part + (size_t)(set * GPC + gi) * WG_PART_FLOATS) + e4, splits,
-            (size_t)SETS * GPC * WG_PART_FLOATS / 4);
-        float4* o = reinterpret_cast<float4*>(g_w + ((size_t)tap * 32 + ci) * 64 + co);
-        const float4 cur = *o;
-        *o = make_float4(cur.x + sum.x, cur.y + sum.y, cur.z + sum.z, cur.w + sum.w);
-      }
+  if (arrive_last_cta(&g_c2wg_ticket[group], splits, 1, CV_CONSUMERS, &s_last)) {
+    for (int e4 = threadIdx.x; e4 < WG_PART_FLOATS / 4; e4 += CV_CONSUMERS) {
+      const int row = e4 >> 4, co = (e4 & 15) * 4;        // row = M-chunk * 32 + ci
+      const int qq = row >> 5, ci = row & 31;
+      const int tap = group < 5 ? qq * 5 + group : (group == 5 ? 20 + qq : (qq == 0 ? 24 : 25));
+      if (tap >= 25) continue;
+      const float4 sum = ordered_sum4(reinterpret_cast<const float4*>(g_c2wg_part + (size_t)group * WG_PART_FLOATS) + e4,
+                                      splits, (size_t)WG_GROUPS * WG_PART_FLOATS / 4);
+      float4* o = reinterpret_cast<float4*>(g_w + ((size_t)tap * 32 + ci) * 64 + co);
+      const float4 cur = *o;
+      *o = make_float4(cur.x + sum.x, cur.y + sum.y, cur.z + sum.z, cur.w + sum.w);
     }
   }
 }
@@ -488,26 +488,17 @@ int dm_conv2_wgrad(const void* a1, const void* dy, void* g_w, int B, void* strea
   if (make_tmap_nhwc_bf16(&tmX, a1, 32, 14, 14, B, 32, 12, 20, 64)) return 101;
   if (make_tmap_nhwc_bf16(&tmDY, dy, 64, 14, 14, B, 64, 8, 16, 128)) return 102;
   const int tiles = 2 * B;
-  static const int gpc = env_int("DMNIST_WGRAD_GPC", 1);      // tap groups per CTA: 1 (first version), 2, 4
-  const int sets = gpc == 1 ? 7 : (gpc == 2 ? 4 : 2);
-  int splits = max_ctas() / sets;
-  if (splits * sets * gpc > WG_MAX_PARTS) splits = WG_MAX_PARTS / (sets * gpc);
+  int splits = max_ctas() / WG_GROUPS;
+  if (splits * WG_GROUPS > WG_MAX_PARTS) splits = WG_MAX_PARTS / WG_GROUPS;
   if (splits > tiles) splits = tiles;
   static bool configured = false;
   if (!configured) {
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel<1>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem::TOTAL));
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel<1>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel<2>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem::TOTAL));
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel<2>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel<4>, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem::TOTAL));
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel<4>, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem::TOTAL));
+    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }
-  cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  float* gw = reinterpret_cast<float*>(g_w);
-  if (gpc == 1) return (int)launch_kernel(conv2_wgrad_kernel<1>, dim3(sets * splits), dim3(CV_THREADS), WgSmem::TOTAL, st, tmX, tmDY, gw, tiles, splits);
-  if (gpc == 2) return (int)launch_kernel(conv2_wgrad_kernel<2>, dim3(sets * splits), dim3(CV_THREADS), WgSmem::TOTAL, st, tmX, tmDY, gw, tiles, splits);
-  return (int)launch_kernel(conv2_wgrad_kernel<4>, dim3(sets * splits), dim3(CV_THREADS), WgSmem::TOTAL, st, tmX, tmDY, gw, tiles, splits);
+  return (int)launch_kernel(conv2_wgrad_kernel, dim3(WG_GROUPS * splits), dim3(CV_THREADS), WgSmem::TOTAL,
+                            reinterpret_cast<cudaStream_t>(stream), tmX, tmDY, reinterpret_cast<float*>(g_w), tiles, splits);
 }
 
 }  // extern "C"

@@ -12,6 +12,7 @@ from __future__ import annotations
 
 import hashlib
 import os
+import re
 import subprocess
 import sys
 from concurrent.futures import ThreadPoolExecutor
@@ -52,6 +53,15 @@ def is_fresh() -> bool:
         return False
 
 
+_SERIALIZED_WGMMA = re.compile(r"\(C7511\).*wgmma\.mma_async instructions are serialized.*in the function '(\S+?)'")
+
+
+def serialized_wgmma_kernels(ptxas_log: str) -> List[str]:
+    """Kernels whose wgmmas ptxas serialized (warning C7511): it then waits for every wgmma to complete before the next
+    is issued, which typically costs a wgmma kernel a large part of its tensor-core throughput."""
+    return [m.group(1) for m in _SERIALIZED_WGMMA.finditer(ptxas_log)]
+
+
 def _compile(src: str) -> str:
     obj = os.path.join(OBJ_DIR, os.path.basename(src)[:-3] + ".o")
     cmd = [NVCC] + ARCH_FLAGS + NVCC_FLAGS + ["-I", CSRC, "-c", src, "-o", obj]
@@ -61,6 +71,10 @@ def _compile(src: str) -> str:
         f.write(" ".join(cmd) + "\n" + r.stdout + r.stderr)
     if r.returncode != 0:
         raise RuntimeError("nvcc failed for %s:\n%s" % (src, (r.stdout + r.stderr)[-6000:]))
+    serialized = serialized_wgmma_kernels(r.stdout + r.stderr)
+    if serialized:
+        raise RuntimeError("ptxas serialized the wgmma pipeline (C7511) of %s in %s; see %s"
+                           % (", ".join(serialized), src, log))
     return obj
 
 
