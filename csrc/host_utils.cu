@@ -108,6 +108,9 @@ extern "C" int dm_set_max_ctas(int n) {
   return dm::max_ctas();
 }
 
+// The grid bound set by dm_set_max_ctas, 0 when the default is in force (so callers can put it back).
+extern "C" int dm_get_max_ctas() { return dm::g_max_ctas; }
+
 extern "C" int dm_num_sms() { return dm::num_sms(); }
 
 extern "C" int dm_set_pdl(int on) {

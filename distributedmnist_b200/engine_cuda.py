@@ -13,7 +13,7 @@ Step = (reference src/distributed_train.py:332 ``sess.run(apply_gradients_op)``)
     fc1_wgrad        wgmma GEMM (MN-major x MN-major) -> gradient arena
     fc1_dgrad        wgmma GEMM -> bf16
     unpool2          maxpool2/ReLU2 backward + conv2 bias grad
-    conv2_wgrad      wgmma, K = pixels, fp32 atomics -> gradient arena
+    conv2_wgrad      wgmma, K = pixels, per-CTA partials summed in fixed order -> gradient arena
     conv2_dgrad      wgmma
     conv1_wgrad      maxpool1/ReLU1 backward + conv1 weight/bias grad
     fused_sync_sgd   arrival -> mask -> NVLink reduce -> 1/count -> SGD -> push -> bf16 shadow

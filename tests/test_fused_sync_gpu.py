@@ -177,8 +177,10 @@ def test_bucketed_overlapped_aggregation_matches_single_kernel(tmp_path):
             assert len({x["fp"] for x in rows}) == 1, (tag, s)                   # replicas bit-identical
             assert all(x["step"] == s + 1 and x["count"] == n and x["mask"] == (1 << n) - 1 for x in rows), (tag, rows)
             assert all(x["shadow_err"] <= 0.01 * x["pmax"] + 1e-6 for x in rows), (tag, rows)
-    # across RUNS the gradients differ in the last bits (fp32 atomics in the conv weight gradients, different CTA counts),
-    # so paths are compared tightly after the first update and loosely after eight
+    # the aggregation paths do not apply bit-identical updates: they add the replicas' gradients in different orders, and
+    # the bucketed v2 path sends its late bucket (everything but fc1's weights) as bf16 by default (DMNIST_LATE_BF16=1), as it
+    # does fc1's gradient.  So they are compared tightly after the first update and loosely after eight, once ReLU /
+    # max-pool / dropout decisions have amplified the differences
     first = {t: torch.tensor(res[t][0]["rows"][0]["sample"]) for t in res}
     last = {t: torch.tensor(res[t][0]["rows"][-1]["sample"]) for t in res}
     assert (first["bucket"] - first["single"]).abs().max().item() < 2e-6

@@ -1,4 +1,4 @@
-"""sm_90a LeNet kernels vs plain PyTorch fp32 references (SURVEY §4 item 2)."""
+"""sm_90a LeNet kernels vs float64 references (ops/refs.py) and the engine-level checks (SURVEY §4 item 2)."""
 import pytest
 
 pytestmark = pytest.mark.gpu
