@@ -613,6 +613,117 @@ class CudaLeNetEngine(ComputeEngine):
         self._launch_forward(images.reshape(B, 28, 28).contiguous(), labels, B, train, logits_out=out)
         return out
 
+    # ---- in-training evaluation (csrc/eval_head.cu) ---------------------------------------------------------------------
+    # The validation set is scored in chunks of EVAL_CHUNK rows by the forward kernels on buffers of its own, then by the
+    # evaluation head, on the training stream right after the step whose weights it scores: nothing is shared with the step
+    # (no activation buffer, no workspace, no ticket), so the next step computes exactly what it would have computed without
+    # the pass.  The pass's record lands in page-locked host memory; the host reads it once an event that follows the pass
+    # has fired (in the training loop: the next step's completion event).
+    EVAL_CHUNK = 2048
+    EVAL_RING = 16                 # host record slots
+
+    def arm_eval(self, images, labels) -> None:
+        """Upload the validation set once (device-resident fp32 images, int64 labels) and allocate the pass's buffers and
+        the host record ring.  With ``use_graph`` the whole pass is captured as one CUDA graph."""
+        self._leave_native_runner()
+        lib, dev = self.lib, self.device
+        x = torch.as_tensor(np.ascontiguousarray(images) if isinstance(images, np.ndarray) else images, dtype=torch.float32)
+        y = torch.as_tensor(np.ascontiguousarray(labels) if isinstance(labels, np.ndarray) else labels).to(torch.int64)
+        n = int(x.shape[0])
+        if n < 1 or y.numel() != n:
+            raise ValueError("arm_eval: %d images, %d labels" % (n, y.numel()))
+        assert self.EVAL_CHUNK <= int(lib.dm_eval_max_rows())
+        self._ev_x = x.reshape(n, 28, 28).to(dev).contiguous()
+        self._ev_y = y.reshape(n).to(dev).contiguous()
+        C = min(self.EVAL_CHUNK, n)
+        bf, u8, f32 = torch.bfloat16, torch.uint8, torch.float32
+        self._ev_a1 = torch.zeros(C, 14, 14, 32, dtype=bf, device=dev)
+        self._ev_code1 = torch.zeros(C, 14, 14, 32, dtype=u8, device=dev)
+        self._ev_a2 = torch.zeros(C, 3136, dtype=bf, device=dev)
+        self._ev_code2 = torch.zeros(C, 3136, dtype=u8, device=dev)
+        self._ev_hpart = torch.zeros(self.fc1_splits, C, 512, dtype=f32, device=dev)
+        self._ev_ws = torch.zeros(2 * int(lib.dm_eval_max_rows()), dtype=f32, device=dev)
+        self._ev_state = torch.zeros(int(lib.dm_eval_state_bytes()), dtype=u8, device=dev)
+        self._ev_ring = torch.zeros(self.EVAL_RING, 8, dtype=torch.int64).pin_memory()
+        self._ev_seen = 0
+        self._ev_last = None
+        self._ev_graph = None
+        self._launch_eval(publish=False)        # sets the kernels' function attributes outside a capture
+        torch.cuda.synchronize()
+        if self.use_graph:
+            gr = torch.cuda.CUDAGraph()
+            cap = torch.cuda.Stream(device=dev)
+            with torch.cuda.graph(gr, stream=cap, capture_error_mode="thread_local"):
+                self._launch_eval(publish=True)
+            self._ev_graph = gr
+
+    def _launch_eval(self, publish: bool, logits_out: Optional[torch.Tensor] = None) -> None:
+        lib, sp, p, pb = self.lib, stream_ptr(), self.p, self.pb
+        n, C = self._ev_x.shape[0], self._ev_a1.shape[0]
+        stride = self._ev_hpart.stride(0)
+        conv1_fwd = lib.dm_conv1_fwd_tc if self._conv1_tc else lib.dm_conv1_fwd
+        null = ctypes.c_void_p(0)
+        ring = ptr(self._ev_ring) if publish else null
+        check(lib.dm_eval_stamp(ptr(self._ev_state), sp), "eval_stamp")
+        for s in range(0, n, C):
+            m = min(C, n - s)
+            check(conv1_fwd(ptr(self._ev_x[s:s + m]), ptr(p["conv1_weights"]), ptr(p["conv1_biases"]), ptr(self._ev_a1),
+                            ptr(self._ev_code1), m, null, 0, null, 0, null, 0, sp), "conv1_fwd")
+            check(lib.dm_conv2_fwd(ptr(self._ev_a1), ptr(pb["conv2_weights"]), ptr(p["conv2_biases"]), ptr(self._ev_a2),
+                                   ptr(self._ev_code2), m, sp), "conv2_fwd")
+            G.gemm_bf16_raw(self._ev_a2, pb["fc1_weights"], self._ev_hpart, m, 512, 3136, 3136, 512, 512, False, True,
+                            G.EPI_STORE_F32, splits=self.fc1_splits, bn=64, split_stride=stride)
+            lg = null if logits_out is None else ptr(logits_out[s:s + m])
+            check(lib.dm_eval_head(ptr(self._ev_hpart), ctypes.c_longlong(stride), self.fc1_splits, ptr(p["fc1_biases"]),
+                                   ptr(p["fc2_weights"]), ptr(p["fc2_biases"]), ptr(self._ev_y[s:s + m]), ptr(self._ev_ws),
+                                   ptr(self._ev_state), self._epoch_ptr, ring, self.EVAL_RING, lg, m, int(s + m == n), sp),
+                  "eval_head")
+
+    def enqueue_eval(self) -> None:
+        """Score the validation set with the current weights, on the current (training) stream, without a host
+        synchronisation.  Enqueue it right after the step whose weights it scores; its record is complete once any event
+        recorded after it -- e.g. the next step's completion event -- has fired (see :meth:`eval_record`)."""
+        if self._ev_graph is not None:
+            self._ev_graph.replay()
+        else:
+            self._launch_eval(publish=True)
+
+    def eval_records(self):
+        """Records completed since the previous call, oldest first: ``(global_step, t_begin_ns, t_end_ns, examples,
+        correct, loss_sum)`` (``%globaltimer`` stamps; ``loss_sum`` is the sum of the per-row cross entropies).
+
+        The ring holds the last EVAL_RING records: call this at least once per EVAL_RING enqueued passes.  A caller that
+        falls further behind loses the overwritten records, and a slot the device is rewriting while it is read is skipped
+        (the training loop reads after every step, with at most two passes outstanding)."""
+        raw = self._ev_ring.numpy()
+        new = []
+        for i in range(self.EVAL_RING):
+            seq = int(raw[i, 0])
+            if seq <= self._ev_seen:
+                continue
+            rec = raw[i].copy()
+            if int(raw[i, 0]) != seq or int(rec[0]) != seq:
+                continue                                 # slot rewritten while it was read: the pass is still running
+            loss = float(rec[6:7].view(np.float64)[0])
+            new.append((seq, (int(rec[1]), int(rec[2]), int(rec[3]), int(rec[4]), int(rec[5]), loss)))
+        new.sort()
+        if new:
+            self._ev_seen = new[-1][0]
+            self._ev_last = new[-1][1]
+        return [r for _, r in new]
+
+    def eval_record(self):
+        """The newest complete record (see :meth:`eval_records`), or None."""
+        self.eval_records()
+        return self._ev_last
+
+    def run_eval(self, logits_out: Optional[torch.Tensor] = None):
+        """One pass, enqueued eagerly and waited for: its record.  ``logits_out`` [n,10] receives the logits."""
+        self.eval_records()
+        self._launch_eval(publish=True, logits_out=logits_out)
+        torch.cuda.current_stream().synchronize()
+        return self.eval_record()
+
 
 class CudaMlpEngine(ComputeEngine):
     """2-/3-layer MLP on the sm_90a kernels: hidden layers = wgmma GEMM with bias+ReLU fused in the

@@ -144,6 +144,32 @@ class _BatchPacker:
             t.join(timeout=2.0)
 
 
+def check_eval_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate: int, dataset_test) -> None:
+    """``--eval_every_steps`` combinations that cannot work, rejected before any device work starts."""
+    if getattr(flags, "eval_every_steps", 0) < 0:
+        raise ValueError("--eval_every_steps must be >= 0 (0 = off)")
+    if not getattr(flags, "eval_every_steps", 0):
+        return
+    if dataset_test is None:
+        raise ValueError("--eval_every_steps needs the validation set, but no dataset_test was given")
+    if not (ctx.on_gpu and flags.backend in ("auto", "fused")):
+        return                     # torch engine: evaluated synchronously with engine.evaluate, every mode and model
+    if flags.model != "lenet":
+        raise ValueError("--eval_every_steps on the GPU path is implemented for lenet, not --model=%s" % flags.model)
+    # the pass reads the chief's live parameter arena between two of its steps: sound only when no peer can write that
+    # arena then, i.e. when every step waits for all N replicas
+    if flags.interval_method:
+        raise ValueError("--eval_every_steps cannot be combined with --interval_method: interval commits push weights into "
+                         "the chief's arena at any time, so the pass would not see one step's weights")
+    # --worker_times_cdf_method (without --interval_method, which wins when both are set) always aggregates all N
+    # gradients behind a full barrier and ignores --num_replicas_to_aggregate
+    cdf = getattr(flags, "worker_times_cdf_method", False)
+    if not cdf and num_replicas_to_aggregate < ctx.world_size:
+        raise ValueError("--eval_every_steps needs --num_replicas_to_aggregate = number of replicas (%d): with K < N the "
+                         "team pushes weights into the chief's arena while it is between steps or late"
+                         % ctx.world_size)
+
+
 def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     num_workers = ctx.world_size
     # reference distributed_train.py:118-121
@@ -153,6 +179,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         num_replicas_to_aggregate = flags.num_replicas_to_aggregate
     assert num_workers > 0
     is_chief = ctx.is_chief
+    check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
 
     backend = make_backend(ctx, flags.backend, flags)
     engine = make_engine(flags, ctx, backend)
@@ -197,6 +224,17 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     if hasattr(engine, "params_updated"):
         engine.params_updated()
     log.info("%s Supervisor" % datetime.now())
+
+    # --eval_every_steps: the chief scores the validation set after every E-th global step and after the last one.  GPU path:
+    # a forward-only pass on the training stream right after the step (engine.enqueue_eval), read back from page-locked
+    # host memory once the following step has been consumed; torch engine: engine.evaluate, synchronously.
+    eval_every = int(getattr(flags, "eval_every_steps", 0) or 0) if is_chief else 0
+    device_eval = bool(eval_every and fused_step)
+    if device_eval:
+        engine.arm_eval(dataset_test.images, dataset_test.labels)
+    eval_rows = []                 # (global_step, t_begin_unix_s, eval_seconds, examples, correct, mean_loss)
+    last_eval_step = -1
+    test_acc_value = 0.0           # newest complete evaluation; hard-wired to 0 in the reference (:363) and when off
 
     def _device_step() -> int:
         torch.cuda.synchronize()
@@ -253,7 +291,6 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         if step > flags.max_steps:
             stop = True
             return
-        test_acc_value = 0.0   # hard-wired in the reference too (:363)
         duration = finish_time - start_time
         examples_per_sec = flags.batch_size / float(max(duration, 1e-9))
         if do_log:
@@ -264,6 +301,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         results["losses"].append(loss_value)
         if step % flags.save_results_period == 0:
             np.save(os.path.join(flags.train_dir, "worker%d_time_acc.npy" % ctx.rank), np.array(time_acc_list))
+            if eval_every:
+                save_evals()
         if is_chief:
             ckpt.maybe_save(engine.params, step)
             if summary is not None and next_summary_time < time.time():
@@ -272,6 +311,35 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                                      "learning_rate": lr_schedule(step)}, step)
                 log.info("Finished running Summary operation.")
                 next_summary_time += flags.save_summaries_secs
+
+    def collect_evals() -> None:
+        """Device records completed so far (%globaltimer ns -> seconds, as push_device_times converts them)."""
+        nonlocal test_acc_value
+        for gs, t0, t1, n_ex, correct, loss_sum in engine.eval_records():
+            eval_rows.append((gs, t0 * 1e-9, (t1 - t0) * 1e-9, n_ex, correct, loss_sum / max(n_ex, 1)))
+            test_acc_value = correct / float(max(n_ex, 1))
+
+    def eval_after_step(global_step: int) -> None:
+        """Non-pipelined loops: called once the step's outcome has been read back."""
+        nonlocal test_acc_value, last_eval_step
+        if device_eval:
+            collect_evals()        # the step read-back above waited for the pass enqueued after the previous step
+        if global_step == last_eval_step or not (global_step % eval_every == 0 or global_step > flags.max_steps):
+            return
+        last_eval_step = global_step
+        if device_eval:
+            engine.enqueue_eval()
+            return
+        t0 = time.time()
+        loss, acc = engine.evaluate(dataset_test.images, dataset_test.labels)
+        n_ex = dataset_test.num_examples
+        correct = int(round(acc * n_ex))
+        eval_rows.append((global_step, t0, time.time() - t0, n_ex, correct, loss))
+        test_acc_value = correct / float(n_ex)
+
+    def save_evals() -> None:
+        np.save(os.path.join(flags.train_dir, "worker%d_eval.npy" % ctx.rank),
+                np.array(eval_rows, dtype=np.float64).reshape(-1, 6))
 
     def push_device_times(upto: int) -> None:
         """Hand the %globaltimer stamps of iterations [cdf_pushed, upto] to the timeout client: 'dequeued' = the step's first
@@ -301,11 +369,15 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 log.info("RUNNING SESSION... %f" % time.time())
             token = (cur_iteration, engine.step_packed(packer.next()))   # input DMA + step graph: one native call
             launched += 1
+            if device_eval and ((restored_step + launched) % eval_every == 0 or restored_step + launched > flags.max_steps):
+                engine.enqueue_eval()          # K == N: restored_step + launched is the global step of the weights it scores
             prev, pending = pending, token
             if prev is not None:
                 it, (ev, lbuf, seq) = prev
                 ev.synchronize()
                 info = opt._account(backend.mirror_info(seq, check=True))
+                if device_eval:
+                    collect_evals()            # passes enqueued before the step just waited for are complete
                 now = time.time()
                 finish_iteration(it, last_consume, info, (float(lbuf[0]), float(lbuf[1])))
                 last_consume = now
@@ -348,6 +420,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 engine.params_updated()
         la = engine.loss_acc() if (do_log or flags.timeline_logging) else None
         t3 = time.perf_counter()
+        if eval_every:
+            eval_after_step(info.global_step)
 
         if cdf:
             if device_times:
@@ -376,6 +450,11 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         pending = None
     if packer is not None:
         packer.close()
+    if device_eval:
+        torch.cuda.synchronize()       # the pass after the final step
+        collect_evals()
+    if eval_every:
+        save_evals()
     if device_times:
         push_device_times(cur_iteration)
 
@@ -392,6 +471,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         ckpt.close()
     if summary is not None:
         summary.close()
+    if eval_every:
+        results["evals"] = eval_rows
     results.update(final_step=step, accepted=opt.accepted_steps, dropped=opt.dropped_steps,
                    params=engine.params, elapsed=time.time() - begin_time,
                    timeout_server=timeout_server, engine=engine, optimizer=opt)

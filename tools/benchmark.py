@@ -204,6 +204,20 @@ def plot_time_precision(outdir: str, dest: str = ".") -> str:
                      "time (s)", "precision")
 
 
+def plot_device_time_precision(train_dir: str, dest: str = ".") -> str:
+    """Accuracy against training time from the chief's in-training evaluations (``--eval_every_steps``,
+    ``worker0_eval.npy``: global_step, t_begin_unix_s, eval_seconds, examples, correct, mean_loss).  The time axis starts at
+    the first evaluation and leaves out the time spent in the evaluations before each point."""
+    rows = np.load(os.path.join(train_dir, "worker0_eval.npy")).reshape(-1, 6)
+    rows = rows[np.argsort(rows[:, 1], kind="stable")]
+    spent = np.concatenate([[0.0], np.cumsum(rows[:-1, 2])])          # evaluation time before each pass began
+    t = rows[:, 1] - rows[0, 1] - spent
+    acc = rows[:, 4] / np.maximum(rows[:, 3], 1)
+    return line_plot(os.path.join(dest, "device_time_precision.png"),
+                     [(os.path.basename(os.path.normpath(train_dir)), t.tolist(), acc.tolist())],
+                     "training time (s, evaluation excluded)", "precision")
+
+
 def plot_step_loss(outdir: str, dest: str = ".") -> str:
     return line_plot(os.path.join(dest, "step_losses.png"), _series(outdir, lambda t, l, p, s: (s, l)),
                      "step", "losses", logy=True)
