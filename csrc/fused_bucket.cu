@@ -175,7 +175,7 @@ __global__ void __launch_bounds__(EARLY2_THREADS) bucket_early_kernel(SyncPeers 
   }
 
   // ---- SGD on my fp32 master copy of fc1 from the (identical everywhere) bf16 gradient sum; fresh bf16 shadow ---------------
-  const float scale = device_lr(a, epoch) / (float)NR;
+  const float scale = cta_scale(a, epoch, (uint32_t)NR);
   float* w = P.params[a.rank] + 4 * (size_t)r.fc1_b4;
   __nv_bfloat16* sh = a.shadow != nullptr ? a.shadow + 4 * (size_t)r.fc1_b4 : nullptr;
   constexpr int A = 2;
@@ -270,7 +270,7 @@ __global__ void __launch_bounds__(LATE2_THREADS, 1) bucket_late_kernel(SyncPeers
   }
 
   // ---- sum the N contributions in rank order, SGD on my copy, bf16 shadow --------------------------------------------------
-  const float scale = device_lr(a, epoch) / (float)NR;
+  const float scale = cta_scale(a, epoch, (uint32_t)NR);
   float* wdst = P.params[a.rank];
   const float* inbox = r.inbox[a.rank];
   for (int j = tid; j < n_late4; j += stride) {
@@ -381,7 +381,7 @@ __global__ void __launch_bounds__(LATE2_THREADS) bucket_late_ll_kernel(SyncPeers
   }
 
   // ---- receive: poll my inbox until the other replicas' lines of this step are there; rank-ordered sum; SGD; shadow -------
-  const float scale = device_lr(a, epoch) / (float)NR;
+  const float scale = cta_scale(a, epoch, (uint32_t)NR);
   float* wdst = P.params[a.rank];
   const uint4* inbox = reinterpret_cast<const uint4*>(r.inbox[a.rank]);
   for (int j = tid; j < n_late4; j += stride) {
@@ -472,8 +472,8 @@ extern "C" {
 //   bf16 (default) or fp32 gradients.
 //   fc1_begin/fc1_end/numel in floats, all multiples of 8 / 8 / 4.
 int dm_bucket_sync(void* const* ctrl, void* const* params, void* const* grads, void* const* g16, void* const* inbox, int rank,
-                   int nranks, int phase, long long fc1_begin, long long fc1_end, long long numel, float lr0,
-                   float decay_rate, int decay_steps, double timeout_ms, void* shadow_bf16, int ctas, void* stream_,
+                   int nranks, int phase, long long fc1_begin, long long fc1_end, long long numel, double lr0,
+                   double decay_rate, int decay_steps, double timeout_ms, void* shadow_bf16, int ctas, void* stream_,
                    void* mc_g16, void* mc_inbox, int late_ll, int late_bf16) {
   using namespace dm;
   if (nranks < 1 || nranks > SYNC_MAX_RANKS || phase < 1 || phase > 4) return -1;

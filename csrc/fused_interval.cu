@@ -170,7 +170,7 @@ __global__ void __launch_bounds__(IV_THREADS, 1) iv_apply_kernel(SyncPeers P, Sy
   const uint32_t e = me->epoch;
   if (me->iv_commit_go != e + 1) return;
   const uint32_t mask = me->iv_commit_mask, total = me->iv_commit_total;
-  const float scale = device_lr(a, e) / (float)max(total, 1u);
+  const float scale = cta_scale(a, e, max(total, 1u));
   int contrib[SYNC_MAX_RANKS];
   int nc = 0;
   for (int q = 0; q < a.nranks; ++q)
@@ -235,7 +235,7 @@ int dm_interval_begin(void* ctrl, const void* params, void* shadow_bf16, long lo
 
 // Last four kernels of an interval-mode iteration: gate, accumulate, close (+ commit attempt), apply (winner only).
 int dm_interval_end(void* const* ctrl, void* const* params, void* const* grads, void* const* acc, int rank, int nranks,
-                    long long numel, float lr0, float decay_rate, int decay_steps, double timeout_ms, int ctas, void* stream_,
+                    long long numel, double lr0, double decay_rate, int decay_steps, double timeout_ms, int ctas, void* stream_,
                     void* mc_params) {
   using namespace dm;
   if (nranks < 1 || nranks > SYNC_MAX_RANKS || (numel & 3)) return -1;

@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(SYNC_THREADS, 1) fused_sync_sgd_kernel(SyncPee
     const int end = min(begin + shard, a.numel4);
     own_begin = begin;
     own_end = end;
-    const float scale = device_lr(a, epoch) / (float)count;
+    const float scale = cta_scale(a, epoch, (uint32_t)count);
     const uint32_t drop_thresh = a.drop_keep > 0.f ? (uint32_t)(a.drop_keep * 16777216.f) : 0u;
     int contrib[SYNC_MAX_RANKS];
     int nc = 0;
@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(EARLY_THREADS) fused_sync_early_kernel(SyncPee
   const int shard = (n4 + a.nranks - 1) / a.nranks;
   const int begin = r.begin4 + a.rank * shard;
   const int end = min(begin + shard, r.end4);
-  const float scale = device_lr(a, epoch) / (float)a.nranks;
+  const float scale = cta_scale(a, epoch, (uint32_t)a.nranks);
   const float* wsrc = P.params[a.rank];
   const int stride = gridDim.x * EARLY_THREADS;
   if (a.mc_grads != nullptr && a.mc_params != nullptr) {
@@ -434,7 +434,7 @@ __global__ void __launch_bounds__(SYNC_THREADS, 1) fused_sync_late_kernel(SyncPe
   if (blockIdx.x == 0 && threadIdx.x == 0) me->t_phase[1] = globaltimer_ns();
 
   // ---- one-shot on the late bucket: every rank sums all contributions in rank order and updates its own copy -------------
-  const float scale = device_lr(a, epoch) / (float)a.nranks;
+  const float scale = cta_scale(a, epoch, (uint32_t)a.nranks);
   float* wdst = P.params[a.rank];
   const int stride = gridDim.x * SYNC_THREADS;
   // late bucket = [begin4, end4) minus the early range: walk a compacted index
@@ -576,7 +576,7 @@ int dm_sync_ctrl_offset(const char* field) {
 
 // peers: arrays of `nranks` device pointers (index = rank; own entries are the local buffers).
 int dm_fused_sync_sgd(void* const* ctrl, void* const* params, void* const* grads, int rank, int nranks, int k,
-                      long long numel, float lr0, float decay_rate, int decay_steps, float drop_keep,
+                      long long numel, double lr0, double decay_rate, int decay_steps, float drop_keep,
                       unsigned int drop_seed, double timeout_ms, void* shadow_bf16, int ctas, void* stream_,
                       const void* mc_grads, void* mc_params) {
   using namespace dm;
@@ -611,8 +611,8 @@ int dm_fused_sync_sgd(void* const* ctrl, void* const* params, void* const* grads
 // Bucketed aggregation, K == N.  phase 1 = early bucket [begin, end) floats, phase 2 = late bucket [begin, end) with the
 // early bucket [early_begin, early_end) named for the shadow refresh.  All offsets are multiples of 4 floats.
 int dm_fused_sync_bucket(void* const* ctrl, void* const* params, void* const* grads, int rank, int nranks, int phase,
-                         long long begin, long long end, long long early_begin, long long early_end, float lr0,
-                         float decay_rate, int decay_steps, double timeout_ms, void* shadow_bf16, int ctas, void* stream_,
+                         long long begin, long long end, long long early_begin, long long early_end, double lr0,
+                         double decay_rate, int decay_steps, double timeout_ms, void* shadow_bf16, int ctas, void* stream_,
                          const void* mc_grads, void* mc_params) {
   using namespace dm;
   if (nranks < 2 || nranks > SYNC_MAX_RANKS || ((begin | end | early_begin | early_end) & 3) || phase < 1 || phase > 2) return -1;

@@ -83,7 +83,7 @@ struct SyncPeers {
 struct SyncArgs {
   int rank, nranks, k;
   int numel4;                 // arena length in float4
-  float lr0, decay_rate;      // staircase exponential decay evaluated on device (reference K12)
+  double lr0, decay_rate;     // staircase exponential decay evaluated on device (reference K12), see cta_scale
   int decay_steps;
   float drop_keep;            // gradient drop-connect keep probability, <= 0: off (reference K14)
   uint32_t drop_seed;
@@ -172,9 +172,18 @@ DMNIST_DEVICE void publish_status(SyncCtrl* me, uint32_t epoch_after, uint32_t a
   me->status_seq = seq + 1;
 }
 
-DMNIST_DEVICE float device_lr(const SyncArgs& a, uint32_t step) {
-  const float p = (float)(step / (uint32_t)max(a.decay_steps, 1));
-  return a.lr0 * __powf(a.decay_rate, p);
+// SGD step size lr(step) / count, as the host schedule (schedule.py) computes it: lr0 * decay_rate^floor(step / decay_steps)
+// and the division in double, rounded to fp32 once.  --use_fast_math leaves double precision alone (fp32 would turn the
+// power into lg2/ex2.approx and the division into div.approx); CUDA's double pow is within 2 ulp, far below fp32 rounding.
+// Thread 0 evaluates it and the CTA reads it after a barrier: every thread of the CTA must call this.
+DMNIST_DEVICE float cta_scale(const SyncArgs& a, uint32_t step, uint32_t count) {
+  __shared__ float s_scale;
+  if (threadIdx.x == 0) {
+    const double p = (double)(step / (uint32_t)max(a.decay_steps, 1));
+    s_scale = (float)(a.lr0 * pow(a.decay_rate, p) / (double)count);
+  }
+  __syncthreads();
+  return s_scale;
 }
 
 // Poll (RELAXED loads inside pred) until pred() or the watchdog fires, then ONE acquire load of the flag the wait was about

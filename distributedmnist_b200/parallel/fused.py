@@ -216,7 +216,7 @@ class FusedBackend(Backend):
         pb, gb = self._by_ptr[params.data_ptr()], self._by_ptr[grads.data_ptr()]
         rc = self.lib.dm_fused_sync_sgd(
             self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), self.ctx.rank, self.ctx.world_size, int(k),
-            ctypes.c_longlong(params.numel()), ctypes.c_float(lr0), ctypes.c_float(decay_rate), int(decay_steps),
+            ctypes.c_longlong(params.numel()), ctypes.c_double(lr0), ctypes.c_double(decay_rate), int(decay_steps),
             ctypes.c_float(self.drop_keep), ctypes.c_uint(self.drop_seed), ctypes.c_double(self.timeout_ms),
             ctypes.c_void_p(0 if self.shadow is None else self.shadow.data_ptr()), int(self.ctas), stream_ptr(stream),
             *self._mc_ptrs(pb, gb))
@@ -235,7 +235,7 @@ class FusedBackend(Backend):
         rc = self.lib.dm_fused_sync_bucket(
             self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), self.ctx.rank, self.ctx.world_size, int(phase),
             ctypes.c_longlong(begin), ctypes.c_longlong(end), ctypes.c_longlong(early_begin), ctypes.c_longlong(early_end),
-            ctypes.c_float(lr0), ctypes.c_float(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
+            ctypes.c_double(lr0), ctypes.c_double(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
             ctypes.c_void_p(0 if self.shadow is None else self.shadow.data_ptr()), int(ctas), stream_ptr(stream),
             *self._mc_ptrs(pb, gb))
         check(rc, "dm_fused_sync_bucket")
@@ -254,7 +254,7 @@ class FusedBackend(Backend):
             self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), g16.ptr_table(),
             inbox.ptr_table() if inbox is not None else None, self.ctx.rank, self.ctx.world_size, int(phase),
             ctypes.c_longlong(fc1_begin), ctypes.c_longlong(fc1_end), ctypes.c_longlong(params.numel()),
-            ctypes.c_float(lr0), ctypes.c_float(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
+            ctypes.c_double(lr0), ctypes.c_double(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
             ctypes.c_void_p(0 if self.shadow is None else self.shadow.data_ptr()), int(ctas), stream_ptr(stream),
             ctypes.c_void_p(mc_g16), ctypes.c_void_p(mc_inbox), int(self.late_ll), int(self.late_bf16))
         check(rc, "dm_bucket_sync(phase %d)" % phase)
@@ -282,8 +282,8 @@ class FusedBackend(Backend):
         pb, gb, ab = self._by_ptr[params.data_ptr()], self._by_ptr[grads.data_ptr()], self._by_ptr[acc.data_ptr()]
         mc = pb.multicast_ptr if (self.use_nvls and pb.multicast_ptr) else 0
         check(self.lib.dm_interval_end(self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), ab.ptr_table(), self.ctx.rank,
-                                       self.ctx.world_size, ctypes.c_longlong(params.numel()), ctypes.c_float(lr0),
-                                       ctypes.c_float(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
+                                       self.ctx.world_size, ctypes.c_longlong(params.numel()), ctypes.c_double(lr0),
+                                       ctypes.c_double(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
                                        int(self.ctas), stream_ptr(stream), ctypes.c_void_p(mc)), "dm_interval_end")
 
     @property
