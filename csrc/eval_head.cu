@@ -46,6 +46,7 @@ struct EvalArgs {
   unsigned int* row_hit;           // [EV_MAX_ROWS]
   EvalState* st;
   const uint32_t* step_ptr;        // device epoch word (global step of the weights), may be null
+  const int32_t* status_ptr;       // snapshot outcome of the pass (csrc/eval_snapshot.cu: attempts, -1 = none), may be null
   unsigned long long* host_ring;   // [slots][EV_RECORD_WORDS] page-locked host memory, null: do not publish
   int ring_slots;
   float* logits_out;               // optional [rows,10]
@@ -164,7 +165,7 @@ __global__ void __launch_bounds__(EV_THREADS) eval_head_kernel(EvalArgs a) {
   rec[4] = st->examples;
   rec[5] = st->correct;
   rec[6] = (unsigned long long)__double_as_longlong(st->loss_sum);
-  rec[7] = 0ull;
+  rec[7] = a.status_ptr ? (unsigned long long)(long long)*a.status_ptr : 0ull;
   __threadfence_system();
   rec[0] = seq;
 }
@@ -182,10 +183,11 @@ int dm_eval_stamp(void* state, void* stream) {
 }
 
 // One chunk of `rows` rows.  row_ws: [EV_MAX_ROWS] fp32 + [EV_MAX_ROWS] u32; state: EvalState opened by dm_eval_stamp.
-// last != 0: the chunk closes the pass and publishes its record into host_ring (if not null).
+// last != 0: the chunk closes the pass and publishes its record into host_ring (if not null).  status_ptr (may be null) is
+// reported in the record's last word: the attempt that produced the pass's weight snapshot, -1 if none was consistent.
 int dm_eval_head(const void* h_part, long long part_stride, int splits, const void* b1, const void* w2, const void* b2,
-                 const void* labels, void* row_ws, void* state, const void* step_ptr, void* host_ring, int ring_slots,
-                 void* logits_out, int rows, int last, void* stream) {
+                 const void* labels, void* row_ws, void* state, const void* step_ptr, const void* status_ptr,
+                 void* host_ring, int ring_slots, void* logits_out, int rows, int last, void* stream) {
   if (splits < 1 || splits > dm::EV_MAX_SPLITS || rows < 1 || rows > dm::EV_MAX_ROWS) return -1;
   if (host_ring != nullptr && ring_slots < 1) return -1;
   dm::EvalArgs a;
@@ -200,6 +202,7 @@ int dm_eval_head(const void* h_part, long long part_stride, int splits, const vo
   a.row_hit = reinterpret_cast<unsigned int*>(reinterpret_cast<float*>(row_ws) + dm::EV_MAX_ROWS);
   a.st = reinterpret_cast<dm::EvalState*>(state);
   a.step_ptr = reinterpret_cast<const uint32_t*>(step_ptr);
+  a.status_ptr = reinterpret_cast<const int32_t*>(status_ptr);
   a.host_ring = reinterpret_cast<unsigned long long*>(host_ring);
   a.ring_slots = ring_slots;
   a.logits_out = reinterpret_cast<float*>(logits_out);

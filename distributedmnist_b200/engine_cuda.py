@@ -621,10 +621,19 @@ class CudaLeNetEngine(ComputeEngine):
     # has fired (in the training loop: the next step's completion event).
     EVAL_CHUNK = 2048
     EVAL_RING = 16                 # host record slots
+    SNAP_ATTEMPTS = 4              # snapshot attempts captured in front of a snapshot pass
+    SNAP_WATCHDOG_MS = 2.0         # how long one attempt waits for the pushes of the newest committed step
+    SNAP_KEEP = False              # also keep the last accepted snapshot (one more 6.65 MB copy per accepted pass), see
+                                   # eval_snapshot(); set before arm_eval
 
-    def arm_eval(self, images, labels) -> None:
+    def arm_eval(self, images, labels, snapshot: bool = False) -> None:
         """Upload the validation set once (device-resident fp32 images, int64 labels) and allocate the pass's buffers and
-        the host record ring.  With ``use_graph`` the whole pass is captured as one CUDA graph."""
+        the host record ring.  With ``use_graph`` the whole pass is captured as one CUDA graph.
+
+        ``snapshot``: peers may push weights into this (the chief's) arena at any time (K < N, interval mode).  The pass then
+        scores a private copy of the newest committed weights that is checked to hold exactly one global step
+        (csrc/eval_snapshot.cu): up to SNAP_ATTEMPTS select / copy / validate attempts run in front of the chunks, and a pass
+        whose attempts all fail is dropped by :meth:`eval_records` (counted in ``eval_dropped``)."""
         self._leave_native_runner()
         lib, dev = self.lib, self.device
         x = torch.as_tensor(np.ascontiguousarray(images) if isinstance(images, np.ndarray) else images, dtype=torch.float32)
@@ -648,8 +657,29 @@ class CudaLeNetEngine(ComputeEngine):
         self._ev_seen = 0
         self._ev_last = None
         self._ev_graph = None
+        self.eval_dropped = 0
+        self._snapshot = bool(snapshot)
+        if self._snapshot:
+            self._snap = torch.zeros(self.spec.arena_numel, dtype=f32, device=dev)
+            # arena-sized so spec.views() applies, but only the conv2 / fc1 weight ranges (_snap_bf_ranges) are ever written
+            # or read: the rest stays zero
+            self._snap16 = torch.zeros(self.spec.arena_numel, dtype=bf, device=dev)
+            self._snap_keep = torch.zeros(self.spec.arena_numel, dtype=f32, device=dev) if self.SNAP_KEEP else None
+            self._snap_state = torch.zeros(int(lib.dm_snap_state_bytes()), dtype=u8, device=dev)
+            # the bf16 operands of the pass: conv2 and fc1 weights (tensor-core kernels); everything else is read as fp32
+            self._snap_bf_ranges = []
+            for name in ("conv2_weights", "fc1_weights"):
+                q = self.spec.param(name)
+                assert q.offset % 4 == 0 and q.numel % 4 == 0, name
+                self._snap_bf_ranges += [q.offset, q.offset + q.numel]
+            self._ev_views = (self.spec.views(self._snap), self.spec.views(self._snap16))
+        else:
+            self._ev_views = (self.p, self.pb)
         self._launch_eval(publish=False)        # sets the kernels' function attributes outside a capture
         torch.cuda.synchronize()
+        if self._snapshot:
+            self._snap_state.zero_()              # statistics count real passes only
+            self._snap_state[40:44].fill_(255)     # SnapState.keep_step: nothing kept yet
         if self.use_graph:
             gr = torch.cuda.CUDAGraph()
             cap = torch.cuda.Stream(device=dev)
@@ -657,13 +687,40 @@ class CudaLeNetEngine(ComputeEngine):
                 self._launch_eval(publish=True)
             self._ev_graph = gr
 
-    def _launch_eval(self, publish: bool, logits_out: Optional[torch.Tensor] = None) -> None:
-        lib, sp, p, pb = self.lib, stream_ptr(), self.p, self.pb
+    def _launch_snapshot(self, attempts: int) -> None:
+        """``attempts`` select / copy / validate rounds (csrc/eval_snapshot.cu); an attempt after an accepted one exits at once."""
+        lib, sp = self.lib, stream_ptr()
+        ctrl = ctypes.c_void_p(self.backend.ctrl.local_ptr)
+        st = ptr(self._snap_state)
+        interval = int(bool(getattr(self, "_interval", False)))
+        r = [ctypes.c_longlong(v) for v in self._snap_bf_ranges]
+        for a in range(attempts):
+            check(lib.dm_snap_select(ctrl, st, a, interval, ctypes.c_double(self.SNAP_WATCHDOG_MS), sp), "snap_select")
+            check(lib.dm_snap_copy(st, ptr(self.params), ptr(self._snap), ptr(self._snap16),
+                                   ctypes.c_longlong(self.spec.arena_numel), *r, sp), "snap_copy")
+            check(lib.dm_snap_validate(ctrl, st, a, attempts, sp), "snap_validate")
+        if self._snap_keep is not None:
+            check(lib.dm_snap_keep(st, ptr(self._snap), ptr(self._snap_keep), ctypes.c_longlong(self.spec.arena_numel), sp),
+                  "snap_keep")
+
+    def _launch_eval(self, publish: bool, logits_out: Optional[torch.Tensor] = None, p=None, pb=None) -> None:
+        """One pass over the validation set with the weight views ``p`` (fp32) / ``pb`` (bf16): by default the armed ones --
+        the live arena, or the snapshot, which the pass then takes first."""
+        if p is None:
+            if self._snapshot:
+                self._launch_snapshot(self.SNAP_ATTEMPTS)
+            p, pb = self._ev_views
+        lib, sp = self.lib, stream_ptr()
         n, C = self._ev_x.shape[0], self._ev_a1.shape[0]
         stride = self._ev_hpart.stride(0)
         conv1_fwd = lib.dm_conv1_fwd_tc if self._conv1_tc else lib.dm_conv1_fwd
         null = ctypes.c_void_p(0)
         ring = ptr(self._ev_ring) if publish else null
+        if self._snapshot and p is self._ev_views[0]:
+            st = self._snap_state.data_ptr()
+            step_ptr, status_ptr = ctypes.c_void_p(st), ctypes.c_void_p(st + 4)     # SnapState.step, SnapState.status
+        else:
+            step_ptr, status_ptr = self._epoch_ptr, null
         check(lib.dm_eval_stamp(ptr(self._ev_state), sp), "eval_stamp")
         for s in range(0, n, C):
             m = min(C, n - s)
@@ -676,8 +733,8 @@ class CudaLeNetEngine(ComputeEngine):
             lg = null if logits_out is None else ptr(logits_out[s:s + m])
             check(lib.dm_eval_head(ptr(self._ev_hpart), ctypes.c_longlong(stride), self.fc1_splits, ptr(p["fc1_biases"]),
                                    ptr(p["fc2_weights"]), ptr(p["fc2_biases"]), ptr(self._ev_y[s:s + m]), ptr(self._ev_ws),
-                                   ptr(self._ev_state), self._epoch_ptr, ring, self.EVAL_RING, lg, m, int(s + m == n), sp),
-                  "eval_head")
+                                   ptr(self._ev_state), step_ptr, status_ptr, ring, self.EVAL_RING, lg, m,
+                                   int(s + m == n), sp), "eval_head")
 
     def enqueue_eval(self) -> None:
         """Score the validation set with the current weights, on the current (training) stream, without a host
@@ -690,11 +747,24 @@ class CudaLeNetEngine(ComputeEngine):
 
     def eval_records(self):
         """Records completed since the previous call, oldest first: ``(global_step, t_begin_ns, t_end_ns, examples,
-        correct, loss_sum)`` (``%globaltimer`` stamps; ``loss_sum`` is the sum of the per-row cross entropies).
+        correct, loss_sum)`` (``%globaltimer`` stamps; ``loss_sum`` is the sum of the per-row cross entropies).  With a
+        snapshot pass, ``global_step`` is the step of the snapshot it scored; a pass that found no consistent snapshot is
+        left out and counted in ``eval_dropped``.
 
         The ring holds the last EVAL_RING records: call this at least once per EVAL_RING enqueued passes.  A caller that
         falls further behind loses the overwritten records, and a slot the device is rewriting while it is read is skipped
         (the training loop reads after every step, with at most two passes outstanding)."""
+        out = []
+        for rec, status in self.eval_records_with_status():
+            if status < 0:
+                self.eval_dropped += 1
+                continue
+            out.append(rec)
+        return out
+
+    def eval_records_with_status(self):
+        """Like :meth:`eval_records`, but every record of the ring, each with its snapshot outcome: 0 for a pass over the
+        live arena, n > 0 when attempt n produced its snapshot, -1 when no attempt did (the record is then meaningless)."""
         raw = self._ev_ring.numpy()
         new = []
         for i in range(self.EVAL_RING):
@@ -705,12 +775,38 @@ class CudaLeNetEngine(ComputeEngine):
             if int(raw[i, 0]) != seq or int(rec[0]) != seq:
                 continue                                 # slot rewritten while it was read: the pass is still running
             loss = float(rec[6:7].view(np.float64)[0])
-            new.append((seq, (int(rec[1]), int(rec[2]), int(rec[3]), int(rec[4]), int(rec[5]), loss)))
+            new.append((seq, (int(rec[1]), int(rec[2]), int(rec[3]), int(rec[4]), int(rec[5]), loss), int(rec[7])))
         new.sort()
         if new:
             self._ev_seen = new[-1][0]
-            self._ev_last = new[-1][1]
-        return [r for _, r in new]
+            good = [r for _, r, st in new if st >= 0]
+            if good:
+                self._ev_last = good[-1]
+        return [(r, st) for _, r, st in new]
+
+    def eval_snapshot(self):
+        """``(fp32 arena, global step)`` of a snapshot, or None (synchronises the current stream).  With ``SNAP_KEEP`` set
+        when the pass was armed: the last ACCEPTED snapshot, kept aside by ``snap_keep``, whatever later passes found.
+        Without it: the newest pass's snapshot if that pass found a consistent one, else None -- a failed attempt overwrites
+        the snapshot buffer, so an older accepted snapshot is gone."""
+        if not getattr(self, "_snapshot", False):
+            return None
+        torch.cuda.current_stream().synchronize()
+        st = self._snap_state[:48].cpu().view(torch.int32).tolist()
+        if self._snap_keep is not None:
+            keep_step = st[10] & 0xFFFFFFFF
+            return None if keep_step == 0xFFFFFFFF else (self._snap_keep.clone(), keep_step)
+        if st[1] <= 0:
+            return None
+        return self._snap.clone(), st[0] & 0xFFFFFFFF
+
+    def eval_snapshot_stats(self) -> dict:
+        """Snapshot attempts since :meth:`arm_eval`: made, rejected by validate, ended by the watchdog, ended because the
+        commit slot of the candidate step was already reused (a ring lap behind); passes accepted / failed (synchronises
+        the current stream)."""
+        torch.cuda.current_stream().synchronize()
+        w = self._snap_state[:40].cpu().view(torch.int32).tolist()
+        return dict(attempts=w[4], rejected=w[5], timeouts=w[6], accepted_passes=w[7], failed_passes=w[8], laps=w[9])
 
     def eval_record(self):
         """The newest complete record (see :meth:`eval_records`), or None."""

@@ -254,7 +254,9 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_integer("log_every", 1, "Log every n-th local iteration (1 = reference behaviour)")
     F.DEFINE_float("dropout_keep_prob", 0.5, "Keep probability of the fc1 dropout (reference mnist.py:139)")
     F.DEFINE_integer("eval_every_steps", 0, "Chief: score the validation set after every E-th global step and after the last "
-                                            "one (test_acc, worker0_eval.npy); 0 = off.  GPU path: lenet, K = N, no interval")
+                                            "one (test_acc, worker0_eval.npy); 0 = off.  GPU path: lenet; K < N or interval need --eval_snapshot")
+    F.DEFINE_boolean("eval_snapshot", False, "GPU path, with --eval_every_steps: score a validated snapshot of the newest "
+                                             "committed weights, so K < N and --interval_method runs can be evaluated too")
     return F
 
 

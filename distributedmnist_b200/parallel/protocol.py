@@ -29,7 +29,7 @@ from __future__ import annotations
 import threading
 import time
 from dataclasses import dataclass
-from typing import Dict, Optional
+from typing import Dict, List, Optional
 
 
 @dataclass
@@ -784,3 +784,114 @@ class KofNModel:
         for r in range(self.n):
             if self.params[r] != [(self.steps, v) for v in w]:
                 raise ProtocolHazard("replica %d ends with %s, expected versions %d values %s" % (r, self.params[r], self.steps, w))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Weight snapshot of the in-training evaluation -- element-level model of csrc/eval_snapshot.cu against the chief's arena
+# ----------------------------------------------------------------------------------------------------------------------
+class SnapshotModel:
+    """The chief's evaluator (``snap_select`` / ``snap_copy`` / ``snap_validate``) against writers that commit steps and push
+    them into the chief's arena element by element, under the same scheduler as :class:`KofNModel`.
+
+    Writers: replica ``g % n`` commits step g (commit word in slot (g - 1) % ring, tag g), pushes every element of the chief's
+    arena as (version g, value), then releases its ``done`` = g.  A writer commits g only after ``done`` of g - 1 (in the
+    kernels a team member of g + 1 is at epoch g, so g's pushes have landed).  ``interval=False`` moves ``global_step`` right
+    after the commit (``decide<KOFN>``), ``interval=True`` after the pushes (``iv_apply``).
+
+    Reader: ``attempts`` attempts, each select / copy / validate as the kernels do it (an attempt whose candidate's commit
+    slot was already reused fails at once); an accepted one must hold every element at exactly the version of the step it
+    reports (``ProtocolHazard`` otherwise).  ``validate=False`` / ``wait_done=False`` remove the two checks the design rests on.
+    """
+
+    def __init__(self, n: int, steps: int, numel: int, interval: bool = False, ring: int = 4, attempts: int = 1,
+                 validate: bool = True, wait_done: bool = True):
+        self.n, self.steps, self.numel, self.interval, self.ring = n, steps, numel, interval, ring
+        self.attempts, self.validate, self.wait_done = attempts, validate, wait_done
+        self.arena = [(0, self.value(0, i)) for i in range(numel)]        # the chief's parameter arena: (version, value)
+        self.commit = [(0, 0)] * ring                                      # chief: (tag, writer)
+        self.global_step = 0
+        self.done = [0] * n                                                # chief's done[q]
+        self.accepted: List[int] = []                                      # steps of accepted snapshots
+
+    @staticmethod
+    def value(g: int, i: int) -> float:
+        return float(100 * g + i)
+
+    def writer(self, r: int):
+        for g in range(1, self.steps + 1):
+            if g % self.n != r:
+                continue
+            yield (lambda g=g: g == 1 or max(self.done) >= g - 1)
+            self.commit[(g - 1) % self.ring] = (g, r)                      # CAS by the committer
+            yield None
+            if not self.interval:
+                self.global_step = max(self.global_step, g)
+                yield None
+            for i in range(self.numel):
+                self.arena[i] = (g, self.value(g, i))                      # one weak push per element
+                yield None
+            if self.interval:
+                self.global_step = max(self.global_step, g)
+                yield None
+            self.done[r] = g                                               # release after the system fence
+            yield None
+
+    def _walk(self, g: int) -> int:
+        for _ in range(self.ring):
+            if self.commit[g % self.ring][0] != g + 1:
+                break
+            g += 1
+        return g
+
+    def reader(self):
+        for _attempt in range(self.attempts):
+            # ---- snap_select ------------------------------------------------------------------------------------------------
+            g = self.global_step
+            yield None
+            g = self._walk(g)
+            yield None
+            lap = False
+            while g > 0:
+                tag, w = self.commit[(g - 1) % self.ring]
+                if tag > g:
+                    lap = True                                             # slot already reused: the attempt fails
+                    break
+                if tag < g or not self.wait_done:
+                    break
+                if self.done[w] >= g:
+                    break
+                # blocked until g's writer releases done or a newer step commits
+                yield (lambda g=g, w=w: self.done[w] >= g or self.commit[g % self.ring][0] == g + 1)
+                g = self._walk(g)
+            if lap:
+                continue
+            # ---- snap_copy --------------------------------------------------------------------------------------------------
+            snap = []
+            for i in range(self.numel):
+                snap.append(self.arena[i])
+                yield None
+            # ---- snap_validate ----------------------------------------------------------------------------------------------
+            if self.validate:
+                tag = self.commit[g % self.ring][0]
+                yield None
+                if tag > g:
+                    continue
+            bad = [(i, v) for i, (v, x) in enumerate(snap) if v != g or x != self.value(g, i)]
+            if bad:
+                raise ProtocolHazard("snapshot accepted as step %d holds element %d of version %d" % (g, bad[0][0], bad[0][1]))
+            self.accepted.append(g)
+            return
+
+    def run(self, choose) -> None:
+        gens = {r: self.writer(r) for r in range(self.n)}
+        gens[self.n] = self.reader()
+        waiting = {}
+        for r in list(gens):
+            BucketV2Model._advance(r, gens, waiting)
+        while gens:
+            runnable = [r for r in sorted(gens) if r not in waiting or waiting[r]()]
+            if not runnable:
+                raise ProtocolHazard("deadlock: %s wait forever (global step %d)" % (sorted(gens), self.global_step))
+            r = choose(runnable)
+            waiting.pop(r, None)
+            BucketV2Model._advance(r, gens, waiting)

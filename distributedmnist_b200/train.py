@@ -156,18 +156,28 @@ def check_eval_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate: int,
         return                     # torch engine: evaluated synchronously with engine.evaluate, every mode and model
     if flags.model != "lenet":
         raise ValueError("--eval_every_steps on the GPU path is implemented for lenet, not --model=%s" % flags.model)
-    # the pass reads the chief's live parameter arena between two of its steps: sound only when no peer can write that
-    # arena then, i.e. when every step waits for all N replicas
+    # the live pass reads the chief's parameter arena between two of its steps: sound only when no peer can write that
+    # arena then, i.e. when every step waits for all N replicas.  --eval_snapshot scores a validated copy instead.
+    if getattr(flags, "eval_snapshot", False):
+        return
+    hint = " (--eval_snapshot=true scores a validated snapshot of the weights instead)"
     if flags.interval_method:
         raise ValueError("--eval_every_steps cannot be combined with --interval_method: interval commits push weights into "
-                         "the chief's arena at any time, so the pass would not see one step's weights")
+                         "the chief's arena at any time, so the pass would not see one step's weights" + hint)
     # --worker_times_cdf_method (without --interval_method, which wins when both are set) always aggregates all N
     # gradients behind a full barrier and ignores --num_replicas_to_aggregate
     cdf = getattr(flags, "worker_times_cdf_method", False)
     if not cdf and num_replicas_to_aggregate < ctx.world_size:
         raise ValueError("--eval_every_steps needs --num_replicas_to_aggregate = number of replicas (%d): with K < N the "
                          "team pushes weights into the chief's arena while it is between steps or late"
-                         % ctx.world_size)
+                         % ctx.world_size + hint)
+
+
+def eval_due(global_step: int, last_mark: int, every: int) -> bool:
+    """Snapshot passes (K < N, interval): the host learns the global step only after a step completes, and it may jump by
+    more than one.  A pass is due once the newest consumed global step has crossed a multiple of ``every`` since
+    ``last_mark``, the global step consumed when the previous pass was enqueued (the restored step before the first)."""
+    return every > 0 and global_step // every > last_mark // every
 
 
 def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
@@ -230,10 +240,16 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     # host memory once the following step has been consumed; torch engine: engine.evaluate, synchronously.
     eval_every = int(getattr(flags, "eval_every_steps", 0) or 0) if is_chief else 0
     device_eval = bool(eval_every and fused_step)
+    exact = isinstance(opt, SyncReplicasOptimizer) and num_replicas_to_aggregate == num_workers \
+        or bool(flags.worker_times_cdf_method and not flags.interval_method)
+    # K < N / interval: peers push into the chief's arena at any time -> score a validated snapshot (--eval_snapshot);
+    # the host cannot name the step a pass scores in advance, so passes follow the consumed global step (eval_due)
+    snapshot_eval = device_eval and bool(getattr(flags, "eval_snapshot", False)) and not exact
     if device_eval:
-        engine.arm_eval(dataset_test.images, dataset_test.labels)
+        engine.arm_eval(dataset_test.images, dataset_test.labels, snapshot=snapshot_eval)
     eval_rows = []                 # (global_step, t_begin_unix_s, eval_seconds, examples, correct, mean_loss)
     last_eval_step = -1
+    eval_mark = restored_step      # snapshot passes: global step consumed when the last one was enqueued
     test_acc_value = 0.0           # newest complete evaluation; hard-wired to 0 in the reference (:363) and when off
 
     def _device_step() -> int:
@@ -275,7 +291,6 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     every = max(flags.log_every, 1)
     pending = None                 # (iteration, start_time, result token) of the step in flight
     launched = 0
-    exact = isinstance(opt, SyncReplicasOptimizer) and num_replicas_to_aggregate == num_workers or cdf
     stop = False
 
     def finish_iteration(it: int, start_time: float, info, loss_acc) -> None:
@@ -321,9 +336,14 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
 
     def eval_after_step(global_step: int) -> None:
         """Non-pipelined loops: called once the step's outcome has been read back."""
-        nonlocal test_acc_value, last_eval_step
+        nonlocal test_acc_value, last_eval_step, eval_mark
         if device_eval:
             collect_evals()        # the step read-back above waited for the pass enqueued after the previous step
+        if snapshot_eval:
+            if global_step <= flags.max_steps and eval_due(global_step, eval_mark, eval_every):
+                eval_mark = global_step
+                engine.enqueue_eval()          # the final pass follows the loop
+            return
         if global_step == last_eval_step or not (global_step % eval_every == 0 or global_step > flags.max_steps):
             return
         last_eval_step = global_step
@@ -369,7 +389,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 log.info("RUNNING SESSION... %f" % time.time())
             token = (cur_iteration, engine.step_packed(packer.next()))   # input DMA + step graph: one native call
             launched += 1
-            if device_eval and ((restored_step + launched) % eval_every == 0 or restored_step + launched > flags.max_steps):
+            if device_eval and not snapshot_eval and \
+                    ((restored_step + launched) % eval_every == 0 or restored_step + launched > flags.max_steps):
                 engine.enqueue_eval()          # K == N: restored_step + launched is the global step of the weights it scores
             prev, pending = pending, token
             if prev is not None:
@@ -381,6 +402,9 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 now = time.time()
                 finish_iteration(it, last_consume, info, (float(lbuf[0]), float(lbuf[1])))
                 last_consume = now
+                if snapshot_eval and not stop and eval_due(step, eval_mark, eval_every):
+                    eval_mark = step
+                    engine.enqueue_eval()      # after the step just launched: scores the newest committed weights then
                 if device_times and it > 10 and (it % 50 == 0 or it == 500):
                     push_device_times(it)
             # K == N: the global step after `launched` steps is known without reading anything -> stop launching exactly there
@@ -450,9 +474,14 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         pending = None
     if packer is not None:
         packer.close()
+    if snapshot_eval:
+        engine.enqueue_eval()          # once after the last step
     if device_eval:
         torch.cuda.synchronize()       # the pass after the final step
         collect_evals()
+        if snapshot_eval and engine.eval_dropped:
+            log.info("in-training evaluation: %d pass(es) found no consistent weight snapshot and were dropped"
+                     % engine.eval_dropped)
     if eval_every:
         save_evals()
     if device_times:

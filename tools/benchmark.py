@@ -20,7 +20,7 @@ import os
 import re
 import sys
 import time
-from typing import Dict, List, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
 
@@ -204,18 +204,30 @@ def plot_time_precision(outdir: str, dest: str = ".") -> str:
                      "time (s)", "precision")
 
 
-def plot_device_time_precision(train_dir: str, dest: str = ".") -> str:
-    """Accuracy against training time from the chief's in-training evaluations (``--eval_every_steps``,
-    ``worker0_eval.npy``: global_step, t_begin_unix_s, eval_seconds, examples, correct, mean_loss).  The time axis starts at
-    the first evaluation and leaves out the time spent in the evaluations before each point."""
+def _device_eval_curve(train_dir: str):
     rows = np.load(os.path.join(train_dir, "worker0_eval.npy")).reshape(-1, 6)
     rows = rows[np.argsort(rows[:, 1], kind="stable")]
     spent = np.concatenate([[0.0], np.cumsum(rows[:-1, 2])])          # evaluation time before each pass began
     t = rows[:, 1] - rows[0, 1] - spent
     acc = rows[:, 4] / np.maximum(rows[:, 3], 1)
-    return line_plot(os.path.join(dest, "device_time_precision.png"),
-                     [(os.path.basename(os.path.normpath(train_dir)), t.tolist(), acc.tolist())],
-                     "training time (s, evaluation excluded)", "precision")
+    return t.tolist(), acc.tolist()
+
+
+def plot_device_time_precision(train_dirs, dest: str = ".", labels: Optional[Sequence[str]] = None) -> str:
+    """Accuracy against training time from the chief's in-training evaluations (``--eval_every_steps``,
+    ``worker0_eval.npy``: global_step, t_begin_unix_s, eval_seconds, examples, correct, mean_loss).  The time axis starts at
+    the first evaluation and leaves out the time spent in the evaluations before each point.
+
+    ``train_dirs``: one train dir, or several (e.g. a K sweep, one run per K) drawn as one curve each, named by ``labels``
+    (default: the directories' base names)."""
+    dirs = [train_dirs] if isinstance(train_dirs, str) else list(train_dirs)
+    if labels is None:
+        labels = [os.path.basename(os.path.normpath(d)) for d in dirs]
+    if len(labels) != len(dirs):
+        raise ValueError("%d labels for %d train dirs" % (len(labels), len(dirs)))
+    series = [(lab,) + _device_eval_curve(d) for lab, d in zip(labels, dirs)]
+    return line_plot(os.path.join(dest, "device_time_precision.png"), series, "training time (s, evaluation excluded)",
+                     "precision")
 
 
 def plot_step_loss(outdir: str, dest: str = ".") -> str:

@@ -9,7 +9,11 @@ the pass's own %globaltimer stamps (records) and from CUDA events around passes 
 only its own device time, the measured overhead matches ``t_eval / (E * t_step)``; a larger one means a pipeline bubble or
 a host stall.
 
-    python tools/eval_overhead.py [--steps 2000] [--rounds 3] [--batch 256] [--out results/eval_overhead.json]
+    python tools/eval_overhead.py [--steps 2000] [--rounds 3] [--batch 256] [--snapshot] [--out results/eval_overhead.json]
+
+``--snapshot`` adds the cost of the weight snapshot that K < N and interval runs score (``--eval_snapshot``): the pass
+with and without it, and the snapshot attempts alone (one accepted attempt and three that exit at once), CUDA events
+between steps, quiescent weights.
 """
 import argparse
 import json
@@ -55,11 +59,43 @@ def window(eng, bufs, steps, every, first):
     return e0.elapsed_time(e1) * 1e-3 / steps, eng.eval_records()
 
 
+def _event_median(eng, bufs, done, fn, reps=20):
+    """Median device time of fn() enqueued between two training steps (CUDA events on the training stream)."""
+    times = []
+    for i in range(reps):
+        tok = eng.step_packed(bufs[(done + i) % len(bufs)])
+        e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+        e0.record()
+        fn()
+        e1.record()
+        tok[0].synchronize()
+        torch.cuda.synchronize()
+        times.append(e0.elapsed_time(e1) * 1e-3)
+    return float(np.median(times)), done + reps
+
+
+def snapshot_cost(eng, tex, tey, bufs, done):
+    eng.arm_eval(tex, tey)
+    live, done = _event_median(eng, bufs, done, eng.enqueue_eval)
+    eng.arm_eval(tex, tey, snapshot=True)
+    snap, done = _event_median(eng, bufs, done, eng.enqueue_eval)
+    attempts, done = _event_median(eng, bufs, done, lambda: eng._launch_snapshot(eng.SNAP_ATTEMPTS))
+    eng.eval_records()
+    st = eng.eval_snapshot_stats()
+    eng._leave_native_runner()
+    arena = eng.spec.arena_numel
+    bf = sum(e - b for b, e in zip(eng._snap_bf_ranges[0::2], eng._snap_bf_ranges[1::2]))
+    return {"pass_live_us": live * 1e6, "pass_snapshot_us": snap * 1e6, "snapshot_attempts_us": attempts * 1e6,
+            "snapshot_share_of_pass": (snap - live) / snap, "bytes_read": 4 * arena, "bytes_written_f32": 4 * arena,
+            "bytes_written_bf16": 2 * bf, "stats": st}
+
+
 def main():
     ap = argparse.ArgumentParser()
     ap.add_argument("--steps", type=int, default=2000)
     ap.add_argument("--rounds", type=int, default=3)
     ap.add_argument("--batch", type=int, default=256)
+    ap.add_argument("--snapshot", action="store_true", help="also measure the weight snapshot of --eval_snapshot")
     ap.add_argument("--out", default="")
     a = ap.parse_args()
     if not torch.cuda.is_available():
@@ -114,6 +150,9 @@ def main():
         res["overhead"]["E=%d" % e] = {"implied": t_eval / (e * base), "measured": float(np.mean(t_step[e])) / base - 1.0,
                                        "measured_min": float(np.min(t_step[e])) / float(np.max(t_step[0])) - 1.0,
                                        "measured_max": float(np.max(t_step[e])) / float(np.min(t_step[0])) - 1.0}
+    if a.snapshot:
+        res["snapshot"] = snapshot_cost(eng, tex, tey, bufs, done)
+        be.check_error()
     line = json.dumps(res)
     print(line)
     if a.out:
