@@ -4,13 +4,14 @@
 //
 // No im2col buffer exists anywhere: activations stay NHWC bf16 and a tile's whole receptive field is
 // one 4-D TMA box (channels, 12 pixels of a row, 20 rows, 1 image); the SAME padding halo and the
-// 14 -> 16 row/column round-up are TMA out-of-bounds zero fill.  An M tile is 128 pixels (16 rows x
-// 8 columns, 112 or 84 of them real) of one image; two tiles cover an image.
+// 14 -> 16 row/column round-up are TMA out-of-bounds zero fill.  In fwd and dgrad an M tile is 128 pixels
+// (16 rows x 8 columns, 112 or 84 of them real) of one image; two tiles cover an image.
 //
 //   fwd    D[pixel, co]  += X[pixel + tap, ci] (A: registers)  * W[tap][ci][co] (B: MN-major smem, 128B swizzle)
 //   dgrad  D[pixel, ci]  += dY[pixel - tap, co] (A: registers) * W[tap][ci][co] (B: K-major smem,  128B swizzle)
 //   wgrad  D[(tap,ci), co] += X[pixel + tap, ci] (A: registers, transposed) * dY[pixel, co] (B: MN-major smem),
-//          K = pixels, split over CTAs whose partial sums are added up in a fixed order (bit-reproducible).
+//          K = the pixels of whole images (an 18 x 18 patch and 208 dY rows per image), split over CTAs whose
+//          partial sums a second kernel adds up in a fixed order (bit-reproducible).
 // The A operand of every tap is the same patch shifted by (kh, kw): a window that starts at an arbitrary
 // pixel of the swizzled patch, so each warp gathers its 16 rows with ldmatrix (addresses computed with the
 // TMA swizzle) and hands them to wgmma in registers; B always starts on a swizzle-atom boundary and is
@@ -309,46 +310,47 @@ conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,1
 }
 
 // ------------------------------------------------------------------------------------------------------
-// wgrad: CTA = (group of 4 taps, slice of the pixel tiles).  Per pixel tile (16 rows x 8 columns) a stage
-// holds the same 20 x 12 input patch as the forward pass (15 KB, A operand for every tap of the group) and
-// the 16 x 8 tile of dY (16 KB, B operand).  M = (tap, ci): the four taps of a group are 32-row M-chunks
-// (warps 2q, 2q + 1 hold chunk q) whose windows start at
+// wgrad: CTA = (group of 4 taps, slice of the images).  K = the 196 pixels of one image, padded to 208 = 13 K steps of
+// 16.  Per image a stage holds the image's 18 x 18 zero-padded input patch (20 KB, A operand for every tap of the
+// group) and the image's dY, 208 pixels x 64 co (26 KB, B operand; pixels 196-207 are TMA out-of-bounds zero fill).
+// M = (tap, ci): the four taps of a group are 32-row M-chunks (warps 2q, 2q + 1 hold chunk q) whose windows start at
 //     group g < 5 : taps (kh = 0..3, kw = g)
 //     group 5     : taps (kh = 4, kw = 0..3)
 //     group 6     : tap  (kh = 4, kw = 4) + three padding chunks (zero operands, never stored)
 // ------------------------------------------------------------------------------------------------------
-constexpr int WG_STAGES = 4;
-constexpr int WG_A_BYTES = 20 * 12 * 32 * 2;   // 15 KB patch
-constexpr int WG_B_BYTES = 128 * 64 * 2;       // 16 KB dY tile
-constexpr int WG_STAGE_BYTES = WG_A_BYTES + WG_B_BYTES + 1024;   // keep the dY tile 1024-aligned (128B swizzle)
+constexpr int WG_STAGES = 3;
+constexpr int WG_KSTEPS = 13;                        // 208 / 16
+constexpr int WG_A_BYTES = 18 * 18 * 32 * 2;         // 20736: the patch
+constexpr int WG_A_SLOT = 21 * 1024;                 // keeps the dY tile 1024-aligned (128B swizzle)
+constexpr int WG_B_BYTES = 16 * WG_KSTEPS * 64 * 2;  // 26624: the dY tile
+constexpr int WG_STAGE_BYTES = WG_A_SLOT + WG_B_BYTES;
 constexpr int WG_GROUPS = 7;
+static_assert(WG_A_BYTES <= WG_A_SLOT, "the patch runs into the dY tile");
 struct WgSmem {
   static constexpr int BAR_OFF = WG_STAGES * WG_STAGE_BYTES;
-  static constexpr int TOTAL = BAR_OFF + 256 + 1024;
+  static constexpr int TOTAL = BAR_OFF + 256 + 1024;   // 145664: a 65 KB conv1_wgrad CTA fits beside it
 };
-// Partial sums of one tap group of one CTA ([4 M-chunks][32 ci][64 co]), reduced in pixel-slice order by the last CTA of
-// the group's set (see arrive_last_cta).
+// Partial sums of one tap group of one CTA ([4 M-chunks][32 ci][64 co]), added up in image-slice order by
+// conv2_wgrad_reduce_kernel.
 constexpr int WG_PART_FLOATS = 4 * 32 * 64;
 constexpr int WG_MAX_PARTS = 160;
-// One launch of this kernel in flight per device: the workspace and ticket are static (see arrive_last_cta).
+// One launch of this kernel pair in flight per device: the workspace is static.
 __device__ float g_c2wg_part[WG_MAX_PARTS * WG_PART_FLOATS];
-__device__ unsigned int g_c2wg_ticket[WG_GROUPS];
 
-// CTA = (tap group, pixel slice): blockIdx.x = split * WG_GROUPS + group.
+// CTA = (tap group, image slice): blockIdx.x = split * WG_GROUPS + group.  Every CTA stores its partial sums: the reduction
+// reads all WG_GROUPS * splits slots of the launch.
 __global__ void __launch_bounds__(CV_THREADS, 1)
-conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,12,20,1), 64B swizzle
-                   const __grid_constant__ CUtensorMap tmDY,   // dY, box (64,8,16,1), 128B swizzle
-                   float* __restrict__ g_w,                    // [25][32][64] fp32, the gradient is added to it
-                   int num_tiles, int splits) {
+conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,18,18,1), 64B swizzle
+                   const __grid_constant__ CUtensorMap tmDY,   // dY as [B][196][64], box (64,208,1), 128B swizzle
+                   int B, int splits) {
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* full = reinterpret_cast<uint64_t*>(smem + WgSmem::BAR_OFF);
   uint64_t* empty = full + WG_STAGES;
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const int group = blockIdx.x % WG_GROUPS, split = blockIdx.x / WG_GROUPS;
-  const int t_begin = (int)(((long long)num_tiles * split) / splits);
-  const int t_end = (int)(((long long)num_tiles * (split + 1)) / splits);
-  const int nt = t_end - t_begin;
+  const int img0 = (int)(((long long)B * split) / splits);
+  const int ni = (int)(((long long)B * (split + 1)) / splits) - img0;
 
   if (warp == 8 && lane == 0) {
     tma_prefetch_desc(&tmX);
@@ -362,54 +364,76 @@ conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,12
 
   if (warp == 8) {
     if (lane == 0) {
-      for (int i = 0; i < nt; ++i) {
-        const int t = t_begin + i, img = t >> 1, w0 = (t & 1) * 8;
+      for (int i = 0; i < ni; ++i) {
         const int s = i % WG_STAGES;
         mbar_wait(&empty[s], ((i / WG_STAGES) & 1) ^ 1);
-        uint8_t* sA = smem + s * WG_STAGE_BYTES;
+        uint8_t* st = smem + s * WG_STAGE_BYTES;
         mbar_expect_tx(&full[s], WG_A_BYTES + WG_B_BYTES);
-        tma_load_4d(sA, &tmX, &full[s], 0, w0 - 2, -2, img);
-        tma_load_4d(sA + WG_A_BYTES + 1024, &tmDY, &full[s], 0, w0, 0, img);
+        tma_load_4d(st, &tmX, &full[s], 0, -2, -2, img0 + i);
+        tma_load_4d(st + WG_A_SLOT, &tmDY, &full[s], 0, 0, img0 + i, 0);
       }
     }
     return;
   }
 
-  // A^T via ldmatrix.trans: x4 tile i covers ci + 8 (i & 1) and pixels + 8 (i >> 1); K step ks = pixels 16 ks ..
-  // 16 ks + 15 = tile rows 2 ks, 2 ks + 1, so this lane's pixel is (h = 2 ks + (lane >> 4), w = lane & 7)
+  // A^T via ldmatrix.trans: x4 tile i covers ci + 8 (i & 1) and pixels + 8 (i >> 1), so in K step ks this lane supplies
+  // the row of pixel p = 16 ks + px, which tap (kh, kw) reads at patch pixel (p / 14 + kh) * 18 + p % 14 + kw.  The pad
+  // pixels 196-207 (K step 12, px >= 4) meet zero dY rows; they read patch pixel 0, halo for every tap, so even their
+  // products are exact zeros.
   const int q = warp >> 1;                         // M-chunk (tap of the group) of this warp's 16 rows
   const int chunk = 2 * (warp & 1) + ((lane >> 3) & 1);   // 16-byte channel chunk (8 ci)
-  const int lh = lane >> 4, lw = lane & 7;
-  // first pixel of this chunk's tap window inside the patch; group 6 chunks 1-3 are padding
-  const int base_px = group < 5 ? q * 12 + group : (group == 5 ? 48 + q : 52);
+  const int px = 8 * (lane >> 4) + (lane & 7);
+  // patch pixel of this chunk's tap window for image pixel 0; group 6 chunks 1-3 are padding
+  const int tap_px = group < 5 ? q * 18 + group : (group == 5 ? 4 * 18 + q : 4 * 18 + 4);
   const bool real_chunk = group < 6 || q == 0;
   float acc[32];
 #pragma unroll
   for (int j = 0; j < 32; ++j) acc[j] = 0.f;
-  for (int i = 0; i < nt; ++i) {
-    const int s = i % WG_STAGES;
-    mbar_wait(&full[s], (i / WG_STAGES) & 1);
-    const uint32_t patch = smem_u32(smem + s * WG_STAGE_BYTES);
-    // B (MN-major, 128B swizzle): [pixel][64 co], 8-pixel groups 1024 B apart; K step = 16 pixels = 2048 B.
-    const uint64_t db0 = make_smem_desc(patch + WG_A_BYTES + 1024, 8192, 1024, SWZ_128B);
-    fence_regs(acc);
+  fence_regs(acc);
+  // One commit group per K step and a two-deep register ring running across image boundaries, as in the forward tap
+  // loop: step k + 1's A fragment is gathered while step k's wgmma runs, and only the wait_group 1 after step k + 1
+  // frees step k's registers.  An image's stage is released once the first wgmma of the next image has been issued and
+  // the wait after it has returned, i.e. the last wgmma reading the stage has completed.  The loop body covers two images
+  // so that the ring's register index is a compile-time constant (13 steps per image).
+  uint32_t a[2][4];
+  uint32_t patch = 0;
+  uint64_t db0 = 0;
+  int s = 0, s_prev = 0;
+  uint32_t phase = 0;
+  for (int i0 = 0; i0 < ni; i0 += 2) {
 #pragma unroll
-    for (int ks = 0; ks < 8; ++ks) {
-      uint32_t a[4];
+    for (int k = 0; k < 2 * WG_KSTEPS; ++k) {
+      const int ks = k % WG_KSTEPS;
+      if (ks == 0) {
+        if (k != 0 && i0 + 1 >= ni) break;
+        mbar_wait(&full[s], phase);
+        patch = smem_u32(smem + s * WG_STAGE_BYTES);
+        // B (MN-major, 128B swizzle): [pixel][64 co], 8-pixel groups 1024 B apart; K step = 16 pixels = 2048 B.
+        db0 = make_smem_desc(patch + WG_A_SLOT, 8192, 1024, SWZ_128B);
+      }
       if (real_chunk) {
-        ldsm_x4_trans(patch_addr<64>(patch, base_px + (2 * ks + lh) * 12 + lw, chunk), a);
+        const int p = 16 * ks + px;
+        const int pix = (ks == WG_KSTEPS - 1 && px >= 4) ? 0 : tap_px + p + 4 * (p / 14);
+        ldsm_x4_trans(patch_addr<64>(patch, pix, chunk), a[k & 1]);
       } else {
-        a[0] = a[1] = a[2] = a[3] = 0u;
+        a[k & 1][0] = a[k & 1][1] = a[k & 1][2] = a[k & 1][3] = 0u;
       }
       wgmma_fence();
-      wgmma_m64n64_rs<1>(acc, a, desc_advance(db0, 2048 * ks), 1);
+      wgmma_m64n64_rs<1>(acc, a[k & 1], desc_advance(db0, 2048 * ks), 1);
+      wgmma_commit();
+      wgmma_wait<1>();
+      if (ks == 0) {
+        if (i0 + k > 0) {
+          __syncwarp();
+          if (lane == 0) mbar_arrive(&empty[s_prev]);
+        }
+        s_prev = s;
+        if (++s == WG_STAGES) { s = 0; phase ^= 1; }
+      }
     }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(acc);
-    __syncwarp();
-    if (lane == 0) mbar_arrive(&empty[s]);
   }
+  wgmma_wait<0>();
+  fence_regs(acc);
 
   const int ci0 = 16 * (warp & 1) + (lane >> 2);
   float* part = g_c2wg_part + (size_t)blockIdx.x * WG_PART_FLOATS;
@@ -419,20 +443,27 @@ conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,12
 #pragma unroll
     for (int j = 0; j < 8; ++j) *reinterpret_cast<float2*>(o + 8 * j) = make_float2(acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
   }
-  __shared__ unsigned int s_last;
-  if (arrive_last_cta(&g_c2wg_ticket[group], splits, 1, CV_CONSUMERS, &s_last)) {
-    for (int e4 = threadIdx.x; e4 < WG_PART_FLOATS / 4; e4 += CV_CONSUMERS) {
-      const int row = e4 >> 4, co = (e4 & 15) * 4;        // row = M-chunk * 32 + ci
-      const int qq = row >> 5, ci = row & 31;
-      const int tap = group < 5 ? qq * 5 + group : (group == 5 ? 20 + qq : (qq == 0 ? 24 : 25));
-      if (tap >= 25) continue;
-      const float4 sum = ordered_sum4(reinterpret_cast<const float4*>(g_c2wg_part + (size_t)group * WG_PART_FLOATS) + e4,
-                                      splits, (size_t)WG_GROUPS * WG_PART_FLOATS / 4);
-      float4* o = reinterpret_cast<float4*>(g_w + ((size_t)tap * 32 + ci) * 64 + co);
-      const float4 cur = *o;
-      *o = make_float4(cur.x + sum.x, cur.y + sum.y, cur.z + sum.z, cur.w + sum.w);
-    }
-  }
+}
+
+// g_w += the sum of the partials over the image slices, in slice order.  Thread = 4 output channels of one (tap, ci):
+// 25 x 32 x 16 = 12800 threads, so the 4 MB of partials are read by the whole machine at once.  Chained to
+// conv2_wgrad_kernel by programmatic dependent launch: its launch overlaps the weight-gradient kernel's last CTAs.
+constexpr int WGR_THREADS = 64;
+constexpr int WGR_ITEMS = 25 * 32 * 64 / 4;
+__global__ void __launch_bounds__(WGR_THREADS)
+conv2_wgrad_reduce_kernel(float* __restrict__ g_w, int splits) {
+  pdl_wait();
+  const int e4 = blockIdx.x * WGR_THREADS + threadIdx.x;
+  if (e4 >= WGR_ITEMS) return;
+  const int tap = e4 >> 9, row4 = e4 & 511;        // row4 = ci * 16 + co / 4
+  const int kh = tap / 5, kw = tap % 5;
+  const int group = kh < 4 ? kw : (kw < 4 ? 5 : 6);
+  const int q = kh < 4 ? kh : (kw < 4 ? kw : 0);
+  const float4 sum = ordered_sum4(reinterpret_cast<const float4*>(g_c2wg_part + (size_t)group * WG_PART_FLOATS) + q * 512 + row4,
+                                  splits, (size_t)WG_GROUPS * WG_PART_FLOATS / 4);
+  float4* o = reinterpret_cast<float4*>(g_w) + e4;
+  const float4 cur = *o;
+  *o = make_float4(cur.x + sum.x, cur.y + sum.y, cur.z + sum.z, cur.w + sum.w);
 }
 
 }  // namespace dm
@@ -481,24 +512,28 @@ int dm_conv2_dgrad_dbg(const void* dy, const void* w_bf16, void* dx, int B, void
                             reinterpret_cast<unsigned long long*>(dbg));
 }
 
-// g_w ([25][32][64] fp32) must be zeroed by the caller; the gradient is added to it.
+// g_w ([25][32][64] fp32) must be zeroed by the caller; the gradient is added to it.  Two launches: the weight-gradient
+// kernel and the reduction of its partial sums.
 int dm_conv2_wgrad(const void* a1, const void* dy, void* g_w, int B, void* stream) {
   using namespace dm;
   CUtensorMap tmX, tmDY;
-  if (make_tmap_nhwc_bf16(&tmX, a1, 32, 14, 14, B, 32, 12, 20, 64)) return 101;
-  if (make_tmap_nhwc_bf16(&tmDY, dy, 64, 14, 14, B, 64, 8, 16, 128)) return 102;
-  const int tiles = 2 * B;
+  if (make_tmap_nhwc_bf16(&tmX, a1, 32, 14, 14, B, 32, 18, 18, 64)) return 101;
+  // dY viewed as [B][196 pixels][64 co]: the 208-pixel box ends in zero fill rather than in the next image
+  if (make_tmap_nhwc_bf16(&tmDY, dy, 64, 196, B, 1, 64, 16 * WG_KSTEPS, 1, 128)) return 102;
   int splits = max_ctas() / WG_GROUPS;
   if (splits * WG_GROUPS > WG_MAX_PARTS) splits = WG_MAX_PARTS / WG_GROUPS;
-  if (splits > tiles) splits = tiles;
+  if (splits > B) splits = B;
   static bool configured = false;
   if (!configured) {
     DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem::TOTAL));
     DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }
-  return (int)launch_kernel(conv2_wgrad_kernel, dim3(WG_GROUPS * splits), dim3(CV_THREADS), WgSmem::TOTAL,
-                            reinterpret_cast<cudaStream_t>(stream), tmX, tmDY, reinterpret_cast<float*>(g_w), tiles, splits);
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  DM_CUDA_OK(launch_kernel(conv2_wgrad_kernel, dim3(WG_GROUPS * splits), dim3(CV_THREADS), WgSmem::TOTAL, st, tmX, tmDY,
+                           B, splits));
+  return (int)launch_kernel(conv2_wgrad_reduce_kernel, dim3(WGR_ITEMS / WGR_THREADS), dim3(WGR_THREADS), 0, st,
+                            reinterpret_cast<float*>(g_w), splits);
 }
 
 }  // extern "C"

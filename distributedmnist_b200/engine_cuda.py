@@ -13,7 +13,8 @@ Step = (reference src/distributed_train.py:332 ``sess.run(apply_gradients_op)``)
     fc1_wgrad        wgmma GEMM (MN-major x MN-major) -> gradient arena
     fc1_dgrad        wgmma GEMM -> bf16
     unpool2          maxpool2/ReLU2 backward + conv2 bias grad
-    conv2_wgrad      wgmma, K = pixels, per-CTA partials summed in fixed order -> gradient arena
+    conv2_wgrad      wgmma, K = whole images, per-CTA partials -> workspace
+    conv2_wgrad_reduce  the partials summed in fixed order -> gradient arena
     conv2_dgrad      wgmma
     conv1_wgrad      maxpool1/ReLU1 backward + conv1 weight/bias grad
     fused_sync_sgd   arrival -> mask -> NVLink reduce -> 1/count -> SGD -> push -> bf16 shadow
@@ -407,7 +408,7 @@ class CudaLeNetEngine(ComputeEngine):
             main.wait_event(join1)
             if early_sync:
                 main.wait_event(join3)
-        return 6 if self._fuse_unpool else 7
+        return 7 if self._fuse_unpool else 8     # (conv2_wgrad is two launches: the kernel and its reduction)
 
     def _zero_args(self, train: bool):
         """Regions conv1_fwd clears at the start of a training step (atomically accumulated gradients + loss)."""
