@@ -31,11 +31,16 @@ DMNIST_DEVICE bool elect_one() {
   return pred != 0;
 }
 
-// Counter-based dropout: identical to models/lenet.py::dropout_keep_mask.
-DMNIST_DEVICE bool dropout_keep(uint32_t seed_mix, uint32_t idx, uint32_t thresh24) {
+// Counter-based hash: murmur3's 32-bit finaliser over idx * golden ratio + seed_mix.
+DMNIST_DEVICE uint32_t hash_mix(uint32_t seed_mix, uint32_t idx) {
   uint32_t x = idx * 0x9E3779B1u + seed_mix;
   x ^= x >> 16; x *= 0x85EBCA6Bu; x ^= x >> 13; x *= 0xC2B2AE35u; x ^= x >> 16;
-  return (x >> 8) < thresh24;
+  return x;
+}
+
+// Counter-based dropout: identical to models/lenet.py::dropout_keep_mask.
+DMNIST_DEVICE bool dropout_keep(uint32_t seed_mix, uint32_t idx, uint32_t thresh24) {
+  return (hash_mix(seed_mix, idx) >> 8) < thresh24;
 }
 
 DMNIST_DEVICE uint32_t pack_bf16x2(float lo, float hi) {

@@ -530,6 +530,41 @@ __global__ void straggler_delay_kernel(const SyncCtrl* ctrl, float prob, unsigne
   }
 }
 
+// Sampled straggler injection (--inject_straggler rank:exp|lognormal|profile:...): every launch draws the delay of the
+// replica's next iteration from a quantile table and spins for it.  The iteration counter lives in a caller-owned state
+// block, so each replay of a captured graph draws the next sample; parallel/straggler.py emulates the draw bit for bit.
+constexpr int STRAGGLER_POINTS = 1025;     // table points at probabilities (i + 0.5) / 1025
+constexpr int STRAGGLER_RING = 1024;
+struct StragglerState {
+  uint32_t counter;                                  // iterations drawn so far = index of the next draw
+  uint32_t pad[3];
+  uint32_t sample_ns[STRAGGLER_RING];                // drawn delay of iteration j, at j % STRAGGLER_RING
+  unsigned long long spin_ns[STRAGGLER_RING];        // %globaltimer end - start of that iteration's spin
+};
+
+// u = hash(seed_mix, j): its top 10 bits pick a table segment, the next 16 the position inside it (linear interpolation).
+__device__ __forceinline__ uint32_t straggler_draw_ns(const uint32_t* __restrict__ table, uint32_t seed_mix, uint32_t j) {
+  const uint32_t u = hash_mix(seed_mix, j);
+  const uint32_t seg = u >> 22, frac = (u >> 6) & 0xFFFFu;
+  const unsigned long long lo = table[seg], hi = table[seg + 1];
+  return (uint32_t)(lo + (((hi - lo) * frac) >> 16));
+}
+
+__global__ void straggler_sample_kernel(StragglerState* st, const uint32_t* __restrict__ table, uint32_t seed_mix) {
+  const uint32_t j = st->counter;
+  st->counter = j + 1;
+  const uint32_t ns = straggler_draw_ns(table, seed_mix, j);
+  const unsigned long long t0 = globaltimer_ns();
+  unsigned long long t = t0;
+  while (t - t0 < ns) {
+    const unsigned long long left = ns - (t - t0);
+    __nanosleep(left < 1000ull ? (unsigned int)left : 1000u);
+    t = globaltimer_ns();
+  }
+  st->sample_ns[j % STRAGGLER_RING] = ns;
+  st->spin_ns[j % STRAGGLER_RING] = t - t0;
+}
+
 // Device-side barrier over NVLink flags: returns on every replica within a flag hop of the LAST replica entering it.
 // Used to align the replicas' streams (e.g. right before a timed region: a host-side barrier leaves tens of microseconds of
 // start skew between the processes).
@@ -674,6 +709,16 @@ int dm_f32_to_bf16(const void* src, void* dst, long long numel, void* stream_) {
 int dm_straggler_delay(const void* ctrl, float prob, unsigned int usec, unsigned int seed, void* stream_) {
   dm::straggler_delay_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
       reinterpret_cast<const dm::SyncCtrl*>(ctrl), prob, usec, seed);
+  return (int)cudaGetLastError();
+}
+
+int dm_straggler_state_bytes() { return (int)sizeof(dm::StragglerState); }
+
+// state: a zeroed block of dm_straggler_state_bytes(); table: dm::STRAGGLER_POINTS monotone uint32 nanosecond points.
+int dm_straggler_sample(void* state, const void* table, unsigned int seed_mix, void* stream_) {
+  if (!state || !table || (reinterpret_cast<uintptr_t>(state) & 7) || (reinterpret_cast<uintptr_t>(table) & 3)) return -1;
+  dm::straggler_sample_kernel<<<1, 1, 0, reinterpret_cast<cudaStream_t>(stream_)>>>(
+      reinterpret_cast<dm::StragglerState*>(state), reinterpret_cast<const uint32_t*>(table), seed_mix);
   return (int)cudaGetLastError();
 }
 

@@ -239,6 +239,8 @@ class CudaLeNetEngine(ComputeEngine):
         if getattr(opt, "drop_connect_probability", None) is not None:
             self.backend.drop_connect_(self.grads, opt.drop_connect_probability, 0)
         self._straggler = getattr(opt, "_straggler", None)
+        if self._straggler is not None:
+            self.backend.arm_straggler(self._straggler)      # sampled forms: table + iteration counter on the device
         self._stamp = getattr(opt, "mode", "") == "cdf"
         self._graphs = [None, None]
         self._runner = None                  # graphs are re-captured: the native runner is rebuilt on demand
@@ -360,7 +362,7 @@ class CudaLeNetEngine(ComputeEngine):
             with torch.cuda.stream(self._side[0]):
                 self._side[0].wait_event(ev_du)
                 if self._straggler is not None and not getattr(self, "_delay_in_chain", False):
-                    self.backend.enqueue_straggler_delay(self._straggler.prob, self._straggler.usec, stream=self._side[0])
+                    self.backend.enqueue_straggler(self._straggler, stream=self._side[0])
                 oa = self._opt_args
                 e0, e1 = self._bucket_early
                 if self._bucket_v2:
@@ -501,7 +503,7 @@ class CudaLeNetEngine(ComputeEngine):
             n += 1
             if bucketed and self._straggler is not None:
                 # cdf telemetry: the injected delay is part of THIS replica's compute (start stamp .. gradient-complete stamp)
-                self.backend.enqueue_straggler_delay(self._straggler.prob, self._straggler.usec)
+                self.backend.enqueue_straggler(self._straggler)
                 self._delay_in_chain = True
                 n += 1
         if interval:
@@ -522,7 +524,7 @@ class CudaLeNetEngine(ComputeEngine):
             n += 2 + (1 if self._straggler is not None else 0)
         elif with_sync:
             if self._straggler is not None:
-                self.backend.enqueue_straggler_delay(self._straggler.prob, self._straggler.usec)
+                self.backend.enqueue_straggler(self._straggler)
                 n += 1
             if interval:
                 oa = self._opt_args
@@ -1002,7 +1004,7 @@ class CudaMlpEngine(ComputeEngine):
         n += self._backward(B, early_sync=bucketed)
         if bucketed:
             if self._straggler is not None:
-                self.backend.enqueue_straggler_delay(self._straggler.prob, self._straggler.usec)
+                self.backend.enqueue_straggler(self._straggler)
                 n += 1
             oa = self._opt_args
             e0, e1 = self._bucket_early
@@ -1011,7 +1013,7 @@ class CudaMlpEngine(ComputeEngine):
             n += 1
         elif with_sync:
             if self._straggler is not None:
-                self.backend.enqueue_straggler_delay(self._straggler.prob, self._straggler.usec)
+                self.backend.enqueue_straggler(self._straggler)
                 n += 1
             if interval:
                 oa = self._opt_args

@@ -243,7 +243,10 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_integer("seed", 66478, "Base RNG seed (per-replica streams are derived from it)")
     F.DEFINE_string("compute_dtype", "bf16", "bf16 | fp32 (activations / tensor-core operand type)")
     F.DEFINE_string("backend", "auto", "auto | fused (sm_90a kernels + symmetric memory) | nccl | gloo")
-    F.DEFINE_string("inject_straggler", "", "rank:prob:usec[,rank:prob:usec...] device-side delay injection")
+    F.DEFINE_string("inject_straggler", "", "Comma-separated device-side delay injection: rank:prob:usec (fixed delay with "
+                    "probability prob), or a delay drawn every iteration from rank:exp:MEAN_US, "
+                    "rank:lognormal:MEDIAN_US:SIGMA or rank:profile:PATH (.npy / text file of delays in us); "
+                    "rank may be * for the drawn forms (every replica, each with its own stream)")
     F.DEFINE_integer("sync_timeout_ms", 30000, "Watchdog for device-side arrival polling")
     F.DEFINE_boolean("use_cuda_graph", True, "Capture the training step in a CUDA graph")
     F.DEFINE_boolean("use_nvls", True, "Use NVLS multimem reductions when the multicast object binds")

@@ -20,30 +20,104 @@ slow EC2 ``t2`` instances) are applied here, before the backend moves any bytes.
 """
 from __future__ import annotations
 
+import dataclasses
 import random
 import time
-from dataclasses import dataclass
+from dataclasses import dataclass, field
 from typing import Callable, Dict, List, Optional
 
+import numpy as np
 import torch
 
 from .backends import Backend, StepInfo
+from .straggler import delay_limit_ns, parametric_table, profile_table, sample_ns, seed_mix
 
 
 @dataclass
 class StragglerSpec:
+    """One replica's injected delay.  ``dist == "fixed"`` (``rank:prob:usec``): ``usec`` with probability ``prob``, decided
+    by a hash of the global step.  Otherwise (``exp``, ``lognormal``, ``profile``) a delay drawn every iteration from the
+    quantile ``table`` (ns, parallel/straggler.py) with the replica's stream key ``seed_mix``."""
     prob: float
     usec: float
+    dist: str = "fixed"
+    params: tuple = ()
+    table: Optional[np.ndarray] = field(default=None, compare=False, repr=False)
+    seed_mix: int = 0
+
+    @property
+    def sampled(self) -> bool:
+        return self.dist != "fixed"
 
 
-def parse_straggler_spec(text: str) -> Dict[int, StragglerSpec]:
-    """``"3:0.5:2000,5:1:500"`` -> {3: (p=.5, 2000us), 5: (p=1, 500us)}."""
-    out: Dict[int, StragglerSpec] = {}
+class StragglerMap(dict):
+    """rank -> StragglerSpec; the key ``"*"`` stands for every rank (each draws from its own stream)."""
+
+    def get(self, rank, default=None):
+        if rank in self:
+            return self[rank]
+        return super().get("*", default)
+
+
+_DISTS = {"exp": ("MEAN_US",), "lognormal": ("MEDIAN_US", "SIGMA"), "profile": ("PATH",)}
+
+
+def _positive(item: str, name: str, text: str) -> float:
+    try:
+        v = float(text)
+    except ValueError:
+        raise ValueError("--inject_straggler %r: %s is not a number: %r" % (item, name, text))
+    if not (np.isfinite(v) and v > 0):
+        raise ValueError("--inject_straggler %r: %s must be a positive number, got %r" % (item, name, text))
+    return v
+
+
+def parse_straggler_spec(text: str, sync_timeout_ms: Optional[float] = None) -> Dict[int, StragglerSpec]:
+    """Comma-separated list of
+    ``rank:prob:usec`` (``"3:0.5:2000"`` -> rank 3 sleeps 2000 us with probability .5),
+    ``rank:exp:MEAN_US``, ``rank:lognormal:MEDIAN_US:SIGMA`` or ``rank:profile:PATH`` (delays in us, ``.npy`` or text),
+    where ``rank`` of the last three may be ``*`` (every replica).  Sampled forms compile to a quantile table whose largest
+    point must stay within ``min(sync_timeout_ms / 4, 4 s)``."""
+    out = StragglerMap()
+    limit = delay_limit_ns(sync_timeout_ms)
     for item in filter(None, (s.strip() for s in (text or "").split(","))):
-        parts = item.split(":")
-        if len(parts) != 3:
-            raise ValueError("--inject_straggler wants rank:prob:usec, got %r" % item)
-        out[int(parts[0])] = StragglerSpec(float(parts[1]), float(parts[2]))
+        head = item.split(":", 2)
+        if len(head) == 3 and head[1] in _DISTS:
+            rank_txt, dist, rest = head
+            if rank_txt.strip() == "*":
+                rank = "*"
+            else:
+                try:
+                    rank = int(rank_txt)
+                except ValueError:
+                    raise ValueError("--inject_straggler %r: rank must be an integer or *, got %r" % (item, rank_txt))
+                if rank < 0:
+                    raise ValueError("--inject_straggler %r: rank must not be negative" % item)
+            if dist == "profile":
+                args = (rest,)
+                table = profile_table(rest, limit)
+            else:
+                vals = rest.split(":")
+                if len(vals) != len(_DISTS[dist]):
+                    raise ValueError("--inject_straggler %r: wants rank:%s:%s" % (item, dist, ":".join(_DISTS[dist])))
+                args = tuple(_positive(item, n, v) for n, v in zip(_DISTS[dist], vals))
+                table = parametric_table(dist, args, limit)
+            spec = StragglerSpec(1.0, 0.0, dist, args, table)
+        else:
+            parts = item.split(":")
+            if len(parts) != 3:
+                raise ValueError("--inject_straggler wants rank:prob:usec, rank:exp:MEAN_US, rank:lognormal:MEDIAN_US:SIGMA "
+                                 "or rank:profile:PATH, got %r" % item)
+            try:
+                float(parts[1])
+            except ValueError:
+                raise ValueError("--inject_straggler %r: unknown distribution %r (known: %s)"
+                                 % (item, parts[1], ", ".join(sorted(_DISTS))))
+            rank = int(parts[0])
+            spec = StragglerSpec(float(parts[1]), float(parts[2]))
+        if rank in out or (out and (rank == "*" or "*" in out)):
+            raise ValueError("--inject_straggler: rank %s is given twice (* stands for every rank)" % rank)
+        out[rank] = spec
     return out
 
 
@@ -55,8 +129,13 @@ class _AggregatorBase:
         self.total_num_replicas = int(total_num_replicas)
         self.local_step = 0          # global step of the weights my next gradient is computed from (X7)
         self.last_info: Optional[StepInfo] = None
-        self._straggler = (straggler or {}).get(backend.ctx.rank)
+        s = (straggler or {}).get(backend.ctx.rank)
+        if s is not None and s.sampled:
+            s = dataclasses.replace(s, seed_mix=seed_mix(seed, backend.ctx.rank))     # this replica's own stream
+        self._straggler = s
         self._rng = random.Random(seed * 7919 + backend.ctx.rank)
+        self._straggler_iter = 0
+        self.straggler_delays_ns: List[int] = []     # sampled forms: what _delay_s handed out, one per local iteration
         self.accepted_steps = 0
         self.dropped_steps = 0
 
@@ -66,6 +145,11 @@ class _AggregatorBase:
 
     def _delay_s(self) -> float:
         s = self._straggler
+        if s is not None and s.sampled:
+            ns = int(sample_ns(s.table, s.seed_mix, self._straggler_iter)[0])
+            self._straggler_iter += 1
+            self.straggler_delays_ns.append(ns)
+            return ns * 1e-9
         if s is not None and self._rng.random() < s.prob:
             return s.usec * 1e-6
         return 0.0

@@ -21,9 +21,11 @@ import ctypes
 import os
 from typing import Dict, List, Optional
 
+import numpy as np
 import torch
 
 from ..ops.lib import check, load, require_hopper, stream_ptr
+from . import straggler
 from .backends import Backend, StepInfo
 from .context import ReplicaContext
 from .symm_mem import SymmetricBuffer, allocate_symmetric
@@ -295,6 +297,44 @@ class FusedBackend(Backend):
         check(self.lib.dm_straggler_delay(ctypes.c_void_p(self.ctrl.local_ptr), ctypes.c_float(prob),
                                           ctypes.c_uint(int(usec)), ctypes.c_uint(seed), stream_ptr(stream)),
               "dm_straggler_delay")
+
+    def arm_straggler(self, spec) -> None:
+        """Sampled forms (``rank:exp|lognormal|profile:...``): upload the quantile table and allocate the sampler's state
+        block (iteration counter + ring of drawn / spun delays).  Arming the spec that is already armed keeps its counter."""
+        if not spec.sampled or getattr(self, "_strag_spec", None) is spec:
+            return
+        limit = straggler.delay_limit_ns(self.timeout_ms)
+        if int(spec.table.max()) > limit:
+            raise ValueError("--inject_straggler: the largest delay of %s, %.0f us, exceeds a quarter of this backend's "
+                             "watchdog (%.0f us)" % (spec.dist, int(spec.table.max()) / 1e3, limit / 1e3))
+        assert spec.table.shape == (straggler.TABLE_POINTS,) and spec.table.dtype == np.uint32
+        assert int(self.lib.dm_straggler_state_bytes()) == straggler.STATE_BYTES
+        self._strag_table = torch.from_numpy(spec.table.view(np.int32).copy()).to(self.ctx.device)
+        self._strag_state = torch.zeros(straggler.STATE_BYTES, dtype=torch.uint8, device=self.ctx.device)
+        self._strag_spec = spec
+
+    def enqueue_straggler(self, spec, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """The injected delay of one iteration, stream-ordered: the fixed form (``rank:prob:usec``) through
+        ``straggler_delay_kernel`` exactly as before, sampled forms through ``straggler_sample_kernel`` (armed first)."""
+        if not spec.sampled:
+            self.enqueue_straggler_delay(spec.prob, spec.usec, stream=stream)
+            return
+        if getattr(self, "_strag_spec", None) is not spec:
+            raise RuntimeError("enqueue_straggler: arm_straggler(spec) has not been called for this spec")
+        check(self.lib.dm_straggler_sample(ctypes.c_void_p(self._strag_state.data_ptr()),
+                                           ctypes.c_void_p(self._strag_table.data_ptr()), ctypes.c_uint(spec.seed_mix),
+                                           stream_ptr(stream)), "dm_straggler_sample")
+
+    def straggler_samples(self):
+        """``(j, drawn_ns, spun_ns)`` of the sampled iterations still in the device ring (the last 1024), oldest first;
+        synchronises the device."""
+        torch.cuda.synchronize()
+        raw = self._strag_state.cpu().numpy()
+        n = int(raw[:4].view("<u4")[0])
+        drawn = raw[16:16 + 4 * straggler.RING].view("<u4")
+        spun = raw[16 + 4 * straggler.RING:].view("<u8")
+        j = np.arange(max(0, n - straggler.RING), n, dtype=np.int64)
+        return j, drawn[j % straggler.RING].copy(), spun[j % straggler.RING].copy()
 
     def device_barrier(self, stream: Optional[torch.cuda.Stream] = None) -> None:
         """Stream-ordered barrier over NVLink flags (csrc/fused_sync.cu): every replica's stream passes it within a flag hop of

@@ -195,7 +195,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     engine = make_engine(flags, ctx, backend)
     spec = engine.spec
     lr_schedule = LearningRateSchedule.from_flags(flags, dataset.num_examples, num_replicas_to_aggregate)
-    straggler = parse_straggler_spec(flags.inject_straggler)
+    straggler = parse_straggler_spec(flags.inject_straggler, flags.sync_timeout_ms)
 
     if flags.interval_method or flags.worker_times_cdf_method:
         # reference :179-183 -- interval wins when both are set, as there.
