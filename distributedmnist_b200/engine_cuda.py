@@ -57,6 +57,8 @@ class _RunnerEvent:
 
 
 class CudaLeNetEngine(ComputeEngine):
+    _kgtn_k = 0                  # K > N: gradients per update (count trigger); 0 = the K <= N / interval paths
+
     def __init__(self, batch_size: int, backend: FusedBackend, seed: int = 66478, rank: int = 0,
                  keep_prob: float = 0.5, use_graph: bool = True):
         self.lib = load()
@@ -234,6 +236,12 @@ class CudaLeNetEngine(ComputeEngine):
         """Bind the aggregation policy so the whole step (compute + fused sync) is one graph."""
         sched = opt.lr_schedule
         k = getattr(opt, "replicas_to_aggregate", opt.total_num_replicas)
+        n = self.backend.ctx.world_size
+        # K > N (mode A): replicas free-run and accumulate; a step commits once K of its gradients are in (count trigger)
+        self._kgtn_k = int(k) if int(k) > n else 0
+        if self._kgtn_k and getattr(opt, "drop_connect_probability", None) is not None:
+            raise ValueError("--drop_connect is not implemented on the GPU path with --num_replicas_to_aggregate (%d) > "
+                             "the number of replicas (%d)" % (int(k), n))
         self._opt_args = dict(k=int(k), lr0=float(sched.initial_learning_rate), decay_rate=float(sched.decay_rate),
                               decay_steps=int(sched.decay_steps))
         if getattr(opt, "drop_connect_probability", None) is not None:
@@ -246,16 +254,18 @@ class CudaLeNetEngine(ComputeEngine):
         self._runner = None                  # graphs are re-captured: the native runner is rebuilt on demand
         # mode C on the device (csrc/fused_interval.cu): every iteration adds its gradient to a symmetric accumulator; ticks
         # are committed by whichever replica first passes the %globaltimer deadline
-        self._interval = getattr(opt, "mode", "") == "interval"
+        # K > N runs the same iteration with the count trigger (same accumulator, same snapshot ordering as interval mode)
+        self._interval = getattr(opt, "mode", "") == "interval" or bool(self._kgtn_k)
         if self._interval and getattr(self, "_acc", None) is None:
             self._acc = self.backend.allocate(self.spec.arena_numel)
+        if self._kgtn_k:
+            self.backend.kgtn_arm()          # nothing else arms it (e.g. bench.py); train.py re-arms after a restore
         # Bucketed aggregation (csrc/fused_sync.cu): full participation on 2/4/8 replicas.  fc1's weight gradient (96.5 % of
         # the bytes) is exchanged by small co-resident CTAs NEXT TO conv2 dgrad/wgrad + conv1 wgrad; the rest goes one-shot.
         #   DMNIST_BUCKET=2 (default): csrc/fused_bucket.cu -- fc1's gradient leaves the GEMM epilogue as bf16, is reduced in
         #     place over NVLink (in-switch fp32 accumulation) and applied to the local fp32 master weights under the backward
         #     pass; the small bucket is pushed into every replica's inbox.  Also used on ONE replica (no exchange, the fc1
         #     update still leaves the critical path).   =1: round-1 fp32 two-shot / one-shot kernels.   =0: single kernel.
-        n = self.backend.ctx.world_size
         mode = os.environ.get("DMNIST_BUCKET", "2")
         can = (hasattr(self, "_bucket_split") and int(k) == n and self._branches and self.backend.drop_keep <= 0.0
                and getattr(opt, "mode", "") != "interval")
@@ -428,13 +438,17 @@ class CudaLeNetEngine(ComputeEngine):
         """Average device time of every kernel of the step, measured in place with CUDA events between
         eager launches (caches warm, as in the replayed graph; includes the launch gap)."""
         names = ["memsets", "conv1_fwd", "conv2_fwd", "fc1_fwd", "fc2_fwd_bwd", "fc1_wgrad", "fc2_wgrad", "fc1_dgrad", "unpool2",
-                 "conv2_wgrad", "conv2_dgrad", "conv1_wgrad", "fused_sync_sgd"]
+                 "conv2_wgrad", "conv2_dgrad", "conv1_wgrad"]
+        # K > N: adopt + shadow refresh, and gate + accumulate + close + apply, in place of the fused sync kernel
+        names = (["kgtn_begin"] + names + ["kgtn_end"]) if self._kgtn_k else names + ["fused_sync_sgd"]
         tot = {n: 0.0 for n in names}
         B, s = self.batch_size, self._slot
         img, lbl = self.images[s], self.labels[s]
         lib, sp, g, p, pb = self.lib, stream_ptr(), self.g, self.p, self.pb
 
         def seq():
+            if self._kgtn_k:
+                yield "kgtn_begin", lambda: self.backend.enqueue_kgtn_begin(self.params)
             yield "memsets", lambda: self._launch_zero()
             fw = []
             # forward / backward are issued kernel by kernel so an event can sit between any two
@@ -473,7 +487,12 @@ class CudaLeNetEngine(ComputeEngine):
             yield "conv1_wgrad", lambda: check((lib.dm_conv1_wgrad_tc if self._conv1_tc else lib.dm_conv1_wgrad)(ptr(img), ptr(self.dx1), ptr(self.code1),
                                                                   ptr(g["conv1_weights"]), ptr(g["conv1_biases"]), B, sp),
                                                "conv1_wgrad")
-            yield "fused_sync_sgd", lambda: self.backend.enqueue(self.params, self.grads, **self._opt_args)
+            if self._kgtn_k:
+                oa = self._opt_args
+                yield "kgtn_end", lambda: self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"],
+                                                                        oa["decay_rate"], oa["decay_steps"])
+            else:
+                yield "fused_sync_sgd", lambda: self.backend.enqueue(self.params, self.grads, **self._opt_args)
 
         for it in range(iters + 3):
             evs = [torch.cuda.Event(enable_timing=True)]
@@ -507,7 +526,7 @@ class CudaLeNetEngine(ComputeEngine):
                 self._delay_in_chain = True
                 n += 1
         if interval:
-            self.backend.enqueue_interval_begin(self.params)
+            self._enqueue_iteration_begin()
             n += 2
         n += self._launch_zero()
         n += self._launch_forward(self.images[slot], self.labels[slot], self.batch_size, True)
@@ -527,8 +546,7 @@ class CudaLeNetEngine(ComputeEngine):
                 self.backend.enqueue_straggler(self._straggler)
                 n += 1
             if interval:
-                oa = self._opt_args
-                self.backend.enqueue_interval_end(self.params, self.grads, self._acc, oa["lr0"], oa["decay_rate"], oa["decay_steps"])
+                self._enqueue_iteration_end()
                 n += 4
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
@@ -536,6 +554,22 @@ class CudaLeNetEngine(ComputeEngine):
         if self._branches:
             torch.cuda.current_stream().wait_event(self._join_loss)      # the loss read-back branch rejoins at the end of the step
         self.launches_per_step = n
+
+    def _enqueue_iteration_begin(self) -> None:
+        """Interval mode / K > N: adopt pushed weights (+ shadow refresh) at the start of an iteration."""
+        if self._kgtn_k:
+            self.backend.enqueue_kgtn_begin(self.params)
+        else:
+            self.backend.enqueue_interval_begin(self.params)
+
+    def _enqueue_iteration_end(self) -> None:
+        """Interval mode / K > N: gate, accumulate, close (+ commit attempt), apply."""
+        oa = self._opt_args
+        if self._kgtn_k:
+            self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"], oa["decay_rate"],
+                                          oa["decay_steps"])
+        else:
+            self.backend.enqueue_interval_end(self.params, self.grads, self._acc, oa["lr0"], oa["decay_rate"], oa["decay_steps"])
 
     def _run(self, with_sync: bool) -> None:
         s = self._slot
@@ -895,6 +929,8 @@ class CudaMlpEngine(ComputeEngine):
     pack_batch = CudaLeNetEngine.pack_batch
     load_packed = CudaLeNetEngine.load_packed
     attach_optimizer = CudaLeNetEngine.attach_optimizer
+    _enqueue_iteration_begin = CudaLeNetEngine._enqueue_iteration_begin
+    _enqueue_iteration_end = CudaLeNetEngine._enqueue_iteration_end
     params_updated = CudaLeNetEngine.params_updated
     _run = CudaLeNetEngine._run
     forward_backward = CudaLeNetEngine.forward_backward
@@ -904,6 +940,7 @@ class CudaMlpEngine(ComputeEngine):
     loss_acc = CudaLeNetEngine.loss_acc
     step_info = CudaLeNetEngine.step_info
     _stamp = False
+    _kgtn_k = 0
 
     def h2d_bytes_per_step(self) -> int:
         return self.batch_size * (784 * 4 + 8)
@@ -996,7 +1033,7 @@ class CudaMlpEngine(ComputeEngine):
         n = 0
         interval = with_sync and getattr(self, "_interval", False)
         if interval:
-            self.backend.enqueue_interval_begin(self.params)
+            self._enqueue_iteration_begin()
             n += 2
         bucketed = with_sync and self._bucket_v2 and not interval
         n += self._launch_zero()
@@ -1016,8 +1053,7 @@ class CudaMlpEngine(ComputeEngine):
                 self.backend.enqueue_straggler(self._straggler)
                 n += 1
             if interval:
-                oa = self._opt_args
-                self.backend.enqueue_interval_end(self.params, self.grads, self._acc, oa["lr0"], oa["decay_rate"], oa["decay_steps"])
+                self._enqueue_iteration_end()
                 n += 4
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)

@@ -174,13 +174,15 @@ class _AggregatorBase:
 
 
 class SyncReplicasOptimizer(_AggregatorBase):
-    """Mode A: synchronous SGD that commits on the first K of N gradients."""
+    """Mode A: synchronous SGD that commits on the first K of N gradients.  K > N: replicas compute several batches per
+    update -- each step commits once at least K gradients computed on its weights are accumulated across the replicas, and
+    the update is their mean over the number accumulated."""
 
     def __init__(self, backend: Backend, lr_schedule, replicas_to_aggregate: int, total_num_replicas: int,
                  drop_connect_probability: Optional[float] = None, straggler=None, seed: int = 0):
         super().__init__(backend, lr_schedule, total_num_replicas, straggler, seed)
-        if not 1 <= replicas_to_aggregate <= total_num_replicas:
-            raise ValueError("replicas_to_aggregate=%d must be in [1, %d]" % (replicas_to_aggregate, total_num_replicas))
+        if replicas_to_aggregate < 1:
+            raise ValueError("replicas_to_aggregate=%d must be >= 1" % replicas_to_aggregate)
         self.replicas_to_aggregate = int(replicas_to_aggregate)
         self.drop_connect_probability = drop_connect_probability
         self._dc_gen: Optional[torch.Generator] = None
@@ -201,6 +203,13 @@ class SyncReplicasOptimizer(_AggregatorBase):
     def apply_gradients(self, params: torch.Tensor, grads: torch.Tensor) -> StepInfo:
         grads = self._drop_connect(grads)
         lr = self.lr_schedule(self.local_step)
+        if self.replicas_to_aggregate > self.total_num_replicas:
+            info = self.backend.accumulate_step(params, grads, lr, self.local_step, self.replicas_to_aggregate,
+                                                delay_s=self._delay_s())
+            self.last_info = info
+            self.local_step = info.global_step
+            self.accepted_steps += info.contributed      # gradients that entered a committed update
+            return info
         info = self.backend.sync_step(params, grads, lr, self.local_step, self.replicas_to_aggregate,
                                       delay_s=self._delay_s())
         return self._account(info)

@@ -39,7 +39,8 @@ class StepInfo:
     mask: int               # contributor bitmap
     count: int              # divisor
     stale: bool = False
-    applied: bool = True    # False when (interval mode) no update happened in this call
+    applied: bool = True    # False when (interval mode, K > N) no update happened in this call
+    contributed: int = 0    # K > N: my gradients in the update this call committed
 
 
 class Backend:
@@ -78,6 +79,23 @@ class Backend:
                       tick: int) -> StepInfo:
         raise NotImplementedError
 
+    def accumulate_step(self, params: torch.Tensor, grads: torch.Tensor, lr: float, local_step: int, k: int,
+                        delay_s: float = 0.0) -> StepInfo:
+        """K > N (mode A): add one batch gradient, computed on the weights of ``local_step``, to this replica's
+        accumulator.  The step commits once at least ``k`` gradients are accumulated across the replicas; the update is
+        their mean over the number actually accumulated."""
+        raise NotImplementedError("%s backend: --num_replicas_to_aggregate > number of replicas" % self.name)
+
+    def _kgtn_add(self, grads: torch.Tensor) -> int:
+        """Local accumulator of the K > N path: the first gradient of a step overwrites, later ones are added."""
+        if getattr(self, "_kgtn_count", 0) == 0:
+            self._kgtn_acc = grads.detach().clone()
+            self._kgtn_count = 0
+        else:
+            self._kgtn_acc.add_(grads)
+        self._kgtn_count += 1
+        return self._kgtn_count
+
 
 class LocalBackend(Backend):
     name = "local"
@@ -99,6 +117,18 @@ class LocalBackend(Backend):
         params.add_(acc, alpha=-float(lr) / count)
         self._global_step += 1
         return StepInfo(self._global_step, True, 1, count)
+
+    def accumulate_step(self, params, grads, lr, local_step, k, delay_s=0.0) -> StepInfo:
+        """One replica: every update is the mean of ``k`` consecutive batch gradients."""
+        if delay_s > 0:
+            time.sleep(delay_s)
+        count = self._kgtn_add(grads)
+        if count < k:
+            return StepInfo(local_step, True, 1, count, applied=False)
+        params.add_(self._kgtn_acc, alpha=-float(lr) / count)
+        self._kgtn_count = 0
+        self._global_step = local_step + 1
+        return StepInfo(self._global_step, True, 1, count, contributed=count)
 
 
 class _CollectiveBackend(Backend):
@@ -153,6 +183,32 @@ class _CollectiveBackend(Backend):
         params.add_(acc, alpha=-float(lr) / total)
         self._global_step += 1
         return StepInfo(self._global_step, count > 0, mask, total)
+
+    def accumulate_step(self, params, grads, lr, local_step, k, delay_s=0.0) -> StepInfo:
+        """K > N over the c10d store: every accumulated gradient takes a ticket from the step's counter (``store.add``).
+        A replica keeps computing batches until its ticket reaches ``k``; then it joins the collective sum of the step, so
+        each replica contributes every gradient it accumulated, and the divisor is the total (>= k).  There is nothing to
+        drop: a step cannot commit before every replica has joined it."""
+        if delay_s > 0:
+            time.sleep(delay_s)
+        mine = self._kgtn_add(grads)
+        assert self.ctx.store is not None, "K > N needs the rendezvous store"
+        ticket = int(self.ctx.store.add("%s/kgtn/%d" % (self._board_prefix, local_step), 1))
+        if ticket < k:
+            return StepInfo(local_step, True, 0, ticket, applied=False)
+        cnt = torch.tensor([float(mine)], dtype=torch.float32, device=self._kgtn_acc.device)
+        dist.all_reduce(cnt, op=dist.ReduceOp.SUM)
+        total = int(cnt.item())
+        dist.all_reduce(self._kgtn_acc, op=dist.ReduceOp.SUM)
+        params.add_(self._kgtn_acc, alpha=-float(lr) / total)
+        self._kgtn_count = 0
+        self._global_step = local_step + 1
+        if self.ctx.rank == 0 and local_step >= 2:
+            try:
+                self.ctx.store.delete_key("%s/kgtn/%d" % (self._board_prefix, local_step - 2))   # bounded store growth
+            except Exception:  # noqa: BLE001  (best effort, as StoreCommitBoard.gc)
+                pass
+        return StepInfo(self._global_step, True, (1 << self.ctx.world_size) - 1, total, contributed=mine)
 
 
 class GlooBackend(_CollectiveBackend):

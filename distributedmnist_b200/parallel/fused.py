@@ -288,6 +288,30 @@ class FusedBackend(Backend):
                                        ctypes.c_double(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
                                        int(self.ctas), stream_ptr(stream), ctypes.c_void_p(mc)), "dm_interval_end")
 
+    # ---- K > N gradients per update (count trigger, csrc/fused_interval.cu with COUNT) ---------------------------------------
+    def kgtn_arm(self) -> None:
+        """Start a fresh accumulation on this replica at its current global step (collective: every rank calls it)."""
+        self.interval_arm(0.0)
+
+    def enqueue_kgtn_begin(self, params: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Start of a K > N iteration: adopt weights a committer has pushed; gradients accumulated for the step after its
+        contributors were frozen are counted as dropped."""
+        check(self.lib.dm_kgtn_begin(ctypes.c_void_p(self.ctrl.local_ptr), self.ctx.rank, ctypes.c_void_p(params.data_ptr()),
+                                     ctypes.c_void_p(0 if self.shadow is None else self.shadow.data_ptr()),
+                                     ctypes.c_longlong(params.numel()), stream_ptr(stream)), "dm_kgtn_begin")
+
+    def enqueue_kgtn_end(self, params: torch.Tensor, grads: torch.Tensor, acc: torch.Tensor, k: int, lr0: float,
+                         decay_rate: float = 1.0, decay_steps: int = 1, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """End of a K > N iteration: accumulate the gradient locally; once ``k`` gradients computed on the current step's
+        weights are accumulated across the replicas, the first replica to see it commits their mean."""
+        pb, gb, ab = self._by_ptr[params.data_ptr()], self._by_ptr[grads.data_ptr()], self._by_ptr[acc.data_ptr()]
+        nv = self.use_nvls and bool(pb.multicast_ptr) and bool(ab.multicast_ptr)
+        check(self.lib.dm_kgtn_end(self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), ab.ptr_table(), self.ctx.rank,
+                                   self.ctx.world_size, int(k), ctypes.c_longlong(params.numel()), ctypes.c_double(lr0),
+                                   ctypes.c_double(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
+                                   int(self.ctas), stream_ptr(stream), ctypes.c_void_p(pb.multicast_ptr if nv else 0),
+                                   ctypes.c_void_p(ab.multicast_ptr if nv else 0)), "dm_kgtn_end")
+
     @property
     def nvls_active(self) -> bool:
         return self.use_nvls and bool(self._buffers) and all(b.multicast_ptr for b in self._buffers[:2])

@@ -29,6 +29,7 @@ from __future__ import annotations
 import threading
 import time
 from dataclasses import dataclass
+from fractions import Fraction
 from typing import Dict, List, Optional
 
 
@@ -895,3 +896,173 @@ class SnapshotModel:
             r = choose(runnable)
             waiting.pop(r, None)
             BucketV2Model._advance(r, gens, waiting)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# K > N gradients per update -- word-level model of the count-triggered interval kernels (csrc/fused_interval.cu, COUNT)
+# ----------------------------------------------------------------------------------------------------------------------
+class CountTriggerModel:
+    """:class:`IntervalBoard` with the count trigger, as generators for :func:`explore_schedules`.  Each replica runs
+    ``iters`` iterations (one number, or one per replica).  The code between two ``yield`` s is one atomic step; the steps are
+
+    * adopt (``iv_adopt``: move past every committed step whose pushes have landed, counting gradients accumulated after a
+      step's mask was frozen as ``lost``), forward/backward on the adopted weights, the gate (``busy := e+1``; fence.sc;
+      commit word present? -> dropped) and the start of ``iv_accumulate`` (``in_flight``);
+    * the end of the accumulate and ``iv_close``: publish ``(step, count + 1)``, ``busy := 0``, fence.sc, read every
+      replica's ``(step, count)`` word.  ``fence=False`` lets those reads overtake the two stores (a store buffer): the
+      stores become visible one step later;
+    * sum >= K: read + CAS of the chief's commit word and its broadcast;
+    * committer: wait until no contributor is mid-accumulate (``busy_wait=False`` skips the wait), read the final counts and
+      the accumulators, SGD, push to every replica, ``done`` flags, credit every contributor's ``accepted``.
+
+    Invariants (``ProtocolHazard`` otherwise): every commit's total is >= K; every accumulated gradient it sums was computed
+    on the committed step's weights; the committer never reads an accumulator mid-add nor one whose count is behind; steps
+    commit in order, once each; at the end every replica holds the serial replay of the commits, no step has K gradients
+    without a commit, the accepted counts add up to the commit totals, and every accumulated gradient is accepted, lost or
+    still pending.  Values are ``Fraction`` s, so the replay is exact."""
+
+    def __init__(self, n: int, k: int, iters, fence: bool = True, busy_wait: bool = True, lr=Fraction(1, 2)):
+        self.n, self.k, self.fence, self.busy_wait, self.lr = n, k, fence, busy_wait, Fraction(lr)
+        self.iters = list(iters) if isinstance(iters, (list, tuple)) else [int(iters)] * n
+        self.epoch = [0] * n
+        self.state = [(1, 0)] * n                          # iv_state: (step + 1, gradients accumulated for it)
+        self.busy = [0] * n
+        self.commit_local: List[Dict[int, tuple]] = [dict() for _ in range(n)]   # step -> (mask, committer)
+        self.commit: Dict[int, tuple] = {}                 # the chief's commit ring
+        self.done = [[0] * n for _ in range(n)]            # done[q][p]: p's pushes of step s landed on q (value s + 1)
+        self.acc: List[list] = [[] for _ in range(n)]      # (step of the weights, value) of every gradient accumulated
+        self.in_flight = [False] * n
+        self.weights = [(0, Fraction(0))] * n              # (version = committed steps applied, value)
+        self.commits: List[tuple] = []                     # (step, committer, mask, counts, total, gradient sum)
+        self.accumulated, self.accepted, self.dropped, self.lost = [0] * n, [0] * n, [0] * n, [0] * n
+
+    @staticmethod
+    def grad(r: int, it: int) -> Fraction:
+        return Fraction(10 * (r + 1) + it)
+
+    def replica(self, r: int):
+        n = self.n
+        for it in range(self.iters[r]):
+            # ---- adopt, forward/backward, gate, accumulate begins ----------------------------------------------------------
+            e = self.epoch[r]
+            while e in self.commit_local[r]:
+                mask, who = self.commit_local[r][e]
+                if self.done[r][who] < e + 1:
+                    break
+                tag, c = self.state[r]
+                if e == self.epoch[r] and tag == e + 1 and c > 0 and not (mask >> r) & 1:
+                    self.lost[r] += c
+                    self.dropped[r] += c
+                e += 1
+            if e != self.epoch[r]:
+                self.epoch[r], self.state[r] = e, (e + 1, 0)
+            ver, _w = self.weights[r]
+            if ver != e:
+                raise ProtocolHazard("replica %d computes on weights of version %d at step %d" % (r, ver, e))
+            if e in self.commit_local[r]:
+                self.dropped[r] += 1                       # stale: computed on weights a commit is replacing
+                yield None
+                continue
+            self.busy[r] = e + 1
+            self.in_flight[r] = True
+            yield None
+            # ---- accumulate ends, close ----------------------------------------------------------------------------------
+            tag, c = self.state[r]
+            if tag != e + 1:
+                raise ProtocolHazard("replica %d closes step %d holding the count of step %d" % (r, e, tag - 1))
+            self.acc[r] = [(e, self.grad(r, it))] if c == 0 else self.acc[r] + [(e, self.grad(r, it))]
+            self.in_flight[r] = False
+            self.accumulated[r] += 1
+            mine = (e + 1, c + 1)
+            if self.fence:
+                self.state[r], self.busy[r] = mine, 0
+                seen = [mine if q == r else self.state[q] for q in range(n)]
+                yield None
+            else:
+                seen = [mine if q == r else self.state[q] for q in range(n)]
+                yield None
+                self.state[r], self.busy[r] = mine, 0
+                yield None
+            if sum(cq for tq, cq in seen if tq == e + 1) < self.k:
+                continue
+            # ---- the trigger fired: CAS the chief's commit word, broadcast it ---------------------------------------------
+            if e in self.commit:
+                continue
+            mask = sum(1 << q for q, (tq, cq) in enumerate(seen) if tq == e + 1 and cq > 0)
+            self.commit[e] = (mask, r)
+            for q in range(n):
+                self.commit_local[q][e] = (mask, r)
+            yield None
+            # ---- committer: busy-wait, final counts, peer loads of the accumulators, SGD, push, done ------------------------
+            if self.busy_wait:
+                for q in range(n):
+                    if (mask >> q) & 1 and q != r:
+                        yield (lambda q=q: self.busy[q] != e + 1)
+            counts, terms = [0] * n, []
+            for q in range(n):
+                if not (mask >> q) & 1:
+                    continue
+                tq, cq = self.state[q]
+                if tq != e + 1:
+                    raise ProtocolHazard("contributor %d of step %d moved on before its accumulator was read" % (q, e))
+                if self.in_flight[q]:
+                    raise ProtocolHazard("committer %d read replica %d's accumulator while it was adding to it" % (r, q))
+                if len(self.acc[q]) != cq:
+                    raise ProtocolHazard("replica %d's accumulator holds %d gradients, its count says %d" % (q, len(self.acc[q]), cq))
+                for s, v in self.acc[q]:
+                    if s != e:
+                        raise ProtocolHazard("commit of step %d sums a gradient computed on the weights of step %d" % (e, s))
+                    terms.append(v)
+                counts[q] = cq
+            total = sum(counts)
+            if total < self.k:
+                raise ProtocolHazard("step %d committed with %d < K = %d gradients" % (e, total, self.k))
+            ver, w = self.weights[r]
+            if ver != e:
+                raise ProtocolHazard("committer %d of step %d holds weights of version %d" % (r, e, ver))
+            new = (e + 1, w - self.lr * sum(terms) / total)
+            for q in range(n):
+                self.weights[q] = new
+                self.done[q][r] = e + 1
+                self.accepted[q] += counts[q]
+            self.commits.append((e, r, mask, tuple(counts), total, sum(terms)))
+            yield None
+
+    def run(self, choose) -> None:
+        gens = {r: self.replica(r) for r in range(self.n)}
+        waiting = {}
+        for r in list(gens):
+            BucketV2Model._advance(r, gens, waiting)
+        while gens:
+            runnable = [r for r in sorted(gens) if r not in waiting or waiting[r]()]
+            if not runnable:
+                raise ProtocolHazard("deadlock: replicas %s wait forever (epochs %s)" % (sorted(gens), self.epoch))
+            r = choose(runnable)
+            waiting.pop(r, None)
+            BucketV2Model._advance(r, gens, waiting)
+        self.check_end()
+
+    def check_end(self) -> None:
+        steps = [c[0] for c in self.commits]
+        if steps != list(range(len(steps))):
+            raise ProtocolHazard("commits out of order or repeated: %s" % steps)
+        w = Fraction(0)
+        for (_e, _r, _m, _c, total, gsum) in self.commits:
+            w -= self.lr * gsum / total
+        for q in range(self.n):
+            if self.weights[q] != (len(steps), w):
+                raise ProtocolHazard("replica %d ends with %s, the serial replay gives %s" % (q, self.weights[q], (len(steps), w)))
+        top = len(steps)
+        pending = sum(c for t, c in self.state if t == top + 1)
+        if pending >= self.k:
+            raise ProtocolHazard("every replica has closed and step %d holds %d >= K = %d gradients without a commit"
+                                 % (top, pending, self.k))
+        if sum(self.accepted) != sum(c[4] for c in self.commits):
+            raise ProtocolHazard("accepted %s do not add up to the commit totals" % self.accepted)
+        for q in range(self.n):
+            t, c = self.state[q]
+            mask = self.commit.get(t - 1, (None,))[0]
+            residual = c if mask is None or not (mask >> q) & 1 else 0   # pending, or lost but not adopted yet
+            if self.accumulated[q] != self.accepted[q] + self.lost[q] + residual:
+                raise ProtocolHazard("replica %d accumulated %d gradients: %d accepted, %d lost, %d pending"
+                                     % (q, self.accumulated[q], self.accepted[q], self.lost[q], residual))

@@ -167,9 +167,9 @@ def check_eval_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate: int,
     # --worker_times_cdf_method (without --interval_method, which wins when both are set) always aggregates all N
     # gradients behind a full barrier and ignores --num_replicas_to_aggregate
     cdf = getattr(flags, "worker_times_cdf_method", False)
-    if not cdf and num_replicas_to_aggregate < ctx.world_size:
-        raise ValueError("--eval_every_steps needs --num_replicas_to_aggregate = number of replicas (%d): with K < N the "
-                         "team pushes weights into the chief's arena while it is between steps or late"
+    if not cdf and num_replicas_to_aggregate != ctx.world_size:
+        raise ValueError("--eval_every_steps needs --num_replicas_to_aggregate = number of replicas (%d): with K < N or "
+                         "K > N peers push weights into the chief's arena while it is between steps or late"
                          % ctx.world_size + hint)
 
 
@@ -271,6 +271,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             backend.interval_arm(float(flags.interval_ms))   # reference :287-288 (chief timer) -> %globaltimer deadline on the device
         else:
             opt.start_interval_updates()   # CPU plumbing path: shared absolute host-clock deadlines
+    elif getattr(engine, "_kgtn_k", 0):
+        backend.kgtn_arm()                 # K > N on the device: a restore moved the step counter, accumulate from there
 
     time_acc_list = []
     step = restored_step
@@ -502,6 +504,12 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         summary.close()
     if eval_every:
         results["evals"] = eval_rows
+    if getattr(engine, "_kgtn_k", 0):
+        # K > N on the device: the control block counts exactly the gradients that entered a committed update (credited
+        # by the committers) and the dropped ones; the per-iteration status words the loop consumed cannot tell them apart
+        torch.cuda.synchronize()
+        st = backend.read_status()
+        opt.accepted_steps, opt.dropped_steps = st["accepted_steps"], st["dropped_steps"]
     results.update(final_step=step, accepted=opt.accepted_steps, dropped=opt.dropped_steps,
                    params=engine.params, elapsed=time.time() - begin_time,
                    timeout_server=timeout_server, engine=engine, optimizer=opt)
