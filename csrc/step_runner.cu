@@ -16,6 +16,11 @@ struct StepRunner {
   size_t in_bytes;
   cudaEvent_t copy_done[2], slot_free[2];
   unsigned long long launched;
+  // device-resident training set (dm_runner_arm_gather): per-slot device index buffers and the table
+  void* idx_dev[2];
+  const float* table_images;
+  const int64_t* table_labels;
+  int batch;
 };
 
 }  // namespace dm
@@ -55,6 +60,42 @@ int dm_runner_step(void* h, const void* src) {
   cudaError_t e;
   if ((e = cudaStreamWaitEvent(r->copy, r->slot_free[s], 0)) != cudaSuccess) return -(int)e;     // the step that last read the slot is done
   if ((e = cudaMemcpyAsync(r->slot_dev[s], src, r->in_bytes, cudaMemcpyDefault, r->copy)) != cudaSuccess) return -(int)e;
+  if ((e = cudaEventRecord(r->copy_done[s], r->copy)) != cudaSuccess) return -(int)e;
+  if ((e = cudaStreamWaitEvent(r->compute, r->copy_done[s], 0)) != cudaSuccess) return -(int)e;
+  if ((e = cudaGraphLaunch(r->graph[s], r->compute)) != cudaSuccess) return -(int)e;
+  if ((e = cudaEventRecord(r->slot_free[s], r->compute)) != cudaSuccess) return -(int)e;
+  r->launched += 1;
+  return s;
+}
+
+// Device-resident training set for dm_runner_step_indices: idx0 / idx1 are the slots' device index buffers (batch int32
+// each), images / labels the table (fp32 [N, 784], int64 [N]).
+int dm_runner_arm_gather(void* h, void* idx0, void* idx1, const void* images, const void* labels, int batch) {
+  dm::StepRunner* r = reinterpret_cast<dm::StepRunner*>(h);
+  r->idx_dev[0] = idx0;
+  r->idx_dev[1] = idx1;
+  r->table_images = reinterpret_cast<const float*>(images);
+  r->table_labels = reinterpret_cast<const int64_t*>(labels);
+  r->batch = batch;
+  return 0;
+}
+
+// One training step from `batch` row indices of the armed table (page-locked host memory, each in [0, N)): the same event
+// chain as dm_runner_step, with the batch DMA replaced by an index DMA plus the gather kernel on the copy stream.
+// Returns the slot used (0 / 1) or a negative CUDA error code.
+int dm_runner_step_indices(void* h, const void* idx_host) {
+  using namespace dm;
+  StepRunner* r = reinterpret_cast<StepRunner*>(h);
+  if (r->table_images == nullptr) return -(int)cudaErrorInvalidValue;
+  const int s = (int)(r->launched & 1ull);
+  cudaError_t e;
+  if ((e = cudaStreamWaitEvent(r->copy, r->slot_free[s], 0)) != cudaSuccess) return -(int)e;
+  if ((e = cudaMemcpyAsync(r->idx_dev[s], idx_host, (size_t)r->batch * sizeof(int32_t), cudaMemcpyHostToDevice, r->copy)) !=
+      cudaSuccess)
+    return -(int)e;
+  if ((e = launch_gather_batch(reinterpret_cast<const int32_t*>(r->idx_dev[s]), r->table_images, r->table_labels, r->batch,
+                               r->slot_dev[s], r->copy)) != cudaSuccess)
+    return -(int)e;
   if ((e = cudaEventRecord(r->copy_done[s], r->copy)) != cudaSuccess) return -(int)e;
   if ((e = cudaStreamWaitEvent(r->compute, r->copy_done[s], 0)) != cudaSuccess) return -(int)e;
   if ((e = cudaGraphLaunch(r->graph[s], r->compute)) != cudaSuccess) return -(int)e;

@@ -58,6 +58,7 @@ class _RunnerEvent:
 
 class CudaLeNetEngine(ComputeEngine):
     _kgtn_k = 0                  # K > N: gradients per update (count trigger); 0 = the K <= N / interval paths
+    _table = None                # device-resident training set (images, labels), see arm_train_data
 
     def __init__(self, batch_size: int, backend: FusedBackend, seed: int = 66478, rank: int = 0,
                  keep_prob: float = 0.5, use_graph: bool = True):
@@ -193,6 +194,85 @@ class CudaLeNetEngine(ComputeEngine):
     def h2d_bytes_per_step(self) -> int:
         return self._h2d_bytes
 
+    # ---- device-resident training set (csrc/batch_gather.cu) ------------------------------------------------------------
+    def arm_train_data(self, images, labels) -> None:
+        """Upload the training set once (fp32 images ``[N,784]``, int64 labels ``[N]``, in the order given) and allocate two
+        device index slots of B int32.  From then on :meth:`step_indices` / :meth:`load_indices` fill an input slot from B
+        row indices: the gather kernel writes the rows in :meth:`pack_batch`'s layout, so the step reads the same bytes."""
+        self._leave_native_runner()
+        x = torch.as_tensor(np.ascontiguousarray(images) if isinstance(images, np.ndarray) else images, dtype=torch.float32)
+        y = torch.as_tensor(np.ascontiguousarray(labels) if isinstance(labels, np.ndarray) else labels).to(torch.int64)
+        n = int(x.shape[0])
+        if n < 1 or x.numel() != n * 784 or y.numel() != n:
+            raise ValueError("arm_train_data: %s images, %d labels (need [N, 784] values and N labels)" % (tuple(x.shape), y.numel()))
+        dev = self.device
+        self._table = (x.reshape(n, 784).to(dev).contiguous(), y.reshape(n).to(dev).contiguous())
+        self._idx_dev = [torch.zeros(self.batch_size, dtype=torch.int32, device=dev) for _ in range(2)]
+        self._h_idx = [torch.zeros(self.batch_size, dtype=torch.int32).pin_memory() for _ in range(2)]
+
+    def _as_indices(self, idx) -> torch.Tensor:
+        """``idx`` as a contiguous int32 host tensor of B rows, each checked to lie in ``[0, N)``."""
+        if self._table is None:
+            raise RuntimeError("arm_train_data() first")
+        t = idx if isinstance(idx, torch.Tensor) else torch.from_numpy(np.asarray(idx))
+        if t.device.type != "cpu" or t.dtype.is_floating_point or t.dtype == torch.bool or t.dtype.is_complex:
+            raise ValueError("row indices must be an integer host array, got %s on %s" % (t.dtype, t.device))
+        if t.numel() != self.batch_size:
+            raise ValueError("%d row indices for a batch of %d" % (t.numel(), self.batch_size))
+        n = self._table[1].numel()
+        lo, hi = int(t.min()), int(t.max())
+        if lo < 0 or hi >= n:
+            raise ValueError("row index %d outside the training set [0, %d)" % (lo if lo < 0 else hi, n))
+        if t.dtype != torch.int32 or not t.is_contiguous():
+            t = t.reshape(-1).to(torch.int32).contiguous()
+        return t.reshape(-1)
+
+    def _gather(self, s: int) -> None:
+        img, lbl = self._table
+        check(self.lib.dm_gather_batch(ptr(self._idx_dev[s]), ptr(img), ptr(lbl), self.batch_size, ptr(self.in_dev[s]),
+                                       stream_ptr(self.copy_stream)), "gather_batch")
+
+    def load_indices(self, idx) -> None:
+        """Counterpart of :meth:`load_batch` for the armed training set: B row indices -> pinned staging -> device index
+        slot, then the gather into the input slot, on the copy stream (overlaps the previous step)."""
+        self._leave_native_runner()
+        t = self._as_indices(idx)
+        s = self._loaded & 1
+        h = self._h_idx[s]
+        h.copy_(t)
+        with torch.cuda.stream(self.copy_stream):
+            self.copy_stream.wait_event(self._slot_free[s])
+            self._idx_dev[s].copy_(h, non_blocking=True)
+            self._gather(s)
+            self._copy_done[s].record(self.copy_stream)
+        self._slot = s
+        self._loaded += 1
+
+    def step_indices(self, idx):
+        """Counterpart of :meth:`step_packed` for the armed training set: one whole step from B row indices (index DMA,
+        gather, event chaining and the graph launch in ONE native call once both slot graphs exist; before that, or with
+        ``DMNIST_NATIVE_RUNNER=0``, the torch-dispatched path).  A page-locked ``idx`` is read by an asynchronous DMA: it must
+        stay untouched until the step after the next one has been enqueued.  Returns ``(waitable, loss buffer, seq)``."""
+        t = self._as_indices(idx)
+        r = getattr(self, "_runner", None)
+        if r is None and self.use_graph and self._opt_args is not None and os.environ.get("DMNIST_NATIVE_RUNNER", "1") != "0" \
+                and all(g is not None and g[1] for g in self._graphs):
+            r = self._make_runner()
+        if r is None:
+            self.load_indices(t)
+            self.train_step()
+            return self.read_result_async()
+        if not t.is_pinned():
+            t = t.pin_memory()
+        s = int(self.lib.dm_runner_step_indices(r, ctypes.c_void_p(t.data_ptr())))
+        if s < 0:
+            raise RuntimeError("dm_runner_step_indices failed: CUDA error %d" % -s)
+        self._keep_alive[s] = t                          # the DMA reads it asynchronously
+        self._slot = s
+        self._loaded += 1
+        self._steps_launched += 1
+        return _RunnerEvent(self.lib, r, s), self.h_loss_bufs[s], self._seq0 + self._steps_launched
+
     # ---- native step executor (csrc/step_runner.cu) ----------------------------------------------------------------------
     def step_packed(self, packed: torch.Tensor):
         """One whole training step from a packed batch (see :meth:`pack_batch`; pinned host or device memory): input DMA,
@@ -227,6 +307,9 @@ class CudaLeNetEngine(ComputeEngine):
                                  ctypes.c_ulonglong(self._in_bytes), int(self._loaded & 1))
         if not r:
             return None
+        if self._table is not None:
+            check(lib.dm_runner_arm_gather(ctypes.c_void_p(r), ptr(self._idx_dev[0]), ptr(self._idx_dev[1]),
+                                           ptr(self._table[0]), ptr(self._table[1]), self.batch_size), "runner_arm_gather")
         self._runner = ctypes.c_void_p(r)
         self._keep_alive = [None, None]
         return self._runner
@@ -928,6 +1011,12 @@ class CudaMlpEngine(ComputeEngine):
     _make_runner = CudaLeNetEngine._make_runner
     pack_batch = CudaLeNetEngine.pack_batch
     load_packed = CudaLeNetEngine.load_packed
+    arm_train_data = CudaLeNetEngine.arm_train_data
+    _as_indices = CudaLeNetEngine._as_indices
+    _gather = CudaLeNetEngine._gather
+    load_indices = CudaLeNetEngine.load_indices
+    step_indices = CudaLeNetEngine.step_indices
+    _table = None
     attach_optimizer = CudaLeNetEngine.attach_optimizer
     _enqueue_iteration_begin = CudaLeNetEngine._enqueue_iteration_begin
     _enqueue_iteration_end = CudaLeNetEngine._enqueue_iteration_end

@@ -254,6 +254,9 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
                                           "when a device-side watchdog fires (reference: the optimizer's debug Print ops)")
     F.DEFINE_boolean("pipeline_steps", True, "GPU path: enqueue step i+1 before reading step i's loss / status words "
                                              "(page-locked result buffers, background batch packer)")
+    F.DEFINE_boolean("device_data", False, "GPU path: keep each replica's training set in GPU memory and feed every step "
+                                           "B int32 row indices, gathered into the input slot on the device, instead of a "
+                                           "batch packed on the host (not with --fake_data; sm_90a engine only)")
     F.DEFINE_integer("log_every", 1, "Log every n-th local iteration (1 = reference behaviour)")
     F.DEFINE_float("dropout_keep_prob", 0.5, "Keep probability of the fc1 dropout (reference mnist.py:139)")
     F.DEFINE_integer("eval_every_steps", 0, "Chief: score the validation set after every E-th global step and after the last "

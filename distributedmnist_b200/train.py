@@ -144,6 +144,39 @@ class _BatchPacker:
             t.join(timeout=2.0)
 
 
+class _IndexFeed:
+    """Input pipeline of ``--device_data``: each step's B row indices (``dataset.next_batch_indices``, cast to int32) in a
+    small ring of page-locked buffers, drawn on the training thread -- one numpy slice per step.  The engine's index DMA
+    reads a buffer asynchronously, so a buffer is rewritten only after the step after the next one has been enqueued: the
+    ring holds ``depth`` >= 3 buffers and the loop enqueues one buffer per step."""
+
+    def __init__(self, dataset, batch_size: int, depth: int = 4):
+        assert depth >= 3
+        self.dataset, self.batch_size = dataset, batch_size
+        self.ring = [torch.empty(batch_size, dtype=torch.int32).pin_memory() for _ in range(depth)]
+        self._i = 0
+
+    def next(self) -> torch.Tensor:
+        buf = self.ring[self._i % len(self.ring)]
+        self._i += 1
+        np.copyto(buf.numpy(), self.dataset.next_batch_indices(self.batch_size), casting="unsafe")
+        return buf
+
+    def close(self) -> None:
+        pass                       # no helper thread to stop (same interface as _BatchPacker)
+
+
+def check_device_data_flags(flags, ctx: ReplicaContext, dataset) -> None:
+    """``--device_data`` combinations that cannot work, rejected before any device work starts."""
+    if not getattr(flags, "device_data", False):
+        return
+    if flags.fake_data or getattr(dataset, "fake_data", False):
+        raise ValueError("--device_data cannot be combined with --fake_data: there is no training set to keep on the GPU")
+    if not (ctx.on_gpu and flags.backend in ("auto", "fused")):
+        raise ValueError("--device_data needs the sm_90a engine (a GPU and --backend=auto or fused); the torch engine "
+                         "(--backend=%s%s) feeds its batches from the host" % (flags.backend, "" if ctx.on_gpu else ", no GPU"))
+
+
 def check_eval_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate: int, dataset_test) -> None:
     """``--eval_every_steps`` combinations that cannot work, rejected before any device work starts."""
     if getattr(flags, "eval_every_steps", 0) < 0:
@@ -190,6 +223,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     assert num_workers > 0
     is_chief = ctx.is_chief
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
+    check_device_data_flags(flags, ctx, dataset)
+    device_data = bool(getattr(flags, "device_data", False))
 
     backend = make_backend(ctx, flags.backend, flags)
     engine = make_engine(flags, ctx, backend)
@@ -247,6 +282,9 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     snapshot_eval = device_eval and bool(getattr(flags, "eval_snapshot", False)) and not exact
     if device_eval:
         engine.arm_eval(dataset_test.images, dataset_test.labels, snapshot=snapshot_eval)
+    if device_data:
+        # every replica keeps its own copy, in its own shuffled order: a step's input is then B row indices
+        engine.arm_train_data(dataset.images, dataset.labels)
     eval_rows = []                 # (global_step, t_begin_unix_s, eval_seconds, examples, correct, mean_loss)
     last_eval_step = -1
     eval_mark = restored_step      # snapshot passes: global step consumed when the last one was enqueued
@@ -289,7 +327,9 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     # batches are packed into page-locked buffers by a helper thread (`_BatchPacker`).
     pipelined = bool(fused_step and getattr(flags, "pipeline_steps", True) and hasattr(engine, "read_result_async")
                      and not flags.timeline_logging)
-    packer = _BatchPacker(engine, dataset, flags.batch_size) if pipelined else None
+    # --device_data: the batch is gathered on the device from B row indices (_IndexFeed) instead of packed on the host
+    packer = (_IndexFeed(dataset, flags.batch_size) if device_data else _BatchPacker(engine, dataset, flags.batch_size)) \
+        if pipelined else None
     every = max(flags.log_every, 1)
     pending = None                 # (iteration, start_time, result token) of the step in flight
     launched = 0
@@ -389,7 +429,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         if pipelined:
             if do_log:
                 log.info("RUNNING SESSION... %f" % time.time())
-            token = (cur_iteration, engine.step_packed(packer.next()))   # input DMA + step graph: one native call
+            # input DMA (+ gather) + step graph: one native call
+            token = (cur_iteration, engine.step_indices(packer.next()) if device_data else engine.step_packed(packer.next()))
             launched += 1
             if device_eval and not snapshot_eval and \
                     ((restored_step + launched) % eval_every == 0 or restored_step + launched > flags.max_steps):
@@ -416,14 +457,20 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
 
         tl = Timeline(pid=ctx.rank) if flags.timeline_logging else None
         start_time = time.time()
-        images, labels = dataset.next_batch(flags.batch_size)
+        if device_data:
+            rows = dataset.next_batch_indices(flags.batch_size)
+        else:
+            images, labels = dataset.next_batch(flags.batch_size)
         if tl:
             tl.add_span("next_batch", 0.0, (time.time() - start_time) * 1e6)
         if do_log:
             log.info("RUNNING SESSION... %f" % time.time())
 
         t0 = time.perf_counter()
-        engine.load_batch(images, labels)
+        if device_data:
+            engine.load_indices(rows)
+        else:
+            engine.load_batch(images, labels)
         t1 = time.perf_counter()
         t_fin = None
         dev_spans = None
