@@ -1,8 +1,8 @@
 // conv1 (5x5 SAME, 1 -> 32 channels, 28x28 images) on the tensor cores: forward and weight gradient.
 // reference ops K1-K4 (tf.nn.conv2d #1 + bias + ReLU + max_pool, src/mnist.py:107-118) and their gradients.
 //
-// K = 25 taps is too thin to be FLOP-relevant, but the SIMT kernels of lenet_simt.cu sit on the fp32 FMA-pipe
-// floor, so the thin GEMMs move to wgmma anyway.  With C_in = 1 no TMA box can express the im2col operand (a K
+// K = 25 taps is too thin to be FLOP-relevant, but SIMT kernels sit on the fp32 FMA-pipe floor, so the thin
+// GEMMs move to wgmma anyway.  With C_in = 1 no TMA box can express the im2col operand (a K
 // step would be 2 bytes), so the operand is built in shared memory by software -- 36 input values per pooled
 // pixel -- in the 64-byte-swizzled layout TMA would write.
 //
@@ -413,7 +413,5 @@ static int launch_conv1_wgrad(const void* images, const void* dpool, const void*
 
 // g_w [25][32] and g_b [32] must be zeroed by the caller (the gradient is added to them).
 extern "C" int dm_conv1_wgrad_tc(const void* images, const void* dpool, const void* code, void* g_w, void* g_b, int B, void* stream) {
-  static const int tile = dm::env_int("DMNIST_C1WG_TILE", 64);
-  if (tile == 64) return launch_conv1_wgrad<64>(images, dpool, code, g_w, g_b, B, stream);
-  return launch_conv1_wgrad<128>(images, dpool, code, g_w, g_b, B, stream);
+  return launch_conv1_wgrad<64>(images, dpool, code, g_w, g_b, B, stream);
 }

@@ -1,7 +1,5 @@
 #include "host_utils.h"
 
-#include <stdlib.h>
-
 #include <mutex>
 
 namespace dm {
@@ -20,11 +18,6 @@ int num_sms() {
       return 1;
   }
   return n;
-}
-
-int env_int(const char* name, int dflt) {
-  const char* v = getenv(name);
-  return (v != nullptr && *v != 0) ? atoi(v) : dflt;
 }
 
 void* driver_symbol(const char* name) {

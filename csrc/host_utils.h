@@ -50,9 +50,6 @@ inline cudaError_t launch_kernel(Kern kern, dim3 grid, dim3 block, size_t smem, 
   return cudaLaunchKernelEx(&cfg, kern, args...);
 }
 
-// Integer knob from the environment (A/B switches between kernel generations), read once by the callers.
-int env_int(const char* name, int dflt);
-
 // Resolve a driver API symbol through the runtime (cudaGetDriverEntryPoint).
 void* driver_symbol(const char* name);
 

@@ -1,230 +1,13 @@
-// SIMT kernels of the LeNet pipeline: the ops whose GEMM view is too thin for tensor cores
-// (SURVEY §2.4 K1: K = 25; K8: N = 10) plus the fused pooling / ReLU / loss bookkeeping.
+// SIMT kernels of the LeNet pipeline: fc2 and the loss, whose GEMM view is too thin for tensor cores
+// (SURVEY §2.4 K8: N = 10), fused with the fc1 epilogue and the loss bookkeeping.
 //
-//   conv1_fwd      K1+K2+K3+K4  conv5x5(1->32,SAME) + bias + ReLU + maxpool2x2   (src/mnist.py:107-118)
-//   fc2_loss       K6 epilogue (bias+ReLU+dropout on the fc1 accumulator, K7) + K8 + K9 + K10 and
-//                  their backward: dlogits, fc2 wgrad/bgrad, d(fc1 pre-activation), fc1 bgrad
-//                  (src/mnist.py:136-145,149-164)
-//   unpool2        backward of maxpool2 + ReLU2 (scatter to the argmax position) + conv2 bias grad
-//   conv1_wgrad    backward of maxpool1 + ReLU1 fused with the conv1 weight/bias gradient
-//
-// Pooling stores one code byte per pooled element: bits 0-1 = argmax position (dy*2+dx),
-// bit 2 = ReLU active; the backward kernels need nothing else.
+//   fc2_fwd_bwd    K6 epilogue (bias+ReLU+dropout on the fc1 split-K partials, K7) + K8 + K9 + K10 and
+//                  their backward: dlogits, d(fc1 pre-activation)   (src/mnist.py:136-145,149-164)
+//   fc2_wgrad      fc2 weight/bias gradients and the fc1 bias gradient
 #include "common.cuh"
 #include "host_utils.h"
 
 namespace dm {
-
-// Two channels per call (the same rounding as one fmaf each): keeps the channel-pair register layout of the loops.
-DMNIST_DEVICE float2 fma2_rn(float2 a, float2 b, float2 c) {
-  return make_float2(__fmaf_rn(a.x, b.x, c.x), __fmaf_rn(a.y, b.y, c.y));
-}
-
-
-// =====================================================================================================
-// conv1 forward, fused.  One CTA per (image, pair of pooled rows): 2 x 14 pooled positions x 32 channels.
-// Work item = (pooled position, group of 8 channels): 4 conv outputs x 8 channels x 25 taps = 800 FMA,
-// fed from shared memory (12 input values + 10 weight vectors per filter row).
-// =====================================================================================================
-constexpr int C1_THREADS = 128;   // 112 work items + 16 idle lanes
-
-struct ZeroRanges {
-  float* ptr[3];
-  int n[3];
-};
-
-__global__ void __launch_bounds__(C1_THREADS) conv1_fwd_kernel(const float* __restrict__ images,  // [B,28,28]
-                                                               const float* __restrict__ w,       // [25][32]
-                                                               const float* __restrict__ bias,    // [32]
-                                                               __nv_bfloat16* __restrict__ out,   // [B,14,14,32]
-                                                               uint8_t* __restrict__ code,        // [B,14,14,32]
-                                                               ZeroRanges zr) {
-  pdl_wait();
-  // (no early launch_dependents: resident-but-blocked CTAs of the next kernel steal SM resources from this one)
-  // First kernel of a training step: also clears the gradient regions that later kernels accumulate into
-  // with atomics and the loss accumulator (replaces three memset nodes of the step graph).
-  {
-    const int gi = blockIdx.x * C1_THREADS + threadIdx.x;
-#pragma unroll
-    for (int r = 0; r < 3; ++r)
-      if (zr.ptr[r] != nullptr)
-        for (int i = gi; i < zr.n[r]; i += gridDim.x * C1_THREADS) zr.ptr[r][i] = 0.f;
-  }
-  __shared__ float s_img[8][32];        // input rows 4*u-2 .. 4*u+5, columns -2 .. 29 (zero halo)
-  __shared__ __align__(16) float s_w[25][32];
-  __shared__ float s_b[32];
-  const int b = blockIdx.x / 7, u = blockIdx.x - b * 7;   // u: pooled rows 2u, 2u+1
-  const int row0 = 4 * u - 2;
-  for (int i = threadIdx.x; i < 8 * 32; i += C1_THREADS) {
-    const int r = i >> 5, c = i & 31;
-    const int y = row0 + r, x = c - 2;
-    s_img[r][c] = (y >= 0 && y < 28 && x >= 0 && x < 28) ? __ldg(images + (size_t)b * 784 + y * 28 + x) : 0.f;
-  }
-  for (int i = threadIdx.x; i < 200; i += C1_THREADS)
-    reinterpret_cast<float4*>(&s_w[0][0])[i] = __ldg(reinterpret_cast<const float4*>(w) + i);
-  if (threadIdx.x < 32) s_b[threadIdx.x] = bias[threadIdx.x];
-  __syncthreads();
-
-  const int cg = threadIdx.x & 3, pos = threadIdx.x >> 2;
-  if (pos >= 28) return;
-  const int pr = pos / 14, pc = pos - pr * 14;          // pooled row (local) / col
-  // channel pairs: input value broadcast to both halves
-  float2 acc2[4][4];
-#pragma unroll
-  for (int p = 0; p < 4; ++p)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc2[p][j] = make_float2(0.f, 0.f);
-#pragma unroll 1
-  for (int kh = 0; kh < 5; ++kh) {
-    float r0[6], r1[6];                                   // the two input rows this filter row touches
-#pragma unroll
-    for (int c = 0; c < 6; ++c) {
-      r0[c] = s_img[2 * pr + kh][2 * pc + c];
-      r1[c] = s_img[2 * pr + kh + 1][2 * pc + c];
-    }
-#pragma unroll
-    for (int kw = 0; kw < 5; ++kw) {
-      const float4 w0 = *reinterpret_cast<const float4*>(&s_w[kh * 5 + kw][cg * 8]);
-      const float4 w1 = *reinterpret_cast<const float4*>(&s_w[kh * 5 + kw][cg * 8 + 4]);
-      const float2 wv[4] = {make_float2(w0.x, w0.y), make_float2(w0.z, w0.w), make_float2(w1.x, w1.y),
-                            make_float2(w1.z, w1.w)};
-      const float2 a00 = make_float2(r0[kw], r0[kw]), a01 = make_float2(r0[kw + 1], r0[kw + 1]);
-      const float2 a10 = make_float2(r1[kw], r1[kw]), a11 = make_float2(r1[kw + 1], r1[kw + 1]);
-#pragma unroll
-      for (int j = 0; j < 4; ++j) {
-        acc2[0][j] = fma2_rn(a00, wv[j], acc2[0][j]);
-        acc2[1][j] = fma2_rn(a01, wv[j], acc2[1][j]);
-        acc2[2][j] = fma2_rn(a10, wv[j], acc2[2][j]);
-        acc2[3][j] = fma2_rn(a11, wv[j], acc2[3][j]);
-      }
-    }
-  }
-  float acc[4][8];
-#pragma unroll
-  for (int p = 0; p < 4; ++p)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) { acc[p][2 * j] = acc2[p][j].x; acc[p][2 * j + 1] = acc2[p][j].y; }
-  uint32_t packed[4];
-  uint32_t cd[2] = {0u, 0u};
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    float m = acc[0][j];
-    uint32_t idx = 0;
-#pragma unroll
-    for (int p = 1; p < 4; ++p)
-      if (acc[p][j] > m) { m = acc[p][j]; idx = p; }
-    m += s_b[cg * 8 + j];
-    const bool active = m > 0.f;
-    cd[j >> 2] |= (idx | (active ? 4u : 0u)) << ((j & 3) * 8);
-    const float o = active ? m : 0.f;
-    if (j & 1) packed[j >> 1] = pack_bf16x2(__uint_as_float(packed[j >> 1]), o);
-    else packed[j >> 1] = __float_as_uint(o);
-  }
-  const size_t o = (((size_t)b * 14 + 2 * u + pr) * 14 + pc) * 32 + cg * 8;
-  *reinterpret_cast<uint4*>(out + o) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-  *reinterpret_cast<uint2*>(code + o) = make_uint2(cd[0], cd[1]);
-}
-
-// conv1 forward, second generation.  Same CTA = (image, pair of pooled rows), but a thread owns TWO horizontally adjacent
-// pooled positions (2 x 4 conv outputs) x 8 channels: the ten 16-byte weight loads of a filter row now feed 160 packed
-// FMAs instead of 80 and the input window is four aligned 16-byte loads, so the loop is bound by the FMA pipe rather
-// than by shared-memory issue slots (the first version spent more instructions on loads and address arithmetic than
-// on FMAs).  64 threads: 56 work items = 2 rows x 7 column pairs x 4 groups.
-constexpr int C1B_THREADS = 64;
-
-__global__ void __launch_bounds__(C1B_THREADS) conv1_fwd2_kernel(const float* __restrict__ images,  // [B,28,28]
-                                                                 const float* __restrict__ w,       // [25][32]
-                                                                 const float* __restrict__ bias,    // [32]
-                                                                 __nv_bfloat16* __restrict__ out,   // [B,14,14,32]
-                                                                 uint8_t* __restrict__ code,        // [B,14,14,32]
-                                                                 ZeroRanges zr) {
-  __shared__ __align__(16) float s_img[8][32];        // input rows 4*u-2 .. 4*u+5, columns -2 .. 29 (zero halo)
-  __shared__ __align__(16) float s_w[25][32];
-  __shared__ float s_b[32];
-  const int b = blockIdx.x / 7, u = blockIdx.x - b * 7;   // u: pooled rows 2u, 2u+1
-  // weights and bias are final long before the previous kernel of the stream started: fetch them ahead of the wait
-  for (int i = threadIdx.x; i < 200; i += C1B_THREADS)
-    reinterpret_cast<float4*>(&s_w[0][0])[i] = __ldg(reinterpret_cast<const float4*>(w) + i);
-  if (threadIdx.x < 32) s_b[threadIdx.x] = __ldg(bias + threadIdx.x);
-  pdl_wait();
-  {
-    const int gi = blockIdx.x * C1B_THREADS + threadIdx.x;
-#pragma unroll
-    for (int r = 0; r < 3; ++r)
-      if (zr.ptr[r] != nullptr)
-        for (int i = gi; i < zr.n[r]; i += gridDim.x * C1B_THREADS) zr.ptr[r][i] = 0.f;
-  }
-  const int row0 = 4 * u - 2;
-  for (int i = threadIdx.x; i < 8 * 32; i += C1B_THREADS) {
-    const int r = i >> 5, c = i & 31;
-    const int y = row0 + r, x = c - 2;
-    s_img[r][c] = (y >= 0 && y < 28 && x >= 0 && x < 28) ? __ldg(images + (size_t)b * 784 + y * 28 + x) : 0.f;
-  }
-  __syncthreads();
-
-  const int cg = threadIdx.x & 3, item = threadIdx.x >> 2;
-  if (item >= 14) return;
-  const int pr = item / 7, pair = item - pr * 7;          // pooled row (local), pair of pooled columns
-  float2 acc[8][4];                                       // [conv output: row * 4 + column][channel pair]
-#pragma unroll
-  for (int p = 0; p < 8; ++p)
-#pragma unroll
-    for (int j = 0; j < 4; ++j) acc[p][j] = make_float2(0.f, 0.f);
-#pragma unroll 1
-  for (int kh = 0; kh < 5; ++kh) {
-    float r0[8], r1[8];                                   // the two input rows this filter row touches, 8 columns
-    {
-      const float4* p0 = reinterpret_cast<const float4*>(&s_img[2 * pr + kh][4 * pair]);
-      const float4* p1 = reinterpret_cast<const float4*>(&s_img[2 * pr + kh + 1][4 * pair]);
-      const float4 a = p0[0], bq = p0[1], c = p1[0], d = p1[1];
-      r0[0] = a.x; r0[1] = a.y; r0[2] = a.z; r0[3] = a.w; r0[4] = bq.x; r0[5] = bq.y; r0[6] = bq.z; r0[7] = bq.w;
-      r1[0] = c.x; r1[1] = c.y; r1[2] = c.z; r1[3] = c.w; r1[4] = d.x; r1[5] = d.y; r1[6] = d.z; r1[7] = d.w;
-    }
-#pragma unroll
-    for (int kw = 0; kw < 5; ++kw) {
-      const float4 w0 = *reinterpret_cast<const float4*>(&s_w[kh * 5 + kw][cg * 8]);
-      const float4 w1 = *reinterpret_cast<const float4*>(&s_w[kh * 5 + kw][cg * 8 + 4]);
-      const float2 wv[4] = {make_float2(w0.x, w0.y), make_float2(w0.z, w0.w), make_float2(w1.x, w1.y),
-                            make_float2(w1.z, w1.w)};
-#pragma unroll
-      for (int col = 0; col < 4; ++col) {
-        const float2 a0 = make_float2(r0[col + kw], r0[col + kw]), a1 = make_float2(r1[col + kw], r1[col + kw]);
-#pragma unroll
-        for (int j = 0; j < 4; ++j) {
-          acc[col][j] = fma2_rn(a0, wv[j], acc[col][j]);
-          acc[4 + col][j] = fma2_rn(a1, wv[j], acc[4 + col][j]);
-        }
-      }
-    }
-  }
-#pragma unroll
-  for (int pos = 0; pos < 2; ++pos) {
-    uint32_t packed[4];
-    uint32_t cd[2] = {0u, 0u};
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      // window order = argmax code: 0 (dy0,dx0), 1 (dy0,dx1), 2 (dy1,dx0), 3 (dy1,dx1)
-      const float v[4] = {(j & 1) ? acc[2 * pos][j >> 1].y : acc[2 * pos][j >> 1].x,
-                          (j & 1) ? acc[2 * pos + 1][j >> 1].y : acc[2 * pos + 1][j >> 1].x,
-                          (j & 1) ? acc[4 + 2 * pos][j >> 1].y : acc[4 + 2 * pos][j >> 1].x,
-                          (j & 1) ? acc[4 + 2 * pos + 1][j >> 1].y : acc[4 + 2 * pos + 1][j >> 1].x};
-      float m = v[0];
-      uint32_t idx = 0;
-#pragma unroll
-      for (int p = 1; p < 4; ++p)
-        if (v[p] > m) { m = v[p]; idx = p; }
-      m += s_b[cg * 8 + j];
-      const bool active = m > 0.f;
-      cd[j >> 2] |= (idx | (active ? 4u : 0u)) << ((j & 3) * 8);
-      const float o = active ? m : 0.f;
-      if (j & 1) packed[j >> 1] = pack_bf16x2(__uint_as_float(packed[j >> 1]), o);
-      else packed[j >> 1] = __float_as_uint(o);
-    }
-    const size_t o = (((size_t)b * 14 + 2 * u + pr) * 14 + 2 * pair + pos) * 32 + cg * 8;
-    *reinterpret_cast<uint4*>(out + o) = make_uint4(packed[0], packed[1], packed[2], packed[3]);
-    *reinterpret_cast<uint2*>(code + o) = make_uint2(cd[0], cd[1]);
-  }
-}
 
 // =====================================================================================================
 // fc2 + softmax cross entropy + accuracy, forward and backward, as two kernels:
@@ -449,167 +232,9 @@ __global__ void __launch_bounds__(256) fc2_wgrad_kernel(const float* __restrict_
   }
 }
 
-// =====================================================================================================
-// unpool2: d(pool2 out) [B,7,7,64] (bf16) -> d(conv2 pre-activation) [B,14,14,64] (bf16, dense with zeros),
-// plus the conv2 bias gradient.
-// =====================================================================================================
-__global__ void __launch_bounds__(256) unpool2_kernel(const __nv_bfloat16* __restrict__ dpool,  // [B,3136]
-                                                      const uint8_t* __restrict__ code,         // [B,3136]
-                                                      __nv_bfloat16* __restrict__ dy,           // [B,14,14,64]
-                                                      float* __restrict__ g_bias,               // [64]
-                                                      int B) {
-  __shared__ float s_gb[64];
-  if (threadIdx.x < 64) s_gb[threadIdx.x] = 0.f;
-  __syncthreads();
-  pdl_wait();
-  // (no early launch_dependents: resident-but-blocked CTAs of the next kernel steal SM resources from this one)
-  const int total = B * 49 * 8;   // (b, pooled position, group of 8 channels)
-  float gsum[8];                  // bias-gradient partials: a thread keeps the same channel group across trips
-#pragma unroll
-  for (int j = 0; j < 8; ++j) gsum[j] = 0.f;
-  for (int t = blockIdx.x * blockDim.x + threadIdx.x; t < total; t += gridDim.x * blockDim.x) {
-    const int cg = t & 7, pos = (t >> 3) % 49, b = (t >> 3) / 49;
-    const int ph = pos / 7, pw = pos - ph * 7;
-    const size_t src = ((size_t)b * 49 + pos) * 64 + cg * 8;
-    const uint4 gv = *reinterpret_cast<const uint4*>(dpool + src);
-    const uint2 cv = *reinterpret_cast<const uint2*>(code + src);
-    const uint32_t g32[4] = {gv.x, gv.y, gv.z, gv.w};
-    uint32_t o[4][4];
-#pragma unroll
-    for (int p = 0; p < 4; ++p)
-#pragma unroll
-      for (int k = 0; k < 4; ++k) o[p][k] = 0u;
-#pragma unroll
-    for (int j = 0; j < 8; ++j) {
-      const uint32_t c = ((j < 4 ? cv.x : cv.y) >> ((j & 3) * 8)) & 0xffu;
-      const uint32_t half = (g32[j >> 1] >> ((j & 1) * 16)) & 0xffffu;
-      if (c & 4u) {
-        o[c & 3u][j >> 1] |= half << ((j & 1) * 16);
-        gsum[j] += __bfloat162float(__ushort_as_bfloat16((unsigned short)half));
-      }
-    }
-#pragma unroll
-    for (int p = 0; p < 4; ++p) {
-      const int y = 2 * ph + (p >> 1), x = 2 * pw + (p & 1);
-      *reinterpret_cast<uint4*>(dy + (((size_t)b * 14 + y) * 14 + x) * 64 + cg * 8) =
-          make_uint4(o[p][0], o[p][1], o[p][2], o[p][3]);
-    }
-  }
-  // lanes l, l+8, l+16, l+24 of a warp share the channel group: fold them with two shuffles
-#pragma unroll
-  for (int j = 0; j < 8; ++j) {
-    gsum[j] += __shfl_xor_sync(0xffffffffu, gsum[j], 8);
-    gsum[j] += __shfl_xor_sync(0xffffffffu, gsum[j], 16);
-  }
-  if ((threadIdx.x & 31) < 8) {
-#pragma unroll
-    for (int j = 0; j < 8; ++j) atomicAdd(&s_gb[(threadIdx.x & 7) * 8 + j], gsum[j]);
-  }
-  __syncthreads();
-  if (threadIdx.x < 64) atomicAdd(g_bias + threadIdx.x, s_gb[threadIdx.x]);
-}
-
-// =====================================================================================================
-// conv1 wgrad fused with the backward of maxpool1 + ReLU1.  One CTA per image, lane = channel.
-//   dW[tap][c] += img[y+kh-2][x+kw-2] * g   where (y,x) is the argmax position of pooled element g.
-// =====================================================================================================
-__global__ void __launch_bounds__(256) conv1_wgrad_kernel(const float* __restrict__ images,        // [B,28,28]
-                                                          const __nv_bfloat16* __restrict__ dpool, // [B,14,14,32]
-                                                          const uint8_t* __restrict__ code,        // [B,14,14,32]
-                                                          float* __restrict__ g_w,                 // [25][32]
-                                                          float* __restrict__ g_b,                 // [32]
-                                                          int B) {
-  // Everything an image needs is staged in shared memory with wide coalesced loads first (the loop below
-  // would otherwise expose one global-load latency per pooled position).
-  __shared__ float s_img[32][34];     // row stride 34: the four argmax positions of a window hit distinct banks
-  __shared__ __align__(16) float s_g[8 * 26 * 32];     // [196][32] masked gradients; reused as [8][26][32] for the reduction
-  __shared__ __align__(8) uint8_t s_pos[196 * 32];     // argmax position code (bits 0-1)
-  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
-  pdl_wait();
-  // (no early launch_dependents: resident-but-blocked CTAs of the next kernel steal SM resources from this one)
-  float acc[26];
-#pragma unroll
-  for (int t = 0; t < 26; ++t) acc[t] = 0.f;
-  for (int b = blockIdx.x; b < B; b += gridDim.x) {
-    __syncthreads();
-    for (int i = threadIdx.x; i < 32 * 32; i += blockDim.x) {
-      const int r = i >> 5, c = i & 31, y = r - 2, x = c - 2;
-      s_img[r][c] = (y >= 0 && y < 28 && x >= 0 && x < 28) ? images[(size_t)b * 784 + y * 28 + x] : 0.f;
-    }
-    for (int i = threadIdx.x; i < 196 * 4; i += blockDim.x) {   // 8 channels per item
-      const size_t o = (size_t)b * 6272 + (size_t)i * 8;
-      const uint4 gv = *reinterpret_cast<const uint4*>(dpool + o);
-      const uint2 cv = *reinterpret_cast<const uint2*>(code + o);
-      const uint32_t g32[4] = {gv.x, gv.y, gv.z, gv.w};
-#pragma unroll
-      for (int j = 0; j < 8; ++j) {
-        const uint32_t c = ((j < 4 ? cv.x : cv.y) >> ((j & 3) * 8)) & 0xffu;
-        const float g = __bfloat162float(__ushort_as_bfloat16((unsigned short)((g32[j >> 1] >> ((j & 1) * 16)) & 0xffffu)));
-        s_g[i * 8 + j] = (c & 4u) ? g : 0.f;
-      }
-      *reinterpret_cast<uint2*>(s_pos + i * 8) = cv;
-    }
-    __syncthreads();
-    for (int pos = warp; pos < 196; pos += 8) {
-      const float g = s_g[pos * 32 + lane];
-      const uint32_t c = s_pos[pos * 32 + lane];
-      const int ph = pos / 14, pw = pos - ph * 14;
-      const int y = 2 * ph + ((c >> 1) & 1), x = 2 * pw + (c & 1);   // conv-output coordinates of the max
-#pragma unroll
-      for (int kh = 0; kh < 5; ++kh)
-#pragma unroll
-        for (int kw = 0; kw < 5; ++kw) acc[kh * 5 + kw] = fmaf(s_img[y + kh][x + kw], g, acc[kh * 5 + kw]);
-      acc[25] += g;
-    }
-  }
-  __syncthreads();
-#pragma unroll
-  for (int t = 0; t < 26; ++t) s_g[(warp * 26 + t) * 32 + lane] = acc[t];
-  __syncthreads();
-  for (int i = threadIdx.x; i < 26 * 32; i += blockDim.x) {
-    const int t = i >> 5, c = i & 31;
-    float s = 0.f;
-#pragma unroll
-    for (int w = 0; w < 8; ++w) s += s_g[(w * 26 + t) * 32 + c];
-    if (t < 25) atomicAdd(g_w + t * 32 + c, s);
-    else atomicAdd(g_b + c, s);
-  }
-}
-
-// bias + ReLU on an fp32 accumulator -> bf16 activations (MLP hidden layers), optionally zeroing the
-// accumulator for the next split-K pass.  Backward companion: mask the incoming gradient.
-__global__ void bias_relu_bf16_kernel(float* __restrict__ acc, const float* __restrict__ bias,
-                                      __nv_bfloat16* __restrict__ out, int rows, int cols, int zero_acc) {
-  pdl_wait();
-  // (no early launch_dependents: resident-but-blocked CTAs of the next kernel steal SM resources from this one)
-  const long long n = (long long)rows * cols;
-  for (long long i = blockIdx.x * (long long)blockDim.x + threadIdx.x; i < n; i += (long long)gridDim.x * blockDim.x) {
-    const float v = acc[i] + bias[i % cols];
-    if (zero_acc) acc[i] = 0.f;
-    out[i] = __float2bfloat16(v > 0.f ? v : 0.f);
-  }
-}
-
 }  // namespace dm
 
 extern "C" {
-
-// zero0/1/2 (+ counts, in floats): optional regions cleared by the kernel.
-int dm_conv1_fwd(const void* images, const void* w, const void* bias, void* out, void* code, int B, void* zero0,
-                 int n0, void* zero1, int n1, void* zero2, int n2, void* stream) {
-  dm::ZeroRanges zr;
-  zr.ptr[0] = reinterpret_cast<float*>(zero0); zr.n[0] = n0;
-  zr.ptr[1] = reinterpret_cast<float*>(zero1); zr.n[1] = n1;
-  zr.ptr[2] = reinterpret_cast<float*>(zero2); zr.n[2] = n2;
-  static const int version = dm::env_int("DMNIST_CONV1_FWD", 2);     // 1: first-generation kernel (kept for A/B runs)
-  if (version == 1)
-    return (int)dm::launch_kernel(dm::conv1_fwd_kernel, dim3(7 * B), dim3(dm::C1_THREADS), 0, reinterpret_cast<cudaStream_t>(stream),
-        reinterpret_cast<const float*>(images), reinterpret_cast<const float*>(w), reinterpret_cast<const float*>(bias),
-        reinterpret_cast<__nv_bfloat16*>(out), reinterpret_cast<uint8_t*>(code), zr);
-  return (int)dm::launch_kernel(dm::conv1_fwd2_kernel, dim3(7 * B), dim3(dm::C1B_THREADS), 0, reinterpret_cast<cudaStream_t>(stream),
-      reinterpret_cast<const float*>(images), reinterpret_cast<const float*>(w), reinterpret_cast<const float*>(bias),
-      reinterpret_cast<__nv_bfloat16*>(out), reinterpret_cast<uint8_t*>(code), zr);
-}
 
 // Critical-path half: logits / loss / accuracy and (train) dh, h_out, dl_out.  scratch_h [B,512] fp32 and
 // scratch_dl [B,12] fp32 are only touched when train != 0.
@@ -657,32 +282,6 @@ int dm_fc2_wgrad(const void* scratch_h, const void* scratch_dl, const void* dh, 
                                 reinterpret_cast<const float*>(scratch_dl), reinterpret_cast<const __nv_bfloat16*>(dh),
                                 reinterpret_cast<float*>(g_w2), reinterpret_cast<float*>(g_b2),
                                 reinterpret_cast<float*>(g_b1), B);
-}
-
-int dm_unpool2(const void* dpool, const void* code, void* dy, void* g_bias, int B, void* stream) {
-  int grid = (B * 49 * 8 + 255) / 256;
-  if (grid > dm::num_sms() * 2) grid = dm::num_sms() * 2;
-  return (int)dm::launch_kernel(dm::unpool2_kernel, dim3(grid), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-      reinterpret_cast<const __nv_bfloat16*>(dpool), reinterpret_cast<const uint8_t*>(code),
-      reinterpret_cast<__nv_bfloat16*>(dy), reinterpret_cast<float*>(g_bias), B);
-}
-
-int dm_conv1_wgrad(const void* images, const void* dpool, const void* code, void* g_w, void* g_b, int B, void* stream) {
-  // one image per CTA (37 KB smem, 57 regs: up to four CTAs share an SM): all B CTAs are resident at once, so the
-  // staging latency of one overlaps the accumulation loop of its neighbours instead of serialising per image
-  int grid = B < dm::num_sms() * 4 ? B : dm::num_sms() * 4;
-  return (int)dm::launch_kernel(dm::conv1_wgrad_kernel, dim3(grid), dim3(256), 0, reinterpret_cast<cudaStream_t>(stream),
-      reinterpret_cast<const float*>(images), reinterpret_cast<const __nv_bfloat16*>(dpool),
-      reinterpret_cast<const uint8_t*>(code), reinterpret_cast<float*>(g_w), reinterpret_cast<float*>(g_b), B);
-}
-
-int dm_bias_relu_bf16(void* acc, const void* bias, void* out, int rows, int cols, int zero_acc, void* stream) {
-  long long n = (long long)rows * cols;
-  int grid = (int)((n + 255) / 256 < dm::num_sms() * 8 ? (n + 255) / 256 : dm::num_sms() * 8);
-  dm::bias_relu_bf16_kernel<<<grid, 256, 0, reinterpret_cast<cudaStream_t>(stream)>>>(
-      reinterpret_cast<float*>(acc), reinterpret_cast<const float*>(bias), reinterpret_cast<__nv_bfloat16*>(out), rows,
-      cols, zero_acc);
-  return (int)cudaGetLastError();
 }
 
 }  // extern "C"

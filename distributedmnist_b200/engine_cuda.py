@@ -3,20 +3,19 @@ replayed from one CUDA graph.
 
 Step = (reference src/distributed_train.py:332 ``sess.run(apply_gradients_op)``)::
 
-    memset(small grads, loss)                              2 memset nodes
-    conv1_fwd        conv+bias+ReLU+pool (SIMT, K=25)       csrc/lenet_simt.cu
+    memset(small grads, loss)                              folded into conv1_fwd
+    conv1_fwd        wgmma, software im2col + bias/ReLU/pool  csrc/conv1_tc.cu
     conv2_fwd        wgmma implicit GEMM + bias/ReLU/pool csrc/conv2_tc.cu
     fc1_fwd          wgmma GEMM, split-K into fp32        csrc/gemm_tc.cu
     fc2_fwd_bwd      bias+ReLU+dropout, fc2, softmax-CE,
                      accuracy, dlogits, d(fc1)              csrc/lenet_simt.cu
     fc2_wgrad        fc2 weight/bias + fc1 bias gradients   (side branch)
     fc1_wgrad        wgmma GEMM (MN-major x MN-major) -> gradient arena
-    fc1_dgrad        wgmma GEMM -> bf16
-    unpool2          maxpool2/ReLU2 backward + conv2 bias grad
+    fc1_dgrad        wgmma GEMM, maxpool2/ReLU2 backward + conv2 bias grad in the epilogue
     conv2_wgrad      wgmma, K = whole images, per-CTA partials -> workspace
     conv2_wgrad_reduce  the partials summed in fixed order -> gradient arena
     conv2_dgrad      wgmma
-    conv1_wgrad      maxpool1/ReLU1 backward + conv1 weight/bias grad
+    conv1_wgrad      wgmma, maxpool1/ReLU1 backward fused into the operand build
     fused_sync_sgd   arrival -> mask -> NVLink reduce -> 1/count -> SGD -> push -> bf16 shadow
 
 Weights live in TF layouts in one flat fp32 arena (symmetric memory); the tensor-core
@@ -25,6 +24,7 @@ calls cuDNN, cuBLAS or NCCL.
 """
 from __future__ import annotations
 
+import contextlib
 import ctypes
 import os
 from typing import Optional, Tuple
@@ -56,90 +56,70 @@ class _RunnerEvent:
         return self.lib.dm_runner_query(self.runner, self.slot) == 1
 
 
-class CudaLeNetEngine(ComputeEngine):
+class _CudaEngine(ComputeEngine):
+    """What the sm_90a engines share: parameter / gradient arenas, two input slots fed on a copy stream, the native step
+    runner, the optimizer binding and the graph-replayed step.  A subclass builds its kernel sequence in ``_launch_step``,
+    clears its gradients in ``_launch_zero`` and names its early bucket (``_bucket_early``, ``_g16_shape``)."""
     _kgtn_k = 0                  # K > N: gradients per update (count trigger); 0 = the K <= N / interval paths
     _table = None                # device-resident training set (images, labels), see arm_train_data
+    _runner = None               # native step runner (csrc/step_runner.cu), see _make_runner
+    _stamp = False               # cdf telemetry stamps in the step
+    _main_priority = 0           # priority of the stream the step graph is captured on
 
-    def __init__(self, batch_size: int, backend: FusedBackend, seed: int = 66478, rank: int = 0,
-                 keep_prob: float = 0.5, use_graph: bool = True):
+    def __init__(self, spec, batch_size: int, backend: FusedBackend, seed: int, use_graph: bool, image_shape):
         self.lib = load()
         self.backend = backend
-        self.device = backend.ctx.device
-        self.spec, _ = get_model("lenet")
+        self.device = dev = backend.ctx.device
+        self.spec = spec
         self.batch_size = B = batch_size
-        self.seed, self.rank, self.keep_prob = seed, rank, keep_prob
         self.use_graph = use_graph
-        dev = self.device
-        self.params = backend.allocate(self.spec.arena_numel)
-        self.params.copy_(self.spec.init_flat(seed).to(dev))
-        self.grads = backend.allocate(self.spec.arena_numel)
+        self.params = backend.allocate(spec.arena_numel)
+        self.params.copy_(spec.init_flat(seed).to(dev))
+        self.grads = backend.allocate(spec.arena_numel)
         self.shadow = backend.attach_shadow(self.params)
-        self.p = self.spec.views(self.params)
-        self.g = self.spec.views(self.grads)
-        self.pb = self.spec.views(self.shadow)
-        bf, u8, f32 = torch.bfloat16, torch.uint8, torch.float32
+        self.p, self.g, self.pb = (spec.views(t) for t in (self.params, self.grads, self.shadow))
+        f32 = torch.float32
         # two input slots so the H2D copy of step i+1 overlaps the compute of step i
         # (images and labels of a slot share one allocation so a packed host batch moves with ONE host->device copy)
         self._in_bytes = B * 784 * 4 + B * 8
-        self.in_dev = [torch.zeros(self._in_bytes, dtype=u8, device=dev) for _ in range(2)]
-        self.images = [t[:B * 784 * 4].view(f32).view(B, 28, 28) for t in self.in_dev]
+        self.in_dev = [torch.zeros(self._in_bytes, dtype=torch.uint8, device=dev) for _ in range(2)]
+        self.images = [t[:B * 784 * 4].view(f32).view(B, *image_shape) for t in self.in_dev]
         self.labels = [t[B * 784 * 4:].view(torch.int64) for t in self.in_dev]
-        self.h_images = [torch.zeros(B, 28, 28, dtype=f32).pin_memory() for _ in range(2)]
+        self.h_images = [torch.zeros(B, *image_shape, dtype=f32).pin_memory() for _ in range(2)]
         self.h_labels = [torch.zeros(B, dtype=torch.int64).pin_memory() for _ in range(2)]
-        self.a1 = torch.zeros(B, 14, 14, 32, dtype=bf, device=dev)
-        self.code1 = torch.zeros(B, 14, 14, 32, dtype=u8, device=dev)
-        self.a2 = torch.zeros(B, 3136, dtype=bf, device=dev)
-        self.code2 = torch.zeros(B, 3136, dtype=u8, device=dev)
-        self.fc1_splits = 7                                         # 49 k-blocks of 64 -> 7 per CTA
-        self.h_part = torch.zeros(self.fc1_splits, B, 512, dtype=f32, device=dev)   # fc1 split-K partial sums
-        self.dh = torch.zeros(B, 512, dtype=bf, device=dev)
-        self.h_act = torch.zeros(B, 512, dtype=f32, device=dev)      # post ReLU/dropout fc1 activations (fc2_wgrad operand)
-        self.dlogits = torch.zeros(B, 12, dtype=f32, device=dev)     # d loss / d logits, 48-byte rows
-        self.dxfc = torch.zeros(B, 3136, dtype=bf, device=dev)
-        self.dy2 = torch.zeros(B, 14, 14, 64, dtype=bf, device=dev)
-        self.dx1 = torch.zeros(B, 14, 14, 32, dtype=bf, device=dev)
         self.d_loss_acc = torch.zeros(2, dtype=f32, device=dev)
         self.h_loss_bufs = [torch.zeros(2, dtype=f32).pin_memory() for _ in range(2)]
-        self.h_loss_acc = self.h_loss_bufs[0]
-        self._loss_reads = 0
         self._slot = 0            # input slot the next step computes from
         self._loaded = 0
-        self._h2d_bytes = B * 784 * 4 + B * 8
         self.copy_stream = torch.cuda.Stream(device=dev)
-        # the data-gradient chain is the critical path: it is captured on a high-priority stream, the weight-gradient
-        # side branches on low-priority ones, so the block scheduler serves the chain first whenever both have CTAs pending
-        lo, hi = (0, -1)
-        self._side = [torch.cuda.Stream(device=dev, priority=lo) for _ in range(4)]
-        self._main_priority = hi if os.environ.get("DMNIST_PRIO", "1") != "0" else lo
-        self._wgrad_late = os.environ.get("DMNIST_WGRAD_LATE", "1") != "0"
-        self._branches = os.environ.get("DMNIST_BRANCHES", "1") != "0"
-        self._fuse_unpool = os.environ.get("DMNIST_FUSE_UNPOOL", "1") != "0"
-        self._conv1_tc = os.environ.get("DMNIST_CONV1_TC", "1") != "0"    # conv1 fwd / wgrad on wgmma (csrc/conv1_tc.cu)
         self._copy_done = [torch.cuda.Event() for _ in range(2)]
         self._slot_free = [torch.cuda.Event() for _ in range(2)]
         self._graphs = [None, None]
         self._opt_args: Optional[dict] = None
         self._straggler = None
-        self._stamp = False
-        p_fc1 = self.spec.param("fc1_weights")
-        self._zero_ranges = [(0, p_fc1.offset), (p_fc1.offset + p_fc1.numel, self.spec.arena_numel)]
-        self._seed_mix0 = dropout_seed_mix(seed, 0, rank)
-        # early bucket = fc1_weights (96.5 % of the bytes, final as soon as fc1_wgrad is done); everything else is late
-        self._bucket_split = p_fc1.offset
-        self._bucket_early = (p_fc1.offset, p_fc1.offset + p_fc1.numel)
         self._bucketed = False
         self._bucket_v2 = False       # bf16-wire early bucket + pushed late bucket (csrc/fused_bucket.cu)
         self._g16 = self._g16_view = self._inbox = None
-        self._epoch_ptr = ctypes.c_void_p(backend.ctrl.local_ptr + backend._off["epoch"])
         self.launches_per_step = 0
 
     # ---- inputs ------------------------------------------------------------------------------
     def _leave_native_runner(self) -> None:
         """The torch-dispatched path takes over again: its events know nothing about steps the native runner launched."""
-        if getattr(self, "_runner", None) is not None:
+        if self._runner is not None:
             torch.cuda.synchronize()
             self.lib.dm_runner_destroy(self._runner)
             self._runner = None
+
+    @contextlib.contextmanager
+    def _filling(self, s: int):
+        """Input slot ``s`` is filled by what the body enqueues on the copy stream: after the step that last read the slot,
+        and before the step that reads it next."""
+        with torch.cuda.stream(self.copy_stream):
+            self.copy_stream.wait_event(self._slot_free[s])   # the step that last read this slot is done
+            yield
+            self._copy_done[s].record(self.copy_stream)
+        self._slot = s
+        self._loaded += 1
 
     def load_batch(self, images, labels) -> None:
         """Pinned host staging -> device slot, on the copy stream (overlaps the previous step)."""
@@ -158,17 +138,13 @@ class CudaLeNetEngine(ComputeEngine):
             else:
                 hi.copy_(images.reshape(hi.shape))
                 hl.copy_(labels)
-        with torch.cuda.stream(self.copy_stream):
-            self.copy_stream.wait_event(self._slot_free[s])   # the step that last read this slot is done
+        with self._filling(s):
             self.images[s].copy_(hi, non_blocking=True)
             self.labels[s].copy_(hl, non_blocking=True)
-            self._copy_done[s].record(self.copy_stream)
-        self._slot = s
-        self._loaded += 1
 
     def pack_batch(self, images, labels, pin: bool = True) -> torch.Tensor:
         """One contiguous (page-locked) host buffer holding a batch in the device slot's layout: fp32 images
-        ``[B,28,28]`` followed by int64 labels ``[B]``.  Input pipelines that fill such buffers hand each batch to
+        ``[B,784]`` followed by int64 labels ``[B]``.  Input pipelines that fill such buffers hand each batch to
         :meth:`load_packed`, which is a single DMA."""
         B = self.batch_size
         buf = torch.empty(self._in_bytes, dtype=torch.uint8)
@@ -184,15 +160,11 @@ class CudaLeNetEngine(ComputeEngine):
         stream.  The buffer must stay untouched until the step after the next one has been enqueued."""
         self._leave_native_runner()
         s = self._loaded & 1
-        with torch.cuda.stream(self.copy_stream):
-            self.copy_stream.wait_event(self._slot_free[s])
+        with self._filling(s):
             self.in_dev[s].copy_(packed, non_blocking=True)
-            self._copy_done[s].record(self.copy_stream)
-        self._slot = s
-        self._loaded += 1
 
     def h2d_bytes_per_step(self) -> int:
-        return self._h2d_bytes
+        return self._in_bytes
 
     # ---- device-resident training set (csrc/batch_gather.cu) ------------------------------------------------------------
     def arm_train_data(self, images, labels) -> None:
@@ -240,13 +212,9 @@ class CudaLeNetEngine(ComputeEngine):
         s = self._loaded & 1
         h = self._h_idx[s]
         h.copy_(t)
-        with torch.cuda.stream(self.copy_stream):
-            self.copy_stream.wait_event(self._slot_free[s])
+        with self._filling(s):
             self._idx_dev[s].copy_(h, non_blocking=True)
             self._gather(s)
-            self._copy_done[s].record(self.copy_stream)
-        self._slot = s
-        self._loaded += 1
 
     def step_indices(self, idx):
         """Counterpart of :meth:`step_packed` for the armed training set: one whole step from B row indices (index DMA,
@@ -254,14 +222,13 @@ class CudaLeNetEngine(ComputeEngine):
         ``DMNIST_NATIVE_RUNNER=0``, the torch-dispatched path).  A page-locked ``idx`` is read by an asynchronous DMA: it must
         stay untouched until the step after the next one has been enqueued.  Returns ``(waitable, loss buffer, seq)``."""
         t = self._as_indices(idx)
-        r = getattr(self, "_runner", None)
-        if r is None and self.use_graph and self._opt_args is not None and os.environ.get("DMNIST_NATIVE_RUNNER", "1") != "0" \
-                and all(g is not None and g[1] for g in self._graphs):
-            r = self._make_runner()
+        r = self._runner
         if r is None:
-            self.load_indices(t)
-            self.train_step()
-            return self.read_result_async()
+            r = self._make_runner()
+            if r is None:
+                self.load_indices(t)
+                self.train_step()
+                return self.read_result_async()
         if not t.is_pinned():
             t = t.pin_memory()
         s = int(self.lib.dm_runner_step_indices(r, ctypes.c_void_p(t.data_ptr())))
@@ -278,14 +245,13 @@ class CudaLeNetEngine(ComputeEngine):
         """One whole training step from a packed batch (see :meth:`pack_batch`; pinned host or device memory): input DMA,
         event chaining and the graph launch happen in ONE native call once both slot graphs exist (``DMNIST_NATIVE_RUNNER=0``
         keeps the torch-dispatched path).  Returns ``(waitable, loss buffer, seq)`` like :meth:`read_result_async`."""
-        r = getattr(self, "_runner", None)
-        if r is None and self.use_graph and self._opt_args is not None and os.environ.get("DMNIST_NATIVE_RUNNER", "1") != "0" \
-                and all(g is not None and g[1] for g in self._graphs):
-            r = self._make_runner()
+        r = self._runner
         if r is None:
-            self.load_packed(packed)
-            self.train_step()
-            return self.read_result_async()
+            r = self._make_runner()
+            if r is None:
+                self.load_packed(packed)
+                self.train_step()
+                return self.read_result_async()
         s = int(self.lib.dm_runner_step(r, ctypes.c_void_p(packed.data_ptr())))
         if s < 0:
             raise RuntimeError("dm_runner_step failed: CUDA error %d" % -s)
@@ -296,6 +262,11 @@ class CudaLeNetEngine(ComputeEngine):
         return _RunnerEvent(self.lib, r, s), self.h_loss_bufs[s], self._seq0 + self._steps_launched
 
     def _make_runner(self):
+        """The native runner, once both slot graphs exist (with an optimizer attached, unless ``DMNIST_NATIVE_RUNNER=0``);
+        None until then: the caller takes the torch-dispatched path."""
+        if not (self.use_graph and self._opt_args is not None and os.environ.get("DMNIST_NATIVE_RUNNER", "1") != "0"
+                and all(g is not None and g[1] for g in self._graphs)):
+            return None
         torch.cuda.synchronize()                         # hand-over point: nothing of the torch-dispatched path is in flight
         lib = self.lib
         lib.dm_runner_create.restype = ctypes.c_void_p
@@ -350,15 +321,14 @@ class CudaLeNetEngine(ComputeEngine):
         #     pass; the small bucket is pushed into every replica's inbox.  Also used on ONE replica (no exchange, the fc1
         #     update still leaves the critical path).   =1: round-1 fp32 two-shot / one-shot kernels.   =0: single kernel.
         mode = os.environ.get("DMNIST_BUCKET", "2")
-        can = (hasattr(self, "_bucket_split") and int(k) == n and self._branches and self.backend.drop_keep <= 0.0
-               and getattr(opt, "mode", "") != "interval")
+        can = int(k) == n and self.backend.drop_keep <= 0.0 and getattr(opt, "mode", "") != "interval"
         self._bucket_v2 = can and mode == "2" and n in (1, 2, 4, 8)
         self._bucketed = can and ((mode == "1" and n in (2, 4, 8)) or self._bucket_v2)
         if self._bucket_v2 and self._g16 is None:
             e0, e1 = self._bucket_early
             assert e0 % 8 == 0 and (e1 - e0) % 8 == 0, "fc1 weights must start on a 32-byte boundary of the arena"
             self._g16 = self.backend.allocate_buffer((e1 - e0) * 2)
-            self._g16_view = self._g16.view(torch.bfloat16, 0, e1 - e0).view(*getattr(self, "_g16_shape", (3136, 512)))
+            self._g16_view = self._g16.view(torch.bfloat16, 0, e1 - e0).view(*self._g16_shape)
             n_late = self.spec.arena_numel - (e1 - e0)
             self._inbox = self.backend.allocate_buffer(2 * n * n_late * 8) if n > 1 else None   # LL lines: 8 bytes per float
         # early-bucket grid: the CTAs share SMs with the tensor-core kernels of the backward pass and every one of them fences
@@ -374,25 +344,195 @@ class CudaLeNetEngine(ComputeEngine):
         """Parameters were written from the host (init / restore): refresh the bf16 shadow."""
         self.backend.refresh_shadow(self.params)
 
+    # ---- step ---------------------------------------------------------------------------------------------------------
+    def _launch_step(self, slot: int, with_sync: bool) -> None:
+        raise NotImplementedError
+
+    def _enqueue_iteration_begin(self) -> None:
+        """Interval mode / K > N: adopt pushed weights (+ shadow refresh) at the start of an iteration."""
+        if self._kgtn_k:
+            self.backend.enqueue_kgtn_begin(self.params)
+        else:
+            self.backend.enqueue_interval_begin(self.params)
+
+    def _enqueue_iteration_end(self) -> None:
+        """Interval mode / K > N: gate, accumulate, close (+ commit attempt), apply."""
+        oa = self._opt_args
+        if self._kgtn_k:
+            self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"], oa["decay_rate"],
+                                          oa["decay_steps"])
+        else:
+            self.backend.enqueue_interval_end(self.params, self.grads, self._acc, oa["lr0"], oa["decay_rate"], oa["decay_steps"])
+
+    def _run(self, with_sync: bool) -> None:
+        s = self._slot
+        cur = torch.cuda.current_stream()
+        cur.wait_event(self._copy_done[s])
+        if self.use_graph:
+            key = s
+            if self._graphs[key] is None or self._graphs[key][1] != with_sync:
+                self._launch_step(s, False)           # warm-up (gradients only): sets func attributes outside capture
+                torch.cuda.synchronize()
+                gr = torch.cuda.CUDAGraph()
+                # thread_local: other threads (NCCL watchdog, pin-memory) may call CUDA while we capture
+                cap = torch.cuda.Stream(device=self.device, priority=self._main_priority)
+                with torch.cuda.graph(gr, stream=cap, capture_error_mode="thread_local"):
+                    self._launch_step(s, with_sync)
+                self._graphs[key] = (gr, with_sync)
+            self._graphs[key][0].replay()
+        else:
+            self._launch_step(s, with_sync)
+        if with_sync:
+            self._steps_launched = getattr(self, "_steps_launched", 0) + 1
+        self._slot_free[s].record(cur)
+
+    # ---- public step API ----------------------------------------------------------------------------------
+    def forward_backward(self, step: int) -> None:
+        """Gradients only (the aggregation is launched separately by the optimizer)."""
+        self._run(with_sync=False)
+
+    def train_step(self) -> None:
+        """Whole step incl. the fused allreduce+SGD kernel, as one CUDA graph replay."""
+        assert self._opt_args is not None, "attach_optimizer() first"
+        self._run(with_sync=True)
+
+    def read_loss_async(self):
+        """``(event, buffer)`` of the step enqueued last: the step copies (loss, accuracy) into a pinned host buffer
+        (two alternate, one per input slot) as its final node; wait on the event, then read ``buffer[0]`` / ``buffer[1]``."""
+        s = self._slot                      # the step just enqueued copied its result into this slot's buffer itself
+        return self._slot_free[s], self.h_loss_bufs[s]
+
+    def read_result_async(self):
+        """``(event, loss buffer, seq)`` of the step enqueued last: wait on the event, then ``loss[0]``/``loss[1]`` are (loss,
+        accuracy) and ``backend.mirror_info(seq)`` is the step's StepInfo -- both were written into page-locked host memory
+        by the step's own kernels, so the host never issues a device read."""
+        s = self._slot
+        return self._slot_free[s], self.h_loss_bufs[s], self._seq0 + self._steps_launched
+
+    def loss_acc(self) -> Tuple[float, float]:
+        ev, buf = self.read_loss_async()
+        ev.synchronize()
+        return float(buf[0]), float(buf[1])
+
+    def step_info(self) -> StepInfo:
+        return self.backend.last_step_info(check=True)     # one packed device->host read
+
+    # ---- inference ------------------------------------------------------------------------------------------
+    def _eval_forward(self, images: torch.Tensor, labels: torch.Tensor, B: int) -> None:
+        """Inference forward of one batch: (mean loss, accuracy) of its B rows into ``d_loss_acc``."""
+        raise NotImplementedError
+
+    @torch.no_grad()
+    def evaluate(self, images, labels) -> Tuple[float, float]:
+        if isinstance(images, np.ndarray):
+            images, labels = torch.from_numpy(np.ascontiguousarray(images)), torch.from_numpy(np.ascontiguousarray(labels))
+        images = images.reshape(-1, *self.images[0].shape[1:]).to(self.device, torch.float32)
+        labels = labels.to(self.device, torch.int64)
+        n, B = images.shape[0], self.batch_size
+        tot_loss = tot_hit = 0.0
+        for s in range(0, n, B):
+            m = min(B, n - s)
+            self._eval_forward(images[s:s + m].contiguous(), labels[s:s + m].contiguous(), m)
+            la = self.d_loss_acc.cpu()
+            tot_loss += float(la[0]) * m      # kernel scales by 1/m
+            tot_hit += float(la[1]) * m
+        return tot_loss / n, tot_hit / n
+
+
+class CudaLeNetEngine(_CudaEngine):
+    _main_priority = -1           # see _side
+
+    def __init__(self, batch_size: int, backend: FusedBackend, seed: int = 66478, rank: int = 0,
+                 keep_prob: float = 0.5, use_graph: bool = True):
+        super().__init__(get_model("lenet")[0], batch_size, backend, seed, use_graph, (28, 28))
+        B, dev = batch_size, self.device
+        self.seed, self.rank, self.keep_prob = seed, rank, keep_prob
+        bf, u8, f32 = torch.bfloat16, torch.uint8, torch.float32
+        self.a1 = torch.zeros(B, 14, 14, 32, dtype=bf, device=dev)
+        self.code1 = torch.zeros(B, 14, 14, 32, dtype=u8, device=dev)
+        self.a2 = torch.zeros(B, 3136, dtype=bf, device=dev)
+        self.code2 = torch.zeros(B, 3136, dtype=u8, device=dev)
+        self.fc1_splits = 7                                         # 49 k-blocks of 64 -> 7 per CTA
+        self.h_part = torch.zeros(self.fc1_splits, B, 512, dtype=f32, device=dev)   # fc1 split-K partial sums
+        self.dh = torch.zeros(B, 512, dtype=bf, device=dev)
+        self.h_act = torch.zeros(B, 512, dtype=f32, device=dev)      # post ReLU/dropout fc1 activations (fc2_wgrad operand)
+        self.dlogits = torch.zeros(B, 12, dtype=f32, device=dev)     # d loss / d logits, 48-byte rows
+        self.dy2 = torch.zeros(B, 14, 14, 64, dtype=bf, device=dev)
+        self.dx1 = torch.zeros(B, 14, 14, 32, dtype=bf, device=dev)
+        # the data-gradient chain is the critical path: it is captured on a high-priority stream (_main_priority), the
+        # weight-gradient side branches on low-priority ones, so the block scheduler serves the chain first whenever both
+        # have CTAs pending
+        self._side = [torch.cuda.Stream(device=dev, priority=0) for _ in range(4)]
+        p_fc1 = self.spec.param("fc1_weights")
+        self._zero_ranges = [(0, p_fc1.offset), (p_fc1.offset + p_fc1.numel, self.spec.arena_numel)]
+        self._seed_mix0 = dropout_seed_mix(seed, 0, rank)
+        # early bucket = fc1_weights (96.5 % of the bytes, final as soon as fc1_wgrad is done); everything else is late
+        self._bucket_early = (p_fc1.offset, p_fc1.offset + p_fc1.numel)
+        self._g16_shape = (3136, 512)
+        self._epoch_ptr = ctypes.c_void_p(backend.ctrl.local_ptr + backend._off["epoch"])
+
+    # ---- kernels of the step, one launch each (the graph builder and time_kernels share them) ---------------------------
+    # ``sp``: the stream to launch on (stream_ptr() of the caller's current stream, taken once per stream)
+    def _conv1_fwd(self, images: torch.Tensor, B: int, train: bool, sp) -> None:
+        p = self.p
+        check(self.lib.dm_conv1_fwd_tc(ptr(images), ptr(p["conv1_weights"]), ptr(p["conv1_biases"]), ptr(self.a1),
+                                       ptr(self.code1), B, *self._zero_args(train), sp), "conv1_fwd")
+
+    def _conv2_fwd(self, B: int, sp) -> None:
+        check(self.lib.dm_conv2_fwd(ptr(self.a1), ptr(self.pb["conv2_weights"]), ptr(self.p["conv2_biases"]), ptr(self.a2),
+                                    ptr(self.code2), B, sp), "conv2_fwd")
+
+    def _fc1_fwd(self, B: int) -> None:
+        # a2[B,3136] (K-major) * W1[3136,512] (MN-major), split-K: 7 partial tiles stored side by side
+        # (no atomics, nothing to zero); fc2_fwd_bwd sums them while applying bias + ReLU + dropout
+        G.gemm_bf16_raw(self.a2, self.pb["fc1_weights"], self.h_part, B, 512, 3136, 3136, 512, 512, False, True,
+                        G.EPI_STORE_F32, splits=self.fc1_splits, bn=64, split_stride=self.h_part.stride(0))
+
+    def _fc2_fwd_bwd(self, labels: torch.Tensor, B: int, train: bool, sp, logits_out: Optional[torch.Tensor] = None) -> None:
+        p = self.p
+        check(self.lib.dm_fc2_fwd_bwd(ptr(self.h_part), ctypes.c_longlong(self.h_part.stride(0)), self.fc1_splits,
+                                      ptr(p["fc1_biases"]), ptr(p["fc2_weights"]), ptr(p["fc2_biases"]), ptr(labels),
+                                      ptr(self.dh), ptr(self.h_act), ptr(self.dlogits), ptr(self.d_loss_acc), ptr(logits_out),
+                                      B, int(train), ctypes.c_uint(self._seed_mix0),
+                                      self._epoch_ptr if train else ctypes.c_void_p(0), ctypes.c_float(self.keep_prob),
+                                      sp), "fc2_fwd_bwd")
+
+    def _fc1_wgrad(self, dst: torch.Tensor, B: int) -> None:
+        # dW1[3136,512] = a2^T (A MN-major) * dh (B MN-major), K = batch: fp32 into the gradient arena, or bf16 (half the
+        # epilogue stores, half the NVLink bytes) into the bucketed aggregation's symmetric wire buffer
+        G.gemm_bf16_raw(self.a2, self.dh, dst, 3136, 512, B, 3136, 512, 512, True, True,
+                        G.EPI_STORE_BF16 if dst.dtype == torch.bfloat16 else G.EPI_STORE_F32, bn=128)
+
+    def _fc2_wgrad(self, B: int, sp) -> None:
+        g = self.g
+        check(self.lib.dm_fc2_wgrad(ptr(self.h_act), ptr(self.dlogits), ptr(self.dh), ptr(g["fc2_weights"]),
+                                    ptr(g["fc2_biases"]), ptr(g["fc1_biases"]), B, sp), "fc2_wgrad")
+
+    def _fc1_dgrad(self, B: int, sp) -> None:
+        # d(pool2 out)[B,3136] = dh[B,512] (K-major) * W1[3136,512] (rows = in, K = out contiguous), with maxpool2/ReLU2
+        # backward and the conv2 bias gradient in the GEMM epilogue (no [B,3136] intermediate)
+        check(self.lib.dm_fc1_dgrad_unpool(ptr(self.dh), ptr(self.pb["fc1_weights"]), ptr(self.code2), ptr(self.dy2),
+                                           ptr(self.g["conv2_biases"]), B, sp), "fc1_dgrad_unpool")
+
+    def _conv2_wgrad(self, B: int, sp) -> None:
+        check(self.lib.dm_conv2_wgrad(ptr(self.a1), ptr(self.dy2), ptr(self.g["conv2_weights"]), B, sp), "conv2_wgrad")
+
+    def _conv2_dgrad(self, B: int, sp) -> None:
+        check(self.lib.dm_conv2_dgrad(ptr(self.dy2), ptr(self.pb["conv2_weights"]), ptr(self.dx1), B, sp), "conv2_dgrad")
+
+    def _conv1_wgrad(self, images: torch.Tensor, B: int, sp) -> None:
+        g = self.g
+        check(self.lib.dm_conv1_wgrad_tc(ptr(images), ptr(self.dx1), ptr(self.code1), ptr(g["conv1_weights"]),
+                                         ptr(g["conv1_biases"]), B, sp), "conv1_wgrad")
+
     # ---- kernel sequence ------------------------------------------------------------------------------
     def _launch_forward(self, images: torch.Tensor, labels: torch.Tensor, B: int, train: bool,
                         logits_out: Optional[torch.Tensor] = None) -> int:
-        lib, sp, p, pb = self.lib, stream_ptr(), self.p, self.pb
-        conv1_fwd = lib.dm_conv1_fwd_tc if self._conv1_tc else lib.dm_conv1_fwd
-        check(conv1_fwd(ptr(images), ptr(p["conv1_weights"]), ptr(p["conv1_biases"]), ptr(self.a1),
-                        ptr(self.code1), B, *self._zero_args(train), sp), "conv1_fwd")
-        check(lib.dm_conv2_fwd(ptr(self.a1), ptr(pb["conv2_weights"]), ptr(p["conv2_biases"]), ptr(self.a2),
-                               ptr(self.code2), B, sp), "conv2_fwd")
-        # fc1: a2[B,3136] (K-major) * W1[3136,512] (MN-major), split-K: 7 partial tiles stored side by side
-        # (no atomics, nothing to zero); fc2_fwd_bwd sums them while applying bias + ReLU + dropout
-        stride = self.h_part.stride(0)
-        G.gemm_bf16_raw(self.a2, pb["fc1_weights"], self.h_part, B, 512, 3136, 3136, 512, 512, False, True,
-                        G.EPI_STORE_F32, splits=self.fc1_splits, bn=64, split_stride=stride)
-        check(lib.dm_fc2_fwd_bwd(ptr(self.h_part), ctypes.c_longlong(stride), self.fc1_splits, ptr(p["fc1_biases"]),
-                                 ptr(p["fc2_weights"]), ptr(p["fc2_biases"]), ptr(labels), ptr(self.dh), ptr(self.h_act),
-                                 ptr(self.dlogits), ptr(self.d_loss_acc), ptr(logits_out), B, int(train),
-                                 ctypes.c_uint(self._seed_mix0), self._epoch_ptr if train else ctypes.c_void_p(0),
-                                 ctypes.c_float(self.keep_prob), sp), "fc2_fwd_bwd")
+        sp = stream_ptr()
+        self._conv1_fwd(images, B, train, sp)
+        self._conv2_fwd(B, sp)
+        self._fc1_fwd(B)
+        self._fc2_fwd_bwd(labels, B, train, sp, logits_out)
         return 4
 
     def _launch_backward(self, images: torch.Tensor, B: int, early_sync: bool = False) -> int:
@@ -400,51 +540,29 @@ class CudaLeNetEngine(ComputeEngine):
         on low-priority side streams (captured as parallel graph branches) next to the data-gradient chain
         fc1_dgrad(+unpool) -> conv2_dgrad -> conv1_wgrad.  ``early_sync``: bucketed aggregation -- the early-bucket
         kernel joins the fc1_wgrad branch and the small fc gradients get a branch of their own."""
-        lib, g, pb = self.lib, self.g, self.pb
         main = torch.cuda.current_stream()
-        branch = self._branches
-        if branch:
-            fork1 = torch.cuda.Event()
-            fork1.record(main)
-            self._side[0].wait_event(fork1)
-            # (loss, accuracy) are final after fc2_fwd_bwd: their copy into the slot's page-locked host buffer is a branch of
-            # the step (a memcpy node of the graph) that runs under the backward pass -- reading the result costs the host
-            # no extra call, only a wait on the step's completion event
-            # (its own branch, joined only at the very end of the step: a memcpy node in front of the aggregation kernel
-            # would cost that kernel its programmatic launch edge)
-            self._side[3].wait_event(fork1)
-            with torch.cuda.stream(self._side[3]):
-                self.h_loss_bufs[self._slot].copy_(self.d_loss_acc, non_blocking=True)
-                self._join_loss = torch.cuda.Event()
-                self._join_loss.record(self._side[3])
-        else:
+        fork1 = torch.cuda.Event()
+        fork1.record(main)
+        self._side[0].wait_event(fork1)
+        # (loss, accuracy) are final after fc2_fwd_bwd: their copy into the slot's page-locked host buffer is a branch of
+        # the step (a memcpy node of the graph) that runs under the backward pass -- reading the result costs the host
+        # no extra call, only a wait on the step's completion event
+        # (its own branch, joined only at the very end of the step: a memcpy node in front of the aggregation kernel
+        # would cost that kernel its programmatic launch edge)
+        self._side[3].wait_event(fork1)
+        with torch.cuda.stream(self._side[3]):
             self.h_loss_bufs[self._slot].copy_(self.d_loss_acc, non_blocking=True)
+            self._join_loss = torch.cuda.Event()
+            self._join_loss.record(self._side[3])
         sp = stream_ptr()
-        # fc1 dgrad: dxfc[B,3136] = dh[B,512] (K-major) * W1[3136,512] (rows = in, K = out contiguous)
-        if self._fuse_unpool:
-            # ... with maxpool2/ReLU2 backward and the conv2 bias gradient in the GEMM epilogue (no [B,3136] intermediate)
-            check(lib.dm_fc1_dgrad_unpool(ptr(self.dh), ptr(pb["fc1_weights"]), ptr(self.code2), ptr(self.dy2),
-                                          ptr(g["conv2_biases"]), B, sp), "fc1_dgrad_unpool")
-        else:
-            G.gemm_bf16_raw(self.dh, pb["fc1_weights"], self.dxfc, B, 3136, 512, 512, 512, 3136, False, False,
-                            G.EPI_STORE_BF16, bn=64)
-            check(lib.dm_unpool2(ptr(self.dxfc), ptr(self.code2), ptr(self.dy2), ptr(g["conv2_biases"]), B, sp), "unpool2")
+        self._fc1_dgrad(B, sp)
         # (the side branch is issued AFTER the chain's kernel: both become ready together and the first one dispatched takes
         #  the SMs -- the data-gradient GEMM must be that one)
-        with torch.cuda.stream(self._side[0] if branch else main):
-            # fc1 wgrad: dW1[3136,512] = a2^T (A MN-major) * dh (B MN-major), K = batch; straight into the arena
-            if early_sync and self._bucket_v2:
-                # ... as bf16 into the symmetric wire buffer: half the epilogue stores, half the NVLink bytes
-                G.gemm_bf16_raw(self.a2, self.dh, self._g16_view, 3136, 512, B, 3136, 512, 512, True, True,
-                                G.EPI_STORE_BF16, bn=128)
-            else:
-                G.gemm_bf16_raw(self.a2, self.dh, g["fc1_weights"], 3136, 512, B, 3136, 512, 512, True, True,
-                                G.EPI_STORE_F32, bn=128)
+        with torch.cuda.stream(self._side[0]):
+            self._fc1_wgrad(self._g16_view if early_sync and self._bucket_v2 else self.g["fc1_weights"], B)
             if not early_sync:
                 # fc2 weight/bias + fc1 bias gradients: only the aggregation kernel consumes them
-                check(lib.dm_fc2_wgrad(ptr(self.h_act), ptr(self.dlogits), ptr(self.dh), ptr(g["fc2_weights"]),
-                                       ptr(g["fc2_biases"]), ptr(g["fc1_biases"]), B, stream_ptr()), "fc2_wgrad")
-            if branch and not early_sync:
+                self._fc2_wgrad(B, stream_ptr())
                 join1 = torch.cuda.Event()
                 join1.record(self._side[0])
         if early_sync:
@@ -470,40 +588,30 @@ class CudaLeNetEngine(ComputeEngine):
             # the small fc gradients (fc2 weights/biases, fc1 biases) belong to the late bucket: their own branch
             self._side[2].wait_event(fork1)
             with torch.cuda.stream(self._side[2]):
-                check(lib.dm_fc2_wgrad(ptr(self.h_act), ptr(self.dlogits), ptr(self.dh), ptr(g["fc2_weights"]),
-                                       ptr(g["fc2_biases"]), ptr(g["fc1_biases"]), B, stream_ptr()), "fc2_wgrad")
+                self._fc2_wgrad(B, stream_ptr())
                 join3 = torch.cuda.Event()
                 join3.record(self._side[2])
-        late = branch and self._wgrad_late
-        if late:
-            # conv2 dgrad and wgrad each fill the machine (1 CTA/SM, ~200 KB smem): side by side they only slow the chain
-            # down.  wgrad is forked AFTER dgrad instead and shares the SMs with conv1_wgrad (LDS/FMA-bound, 37 KB/CTA).
-            check(lib.dm_conv2_dgrad(ptr(self.dy2), ptr(pb["conv2_weights"]), ptr(self.dx1), B, sp), "conv2_dgrad")
-        if branch:
-            fork2 = torch.cuda.Event()
-            fork2.record(main)
-            self._side[1].wait_event(fork2)
-        with torch.cuda.stream(self._side[1] if branch else main):
-            check(lib.dm_conv2_wgrad(ptr(self.a1), ptr(self.dy2), ptr(g["conv2_weights"]), B, stream_ptr()), "conv2_wgrad")
-            if branch:
-                join2 = torch.cuda.Event()
-                join2.record(self._side[1])
-        if not late:
-            check(lib.dm_conv2_dgrad(ptr(self.dy2), ptr(pb["conv2_weights"]), ptr(self.dx1), B, sp), "conv2_dgrad")
-        conv1_wgrad = lib.dm_conv1_wgrad_tc if self._conv1_tc else lib.dm_conv1_wgrad
-        check(conv1_wgrad(ptr(images), ptr(self.dx1), ptr(self.code1), ptr(g["conv1_weights"]),
-                          ptr(g["conv1_biases"]), B, sp), "conv1_wgrad")
-        if branch:
-            main.wait_event(join2)
-            if self._stamp and early_sync:
-                # every backward kernel of THIS replica is done (conv1_wgrad on the chain, conv2_wgrad joined): stamp it before
-                # waiting for the exchange branch, which contains the all-to-all with the other replicas
-                main.wait_event(join3)
-                self.backend.enqueue_stamp_arrive()
-            main.wait_event(join1)
-            if early_sync:
-                main.wait_event(join3)
-        return 7 if self._fuse_unpool else 8     # (conv2_wgrad is two launches: the kernel and its reduction)
+        # conv2 dgrad and wgrad each fill the machine (1 CTA/SM, ~200 KB smem): side by side they only slow the chain
+        # down.  wgrad is forked AFTER dgrad instead and shares the SMs with conv1_wgrad.
+        self._conv2_dgrad(B, sp)
+        fork2 = torch.cuda.Event()
+        fork2.record(main)
+        self._side[1].wait_event(fork2)
+        with torch.cuda.stream(self._side[1]):
+            self._conv2_wgrad(B, stream_ptr())
+            join2 = torch.cuda.Event()
+            join2.record(self._side[1])
+        self._conv1_wgrad(images, B, sp)
+        main.wait_event(join2)
+        if self._stamp and early_sync:
+            # every backward kernel of THIS replica is done (conv1_wgrad on the chain, conv2_wgrad joined): stamp it before
+            # waiting for the exchange branch, which contains the all-to-all with the other replicas
+            main.wait_event(join3)
+            self.backend.enqueue_stamp_arrive()
+        main.wait_event(join1)
+        if early_sync:
+            main.wait_event(join3)
+        return 7     # (conv2_wgrad is two launches: the kernel and its reduction)
 
     def _zero_args(self, train: bool):
         """Regions conv1_fwd clears at the start of a training step (atomically accumulated gradients + loss)."""
@@ -519,7 +627,8 @@ class CudaLeNetEngine(ComputeEngine):
 
     def time_kernels(self, iters: int = 20) -> dict:
         """Average device time of every kernel of the step, measured in place with CUDA events between
-        eager launches (caches warm, as in the replayed graph; includes the launch gap)."""
+        eager launches (caches warm, as in the replayed graph; includes the launch gap).  ``unpool2`` is part of
+        fc1_dgrad's epilogue and stays at 0."""
         names = ["memsets", "conv1_fwd", "conv2_fwd", "fc1_fwd", "fc2_fwd_bwd", "fc1_wgrad", "fc2_wgrad", "fc1_dgrad", "unpool2",
                  "conv2_wgrad", "conv2_dgrad", "conv1_wgrad"]
         # K > N: adopt + shadow refresh, and gate + accumulate + close + apply, in place of the fused sync kernel
@@ -527,49 +636,23 @@ class CudaLeNetEngine(ComputeEngine):
         tot = {n: 0.0 for n in names}
         B, s = self.batch_size, self._slot
         img, lbl = self.images[s], self.labels[s]
-        lib, sp, g, p, pb = self.lib, stream_ptr(), self.g, self.p, self.pb
+        sp = stream_ptr()
 
         def seq():
             if self._kgtn_k:
                 yield "kgtn_begin", lambda: self.backend.enqueue_kgtn_begin(self.params)
             yield "memsets", lambda: self._launch_zero()
-            fw = []
             # forward / backward are issued kernel by kernel so an event can sit between any two
-            yield "conv1_fwd", lambda: check((lib.dm_conv1_fwd_tc if self._conv1_tc else lib.dm_conv1_fwd)(ptr(img), ptr(p["conv1_weights"]), ptr(p["conv1_biases"]),
-                                                              ptr(self.a1), ptr(self.code1), B, *self._zero_args(True), sp),
-                                             "conv1_fwd")
-            yield "conv2_fwd", lambda: check(lib.dm_conv2_fwd(ptr(self.a1), ptr(pb["conv2_weights"]), ptr(p["conv2_biases"]),
-                                                              ptr(self.a2), ptr(self.code2), B, sp), "conv2_fwd")
-            stride = self.h_part.stride(0)
-            yield "fc1_fwd", lambda: G.gemm_bf16_raw(self.a2, pb["fc1_weights"], self.h_part, B, 512, 3136, 3136, 512, 512,
-                                                     False, True, G.EPI_STORE_F32, splits=self.fc1_splits, bn=64,
-                                                     split_stride=stride)
-            yield "fc2_fwd_bwd", lambda: check(lib.dm_fc2_fwd_bwd(
-                ptr(self.h_part), ctypes.c_longlong(stride), self.fc1_splits, ptr(p["fc1_biases"]), ptr(p["fc2_weights"]),
-                ptr(p["fc2_biases"]), ptr(lbl), ptr(self.dh), ptr(self.h_act), ptr(self.dlogits), ptr(self.d_loss_acc),
-                ctypes.c_void_p(0), B, 1, ctypes.c_uint(self._seed_mix0), self._epoch_ptr, ctypes.c_float(self.keep_prob), sp),
-                "fc2_fwd_bwd")
-            yield "fc1_wgrad", lambda: G.gemm_bf16_raw(self.a2, self.dh, g["fc1_weights"], 3136, 512, B, 3136, 512, 512,
-                                                       True, True, G.EPI_STORE_F32, bn=128)
-            yield "fc2_wgrad", lambda: check(lib.dm_fc2_wgrad(ptr(self.h_act), ptr(self.dlogits), ptr(self.dh),
-                                                              ptr(g["fc2_weights"]), ptr(g["fc2_biases"]),
-                                                              ptr(g["fc1_biases"]), B, sp), "fc2_wgrad")
-            if self._fuse_unpool:
-                yield "fc1_dgrad", lambda: check(lib.dm_fc1_dgrad_unpool(ptr(self.dh), ptr(pb["fc1_weights"]), ptr(self.code2),
-                                                                         ptr(self.dy2), ptr(g["conv2_biases"]), B, sp),
-                                                 "fc1_dgrad_unpool")
-            else:
-                yield "fc1_dgrad", lambda: G.gemm_bf16_raw(self.dh, pb["fc1_weights"], self.dxfc, B, 3136, 512, 512, 512, 3136,
-                                                           False, False, G.EPI_STORE_BF16, bn=64)
-                yield "unpool2", lambda: check(lib.dm_unpool2(ptr(self.dxfc), ptr(self.code2), ptr(self.dy2),
-                                                              ptr(g["conv2_biases"]), B, sp), "unpool2")
-            yield "conv2_wgrad", lambda: check(lib.dm_conv2_wgrad(ptr(self.a1), ptr(self.dy2), ptr(g["conv2_weights"]), B, sp),
-                                               "conv2_wgrad")
-            yield "conv2_dgrad", lambda: check(lib.dm_conv2_dgrad(ptr(self.dy2), ptr(pb["conv2_weights"]), ptr(self.dx1), B, sp),
-                                               "conv2_dgrad")
-            yield "conv1_wgrad", lambda: check((lib.dm_conv1_wgrad_tc if self._conv1_tc else lib.dm_conv1_wgrad)(ptr(img), ptr(self.dx1), ptr(self.code1),
-                                                                  ptr(g["conv1_weights"]), ptr(g["conv1_biases"]), B, sp),
-                                               "conv1_wgrad")
+            yield "conv1_fwd", lambda: self._conv1_fwd(img, B, True, sp)
+            yield "conv2_fwd", lambda: self._conv2_fwd(B, sp)
+            yield "fc1_fwd", lambda: self._fc1_fwd(B)
+            yield "fc2_fwd_bwd", lambda: self._fc2_fwd_bwd(lbl, B, True, sp)
+            yield "fc1_wgrad", lambda: self._fc1_wgrad(self.g["fc1_weights"], B)
+            yield "fc2_wgrad", lambda: self._fc2_wgrad(B, sp)
+            yield "fc1_dgrad", lambda: self._fc1_dgrad(B, sp)
+            yield "conv2_wgrad", lambda: self._conv2_wgrad(B, sp)
+            yield "conv2_dgrad", lambda: self._conv2_dgrad(B, sp)
+            yield "conv1_wgrad", lambda: self._conv1_wgrad(img, B, sp)
             if self._kgtn_k:
                 oa = self._opt_args
                 yield "kgtn_end", lambda: self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"],
@@ -634,96 +717,12 @@ class CudaLeNetEngine(ComputeEngine):
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1
-        if self._branches:
-            torch.cuda.current_stream().wait_event(self._join_loss)      # the loss read-back branch rejoins at the end of the step
+        torch.cuda.current_stream().wait_event(self._join_loss)      # the loss read-back branch rejoins at the end of the step
         self.launches_per_step = n
 
-    def _enqueue_iteration_begin(self) -> None:
-        """Interval mode / K > N: adopt pushed weights (+ shadow refresh) at the start of an iteration."""
-        if self._kgtn_k:
-            self.backend.enqueue_kgtn_begin(self.params)
-        else:
-            self.backend.enqueue_interval_begin(self.params)
-
-    def _enqueue_iteration_end(self) -> None:
-        """Interval mode / K > N: gate, accumulate, close (+ commit attempt), apply."""
-        oa = self._opt_args
-        if self._kgtn_k:
-            self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"], oa["decay_rate"],
-                                          oa["decay_steps"])
-        else:
-            self.backend.enqueue_interval_end(self.params, self.grads, self._acc, oa["lr0"], oa["decay_rate"], oa["decay_steps"])
-
-    def _run(self, with_sync: bool) -> None:
-        s = self._slot
-        cur = torch.cuda.current_stream()
-        cur.wait_event(self._copy_done[s])
-        if self.use_graph:
-            key = s
-            if self._graphs[key] is None or self._graphs[key][1] != with_sync:
-                self._launch_step(s, False)           # warm-up (gradients only): sets func attributes outside capture
-                torch.cuda.synchronize()
-                gr = torch.cuda.CUDAGraph()
-                # thread_local: other threads (NCCL watchdog, pin-memory) may call CUDA while we capture
-                cap = torch.cuda.Stream(device=self.device, priority=getattr(self, "_main_priority", 0))
-                with torch.cuda.graph(gr, stream=cap, capture_error_mode="thread_local"):
-                    self._launch_step(s, with_sync)
-                self._graphs[key] = (gr, with_sync)
-            self._graphs[key][0].replay()
-        else:
-            self._launch_step(s, with_sync)
-        if with_sync:
-            self._steps_launched = getattr(self, "_steps_launched", 0) + 1
-        self._slot_free[s].record(cur)
-
-    # ---- public step API ----------------------------------------------------------------------------------
-    def forward_backward(self, step: int) -> None:
-        """Gradients only (the aggregation is launched separately by the optimizer)."""
-        self._run(with_sync=False)
-
-    def train_step(self) -> None:
-        """Whole step incl. the fused allreduce+SGD kernel, as one CUDA graph replay."""
-        assert self._opt_args is not None, "attach_optimizer() first"
-        self._run(with_sync=True)
-
-    def read_loss_async(self):
-        """``(event, buffer)`` of the step enqueued last: the step copies (loss, accuracy) into a pinned host buffer
-        (two alternate, one per input slot) as its final node; wait on the event, then read ``buffer[0]`` / ``buffer[1]``."""
-        s = self._slot                      # the step just enqueued copied its result into this slot's buffer itself
-        self.h_loss_acc = self.h_loss_bufs[s]
-        return self._slot_free[s], self.h_loss_bufs[s]
-
-    def read_result_async(self):
-        """``(event, loss buffer, seq)`` of the step enqueued last: wait on the event, then ``loss[0]``/``loss[1]`` are (loss,
-        accuracy) and ``backend.mirror_info(seq)`` is the step's StepInfo -- both were written into page-locked host memory
-        by the step's own kernels, so the host never issues a device read."""
-        s = self._slot
-        return self._slot_free[s], self.h_loss_bufs[s], self._seq0 + self._steps_launched
-
-    def loss_acc(self) -> Tuple[float, float]:
-        ev, buf = self.read_loss_async()
-        ev.synchronize()
-        return float(buf[0]), float(buf[1])
-
-    def step_info(self) -> StepInfo:
-        return self.backend.last_step_info(check=True)     # one packed device->host read
-
     # ---- inference ------------------------------------------------------------------------------------------
-    @torch.no_grad()
-    def evaluate(self, images, labels) -> Tuple[float, float]:
-        if isinstance(images, np.ndarray):
-            images, labels = torch.from_numpy(np.ascontiguousarray(images)), torch.from_numpy(np.ascontiguousarray(labels))
-        images = images.reshape(-1, 28, 28).to(self.device, torch.float32)
-        labels = labels.to(self.device, torch.int64)
-        n, B = images.shape[0], self.batch_size
-        tot_loss = tot_hit = 0.0
-        for s in range(0, n, B):
-            m = min(B, n - s)
-            self._launch_forward(images[s:s + m].contiguous(), labels[s:s + m].contiguous(), m, False)
-            la = self.d_loss_acc.cpu()
-            tot_loss += float(la[0]) * m      # kernel scales by 1/m
-            tot_hit += float(la[1]) * m
-        return tot_loss / n, tot_hit / n
+    def _eval_forward(self, images: torch.Tensor, labels: torch.Tensor, B: int) -> None:
+        self._launch_forward(images, labels, B, False)          # conv1_fwd clears the loss accumulator
 
     def forward_logits(self, images: torch.Tensor, labels: torch.Tensor, train: bool) -> torch.Tensor:
         """Debug/test helper: logits of one batch through the CUDA forward."""
@@ -833,7 +832,6 @@ class CudaLeNetEngine(ComputeEngine):
         lib, sp = self.lib, stream_ptr()
         n, C = self._ev_x.shape[0], self._ev_a1.shape[0]
         stride = self._ev_hpart.stride(0)
-        conv1_fwd = lib.dm_conv1_fwd_tc if self._conv1_tc else lib.dm_conv1_fwd
         null = ctypes.c_void_p(0)
         ring = ptr(self._ev_ring) if publish else null
         if self._snapshot and p is self._ev_views[0]:
@@ -844,8 +842,8 @@ class CudaLeNetEngine(ComputeEngine):
         check(lib.dm_eval_stamp(ptr(self._ev_state), sp), "eval_stamp")
         for s in range(0, n, C):
             m = min(C, n - s)
-            check(conv1_fwd(ptr(self._ev_x[s:s + m]), ptr(p["conv1_weights"]), ptr(p["conv1_biases"]), ptr(self._ev_a1),
-                            ptr(self._ev_code1), m, null, 0, null, 0, null, 0, sp), "conv1_fwd")
+            check(lib.dm_conv1_fwd_tc(ptr(self._ev_x[s:s + m]), ptr(p["conv1_weights"]), ptr(p["conv1_biases"]),
+                                      ptr(self._ev_a1), ptr(self._ev_code1), m, null, 0, null, 0, null, 0, sp), "conv1_fwd")
             check(lib.dm_conv2_fwd(ptr(self._ev_a1), ptr(pb["conv2_weights"]), ptr(p["conv2_biases"]), ptr(self._ev_a2),
                                    ptr(self._ev_code2), m, sp), "conv2_fwd")
             G.gemm_bf16_raw(self._ev_a2, pb["fc1_weights"], self._ev_hpart, m, 512, 3136, 3136, 512, 512, False, True,
@@ -941,7 +939,7 @@ class CudaLeNetEngine(ComputeEngine):
         return self.eval_record()
 
 
-class CudaMlpEngine(ComputeEngine):
+class CudaMlpEngine(_CudaEngine):
     """2-/3-layer MLP on the sm_90a kernels: hidden layers = wgmma GEMM with bias+ReLU fused in the
     epilogue, output layer + softmax-CE = SIMT (csrc/mlp_simt.cu), every weight gradient = wgmma GEMM
     with MN-major operands writing straight into the gradient arena."""
@@ -949,50 +947,22 @@ class CudaMlpEngine(ComputeEngine):
     def __init__(self, model: str, batch_size: int, backend: FusedBackend, hidden: int = 1024, seed: int = 66478,
                  rank: int = 0, use_graph: bool = True):
         assert hidden % 64 == 0, "--mlp_hidden must be a multiple of 64 on the GPU path"
-        self.lib, self.backend, self.device = load(), backend, backend.ctx.device
-        self.spec, _ = get_model(model, hidden)
-        self.model, self.batch_size, self.hidden = model, batch_size, hidden
+        super().__init__(get_model(model, hidden)[0], batch_size, backend, seed, use_graph, (784,))
+        self.model, self.hidden = model, hidden
         self.n_layers = len(self.spec.params) // 2
-        self.use_graph = use_graph
         # 128 x 256 GEMM tiles when the hidden width allows: half the L2->SM operand traffic per FLOP of 128 x 128
-        self._bn = 256 if (hidden % 256 == 0 and os.environ.get("DMNIST_GEMM_BN256", "1") != "0") else 128
+        self._bn = 256 if hidden % 256 == 0 else 128
         B, dev, bf = batch_size, self.device, torch.bfloat16
-        self.params = backend.allocate(self.spec.arena_numel)
-        self.params.copy_(self.spec.init_flat(seed).to(dev))
-        self.grads = backend.allocate(self.spec.arena_numel)
-        self.shadow = backend.attach_shadow(self.params)
-        self.p, self.g, self.pb = (self.spec.views(t) for t in (self.params, self.grads, self.shadow))
-        self._in_bytes = B * 784 * 4 + B * 8
-        self.in_dev = [torch.zeros(self._in_bytes, dtype=torch.uint8, device=dev) for _ in range(2)]
-        self.images = [t[:B * 784 * 4].view(torch.float32).view(B, 784) for t in self.in_dev]
-        self.labels = [t[B * 784 * 4:].view(torch.int64) for t in self.in_dev]
-        self.h_images = [torch.zeros(B, 784, dtype=torch.float32).pin_memory() for _ in range(2)]
-        self.h_labels = [torch.zeros(B, dtype=torch.int64).pin_memory() for _ in range(2)]
         self.x16 = torch.zeros(B, 784, dtype=bf, device=dev)
         self.h = [torch.zeros(B, hidden, dtype=bf, device=dev) for _ in range(self.n_layers - 1)]
         self.dh = [torch.zeros(B, hidden, dtype=bf, device=dev) for _ in range(self.n_layers - 1)]
         self.dl_pad = torch.zeros(B, 64, dtype=bf, device=dev)
-        self.d_loss_acc = torch.zeros(2, dtype=torch.float32, device=dev)
-        self.h_loss_bufs = [torch.zeros(2, dtype=torch.float32).pin_memory() for _ in range(2)]
-        self._loss_reads = 0
-        self._slot = self._loaded = 0
-        self.copy_stream = torch.cuda.Stream(device=dev)
-        self._copy_done = [torch.cuda.Event() for _ in range(2)]
-        self._slot_free = [torch.cuda.Event() for _ in range(2)]
-        self._graphs = [None, None]
-        self._opt_args: Optional[dict] = None
-        self._straggler = None
-        self.launches_per_step = 0
         # bucketed aggregation (csrc/fused_bucket.cu): the largest weight matrix is the early bucket (bf16 wire, exchanged next
         # to the remaining backward GEMMs), everything else the pushed late bucket
         big = max((q for q in self.spec.params if q.name.endswith("weights")), key=lambda q: q.numel)
         self._early_name = big.name
-        self._bucket_split = big.offset
         self._bucket_early = (big.offset, big.offset + big.numel)
         self._g16_shape = (784 if big.name == "fc1_weights" else hidden, hidden if big.name != "fc%d_weights" % self.n_layers else 10)
-        self._branches = True
-        self._bucketed = self._bucket_v2 = False
-        self._g16 = self._g16_view = self._inbox = None
         self._side = [torch.cuda.Stream(device=dev)]
         # everything except the weight matrices (written whole by GEMM stores) is accumulated with atomics
         stored = sorted((q.offset, q.offset + q.numel) for q in self.spec.params if q.name.endswith("weights"))
@@ -1003,36 +973,6 @@ class CudaMlpEngine(ComputeEngine):
             pos = a1
         if pos < self.spec.arena_numel:
             self._zero_ranges.append((pos, self.spec.arena_numel))
-
-    # shared plumbing with the convnet engine
-    load_batch = CudaLeNetEngine.load_batch
-    _leave_native_runner = CudaLeNetEngine._leave_native_runner
-    step_packed = CudaLeNetEngine.step_packed
-    _make_runner = CudaLeNetEngine._make_runner
-    pack_batch = CudaLeNetEngine.pack_batch
-    load_packed = CudaLeNetEngine.load_packed
-    arm_train_data = CudaLeNetEngine.arm_train_data
-    _as_indices = CudaLeNetEngine._as_indices
-    _gather = CudaLeNetEngine._gather
-    load_indices = CudaLeNetEngine.load_indices
-    step_indices = CudaLeNetEngine.step_indices
-    _table = None
-    attach_optimizer = CudaLeNetEngine.attach_optimizer
-    _enqueue_iteration_begin = CudaLeNetEngine._enqueue_iteration_begin
-    _enqueue_iteration_end = CudaLeNetEngine._enqueue_iteration_end
-    params_updated = CudaLeNetEngine.params_updated
-    _run = CudaLeNetEngine._run
-    forward_backward = CudaLeNetEngine.forward_backward
-    train_step = CudaLeNetEngine.train_step
-    read_loss_async = CudaLeNetEngine.read_loss_async
-    read_result_async = CudaLeNetEngine.read_result_async
-    loss_acc = CudaLeNetEngine.loss_acc
-    step_info = CudaLeNetEngine.step_info
-    _stamp = False
-    _kgtn_k = 0
-
-    def h2d_bytes_per_step(self) -> int:
-        return self.batch_size * (784 * 4 + 8)
 
     def _forward(self, images: torch.Tensor, labels: torch.Tensor, B: int, train: bool,
                  logits_out: Optional[torch.Tensor] = None) -> int:
@@ -1150,22 +1090,9 @@ class CudaMlpEngine(ComputeEngine):
         self.h_loss_bufs[slot].copy_(self.d_loss_acc, non_blocking=True)     # result read-back is part of the step
         self.launches_per_step = n
 
-    @torch.no_grad()
-    def evaluate(self, images, labels) -> Tuple[float, float]:
-        if isinstance(images, np.ndarray):
-            images, labels = torch.from_numpy(np.ascontiguousarray(images)), torch.from_numpy(np.ascontiguousarray(labels))
-        images = images.reshape(-1, 784).to(self.device, torch.float32)
-        labels = labels.to(self.device, torch.int64)
-        n, B = images.shape[0], self.batch_size
-        tot_loss = tot_hit = 0.0
-        for s in range(0, n, B):
-            m = min(B, n - s)
-            self.d_loss_acc.zero_()
-            self._forward(images[s:s + m].contiguous(), labels[s:s + m].contiguous(), m, False)
-            la = self.d_loss_acc.cpu()
-            tot_loss += float(la[0]) * m
-            tot_hit += float(la[1]) * m
-        return tot_loss / n, tot_hit / n
+    def _eval_forward(self, images: torch.Tensor, labels: torch.Tensor, B: int) -> None:
+        self.d_loss_acc.zero_()
+        self._forward(images, labels, B, False)
 
 
 def make_cuda_engine(flags, ctx, backend) -> ComputeEngine:

@@ -41,23 +41,24 @@ def _dev(*ts):
 # ---------------------------------------------------------------------------------------------------------------------
 # launchers: one kernel, fresh outputs
 # ---------------------------------------------------------------------------------------------------------------------
-def run_conv1_fwd(x, w, b, tc: bool = True):
+def run_conv1_fwd(x, w, b):
     """x [B,28,28] fp32, w [5,5,1,32] fp32, b [32] -> (pooled bf16 [B,14,14,32], code, the cleared junk range)."""
-    lib, B = load(), x.shape[0]
+    B = x.shape[0]
     out = torch.zeros(B, 14, 14, 32, dtype=BF, device="cuda")
     code = torch.zeros(B, 14, 14, 32, dtype=torch.uint8, device="cuda")
     junk = torch.ones(100, device="cuda")
-    fn = lib.dm_conv1_fwd_tc if tc else lib.dm_conv1_fwd
-    check(fn(ptr(x), ptr(w), ptr(b), ptr(out), ptr(code), B, ptr(junk), 100, ctypes.c_void_p(0), 0,
-             ctypes.c_void_p(0), 0, stream_ptr()), "conv1_fwd")
+    check(load().dm_conv1_fwd_tc(ptr(x), ptr(w), ptr(b), ptr(out), ptr(code), B, ptr(junk), 100, ctypes.c_void_p(0), 0,
+                                 ctypes.c_void_p(0), 0, stream_ptr()), "conv1_fwd")
     return out, code, junk
 
 
 def run_conv1_wgrad(x, dpool, code, tc: bool = True):
-    lib, B = load(), x.shape[0]
+    """``tc``: the wgmma kernel, the only conv1 weight gradient there is (False, the removed SIMT kernel, is an error)."""
+    if not tc:
+        raise ValueError("the SIMT conv1 weight-gradient kernel was removed: only tc=True exists")
+    B = x.shape[0]
     gw, gb = torch.zeros(25, 32, device="cuda"), torch.zeros(32, device="cuda")
-    fn = lib.dm_conv1_wgrad_tc if tc else lib.dm_conv1_wgrad
-    check(fn(ptr(x), ptr(dpool), ptr(code), ptr(gw), ptr(gb), B, stream_ptr()), "conv1_wgrad")
+    check(load().dm_conv1_wgrad_tc(ptr(x), ptr(dpool), ptr(code), ptr(gw), ptr(gb), B, stream_ptr()), "conv1_wgrad")
     return gw, gb
 
 
@@ -140,7 +141,7 @@ def prime_workspace(kernel: str, B: int, seed: int = 99) -> None:
     if kernel == "conv1_wgrad_tc":
         x, dp, c = _dev(torch.rand(B, 28, 28, generator=g) - 0.5, _bf(torch.randn(B, 14, 14, 32, generator=g)),
                         _codes(g, (B, 14, 14, 32)))
-        run_conv1_wgrad(x, dp, c, tc=True)
+        run_conv1_wgrad(x, dp, c)
     elif kernel == "conv2_wgrad":
         a1, dy = _dev(_bf(torch.rand(B, 14, 14, 32, generator=g)), _bf(torch.randn(B, 14, 14, 64, generator=g)))
         run_conv2_wgrad(a1, dy)
@@ -228,16 +229,14 @@ def _pool_results(tag: str, kind: str, out, code, z, za, bias, n_terms: int) -> 
     return res + R.cmp_pool(tag, "grid" if kind == "edges" else kind, code, ref, slack)
 
 
-def check_conv1_fwd(B: int = 8, seed: int = 0, tc: bool = False, kinds: Sequence[str] = KINDS) -> List[Result]:
-    tag0 = "conv1_fwd_tc" if tc else "conv1_fwd"
+def check_conv1_fwd(B: int = 8, seed: int = 0, kinds: Sequence[str] = KINDS) -> List[Result]:
     res: List[Result] = []
     for kind in kinds:
-        tag = "%s.%s" % (tag0, kind)
+        tag = "conv1_fwd_tc.%s" % kind
         x, w, b = _conv1_data(kind, _gen(seed), B)
         x, w, b = _dev(x, w, b)
-        out, code, junk = run_conv1_fwd(x, w, b, tc)
-        if tc:      # the tensor-core path rounds its operands to bf16 (grid values are bf16 numbers already)
-            x, w = x.to(BF), w.to(BF)
+        out, code, junk = run_conv1_fwd(x, w, b)
+        x, w = x.to(BF), w.to(BF)       # the kernel rounds its operands to bf16 (grid values are bf16 numbers already)
         z = R.conv5x5(x[..., None], w)
         za = R.conv5x5(x.abs()[..., None], w.abs())
         if kind != "rand":
@@ -247,27 +246,24 @@ def check_conv1_fwd(B: int = 8, seed: int = 0, tc: bool = False, kinds: Sequence
     return res
 
 
-def check_conv1_fwd_tc(B: int = 8, seed: int = 0, kinds: Sequence[str] = KINDS) -> List[Result]:
-    return check_conv1_fwd(B, seed, tc=True, kinds=kinds)
+check_conv1_fwd_tc = check_conv1_fwd       # the name the kernel tests call it by
 
 
-def check_conv1_wgrad(B: int = 8, seed: int = 7, tc: bool = True, kinds: Sequence[str] = KINDS,
-                      stale_B: int = 0) -> List[Result]:
-    """conv1 weight/bias gradient fused with the maxpool1/ReLU1 backward (SIMT and wgmma versions)."""
-    tag0 = "conv1_wgrad_tc" if tc else "conv1_wgrad"
+def check_conv1_wgrad(B: int = 8, seed: int = 7, kinds: Sequence[str] = KINDS, stale_B: int = 0) -> List[Result]:
+    """conv1 weight/bias gradient fused with the maxpool1/ReLU1 backward."""
     res: List[Result] = []
     for kind in kinds:
-        tag = "%s.%s" % (tag0, kind)
+        tag = "conv1_wgrad_tc.%s" % kind
         g = _gen(seed)
         if kind == "rand":
             x, dp = torch.rand(B, 28, 28, generator=g) - 0.5, _bf(torch.randn(B, 14, 14, 32, generator=g) * 0.1)
         else:
             x, dp = R.grid(g, (B, 28, 28), -4, 4, 8), _bf(R.grid(g, (B, 14, 14, 32), -4, 4))
         x, dp, code = _dev(x, dp, _codes(g, (B, 14, 14, 32)))
-        if stale_B and tc:
+        if stale_B:
             prime_workspace("conv1_wgrad_tc", stale_B)
-        gw, gb = run_conv1_wgrad(x, dp, code, tc)
-        xr = x.to(BF) if tc else x          # the wgmma path rounds the images to bf16
+        gw, gb = run_conv1_wgrad(x, dp, code)
+        xr = x.to(BF)                       # the kernel rounds the images to bf16
         rw, rb = R.conv1_wgrad(xr, dp, code)
         if kind == "grid":
             aw, ab = R.conv1_wgrad(xr.abs(), dp.abs(), code)
@@ -275,10 +271,6 @@ def check_conv1_wgrad(B: int = 8, seed: int = 7, tc: bool = True, kinds: Sequenc
             R.assert_exact_grid(ab, 1.0, tag + ".g_b")
         res += R.compare(tag + ".g_w", kind, gw, rw) + R.compare(tag + ".g_b", kind, gb, rb)
     return res
-
-
-def check_conv1_wgrad_simt(B: int = 8, seed: int = 7, kinds: Sequence[str] = KINDS) -> List[Result]:
-    return check_conv1_wgrad(B, seed, tc=False, kinds=kinds)
 
 
 def check_conv2_fwd(B: int = 8, seed: int = 1, kinds: Sequence[str] = KINDS) -> List[Result]:
@@ -519,7 +511,7 @@ def check_end_to_end(B: int = 64, seed: int = 5, images: str = "rand") -> List[R
     flat = eng.params.detach().clone().requires_grad_(True)
     mask = dropout_keep_mask(dropout_seed_mix(seed, 0, 0), B, 512, 0.5, device="cuda")
     logits = lenet_forward(spec.views(flat), x.cuda(), train=True, keep_mask=mask, emulate_bf16=True,
-                           conv1_bf16=eng._conv1_tc)
+                           conv1_bf16=True)
     rloss, racc = loss_and_accuracy(logits, y.cuda())
     rloss.backward()
     out: List[Result] = [("e2e.loss", abs(loss - rloss.item()), 0.02 * max(1.0, abs(rloss.item()))),
@@ -746,8 +738,7 @@ def check_mlp2_end_to_end() -> List[Result]:
     return check_mlp_end_to_end("mlp2", B=96, hidden=128, seed=22)
 
 
-ALL_CHECKS = [check_conv1_fwd, check_conv1_fwd_tc, check_conv1_wgrad, check_conv1_wgrad_simt, check_conv2_fwd, check_conv2_dgrad,
-              check_conv2_wgrad, check_fc2_loss, check_fc1_fwd, check_fc2_wgrad, check_fc1_wgrad, check_fc1_dgrad_unpool,
+ALL_CHECKS = [check_conv1_fwd, check_conv1_wgrad, check_conv2_fwd, check_conv2_dgrad, check_conv2_wgrad, check_fc2_loss, check_fc1_fwd, check_fc2_wgrad, check_fc1_wgrad, check_fc1_dgrad_unpool,
               check_evaluate,
               check_end_to_end, check_bucketed_step_matches_single_kernel, check_bucketed_mlp_step_matches_single_kernel,
               check_training_reduces_loss, check_mlp_end_to_end, check_mlp2_end_to_end]

@@ -28,6 +28,7 @@ def _backend():
 def _engine_commits(make_engine, k, commits=3):
     """``commits`` x ``k`` graph-replayed iterations on one replica: after every k-th the fp32 arena must be
     sgd(w, interval_accumulate(the k gradients), fp32(lr(step) / k)) bit for bit."""
+    from distributedmnist_b200.engine_cuda import CudaLeNetEngine
     from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
     be = _backend()
     eng = make_engine(be)
@@ -38,7 +39,7 @@ def _engine_commits(make_engine, k, commits=3):
     be.kgtn_arm()
     gen = torch.Generator().manual_seed(9)
     B = eng.batch_size
-    shape = (B, 28, 28) if hasattr(eng, "_conv1_tc") else (B, 784)
+    shape = (B, 28, 28) if isinstance(eng, CudaLeNetEngine) else (B, 784)
     for c in range(commits):
         torch.cuda.synchronize()
         step = be.device_epoch if c == 0 else step + 1

@@ -11,21 +11,15 @@ def _run(fn, **kw):
     assert not bad, "failed: %s\nall: %s" % (bad, results)
 
 
-def test_conv1_fwd_fused_bias_relu_pool():
-    _run("check_conv1_fwd")
-    _run("check_conv1_fwd", B=3, seed=9)       # batch not a multiple of anything
-
-
 def test_conv1_fwd_tcgen05_software_im2col():
     _run("check_conv1_fwd_tc")
     _run("check_conv1_fwd_tc", B=3, seed=9)        # one partial tile
     _run("check_conv1_fwd_tc", B=150, seed=19)     # 230 tiles > one CTA per SM: persistent loop over the two-stage operand ring
 
 
-def test_conv1_wgrad_tcgen05_and_simt():
+def test_conv1_wgrad_tcgen05():
     _run("check_conv1_wgrad")
     _run("check_conv1_wgrad", B=150, seed=20)
-    _run("check_conv1_wgrad_simt")
 
 
 def test_conv2_fwd_tcgen05_implicit_gemm():
