@@ -56,6 +56,52 @@ class _RunnerEvent:
         return self.lib.dm_runner_query(self.runner, self.slot) == 1
 
 
+class _Snapshot:
+    """Validated copy of the newest committed weights of an engine's arena (csrc/eval_snapshot.cu) into its owner's buffers:
+    a SnapState of its own, an fp32 arena ``snap`` and, for the ``bf_ranges`` ([begin, end) pairs, multiples of 4), their
+    bf16 shadow in ``snap16``.  Each owner (the evaluation pass, the checkpoint capture) instantiates one, so their statistics
+    and accepted steps stay apart."""
+
+    def __init__(self, engine: "_CudaEngine", snap: torch.Tensor, snap16: Optional[torch.Tensor] = None, bf_ranges=(),
+                 keep: Optional[torch.Tensor] = None):
+        assert len(bf_ranges) in (0, 4) and (snap16 is not None or not bf_ranges)
+        self.eng, self.snap, self.snap16, self.keep = engine, snap, snap16, keep
+        self.bf_ranges = list(bf_ranges)
+        self.state = torch.zeros(int(engine.lib.dm_snap_state_bytes()), dtype=torch.uint8, device=engine.device)
+        self.reset()
+
+    def reset(self) -> None:
+        """Statistics and the kept step start over (enqueued on the current stream)."""
+        self.state.zero_()
+        self.state[40:44].fill_(255)             # SnapState.keep_step: nothing kept yet
+
+    def launch(self, attempts: int) -> None:
+        """``attempts`` select / copy / validate rounds on the current stream; an attempt after an accepted one exits at
+        once.  ``SnapState.step`` / ``.status`` (the first 8 bytes of ``state``) then hold the outcome."""
+        eng = self.eng
+        lib, sp = eng.lib, stream_ptr()
+        ctrl = ctypes.c_void_p(eng.backend.ctrl.local_ptr)
+        st = ptr(self.state)
+        interval = int(bool(getattr(eng, "_interval", False)))      # K > N runs the interval commit ordering too
+        r = [ctypes.c_longlong(v) for v in (self.bf_ranges or (0, 0, 0, 0))]
+        s16 = ptr(self.snap16) if self.snap16 is not None else ctypes.c_void_p(0)
+        for a in range(attempts):
+            check(lib.dm_snap_select(ctrl, st, a, interval, ctypes.c_double(eng.SNAP_WATCHDOG_MS), sp), "snap_select")
+            check(lib.dm_snap_copy(st, ptr(eng.params), ptr(self.snap), s16, ctypes.c_longlong(eng.spec.arena_numel), *r, sp),
+                  "snap_copy")
+            check(lib.dm_snap_validate(ctrl, st, a, attempts, sp), "snap_validate")
+        if self.keep is not None:
+            check(lib.dm_snap_keep(st, ptr(self.snap), ptr(self.keep), ctypes.c_longlong(eng.spec.arena_numel), sp),
+                  "snap_keep")
+
+    def stats(self) -> dict:
+        """Attempts made, rejected by validate, ended by the watchdog, ended a ring lap behind; passes accepted / failed
+        (synchronises the current stream)."""
+        torch.cuda.current_stream().synchronize()
+        w = self.state[:40].cpu().view(torch.int32).tolist()
+        return dict(attempts=w[4], rejected=w[5], timeouts=w[6], accepted_passes=w[7], failed_passes=w[8], laps=w[9])
+
+
 class _CudaEngine(ComputeEngine):
     """What the sm_90a engines share: parameter / gradient arenas, two input slots fed on a copy stream, the native step
     runner, the optimizer binding and the graph-replayed step.  A subclass builds its kernel sequence in ``_launch_step``,
@@ -417,6 +463,89 @@ class _CudaEngine(ComputeEngine):
     def step_info(self) -> StepInfo:
         return self.backend.last_step_info(check=True)     # one packed device->host read
 
+    # ---- checkpoint capture ------------------------------------------------------------------------------------------------
+    # A checkpoint is staged on the training stream right after the launched step, in a device buffer of its own, and copied
+    # from there to one of CKPT_HOST_BUFFERS page-locked host arenas on a dedicated stream (not the copy stream: a multi-MB
+    # DMA there would queue ahead of the next step's input).  The host learns that it landed from an event query.
+    SNAP_ATTEMPTS = 4              # select / copy / validate attempts of one snapshot (evaluation pass, checkpoint capture)
+    SNAP_WATCHDOG_MS = 2.0         # how long one attempt waits for the pushes of the newest committed step
+    CKPT_HOST_BUFFERS = 2
+
+    def arm_checkpoint(self, snapshot: bool) -> None:
+        """Allocate the capture's buffers.  ``snapshot=False``: no peer writes this arena between two of its steps (K = N, cdf
+        mode), so a capture is a device-to-device copy of the live arena plus the epoch word.  ``snapshot=True`` (K < N,
+        K > N, interval): peers push weights into it at any time, so a capture is SNAP_ATTEMPTS select / copy / validate
+        attempts (csrc/eval_snapshot.cu) into the staging buffer, and one whose attempts all fail reports step -1."""
+        dev, n = self.device, self.spec.arena_numel
+        self._ck_dev = torch.zeros(n, dtype=torch.float32, device=dev)
+        self._ck_snap = _Snapshot(self, self._ck_dev) if snapshot else None      # no bf16 shadow: the file holds fp32 only
+        # (step, status) of the capture: SnapState.step / .status; the live capture copies the epoch word into .step and
+        # leaves .status at 0
+        self._ck_state = self._ck_snap.state if snapshot else \
+            torch.zeros(int(self.lib.dm_snap_state_bytes()), dtype=torch.uint8, device=dev)
+        off = self.backend._off["epoch"]
+        self._ck_epoch = self.backend._ctrl_bytes[off:off + 4]
+        self.ckpt_host = [torch.zeros(n, dtype=torch.float32).pin_memory() for _ in range(self.CKPT_HOST_BUFFERS)]
+        self._ck_rec = [torch.zeros(2, dtype=torch.int32).pin_memory() for _ in range(self.CKPT_HOST_BUFFERS)]  # step, status
+        self._ck_stream = torch.cuda.Stream(device=dev)
+        self._ck_staged, self._ck_landed = torch.cuda.Event(), torch.cuda.Event()
+        self._ck_seq = 0
+        self._ck_inflight: Optional[Tuple[int, int]] = None       # (seq, host buffer) of the capture not yet seen landed
+        if snapshot:
+            self._ck_snap.launch(self.SNAP_ATTEMPTS)   # loads the kernels now rather than at the first capture in training
+            torch.cuda.synchronize()
+            self._ck_snap.reset()                      # statistics count real captures only
+        torch.cuda.synchronize()
+
+    def enqueue_checkpoint(self, buf: int) -> int:
+        """Capture the weights after the step enqueued last into page-locked host arena ``ckpt_host[buf]``, which the caller
+        must not read or hand out again until :meth:`checkpoint_poll` / :meth:`checkpoint_wait` returned this capture.  One
+        capture at a time.  No host synchronisation.  Returns the capture's sequence number."""
+        if self._ck_inflight is not None:
+            raise RuntimeError("enqueue_checkpoint: capture %d has not landed yet" % self._ck_inflight[0])
+        cur = torch.cuda.current_stream()
+        cur.wait_event(self._ck_landed)              # the staging buffer's previous device->host copy has completed
+        if self._ck_snap is not None:
+            self._ck_snap.launch(self.SNAP_ATTEMPTS)
+        else:
+            self._ck_dev.copy_(self.params)
+            self._ck_state[0:4].copy_(self._ck_epoch)
+        self._ck_staged.record(cur)
+        self._ck_seq += 1
+        with torch.cuda.stream(self._ck_stream):
+            self._ck_stream.wait_event(self._ck_staged)
+            self.ckpt_host[buf].copy_(self._ck_dev, non_blocking=True)
+            self._ck_rec[buf].copy_(self._ck_state[0:8].view(torch.int32), non_blocking=True)
+            self._ck_landed.record(self._ck_stream)
+        self._ck_inflight = (self._ck_seq, buf)
+        return self._ck_seq
+
+    def _checkpoint_landed(self) -> Tuple[int, int, int]:
+        seq, buf = self._ck_inflight
+        self._ck_inflight = None
+        step, status = (int(v) for v in self._ck_rec[buf].tolist())
+        return seq, buf, (step & 0xFFFFFFFF) if status >= 0 else -1
+
+    def checkpoint_poll(self) -> Optional[Tuple[int, int, int]]:
+        """``(seq, host buffer, global step)`` once the capture in flight has landed in host memory (an event query, never
+        a wait), else None.  Step -1: no consistent snapshot, the buffer holds nothing usable.  Landing is established by
+        the event recorded after the device-to-host copies of the arena and of the (step, status) record; ``seq`` is the
+        host's count of captures (the one :meth:`enqueue_checkpoint` returned), not read back from the device."""
+        if self._ck_inflight is None or not self._ck_landed.query():
+            return None
+        return self._checkpoint_landed()
+
+    def checkpoint_wait(self) -> Optional[Tuple[int, int, int]]:
+        """Like :meth:`checkpoint_poll`, but waits for the capture in flight (None if there is none)."""
+        if self._ck_inflight is None:
+            return None
+        self._ck_landed.synchronize()
+        return self._checkpoint_landed()
+
+    def checkpoint_stats(self) -> Optional[dict]:
+        """Snapshot statistics of the capture (see :class:`_Snapshot`), None for the live capture."""
+        return self._ck_snap.stats() if self._ck_snap is not None else None
+
     # ---- inference ------------------------------------------------------------------------------------------
     def _eval_forward(self, images: torch.Tensor, labels: torch.Tensor, B: int) -> None:
         """Inference forward of one batch: (mean loss, accuracy) of its B rows into ``d_loss_acc``."""
@@ -740,8 +869,6 @@ class CudaLeNetEngine(_CudaEngine):
     # has fired (in the training loop: the next step's completion event).
     EVAL_CHUNK = 2048
     EVAL_RING = 16                 # host record slots
-    SNAP_ATTEMPTS = 4              # snapshot attempts captured in front of a snapshot pass
-    SNAP_WATCHDOG_MS = 2.0         # how long one attempt waits for the pushes of the newest committed step
     SNAP_KEEP = False              # also keep the last accepted snapshot (one more 6.65 MB copy per accepted pass), see
                                    # eval_snapshot(); set before arm_eval
 
@@ -784,21 +911,21 @@ class CudaLeNetEngine(_CudaEngine):
             # or read: the rest stays zero
             self._snap16 = torch.zeros(self.spec.arena_numel, dtype=bf, device=dev)
             self._snap_keep = torch.zeros(self.spec.arena_numel, dtype=f32, device=dev) if self.SNAP_KEEP else None
-            self._snap_state = torch.zeros(int(lib.dm_snap_state_bytes()), dtype=u8, device=dev)
             # the bf16 operands of the pass: conv2 and fc1 weights (tensor-core kernels); everything else is read as fp32
             self._snap_bf_ranges = []
             for name in ("conv2_weights", "fc1_weights"):
                 q = self.spec.param(name)
                 assert q.offset % 4 == 0 and q.numel % 4 == 0, name
                 self._snap_bf_ranges += [q.offset, q.offset + q.numel]
+            self._ev_snap = _Snapshot(self, self._snap, self._snap16, self._snap_bf_ranges, self._snap_keep)
+            self._snap_state = self._ev_snap.state
             self._ev_views = (self.spec.views(self._snap), self.spec.views(self._snap16))
         else:
             self._ev_views = (self.p, self.pb)
         self._launch_eval(publish=False)        # sets the kernels' function attributes outside a capture
         torch.cuda.synchronize()
         if self._snapshot:
-            self._snap_state.zero_()              # statistics count real passes only
-            self._snap_state[40:44].fill_(255)     # SnapState.keep_step: nothing kept yet
+            self._ev_snap.reset()                 # statistics count real passes only
         if self.use_graph:
             gr = torch.cuda.CUDAGraph()
             cap = torch.cuda.Stream(device=dev)
@@ -807,20 +934,8 @@ class CudaLeNetEngine(_CudaEngine):
             self._ev_graph = gr
 
     def _launch_snapshot(self, attempts: int) -> None:
-        """``attempts`` select / copy / validate rounds (csrc/eval_snapshot.cu); an attempt after an accepted one exits at once."""
-        lib, sp = self.lib, stream_ptr()
-        ctrl = ctypes.c_void_p(self.backend.ctrl.local_ptr)
-        st = ptr(self._snap_state)
-        interval = int(bool(getattr(self, "_interval", False)))
-        r = [ctypes.c_longlong(v) for v in self._snap_bf_ranges]
-        for a in range(attempts):
-            check(lib.dm_snap_select(ctrl, st, a, interval, ctypes.c_double(self.SNAP_WATCHDOG_MS), sp), "snap_select")
-            check(lib.dm_snap_copy(st, ptr(self.params), ptr(self._snap), ptr(self._snap16),
-                                   ctypes.c_longlong(self.spec.arena_numel), *r, sp), "snap_copy")
-            check(lib.dm_snap_validate(ctrl, st, a, attempts, sp), "snap_validate")
-        if self._snap_keep is not None:
-            check(lib.dm_snap_keep(st, ptr(self._snap), ptr(self._snap_keep), ctypes.c_longlong(self.spec.arena_numel), sp),
-                  "snap_keep")
+        """The pass's ``attempts`` select / copy / validate rounds (see :meth:`_Snapshot.launch`)."""
+        self._ev_snap.launch(attempts)
 
     def _launch_eval(self, publish: bool, logits_out: Optional[torch.Tensor] = None, p=None, pb=None) -> None:
         """One pass over the validation set with the weight views ``p`` (fp32) / ``pb`` (bf16): by default the armed ones --
@@ -922,9 +1037,7 @@ class CudaLeNetEngine(_CudaEngine):
         """Snapshot attempts since :meth:`arm_eval`: made, rejected by validate, ended by the watchdog, ended because the
         commit slot of the candidate step was already reused (a ring lap behind); passes accepted / failed (synchronises
         the current stream)."""
-        torch.cuda.current_stream().synchronize()
-        w = self._snap_state[:40].cpu().view(torch.int32).tolist()
-        return dict(attempts=w[4], rejected=w[5], timeouts=w[6], accepted_passes=w[7], failed_passes=w[8], laps=w[9])
+        return self._ev_snap.stats()
 
     def eval_record(self):
         """The newest complete record (see :meth:`eval_records`), or None."""

@@ -19,6 +19,7 @@ reference runs only to log loss/accuracy (:334), ``sess.kill()/reset_kill()``
 from __future__ import annotations
 
 import os
+import queue
 import threading
 import time
 from datetime import datetime
@@ -47,23 +48,54 @@ LOG_FORMAT = ("Worker %d: %s: step %d, loss = %f, train_acc = %f, test_acc = %f"
 
 
 class _AsyncCheckpointer:
-    """Chief-side saver: snapshot on the training thread, file IO on a helper thread."""
+    """Chief-side saver; file IO runs on a helper thread.
 
-    def __init__(self, train_dir: str, spec, interval_s: float, step_fn=None):
+    Without ``engine`` (torch engine, CPU path) the weights are copied to the host on the training thread.  With the sm_90a
+    engine (``engine`` armed by ``arm_checkpoint``) a checkpoint is a device capture: ``maybe_save`` enqueues it on the
+    training stream after the launched step and returns; later calls poll its event (never a wait) and, once it has landed
+    in one of the engine's page-locked host arenas, hand that arena and the step the capture names to the saver thread,
+    which slices it into the state dict and writes the files.  An arena goes back into use only after the saver thread is
+    done with it, and at most one capture is in flight.  A capture that found no consistent snapshot writes no file; it is
+    counted in ``failed`` and retried at the next call instead of after another ``interval_s``."""
+
+    def __init__(self, train_dir: str, spec, interval_s: float, engine=None, timeout_s: float = 30.0):
         self.train_dir, self.spec, self.interval_s = train_dir, spec, interval_s
-        self.step_fn = step_fn       # GPU path: drain the step in flight and read the device step counter (consistent snapshot)
         self.saver = Saver()
         self._next = time.time() + interval_s
         self._thread: Optional[threading.Thread] = None
+        self.engine, self.timeout_s = engine, timeout_s
+        self.failed = 0                          # captures without a consistent snapshot (each retried)
+        self._retry = False
+        self._pending = False                    # a capture is in flight
+        if engine is not None:
+            self._lock = threading.Lock()
+            self._free = [True] * len(engine.ckpt_host)
+            self._queue: "queue.Queue" = queue.Queue()
+            self._error: Optional[BaseException] = None
+            self._thread = threading.Thread(target=self._write_loop, daemon=True)
+            self._thread.start()
 
     def maybe_save(self, params: torch.Tensor, global_step: int) -> None:
+        if self.engine is not None:
+            self._collect(self.engine.checkpoint_poll() if self._pending else None)
+            if self._pending or not (self._retry or time.time() >= self._next):
+                return
+            with self._lock:
+                buf = next((b for b, free in enumerate(self._free) if free), None)
+            if buf is None:
+                return                           # both arenas are still being written: try again at the next step
+            self._next = time.time() + self.interval_s
+            self._enqueue(buf)
+            return
         if time.time() >= self._next:
             self._next = time.time() + self.interval_s
             self.save(params, global_step, blocking=False)
 
     def save(self, params: torch.Tensor, global_step: int, blocking: bool = True) -> None:
-        if self.step_fn is not None:
-            global_step = self.step_fn()         # the host loop runs one step ahead of what it has consumed
+        if self.engine is not None:
+            assert blocking, "device captures are saved without blocking through maybe_save"
+            self._save_final()
+            return
         state = self.spec.to_state_dict(params)  # consistent snapshot (device -> host copy)
         if self._thread is not None:
             self._thread.join()
@@ -73,8 +105,67 @@ class _AsyncCheckpointer:
             self._thread.join()
 
     def close(self) -> None:
+        if self.engine is not None:
+            self._queue.put(None)
         if self._thread is not None:
             self._thread.join()
+        if self.engine is not None and self._error is not None:
+            raise RuntimeError("writing a checkpoint failed") from self._error
+
+    # ---- device captures -----------------------------------------------------------------------------------------------
+    def _enqueue(self, buf: int) -> None:
+        with self._lock:
+            self._free[buf] = False
+        self.engine.enqueue_checkpoint(buf)
+        self._pending = True
+        self._retry = False
+
+    def _collect(self, landed) -> bool:
+        """Hand a landed capture ``(seq, buffer, step)`` to the saver thread, or count it as failed.  True if it was accepted."""
+        if landed is None:
+            return False
+        self._pending = False
+        _seq, buf, step = landed
+        if step < 0:
+            self.failed += 1
+            self._retry = True
+            with self._lock:
+                self._free[buf] = True
+            return False
+        self._queue.put((buf, step))
+        return True
+
+    def _save_final(self) -> None:
+        """Blocking capture after the last step, retried until one is accepted or ``timeout_s`` has passed.  The file's step
+        is the step the captured weights hold."""
+        self._collect(self.engine.checkpoint_wait())      # a periodic capture still in flight is a checkpoint too
+        deadline = time.time() + self.timeout_s
+        while True:
+            self._queue.join()                   # every arena is free again
+            self._enqueue(0)
+            if self._collect(self.engine.checkpoint_wait()):
+                break
+            if time.time() >= deadline:
+                raise RuntimeError("final checkpoint: no consistent snapshot of the weights within %.0f ms (%d capture(s) "
+                                   "failed)" % (self.timeout_s * 1e3, self.failed))
+        self._queue.join()
+
+    def _write_loop(self) -> None:
+        while True:
+            item = self._queue.get()
+            try:
+                if item is None:
+                    return
+                buf, step = item
+                try:
+                    self.saver.save(self.train_dir, self.spec.to_state_dict(self.engine.ckpt_host[buf]), step)
+                except BaseException as e:  # noqa: BLE001  (re-raised by close())
+                    self._error = e
+                finally:
+                    with self._lock:
+                        self._free[buf] = True
+            finally:
+                self._queue.task_done()
 
 
 class _BatchPacker:
@@ -290,12 +381,15 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     eval_mark = restored_step      # snapshot passes: global step consumed when the last one was enqueued
     test_acc_value = 0.0           # newest complete evaluation; hard-wired to 0 in the reference (:363) and when off
 
-    def _device_step() -> int:
-        torch.cuda.synchronize()
-        return int(backend.device_epoch)
-    ckpt = _AsyncCheckpointer(flags.train_dir, spec, flags.save_interval_secs,
-                              step_fn=_device_step if (fused_step and hasattr(backend, "device_epoch")) else None) \
-        if is_chief else None
+    ckpt = None
+    if is_chief:
+        # GPU path: checkpoints are device captures of the chief's arena after a launched step -- a copy of the live arena
+        # when no peer writes it between steps (the same `exact` test as the evaluation pass), else a validated snapshot
+        device_ckpt = fused_step and hasattr(engine, "arm_checkpoint")
+        if device_ckpt:
+            engine.arm_checkpoint(snapshot=not exact)
+        ckpt = _AsyncCheckpointer(flags.train_dir, spec, flags.save_interval_secs, engine=engine if device_ckpt else None,
+                                  timeout_s=flags.sync_timeout_ms * 1e-3)
     summary = SummaryWriter(flags.train_dir) if (is_chief and flags.should_summarize) else None
 
     # Even if not using timeout, we want to wait until all machines are ready (reference :275-277).
@@ -547,6 +641,9 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     if is_chief:
         ckpt.save(engine.params, step, blocking=True)
         ckpt.close()
+        if ckpt.failed:
+            log.info("checkpoints: %d capture(s) found no consistent weight snapshot; each was retried at the next step"
+                     % ckpt.failed)
     if summary is not None:
         summary.close()
     if eval_every:
