@@ -12,6 +12,7 @@
 // record does not depend on CTA scheduling.  The last chunk's last CTA writes the record straight into page-locked host
 // memory, like publish_status (csrc/fused_sync.cuh): the host reads it after an event that follows the pass.
 #include "common.cuh"
+#include "eval_state.cuh"
 #include "host_utils.h"
 
 namespace dm {
@@ -22,16 +23,6 @@ constexpr int EV_THREADS = EV_HID / 4;
 constexpr int EV_MAX_SPLITS = 8;
 constexpr int EV_MAX_ROWS = 4096;          // rows per chunk (the per-row workspace holds this many)
 constexpr int EV_RECORD_WORDS = 8;         // u64 words per host record
-
-// Device-resident running state of a pass (caller-owned, zero-initialised once).
-struct EvalState {
-  double loss_sum;                 // sum of per-row cross entropies, chunk after chunk
-  unsigned long long t_begin;      // %globaltimer at the start of the pass
-  unsigned int correct;
-  unsigned int examples;
-  unsigned int ticket;             // arrive_last_cta ticket of the chunk in flight
-  unsigned int seq;                // records published so far
-};
 
 // Per-row workspace: loss terms [EV_MAX_ROWS] fp32, then hit flags [EV_MAX_ROWS] u32.
 struct EvalArgs {

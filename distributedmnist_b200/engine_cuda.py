@@ -847,6 +847,9 @@ class CudaLeNetEngine(_CudaEngine):
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1
         torch.cuda.current_stream().wait_event(self._join_loss)      # the loss read-back branch rejoins at the end of the step
+        if with_sync and self._stop is not None:
+            self._launch_stop_publish()          # the step's last node: after its exchange, and after the loss read-back
+            n += 1
         self.launches_per_step = n
 
     # ---- inference ------------------------------------------------------------------------------------------
@@ -922,13 +925,17 @@ class CudaLeNetEngine(_CudaEngine):
             self._ev_views = (self.spec.views(self._snap), self.spec.views(self._snap16))
         else:
             self._ev_views = (self.p, self.pb)
+        self._target = None
         self._launch_eval(publish=False)        # sets the kernels' function attributes outside a capture
         torch.cuda.synchronize()
         if self._snapshot:
             self._ev_snap.reset()                 # statistics count real passes only
+        self._capture_eval()
+
+    def _capture_eval(self) -> None:
         if self.use_graph:
             gr = torch.cuda.CUDAGraph()
-            cap = torch.cuda.Stream(device=dev)
+            cap = torch.cuda.Stream(device=self.device)
             with torch.cuda.graph(gr, stream=cap, capture_error_mode="thread_local"):
                 self._launch_eval(publish=True)
             self._ev_graph = gr
@@ -968,6 +975,11 @@ class CudaLeNetEngine(_CudaEngine):
                                    ptr(p["fc2_weights"]), ptr(p["fc2_biases"]), ptr(self._ev_y[s:s + m]), ptr(self._ev_ws),
                                    ptr(self._ev_state), step_ptr, status_ptr, ring, self.EVAL_RING, lg, m,
                                    int(s + m == n), sp), "eval_head")
+        if publish and self._target is not None:
+            need, margin = self._target
+            check(lib.dm_eval_target(ptr(self._ev_state), step_ptr, status_ptr, ctypes.c_uint(need), ctypes.c_uint(n),
+                                     ctypes.c_uint(margin), self._stop.ptr_table(), self.backend.ctx.rank,
+                                     self.backend.ctx.world_size, sp), "eval_target")
 
     def enqueue_eval(self) -> None:
         """Score the validation set with the current weights, on the current (training) stream, without a host
@@ -1050,6 +1062,58 @@ class CudaLeNetEngine(_CudaEngine):
         self._launch_eval(publish=True, logits_out=logits_out)
         torch.cuda.current_stream().synchronize()
         return self.eval_record()
+
+    # ---- quality target (csrc/eval_target.cu) -----------------------------------------------------------------------------
+    # With a target armed, the chief's evaluation pass ends with eval_target, which sets the stop step in every replica's
+    # stop word, and every replica's step graph ends with stop_publish, which copies its own stop word into page-locked host
+    # memory.  The host reads that word after the step's completion event, which the training loop waits for anyway.  Why a
+    # K = N run then stops every replica after the same step: DESIGN §4.4.
+    _stop = None                   # symmetric u32 stop word (0: no stop set), see arm_stop
+    _target = None                 # (need, margin) of the chief's target test, see arm_target
+
+    def arm_stop(self) -> None:
+        """Allocate this replica's stop word (symmetric memory: collective, every rank calls it at the same point) and its
+        page-locked host copy.  From then on every training step ends with stop_publish: the step graphs are re-captured."""
+        self._leave_native_runner()
+        self._stop = self.backend.allocate_buffer(4)
+        self._stop.view(torch.int32, 0, 1).zero_()
+        self._stop_host = torch.zeros(1, dtype=torch.int32).pin_memory()
+        self._stop_host_np = self._stop_host.numpy().view(np.uint32)
+        self._tta_t0 = torch.zeros(1, dtype=torch.int64, device=self.device)
+        self._graphs = [None, None]
+        torch.cuda.synchronize()
+        if self.backend.ctx.world_size > 1:
+            self.backend.barrier()             # every stop word is zero before the chief can set one
+
+    def arm_target(self, need: int, margin: int) -> None:
+        """Chief, after :meth:`arm_eval` and :meth:`arm_stop`: every evaluation pass ends with eval_target.  The first pass
+        over the whole validation set with at least ``need`` correct rows (a snapshot pass only if its snapshot was
+        accepted) stores S = (global step it scored) + ``margin`` into every replica's stop word."""
+        if self._stop is None or getattr(self, "_ev_x", None) is None:
+            raise RuntimeError("arm_target: arm_eval() and arm_stop() first")
+        n = int(self._ev_x.shape[0])
+        if not 1 <= int(need) <= n or int(margin) < 1:
+            raise ValueError("arm_target: need %d of %d examples, margin %d" % (need, n, margin))
+        self._leave_native_runner()
+        self._target = (int(need), int(margin))
+        self._capture_eval()
+
+    def _launch_stop_publish(self) -> None:
+        check(self.lib.dm_stop_publish(ctypes.c_void_p(self._stop.local_ptr), ptr(self._stop_host), stream_ptr()),
+              "stop_publish")
+
+    def stop_step(self) -> int:
+        """Stop step S of this replica's stop word, 0 while none is set, as its newest completed step saw it (a host read:
+        valid after waiting for a step's completion)."""
+        return int(self._stop_host_np[0])
+
+    def enqueue_start_stamp(self) -> None:
+        """``%globaltimer`` into a device word, on the current stream: enqueue it right before the run's first step."""
+        check(self.lib.dm_tta_stamp(ptr(self._tta_t0), stream_ptr()), "tta_stamp")
+
+    def start_stamp_ns(self) -> int:
+        """The stamp of :meth:`enqueue_start_stamp` (a device read, ordered after the current stream's work)."""
+        return int(self._tta_t0.cpu()[0])
 
 
 class CudaMlpEngine(_CudaEngine):

@@ -263,6 +263,9 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
                                             "one (test_acc, worker0_eval.npy); 0 = off.  GPU path: lenet; K < N or interval need --eval_snapshot")
     F.DEFINE_boolean("eval_snapshot", False, "GPU path, with --eval_every_steps: score a validated snapshot of the newest "
                                              "committed weights, so K < N and --interval_method runs can be evaluated too")
+    F.DEFINE_float("target_accuracy", 0.0, "With --eval_every_steps: stop the run after the first in-training evaluation "
+                                           "whose validation accuracy is >= this value, and report the training time it "
+                                           "took (worker0_time_to_accuracy.json); 0 = off, else 0 < A <= 1")
     return F
 
 

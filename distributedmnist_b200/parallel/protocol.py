@@ -1066,3 +1066,107 @@ class CountTriggerModel:
             if self.accumulated[q] != self.accepted[q] + self.lost[q] + residual:
                 raise ProtocolHazard("replica %d accumulated %d gradients: %d accepted, %d lost, %d pending"
                                      % (q, self.accumulated[q], self.accepted[q], self.lost[q], residual))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# --target_accuracy -- host loops of N lock-step replicas against the stop word (csrc/eval_target.cu, train.py)
+# ----------------------------------------------------------------------------------------------------------------------
+class TargetStopModel:
+    """N replicas with K = N: one host loop (``train.train``'s pipelined or non-pipelined loop) and one device stream each,
+    as generators for :func:`run_random` / :func:`explore_schedules` (actors 0..N-1 are the hosts, N..2N-1 the devices).
+
+    * host: launch step j; the chief enqueues a pass after it when ``j % every == 0`` or ``j > max``; wait for step j - 1
+      (pipelined) or j (non-pipelined), read the host word, lower ``max`` to a stop step found there; stop launching once
+      ``j > max``.
+    * device: step j publishes its exchange (on the chief after the target test of the pass after step j - 1), waits for
+      every replica's exchange of step j, then ``stop_publish`` copies the replica's stop word into its host word.  The
+      chief's pass after step j reaches the target iff ``j >= reach``; its test stores S = j + ``margin`` into every
+      replica's stop word if none is set.
+
+    Invariants (``ProtocolHazard`` otherwise): no deadlock, every replica launches exactly the steps a run with
+    ``--max_steps=S`` launches (S = min(max_steps, stop step)), and the chief enqueues exactly that run's passes."""
+
+    def __init__(self, n: int, every: int, reach: int, margin: int, max_steps: int = 1000, pipelined: bool = True):
+        self.n, self.every, self.reach, self.margin, self.max_steps, self.pipelined = n, every, reach, margin, max_steps, pipelined
+        self.launched = [0] * n
+        self.host_done = [False] * n
+        self.exchanged = [0] * n       # newest step whose exchange the replica has published
+        self.completed = [0] * n
+        self.stop = [0] * n            # stop words (device)
+        self.host_word = [0] * n       # page-locked copies (host)
+        self.evals: List[int] = []     # steps after which the chief enqueued a pass
+
+    def host(self, r: int):
+        mx, j = self.max_steps, 0
+        while True:
+            j += 1
+            self.launched[r] = j
+            if r == 0 and (j % self.every == 0 or j > mx):
+                self.evals.append(j)
+            yield None
+            wait = j - 1 if self.pipelined else j
+            if wait > 0:
+                yield (lambda w=wait: self.completed[r] >= w)
+                if self.host_word[r]:
+                    mx = min(mx, self.host_word[r])
+            if j > mx:
+                break
+            yield None
+        yield (lambda: self.completed[r] >= j)            # the step still in flight is drained
+        self.host_done[r] = True
+
+    def device(self, r: int):
+        j = 0
+        while True:
+            yield (lambda: self.launched[r] > j or self.host_done[r])
+            if self.launched[r] <= j:
+                return
+            j += 1
+            self.exchanged[r] = j
+            yield None
+            yield (lambda s=j: all(e >= s for e in self.exchanged))
+            self.host_word[r] = self.stop[r]
+            self.completed[r] = j
+            yield None
+            if r == 0:
+                # the pass after step j (if any) is known once step j + 1 is launched or the host has finished
+                yield (lambda s=j: self.launched[0] > s or self.host_done[0])
+                if j in self.evals and j >= self.reach and not self.stop[0]:
+                    for q in range(self.n):
+                        self.stop[q] = j + self.margin
+                yield None
+
+    def run(self, choose) -> None:
+        n = self.n
+        gens = {a: (self.host(a) if a < n else self.device(a - n)) for a in range(2 * n)}
+        waiting = {}
+        for a in list(gens):
+            BucketV2Model._advance(a, gens, waiting)
+        while gens:
+            runnable = [a for a in sorted(gens) if a not in waiting or waiting[a]()]
+            if not runnable:
+                raise ProtocolHazard("deadlock: %s wait forever (launched %s, completed %s)"
+                                     % (sorted(gens), self.launched, self.completed))
+            a = choose(runnable)
+            waiting.pop(a, None)
+            BucketV2Model._advance(a, gens, waiting)
+        first = next((j for j in range(1, self.max_steps + 2) if j >= self.reach and
+                      (j % self.every == 0 or j > self.max_steps)), None)
+        s = min(self.max_steps, first + self.margin) if first is not None else self.max_steps
+        if self.launched != [s + 1] * n:
+            raise ProtocolHazard("replicas launched %s steps, a run with --max_steps=%d launches %d"
+                                 % (self.launched, s, s + 1))
+        want = [j for j in range(1, s + 2) if j % self.every == 0 or j > s]
+        if self.evals != want:
+            raise ProtocolHazard("the chief enqueued passes after steps %s, a run with --max_steps=%d after %s"
+                                 % (self.evals, s, want))
+
+
+def run_random(make_model, seeds) -> int:
+    """Run ``make_model().run`` once per seed, every choice drawn at random.  Returns the number of runs; raises the first
+    ``ProtocolHazard``."""
+    import random
+    for seed in seeds:
+        rng = random.Random(seed)
+        make_model().run(lambda runnable: runnable[rng.randrange(len(runnable))])
+    return len(seeds)

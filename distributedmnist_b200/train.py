@@ -18,11 +18,14 @@ reference runs only to log loss/accuracy (:334), ``sess.kill()/reset_kill()``
 """
 from __future__ import annotations
 
+import json
+import math
 import os
 import queue
 import threading
 import time
 from datetime import datetime
+from fractions import Fraction
 from typing import Dict, Optional
 
 import numpy as np
@@ -297,6 +300,69 @@ def check_eval_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate: int,
                          % ctx.world_size + hint)
 
 
+def check_target_flags(flags, ctx: ReplicaContext) -> None:
+    """``--target_accuracy`` combinations that cannot work, rejected before any device work starts."""
+    a = float(getattr(flags, "target_accuracy", 0.0) or 0.0)
+    if a == 0.0:
+        return
+    if not 0.0 < a <= 1.0:
+        raise ValueError("--target_accuracy must lie in (0, 1] (0 = off), got %r" % a)
+    if getattr(flags, "eval_every_steps", 0) <= 0:
+        raise ValueError("--target_accuracy needs --eval_every_steps > 0: the run stops after the first in-training "
+                         "evaluation that reaches the target")
+    if not (ctx.on_gpu and flags.backend in ("auto", "fused")) and ctx.world_size > 1:
+        raise ValueError("--target_accuracy with the torch engine (--backend=%s%s) is implemented for one replica, not %d: "
+                         "only the chief evaluates and nothing tells the other replicas to stop"
+                         % (flags.backend, "" if ctx.on_gpu else ", no GPU", ctx.world_size))
+
+
+def need_count(target: float, examples: int) -> int:
+    """Smallest correct count ``need`` with ``need / examples >= target``, exactly (the decimal value of ``target``)."""
+    return math.ceil(Fraction(str(target)) * examples)
+
+
+# Stop step S = g + STOP_MARGIN for the first evaluation of global step g that reaches the target.  With K = N or cdf mode
+# (replicas in lock step) this is the smallest margin with which every replica's host knows S before it launches step
+# S + 1, so each one ends exactly as a run with --max_steps=S does (DESIGN §4.4 has the ordering argument):
+#   the pass of g and its target test run on the chief's stream after step g, so step g + 1's last kernel, on every
+#   replica, reads S -- and each host reads that word after waiting for step g + 1, which the pipelined loop does right
+#   after launching step g + 2 and the non-pipelined loop right after running it.  Launching step S + 1 = g + 3 is then
+#   decided with S known; with a margin of 1 step S + 1 = g + 2 would already be launched (and its final evaluation pass
+#   decided) before S is known.
+STOP_MARGIN = 2
+
+
+class _TimeToAccuracy:
+    """``--target_accuracy`` on the chief: the first evaluation that reaches ``need`` correct rows, and the training time up
+    to it.  Clock values are in one unit per run (%globaltimer ns on the sm_90a path, host seconds with the torch engine);
+    ``scale`` converts them to seconds."""
+
+    def __init__(self, target: float, need: int, examples: int, scale: float, clock: str):
+        self.target, self.need, self.examples, self.scale, self.clock = target, need, examples, scale, clock
+        self.reached = None          # (global step, t_begin, correct, wall seconds) of the reaching pass
+        self._eval_time = 0          # sum of (t_end - t_begin) over the passes before it
+
+    def add(self, step: int, t_begin, t_end, examples: int, correct: int, counts: bool, wall_s: float) -> bool:
+        """One completed pass (``counts``: its record is valid, i.e. not a dropped snapshot pass).  True if it is the first
+        one to reach the target."""
+        if self.reached is not None:
+            return False
+        if counts and examples == self.examples and correct >= self.need:
+            self.reached = (step, t_begin, correct, wall_s)
+            return True
+        self._eval_time += t_end - t_begin
+        return False
+
+    def report(self, t0) -> Dict:
+        out = dict(target=self.target, need=self.need, examples=self.examples, reached=self.reached is not None,
+                   global_step=None, correct=None, accuracy=None, train_time_s=None, wall_time_s=None, clock=self.clock)
+        if self.reached is not None:
+            step, t_begin, correct, wall_s = self.reached
+            out.update(global_step=step, correct=correct, accuracy=correct / float(self.examples),
+                       train_time_s=(t_begin - t0 - self._eval_time) * self.scale, wall_time_s=wall_s)
+        return out
+
+
 def eval_due(global_step: int, last_mark: int, every: int) -> bool:
     """Snapshot passes (K < N, interval): the host learns the global step only after a step completes, and it may jump by
     more than one.  A pass is due once the newest consumed global step has crossed a multiple of ``every`` since
@@ -314,8 +380,10 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     assert num_workers > 0
     is_chief = ctx.is_chief
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
+    check_target_flags(flags, ctx)
     check_device_data_flags(flags, ctx, dataset)
     device_data = bool(getattr(flags, "device_data", False))
+    target = float(getattr(flags, "target_accuracy", 0.0) or 0.0)
 
     backend = make_backend(ctx, flags.backend, flags)
     engine = make_engine(flags, ctx, backend)
@@ -376,6 +444,20 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     if device_data:
         # every replica keeps its own copy, in its own shuffled order: a step's input is then B row indices
         engine.arm_train_data(dataset.images, dataset.labels)
+    # --target_accuracy: the run ends as --max_steps = min(--max_steps, S) would end it, S = the stop step of the first
+    # evaluation that reaches the target.  GPU path: the chief's pass sets S in every replica's stop word on the device and
+    # every step's last kernel copies it to the host; torch engine (one replica): decided on the host after `evaluate`.
+    max_steps = flags.max_steps
+    tta = None
+    if target:
+        if fused_step:
+            engine.arm_stop()              # every replica (a symmetric allocation)
+        if is_chief:
+            n_val = dataset_test.num_examples
+            tta = _TimeToAccuracy(target, need_count(target, n_val), n_val, 1e-9 if device_eval else 1.0,
+                                  "device %globaltimer" if device_eval else "host")
+            if device_eval:
+                engine.arm_target(tta.need, STOP_MARGIN)
     eval_rows = []                 # (global_step, t_begin_unix_s, eval_seconds, examples, correct, mean_loss)
     last_eval_step = -1
     eval_mark = restored_step      # snapshot passes: global step consumed when the last one was enqueued
@@ -439,7 +521,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             log.info("Global step attained: %d" % step)
             log.info("DONE RUNNING SESSION...")
         finish_time = time.time()
-        if step > flags.max_steps:
+        if step > max_steps:
             stop = True
             return
         duration = finish_time - start_time
@@ -466,21 +548,37 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     def collect_evals() -> None:
         """Device records completed so far (%globaltimer ns -> seconds, as push_device_times converts them)."""
         nonlocal test_acc_value
-        for gs, t0, t1, n_ex, correct, loss_sum in engine.eval_records():
+        if tta is None:
+            recs = [(r, 0) for r in engine.eval_records()]
+        else:                      # dropped snapshot passes took training-stream time too
+            recs = engine.eval_records_with_status()
+            engine.eval_dropped += sum(1 for _r, status in recs if status < 0)
+        for (gs, t0, t1, n_ex, correct, loss_sum), status in recs:
+            if tta is not None:
+                tta.add(gs, t0, t1, n_ex, correct, status >= 0, time.time() - tta_wall0)
+            if status < 0:
+                continue
             eval_rows.append((gs, t0 * 1e-9, (t1 - t0) * 1e-9, n_ex, correct, loss_sum / max(n_ex, 1)))
             test_acc_value = correct / float(max(n_ex, 1))
 
+    def note_stop() -> None:
+        """GPU path: the stop step S the chief's target test set, as the step just waited for read it."""
+        nonlocal max_steps
+        s = engine.stop_step()
+        if s:
+            max_steps = min(max_steps, s)
+
     def eval_after_step(global_step: int) -> None:
         """Non-pipelined loops: called once the step's outcome has been read back."""
-        nonlocal test_acc_value, last_eval_step, eval_mark
+        nonlocal test_acc_value, last_eval_step, eval_mark, max_steps
         if device_eval:
             collect_evals()        # the step read-back above waited for the pass enqueued after the previous step
         if snapshot_eval:
-            if global_step <= flags.max_steps and eval_due(global_step, eval_mark, eval_every):
+            if global_step <= max_steps and eval_due(global_step, eval_mark, eval_every):
                 eval_mark = global_step
                 engine.enqueue_eval()          # the final pass follows the loop
             return
-        if global_step == last_eval_step or not (global_step % eval_every == 0 or global_step > flags.max_steps):
+        if global_step == last_eval_step or not (global_step % eval_every == 0 or global_step > max_steps):
             return
         last_eval_step = global_step
         if device_eval:
@@ -488,10 +586,13 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             return
         t0 = time.time()
         loss, acc = engine.evaluate(dataset_test.images, dataset_test.labels)
+        t1 = time.time()
         n_ex = dataset_test.num_examples
         correct = int(round(acc * n_ex))
-        eval_rows.append((global_step, t0, time.time() - t0, n_ex, correct, loss))
+        eval_rows.append((global_step, t0, t1 - t0, n_ex, correct, loss))
         test_acc_value = correct / float(n_ex)
+        if tta is not None and tta.add(global_step, t0, t1, n_ex, correct, True, t1 - tta_wall0):
+            max_steps = min(max_steps, global_step + STOP_MARGIN)
 
     def save_evals() -> None:
         np.save(os.path.join(flags.train_dir, "worker%d_eval.npy" % ctx.rank),
@@ -510,6 +611,9 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         cdf_pushed = upto + 1
 
     last_consume = time.time()
+    tta_wall0 = time.time()        # --target_accuracy: the run's first step starts now (host clock) ...
+    if tta is not None and device_eval:
+        engine.enqueue_start_stamp()   # ... and on the chief's device clock, in stream order before that step
     while not stop:
         cur_iteration += 1
         do_log = (cur_iteration % every == 0)
@@ -527,7 +631,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             token = (cur_iteration, engine.step_indices(packer.next()) if device_data else engine.step_packed(packer.next()))
             launched += 1
             if device_eval and not snapshot_eval and \
-                    ((restored_step + launched) % eval_every == 0 or restored_step + launched > flags.max_steps):
+                    ((restored_step + launched) % eval_every == 0 or restored_step + launched > max_steps):
                 engine.enqueue_eval()          # K == N: restored_step + launched is the global step of the weights it scores
             prev, pending = pending, token
             if prev is not None:
@@ -536,6 +640,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 info = opt._account(backend.mirror_info(seq, check=True))
                 if device_eval:
                     collect_evals()            # passes enqueued before the step just waited for are complete
+                if target:
+                    note_stop()
                 now = time.time()
                 finish_iteration(it, last_consume, info, (float(lbuf[0]), float(lbuf[1])))
                 last_consume = now
@@ -545,7 +651,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 if device_times and it > 10 and (it % 50 == 0 or it == 500):
                     push_device_times(it)
             # K == N: the global step after `launched` steps is known without reading anything -> stop launching exactly there
-            if exact and restored_step + launched > flags.max_steps:
+            if exact and restored_step + launched > max_steps:
                 break
             continue
 
@@ -577,6 +683,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 engine.train_step()
             t2 = time.perf_counter()
             info = opt._account(engine.step_info())   # device -> host read of the step's outcome (one packed copy)
+            if target:
+                note_stop()                           # (the read above waited for the whole step)
         else:
             engine.forward_backward(opt.local_step)
             t2 = time.perf_counter()
@@ -627,6 +735,19 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                      % engine.eval_dropped)
     if eval_every:
         save_evals()
+    if tta is not None:
+        report = tta.report(engine.start_stamp_ns() if device_eval else tta_wall0)
+        results["time_to_accuracy"] = report
+        with open(os.path.join(flags.train_dir, "worker%d_time_to_accuracy.json" % ctx.rank), "w") as f:
+            json.dump(report, f, indent=1)
+            f.write("\n")
+        if report["reached"]:
+            log.info("Time to accuracy: target %g reached by the evaluation of global step #%d (accuracy %f, %d of %d "
+                     "correct); training time %.6f s without the evaluations (%s clock); wall time %.6f s"
+                     % (target, report["global_step"], report["accuracy"], report["correct"], report["examples"],
+                        report["train_time_s"], tta.clock, report["wall_time_s"]))
+        else:
+            log.info("Time to accuracy: target %g not reached" % target)
     if device_times:
         push_device_times(cur_iteration)
 
