@@ -1116,6 +1116,11 @@ class CudaLeNetEngine(_CudaEngine):
         return int(self._tta_t0.cpu()[0])
 
 
+# dm_dense10_xent (csrc/mlp_simt.cu) stages the output-layer weights as [H][11] floats and refuses more than 220 KiB
+MLP_XENT_SMEM_PER_UNIT = 11 * 4
+MLP_XENT_SMEM_LIMIT = 220 * 1024
+
+
 class CudaMlpEngine(_CudaEngine):
     """2-/3-layer MLP on the sm_90a kernels: hidden layers = wgmma GEMM with bias+ReLU fused in the
     epilogue, output layer + softmax-CE = SIMT (csrc/mlp_simt.cu), every weight gradient = wgmma GEMM
@@ -1124,6 +1129,11 @@ class CudaMlpEngine(_CudaEngine):
     def __init__(self, model: str, batch_size: int, backend: FusedBackend, hidden: int = 1024, seed: int = 66478,
                  rank: int = 0, use_graph: bool = True):
         assert hidden % 64 == 0, "--mlp_hidden must be a multiple of 64 on the GPU path"
+        if hidden * MLP_XENT_SMEM_PER_UNIT > MLP_XENT_SMEM_LIMIT:
+            raise ValueError("--mlp_hidden=%d is too wide for the output-layer kernel (dense10_xent keeps the [H,10] weights "
+                             "in %d bytes of shared memory per hidden unit, at most %d bytes): use --mlp_hidden <= %d"
+                             % (hidden, MLP_XENT_SMEM_PER_UNIT, MLP_XENT_SMEM_LIMIT,
+                                MLP_XENT_SMEM_LIMIT // MLP_XENT_SMEM_PER_UNIT // 64 * 64))
         super().__init__(get_model(model, hidden)[0], batch_size, backend, seed, use_graph, (784,))
         self.model, self.hidden = model, hidden
         self.n_layers = len(self.spec.params) // 2

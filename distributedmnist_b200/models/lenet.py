@@ -15,6 +15,7 @@ from __future__ import annotations
 
 from typing import Dict, Optional, Tuple
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -55,13 +56,21 @@ def dropout_seed_mix(seed: int, step: int, rank: int = 0) -> int:
     return (seed * 0x632BE5AB + step * 0x9E3779B9 + rank * 0x85EBCA77 + 0x7F4A7C15) & _M32
 
 
+def dropout_threshold(keep_prob: float) -> int:
+    """The 24-bit keep threshold as the kernels compute it: ``(uint32_t)(keep_prob * 16777216.f)`` with ``keep_prob``
+    an fp32.  The product is exact (a power of two), so this is floor(fp32(keep_prob) * 2^24).  It differs from
+    floor(keep_prob * 2^24) wherever fp32 rounds ``keep_prob`` up (0.3, 0.8, 0.99, ...)."""
+    return int(float(np.float32(keep_prob)) * (1 << 24))
+
+
 def dropout_keep_mask(seed_mix: int, rows: int, cols: int, keep_prob: float,
                       device: str = "cpu") -> torch.Tensor:
     """Deterministic Bernoulli(keep_prob) mask ``[rows, cols]`` (bool).
 
     A murmur3-style finaliser over the element index; the CUDA epilogue
-    (csrc/common.cuh ``dropout_keep``) computes the identical function, so the
-    backward pass regenerates the mask instead of storing it (SURVEY §2.4 K7).
+    (csrc/common.cuh ``dropout_keep``) computes the identical function, with the
+    threshold of :func:`dropout_threshold`, so the backward pass regenerates the
+    mask instead of storing it (SURVEY §2.4 K7).
     """
     idx = torch.arange(rows * cols, dtype=torch.int64, device=device)
     x = (idx * 0x9E3779B1 + seed_mix) & _M32
@@ -70,8 +79,7 @@ def dropout_keep_mask(seed_mix: int, rows: int, cols: int, keep_prob: float,
     x = x ^ (x >> 13)
     x = (x * 0xC2B2AE35) & _M32
     x = x ^ (x >> 16)
-    thresh = int(keep_prob * (1 << 24))
-    return ((x >> 8) < thresh).view(rows, cols)
+    return ((x >> 8) < dropout_threshold(keep_prob)).view(rows, cols)
 
 
 def _q(t: torch.Tensor, on: bool) -> torch.Tensor:

@@ -137,10 +137,9 @@ def drop_seed_mix(seed: int, step: int, rank: int) -> int:
 
 
 def drop_keep(seed: int, step: int, rank: int, keep_prob: float, n: int) -> np.ndarray:
-    """Contributor ``rank``'s keep mask at ``step``.  The kernel's threshold is ``fp32(keep) * 2^24``, truncated."""
+    """Contributor ``rank``'s keep mask at ``step``, with the kernel's threshold (``models.lenet.dropout_threshold``)."""
     from ..models import dropout_keep_mask
-    keep = float(np.float32(keep_prob))
-    return dropout_keep_mask(drop_seed_mix(seed, step, rank), 1, n, keep).view(-1).numpy()
+    return dropout_keep_mask(drop_seed_mix(seed, step, rank), 1, n, keep_prob).view(-1).numpy()
 
 
 # ---------------------------------------------------------------------------------------------------------------------

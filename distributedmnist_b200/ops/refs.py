@@ -1,4 +1,4 @@
-"""Float64 references of the LeNet step kernels and the one rule every kernel check compares by.
+"""Float64 references of the LeNet and MLP step kernels and the one rule every kernel check compares by.
 
 The references compute in float64 (TF32 never applies), on whatever device their inputs live on, and round to bf16 only
 where a kernel stores bf16 (round-to-nearest-even, as ``__floats2bfloat162_rn``).  Layouts are the kernels' own: NHWC
@@ -24,6 +24,7 @@ from __future__ import annotations
 
 from typing import Dict, List, Optional, Tuple
 
+import numpy as np
 import torch
 import torch.nn.functional as F
 
@@ -214,13 +215,15 @@ def fc1_dgrad_unpool(dh: torch.Tensor, w1: torch.Tensor, code2: torch.Tensor) ->
 def fc2_fwd_bwd(hsum: torch.Tensor, b1: torch.Tensor, w2: torch.Tensor, b2: torch.Tensor, labels: torch.Tensor,
                 keep: Optional[torch.Tensor], keep_prob: float) -> Dict[str, torch.Tensor]:
     """fc1 bias + ReLU (+ dropout when ``keep`` is given), fc2, mean softmax CE, accuracy, d logits [B,12] and d fc1
-    pre-activation (before its bf16 store).  ``hsum``: the fc1 GEMM result without bias."""
+    pre-activation (before its bf16 store).  ``hsum``: the fc1 GEMM result without bias.  The dropout scale is the
+    kernel's fp32 ``1.f / keep_prob`` of an fp32 ``keep_prob``, not the float64 1 / keep_prob (under --use_fast_math
+    the kernel's reciprocal is ``rcp.approx``, within one ulp of this; exact for powers of two)."""
     hp = hsum.to(F64) + b1.to(F64)
     on = hp > 0
     inv_keep = 1.0
     if keep is not None:
         on &= keep
-        inv_keep = 1.0 / keep_prob
+        inv_keep = float(np.float32(1.0) / np.float32(keep_prob))
     h = torch.where(on, hp * inv_keep, torch.zeros_like(hp))
     logits = h @ w2.to(F64) + b2.to(F64)
     B = logits.shape[0]
@@ -247,3 +250,118 @@ def fc2_wgrad(h: torch.Tensor, dl: torch.Tensor, dh: torch.Tensor) -> Tuple[torc
     """fc2 weight [512,10] / bias [10] and fc1 bias [512] gradients; dh is summed as the bf16 values the kernel reads."""
     h, dl = h.to(F64), dl.to(F64)[:, :10]
     return h.t() @ dl, dl.sum(0), dh.to(F64).sum(0)
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# MLP (csrc/mlp_simt.cu for the output layer and the bias gradients; hidden layers and weight gradients on the wgmma GEMM)
+# ---------------------------------------------------------------------------------------------------------------------
+U32 = 2.0 ** -23               # one fp32 ulp, relative (an upper bound for round-to-nearest and the approximate intrinsics)
+LOGF_ABS = 2.0 ** -20          # __logf on [1, 10]: 2^-21.41 absolute on [0.5, 2], 3 ulps above
+FTZ = 2.0 ** -126              # --use_fast_math flushes fp32 results (and bf16 conversions) below this to zero
+
+
+def cmp_bound(name: str, got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor) -> List[Result]:
+    """Elementwise |got - ref| <= bound, reported as the largest ratio (a zero bound demands equality)."""
+    d = (got.to(F64) - ref.to(F64)).abs()
+    bound = torch.as_tensor(bound, dtype=F64, device=d.device).expand_as(d)
+    ratio = torch.where(d == 0, torch.zeros_like(d), d / bound)       # d / 0 = inf: a zero bound fails on any difference
+    return [(name + "[err/bound]", float(ratio.max()) if ratio.numel() else 0.0, 1.0)]
+
+
+def cmp_bf16_bound(name: str, got: torch.Tensor, ref: torch.Tensor, bound: torch.Tensor) -> List[Result]:
+    """bf16 outputs of an fp32 value known to lie within ``bound`` of ``ref``: RNE is monotonic, so each output must lie
+    in [RNE(ref - bound), RNE(ref + bound)] -- no exceptions, and exactly RNE(ref) wherever that interval holds one bf16
+    number.  For values that pass through exp / log, where cancellation (p - 1 of a confident row) can leave the fp32
+    value with no correct bits and the one-ulp / 99 % rule of :func:`cmp_bf16` does not describe the kernel."""
+    assert got.dtype == torch.bfloat16
+    ref, bound = ref.to(F64), torch.as_tensor(bound, dtype=F64, device=ref.device)
+    o = _ordered(got)
+    lo = _ordered(rne_bf16(ref - bound).to(torch.bfloat16))
+    hi = _ordered(rne_bf16(ref + bound).to(torch.bfloat16))
+    return [(name + "[outside RNE(ref+-bound)]", float(((o < lo) | (o > hi)).sum()), 0.0)]
+
+
+def dense10_xent(h: torch.Tensor, w: torch.Tensor, b: torch.Tensor, labels: torch.Tensor) -> Dict[str, torch.Tensor]:
+    """float64 reference of ``dense10_xent`` -- h bf16 [B,H], w the fp32 [H,10] arena weights (NOT the bf16 shadow), b
+    [10] -- and the kernel's fp32 error bounds of everything that goes through exp / log:
+
+    ``logits`` = h w + b, ``loss_terms`` per row (logsumexp - logit[label]), ``hits`` per row by the FIRST maximum,
+    ``dl`` = (softmax - onehot) / B, ``dh`` = dl w^T where h > 0 else 0 (before its bf16 store), ``logit_err`` [B] bounds
+    the kernel's fp32 logits (zero error on grid data), ``term_err`` [B] a row's contribution to the loss sum,
+    ``dl_err`` [B,10] the kernel's fp32 dl, ``gap`` the top-two logit distance."""
+    B, H = h.shape
+    h64, w64, b64 = h.to(F64), w.to(F64), b.to(F64)
+    lab = labels.long()
+    logits = h64 @ w64 + b64
+    logit_abs = h64.abs() @ w64.abs() + b64.abs()
+    logit_err = fp32_slack(logit_abs, H + 1).max(dim=1).values             # one lane's fma chain, the shuffle tree, + b
+    lse = torch.logsumexp(logits, dim=1)
+    lg_label = logits.gather(1, lab[:, None])[:, 0]
+    mx = logits.max(dim=1).values
+    first = (logits == mx[:, None]).to(torch.int8).argmax(dim=1)
+    p = torch.softmax(logits, dim=1)
+    y = F.one_hot(lab, 10).to(F64)
+    # __expf(x), x = logit - max <= 0: at most 2 + 1.173 |x| ulps; the subtraction adds |x| ulps more
+    x = (logits - mx[:, None]).abs()
+    e_c = (2.0 + 2.5 * x) * U32
+    # relative error of s = sum exp(x_c) (s >= 1; each flushed exp loses less than 2^-126)
+    e_s = (p * e_c).sum(dim=1) + 10 * U32 + 10 * FTZ
+    L = logit_err[:, None]
+    # softmax moves by at most 2 p_c L when every logit moves by L; p * (1 / s), the rcp, - onehot, * (1/B); an exp or a
+    # product below 2^-126 is flushed to zero
+    dl_err = (p * (e_c + e_s[:, None] + 2 * L + 3 * U32) + U32 * (p - y).abs()) / B + 2 * U32 * ((p - y).abs() / B) \
+        + 2 * FTZ
+    term = lse - lg_label
+    term_err = (e_s + LOGF_ABS + 2 * logit_err + U32 * ((lg_label - mx).abs() + 3 * term.abs())) / B
+    dl = (p - y) / B
+    on = h64 > 0
+    dh = torch.where(on, dl @ w64.t(), torch.zeros_like(h64))
+    return dict(logits=logits, logit_abs=logit_abs, logit_err=logit_err, loss_terms=term, term_err=term_err,
+                hits=(first == lab), dl=dl, dl_err=dl_err, dh=dh, on=on, gap=_top2_gap(logits))
+
+
+def relu_bwd_colsum(dh: torch.Tensor, h: Optional[torch.Tensor]) -> Tuple[torch.Tensor, torch.Tensor, torch.Tensor]:
+    """(dpre, column sums, column sums of |dpre|), float64: dpre = dh where h > 0, else 0 (dh itself when h is None)."""
+    d = dh.to(F64)
+    if h is not None:
+        d = torch.where(h.to(F64) > 0, d, torch.zeros_like(d))
+    return d, d.sum(0), d.abs().sum(0)
+
+
+def mlp_hidden(src: torch.Tensor, w16: torch.Tensor, b: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(relu(src w16 + b) before its bf16 store, sum of |terms|): one hidden layer, src / w16 the bf16 operands."""
+    s, w = src.to(F64), w16.to(F64)
+    return torch.clamp(s @ w + b.to(F64), min=0.0), s.abs() @ w.abs() + b.to(F64).abs()
+
+
+def mlp_dgrad(dh: torch.Tensor, w16: torch.Tensor, h: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
+    """(d pre-activation of the layer below, before its bf16 store and with the ReLU mask of ``h``, sum of |terms|):
+    dh [B,out] times the bf16 shadow w16 [in,out] transposed."""
+    d, w = dh.to(F64), w16.to(F64)
+    on = h.to(F64) > 0
+    z = torch.zeros(1, dtype=F64, device=d.device)
+    return torch.where(on, d @ w.t(), z), torch.where(on, d.abs() @ w.abs().t(), z)
+
+
+def mlp_step_f64(p: Dict[str, torch.Tensor], pb: Dict[str, torch.Tensor], images: torch.Tensor, labels: torch.Tensor,
+                 n_layers: int) -> Dict[str, object]:
+    """Float64 MLP step with the engine's storage roundings: the input through RNE to bf16, hidden layers on the bf16
+    shadow ``pb`` with bias and ReLU and a bf16 store, the output layer on the fp32 weights ``p``, data gradients on the
+    shadow with a bf16 store and then the mask, weight / bias gradients from those stored operands."""
+    B = images.shape[0]
+    src = rne_bf16(images.reshape(B, -1))
+    hs = []
+    for i in range(1, n_layers):
+        src = rne_bf16(mlp_hidden(src, pb["fc%d_weights" % i], p["fc%d_biases" % i])[0])
+        hs.append(src)
+    out = dense10_xent(src, p["fc%d_weights" % n_layers], p["fc%d_biases" % n_layers], labels)
+    g = {"fc%d_weights" % n_layers: src.t() @ rne_bf16(out["dl"]), "fc%d_biases" % n_layers: out["dl"].sum(0)}
+    d = rne_bf16(out["dh"])
+    for i in range(n_layers - 1, 0, -1):
+        below = hs[i - 2] if i > 1 else rne_bf16(images.reshape(B, -1))
+        g["fc%d_biases" % i] = d.sum(0)
+        g["fc%d_weights" % i] = below.t() @ d
+        if i > 1:
+            d = rne_bf16(mlp_dgrad(d, pb["fc%d_weights" % i], hs[i - 2])[0])
+    out.update(h=hs, grads=g, loss=out["loss_terms"].mean(), acc=out["hits"].to(F64).mean())
+    return out

@@ -1,7 +1,7 @@
-"""Numerics self-checks of the sm_90a LeNet kernels against float64 references (``ops/refs.py``).
+"""Numerics self-checks of the sm_90a LeNet and MLP kernels against float64 references (``ops/refs.py``).
 
-Each check returns ``(name, error, tolerance)`` tuples; ``tests/test_lenet_kernels_gpu.py`` and
-``tests/test_kernel_refs_gpu.py`` assert on them and ``tools/gpu_diag_lenet.py`` prints them all (one GPU call gives the
+Each check returns ``(name, error, tolerance)`` tuples; ``tests/test_lenet_kernels_gpu.py``,
+``tests/test_kernel_refs_gpu.py`` and ``tests/test_mlp_kernels_gpu.py`` assert on them and ``tools/gpu_diag_lenet.py`` prints them all (one GPU call gives the
 full picture when bringing a kernel up).  Every kernel-level check runs on exact-grid data (bitwise comparisons) and on
 continuous random data (precision bounds); see ``refs.py`` for the rule.  ``stale_B`` runs a slot-reduced kernel at
 that batch first, so the check's own launch finds stale partial sums in the workspace and a ticket last reset by a
@@ -10,11 +10,13 @@ launch with a different CTA count.
 from __future__ import annotations
 
 import ctypes
-from typing import Dict, List, Sequence, Tuple
+from typing import Dict, List, Optional, Sequence, Tuple
 
+import numpy as np
 import torch
 
 from ..models import dropout_keep_mask, dropout_seed_mix, get_model, lenet_forward, loss_and_accuracy
+from ..models.lenet import dropout_threshold
 from ..parallel.context import ReplicaContext
 from ..parallel.fused import FusedBackend
 from . import gemm as G
@@ -364,20 +366,52 @@ def _fc2_results(tag: str, kind: str, o: Dict[str, torch.Tensor], ref: Dict[str,
     return res
 
 
-def check_fc2_loss(B: int = 64, seed: int = 4, stale_B: int = 0) -> List[Result]:
-    """fc2_fwd_bwd on three hand-made split-K partials, then fc2_wgrad on what it saved (continuous data)."""
+_M32 = 0xFFFFFFFF
+_GOLDEN, _STEP_MIX = 0x9E3779B1, 0x9E3779B9        # csrc/common.cuh hash_mix, csrc/lenet_simt.cu per-step seed
+
+
+def _unhash(u: int) -> int:
+    """Inverse of the murmur3 32-bit finaliser in ``hash_mix``: the x with fmix32(x) == u (each step is a bijection)."""
+    x = u ^ (u >> 16)
+    x = (x * pow(0xC2B2AE35, -1, 1 << 32)) & _M32
+    x ^= (x >> 13) ^ (x >> 26)
+    x = (x * pow(0x85EBCA6B, -1, 1 << 32)) & _M32
+    return x ^ (x >> 16)
+
+
+def check_fc2_loss(B: int = 64, seed: int = 4, stale_B: int = 0, keep_prob: float = 0.5,
+                   probe: Optional[int] = None) -> List[Result]:
+    """fc2_fwd_bwd on three hand-made split-K partials, then fc2_wgrad on what it saved (continuous data).  The keep
+    pattern of the dropout must match the host mask exactly.  ``probe`` = -1 / 0 / +1: the seed is chosen so that one
+    element (with a positive pre-activation) hashes to exactly threshold - 1 / threshold / threshold + 1, the values
+    where an off-by-one threshold on either side changes the decision."""
     g = _gen(seed)
     h_pre = torch.randn(B, 512, generator=g)
     b1, w2, b2, labels = _fc2_inputs("rand", g, B)
+    step, mix0 = 7, dropout_seed_mix(123, 0, 2)
+    thresh = dropout_threshold(keep_prob)
+    if probe is not None:
+        r, j = B // 2, 77
+        h_pre[r, j] = h_pre[r, j].abs() + 1.0 + b1[j].abs()
+        target = thresh + probe
+        assert 0 <= target < 1 << 24, "threshold %d + %d is not a 24-bit hash value" % (thresh, probe)
+        mix = (_unhash((target << 8) | 0x5A) - (r * 512 + j) * _GOLDEN) & _M32
+        mix0 = (mix - step * _STEP_MIX) & _M32
+    mix = (mix0 + step * _STEP_MIX) & _M32
     h_pre, b1, w2, b2, labels = _dev(h_pre, b1, w2, b2, labels)
     parts = torch.stack([h_pre * 0.5, h_pre * 0.25, h_pre * 0.25]).contiguous()   # exact split of h_pre
-    mix = dropout_seed_mix(123, 7, 2)
     if stale_B:
         prime_workspace("fc2_fwd_bwd", stale_B)
-    o = run_fc2_fwd_bwd(parts, b1, w2, b2, labels, True, dropout_seed_mix(123, 0, 2), 7, 0.5)
-    keep = dropout_keep_mask(mix, B, 512, 0.5, device="cuda")
-    ref = R.fc2_fwd_bwd(h_pre, b1, w2, b2, labels, keep, 0.5)
+    o = run_fc2_fwd_bwd(parts, b1, w2, b2, labels, True, mix0, step, keep_prob)
+    keep = dropout_keep_mask(mix, B, 512, keep_prob, device="cuda")
+    ref = R.fc2_fwd_bwd(h_pre, b1, w2, b2, labels, keep, keep_prob)
     res = _fc2_results("fc2.rand", "rand", o, ref, w2, B, True)
+    # the keep pattern, exactly: apart from pre-activations within fp32 rounding of zero, h != 0 iff ReLU and the mask keep
+    hp, ha = h_pre.double() + b1.double(), h_pre.double().abs() + b1.double().abs()
+    settled = hp.abs() > 4 * R.FP32_UNIT * ha
+    res.append(("fc2.keep_pattern(keep=%g)" % keep_prob, float((((o["h"] != 0) != (ref["h"] != 0)) & settled).sum()), 0.0))
+    if probe is not None:
+        res.append(("fc2.probe(thresh%+d)_decision" % probe, float(bool(o["h"][r, j] != 0) != (probe < 0)), 0.0))
     gw2, gb2, gb1 = run_fc2_wgrad(o["h"], o["dl"], o["dh"])
     rw2, rb2, rb1 = R.fc2_wgrad(o["h"], o["dl"], o["dh"])
     return res + R.cmp_fp32("fc2_wgrad.g_w2", gw2, rw2) + R.cmp_fp32("fc2_wgrad.g_b2", gb2, rb2) + \
@@ -669,19 +703,24 @@ def check_evaluate(B: int = 1000, n: int = 2500, seed: int = 23) -> List[Result]
     loss, acc = eng.evaluate(x.numpy(), y.numpy())
     xd, yd = x.cuda(), y.cuda()
     ref = lenet_eval_f64(eng.p, eng.pb, xd, yd)
-    lg = ref["logits"]
     # the kernels' logits, batch by batch as evaluate() runs them
     got = torch.cat([eng.forward_logits(xd[s:s + B], yd[s:s + B], False) for s in range(0, n, B)]).double()
+    return _eval_results("evaluate", loss, acc, got, ref, yd)
+
+
+def _eval_results(tag: str, loss: float, acc: float, got: torch.Tensor, ref: Dict[str, torch.Tensor], yd) -> List[Result]:
+    """evaluate()'s (loss, accuracy) and the kernels' logits ``got`` vs a float64 forward ``ref`` (see the bounds above)."""
+    lg, n = ref["logits"], yd.shape[0]
     dev = (got - lg).abs().max(dim=1).values
     dev_rel = float((dev / (1.0 + lg.abs().max(dim=1).values)).max())
     near = ref["gap"] <= 2 * float(dev.max())            # argmax may differ only here
     hits = (lg.argmax(dim=1) == yd) & ~near
     lo, hi = float(hits.sum()) / n, float((hits | near).sum()) / n
     acc_excess = max(lo - acc, acc - hi, 0.0) * n
-    return [("evaluate.logit_deviation(rel)", dev_rel, EVAL_LOGIT_BOUND),
-            ("evaluate.loss(rel)", abs(loss - float(ref["loss"])) / float(ref["loss"]), EVAL_LOSS_REL),
-            ("evaluate.acc(rows outside near-ties)", acc_excess, 1e-6),
-            ("evaluate.near_tie_fraction", float(near.sum()) / n, EVAL_MAX_NEAR_TIES)]
+    return [(tag + ".logit_deviation(rel)", dev_rel, EVAL_LOGIT_BOUND),
+            (tag + ".loss(rel)", abs(loss - float(ref["loss"])) / float(ref["loss"]), EVAL_LOSS_REL),
+            (tag + ".acc(rows outside near-ties)", acc_excess, 1e-6),
+            (tag + ".near_tie_fraction", float(near.sum()) / n, EVAL_MAX_NEAR_TIES)]
 
 
 def check_training_reduces_loss(B: int = 128, steps: int = 40) -> List[Result]:
@@ -738,7 +777,303 @@ def check_mlp2_end_to_end() -> List[Result]:
     return check_mlp_end_to_end("mlp2", B=96, hidden=128, seed=22)
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# MLP kernels (csrc/mlp_simt.cu, the input conversion) and the MLP step, stage by stage
+# ---------------------------------------------------------------------------------------------------------------------
+XN_PAD = 64
+SENTINEL = 7.0          # prefilled into every output buffer: an element a kernel should write but does not stays 7
+
+
+def _randint(g: torch.Generator, shape, lo: int, hi: int, denom: int = 1) -> torch.Tensor:
+    """:func:`refs.grid` on the generator's own device (the large MLP shapes are generated on the GPU)."""
+    return torch.randint(lo, hi + 1, tuple(shape), generator=g, device=g.device).to(torch.float32) / denom
+
+
+def run_dense10_xent(h, w, b, labels, train: bool, g_b0, la0, logits: bool = True) -> Dict[str, torch.Tensor]:
+    """One dense10_xent launch.  dh, dl_pad and logits start as SENTINEL; g_b and loss_acc start at g_b0 / la0 (the
+    kernel adds to them)."""
+    B, H = h.shape
+    dev = h.device
+    o = dict(dh=torch.full((B, H), SENTINEL, dtype=BF, device=dev), dl_pad=torch.full((B, XN_PAD), SENTINEL, dtype=BF, device=dev),
+             g_b=g_b0.clone(), la=la0.clone(), logits=torch.full((B, 10), SENTINEL, device=dev) if logits else None)
+    check(load().dm_dense10_xent(ptr(h), ptr(w), ptr(b), ptr(labels), ptr(o["dh"]), ptr(o["dl_pad"]), ptr(o["g_b"]),
+                                 ptr(o["la"]), ptr(o["logits"]), B, H, int(train), stream_ptr()), "dense10_xent")
+    return o
+
+
+def run_relu_bwd_colsum(dh, h, mode: str, g0) -> Tuple[Optional[torch.Tensor], torch.Tensor]:
+    """``mode``: "inplace" (dpre = dh, the engine's use), "out" (a separate SENTINEL-filled dpre) or "none" (h = null: no
+    store, column sums of dh only).  Returns (dpre or None, g_bias started at g0)."""
+    B, H = dh.shape
+    g = g0.clone()
+    if mode == "none":
+        d, hp = None, None
+    elif mode == "inplace":
+        d, hp = dh.clone(), h
+    else:
+        d, hp = torch.full_like(dh, SENTINEL), h
+    src = d if mode == "inplace" else dh
+    check(load().dm_relu_bwd_colsum(ptr(src), ptr(hp), ptr(d), ptr(g), B, H, stream_ptr()), "relu_bwd_colsum")
+    return d, g
+
+
+def _dense10_data(kind: str, g: torch.Generator, B: int, H: int):
+    """(h bf16 [B,H], w fp32 [H,10], b [10], labels [B]).  Rows 1 mod 5 carry logits near +80 and rows 3 mod 5 near -80
+    (hidden units H-1 / H-2 at 64, weights of magnitude 1 .. 1.5): exp overflows / underflows there unless the row
+    maximum is subtracted first.  Grid data: h = k/8 in [0, 2] (about half exact zeros), w = k/64; classes 3 and 7 have
+    identical weights and bias, so they tie exactly in every row and the first-max rule decides the accuracy wherever
+    they lead (the even rows are labelled 3: a hit for the first maximum, a miss for the last)."""
+    dev = g.device
+    rows = torch.arange(B, device=dev)
+    if kind == "grid":
+        h = _randint(g, (B, H), 0, 16, 8) * (torch.rand(B, H, generator=g, device=dev) < 0.5)
+        w = _randint(g, (H, 10), -8, 8, 64)
+        b = _randint(g, (10,), -16, 16, 64)
+        big = _randint(g, (10,), 64, 96, 64)
+    else:
+        h = torch.relu(torch.randn(B, H, generator=g, device=dev))
+        w = torch.randn(H, 10, generator=g, device=dev) * 0.05
+        b = torch.randn(10, generator=g, device=dev) * 0.1
+        big = 1.0 + 0.5 * torch.rand(10, generator=g, device=dev)
+    h[:, H - 1] = torch.where(rows % 5 == 1, torch.full_like(h[:, 0], 64.0), h[:, H - 1])
+    h[:, H - 2] = torch.where(rows % 5 == 3, torch.full_like(h[:, 0], 64.0), h[:, H - 2])
+    w[H - 1], w[H - 2] = big, -big
+    labels = torch.randint(0, 10, (B,), generator=g, device=dev)
+    if kind == "grid":
+        w[:, 7] = w[:, 3]
+        b[3] = b[7] = 0.25
+        labels = torch.where(rows % 2 == 0, torch.full_like(labels, 3), labels)
+    return h.to(BF), w, b, labels
+
+
+def _dense10_results(tag: str, kind: str, o: Dict[str, Optional[torch.Tensor]], h, w, b, labels, g_b0, la0, train: bool,
+                     logit_unit: float, pad_value: float = SENTINEL) -> List[Result]:
+    """dense10_xent outputs vs :func:`refs.dense10_xent`.  Logits: exact on grid data (the premise is asserted), within
+    the fp32 bound otherwise.  Loss, dl, g_b and dh go through exp / log: bounded on both kinds (bf16 ones by
+    :func:`refs.cmp_bf16_bound`; masked dh elements must be exactly zero).  Accuracy: exact on grid
+    data and for a power-of-two B (every partial sum of 1/B terms is an fp32 number), else within the fp32 sum bound;
+    on continuous data rows whose top two logits are within twice the logit bound may go either way.  ``pad_value``: what
+    dl_pad columns 16..63 held before the launch (the kernel never writes them)."""
+    B = h.shape[0]
+    ref = R.dense10_xent(h, w, b, labels)
+    res: List[Result] = []
+    grid = kind == "grid"
+    if grid:
+        R.assert_exact_grid(ref["logit_abs"], logit_unit, tag + ".logits")
+    if o.get("logits") is not None:
+        res += R.cmp_bound(tag + ".logits", o["logits"], ref["logits"], 0.0 if grid else ref["logit_err"][:, None])
+    la, la0 = o["la"].double(), la0.double()
+    inv = float(np.float32(1.0) / np.float32(B))                        # the host's 1.f / B
+    terms = ref["loss_terms"] / B
+    res += R.cmp_bound(tag + ".loss", la[0], la0[0] + terms.sum(),
+                       ref["term_err"].sum() + R.fp32_slack(la0[0].abs() + terms.abs().sum(), B + 1))
+    near = torch.zeros_like(ref["hits"]) if grid else ref["gap"] <= 2 * ref["logit_err"]
+    lo, hi = float((ref["hits"] & ~near).sum()), float((ref["hits"] | near).sum())
+    acc_bound = 0.0 if B & (B - 1) == 0 else float(R.fp32_slack(la0[1].abs() + hi * inv, B + 1))
+    a, a0 = float(la[1]), float(la0[1])
+    res.append((tag + ".acc", max(a0 + lo * inv - a, a - a0 - hi * inv, 0.0), acc_bound))
+    if not train:
+        untouched = (o["dh"].double() != SENTINEL).sum() + (o["dl_pad"].double() != SENTINEL).sum() + (o["g_b"] != g_b0).sum()
+        return res + [(tag + ".eval_wrote(dh,dl_pad,g_b)", float(untouched), 0.0)]
+    dl_pad = o["dl_pad"]
+    res += R.cmp_bf16_bound(tag + ".dl_pad", dl_pad[:, :10], ref["dl"], ref["dl_err"])
+    res.append((tag + ".dl_pad[10:16]_nonzero", float((dl_pad[:, 10:16].double() != 0).sum()), 0.0))
+    res.append((tag + ".dl_pad[16:]_changed", float((dl_pad[:, 16:].double() != pad_value).sum()), 0.0))
+    res += R.cmp_bound(tag + ".g_b", o["g_b"], g_b0.double() + ref["dl"].sum(0),
+                       ref["dl_err"].sum(0) + R.fp32_slack(g_b0.double().abs() + ref["dl"].abs().sum(0), B + 1))
+    # dh = sum_c dl_c w[j,c]: the dl error through w, the 10-term fp32 sum, a result flushed below 2^-126
+    wa = w.double().abs()
+    dh_bound = ref["dl_err"] @ wa.t() + R.fp32_slack(ref["dl"].abs() @ wa.t(), 10) + R.FTZ
+    res += R.cmp_bf16_bound(tag + ".dh", o["dh"], ref["dh"], torch.where(ref["on"], dh_bound, torch.zeros_like(dh_bound)))
+    res.append((tag + ".dh.relu_mask", float(((o["dh"].double() != 0) & ~ref["on"]).sum()), 0.0))
+    return res
+
+
+def check_dense10_xent(B: int = 1000, H: int = 192, seed: int = 60, kinds: Sequence[str] = KINDS,
+                       train: bool = True) -> List[Result]:
+    """dense10_xent at batch B, width H: sentinel-filled outputs, non-zero starting g_b and loss_acc."""
+    res: List[Result] = []
+    for kind in kinds:
+        tag = "dense10_xent.%s.B%d.H%d.%s" % (kind, B, H, "train" if train else "eval")
+        g = torch.Generator(device="cuda").manual_seed(seed)
+        h, w, b, labels = _dense10_data(kind, g, B, H)
+        g_b0 = _randint(g, (10,), -16, 16, 64)
+        la0 = torch.tensor([0.5, 0.25], device="cuda")
+        o = run_dense10_xent(h, w, b, labels, train, g_b0, la0)
+        res += _dense10_results(tag, kind, o, h, w, b, labels, g_b0, la0, train, 1.0 / 512)
+        if kind == "grid" and B >= 64:          # the data must hold the ties it is for
+            ref_gap = R.dense10_xent(h, w, b, labels)["gap"]
+            ties = int(((ref_gap == 0) & (labels == 3)).sum())
+            res.append((tag + ".tie_rows_missing", float(ties == 0), 0.0))
+    return res
+
+
+def _colsum_data(kind: str, g: torch.Generator, B: int, H: int):
+    """(dh bf16, h bf16).  h holds exact +0 and -0 (masked) and 2^-126, the smallest normal bf16 (kept), at fixed
+    positions where dh is 1.  (The kernels run with flush-to-zero, and no stage produces a subnormal activation.)"""
+    dev = g.device
+    if kind == "grid":
+        dh, h = _randint(g, (B, H), -64, 64, 64), _randint(g, (B, H), -2, 2)
+    else:
+        dh, h = torch.randn(B, H, generator=g, device=dev) * 0.1, torch.randn(B, H, generator=g, device=dev)
+    flat_dh, flat_h = dh.view(-1), h.view(-1)
+    for k, v in enumerate((0.0, -0.0, 2.0 ** -126)):
+        flat_h[k::7] = v
+        flat_dh[k::7] = 1.0
+    return dh.to(BF), h.to(BF)
+
+
+def _colsum_results(tag: str, kind: str, dh, h, mode: str, dpre, g, g0) -> List[Result]:
+    """dpre: the selection, exact.  g_bias = g0 + column sums of dpre: exact on grid data, fp32-bounded otherwise."""
+    rd, rs, ra = R.relu_bwd_colsum(dh, None if mode == "none" else h)
+    res: List[Result] = []
+    if dpre is not None:
+        res += R.cmp_exact(tag + ".dpre", dpre, rd)
+    ref, a = g0.double() + rs, g0.double().abs() + ra
+    if kind == "grid":
+        R.assert_exact_grid(a, 1.0 / 64, tag + ".g_bias")
+        res += R.cmp_exact(tag + ".g_bias", g, ref)
+    else:
+        res += R.cmp_bound(tag + ".g_bias", g, ref, R.fp32_slack(a, dh.shape[0] + 1))
+    return res
+
+
+def check_relu_bwd_colsum(B: int = 257, H: int = 66, seed: int = 61, kinds: Sequence[str] = KINDS,
+                          modes: Sequence[str] = ("inplace", "out", "none")) -> List[Result]:
+    """relu_bwd_colsum, masked in place, masked into a separate buffer and unmasked (h = null), from a non-zero g_bias."""
+    res: List[Result] = []
+    for kind in kinds:
+        g = torch.Generator(device="cuda").manual_seed(seed)
+        dh, h = _colsum_data(kind, g, B, H)
+        g0 = _randint(g, (H,), -16, 16, 64)
+        if kind == "grid" and B * H >= 3:   # the data must hold its edge values
+            on = (h.view(-1)[:3].double() > 0).tolist()
+            res.append(("relu_bwd_colsum.edges(+0,-0,min_normal)", float(on != [False, False, True]), 0.0))
+        for mode in modes:
+            d, gb = run_relu_bwd_colsum(dh, h, mode, g0)
+            res += _colsum_results("relu_bwd_colsum.%s.B%d.H%d.%s" % (kind, B, H, mode), kind, dh, h, mode, d, gb, g0)
+    return res
+
+
+def check_f32_to_bf16(B: int = 3, seed: int = 62) -> List[Result]:
+    """dm_f32_to_bf16 on B images' worth of values (n = 784 B): bit for bit round-to-nearest-even.  Random finite normal
+    fp32 bit patterns and +-0; a quarter of them exact ties (low half 0x8000), a quarter one below / above a tie."""
+    n = B * 784
+    g = _gen(seed)
+    hi = torch.randint(0, 1 << 16, (n,), generator=g, dtype=torch.int64)
+    lo = torch.randint(0, 1 << 16, (n,), generator=g, dtype=torch.int64)
+    lo[0::4] = 0x8000
+    lo[1::4] = torch.where(lo[1::4] < 0x8000, torch.full_like(lo[1::4], 0x7FFF), torch.full_like(lo[1::4], 0x8001))
+    e = (hi >> 7) & 0xFF
+    hi = torch.where((e == 0) | (e == 0xFF), (hi & 0x807F) | (127 << 7), hi)     # no subnormals, infinities or NaNs
+    hi[:2], lo[:2] = torch.tensor([0x0000, 0x8000]), 0                            # +0, -0
+    bits = (hi << 16) | lo
+    x = torch.where(bits >= 1 << 31, bits - (1 << 32), bits).to(torch.int32).view(torch.float32)
+    xd = x.cuda()
+    out = torch.full((n,), SENTINEL, dtype=BF, device="cuda")
+    check(load().dm_f32_to_bf16(ptr(xd), ptr(out), ctypes.c_longlong(n), stream_ptr()), "f32_to_bf16")
+    want = x.to(BF).view(torch.int16)
+    return [("f32_to_bf16.n%d.bits_differ" % n, float((out.cpu().view(torch.int16) != want).sum()), 0.0)]
+
+
+def _mlp_engine(model: str, B: int, hidden: int, seed: int):
+    from ..engine_cuda import CudaMlpEngine
+    ctx = ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none")
+    return CudaMlpEngine(model, B, FusedBackend(ctx), hidden=hidden, seed=seed, use_graph=False)
+
+
+def _dgrad_results(tag: str, dh_in, w16, h, dh_out, g_bias, g_bias0) -> List[Result]:
+    """A hidden layer's data gradient: dh_out = mask_h(RNE(dh_in w16^T)) on the bf16 shadow w16 (one ulp, with the fp32
+    sum bound as slack; masked elements exactly zero), then g_bias = g_bias0 + column sums of the stored dh_out."""
+    ref, ra = R.mlp_dgrad(dh_in, w16, h)
+    res = R.cmp_bf16(tag, dh_out, ref, R.fp32_slack(ra, dh_in.shape[1]) + 2.0 ** -23 * ref.abs())
+    res.append((tag + ".relu_mask", float(((dh_out.double() != 0) & (h.double() <= 0)).sum()), 0.0))
+    _, cs, ca = R.relu_bwd_colsum(dh_out, None)
+    return res + R.cmp_bound(tag + ".g_bias", g_bias, g_bias0.double() + cs,
+                             R.fp32_slack(ca + g_bias0.double().abs(), dh_out.shape[0] + 1))
+
+
+def _mlp_step_results(tag: str, kind: str, eng, images, labels) -> List[Result]:
+    """One ``forward_backward`` of a CudaMlpEngine, every stage against its float64 reference computed from the engine's
+    own input buffers for that stage (x16, h[i], dh[i], dl_pad, the shadow pb, the fp32 arena p): one stage's rounding
+    never loosens the next stage's bound, and bf16 inputs keep the forward stages exact on grid data.  Everything
+    downstream of the softmax is continuous on both kinds and held to fp32 bounds."""
+    p, pb, gr, L, B = eng.p, eng.pb, eng.g, eng.n_layers, eng.batch_size
+    res = R.cmp_exact(tag + ".x16", eng.x16, images)                       # RNE of the fp32 images
+    src = eng.x16
+    for i in range(1, L):
+        ref, ra = R.mlp_hidden(src, pb["fc%d_weights" % i], p["fc%d_biases" % i])
+        if kind == "grid":                      # images k/8, weights k/8, biases k/64
+            R.assert_exact_grid(ra, 2.0 ** -(3 + 3 * i), "%s.h%d" % (tag, i))
+        res += R.compare("%s.h%d" % (tag, i), kind, eng.h[i - 1], ref, R.fp32_slack(ra, src.shape[1] + 1) + 2.0 ** -23 * ref.abs())
+        src = eng.h[i - 1]
+    zeros = torch.zeros(10, device=src.device)
+    o = dict(dh=eng.dh[-1], dl_pad=eng.dl_pad, g_b=gr["fc%d_biases" % L], la=eng.d_loss_acc, logits=None)
+    res += _dense10_results(tag + ".dense10_xent", kind, o, src, p["fc%d_weights" % L], p["fc%d_biases" % L], labels,
+                            zeros, zeros[:2], True, 2.0 ** -(3 + 3 * L), pad_value=0.0)
+    dl = eng.dl_pad[:, :10].double()
+    res += R.cmp_bound("%s.g_fc%d_weights" % (tag, L), gr["fc%d_weights" % L], src.double().t() @ dl,
+                       R.fp32_slack(src.double().abs().t() @ dl.abs(), B))
+    _, cs, ca = R.relu_bwd_colsum(eng.dh[-1], None)
+    res += R.cmp_bound("%s.g_fc%d_biases" % (tag, L - 1), gr["fc%d_biases" % (L - 1)], cs, R.fp32_slack(ca, B + 1))
+    for i in range(L - 1, 0, -1):
+        below = eng.h[i - 2] if i > 1 else eng.x16
+        d = eng.dh[i - 1].double()
+        res += R.cmp_bound("%s.g_fc%d_weights" % (tag, i), gr["fc%d_weights" % i], below.double().t() @ d,
+                           R.fp32_slack(below.double().abs().t() @ d.abs(), B))
+        if i > 1:
+            res += _dgrad_results("%s.dh%d" % (tag, i - 1), eng.dh[i - 1], pb["fc%d_weights" % i], eng.h[i - 2],
+                                  eng.dh[i - 2], gr["fc%d_biases" % (i - 1)], zeros[:1])
+    res.append((tag + ".grad_padding", float(eng.grads[~eng.spec.valid_mask().to(eng.grads.device)].abs().max()), 0.0))
+    return res
+
+
+def check_mlp_step(model: str = "mlp3", B: int = 96, hidden: int = 192, seed: int = 63,
+                   kinds: Sequence[str] = KINDS) -> List[Result]:
+    """CudaMlpEngine.forward_backward, stage by stage.  Grid data: the parameters are overwritten with grid values
+    (weights k/8 in [-1, 1], biases k/64) and the shadow refreshed; continuous data: the engine's own initialisation."""
+    res: List[Result] = []
+    for kind in kinds:
+        eng = _mlp_engine(model, B, hidden, seed)
+        g = _gen(seed)
+        if kind == "grid":
+            for name, t in eng.p.items():
+                t.copy_(R.grid(g, t.shape, -1, 1, 8) if name.endswith("weights") else R.grid(g, t.shape, -16, 16, 64))
+            eng.params_updated()
+            x = R.grid(g, (B, 784), -4, 4, 8)
+        else:
+            x = torch.rand(B, 784, generator=g) - 0.5
+        y = torch.randint(0, 10, (B,), generator=g)
+        eng.load_batch(x.numpy(), y.numpy())
+        eng.forward_backward(0)
+        torch.cuda.synchronize()
+        res += _mlp_step_results("mlp_step.%s.B%d.H%d.%s" % (model, B, hidden, kind), kind, eng, x.cuda(), y.cuda())
+        del eng
+    return res
+
+
+def check_mlp_evaluate(model: str = "mlp3", hidden: int = 1024, B: int = 1000, n: int = 2500, seed: int = 64) -> List[Result]:
+    """``CudaMlpEngine.evaluate`` (the evaluator's batch 1000; the last batch is partial) vs :func:`refs.mlp_step_f64`."""
+    eng = _mlp_engine(model, B, hidden, seed)
+    g = _gen(seed)
+    x = mnist_like(g, n).reshape(n, 784)
+    y = torch.randint(0, 10, (n,), generator=g)
+    loss, acc = eng.evaluate(x.numpy(), y.numpy())
+    xd, yd = x.cuda(), y.cuda()
+    ref = R.mlp_step_f64(eng.p, eng.pb, xd, yd, eng.n_layers)
+    got = []
+    with torch.no_grad():
+        for s in range(0, n, B):               # the kernels' logits, batch by batch as evaluate() runs them
+            m = min(B, n - s)
+            out = torch.full((m, 10), SENTINEL, device="cuda")
+            eng.d_loss_acc.zero_()
+            eng._forward(xd[s:s + m].contiguous(), yd[s:s + m].contiguous(), m, False, logits_out=out)
+            got.append(out)
+    return _eval_results("mlp_evaluate", loss, acc, torch.cat(got).double(), ref, yd)
+
+
 ALL_CHECKS = [check_conv1_fwd, check_conv1_wgrad, check_conv2_fwd, check_conv2_dgrad, check_conv2_wgrad, check_fc2_loss, check_fc1_fwd, check_fc2_wgrad, check_fc1_wgrad, check_fc1_dgrad_unpool,
               check_evaluate,
               check_end_to_end, check_bucketed_step_matches_single_kernel, check_bucketed_mlp_step_matches_single_kernel,
-              check_training_reduces_loss, check_mlp_end_to_end, check_mlp2_end_to_end]
+              check_training_reduces_loss, check_mlp_end_to_end, check_mlp2_end_to_end,
+              check_dense10_xent, check_relu_bwd_colsum, check_f32_to_bf16, check_mlp_step, check_mlp_evaluate]

@@ -116,6 +116,17 @@ def test_gemm_n10_ldo10_output_layer_wgrad(kind):
 
 
 @pytest.mark.parametrize("kind", ["grid", "rand"])
+@pytest.mark.parametrize("M,N,K,a_mn,b_mn,epi", [
+    (4096, 4096, 8192, True, True, 0),      # hidden weight gradient h^T dh: K = batch, both operands MN-major
+    (8192, 4096, 4096, False, False, 2),    # data gradient dh W^T: K-major / K-major, bf16 store
+    (784, 4096, 8192, True, True, 0),       # fc1 weight gradient x^T dh: M = 784, a partial M tile
+])
+def test_gemm_mlp_batch_8192_shapes(kind, M, N, K, a_mn, b_mn, epi):
+    """The GEMMs of the 3-layer MLP step at batch 8192, width 4096 (bn = 256) that no other test runs, in full."""
+    _check(_gemm_case(kind, M, N, K, a_mn, b_mn, epi, 256, seed=M + K + epi))
+
+
+@pytest.mark.parametrize("kind", ["grid", "rand"])
 def test_gemm_lenet_shapes_at_batch_256(kind):
     """Every GEMM the LeNet engine issues at B=256: fc1 forward (strided split-K, checked per split by check_fc1_fwd),
     fc1 weight gradient fp32 / bf16, and the unfused fc1 data gradient."""

@@ -60,6 +60,13 @@ def test_fc2_fwd_bwd_after_stale_launch(B):
     _run("check_fc2_loss", B=B, seed=660 + B, stale_B=_stale(B))
 
 
+@pytest.mark.parametrize("keep_prob,probe", [(0.25, -1), (0.25, 0), (0.25, 1), (0.8, -1), (0.8, 0), (0.8, 1), (1.0, -1)])
+def test_fc2_dropout_threshold_edges(keep_prob, probe):
+    """One element hashed exactly to threshold - 1 / threshold / threshold + 1 (at keep 1.0 the threshold is 2^24, one
+    past every hash value).  0.8: fp32 rounds it up, so the kernel's threshold is one above floor(0.8 * 2^24)."""
+    _run("check_fc2_loss", B=64, seed=670, keep_prob=keep_prob, probe=probe)
+
+
 @pytest.mark.parametrize("B", BATCHES)
 def test_fc2_wgrad(B):
     _run("check_fc2_wgrad", B=B, seed=700 + B)

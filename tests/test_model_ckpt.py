@@ -57,6 +57,37 @@ def test_dropout_mask_rate_and_determinism():
     assert not torch.equal(m, dropout_keep_mask(0xDEADBEF0, 256, 512, 0.5))
 
 
+def test_dropout_threshold_is_the_kernels():
+    """The kernels compute (uint32_t)(keep_prob * 16777216.f) from an fp32 keep_prob; fp32 rounds 0.3, 0.8 and 0.99 up,
+    one unit above floor(keep_prob * 2^24)."""
+    import numpy as np
+    from distributedmnist_b200.models.lenet import dropout_threshold
+    from distributedmnist_b200.ops.selfcheck import _unhash
+    sweep = [k / 100 for k in range(101)] + [0.25, 0.3, 0.75, 0.8, 0.99, 1 / 3, 0.9999999, 1e-7]
+    for kp in sweep:
+        device = int(np.uint32(np.float32(kp) * np.float32(16777216.0)))
+        assert dropout_threshold(kp) == device, kp
+    assert [dropout_threshold(k) for k in (0.3, 0.8, 0.99)] == [5033165, 13421773, 16609444]
+
+
+def test_dropout_mask_decides_at_the_kernels_threshold():
+    """An element whose hash lands one below the kernel's threshold is kept (floor(0.8 * 2^24) would drop it), one
+    that lands on it is dropped."""
+    import numpy as np
+    from distributedmnist_b200.ops.selfcheck import _unhash
+    for kp in (0.3, 0.8, 0.99):
+        t = int(np.uint32(np.float32(kp) * np.float32(16777216.0)))
+        for v, kept in ((t - 1, True), (t, False)):
+            mix = _unhash((v << 8) | 0xA5)           # element 0: hash_mix(mix, 0) = fmix32(mix)
+            assert bool(dropout_keep_mask(mix, 1, 1, kp)[0, 0]) == kept, (kp, v)
+
+
+def test_mlp_engine_refuses_a_hidden_width_its_output_kernel_cannot_hold():
+    from distributedmnist_b200.engine_cuda import CudaMlpEngine
+    with pytest.raises(ValueError, match="--mlp_hidden=5184"):
+        CudaMlpEngine("mlp3", 8, None, hidden=5184)
+
+
 @pytest.mark.parametrize("name", ["mlp2", "mlp3"])
 def test_mlp_specs(name):
     spec, fwd = get_model(name, mlp_hidden=64)
