@@ -110,6 +110,13 @@ int dm_runner_wait(void* h, int slot) {
   return (int)cudaEventSynchronize(r->slot_free[slot & 1]);
 }
 
+// Block the calling host thread until the input DMA (and gather) last enqueued for `slot` has completed: its host source
+// may then be rewritten or freed.
+int dm_runner_wait_copy(void* h, int slot) {
+  dm::StepRunner* r = reinterpret_cast<dm::StepRunner*>(h);
+  return (int)cudaEventSynchronize(r->copy_done[slot & 1]);
+}
+
 // 1: that step has completed, 0: still running, < 0: error.
 int dm_runner_query(void* h, int slot) {
   dm::StepRunner* r = reinterpret_cast<dm::StepRunner*>(h);

@@ -178,6 +178,9 @@ class _CudaEngine(ComputeEngine):
             hi, hl = images.view(self.images[0].shape), labels
         else:
             hi, hl = self.h_images[s], self.h_labels[s]
+            # the DMA of this buffer's previous fill waits for the step two loads back: it must have run before the host
+            # overwrites the buffer (returns at once unless the caller enqueues steps without ever waiting for one)
+            self._copy_done[s].synchronize()
             if isinstance(images, np.ndarray):
                 hi.copy_(torch.from_numpy(images).view(hi.shape))
                 hl.copy_(torch.from_numpy(labels))
@@ -257,6 +260,7 @@ class _CudaEngine(ComputeEngine):
         t = self._as_indices(idx)
         s = self._loaded & 1
         h = self._h_idx[s]
+        self._copy_done[s].synchronize()                 # the previous fill's DMA has read h (see load_batch)
         h.copy_(t)
         with self._filling(s):
             self._idx_dev[s].copy_(h, non_blocking=True)
@@ -276,7 +280,12 @@ class _CudaEngine(ComputeEngine):
                 self.train_step()
                 return self.read_result_async()
         if not t.is_pinned():
-            t = t.pin_memory()
+            # into the slot's page-locked staging buffer, once the DMA of its previous fill has read it (a fresh pinned copy
+            # per call would go back to torch's host allocator, and be handed out again, while its DMA may still wait)
+            s = self._loaded & 1
+            check(self.lib.dm_runner_wait_copy(r, s), "runner_wait_copy")
+            self._h_idx[s].copy_(t)
+            t = self._h_idx[s]
         s = int(self.lib.dm_runner_step_indices(r, ctypes.c_void_p(t.data_ptr())))
         if s < 0:
             raise RuntimeError("dm_runner_step_indices failed: CUDA error %d" % -s)

@@ -231,6 +231,16 @@ def _pool_results(tag: str, kind: str, out, code, z, za, bias, n_terms: int) -> 
     return res + R.cmp_pool(tag, "grid" if kind == "edges" else kind, code, ref, slack)
 
 
+def conv1_fwd_results(tag: str, kind: str, x, w, b, out, code) -> List[Result]:
+    """conv1_fwd's pooled output and codes from images x [B,28,28] fp32, weights w [5,5,1,32] fp32, bias b."""
+    x, w = x.to(BF), w.to(BF)       # the kernel rounds its operands to bf16 (grid values are bf16 numbers already)
+    z = R.conv5x5(x[..., None], w)
+    za = R.conv5x5(x.abs()[..., None], w.abs())
+    if kind != "rand":
+        R.assert_exact_grid(za + b.abs().double().max(), 1.0 / 512, tag)
+    return _pool_results(tag, kind, out, code, z, za, b, 25)
+
+
 def check_conv1_fwd(B: int = 8, seed: int = 0, kinds: Sequence[str] = KINDS) -> List[Result]:
     res: List[Result] = []
     for kind in kinds:
@@ -238,12 +248,7 @@ def check_conv1_fwd(B: int = 8, seed: int = 0, kinds: Sequence[str] = KINDS) -> 
         x, w, b = _conv1_data(kind, _gen(seed), B)
         x, w, b = _dev(x, w, b)
         out, code, junk = run_conv1_fwd(x, w, b)
-        x, w = x.to(BF), w.to(BF)       # the kernel rounds its operands to bf16 (grid values are bf16 numbers already)
-        z = R.conv5x5(x[..., None], w)
-        za = R.conv5x5(x.abs()[..., None], w.abs())
-        if kind != "rand":
-            R.assert_exact_grid(za + b.abs().double().max(), 1.0 / 512, tag)
-        res += _pool_results(tag, kind, out, code, z, za, b, 25)
+        res += conv1_fwd_results(tag, kind, x, w, b, out, code)
         res.append((tag + ".zeroing", float(junk.abs().max()), 0.0))
     return res
 
@@ -265,14 +270,27 @@ def check_conv1_wgrad(B: int = 8, seed: int = 7, kinds: Sequence[str] = KINDS, s
         if stale_B:
             prime_workspace("conv1_wgrad_tc", stale_B)
         gw, gb = run_conv1_wgrad(x, dp, code)
-        xr = x.to(BF)                       # the kernel rounds the images to bf16
-        rw, rb = R.conv1_wgrad(xr, dp, code)
-        if kind == "grid":
-            aw, ab = R.conv1_wgrad(xr.abs(), dp.abs(), code)
-            R.assert_exact_grid(aw, 1.0 / 8, tag + ".g_w")
-            R.assert_exact_grid(ab, 1.0, tag + ".g_b")
-        res += R.compare(tag + ".g_w", kind, gw, rw) + R.compare(tag + ".g_b", kind, gb, rb)
+        res += conv1_wgrad_results(tag, kind, x, dp, code, gw, gb)
     return res
+
+
+def conv1_wgrad_results(tag: str, kind: str, x, dp, code, gw, gb) -> List[Result]:
+    """conv1 weight [25,32] / bias gradients from images x [B,28,28] fp32, d pool1 output dp and pool1 codes."""
+    xr = x.to(BF)                       # the kernel rounds the images to bf16
+    rw, rb = R.conv1_wgrad(xr, dp, code)
+    if kind == "grid":
+        aw, ab = R.conv1_wgrad(xr.abs(), dp.abs(), code)
+        R.assert_exact_grid(aw, 1.0 / 8, tag + ".g_w")
+        R.assert_exact_grid(ab, 1.0, tag + ".g_b")
+    return R.compare(tag + ".g_w", kind, gw, rw) + R.compare(tag + ".g_b", kind, gb, rb)
+
+
+def conv2_fwd_results(tag: str, kind: str, a1, w, b, out, code) -> List[Result]:
+    """conv2_fwd's pooled output and codes [B,7,7,64] from a1 and the bf16 weights w."""
+    z, za = R.conv5x5(a1, w), R.conv5x5(a1.abs(), w.abs())
+    if kind != "rand":
+        R.assert_exact_grid(za + b.abs().double().max(), 1.0 / 64, tag)
+    return _pool_results(tag, kind, out, code, z, za, b, 800)
 
 
 def check_conv2_fwd(B: int = 8, seed: int = 1, kinds: Sequence[str] = KINDS) -> List[Result]:
@@ -281,11 +299,15 @@ def check_conv2_fwd(B: int = 8, seed: int = 1, kinds: Sequence[str] = KINDS) -> 
         tag = "conv2_fwd.%s" % kind
         a1, w, b = _dev(*_conv2_data(kind, _gen(seed), B))
         out, code = run_conv2_fwd(a1, w, b)
-        z, za = R.conv5x5(a1, w), R.conv5x5(a1.abs(), w.abs())
-        if kind != "rand":
-            R.assert_exact_grid(za + b.abs().double().max(), 1.0 / 64, tag)
-        res += _pool_results(tag, kind, out, code, z, za, b, 800)
+        res += conv2_fwd_results(tag, kind, a1, w, b, out, code)
     return res
+
+
+def conv2_dgrad_results(tag: str, kind: str, dy, w, dx) -> List[Result]:
+    ref, ra = R.conv5x5_dgrad(dy, w), R.conv5x5_dgrad(dy.abs(), w.abs())
+    if kind == "grid":
+        R.assert_exact_grid(ra, 1.0 / 64, tag)
+    return R.compare(tag, kind, dx, ref, R.fp32_slack(ra, 1600))
 
 
 def check_conv2_dgrad(B: int = 8, seed: int = 2, kinds: Sequence[str] = KINDS) -> List[Result]:
@@ -298,12 +320,15 @@ def check_conv2_dgrad(B: int = 8, seed: int = 2, kinds: Sequence[str] = KINDS) -
         else:
             dy, w = _bf(R.grid(g, (B, 14, 14, 64), -4, 4)), _bf(R.grid(g, (5, 5, 32, 64), -8, 8, 64))
         dy, w = _dev(dy, w)
-        dx = run_conv2_dgrad(dy, w)
-        ref, ra = R.conv5x5_dgrad(dy, w), R.conv5x5_dgrad(dy.abs(), w.abs())
-        if kind == "grid":
-            R.assert_exact_grid(ra, 1.0 / 64, tag)
-        res += R.compare(tag, kind, dx, ref, R.fp32_slack(ra, 1600))
+        res += conv2_dgrad_results(tag, kind, dy, w, run_conv2_dgrad(dy, w))
     return res
+
+
+def conv2_wgrad_results(tag: str, kind: str, a1, dy, gw) -> List[Result]:
+    ref = R.conv5x5_wgrad(a1, dy)
+    if kind == "grid":
+        R.assert_exact_grid(R.conv5x5_wgrad(a1.abs(), dy.abs()), 1.0, tag)
+    return R.compare(tag, kind, gw, ref)
 
 
 def check_conv2_wgrad(B: int = 8, seed: int = 3, kinds: Sequence[str] = KINDS, stale_B: int = 0) -> List[Result]:
@@ -318,11 +343,7 @@ def check_conv2_wgrad(B: int = 8, seed: int = 3, kinds: Sequence[str] = KINDS, s
         a1, dy = _dev(a1, dy)
         if stale_B:
             prime_workspace("conv2_wgrad", stale_B)
-        gw = run_conv2_wgrad(a1, dy)
-        ref = R.conv5x5_wgrad(a1, dy)
-        if kind == "grid":
-            R.assert_exact_grid(R.conv5x5_wgrad(a1.abs(), dy.abs()), 1.0, tag)
-        res += R.compare(tag, kind, gw, ref)
+        res += conv2_wgrad_results(tag, kind, a1, dy, run_conv2_wgrad(a1, dy))
     return res
 
 
@@ -340,13 +361,15 @@ def _fc2_results(tag: str, kind: str, o: Dict[str, torch.Tensor], ref: Dict[str,
     """fc2_fwd_bwd outputs.  logits and activations follow the data kind (exact on grid data, where the fc1 sum, bias,
     x2 dropout scale and fc2 products are all grid numbers).  Loss, d logits and d h go through exp/log (the kernel uses
     the fast __expf/__logf) and are compared by the continuous rule on both kinds.  The accuracy is exact, except for
-    rows whose top two reference logits are closer than the logits' fp32 error."""
+    rows whose top two reference logits are closer than the logits' fp32 error.  A training step stores no logits: with
+    ``o["logits"]`` None they are judged through the loss and the accuracy alone."""
     res: List[Result] = []
     la = o["la"].double()
     if kind == "grid":
         # h: fc1 sum + bias in units of 1/64, times 2 under dropout (keep 0.5); w2 in units of 1/64
         R.assert_exact_grid(ref["h"].abs() @ w2.abs().double() + 1, 1.0 / (2048 if train else 4096), tag + ".logits")
-    res += R.compare(tag + ".logits", kind, o["logits"], ref["logits"])
+    if o.get("logits") is not None:
+        res += R.compare(tag + ".logits", kind, o["logits"], ref["logits"])
     res += R.cmp_fp32(tag + ".loss", la[0:1], ref["loss"].reshape(1))
     lg_slack = R.fp32_slack(ref["h"].abs() @ w2.abs().double(), 512).max(dim=1).values
     ok = ref["gap"] > 2 * lg_slack
@@ -406,16 +429,37 @@ def check_fc2_loss(B: int = 64, seed: int = 4, stale_B: int = 0, keep_prob: floa
     keep = dropout_keep_mask(mix, B, 512, keep_prob, device="cuda")
     ref = R.fc2_fwd_bwd(h_pre, b1, w2, b2, labels, keep, keep_prob)
     res = _fc2_results("fc2.rand", "rand", o, ref, w2, B, True)
-    # the keep pattern, exactly: apart from pre-activations within fp32 rounding of zero, h != 0 iff ReLU and the mask keep
     hp, ha = h_pre.double() + b1.double(), h_pre.double().abs() + b1.double().abs()
-    settled = hp.abs() > 4 * R.FP32_UNIT * ha
-    res.append(("fc2.keep_pattern(keep=%g)" % keep_prob, float((((o["h"] != 0) != (ref["h"] != 0)) & settled).sum()), 0.0))
+    res += keep_pattern_results("fc2.keep_pattern(keep=%g)" % keep_prob, o["h"], ref["h"], hp, 4 * R.FP32_UNIT * ha)
     if probe is not None:
         res.append(("fc2.probe(thresh%+d)_decision" % probe, float(bool(o["h"][r, j] != 0) != (probe < 0)), 0.0))
-    gw2, gb2, gb1 = run_fc2_wgrad(o["h"], o["dl"], o["dh"])
-    rw2, rb2, rb1 = R.fc2_wgrad(o["h"], o["dl"], o["dh"])
-    return res + R.cmp_fp32("fc2_wgrad.g_w2", gw2, rw2) + R.cmp_fp32("fc2_wgrad.g_b2", gb2, rb2) + \
-        R.cmp_fp32("fc2_wgrad.g_b1", gb1, rb1)
+    return res + fc2_wgrad_results("fc2_wgrad", o["h"], o["dl"], o["dh"], *run_fc2_wgrad(o["h"], o["dl"], o["dh"]))
+
+
+def keep_pattern_results(tag: str, h, ref_h, hp, slack) -> List[Result]:
+    """The dropout keep pattern, exactly: apart from pre-activations ``hp`` within ``slack`` (the kernel's fp32 error) of
+    zero, h != 0 iff ReLU and the mask keep."""
+    settled = hp.abs() > slack
+    return [(tag, float((((h != 0) != (ref_h != 0)) & settled).sum()), 0.0)]
+
+
+def fc2_wgrad_results(tag: str, h, dl, dh, gw2, gb2, gb1) -> List[Result]:
+    """fc2_wgrad on continuous data: fc2 weight / bias and fc1 bias gradients from h_act, dlogits and dh."""
+    rw2, rb2, rb1 = R.fc2_wgrad(h, dl, dh)
+    return R.cmp_fp32(tag + ".g_w2", gw2, rw2) + R.cmp_fp32(tag + ".g_b2", gb2, rb2) + R.cmp_fp32(tag + ".g_b1", gb1, rb1)
+
+
+def fc1_fwd_results(tag: str, kind: str, a2, w1, part) -> List[Result]:
+    """The fc1 GEMM's 7 split-K partials [7,B,512] from a2 [B,3136] and the bf16 weights w1 [3136,512]."""
+    res: List[Result] = []
+    # split z owns k-blocks [49 z / 7, 49 (z + 1) / 7) of 64
+    for z in range(FC1_SPLITS):
+        k0, k1 = 64 * (49 * z // FC1_SPLITS), 64 * (49 * (z + 1) // FC1_SPLITS)
+        rz = a2[:, k0:k1].double() @ w1[k0:k1].double()
+        res += R.compare("%s.partial%d" % (tag, z), kind, part[z], rz)
+    if kind == "grid":
+        R.assert_exact_grid(a2.double().abs() @ w1.double().abs(), 1.0 / 64, tag + ".gemm")
+    return res
 
 
 def check_fc1_fwd(B: int = 64, seed: int = 16, kinds: Sequence[str] = KINDS, train: bool = True) -> List[Result]:
@@ -431,15 +475,8 @@ def check_fc1_fwd(B: int = 64, seed: int = 16, kinds: Sequence[str] = KINDS, tra
         b1, w2, b2, labels = _fc2_inputs(kind, g, B)
         a2, w1, b1, w2, b2, labels = _dev(a2, w1, b1, w2, b2, labels)
         part = run_fc1_fwd(a2, w1)
-        # split z owns k-blocks [49 z / 7, 49 (z + 1) / 7) of 64
-        for z in range(FC1_SPLITS):
-            k0, k1 = 64 * (49 * z // FC1_SPLITS), 64 * (49 * (z + 1) // FC1_SPLITS)
-            rz = a2[:, k0:k1].double() @ w1[k0:k1].double()
-            res += R.compare("%s.partial%d" % (tag, z), kind, part[z], rz)
+        res += fc1_fwd_results(tag, kind, a2, w1, part)
         hsum = a2.double() @ w1.double()
-        habs = a2.double().abs() @ w1.double().abs()
-        if kind == "grid":
-            R.assert_exact_grid(habs, 1.0 / 64, tag + ".gemm")
         mix0 = dropout_seed_mix(seed, 0, 0)
         o = run_fc2_fwd_bwd(part, b1, w2, b2, labels, train, mix0, 3, 0.5)
         keep = dropout_keep_mask(dropout_seed_mix(seed, 3, 0), B, 512, 0.5, device="cuda") if train else None
@@ -477,14 +514,30 @@ def check_fc1_wgrad(B: int = 64, seed: int = 18, kinds: Sequence[str] = KINDS) -
         else:
             a2, dh = _bf(R.grid(g, (B, 3136), 0, 2)), _bf(R.grid(g, (B, 512), -64, 64, 64))
         a2, dh = _dev(a2, dh)
-        ref = a2.double().t() @ dh.double()
-        ra = a2.double().abs().t() @ dh.double().abs()
-        if kind == "grid":
-            R.assert_exact_grid(ra, 1.0 / 64, "fc1_wgrad")
         for bf in (False, True):
             out = run_fc1_wgrad(a2, dh, bf)
-            res += R.compare("fc1_wgrad.%s.%s" % (kind, "bf16" if bf else "f32"), kind, out, ref, R.fp32_slack(ra, B))
+            res += fc1_wgrad_results("fc1_wgrad.%s.%s" % (kind, "bf16" if bf else "f32"), kind, a2, dh, out)
     return res
+
+
+def fc1_wgrad_results(tag: str, kind: str, a2, dh, out) -> List[Result]:
+    """dW1 = a2^T dh, stored as fp32 (gradient arena) or bf16 (the bucketed aggregation's wire buffer)."""
+    ref = a2.double().t() @ dh.double()
+    ra = a2.double().abs().t() @ dh.double().abs()
+    if kind == "grid":
+        R.assert_exact_grid(ra, 1.0 / 64, "fc1_wgrad")
+    return R.compare(tag, kind, out, ref, R.fp32_slack(ra, a2.shape[0]))
+
+
+def fc1_dgrad_results(tag: str, kind: str, dh, w1, code, dy, gb) -> List[Result]:
+    """fc1_dgrad_unpool's dy2 [B,14,14,64] and conv2 bias gradient from dh, the bf16 weights w1 and the pool2 codes."""
+    rdy, rgb = R.fc1_dgrad_unpool(dh, w1, code)
+    ady, _ = R.fc1_dgrad_unpool(dh.abs(), w1.abs(), code)
+    if kind == "grid":
+        R.assert_exact_grid(ady, 1.0 / 64, tag + ".dy")
+        # the bias gradient adds the exact fp32 values: its partial sums are bounded by the sum of their magnitudes
+        R.assert_exact_grid(rdy.abs().sum((0, 1, 2)), 1.0 / 64, tag + ".g_bias")
+    return R.compare(tag + ".dy", kind, dy, rdy, R.fp32_slack(ady, 512)) + R.compare(tag + ".g_bias", kind, gb, rgb)
 
 
 def check_fc1_dgrad_unpool(B: int = 200, seed: int = 6, kinds: Sequence[str] = KINDS, stale_B: int = 0) -> List[Result]:
@@ -501,14 +554,7 @@ def check_fc1_dgrad_unpool(B: int = 200, seed: int = 6, kinds: Sequence[str] = K
         if stale_B:
             prime_workspace("fc1_dgrad_unpool", stale_B)
         dy, gb = run_fc1_dgrad_unpool(dh, w1, code)
-        rdy, rgb = R.fc1_dgrad_unpool(dh, w1, code)
-        ady, _ = R.fc1_dgrad_unpool(dh.abs(), w1.abs(), code)
-        if kind == "grid":
-            R.assert_exact_grid(ady, 1.0 / 64, tag + ".dy")
-            # the bias gradient adds the exact fp32 values: its partial sums are bounded by the sum of their magnitudes
-            R.assert_exact_grid(rdy.abs().sum((0, 1, 2)), 1.0 / 64, tag + ".g_bias")
-        res += R.compare(tag + ".dy", kind, dy, rdy, R.fp32_slack(ady, 512))
-        res += R.compare(tag + ".g_bias", kind, gb, rgb)
+        res += fc1_dgrad_results(tag, kind, dh, w1, code, dy, gb)
     return res
 
 
@@ -994,7 +1040,8 @@ def _dgrad_results(tag: str, dh_in, w16, h, dh_out, g_bias, g_bias0) -> List[Res
 
 
 def _mlp_step_results(tag: str, kind: str, eng, images, labels) -> List[Result]:
-    """One ``forward_backward`` of a CudaMlpEngine, every stage against its float64 reference computed from the engine's
+    """One ``forward_backward`` of a CudaMlpEngine (``eng``: the engine, or a step's record with the same attributes, see
+    ``ops/trajectory.py``), every stage against its float64 reference computed from the engine's
     own input buffers for that stage (x16, h[i], dh[i], dl_pad, the shadow pb, the fp32 arena p): one stage's rounding
     never loosens the next stage's bound, and bf16 inputs keep the forward stages exact on grid data.  Everything
     downstream of the softmax is continuous on both kinds and held to fp32 bounds."""
@@ -1011,16 +1058,19 @@ def _mlp_step_results(tag: str, kind: str, eng, images, labels) -> List[Result]:
     o = dict(dh=eng.dh[-1], dl_pad=eng.dl_pad, g_b=gr["fc%d_biases" % L], la=eng.d_loss_acc, logits=None)
     res += _dense10_results(tag + ".dense10_xent", kind, o, src, p["fc%d_weights" % L], p["fc%d_biases" % L], labels,
                             zeros, zeros[:2], True, 2.0 ** -(3 + 3 * L), pad_value=0.0)
+    def wgrad(name, got, ref, bound):
+        # the bucketed aggregation's early layer leaves its GEMM as bf16 (the wire buffer): RNE of the bounded fp32 value
+        return (R.cmp_bf16_bound if got.dtype == BF else R.cmp_bound)(name, got, ref, bound)
     dl = eng.dl_pad[:, :10].double()
-    res += R.cmp_bound("%s.g_fc%d_weights" % (tag, L), gr["fc%d_weights" % L], src.double().t() @ dl,
-                       R.fp32_slack(src.double().abs().t() @ dl.abs(), B))
+    res += wgrad("%s.g_fc%d_weights" % (tag, L), gr["fc%d_weights" % L], src.double().t() @ dl,
+                 R.fp32_slack(src.double().abs().t() @ dl.abs(), B))
     _, cs, ca = R.relu_bwd_colsum(eng.dh[-1], None)
     res += R.cmp_bound("%s.g_fc%d_biases" % (tag, L - 1), gr["fc%d_biases" % (L - 1)], cs, R.fp32_slack(ca, B + 1))
     for i in range(L - 1, 0, -1):
         below = eng.h[i - 2] if i > 1 else eng.x16
         d = eng.dh[i - 1].double()
-        res += R.cmp_bound("%s.g_fc%d_weights" % (tag, i), gr["fc%d_weights" % i], below.double().t() @ d,
-                           R.fp32_slack(below.double().abs().t() @ d.abs(), B))
+        res += wgrad("%s.g_fc%d_weights" % (tag, i), gr["fc%d_weights" % i], below.double().t() @ d,
+                     R.fp32_slack(below.double().abs().t() @ d.abs(), B))
         if i > 1:
             res += _dgrad_results("%s.dh%d" % (tag, i - 1), eng.dh[i - 1], pb["fc%d_weights" % i], eng.h[i - 2],
                                   eng.dh[i - 2], gr["fc%d_biases" % (i - 1)], zeros[:1])

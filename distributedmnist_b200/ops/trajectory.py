@@ -1,0 +1,188 @@
+"""Back-to-back training steps checked stage by stage against the float64 references.
+
+:class:`StepRecorder` clones, after each enqueued step and on that step's stream (no host synchronisation), the buffers
+every stage of the step wrote, and the gradients, weights, bf16 shadow and (loss, accuracy) it left.
+:func:`lenet_trajectory_results` / :func:`mlp_trajectory_results` then judge each step from the records alone, with the
+bounds the kernel checks use (``ops/selfcheck.py``):
+
+* each stage from its recorded inputs, on the weights the previous step committed (the initial arena for the first);
+  the bf16 shadow a step reads is RNE of those weights, the dropout mask the one of the epoch word the step read;
+* the update bit for bit against ``ops/aggrefs.py``, and the recorded shadow as RNE of the recorded weights.
+
+The input slots are not recorded: the copy stream may refill a slot as soon as the step that read it is done.  The caller
+passes what it fed each step, so a step that computed on another batch fails its stage checks.
+"""
+from __future__ import annotations
+
+import re
+from types import SimpleNamespace
+from typing import Dict, List, Sequence
+
+import torch
+
+from ..models import dropout_keep_mask, dropout_seed_mix
+from . import aggrefs as A
+from . import refs as R
+from . import selfcheck as S
+
+Result = S.Result
+LENET_BUFFERS = ("a1", "code1", "a2", "code2", "h_part", "dh", "h_act", "dlogits", "dy2", "dx1")
+MLP_BUFFERS = ("x16", "h", "dh", "dl_pad")
+
+
+class StepRecorder:
+    """Call :meth:`record` right after each step is enqueued (``train_step``, ``step_packed``, ``step_indices``), on the
+    stream the step was enqueued on: the clones then run after the step and before the next one.  The native runner
+    launches on the stream that was current when it was created, so this holds for its steps too."""
+
+    def __init__(self, eng):
+        self.eng = eng
+        self.init = dict(params=eng.params.clone(), shadow=eng.shadow.clone())
+        self.records: List[Dict[str, object]] = []
+
+    def record(self) -> None:
+        e = self.eng
+        r: Dict[str, object] = {}
+        for name in (LENET_BUFFERS if hasattr(e, "h_part") else MLP_BUFFERS):
+            v = getattr(e, name)
+            r[name] = [t.clone() for t in v] if isinstance(v, list) else v.clone()
+        r.update(grads=e.grads.clone(), params=e.params.clone(), shadow=e.shadow.clone(), loss_acc=e.d_loss_acc.clone())
+        if e._bucket_v2:
+            r["g16"] = e._g16_view.clone()
+        self.records.append(r)
+
+
+def update_of(eng, sched, step0: int) -> dict:
+    """How ``eng`` applies its gradients: ``mode`` "fused" (fused_sync_sgd), "bucket" (the bf16-wire bucketed kernels)
+    or "kgtn" (K > N: every k-th iteration commits), the schedule and the global step of the first step."""
+    be = eng.backend
+    e0, e1 = eng._bucket_early
+    mode = "kgtn" if eng._kgtn_k else ("bucket" if eng._bucket_v2 else "fused")
+    return dict(mode=mode, sched=sched, step0=step0, k=max(eng._kgtn_k, 1), early=(e0, e1),
+                late_bf16=A.late_bucket_rounds_bf16(eng.spec.arena_numel, e1 - e0, be.late_ll, be.late_bf16))
+
+
+def epoch_of(upd: dict, t: int) -> int:
+    """The epoch word step t reads: the global step, which with K > N stays put over the k iterations of a commit."""
+    return upd["step0"] + t // upd["k"]
+
+
+def _shadow_bits(t: torch.Tensor):
+    return t.detach().cpu().view(torch.int16).numpy().view("<u2")
+
+
+def update_results(tag: str, init: dict, records: Sequence[dict], upd: dict) -> List[Result]:
+    """Each step's weights from the previous record (or ``init``) and the step's recorded gradients, bit for bit; with
+    K > N the weights stay put until the k-th iteration, which applies the accumulated k gradients."""
+    res: List[Result] = []
+    mode, k = upd["mode"], upd["k"]
+    res.append((tag + ".init.shadow_bits_differ", float((_shadow_bits(init["shadow"]) != A.bf16_bits(init["params"])).sum()), 0.0))
+    w, acc = A.f32(init["params"]), []
+    for t, r in enumerate(records):
+        scale = A.step_scale(upd["sched"], epoch_of(upd, t), k)
+        g = A.f32(r["grads"])
+        if mode == "kgtn":
+            acc.append(g)
+            want = A.sgd(w, A.interval_accumulate(acc), scale) if len(acc) == k else w
+            acc = [] if len(acc) == k else acc
+        elif mode == "bucket":
+            want = A.bucket_step(w, [g], [A.f32(r["g16"].float()).reshape(-1)], upd["early"], scale, upd["late_bf16"])
+        else:
+            want = A.fused_sync_step(w, [g], 1, scale)
+        got = A.bits(r["params"])
+        res.append(("%s.step%d.update_bits_differ" % (tag, t), float((got != A.bits(want)).sum()), 0.0))
+        if mode != "kgtn":          # K > N refreshes the shadow when the next iteration adopts the commit
+            res.append(("%s.step%d.shadow_bits_differ" % (tag, t),
+                        float((_shadow_bits(r["shadow"]) != A.bf16_bits(r["params"])).sum()), 0.0))
+        w = A.f32(r["params"])
+    return res
+
+
+def _inputs(spec, init: dict, records: Sequence[dict], t: int, dev):
+    """(fp32 views, bf16 shadow views) of the weights step t read: RNE of the previous step's committed weights."""
+    p = (init if t == 0 else records[t - 1])["params"].to(dev)
+    return spec.views(p), spec.views(p.to(torch.bfloat16))
+
+
+def lenet_step_results(tag: str, spec, r: dict, p, pb, images, labels, mask, keep_prob: float) -> List[Result]:
+    """One LeNet training step from its record ``r``: every stage from the recorded inputs of that stage.  ``p`` / ``pb``:
+    the fp32 / bf16 weights the step read, ``images`` [B,28,28] / ``labels`` what it was fed, ``mask`` its dropout mask."""
+    kind = "rand"
+    B = labels.shape[0]
+    x = images.reshape(B, 28, 28)
+    a2 = r["a2"]
+    g = spec.views(r["grads"])
+    res = S.conv1_fwd_results(tag + ".conv1_fwd", kind, x, p["conv1_weights"], p["conv1_biases"], r["a1"], r["code1"])
+    res += S.conv2_fwd_results(tag + ".conv2_fwd", kind, r["a1"], pb["conv2_weights"], p["conv2_biases"],
+                               a2.view(B, 7, 7, 64), r["code2"].view(B, 7, 7, 64))
+    res += S.fc1_fwd_results(tag + ".fc1_fwd", kind, a2, pb["fc1_weights"], r["h_part"])
+    w1 = pb["fc1_weights"].double()
+    hsum = a2.double() @ w1
+    ref = R.fc2_fwd_bwd(hsum, p["fc1_biases"], p["fc2_weights"], p["fc2_biases"], labels, mask, keep_prob)
+    o = dict(la=r["loss_acc"], h=r["h_act"], dl=r["dlogits"], dh=r["dh"])
+    res += S._fc2_results(tag + ".fc2_fwd_bwd", kind, o, ref, p["fc2_weights"], B, True)
+    b1 = p["fc1_biases"].double()
+    # the kernel's pre-activation: 7 fp32 GEMM partials of 448 products each, summed with the bias in fp32
+    res += S.keep_pattern_results(tag + ".fc2_fwd_bwd.keep_pattern", r["h_act"], ref["h"], hsum + b1,
+                                  R.fp32_slack(a2.double().abs() @ w1.abs() + b1.abs(), 3136 + 8))
+    res += S.fc2_wgrad_results(tag + ".fc2_wgrad", r["h_act"], r["dlogits"], r["dh"], g["fc2_weights"], g["fc2_biases"],
+                               g["fc1_biases"])
+    res += S.fc1_wgrad_results(tag + ".fc1_wgrad", kind, a2, r["dh"], r.get("g16", g["fc1_weights"]))
+    res += S.fc1_dgrad_results(tag + ".fc1_dgrad_unpool", kind, r["dh"], pb["fc1_weights"], r["code2"], r["dy2"],
+                               g["conv2_biases"])
+    res += S.conv2_dgrad_results(tag + ".conv2_dgrad", kind, r["dy2"], pb["conv2_weights"], r["dx1"])
+    res += S.conv2_wgrad_results(tag + ".conv2_wgrad", kind, r["a1"], r["dy2"], g["conv2_weights"])
+    res += S.conv1_wgrad_results(tag + ".conv1_wgrad", kind, x, r["dx1"], r["code1"], g["conv1_weights"].reshape(25, 32),
+                                 g["conv1_biases"])
+    valid = spec.valid_mask().to(r["grads"].device)
+    res.append((tag + ".grad_padding", float(r["grads"][~valid].abs().max()), 0.0))
+    return res
+
+
+def lenet_trajectory_results(tag: str, spec, init: dict, records: Sequence[dict], batches: Sequence, upd: dict,
+                             seed: int, rank: int, keep_prob: float) -> List[Result]:
+    """Every step of a LeNet run (``batches[t]`` = (images, labels) fed to step t) and every update."""
+    res = update_results(tag, init, records, upd)
+    for t, (r, (x, y)) in enumerate(zip(records, batches)):
+        dev = r["a1"].device
+        p, pb = _inputs(spec, init, records, t, dev)
+        y = torch.as_tensor(y).to(dev)
+        mask = dropout_keep_mask(dropout_seed_mix(seed, epoch_of(upd, t), rank), y.shape[0], 512, keep_prob, device=dev)
+        res += lenet_step_results("%s.step%d" % (tag, t), spec, r, p, pb, torch.as_tensor(x).to(dev), y, mask, keep_prob)
+    return res
+
+
+def mlp_trajectory_results(tag: str, spec, init: dict, records: Sequence[dict], batches: Sequence,
+                           upd: dict) -> List[Result]:
+    """Every step of an MLP run through :func:`selfcheck._mlp_step_results`, and every update.  With the bucketed
+    aggregation the early layer's weight gradient is the bf16 wire buffer."""
+    res = update_results(tag, init, records, upd)
+    n_layers = len(spec.params) // 2
+    early = next(q.name for q in spec.params if q.offset == upd["early"][0])
+    for t, (r, (x, y)) in enumerate(zip(records, batches)):
+        dev = r["x16"].device
+        p, pb = _inputs(spec, init, records, t, dev)
+        g = dict(spec.views(r["grads"]))
+        if "g16" in r:
+            g[early] = r["g16"]
+        B = r["x16"].shape[0]
+        rec = SimpleNamespace(p=p, pb=pb, g=g, n_layers=n_layers, batch_size=B, x16=r["x16"], h=r["h"], dh=r["dh"],
+                              dl_pad=r["dl_pad"], d_loss_acc=r["loss_acc"], grads=r["grads"], spec=spec)
+        res += S._mlp_step_results("%s.step%d" % (tag, t), "rand", rec, torch.as_tensor(x).to(dev).reshape(B, 784),
+                                   torch.as_tensor(y).to(dev))
+    return res
+
+
+def failures(results: Sequence[Result]) -> List[Result]:
+    return [(n, e, b) for (n, e, b) in results if not e <= b]
+
+
+def worst_by_stage(tag: str, results: Sequence[Result]) -> Dict[str, float]:
+    """Largest error-to-bound ratio of each check over all steps (its name without ``tag`` and ``stepN``); checks with a
+    zero bound count as 0 when they pass."""
+    out: Dict[str, float] = {}
+    for n, e, b in results:
+        stage = re.sub(r"^step\d+\.", "", n[len(tag) + 1:] if n.startswith(tag + ".") else n)
+        ratio = e / b if b > 0 else (0.0 if e <= b else float("inf"))
+        out[stage] = max(out.get(stage, 0.0), ratio)
+    return out

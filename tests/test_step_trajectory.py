@@ -1,0 +1,174 @@
+"""The trajectory checker (ops/trajectory.py) on CPU-built records: small LeNet and MLP runs emulated from the float64
+references in the engine's storage formats pass unchanged, and each seeded ordering fault fails."""
+import pytest
+import torch
+
+from distributedmnist_b200.models import dropout_keep_mask, dropout_seed_mix, get_model
+from distributedmnist_b200.ops import aggrefs as A
+from distributedmnist_b200.ops import refs as R
+from distributedmnist_b200.ops import trajectory as T
+from distributedmnist_b200.schedule import LearningRateSchedule
+
+BF = torch.bfloat16
+SEED, RANK, KEEP = 5, 0, 0.5
+# a large step size, so that one step's update moves the bf16 shadow and the activations visibly
+SCHED = LearningRateSchedule(4.0, 1, 0.999)
+STEP0 = 3001
+
+
+def _bf(x):
+    return x.to(torch.float32).to(BF)           # RNE of the fp32 value, as the kernels store bf16
+
+
+def _ftz(grads):
+    """The kernels run with flush-to-zero: no subnormal gradient reaches the update."""
+    return grads.masked_fill_(grads.abs() < A.FLT_MIN, 0.0)
+
+
+def _update(w, g):
+    """fused_sync_sgd on one replica, in place of the engine's aggregation."""
+    return lambda t: torch.from_numpy(A.fused_sync_step(A.f32(w), [A.f32(g)], 1, A.step_scale(SCHED, STEP0 + t, 1)))
+
+
+def _lenet_step(spec, params, x, y, mask, fault, prev):
+    """One LeNet step as the kernels store it.  ``fault``: "dgrad_post_update" runs fc1 dgrad on the updated shadow."""
+    B = x.shape[0]
+    p, pb = spec.views(params), spec.views(params.to(BF))
+    f1 = R.pool_fwd(R.conv5x5(x.to(BF)[..., None], p["conv1_weights"].to(BF)), p["conv1_biases"])
+    a1, code1 = _bf(f1["out"]), f1["code"]
+    f2 = R.pool_fwd(R.conv5x5(a1, pb["conv2_weights"]), p["conv2_biases"])
+    a2, code2 = _bf(f2["out"]).reshape(B, 3136), f2["code"].reshape(B, 3136)
+    w1 = pb["fc1_weights"].double()
+    ks = [64 * (49 * z // 7) for z in range(8)]
+    h_part = torch.stack([(a2[:, ks[z]:ks[z + 1]].double() @ w1[ks[z]:ks[z + 1]]).float() for z in range(7)])
+    ref = R.fc2_fwd_bwd(a2.double() @ w1, p["fc1_biases"], p["fc2_weights"], p["fc2_biases"], y, mask, KEEP)
+    dh, h_act, dlogits = _bf(ref["dh"]), ref["h"].float(), ref["dl"].float()
+    grads = torch.zeros(spec.arena_numel)
+    g = spec.views(grads)
+    gw2, gb2, gb1 = R.fc2_wgrad(h_act, dlogits, dh)
+    g["fc2_weights"].copy_(gw2), g["fc2_biases"].copy_(gb2), g["fc1_biases"].copy_(gb1)
+    g["fc1_weights"].copy_(a2.double().t() @ dh.double())
+    w1_dgrad = pb["fc1_weights"]
+    if fault == "dgrad_post_update":
+        w1_dgrad = spec.views(_update(params, grads)(prev["t"]).to(BF))["fc1_weights"]
+    dy, gbc2 = R.fc1_dgrad_unpool(dh, w1_dgrad, code2)
+    dy2 = _bf(dy)
+    g["conv2_biases"].copy_(gbc2)
+    dx1 = _bf(R.conv5x5_dgrad(dy2, pb["conv2_weights"]))
+    g["conv2_weights"].copy_(R.conv5x5_wgrad(a1, dy2))
+    gw1, gbc1 = R.conv1_wgrad(x.to(BF), dx1, code1)
+    g["conv1_weights"].copy_(gw1.reshape(5, 5, 1, 32)), g["conv1_biases"].copy_(gbc1)
+    la = torch.tensor([float(ref["loss"]), float(ref["acc"])], dtype=torch.float32)
+    return dict(a1=a1, code1=code1, a2=a2, code2=code2, h_part=h_part, dh=dh, h_act=h_act, dlogits=dlogits, dy2=dy2,
+                dx1=dx1, grads=_ftz(grads), loss_acc=la)
+
+
+def _mlp_step(spec, params, x, y, fault, prev):
+    """One MLP step as the kernels store it.  ``fault``: "bias_not_cleared" adds the previous step's atomically
+    accumulated output-layer bias gradient."""
+    L = len(spec.params) // 2
+    B = x.shape[0]
+    p, pb = spec.views(params), spec.views(params.to(BF))
+    x16 = _bf(x.reshape(B, 784))
+    hs, src = [], x16
+    for i in range(1, L):
+        src = _bf(R.mlp_hidden(src, pb["fc%d_weights" % i], p["fc%d_biases" % i])[0])
+        hs.append(src)
+    out = R.dense10_xent(src, p["fc%d_weights" % L], p["fc%d_biases" % L], y)
+    dl_pad = torch.zeros(B, 64, dtype=BF)
+    dl_pad[:, :10] = _bf(out["dl"])
+    dhs = [None] * (L - 1)
+    dhs[-1] = _bf(out["dh"])
+    grads = torch.zeros(spec.arena_numel)
+    g = spec.views(grads)
+    g["fc%d_weights" % L].copy_(src.double().t() @ dl_pad[:, :10].double())
+    g["fc%d_biases" % L].copy_(out["dl"].sum(0))
+    if fault == "bias_not_cleared" and prev["t"] > 0:
+        g["fc%d_biases" % L].add_(spec.views(prev["grads"])["fc%d_biases" % L])
+    for i in range(L - 1, 0, -1):
+        below = hs[i - 2] if i > 1 else x16
+        g["fc%d_biases" % i].copy_(dhs[i - 1].double().sum(0))
+        g["fc%d_weights" % i].copy_(below.double().t() @ dhs[i - 1].double())
+        if i > 1:
+            dhs[i - 2] = _bf(R.mlp_dgrad(dhs[i - 1], pb["fc%d_weights" % i], hs[i - 2])[0])
+    la = torch.tensor([float(out["loss_terms"].mean()), float(out["hits"].double().mean())], dtype=torch.float32)
+    return dict(x16=x16, h=hs, dh=dhs, dl_pad=dl_pad, grads=_ftz(grads), loss_acc=la)
+
+
+def _run(model, fault=None, steps=4, B=8):
+    """(spec, init, records, batches fed, update) of an emulated run with at most one seeded fault."""
+    spec = get_model(model, 64)[0]
+    gen = torch.Generator().manual_seed(11)
+    shape = (B, 28, 28) if model == "lenet" else (B, 784)
+    batches = [(torch.rand(*shape, generator=gen) - 0.5, torch.randint(0, 10, (B,), generator=gen)) for _ in range(steps)]
+    params = spec.init_flat(SEED)
+    init = dict(params=params.clone(), shadow=params.to(BF))
+    records, prev = [], dict(t=0, grads=None)
+    for t in range(steps):
+        x, y = batches[t]
+        if fault == "batch_t_plus_2" and t == 1:
+            x, y = batches[t + 2]
+        if fault == "slot1_reads_slot0" and t % 2 == 1:
+            x, y = batches[t - 1]
+        prev["t"] = t
+        if model == "lenet":
+            e = STEP0 + t - (1 if fault == "mask_previous_epoch" and t > 0 else 0)
+            mask = dropout_keep_mask(dropout_seed_mix(SEED, e, RANK), B, 512, KEEP)
+            r = _lenet_step(spec, params, x, y, mask, fault, prev)
+        else:
+            r = _mlp_step(spec, params, x, y, fault, prev)
+        g = prev["grads"] if fault == "stale_gradient" and t > 0 else r["grads"]
+        params = _update(params, g)(t)
+        r.update(params=params.clone(), shadow=params.to(BF))
+        records.append(r)
+        prev["grads"] = r["grads"]
+    upd = dict(mode="fused", sched=SCHED, step0=STEP0, k=1, early=(spec.param("fc1_weights").offset,) * 2, late_bf16=False)
+    return spec, init, records, batches, upd
+
+
+def _results(model, fault=None):
+    spec, init, records, batches, upd = _run(model, fault)
+    if model == "lenet":
+        return T.lenet_trajectory_results("lenet", spec, init, records, batches, upd, SEED, RANK, KEEP)
+    return T.mlp_trajectory_results("mlp3", spec, init, records, batches, upd)
+
+
+@pytest.mark.parametrize("model", ["lenet", "mlp3"])
+def test_emulated_trajectory_passes(model):
+    res = _results(model)
+    assert not T.failures(res), T.failures(res)
+    assert sum(1 for n, _, _ in res if ".step3." in n) > 10
+    worst = T.worst_by_stage(model, res)
+    assert "update_bits_differ" in worst and all(0 <= v <= 1 for v in worst.values()), worst
+
+
+@pytest.mark.parametrize("model,fault,stage", [
+    ("lenet", "dgrad_post_update", "fc1_dgrad_unpool"),
+    ("lenet", "mask_previous_epoch", "fc2_fwd_bwd"),
+    ("lenet", "batch_t_plus_2", "step1.conv1_fwd"),
+    ("mlp3", "bias_not_cleared", "dense10_xent.g_b"),
+    ("lenet", "slot1_reads_slot0", "step1.conv1_fwd"),
+    ("mlp3", "slot1_reads_slot0", "step1.x16"),
+    ("lenet", "stale_gradient", "update_bits_differ"),
+    ("mlp3", "stale_gradient", "update_bits_differ"),
+])
+def test_seeded_fault_fails(model, fault, stage):
+    bad = T.failures(_results(model, fault))
+    assert any(stage in n for n, _, _ in bad), (fault, bad[:10])
+
+
+def test_kgtn_update_commits_every_k_th_iteration():
+    """K > N: the weights stay put for k - 1 iterations, then take the accumulated k gradients at the commit's step size."""
+    spec = get_model("mlp2", 64)[0]
+    gen = torch.Generator().manual_seed(3)
+    w = spec.init_flat(SEED)
+    init = dict(params=w.clone(), shadow=w.to(BF))
+    gs = [torch.randn(spec.arena_numel, generator=gen) * 1e-2 * spec.valid_mask() for _ in range(4)]
+    c1 = torch.from_numpy(A.sgd(A.f32(w), A.interval_accumulate([A.f32(g) for g in gs[:2]]), A.step_scale(SCHED, STEP0, 2)))
+    c2 = torch.from_numpy(A.sgd(A.f32(c1), A.interval_accumulate([A.f32(g) for g in gs[2:]]), A.step_scale(SCHED, STEP0 + 1, 2)))
+    upd = dict(mode="kgtn", sched=SCHED, step0=STEP0, k=2, early=(0, 0), late_bf16=False)
+    recs = [dict(grads=g, params=p, shadow=p.to(BF)) for g, p in zip(gs, (w, c1, c1, c2))]
+    assert not T.failures(T.update_results("kgtn", init, recs, upd))
+    assert [T.epoch_of(upd, t) for t in range(4)] == [STEP0, STEP0, STEP0 + 1, STEP0 + 1]
+    recs[1] = dict(recs[1], params=w)                  # the commit not applied
+    assert T.failures(T.update_results("kgtn", init, recs, upd))
