@@ -24,6 +24,7 @@ from typing import Callable, Optional, Tuple
 import numpy as np
 import torch
 
+from . import moving_average as ema
 from .models import ModelSpec, dropout_keep_mask, dropout_seed_mix, get_model, loss_and_accuracy
 from .models.lenet import FC1_OUT
 
@@ -116,14 +117,41 @@ class TorchEngine(ComputeEngine):
     def loss_acc(self) -> Tuple[float, float]:
         return float(self._loss.item()), float(self._acc.item())
 
+    # ---- moving average of the weights (see moving_average.py) ------------------------------------------------------------
+    _ema: Optional[torch.Tensor] = None
+
+    def arm_moving_average(self, decay: float, global_step: int = 0) -> None:
+        """Keep an fp32 average arena, starting from the current weights, which :meth:`update_moving_average` moves
+        towards the weights after every global step."""
+        if not 0.0 < float(decay) < 1.0:
+            raise ValueError("moving average decay must lie in (0, 1), got %r" % decay)
+        self._ema_decay = float(decay)
+        self._ema = self.params.detach().clone()
+        self._ema_step = int(global_step)
+
+    def update_moving_average(self, global_step: int) -> None:
+        """The update after the step that produced ``global_step``, from the current weights."""
+        m = torch.tensor(float(ema.multiplier(self._ema_decay, global_step)), dtype=torch.float32, device=self._ema.device)
+        self._ema.sub_((self._ema - self.params.detach()) * m)      # three float32 operations, each rounded on its own
+        self._ema_step = int(global_step)
+
+    def moving_average(self) -> Tuple[torch.Tensor, int]:
+        """(copy of the average arena, global step of the weights it was last updated from)."""
+        return self._ema.clone(), self._ema_step
+
+    def load_moving_average(self, flat: torch.Tensor) -> None:
+        self._ema.copy_(flat.to(self._ema.device, torch.float32))
+
     @torch.no_grad()
-    def evaluate(self, images, labels) -> Tuple[float, float]:
+    def evaluate(self, images, labels, moving_average: bool = False) -> Tuple[float, float]:
+        """``moving_average``: score the average arena instead of the weights."""
         if isinstance(images, np.ndarray):
             images, labels = torch.from_numpy(np.ascontiguousarray(images)), torch.from_numpy(np.ascontiguousarray(labels))
         images, labels = images.to(self.device), labels.to(self.device)
+        flat = self._ema if moving_average else self.params
         tot_loss, tot_hit, n = 0.0, 0.0, images.shape[0]
         for s in range(0, n, 2048):
-            lg = self._logits(self.params, images[s:s + 2048], False, 0)
+            lg = self._logits(flat, images[s:s + 2048], False, 0)
             loss, acc = loss_and_accuracy(lg, labels[s:s + 2048])
             m = lg.shape[0]
             tot_loss += float(loss) * m

@@ -495,6 +495,8 @@ class _CudaEngine(ComputeEngine):
         off = self.backend._off["epoch"]
         self._ck_epoch = self.backend._ctrl_bytes[off:off + 4]
         self.ckpt_host = [torch.zeros(n, dtype=torch.float32).pin_memory() for _ in range(self.CKPT_HOST_BUFFERS)]
+        if self._ema is not None:
+            self._arm_checkpoint_average()
         self._ck_rec = [torch.zeros(2, dtype=torch.int32).pin_memory() for _ in range(self.CKPT_HOST_BUFFERS)]  # step, status
         self._ck_stream = torch.cuda.Stream(device=dev)
         self._ck_staged, self._ck_landed = torch.cuda.Event(), torch.cuda.Event()
@@ -519,11 +521,15 @@ class _CudaEngine(ComputeEngine):
         else:
             self._ck_dev.copy_(self.params)
             self._ck_state[0:4].copy_(self._ck_epoch)
+            if self._ck_ema_dev is not None:
+                self._ck_ema_dev.copy_(self._ema)        # the average after the same step as the weights
         self._ck_staged.record(cur)
         self._ck_seq += 1
         with torch.cuda.stream(self._ck_stream):
             self._ck_stream.wait_event(self._ck_staged)
             self.ckpt_host[buf].copy_(self._ck_dev, non_blocking=True)
+            if self._ck_ema_dev is not None:
+                self.ckpt_ema_host[buf].copy_(self._ck_ema_dev, non_blocking=True)
             self._ck_rec[buf].copy_(self._ck_state[0:8].view(torch.int32), non_blocking=True)
             self._ck_landed.record(self._ck_stream)
         self._ck_inflight = (self._ck_seq, buf)
@@ -554,6 +560,60 @@ class _CudaEngine(ComputeEngine):
     def checkpoint_stats(self) -> Optional[dict]:
         """Snapshot statistics of the capture (see :class:`_Snapshot`), None for the live capture."""
         return self._ck_snap.stats() if self._ck_snap is not None else None
+
+    def _arm_checkpoint_average(self) -> None:
+        """The capture's buffers for the moving average: a device staging arena and one page-locked host arena per host
+        buffer of the weights."""
+        n = self.spec.arena_numel
+        self._ck_ema_dev = torch.zeros(n, dtype=torch.float32, device=self.device)
+        self.ckpt_ema_host = [torch.zeros(n, dtype=torch.float32).pin_memory() for _ in range(self.CKPT_HOST_BUFFERS)]
+
+    # ---- moving average of the weights (csrc/moving_average.cu) ---------------------------------------------------------
+    # The chief keeps TF's ExponentialMovingAverage of its arena in a shadow arena of its own (plain device memory: no peer
+    # reads it).  Each training step ends with one streaming kernel that moves the shadow towards the weights the step
+    # committed; it reads the global step from the epoch word, so the captured graph holds no host value.  Only K = N and
+    # cdf mode are supported: there no peer writes the chief's arena between two of its steps, so the arena holds exactly
+    # one global step when the kernel runs.
+    _ema = None                    # fp32 shadow arena of the average, see arm_moving_average
+    _ck_ema_dev = None
+
+    def arm_moving_average(self, decay: float) -> None:
+        """Allocate the shadow arena, starting from the current weights, and re-capture the step graphs so that every
+        training step ends with the average's update (before stop_publish when a stop is armed).  After
+        :meth:`attach_optimizer`; K = N or cdf mode only."""
+        if not 0.0 < float(decay) < 1.0:
+            raise ValueError("moving average decay must lie in (0, 1), got %r" % decay)
+        if self._opt_args is None:
+            raise RuntimeError("arm_moving_average: attach_optimizer() first")
+        if getattr(self, "_interval", False) or self._opt_args["k"] != self.backend.ctx.world_size:
+            raise ValueError("the moving average is kept for K = N and cdf mode only: with K < N, K > N or interval "
+                             "aggregation peers write the chief's arena at any time")
+        self._leave_native_runner()
+        torch.cuda.synchronize()
+        off = self.backend._off["epoch"]
+        self._ema_epoch = ctypes.c_void_p(self.backend.ctrl.local_ptr + off)
+        self._ema_decay = float(decay)
+        self._ema = self.params.detach().clone()
+        self._ema_step = self.backend._ctrl_bytes[off:off + 4].view(torch.int32).clone()    # step the shadow holds
+        if getattr(self, "_ck_dev", None) is not None and self._ck_ema_dev is None:
+            self._arm_checkpoint_average()
+        self._graphs = [None, None]
+        torch.cuda.synchronize()
+
+    def _launch_moving_average(self) -> None:
+        check(self.lib.dm_moving_average(ptr(self._ema), ptr(self.params), ctypes.c_longlong(self.spec.arena_numel),
+                                         self._ema_epoch, ctypes.c_double(self._ema_decay), ptr(self._ema_step),
+                                         ctypes.c_void_p(0), *([ctypes.c_longlong(0)] * 4), stream_ptr()), "moving_average")
+
+    def moving_average(self) -> Tuple[torch.Tensor, int]:
+        """(copy of the shadow arena, global step of the weights it was last updated from); synchronises the device."""
+        torch.cuda.synchronize()
+        return self._ema.clone(), int(self._ema_step.item()) & 0xFFFFFFFF
+
+    def load_moving_average(self, flat: torch.Tensor) -> None:
+        """Restore: the shadow arena from a host or device arena (the step it holds stays the current global step)."""
+        self._ema.copy_(flat.to(self.device, torch.float32))
+        torch.cuda.synchronize()
 
     # ---- inference ------------------------------------------------------------------------------------------
     def _eval_forward(self, images: torch.Tensor, labels: torch.Tensor, B: int) -> None:
@@ -856,6 +916,9 @@ class CudaLeNetEngine(_CudaEngine):
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1
         torch.cuda.current_stream().wait_event(self._join_loss)      # the loss read-back branch rejoins at the end of the step
+        if with_sync and self._ema is not None:
+            self._launch_moving_average()        # after the exchange has committed the step's weights and the epoch word
+            n += 1
         if with_sync and self._stop is not None:
             self._launch_stop_publish()          # the step's last node: after its exchange, and after the loss read-back
             n += 1
@@ -883,15 +946,22 @@ class CudaLeNetEngine(_CudaEngine):
     EVAL_RING = 16                 # host record slots
     SNAP_KEEP = False              # also keep the last accepted snapshot (one more 6.65 MB copy per accepted pass), see
                                    # eval_snapshot(); set before arm_eval
+    _ev_average = False            # the pass scores the moving average, see arm_eval
 
-    def arm_eval(self, images, labels, snapshot: bool = False) -> None:
+    def arm_eval(self, images, labels, snapshot: bool = False, moving_average: bool = False) -> None:
         """Upload the validation set once (device-resident fp32 images, int64 labels) and allocate the pass's buffers and
         the host record ring.  With ``use_graph`` the whole pass is captured as one CUDA graph.
 
         ``snapshot``: peers may push weights into this (the chief's) arena at any time (K < N, interval mode).  The pass then
         scores a private copy of the newest committed weights that is checked to hold exactly one global step
         (csrc/eval_snapshot.cu): up to SNAP_ATTEMPTS select / copy / validate attempts run in front of the chunks, and a pass
-        whose attempts all fail is dropped by :meth:`eval_records` (counted in ``eval_dropped``)."""
+        whose attempts all fail is dropped by :meth:`eval_records` (counted in ``eval_dropped``).
+
+        ``moving_average``: score the moving average (after :meth:`arm_moving_average`) instead of the weights.  The pass
+        first writes the bf16 copy of the average's conv2 / fc1 weights (its tensor-core operands), rounded as the training
+        shadow is, and its record names the step of the averaged weights."""
+        if moving_average and (self._ema is None or snapshot):
+            raise ValueError("arm_eval(moving_average=True) needs arm_moving_average() first and no snapshot")
         self._leave_native_runner()
         lib, dev = self.lib, self.device
         x = torch.as_tensor(np.ascontiguousarray(images) if isinstance(images, np.ndarray) else images, dtype=torch.float32)
@@ -932,8 +1002,18 @@ class CudaLeNetEngine(_CudaEngine):
             self._ev_snap = _Snapshot(self, self._snap, self._snap16, self._snap_bf_ranges, self._snap_keep)
             self._snap_state = self._ev_snap.state
             self._ev_views = (self.spec.views(self._snap), self.spec.views(self._snap16))
+        elif moving_average:
+            # arena-sized like _snap16; only the conv2 / fc1 weight ranges are written
+            self._ev_ema16 = torch.zeros(self.spec.arena_numel, dtype=bf, device=dev)
+            self._ev_ema_ranges = []
+            for name in ("conv2_weights", "fc1_weights"):
+                q = self.spec.param(name)
+                assert q.offset % 4 == 0 and q.numel % 4 == 0, name
+                self._ev_ema_ranges += [q.offset, q.offset + q.numel]
+            self._ev_views = (self.spec.views(self._ema), self.spec.views(self._ev_ema16))
         else:
             self._ev_views = (self.p, self.pb)
+        self._ev_average = bool(moving_average)
         self._target = None
         self._launch_eval(publish=False)        # sets the kernels' function attributes outside a capture
         torch.cuda.synchronize()
@@ -956,18 +1036,25 @@ class CudaLeNetEngine(_CudaEngine):
     def _launch_eval(self, publish: bool, logits_out: Optional[torch.Tensor] = None, p=None, pb=None) -> None:
         """One pass over the validation set with the weight views ``p`` (fp32) / ``pb`` (bf16): by default the armed ones --
         the live arena, or the snapshot, which the pass then takes first."""
+        lib, sp = self.lib, stream_ptr()
+        null = ctypes.c_void_p(0)
         if p is None:
             if self._snapshot:
                 self._launch_snapshot(self.SNAP_ATTEMPTS)
+            elif self._ev_average:
+                # the bf16 operands of the average (no weights: the kernel only converts)
+                check(lib.dm_moving_average(ptr(self._ema), null, ctypes.c_longlong(self.spec.arena_numel), null,
+                                            ctypes.c_double(0.0), null, ptr(self._ev_ema16),
+                                            *[ctypes.c_longlong(v) for v in self._ev_ema_ranges], sp), "moving_average_bf16")
             p, pb = self._ev_views
-        lib, sp = self.lib, stream_ptr()
         n, C = self._ev_x.shape[0], self._ev_a1.shape[0]
         stride = self._ev_hpart.stride(0)
-        null = ctypes.c_void_p(0)
         ring = ptr(self._ev_ring) if publish else null
         if self._snapshot and p is self._ev_views[0]:
             st = self._snap_state.data_ptr()
             step_ptr, status_ptr = ctypes.c_void_p(st), ctypes.c_void_p(st + 4)     # SnapState.step, SnapState.status
+        elif self._ev_average and p is self._ev_views[0]:
+            step_ptr, status_ptr = ptr(self._ema_step), null                         # step of the averaged weights
         else:
             step_ptr, status_ptr = self._epoch_ptr, null
         check(lib.dm_eval_stamp(ptr(self._ev_state), sp), "eval_stamp")
@@ -1284,6 +1371,9 @@ class CudaMlpEngine(_CudaEngine):
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1
         self.h_loss_bufs[slot].copy_(self.d_loss_acc, non_blocking=True)     # result read-back is part of the step
+        if with_sync and self._ema is not None:
+            self._launch_moving_average()
+            n += 1
         self.launches_per_step = n
 
     def _eval_forward(self, images: torch.Tensor, labels: torch.Tensor, B: int) -> None:

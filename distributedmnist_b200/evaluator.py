@@ -20,6 +20,7 @@ from typing import Optional
 
 import torch
 
+from . import moving_average
 from .checkpoint import Saver, get_checkpoint_state, resolve_checkpoint_path
 from .engine import TorchEngine
 from .flags import FLAGS
@@ -55,7 +56,17 @@ def do_eval(engine, writer: Optional[SummaryWriter], data_set, flags=FLAGS, prev
         print("Could not restore %s: %s" % (path, e))
         sys.stdout.flush()
         return prev_global_step
-    engine.params.copy_(engine.spec.from_state_dict(state).to(engine.params.device))
+    if getattr(flags, "eval_moving_average", False):
+        # TF's variables_to_restore(): every variable is loaded from its moving average
+        flat = moving_average.from_state_dict(engine.spec, state)
+        if flat is None:
+            print("Could not restore %s: the checkpoint holds no moving averages (<variable>%s); it was written without "
+                  "--moving_average_decay" % (path, moving_average.SUFFIX))
+            sys.stdout.flush()
+            return prev_global_step
+        engine.params.copy_(flat.to(engine.params.device))
+    else:
+        engine.params.copy_(engine.spec.from_state_dict(state).to(engine.params.device))
     if hasattr(engine, "params_updated"):
         engine.params_updated()
     print("Succesfully loaded model from %s at step=%s." % (ckpt.model_checkpoint_path, global_step))

@@ -266,6 +266,14 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_float("target_accuracy", 0.0, "With --eval_every_steps: stop the run after the first in-training evaluation "
                                            "whose validation accuracy is >= this value, and report the training time it "
                                            "took (worker0_time_to_accuracy.json); 0 = off, else 0 < A <= 1")
+    F.DEFINE_float("moving_average_decay", 0.0, "Chief: keep an exponential moving average of the weights with this decay "
+                                                "(TF's ExponentialMovingAverage, num_updates = global step), saved in every "
+                                                "checkpoint as <variable>/ExponentialMovingAverage; 0 = off, else 0 < D < 1.  "
+                                                "K = N or --worker_times_cdf_method only")
+    F.DEFINE_boolean("eval_moving_average", False, "Score the moving average instead of the live weights: in training, the "
+                                                   "in-training evaluation and --target_accuracy (needs --moving_average_decay "
+                                                   "and --eval_every_steps); in the evaluator, the checkpoint's "
+                                                   "<variable>/ExponentialMovingAverage tensors")
     return F
 
 

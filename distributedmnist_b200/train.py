@@ -31,6 +31,7 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
+from . import moving_average
 from .checkpoint import Saver
 from .engine import make_engine
 from .flags import FLAGS
@@ -61,8 +62,13 @@ class _AsyncCheckpointer:
     done with it, and at most one capture is in flight.  A capture that found no consistent snapshot writes no file; it is
     counted in ``failed`` and retried at the next call instead of after another ``interval_s``."""
 
-    def __init__(self, train_dir: str, spec, interval_s: float, engine=None, timeout_s: float = 30.0):
+    def __init__(self, train_dir: str, spec, interval_s: float, engine=None, timeout_s: float = 30.0, average=None):
         self.train_dir, self.spec, self.interval_s = train_dir, spec, interval_s
+        # --moving_average_decay: every file also holds <variable>/ExponentialMovingAverage.  ``average`` is the torch
+        # engine's average arena (saved with the weights, on the training thread); a device capture carries its own copy
+        # of the average, taken after the same step as the weights
+        self.average = average
+        self._device_average = engine is not None and getattr(engine, "_ck_ema_dev", None) is not None
         self.saver = Saver()
         self._next = time.time() + interval_s
         self._thread: Optional[threading.Thread] = None
@@ -100,6 +106,8 @@ class _AsyncCheckpointer:
             self._save_final()
             return
         state = self.spec.to_state_dict(params)  # consistent snapshot (device -> host copy)
+        if self.average is not None:
+            state.update(moving_average.to_state_dict(self.spec, self.average))
         if self._thread is not None:
             self._thread.join()
         self._thread = threading.Thread(target=self.saver.save, args=(self.train_dir, state, global_step))
@@ -161,7 +169,10 @@ class _AsyncCheckpointer:
                     return
                 buf, step = item
                 try:
-                    self.saver.save(self.train_dir, self.spec.to_state_dict(self.engine.ckpt_host[buf]), step)
+                    state = self.spec.to_state_dict(self.engine.ckpt_host[buf])
+                    if self._device_average:
+                        state.update(moving_average.to_state_dict(self.spec, self.engine.ckpt_ema_host[buf]))
+                    self.saver.save(self.train_dir, state, step)
                 except BaseException as e:  # noqa: BLE001  (re-raised by close())
                     self._error = e
                 finally:
@@ -316,6 +327,32 @@ def check_target_flags(flags, ctx: ReplicaContext) -> None:
                          % (flags.backend, "" if ctx.on_gpu else ", no GPU", ctx.world_size))
 
 
+def check_moving_average_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate: int) -> None:
+    """``--moving_average_decay`` / ``--eval_moving_average`` combinations that cannot work, rejected before any device
+    work starts.  The same rule holds on every engine, so a flag set means the same thing everywhere."""
+    d = float(getattr(flags, "moving_average_decay", 0.0) or 0.0)
+    on_eval = bool(getattr(flags, "eval_moving_average", False))
+    if d == 0.0:
+        if on_eval:
+            raise ValueError("--eval_moving_average needs --moving_average_decay: there is no moving average to score")
+        return
+    if not 0.0 < d < 1.0:
+        raise ValueError("--moving_average_decay must lie in (0, 1) (0 = off), got %r" % d)
+    # the chief updates the average from its arena after each of its steps: that arena must hold exactly one global step
+    # then, and name it -- true only when every step waits for all N replicas and no peer pushes weights in between
+    why = ": peers push weights into the chief's arena at any time, so the chief cannot name the global steps it would " \
+          "average (supported: K = N, or --worker_times_cdf_method without --interval_method)"
+    if flags.interval_method:
+        raise ValueError("--moving_average_decay cannot be combined with --interval_method" + why)
+    if not getattr(flags, "worker_times_cdf_method", False) and num_replicas_to_aggregate != ctx.world_size:
+        raise ValueError("--moving_average_decay needs --num_replicas_to_aggregate = number of replicas (%d), got %d (K %s N)"
+                         % (ctx.world_size, num_replicas_to_aggregate,
+                            "<" if num_replicas_to_aggregate < ctx.world_size else ">") + why)
+    if on_eval and getattr(flags, "eval_every_steps", 0) <= 0:
+        raise ValueError("--eval_moving_average needs --eval_every_steps > 0: it selects the weights the in-training "
+                         "evaluation scores")
+
+
 def need_count(target: float, examples: int) -> int:
     """Smallest correct count ``need`` with ``need / examples >= target``, exactly (the decimal value of ``target``)."""
     return math.ceil(Fraction(str(target)) * examples)
@@ -381,9 +418,12 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     is_chief = ctx.is_chief
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
     check_target_flags(flags, ctx)
+    check_moving_average_flags(flags, ctx, num_replicas_to_aggregate)
     check_device_data_flags(flags, ctx, dataset)
     device_data = bool(getattr(flags, "device_data", False))
     target = float(getattr(flags, "target_accuracy", 0.0) or 0.0)
+    ema_decay = float(getattr(flags, "moving_average_decay", 0.0) or 0.0) if is_chief else 0.0
+    eval_average = bool(ema_decay and getattr(flags, "eval_moving_average", False))
 
     backend = make_backend(ctx, flags.backend, flags)
     engine = make_engine(flags, ctx, backend)
@@ -410,6 +450,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
 
     # Supervisor semantics: chief restores the newest checkpoint, everyone gets it.
     restored_step = 0
+    restored_average = None        # --moving_average_decay: the averages of the restored checkpoint, if it holds all
+    restored = False
     if is_chief:
         os.makedirs(flags.train_dir, exist_ok=True)
         latest = Saver.latest(flags.train_dir)
@@ -417,6 +459,9 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             state, restored_step = Saver.restore(latest)
             engine.params.copy_(spec.from_state_dict(state).to(engine.params.device))
             log.info("Restored model from %s at step=%d" % (latest, restored_step))
+            restored = True
+            if ema_decay:
+                restored_average = moving_average.from_state_dict(spec, state)
     if num_workers > 1:
         restored_step = backend.all_gather_object(restored_step)[0]
         if restored_step > 0:
@@ -427,6 +472,20 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             backend.set_global_step(restored_step)
     if hasattr(engine, "params_updated"):
         engine.params_updated()
+    if ema_decay:
+        # the chief's average starts from the restored averages, else from the (initial or restored) weights; from here on
+        # every global step ends with its update (GPU path: a node at the end of the chief's step graph)
+        if fused_step:
+            engine.arm_moving_average(ema_decay)
+        else:
+            engine.arm_moving_average(ema_decay, restored_step)
+        if restored_average is not None:
+            engine.load_moving_average(restored_average)
+        elif restored:
+            log.info("Moving average: the restored checkpoint holds no complete set of averages; they start from the "
+                     "restored weights")
+        log.info("Moving average of the weights: decay %g; the in-training evaluation scores the %s weights"
+                 % (ema_decay, "averaged" if eval_average else "live"))
     log.info("%s Supervisor" % datetime.now())
 
     # --eval_every_steps: the chief scores the validation set after every E-th global step and after the last one.  GPU path:
@@ -440,7 +499,10 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     # the host cannot name the step a pass scores in advance, so passes follow the consumed global step (eval_due)
     snapshot_eval = device_eval and bool(getattr(flags, "eval_snapshot", False)) and not exact
     if device_eval:
-        engine.arm_eval(dataset_test.images, dataset_test.labels, snapshot=snapshot_eval)
+        if eval_average:
+            engine.arm_eval(dataset_test.images, dataset_test.labels, snapshot=snapshot_eval, moving_average=True)
+        else:
+            engine.arm_eval(dataset_test.images, dataset_test.labels, snapshot=snapshot_eval)
     if device_data:
         # every replica keeps its own copy, in its own shuffled order: a step's input is then B row indices
         engine.arm_train_data(dataset.images, dataset.labels)
@@ -471,7 +533,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         if device_ckpt:
             engine.arm_checkpoint(snapshot=not exact)
         ckpt = _AsyncCheckpointer(flags.train_dir, spec, flags.save_interval_secs, engine=engine if device_ckpt else None,
-                                  timeout_s=flags.sync_timeout_ms * 1e-3)
+                                  timeout_s=flags.sync_timeout_ms * 1e-3,
+                                  average=engine._ema if ema_decay and not device_ckpt else None)
     summary = SummaryWriter(flags.train_dir) if (is_chief and flags.should_summarize) else None
 
     # Even if not using timeout, we want to wait until all machines are ready (reference :275-277).
@@ -585,7 +648,10 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             engine.enqueue_eval()
             return
         t0 = time.time()
-        loss, acc = engine.evaluate(dataset_test.images, dataset_test.labels)
+        if eval_average:
+            loss, acc = engine.evaluate(dataset_test.images, dataset_test.labels, moving_average=True)
+        else:
+            loss, acc = engine.evaluate(dataset_test.images, dataset_test.labels)
         t1 = time.time()
         n_ex = dataset_test.num_examples
         correct = int(round(acc * n_ex))
@@ -693,6 +759,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 else opt.apply_gradients(engine.params, engine.grads, ctx.rank, cdf)
             if info.applied and hasattr(engine, "params_updated") and not hasattr(engine, "train_step"):
                 engine.params_updated()
+            if ema_decay and info.applied:
+                engine.update_moving_average(info.global_step)
         la = engine.loss_acc() if (do_log or flags.timeline_logging) else None
         t3 = time.perf_counter()
         if eval_every:
@@ -737,6 +805,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         save_evals()
     if tta is not None:
         report = tta.report(engine.start_stamp_ns() if device_eval else tta_wall0)
+        if eval_average:
+            report["weights"] = "moving_average"       # the evaluations scored the averaged weights
         results["time_to_accuracy"] = report
         with open(os.path.join(flags.train_dir, "worker%d_time_to_accuracy.json" % ctx.rank), "w") as f:
             json.dump(report, f, indent=1)

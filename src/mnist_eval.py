@@ -1,7 +1,8 @@
 """Evaluator binary: wipe eval_dir, then score checkpoints as they appear.
 
 Command-line compatible with the reference's src/mnist_eval.py:30-35
-(``--eval_dir --checkpoint_dir --eval_interval_secs --run_once``).
+(``--eval_dir --checkpoint_dir --eval_interval_secs --run_once``).  ``--eval_moving_average`` scores each checkpoint's
+``<variable>/ExponentialMovingAverage`` tensors instead of its weights, and skips a checkpoint that has none.
 """
 import _bootstrap  # noqa: F401
 

@@ -1,0 +1,189 @@
+#!/usr/bin/env python
+"""Cost and benefit of ``--moving_average_decay`` on one GPU.  Prints one JSON line.
+
+1. Step time with and without the average: each configuration in a process of its own, alternated for ``--rounds`` rounds.
+   A process builds the engine (K = N = 1), replays ``--warmup`` steps, then times ``--steps`` back-to-back steps from a
+   device-resident packed batch with CUDA events around the whole window.  Configurations: lenet at batch 256, and mlp3 at
+   batch 8192 / hidden 4096 (an arena of about 20 M floats).
+2. The update kernel alone on each arena (CUDA events over 200 launches): the update, the update plus the bf16 copy of
+   lenet's conv2 / fc1 ranges, and that copy alone (what an averaged evaluation pass runs first).
+3. Time to accuracy at K = N on one GPU, scoring the live weights versus the averaged ones: ``train()`` with the data, the
+   target and the evaluation period of ``tools/time_to_accuracy.py``, alternated for ``--rounds`` rounds.
+
+    python tools/moving_average.py [--rounds 3] [--decay 0.999] [--target 0.95] [--out results/moving_average.json]
+"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import tempfile
+
+ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
+sys.path.insert(0, ROOT)
+
+STEP_CONFIGS = [("lenet", 256, 1024), ("mlp3", 8192, 4096)]
+
+
+def gpu_info():
+    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
+                       capture_output=True, text=True)
+    name, power, clock = [v.strip() for v in r.stdout.strip().split(",")] if r.returncode == 0 else ("?", "?", "?")
+    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
+
+
+def _engine(model, batch, hidden, decay):
+    import torch
+    from distributedmnist_b200.engine_cuda import CudaLeNetEngine, CudaMlpEngine
+    from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
+    from distributedmnist_b200.parallel.context import ReplicaContext
+    from distributedmnist_b200.parallel.fused import FusedBackend
+    from distributedmnist_b200.schedule import LearningRateSchedule
+    torch.cuda.set_device(0)
+    be = FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
+    eng = CudaLeNetEngine(batch, be, use_graph=True) if model == "lenet" else \
+        CudaMlpEngine(model, batch, be, hidden=hidden, use_graph=True)
+    eng.attach_optimizer(SyncReplicasOptimizer(be, LearningRateSchedule(0.01, 10 ** 6, 1.0), 1, 1))
+    if decay:
+        eng.arm_moving_average(decay)
+    return eng, be
+
+
+def child_step_time(model, batch, hidden, decay, steps, warmup):
+    import torch
+    eng, be = _engine(model, batch, hidden, decay)
+    g = torch.Generator().manual_seed(1)
+    packed = [eng.pack_batch(torch.rand(batch, 784, generator=g) - 0.5, torch.randint(0, 10, (batch,), generator=g),
+                             pin=False).cuda() for _ in range(2)]
+    for i in range(warmup):
+        eng.step_packed(packed[i & 1])
+    torch.cuda.synchronize()
+    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    t0.record()
+    for i in range(steps):
+        eng.step_packed(packed[i & 1])
+    t1.record()
+    torch.cuda.synchronize()
+    be.check_error()
+    us = t0.elapsed_time(t1) * 1e3 / steps
+    eng._leave_native_runner()
+    return dict(model=model, batch=batch, hidden=hidden if model != "lenet" else None, average=bool(decay),
+                arena_floats=eng.spec.arena_numel, launches_per_step=eng.launches_per_step, us_per_step=us)
+
+
+def kernel_times(iters=200):
+    import ctypes
+    import torch
+    from distributedmnist_b200.models import get_model
+    from distributedmnist_b200.ops.lib import check, load, ptr, stream_ptr
+    lib = load()
+    out = []
+    for model, hidden in (("lenet", 1024), ("mlp3", 4096)):
+        spec = get_model(model, hidden)[0]
+        n = spec.arena_numel
+        s, w = torch.randn(n, device="cuda"), torch.randn(n, device="cuda")
+        bf = torch.zeros(n, dtype=torch.bfloat16, device="cuda")
+        epoch = torch.full((1,), 1000, dtype=torch.int32, device="cuda")
+        rg = [0, 0, 0, 0]
+        if model == "lenet":
+            rg = []
+            for name in ("conv2_weights", "fc1_weights"):
+                q = spec.param(name)
+                rg += [q.offset, q.offset + q.numel]
+        L = ctypes.c_longlong
+        variants = {"update": (ptr(w), None, [0, 0, 0, 0]), "update_bf16": (ptr(w), ptr(bf), rg),
+                    "bf16_only": (ctypes.c_void_p(0), ptr(bf), rg)}
+        row = dict(model=model, arena_floats=n)
+        for name, (wp, bp, r) in variants.items():
+            if model != "lenet" and name != "update":
+                continue
+
+            def launch():
+                check(lib.dm_moving_average(ptr(s), wp, L(n), ptr(epoch), ctypes.c_double(0.999), None, bp,
+                                            *map(L, r), stream_ptr()), "moving_average")
+            for _ in range(10):
+                launch()
+            t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            t0.record()
+            for _ in range(iters):
+                launch()
+            t1.record()
+            torch.cuda.synchronize()
+            us = t0.elapsed_time(t1) * 1e3 / iters
+            nbytes = n * 12 if name == "update" else (n * 12 + (rg[1] - rg[0] + rg[3] - rg[2]) * 2 if name == "update_bf16"
+                                                      else n * 4 + (rg[1] - rg[0] + rg[3] - rg[2]) * 2)
+            row[name + "_us"] = us
+            row[name + "_gbps"] = nbytes / us * 1e-3
+        out.append(row)
+    return out
+
+
+def tta_run(ds, args, average: bool) -> dict:
+    from distributedmnist_b200.flags import FLAGS
+    from distributedmnist_b200.parallel.context import init_context
+    from distributedmnist_b200.train import train
+    FLAGS.reset()
+    with tempfile.TemporaryDirectory() as d:
+        FLAGS.parse(["--train_dir=%s" % d, "--batch_size=128", "--max_steps=%d" % args.max_steps, "--model=lenet",
+                     "--device_data=true", "--eval_every_steps=%d" % args.eval_every, "--target_accuracy=%r" % args.target,
+                     "--initial_learning_rate=0.05", "--log_every=100000", "--save_results_period=100000000",
+                     "--save_interval_secs=1e9", "--moving_average_decay=%r" % args.decay]
+                    + (["--eval_moving_average=true"] if average else []))
+        ctx = init_context(FLAGS)
+        res = train(ctx, ds.train, ds.validation, FLAGS)
+    rep = res["time_to_accuracy"]
+    return dict(weights="moving_average" if average else "live", reached=rep["reached"], global_step=rep["global_step"],
+                accuracy=rep["accuracy"], train_time_s=rep["train_time_s"], wall_time_s=rep["wall_time_s"],
+                final_step=res["final_step"])
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--rounds", type=int, default=3)
+    ap.add_argument("--steps", type=int, default=2000)
+    ap.add_argument("--warmup", type=int, default=200)
+    ap.add_argument("--decay", type=float, default=0.999)
+    ap.add_argument("--target", type=float, default=0.95)
+    ap.add_argument("--eval-every", type=int, default=20)
+    ap.add_argument("--max-steps", type=int, default=5000)
+    ap.add_argument("--out", default=None)
+    ap.add_argument("--child", default=None, help=argparse.SUPPRESS)
+    args = ap.parse_args()
+    for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
+        os.environ.pop(k, None)
+    if args.child:
+        model, batch, hidden, decay = args.child.split(":")
+        print(json.dumps(child_step_time(model, int(batch), int(hidden), float(decay), args.steps, args.warmup)))
+        return
+    steps = []
+    for _ in range(args.rounds):
+        for model, batch, hidden in STEP_CONFIGS:
+            for decay in (0.0, args.decay):
+                r = subprocess.run([sys.executable, os.path.abspath(__file__), "--steps=%d" % args.steps,
+                                    "--warmup=%d" % args.warmup, "--child=%s:%d:%d:%r" % (model, batch, hidden, decay)],
+                                   capture_output=True, text=True)
+                if r.returncode != 0:
+                    raise RuntimeError(r.stdout[-2000:] + r.stderr[-4000:])
+                steps.append(json.loads(r.stdout.strip().splitlines()[-1]))
+    from distributedmnist_b200 import data as mnist_data
+    from distributedmnist_b200.flags import FLAGS
+    kern = kernel_times()
+    FLAGS.reset()
+    ds = mnist_data.load_mnist(FLAGS.data_dir, seed=FLAGS.seed, synthetic=True)
+    tta = []
+    for _ in range(args.rounds):
+        for average in (False, True):
+            tta.append(tta_run(ds, args, average))
+    out = dict(tool="moving_average", decay=args.decay, step_time=steps, kernel=kern,
+               time_to_accuracy=dict(data="synthetic MNIST-shaped (not MNIST)", target=args.target, batch_size=128,
+                                     eval_every_steps=args.eval_every, runs=tta), **gpu_info())
+    line = json.dumps(out)
+    if args.out:
+        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
+        with open(args.out, "w") as f:
+            f.write(line + "\n")
+    print(line)
+
+
+if __name__ == "__main__":
+    main()
