@@ -84,6 +84,14 @@ class Saver:
         self._kept: List[str] = []
         self._lock = threading.Lock()
 
+    def adopt(self, train_dir: str) -> None:
+        """Continue the retention list of ``train_dir``'s state file, so ``max_to_keep`` also removes the checkpoints an
+        earlier run wrote there."""
+        st = get_checkpoint_state(train_dir)
+        if st is not None:
+            with self._lock:
+                self._kept = [os.path.basename(p) for p in st.all_model_checkpoint_paths]
+
     # ---- write ------------------------------------------------------------
     def save(self, train_dir: str, tensors: Dict[str, torch.Tensor], global_step: int) -> str:
         os.makedirs(train_dir, exist_ok=True)

@@ -24,6 +24,7 @@ from typing import Callable, Optional, Tuple
 import numpy as np
 import torch
 
+from . import best
 from . import moving_average as ema
 from .models import ModelSpec, dropout_keep_mask, dropout_seed_mix, get_model, loss_and_accuracy
 from .models.lenet import FC1_OUT
@@ -160,6 +161,29 @@ class TorchEngine(ComputeEngine):
 
     def h2d_bytes_per_step(self) -> int:
         return self._h2d
+
+    # ---- best-scoring weights (see best.py) -------------------------------------------------------------------------------
+    _best_correct = 0
+    _best: Optional[Tuple] = None
+
+    def arm_best(self, initial_correct: int = 0) -> None:
+        """Keep the weights of the best evaluation from here on; ``initial_correct``: an earlier run's best count."""
+        self._best_correct, self._best = int(initial_correct), None
+
+    def note_eval(self, step: int, n: int, examples: int, correct: int, loss_sum: float,
+                  moving_average: bool = False) -> bool:
+        """After an ``evaluate`` of global step ``step`` (``moving_average``: of the average arena): keep a copy of the
+        scored arena if the pass is the new best.  True if it is."""
+        if not best.improves(correct, examples, n, self._best_correct):
+            return False
+        flat = self._ema if moving_average else self.params
+        self._best_correct = int(correct)
+        self._best = (flat.detach().clone(), int(step), int(correct), int(examples), float(loss_sum))
+        return True
+
+    def best_weights(self) -> Optional[Tuple]:
+        """``(fp32 arena, global step, correct, examples, loss_sum)`` of the best pass since :meth:`arm_best`, or None."""
+        return self._best
 
 
 def make_engine(flags, ctx, backend, force_torch: bool = False) -> ComputeEngine:

@@ -26,12 +26,14 @@ from __future__ import annotations
 
 import contextlib
 import ctypes
+import gc
 import os
 from typing import Optional, Tuple
 
 import numpy as np
 import torch
 
+from .best import BEST_CORRECT_WORD, BEST_EXAMPLES_WORD, BEST_STEP_WORD, BEST_VALID_WORD
 from .engine import ComputeEngine
 from .models import get_model
 from .models.lenet import dropout_seed_mix
@@ -39,6 +41,22 @@ from .ops import gemm as G
 from .ops.lib import check, load, ptr, stream_ptr
 from .parallel.backends import StepInfo
 from .parallel.fused import FusedBackend
+
+
+@contextlib.contextmanager
+def _capture(graph: torch.cuda.CUDAGraph, stream: torch.cuda.Stream):
+    """Capture into ``graph`` on ``stream`` with the cyclic garbage collector paused.  Engines sit in reference cycles (an
+    engine and its _Snapshot), so only the collector frees an old one, and its graphs' destructors would then run inside
+    this capture, where destroying a graph is not permitted: the capture would be invalidated.  thread_local: other threads
+    (NCCL watchdog, pin-memory) may call CUDA while we capture."""
+    enabled = gc.isenabled()
+    gc.disable()
+    try:
+        with torch.cuda.graph(graph, stream=stream, capture_error_mode="thread_local"):
+            yield
+    finally:
+        if enabled:
+            gc.enable()
 
 
 class _RunnerEvent:
@@ -429,9 +447,8 @@ class _CudaEngine(ComputeEngine):
                 self._launch_step(s, False)           # warm-up (gradients only): sets func attributes outside capture
                 torch.cuda.synchronize()
                 gr = torch.cuda.CUDAGraph()
-                # thread_local: other threads (NCCL watchdog, pin-memory) may call CUDA while we capture
                 cap = torch.cuda.Stream(device=self.device, priority=self._main_priority)
-                with torch.cuda.graph(gr, stream=cap, capture_error_mode="thread_local"):
+                with _capture(gr, cap):
                     self._launch_step(s, with_sync)
                 self._graphs[key] = (gr, with_sync)
             self._graphs[key][0].replay()
@@ -1015,6 +1032,7 @@ class CudaLeNetEngine(_CudaEngine):
             self._ev_views = (self.p, self.pb)
         self._ev_average = bool(moving_average)
         self._target = None
+        self._best = None
         self._launch_eval(publish=False)        # sets the kernels' function attributes outside a capture
         torch.cuda.synchronize()
         if self._snapshot:
@@ -1025,7 +1043,7 @@ class CudaLeNetEngine(_CudaEngine):
         if self.use_graph:
             gr = torch.cuda.CUDAGraph()
             cap = torch.cuda.Stream(device=self.device)
-            with torch.cuda.graph(gr, stream=cap, capture_error_mode="thread_local"):
+            with _capture(gr, cap):
                 self._launch_eval(publish=True)
             self._ev_graph = gr
 
@@ -1050,13 +1068,17 @@ class CudaLeNetEngine(_CudaEngine):
         n, C = self._ev_x.shape[0], self._ev_a1.shape[0]
         stride = self._ev_hpart.stride(0)
         ring = ptr(self._ev_ring) if publish else null
-        if self._snapshot and p is self._ev_views[0]:
+        armed = p is self._ev_views[0]
+        if self._snapshot and armed:
             st = self._snap_state.data_ptr()
             step_ptr, status_ptr = ctypes.c_void_p(st), ctypes.c_void_p(st + 4)     # SnapState.step, SnapState.status
-        elif self._ev_average and p is self._ev_views[0]:
+            scored = self._snap
+        elif self._ev_average and armed:
             step_ptr, status_ptr = ptr(self._ema_step), null                         # step of the averaged weights
+            scored = self._ema
         else:
             step_ptr, status_ptr = self._epoch_ptr, null
+            scored = self.params if armed else None                                  # fp32 arena the pass scores
         check(lib.dm_eval_stamp(ptr(self._ev_state), sp), "eval_stamp")
         for s in range(0, n, C):
             m = min(C, n - s)
@@ -1071,6 +1093,12 @@ class CudaLeNetEngine(_CudaEngine):
                                    ptr(p["fc2_weights"]), ptr(p["fc2_biases"]), ptr(self._ev_y[s:s + m]), ptr(self._ev_ws),
                                    ptr(self._ev_state), step_ptr, status_ptr, ring, self.EVAL_RING, lg, m,
                                    int(s + m == n), sp), "eval_head")
+        if publish and self._best is not None and scored is not None:
+            state, decision, arena = self._best
+            check(lib.dm_eval_best_decide(ptr(self._ev_state), step_ptr, status_ptr, ctypes.c_uint(n), ptr(state),
+                                          ptr(decision), sp), "eval_best_decide")
+            check(lib.dm_eval_best_copy(ptr(decision), ptr(scored), ptr(arena), ctypes.c_longlong(arena.numel()), sp),
+                  "eval_best_copy")
         if publish and self._target is not None:
             need, margin = self._target
             check(lib.dm_eval_target(ptr(self._ev_state), step_ptr, status_ptr, ctypes.c_uint(need), ctypes.c_uint(n),
@@ -1210,6 +1238,41 @@ class CudaLeNetEngine(_CudaEngine):
     def start_stamp_ns(self) -> int:
         """The stamp of :meth:`enqueue_start_stamp` (a device read, ordered after the current stream's work)."""
         return int(self._tta_t0.cpu()[0])
+
+    # ---- best-scoring weights (csrc/eval_best.cu) -------------------------------------------------------------------------
+    # With best-keeping armed, every evaluation pass ends (before eval_target) with eval_best_decide, which applies the
+    # selection rule of best.improves to the pass's record and BestState, and eval_best_copy, which copies the arena the pass
+    # scored into the best arena when decide chose it.  Nothing is read back until best_weights().
+    _best = None                   # (BestState bytes, decision word, best arena), see arm_best
+
+    def arm_best(self, initial_correct: int = 0) -> None:
+        """Chief, after :meth:`arm_eval`: every evaluation pass keeps its weights if it beats every earlier pass and
+        ``initial_correct`` (an earlier run's best count).  Re-captures the evaluation graph."""
+        if getattr(self, "_ev_x", None) is None:
+            raise RuntimeError("arm_best: arm_eval() first")
+        n = int(self._ev_x.shape[0])
+        if not 0 <= int(initial_correct) <= n:
+            raise ValueError("arm_best: initial count %d of %d examples" % (initial_correct, n))
+        self._leave_native_runner()
+        words = torch.zeros(int(self.lib.dm_best_state_bytes()) // 4, dtype=torch.int32)
+        words[BEST_CORRECT_WORD] = int(initial_correct)
+        self._best = (words.to(self.device), torch.zeros(1, dtype=torch.int32, device=self.device),
+                      torch.zeros(self.spec.arena_numel, dtype=torch.float32, device=self.device))
+        self._capture_eval()
+
+    def best_weights(self):
+        """``(fp32 arena, global step, correct, examples, loss_sum)`` of the best pass since :meth:`arm_best`, or None when
+        no pass beat the initial count (synchronises the device)."""
+        if self._best is None:
+            return None
+        torch.cuda.synchronize()
+        state, _decision, arena = self._best
+        w = state.cpu()
+        if int(w[BEST_VALID_WORD]) == 0:
+            return None
+        u = w.numpy().view(np.uint32)
+        return (arena.clone(), int(u[BEST_STEP_WORD]), int(u[BEST_CORRECT_WORD]), int(u[BEST_EXAMPLES_WORD]),
+                float(w[:2].numpy().view(np.float64)[0]))
 
 
 # dm_dense10_xent (csrc/mlp_simt.cu) stages the output-layer weights as [H][11] floats and refuses more than 220 KiB

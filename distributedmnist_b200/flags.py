@@ -274,6 +274,9 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
                                                    "in-training evaluation and --target_accuracy (needs --moving_average_decay "
                                                    "and --eval_every_steps); in the evaluator, the checkpoint's "
                                                    "<variable>/ExponentialMovingAverage tensors")
+    F.DEFINE_boolean("keep_best_checkpoint", False, "With --eval_every_steps: keep the weights of the best-scoring "
+                                                    "in-training evaluation and save them at the end of the run as "
+                                                    "train_dir/best/model.ckpt-<step> plus worker0_best.json")
     return F
 
 

@@ -32,6 +32,7 @@ import numpy as np
 import torch
 
 from . import moving_average
+from .best import BEST_DIR, BEST_JSON
 from .checkpoint import Saver
 from .engine import make_engine
 from .flags import FLAGS
@@ -327,6 +328,43 @@ def check_target_flags(flags, ctx: ReplicaContext) -> None:
                          % (flags.backend, "" if ctx.on_gpu else ", no GPU", ctx.world_size))
 
 
+def check_best_flags(flags) -> None:
+    """``--keep_best_checkpoint`` combinations that cannot work, rejected before any device work starts.  Where the
+    in-training evaluation itself is refused (check_eval_flags), so is keeping its best weights."""
+    if getattr(flags, "keep_best_checkpoint", False) and getattr(flags, "eval_every_steps", 0) <= 0:
+        raise ValueError("--keep_best_checkpoint needs --eval_every_steps > 0: the best weights are those of the "
+                         "best-scoring in-training evaluation")
+
+
+def read_best(train_dir: str, rank: int) -> Optional[Dict]:
+    """The best-weights summary an earlier run left in ``train_dir``, or None."""
+    try:
+        with open(os.path.join(train_dir, BEST_JSON % rank)) as f:
+            return json.load(f)
+    except FileNotFoundError:
+        return None
+
+
+def save_best(engine, spec, train_dir: str, rank: int, weights: str) -> Optional[Dict]:
+    """Write the best weights the engine kept, if any pass of this run qualified: ``train_dir/best/model.ckpt-<step>``
+    under the plain variable names (the evaluator scores it as it is), then ``worker<rank>_best.json``.  Returns the
+    summary, or None when nothing was written."""
+    b = engine.best_weights()
+    if b is None:
+        return None
+    arena, step, correct, examples, loss_sum = b
+    d = os.path.join(train_dir, BEST_DIR)
+    saver = Saver(max_to_keep=1)
+    saver.adopt(d)                 # a restarted run's better best replaces the earlier one
+    saver.save(d, spec.to_state_dict(arena), step)
+    report = dict(global_step=step, correct=correct, examples=examples, accuracy=correct / float(examples),
+                  mean_loss=loss_sum / examples, weights=weights)
+    with open(os.path.join(train_dir, BEST_JSON % rank), "w") as f:
+        json.dump(report, f, indent=1)
+        f.write("\n")
+    return report
+
+
 def check_moving_average_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate: int) -> None:
     """``--moving_average_decay`` / ``--eval_moving_average`` combinations that cannot work, rejected before any device
     work starts.  The same rule holds on every engine, so a flag set means the same thing everywhere."""
@@ -418,6 +456,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     is_chief = ctx.is_chief
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
     check_target_flags(flags, ctx)
+    check_best_flags(flags)
     check_moving_average_flags(flags, ctx, num_replicas_to_aggregate)
     check_device_data_flags(flags, ctx, dataset)
     device_data = bool(getattr(flags, "device_data", False))
@@ -520,6 +559,17 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                                   "device %globaltimer" if device_eval else "host")
             if device_eval:
                 engine.arm_target(tta.need, STOP_MARGIN)
+    # --keep_best_checkpoint: the chief keeps the weights of its best-scoring evaluation (GPU path: decided and copied on the
+    # device inside the pass's graph; torch engine: after `evaluate`) and writes them once, after the final pass.  A best
+    # file of an earlier run sets the count to beat.
+    keep_best = bool(eval_every and getattr(flags, "keep_best_checkpoint", False))
+    if keep_best:
+        earlier = read_best(flags.train_dir, ctx.rank)
+        best_seed = int(earlier["correct"]) if earlier else 0
+        engine.arm_best(best_seed)
+        if earlier:
+            log.info("Best weights: an earlier run kept the evaluation of global step #%d (%d of %d correct); only a "
+                     "better one replaces it" % (earlier["global_step"], earlier["correct"], earlier["examples"]))
     eval_rows = []                 # (global_step, t_begin_unix_s, eval_seconds, examples, correct, mean_loss)
     last_eval_step = -1
     eval_mark = restored_step      # snapshot passes: global step consumed when the last one was enqueued
@@ -657,6 +707,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         correct = int(round(acc * n_ex))
         eval_rows.append((global_step, t0, t1 - t0, n_ex, correct, loss))
         test_acc_value = correct / float(n_ex)
+        if keep_best:
+            engine.note_eval(global_step, n_ex, n_ex, correct, loss * n_ex, moving_average=eval_average)
         if tta is not None and tta.add(global_step, t0, t1, n_ex, correct, True, t1 - tta_wall0):
             max_steps = min(max_steps, global_step + STOP_MARGIN)
 
@@ -818,6 +870,16 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                         report["train_time_s"], tta.clock, report["wall_time_s"]))
         else:
             log.info("Time to accuracy: target %g not reached" % target)
+    if keep_best:
+        kind = "snapshot" if snapshot_eval else ("moving_average" if eval_average else "live")
+        rep = results["best"] = save_best(engine, spec, flags.train_dir, ctx.rank, kind)
+        if rep is not None:
+            log.info("Best weights: the evaluation of global step #%d (accuracy %f, %d of %d correct, mean loss %f, %s "
+                     "weights) saved under %s" % (rep["global_step"], rep["accuracy"], rep["correct"], rep["examples"],
+                                                  rep["mean_loss"], kind, os.path.join(flags.train_dir, BEST_DIR)))
+        else:
+            log.info("Best weights: no complete evaluation of this run scored more than %d correct; nothing written"
+                     % best_seed)
     if device_times:
         push_device_times(cur_iteration)
 
