@@ -490,11 +490,7 @@ int dm_conv2_fwd(const void* a1, const void* w_bf16, const void* bias, void* out
 }
 
 // dy: [B,14,14,64] bf16 -> dx: [B,14,14,32] bf16
-int dm_conv2_dgrad_dbg(const void* dy, const void* w_bf16, void* dx, int B, void* dbg, void* stream);
 int dm_conv2_dgrad(const void* dy, const void* w_bf16, void* dx, int B, void* stream) {
-  return dm_conv2_dgrad_dbg(dy, w_bf16, dx, B, nullptr, stream);
-}
-int dm_conv2_dgrad_dbg(const void* dy, const void* w_bf16, void* dx, int B, void* dbg, void* stream) {
   using namespace dm;
   CUtensorMap tmDY, tmW;
   if (make_tmap_nhwc_bf16(&tmDY, dy, 64, 14, 14, B, 64, 12, 20, 128)) return 101;
@@ -509,7 +505,7 @@ int dm_conv2_dgrad_dbg(const void* dy, const void* w_bf16, void* dx, int B, void
   const int grid = tiles < max_ctas() ? tiles : max_ctas();
   return (int)launch_kernel(conv2_dgrad_kernel, dim3(grid), dim3(CV_THREADS), DgSmem::TOTAL,
                             reinterpret_cast<cudaStream_t>(stream), tmDY, tmW, reinterpret_cast<__nv_bfloat16*>(dx), tiles,
-                            reinterpret_cast<unsigned long long*>(dbg));
+                            static_cast<unsigned long long*>(nullptr));
 }
 
 // g_w ([25][32][64] fp32) must be zeroed by the caller; the gradient is added to it.  Two launches: the weight-gradient

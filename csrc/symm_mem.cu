@@ -138,11 +138,6 @@ int dm_symm_alloc(unsigned long long bytes, void** out) {
   return 0;
 }
 
-int dm_symm_free(void* p) {
-  DM_CUDA_OK(cudaFree(p));
-  return 0;
-}
-
 int dm_symm_ipc_handle(void* p, void* handle64) {
   cudaIpcMemHandle_t h;
   DM_CUDA_OK(cudaIpcGetMemHandle(&h, p));
@@ -163,12 +158,6 @@ int dm_symm_ipc_open(const void* handle64, void** out) {
 int dm_symm_ipc_close(void* p) {
   DM_CUDA_OK(cudaIpcCloseMemHandle(p));
   return 0;
-}
-
-int dm_can_access_peer(int dev, int peer) {
-  int ok = 0;
-  if (cudaDeviceCanAccessPeer(&ok, dev, peer) != cudaSuccess) return -1;
-  return ok;
 }
 
 int dm_memset_async(void* p, int value, unsigned long long bytes, void* stream) {
@@ -255,23 +244,6 @@ int dm_vmm_map(unsigned long long handle, unsigned long long bytes, int device, 
   int rc = map_handle(api, (CUmemGenericAllocationHandle)handle, bytes, 0, device, &va);
   if (rc) return rc;
   *ptr_out = reinterpret_cast<void*>(va);
-  return 0;
-}
-
-int dm_vmm_unmap(void* ptr, unsigned long long bytes) {
-  using namespace dm;
-  VmmApi* api = vmm_api();
-  if (!api) return -1;
-  DM_DRV_OK(api->MemUnmap(reinterpret_cast<CUdeviceptr>(ptr), bytes));
-  DM_DRV_OK(api->MemAddressFree(reinterpret_cast<CUdeviceptr>(ptr), bytes));
-  return 0;
-}
-
-int dm_vmm_release(unsigned long long handle) {
-  using namespace dm;
-  VmmApi* api = vmm_api();
-  if (!api) return -1;
-  DM_DRV_OK(api->MemRelease((CUmemGenericAllocationHandle)handle));
   return 0;
 }
 

@@ -25,7 +25,6 @@ calls cuDNN, cuBLAS or NCCL.
 from __future__ import annotations
 
 import contextlib
-import ctypes
 import gc
 import os
 from typing import Optional, Tuple
@@ -38,7 +37,7 @@ from .engine import ComputeEngine
 from .models import get_model
 from .models.lenet import dropout_seed_mix
 from .ops import gemm as G
-from .ops.lib import check, load, ptr, stream_ptr
+from .ops.lib import load, stream_ptr
 from .parallel.backends import StepInfo
 from .parallel.fused import FusedBackend
 
@@ -66,9 +65,7 @@ class _RunnerEvent:
         self.lib, self.runner, self.slot = lib, runner, slot
 
     def synchronize(self) -> None:
-        rc = self.lib.dm_runner_wait(self.runner, self.slot)
-        if rc != 0:
-            raise RuntimeError("dm_runner_wait failed: CUDA error %d" % rc)
+        self.lib.dm_runner_wait(self.runner, self.slot)
 
     def query(self) -> bool:
         return self.lib.dm_runner_query(self.runner, self.slot) == 1
@@ -98,19 +95,16 @@ class _Snapshot:
         once.  ``SnapState.step`` / ``.status`` (the first 8 bytes of ``state``) then hold the outcome."""
         eng = self.eng
         lib, sp = eng.lib, stream_ptr()
-        ctrl = ctypes.c_void_p(eng.backend.ctrl.local_ptr)
-        st = ptr(self.state)
+        ctrl = eng.backend.ctrl.local_ptr
+        st = self.state
         interval = int(bool(getattr(eng, "_interval", False)))      # K > N runs the interval commit ordering too
-        r = [ctypes.c_longlong(v) for v in (self.bf_ranges or (0, 0, 0, 0))]
-        s16 = ptr(self.snap16) if self.snap16 is not None else ctypes.c_void_p(0)
+        r = self.bf_ranges or (0, 0, 0, 0)
         for a in range(attempts):
-            check(lib.dm_snap_select(ctrl, st, a, interval, ctypes.c_double(eng.SNAP_WATCHDOG_MS), sp), "snap_select")
-            check(lib.dm_snap_copy(st, ptr(eng.params), ptr(self.snap), s16, ctypes.c_longlong(eng.spec.arena_numel), *r, sp),
-                  "snap_copy")
-            check(lib.dm_snap_validate(ctrl, st, a, attempts, sp), "snap_validate")
+            lib.dm_snap_select(ctrl, st, a, interval, eng.SNAP_WATCHDOG_MS, sp)
+            lib.dm_snap_copy(st, eng.params, self.snap, self.snap16, eng.spec.arena_numel, *r, sp)
+            lib.dm_snap_validate(ctrl, st, a, attempts, sp)
         if self.keep is not None:
-            check(lib.dm_snap_keep(st, ptr(self.snap), ptr(self.keep), ctypes.c_longlong(eng.spec.arena_numel), sp),
-                  "snap_keep")
+            lib.dm_snap_keep(st, self.snap, self.keep, eng.spec.arena_numel, sp)
 
     def stats(self) -> dict:
         """Attempts made, rejected by validate, ended by the watchdog, ended a ring lap behind; passes accepted / failed
@@ -268,8 +262,7 @@ class _CudaEngine(ComputeEngine):
 
     def _gather(self, s: int) -> None:
         img, lbl = self._table
-        check(self.lib.dm_gather_batch(ptr(self._idx_dev[s]), ptr(img), ptr(lbl), self.batch_size, ptr(self.in_dev[s]),
-                                       stream_ptr(self.copy_stream)), "gather_batch")
+        self.lib.dm_gather_batch(self._idx_dev[s], img, lbl, self.batch_size, self.in_dev[s], stream_ptr(self.copy_stream))
 
     def load_indices(self, idx) -> None:
         """Counterpart of :meth:`load_batch` for the armed training set: B row indices -> pinned staging -> device index
@@ -301,10 +294,10 @@ class _CudaEngine(ComputeEngine):
             # into the slot's page-locked staging buffer, once the DMA of its previous fill has read it (a fresh pinned copy
             # per call would go back to torch's host allocator, and be handed out again, while its DMA may still wait)
             s = self._loaded & 1
-            check(self.lib.dm_runner_wait_copy(r, s), "runner_wait_copy")
+            self.lib.dm_runner_wait_copy(r, s)
             self._h_idx[s].copy_(t)
             t = self._h_idx[s]
-        s = int(self.lib.dm_runner_step_indices(r, ctypes.c_void_p(t.data_ptr())))
+        s = int(self.lib.dm_runner_step_indices(r, t))
         if s < 0:
             raise RuntimeError("dm_runner_step_indices failed: CUDA error %d" % -s)
         self._keep_alive[s] = t                          # the DMA reads it asynchronously
@@ -325,7 +318,7 @@ class _CudaEngine(ComputeEngine):
                 self.load_packed(packed)
                 self.train_step()
                 return self.read_result_async()
-        s = int(self.lib.dm_runner_step(r, ctypes.c_void_p(packed.data_ptr())))
+        s = int(self.lib.dm_runner_step(r, packed))
         if s < 0:
             raise RuntimeError("dm_runner_step failed: CUDA error %d" % -s)
         self._keep_alive[s] = packed                     # the DMA reads it asynchronously
@@ -342,19 +335,15 @@ class _CudaEngine(ComputeEngine):
             return None
         torch.cuda.synchronize()                         # hand-over point: nothing of the torch-dispatched path is in flight
         lib = self.lib
-        lib.dm_runner_create.restype = ctypes.c_void_p
         cur = torch.cuda.current_stream()
-        r = lib.dm_runner_create(ctypes.c_void_p(cur.cuda_stream), ctypes.c_void_p(self.copy_stream.cuda_stream),
-                                 ctypes.c_void_p(self._graphs[0][0].raw_cuda_graph_exec()),
-                                 ctypes.c_void_p(self._graphs[1][0].raw_cuda_graph_exec()),
-                                 ctypes.c_void_p(self.in_dev[0].data_ptr()), ctypes.c_void_p(self.in_dev[1].data_ptr()),
-                                 ctypes.c_ulonglong(self._in_bytes), int(self._loaded & 1))
+        r = lib.dm_runner_create(cur.cuda_stream, self.copy_stream.cuda_stream, self._graphs[0][0].raw_cuda_graph_exec(),
+                                 self._graphs[1][0].raw_cuda_graph_exec(), self.in_dev[0], self.in_dev[1], self._in_bytes,
+                                 int(self._loaded & 1))
         if not r:
             return None
         if self._table is not None:
-            check(lib.dm_runner_arm_gather(ctypes.c_void_p(r), ptr(self._idx_dev[0]), ptr(self._idx_dev[1]),
-                                           ptr(self._table[0]), ptr(self._table[1]), self.batch_size), "runner_arm_gather")
-        self._runner = ctypes.c_void_p(r)
+            lib.dm_runner_arm_gather(r, self._idx_dev[0], self._idx_dev[1], self._table[0], self._table[1], self.batch_size)
+        self._runner = r
         self._keep_alive = [None, None]
         return self._runner
 
@@ -608,7 +597,7 @@ class _CudaEngine(ComputeEngine):
         self._leave_native_runner()
         torch.cuda.synchronize()
         off = self.backend._off["epoch"]
-        self._ema_epoch = ctypes.c_void_p(self.backend.ctrl.local_ptr + off)
+        self._ema_epoch = self.backend.ctrl.local_ptr + off
         self._ema_decay = float(decay)
         self._ema = self.params.detach().clone()
         self._ema_step = self.backend._ctrl_bytes[off:off + 4].view(torch.int32).clone()    # step the shadow holds
@@ -618,9 +607,8 @@ class _CudaEngine(ComputeEngine):
         torch.cuda.synchronize()
 
     def _launch_moving_average(self) -> None:
-        check(self.lib.dm_moving_average(ptr(self._ema), ptr(self.params), ctypes.c_longlong(self.spec.arena_numel),
-                                         self._ema_epoch, ctypes.c_double(self._ema_decay), ptr(self._ema_step),
-                                         ctypes.c_void_p(0), *([ctypes.c_longlong(0)] * 4), stream_ptr()), "moving_average")
+        self.lib.dm_moving_average(self._ema, self.params, self.spec.arena_numel, self._ema_epoch, self._ema_decay,
+                                   self._ema_step, None, 0, 0, 0, 0, stream_ptr())
 
     def moving_average(self) -> Tuple[torch.Tensor, int]:
         """(copy of the shadow arena, global step of the weights it was last updated from); synchronises the device."""
@@ -684,18 +672,17 @@ class CudaLeNetEngine(_CudaEngine):
         # early bucket = fc1_weights (96.5 % of the bytes, final as soon as fc1_wgrad is done); everything else is late
         self._bucket_early = (p_fc1.offset, p_fc1.offset + p_fc1.numel)
         self._g16_shape = (3136, 512)
-        self._epoch_ptr = ctypes.c_void_p(backend.ctrl.local_ptr + backend._off["epoch"])
+        self._epoch_ptr = backend.ctrl.local_ptr + backend._off["epoch"]
 
     # ---- kernels of the step, one launch each (the graph builder and time_kernels share them) ---------------------------
     # ``sp``: the stream to launch on (stream_ptr() of the caller's current stream, taken once per stream)
     def _conv1_fwd(self, images: torch.Tensor, B: int, train: bool, sp) -> None:
         p = self.p
-        check(self.lib.dm_conv1_fwd_tc(ptr(images), ptr(p["conv1_weights"]), ptr(p["conv1_biases"]), ptr(self.a1),
-                                       ptr(self.code1), B, *self._zero_args(train), sp), "conv1_fwd")
+        self.lib.dm_conv1_fwd_tc(images, p["conv1_weights"], p["conv1_biases"], self.a1, self.code1, B,
+                                 *self._zero_args(train), sp)
 
     def _conv2_fwd(self, B: int, sp) -> None:
-        check(self.lib.dm_conv2_fwd(ptr(self.a1), ptr(self.pb["conv2_weights"]), ptr(self.p["conv2_biases"]), ptr(self.a2),
-                                    ptr(self.code2), B, sp), "conv2_fwd")
+        self.lib.dm_conv2_fwd(self.a1, self.pb["conv2_weights"], self.p["conv2_biases"], self.a2, self.code2, B, sp)
 
     def _fc1_fwd(self, B: int) -> None:
         # a2[B,3136] (K-major) * W1[3136,512] (MN-major), split-K: 7 partial tiles stored side by side
@@ -705,12 +692,9 @@ class CudaLeNetEngine(_CudaEngine):
 
     def _fc2_fwd_bwd(self, labels: torch.Tensor, B: int, train: bool, sp, logits_out: Optional[torch.Tensor] = None) -> None:
         p = self.p
-        check(self.lib.dm_fc2_fwd_bwd(ptr(self.h_part), ctypes.c_longlong(self.h_part.stride(0)), self.fc1_splits,
-                                      ptr(p["fc1_biases"]), ptr(p["fc2_weights"]), ptr(p["fc2_biases"]), ptr(labels),
-                                      ptr(self.dh), ptr(self.h_act), ptr(self.dlogits), ptr(self.d_loss_acc), ptr(logits_out),
-                                      B, int(train), ctypes.c_uint(self._seed_mix0),
-                                      self._epoch_ptr if train else ctypes.c_void_p(0), ctypes.c_float(self.keep_prob),
-                                      sp), "fc2_fwd_bwd")
+        self.lib.dm_fc2_fwd_bwd(self.h_part, self.h_part.stride(0), self.fc1_splits, p["fc1_biases"], p["fc2_weights"],
+                                p["fc2_biases"], labels, self.dh, self.h_act, self.dlogits, self.d_loss_acc, logits_out, B,
+                                int(train), self._seed_mix0, self._epoch_ptr if train else None, self.keep_prob, sp)
 
     def _fc1_wgrad(self, dst: torch.Tensor, B: int) -> None:
         # dW1[3136,512] = a2^T (A MN-major) * dh (B MN-major), K = batch: fp32 into the gradient arena, or bf16 (half the
@@ -720,25 +704,22 @@ class CudaLeNetEngine(_CudaEngine):
 
     def _fc2_wgrad(self, B: int, sp) -> None:
         g = self.g
-        check(self.lib.dm_fc2_wgrad(ptr(self.h_act), ptr(self.dlogits), ptr(self.dh), ptr(g["fc2_weights"]),
-                                    ptr(g["fc2_biases"]), ptr(g["fc1_biases"]), B, sp), "fc2_wgrad")
+        self.lib.dm_fc2_wgrad(self.h_act, self.dlogits, self.dh, g["fc2_weights"], g["fc2_biases"], g["fc1_biases"], B, sp)
 
     def _fc1_dgrad(self, B: int, sp) -> None:
         # d(pool2 out)[B,3136] = dh[B,512] (K-major) * W1[3136,512] (rows = in, K = out contiguous), with maxpool2/ReLU2
         # backward and the conv2 bias gradient in the GEMM epilogue (no [B,3136] intermediate)
-        check(self.lib.dm_fc1_dgrad_unpool(ptr(self.dh), ptr(self.pb["fc1_weights"]), ptr(self.code2), ptr(self.dy2),
-                                           ptr(self.g["conv2_biases"]), B, sp), "fc1_dgrad_unpool")
+        self.lib.dm_fc1_dgrad_unpool(self.dh, self.pb["fc1_weights"], self.code2, self.dy2, self.g["conv2_biases"], B, sp)
 
     def _conv2_wgrad(self, B: int, sp) -> None:
-        check(self.lib.dm_conv2_wgrad(ptr(self.a1), ptr(self.dy2), ptr(self.g["conv2_weights"]), B, sp), "conv2_wgrad")
+        self.lib.dm_conv2_wgrad(self.a1, self.dy2, self.g["conv2_weights"], B, sp)
 
     def _conv2_dgrad(self, B: int, sp) -> None:
-        check(self.lib.dm_conv2_dgrad(ptr(self.dy2), ptr(self.pb["conv2_weights"]), ptr(self.dx1), B, sp), "conv2_dgrad")
+        self.lib.dm_conv2_dgrad(self.dy2, self.pb["conv2_weights"], self.dx1, B, sp)
 
     def _conv1_wgrad(self, images: torch.Tensor, B: int, sp) -> None:
         g = self.g
-        check(self.lib.dm_conv1_wgrad_tc(ptr(images), ptr(self.dx1), ptr(self.code1), ptr(g["conv1_weights"]),
-                                         ptr(g["conv1_biases"]), B, sp), "conv1_wgrad")
+        self.lib.dm_conv1_wgrad_tc(images, self.dx1, self.code1, g["conv1_weights"], g["conv1_biases"], B, sp)
 
     # ---- kernel sequence ------------------------------------------------------------------------------
     def _launch_forward(self, images: torch.Tensor, labels: torch.Tensor, B: int, train: bool,
@@ -831,11 +812,10 @@ class CudaLeNetEngine(_CudaEngine):
     def _zero_args(self, train: bool):
         """Regions conv1_fwd clears at the start of a training step (atomically accumulated gradients + loss)."""
         if not train:
-            return (ctypes.c_void_p(0), 0, ctypes.c_void_p(0), 0, ptr(self.d_loss_acc), 2)
+            return (None, 0, None, 0, self.d_loss_acc, 2)
         base = self.grads.data_ptr()
         (a0, b0), (a1, b1) = self._zero_ranges
-        return (ctypes.c_void_p(base + 4 * a0), b0 - a0, ctypes.c_void_p(base + 4 * a1), b1 - a1,
-                ptr(self.d_loss_acc), 2)
+        return (base + 4 * a0, b0 - a0, base + 4 * a1, b1 - a1, self.d_loss_acc, 2)
 
     def _launch_zero(self) -> int:
         return 0    # folded into conv1_fwd
@@ -1055,55 +1035,48 @@ class CudaLeNetEngine(_CudaEngine):
         """One pass over the validation set with the weight views ``p`` (fp32) / ``pb`` (bf16): by default the armed ones --
         the live arena, or the snapshot, which the pass then takes first."""
         lib, sp = self.lib, stream_ptr()
-        null = ctypes.c_void_p(0)
         if p is None:
             if self._snapshot:
                 self._launch_snapshot(self.SNAP_ATTEMPTS)
             elif self._ev_average:
                 # the bf16 operands of the average (no weights: the kernel only converts)
-                check(lib.dm_moving_average(ptr(self._ema), null, ctypes.c_longlong(self.spec.arena_numel), null,
-                                            ctypes.c_double(0.0), null, ptr(self._ev_ema16),
-                                            *[ctypes.c_longlong(v) for v in self._ev_ema_ranges], sp), "moving_average_bf16")
+                lib.dm_moving_average(self._ema, None, self.spec.arena_numel, None, 0.0, None, self._ev_ema16,
+                                      *self._ev_ema_ranges, sp)
             p, pb = self._ev_views
         n, C = self._ev_x.shape[0], self._ev_a1.shape[0]
         stride = self._ev_hpart.stride(0)
-        ring = ptr(self._ev_ring) if publish else null
+        ring = self._ev_ring if publish else None
         armed = p is self._ev_views[0]
         if self._snapshot and armed:
             st = self._snap_state.data_ptr()
-            step_ptr, status_ptr = ctypes.c_void_p(st), ctypes.c_void_p(st + 4)     # SnapState.step, SnapState.status
+            step_ptr, status_ptr = st, st + 4                                        # SnapState.step, SnapState.status
             scored = self._snap
         elif self._ev_average and armed:
-            step_ptr, status_ptr = ptr(self._ema_step), null                         # step of the averaged weights
+            step_ptr, status_ptr = self._ema_step, None                              # step of the averaged weights
             scored = self._ema
         else:
-            step_ptr, status_ptr = self._epoch_ptr, null
+            step_ptr, status_ptr = self._epoch_ptr, None
             scored = self.params if armed else None                                  # fp32 arena the pass scores
-        check(lib.dm_eval_stamp(ptr(self._ev_state), sp), "eval_stamp")
+        lib.dm_eval_stamp(self._ev_state, sp)
         for s in range(0, n, C):
             m = min(C, n - s)
-            check(lib.dm_conv1_fwd_tc(ptr(self._ev_x[s:s + m]), ptr(p["conv1_weights"]), ptr(p["conv1_biases"]),
-                                      ptr(self._ev_a1), ptr(self._ev_code1), m, null, 0, null, 0, null, 0, sp), "conv1_fwd")
-            check(lib.dm_conv2_fwd(ptr(self._ev_a1), ptr(pb["conv2_weights"]), ptr(p["conv2_biases"]), ptr(self._ev_a2),
-                                   ptr(self._ev_code2), m, sp), "conv2_fwd")
+            lib.dm_conv1_fwd_tc(self._ev_x[s:s + m], p["conv1_weights"], p["conv1_biases"], self._ev_a1, self._ev_code1, m,
+                                None, 0, None, 0, None, 0, sp)
+            lib.dm_conv2_fwd(self._ev_a1, pb["conv2_weights"], p["conv2_biases"], self._ev_a2, self._ev_code2, m, sp)
             G.gemm_bf16_raw(self._ev_a2, pb["fc1_weights"], self._ev_hpart, m, 512, 3136, 3136, 512, 512, False, True,
                             G.EPI_STORE_F32, splits=self.fc1_splits, bn=64, split_stride=stride)
-            lg = null if logits_out is None else ptr(logits_out[s:s + m])
-            check(lib.dm_eval_head(ptr(self._ev_hpart), ctypes.c_longlong(stride), self.fc1_splits, ptr(p["fc1_biases"]),
-                                   ptr(p["fc2_weights"]), ptr(p["fc2_biases"]), ptr(self._ev_y[s:s + m]), ptr(self._ev_ws),
-                                   ptr(self._ev_state), step_ptr, status_ptr, ring, self.EVAL_RING, lg, m,
-                                   int(s + m == n), sp), "eval_head")
+            lg = None if logits_out is None else logits_out[s:s + m]
+            lib.dm_eval_head(self._ev_hpart, stride, self.fc1_splits, p["fc1_biases"], p["fc2_weights"], p["fc2_biases"],
+                             self._ev_y[s:s + m], self._ev_ws, self._ev_state, step_ptr, status_ptr, ring, self.EVAL_RING,
+                             lg, m, int(s + m == n), sp)
         if publish and self._best is not None and scored is not None:
             state, decision, arena = self._best
-            check(lib.dm_eval_best_decide(ptr(self._ev_state), step_ptr, status_ptr, ctypes.c_uint(n), ptr(state),
-                                          ptr(decision), sp), "eval_best_decide")
-            check(lib.dm_eval_best_copy(ptr(decision), ptr(scored), ptr(arena), ctypes.c_longlong(arena.numel()), sp),
-                  "eval_best_copy")
+            lib.dm_eval_best_decide(self._ev_state, step_ptr, status_ptr, n, state, decision, sp)
+            lib.dm_eval_best_copy(decision, scored, arena, arena.numel(), sp)
         if publish and self._target is not None:
             need, margin = self._target
-            check(lib.dm_eval_target(ptr(self._ev_state), step_ptr, status_ptr, ctypes.c_uint(need), ctypes.c_uint(n),
-                                     ctypes.c_uint(margin), self._stop.ptr_table(), self.backend.ctx.rank,
-                                     self.backend.ctx.world_size, sp), "eval_target")
+            lib.dm_eval_target(self._ev_state, step_ptr, status_ptr, need, n, margin, self._stop.ptr_table(),
+                               self.backend.ctx.rank, self.backend.ctx.world_size, sp)
 
     def enqueue_eval(self) -> None:
         """Score the validation set with the current weights, on the current (training) stream, without a host
@@ -1223,8 +1196,7 @@ class CudaLeNetEngine(_CudaEngine):
         self._capture_eval()
 
     def _launch_stop_publish(self) -> None:
-        check(self.lib.dm_stop_publish(ctypes.c_void_p(self._stop.local_ptr), ptr(self._stop_host), stream_ptr()),
-              "stop_publish")
+        self.lib.dm_stop_publish(self._stop.local_ptr, self._stop_host, stream_ptr())
 
     def stop_step(self) -> int:
         """Stop step S of this replica's stop word, 0 while none is set, as its newest completed step saw it (a host read:
@@ -1233,7 +1205,7 @@ class CudaLeNetEngine(_CudaEngine):
 
     def enqueue_start_stamp(self) -> None:
         """``%globaltimer`` into a device word, on the current stream: enqueue it right before the run's first step."""
-        check(self.lib.dm_tta_stamp(ptr(self._tta_t0), stream_ptr()), "tta_stamp")
+        self.lib.dm_tta_stamp(self._tta_t0, stream_ptr())
 
     def start_stamp_ns(self) -> int:
         """The stamp of :meth:`enqueue_start_stamp` (a device read, ordered after the current stream's work)."""
@@ -1324,7 +1296,7 @@ class CudaMlpEngine(_CudaEngine):
                  logits_out: Optional[torch.Tensor] = None) -> int:
         lib, sp, p, pb, H = self.lib, stream_ptr(), self.p, self.pb, self.hidden
         n = 0
-        check(lib.dm_f32_to_bf16(ptr(images), ptr(self.x16), ctypes.c_longlong(B * 784), sp), "f32_to_bf16")
+        lib.dm_f32_to_bf16(images, self.x16, B * 784, sp)
         src, K = self.x16, 784
         for i in range(1, self.n_layers):
             # h_i = relu(src @ W_i + b_i): A K-major, B = W_i [in,out] MN-major, bias+ReLU in the epilogue
@@ -1333,9 +1305,8 @@ class CudaMlpEngine(_CudaEngine):
             src, K = self.h[i - 1], H
             n += 1
         L = self.n_layers
-        check(lib.dm_dense10_xent(ptr(src), ptr(p["fc%d_weights" % L]), ptr(p["fc%d_biases" % L]), ptr(labels),
-                                  ptr(self.dh[-1]), ptr(self.dl_pad), ptr(self.g["fc%d_biases" % L]),
-                                  ptr(self.d_loss_acc), ptr(logits_out), B, H, int(train), sp), "dense10_xent")
+        lib.dm_dense10_xent(src, p["fc%d_weights" % L], p["fc%d_biases" % L], labels, self.dh[-1], self.dl_pad,
+                            self.g["fc%d_biases" % L], self.d_loss_acc, logits_out, B, H, int(train), sp)
         return n + 2
 
     def _backward(self, B: int, early_sync: bool = False) -> int:
@@ -1350,8 +1321,7 @@ class CudaMlpEngine(_CudaEngine):
         # output layer: dW_L[H,10] = h_last^T (MN-major) * dl (MN-major, 64-wide zero-padded rows, N = 10)
         G.gemm_bf16_raw(self.h[-1], self.dl_pad, g["fc%d_weights" % L], H, 10, B, H, 64, 10, True, True,
                         G.EPI_STORE_F32, bn=64)
-        check(lib.dm_relu_bwd_colsum(ptr(self.dh[-1]), ctypes.c_void_p(0), ctypes.c_void_p(0),
-                                     ptr(g["fc%d_biases" % (L - 1)]), B, H, sp), "colsum")
+        lib.dm_relu_bwd_colsum(self.dh[-1], None, None, g["fc%d_biases" % (L - 1)], B, H, sp)
         n += 2
         for i in range(L - 1, 0, -1):
             src, K = (self.h[i - 2], H) if i > 1 else (self.x16, 784)
@@ -1389,8 +1359,7 @@ class CudaMlpEngine(_CudaEngine):
                     n += 1
                     self._join_early = torch.cuda.Event()
                     self._join_early.record(side)
-                check(lib.dm_relu_bwd_colsum(ptr(self.dh[i - 2]), ptr(self.h[i - 2]), ptr(self.dh[i - 2]),
-                                             ptr(g["fc%d_biases" % (i - 1)]), B, H, sp), "relu_bwd_colsum")
+                lib.dm_relu_bwd_colsum(self.dh[i - 2], self.h[i - 2], self.dh[i - 2], g["fc%d_biases" % (i - 1)], B, H, sp)
                 n += 2
         if self._join_early is not None:
             main.wait_event(self._join_early)
@@ -1399,8 +1368,8 @@ class CudaMlpEngine(_CudaEngine):
     def _launch_zero(self) -> int:
         sp, base = stream_ptr(), self.grads.data_ptr()
         for (a, b) in self._zero_ranges:
-            check(self.lib.dm_memset_async(ctypes.c_void_p(base + 4 * a), 0, ctypes.c_ulonglong(4 * (b - a)), sp), "memset")
-        check(self.lib.dm_memset_async(ptr(self.d_loss_acc), 0, ctypes.c_ulonglong(8), sp), "memset")
+            self.lib.dm_memset_async(base + 4 * a, 0, 4 * (b - a), sp)
+        self.lib.dm_memset_async(self.d_loss_acc, 0, 8, sp)
         return 0
 
     def _launch_step(self, slot: int, with_sync: bool) -> None:

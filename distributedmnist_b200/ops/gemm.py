@@ -6,12 +6,11 @@ stored ``[K, M]``; likewise ``b`` is ``[N, K]`` (``"k"``) or ``[K, N]`` (``"mn"`
 """
 from __future__ import annotations
 
-import ctypes
 from typing import Optional
 
 import torch
 
-from .lib import check, load, ptr, stream_ptr
+from .lib import load, stream_ptr
 
 EPI_STORE_F32, EPI_ATOMIC_F32, EPI_STORE_BF16, EPI_BIAS_RELU_BF16 = 0, 1, 2, 3
 
@@ -20,9 +19,8 @@ def gemm_bf16_raw(a: torch.Tensor, b: torch.Tensor, out: torch.Tensor, M: int, N
                   ldo: int, a_mn: bool, b_mn: bool, epi: int, splits: int = 1, bn: int = 128,
                   split_stride: int = 0, bias: Optional[torch.Tensor] = None,
                   stream: Optional[torch.cuda.Stream] = None) -> None:
-    rc = load().dm_gemm_bf16(ptr(a), ptr(b), ptr(out), M, N, K, lda, ldb, ldo, int(a_mn), int(b_mn), epi, splits, bn,
-                             ctypes.c_longlong(split_stride), ptr(bias), stream_ptr(stream))
-    check(rc, "dm_gemm_bf16")
+    load().dm_gemm_bf16(a, b, out, M, N, K, lda, ldb, ldo, int(a_mn), int(b_mn), epi, splits, bn, split_stride, bias,
+                        stream_ptr(stream))
 
 
 def gemm_bf16(a: torch.Tensor, b: torch.Tensor, a_major: str = "k", b_major: str = "mn",

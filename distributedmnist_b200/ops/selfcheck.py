@@ -9,7 +9,6 @@ launch with a different CTA count.
 """
 from __future__ import annotations
 
-import ctypes
 from typing import Dict, List, Optional, Sequence, Tuple
 
 import numpy as np
@@ -21,7 +20,7 @@ from ..parallel.context import ReplicaContext
 from ..parallel.fused import FusedBackend
 from . import gemm as G
 from . import refs as R
-from .lib import check, load, ptr, stream_ptr
+from .lib import load, stream_ptr
 
 Result = Tuple[str, float, float]
 KINDS = ("grid", "rand")
@@ -49,8 +48,7 @@ def run_conv1_fwd(x, w, b):
     out = torch.zeros(B, 14, 14, 32, dtype=BF, device="cuda")
     code = torch.zeros(B, 14, 14, 32, dtype=torch.uint8, device="cuda")
     junk = torch.ones(100, device="cuda")
-    check(load().dm_conv1_fwd_tc(ptr(x), ptr(w), ptr(b), ptr(out), ptr(code), B, ptr(junk), 100, ctypes.c_void_p(0), 0,
-                                 ctypes.c_void_p(0), 0, stream_ptr()), "conv1_fwd")
+    load().dm_conv1_fwd_tc(x, w, b, out, code, B, junk, 100, None, 0, None, 0, stream_ptr())
     return out, code, junk
 
 
@@ -60,7 +58,7 @@ def run_conv1_wgrad(x, dpool, code, tc: bool = True):
         raise ValueError("the SIMT conv1 weight-gradient kernel was removed: only tc=True exists")
     B = x.shape[0]
     gw, gb = torch.zeros(25, 32, device="cuda"), torch.zeros(32, device="cuda")
-    check(load().dm_conv1_wgrad_tc(ptr(x), ptr(dpool), ptr(code), ptr(gw), ptr(gb), B, stream_ptr()), "conv1_wgrad")
+    load().dm_conv1_wgrad_tc(x, dpool, code, gw, gb, B, stream_ptr())
     return gw, gb
 
 
@@ -68,19 +66,19 @@ def run_conv2_fwd(a1, w, b):
     B = a1.shape[0]
     out = torch.zeros(B, 7, 7, 64, dtype=BF, device="cuda")
     code = torch.zeros(B, 7, 7, 64, dtype=torch.uint8, device="cuda")
-    check(load().dm_conv2_fwd(ptr(a1), ptr(w), ptr(b), ptr(out), ptr(code), B, stream_ptr()), "conv2_fwd")
+    load().dm_conv2_fwd(a1, w, b, out, code, B, stream_ptr())
     return out, code
 
 
 def run_conv2_dgrad(dy, w):
     dx = torch.zeros(dy.shape[0], 14, 14, 32, dtype=BF, device="cuda")
-    check(load().dm_conv2_dgrad(ptr(dy), ptr(w), ptr(dx), dy.shape[0], stream_ptr()), "conv2_dgrad")
+    load().dm_conv2_dgrad(dy, w, dx, dy.shape[0], stream_ptr())
     return dx
 
 
 def run_conv2_wgrad(a1, dy):
     gw = torch.zeros(5, 5, 32, 64, device="cuda")
-    check(load().dm_conv2_wgrad(ptr(a1), ptr(dy), ptr(gw), a1.shape[0], stream_ptr()), "conv2_wgrad")
+    load().dm_conv2_wgrad(a1, dy, gw, a1.shape[0], stream_ptr())
     return gw
 
 
@@ -101,17 +99,15 @@ def run_fc2_fwd_bwd(parts, b1, w2, b2, labels, train: bool = True, mix0: int = 0
     o = dict(dh=torch.zeros(B, 512, dtype=BF, device="cuda"), h=torch.zeros(B, 512, device="cuda"),
              dl=torch.zeros(B, 12, device="cuda"), la=torch.zeros(2, device="cuda"), logits=torch.zeros(B, 10, device="cuda"))
     st = torch.tensor([step], dtype=torch.int32, device="cuda")
-    check(lib.dm_fc2_fwd_bwd(ptr(parts), ctypes.c_longlong(parts.stride(0)), parts.shape[0], ptr(b1), ptr(w2), ptr(b2),
-                             ptr(labels), ptr(o["dh"]), ptr(o["h"]), ptr(o["dl"]), ptr(o["la"]), ptr(o["logits"]), B,
-                             int(train), ctypes.c_uint(mix0), ptr(st), ctypes.c_float(keep_prob), stream_ptr()),
-          "fc2_fwd_bwd")
+    lib.dm_fc2_fwd_bwd(parts, parts.stride(0), parts.shape[0], b1, w2, b2, labels, o["dh"], o["h"], o["dl"], o["la"],
+                       o["logits"], B, int(train), mix0, st, keep_prob, stream_ptr())
     return o
 
 
 def run_fc2_wgrad(h, dl, dh):
     gw2, gb2, gb1 = torch.full((512, 10), 7.0, device="cuda"), torch.full((10,), 7.0, device="cuda"), \
         torch.full((512,), 7.0, device="cuda")                          # plain stores: stale contents must not matter
-    check(load().dm_fc2_wgrad(ptr(h), ptr(dl), ptr(dh), ptr(gw2), ptr(gb2), ptr(gb1), h.shape[0], stream_ptr()), "fc2_wgrad")
+    load().dm_fc2_wgrad(h, dl, dh, gw2, gb2, gb1, h.shape[0], stream_ptr())
     return gw2, gb2, gb1
 
 
@@ -128,7 +124,7 @@ def run_fc1_dgrad_unpool(dh, w1, code2):
     B = dh.shape[0]
     dy = torch.full((B, 14, 14, 64), 7.0, dtype=BF, device="cuda")      # every element must be overwritten
     gb = torch.zeros(64, device="cuda")
-    check(load().dm_fc1_dgrad_unpool(ptr(dh), ptr(w1), ptr(code2), ptr(dy), ptr(gb), B, stream_ptr()), "fc1_dgrad_unpool")
+    load().dm_fc1_dgrad_unpool(dh, w1, code2, dy, gb, B, stream_ptr())
     return dy, gb
 
 
@@ -842,8 +838,8 @@ def run_dense10_xent(h, w, b, labels, train: bool, g_b0, la0, logits: bool = Tru
     dev = h.device
     o = dict(dh=torch.full((B, H), SENTINEL, dtype=BF, device=dev), dl_pad=torch.full((B, XN_PAD), SENTINEL, dtype=BF, device=dev),
              g_b=g_b0.clone(), la=la0.clone(), logits=torch.full((B, 10), SENTINEL, device=dev) if logits else None)
-    check(load().dm_dense10_xent(ptr(h), ptr(w), ptr(b), ptr(labels), ptr(o["dh"]), ptr(o["dl_pad"]), ptr(o["g_b"]),
-                                 ptr(o["la"]), ptr(o["logits"]), B, H, int(train), stream_ptr()), "dense10_xent")
+    load().dm_dense10_xent(h, w, b, labels, o["dh"], o["dl_pad"], o["g_b"], o["la"], o["logits"], B, H, int(train),
+                           stream_ptr())
     return o
 
 
@@ -859,7 +855,7 @@ def run_relu_bwd_colsum(dh, h, mode: str, g0) -> Tuple[Optional[torch.Tensor], t
     else:
         d, hp = torch.full_like(dh, SENTINEL), h
     src = d if mode == "inplace" else dh
-    check(load().dm_relu_bwd_colsum(ptr(src), ptr(hp), ptr(d), ptr(g), B, H, stream_ptr()), "relu_bwd_colsum")
+    load().dm_relu_bwd_colsum(src, hp, d, g, B, H, stream_ptr())
     return d, g
 
 
@@ -1017,7 +1013,7 @@ def check_f32_to_bf16(B: int = 3, seed: int = 62) -> List[Result]:
     x = torch.where(bits >= 1 << 31, bits - (1 << 32), bits).to(torch.int32).view(torch.float32)
     xd = x.cuda()
     out = torch.full((n,), SENTINEL, dtype=BF, device="cuda")
-    check(load().dm_f32_to_bf16(ptr(xd), ptr(out), ctypes.c_longlong(n), stream_ptr()), "f32_to_bf16")
+    load().dm_f32_to_bf16(xd, out, n, stream_ptr())
     want = x.to(BF).view(torch.int16)
     return [("f32_to_bf16.n%d.bits_differ" % n, float((out.cpu().view(torch.int16) != want).sum()), 0.0)]
 

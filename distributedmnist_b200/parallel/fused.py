@@ -17,14 +17,13 @@ Two ways to drive it:
 """
 from __future__ import annotations
 
-import ctypes
 import os
 from typing import Dict, List, Optional
 
 import numpy as np
 import torch
 
-from ..ops.lib import check, load, require_hopper, stream_ptr
+from ..ops.lib import load, require_hopper, stream_ptr
 from . import straggler
 from .backends import Backend, StepInfo
 from .context import ReplicaContext
@@ -41,7 +40,7 @@ class FusedBackend(Backend):
         assert ctx.on_gpu, "FusedBackend needs a GPU"
         self.lib = load()
         require_hopper(ctx.device)
-        check(self.lib.dm_set_device(ctx.device.index or 0), "dm_set_device")
+        self.lib.dm_set_device(ctx.device.index or 0)
         # programmatic dependent launch between the kernels of a step (DMNIST_PDL=0 disables)
         self.lib.dm_set_pdl(0 if os.environ.get("DMNIST_PDL", "1") == "0" else 1)
         self.ctas = ctas or int(os.environ.get("DMNIST_SYNC_CTAS", "0")) or int(self.lib.dm_num_sms())
@@ -73,8 +72,7 @@ class FusedBackend(Backend):
         self.late_bf16 = os.environ.get("DMNIST_LATE_BF16", "1") != "0"  # ... carrying bf16 gradients (half the bytes)
         # host mirror of the status words: the kernel that closes a step stores them into page-locked host memory itself
         self._mirror = torch.zeros(4 * 8, dtype=torch.int32).pin_memory()
-        check(self.lib.dm_sync_set_host_mirror(ctypes.c_void_p(self.ctrl.local_ptr), ctypes.c_void_p(self._mirror.data_ptr())),
-              "dm_sync_set_host_mirror")
+        self.lib.dm_sync_set_host_mirror(self.ctrl.local_ptr, self._mirror)
         self._mirror_np = self._mirror.numpy().view("<u4")
         self.shadow: Optional[torch.Tensor] = None     # bf16 copy of the parameter arena
         self.drop_keep = 0.0
@@ -103,8 +101,7 @@ class FusedBackend(Backend):
 
     def refresh_shadow(self, params: torch.Tensor) -> None:
         if self.shadow is not None:
-            check(self.lib.dm_f32_to_bf16(ctypes.c_void_p(params.data_ptr()), ctypes.c_void_p(self.shadow.data_ptr()),
-                                          ctypes.c_longlong(params.numel()), stream_ptr()), "dm_f32_to_bf16")
+            self.lib.dm_f32_to_bf16(params, self.shadow, params.numel(), stream_ptr())
 
     # ---- control-block access ---------------------------------------------------------------
     def _read_u32(self, field: str, index: int = 0) -> int:
@@ -216,17 +213,14 @@ class FusedBackend(Backend):
     def enqueue(self, params: torch.Tensor, grads: torch.Tensor, k: int, lr0: float, decay_rate: float = 1.0,
                 decay_steps: int = 1, stream: Optional[torch.cuda.Stream] = None) -> None:
         pb, gb = self._by_ptr[params.data_ptr()], self._by_ptr[grads.data_ptr()]
-        rc = self.lib.dm_fused_sync_sgd(
-            self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), self.ctx.rank, self.ctx.world_size, int(k),
-            ctypes.c_longlong(params.numel()), ctypes.c_double(lr0), ctypes.c_double(decay_rate), int(decay_steps),
-            ctypes.c_float(self.drop_keep), ctypes.c_uint(self.drop_seed), ctypes.c_double(self.timeout_ms),
-            ctypes.c_void_p(0 if self.shadow is None else self.shadow.data_ptr()), int(self.ctas), stream_ptr(stream),
-            *self._mc_ptrs(pb, gb))
-        check(rc, "dm_fused_sync_sgd")
+        self.lib.dm_fused_sync_sgd(
+            self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), self.ctx.rank, self.ctx.world_size, int(k), params.numel(),
+            lr0, decay_rate, int(decay_steps), self.drop_keep, self.drop_seed, self.timeout_ms, self.shadow, int(self.ctas),
+            stream_ptr(stream), *self._mc_ptrs(pb, gb))
 
     def _mc_ptrs(self, pb, gb):
         on = self.use_nvls and pb.multicast_ptr and gb.multicast_ptr
-        return ctypes.c_void_p(gb.multicast_ptr if on else 0), ctypes.c_void_p(pb.multicast_ptr if on else 0)
+        return gb.multicast_ptr if on else 0, pb.multicast_ptr if on else 0
 
     def enqueue_bucket(self, params: torch.Tensor, grads: torch.Tensor, phase: int, begin: int, end: int,
                        early_begin: int, early_end: int, lr0: float, decay_rate: float = 1.0, decay_steps: int = 1,
@@ -234,13 +228,10 @@ class FusedBackend(Backend):
         """Bucketed aggregation (K == N, world_size > 1): ``phase`` 1 = early bucket ``[begin, end)`` (floats) on a few
         CTAs next to the remaining backward kernels, 2 = late bucket + completion of the step (csrc/fused_sync.cu)."""
         pb, gb = self._by_ptr[params.data_ptr()], self._by_ptr[grads.data_ptr()]
-        rc = self.lib.dm_fused_sync_bucket(
-            self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), self.ctx.rank, self.ctx.world_size, int(phase),
-            ctypes.c_longlong(begin), ctypes.c_longlong(end), ctypes.c_longlong(early_begin), ctypes.c_longlong(early_end),
-            ctypes.c_double(lr0), ctypes.c_double(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
-            ctypes.c_void_p(0 if self.shadow is None else self.shadow.data_ptr()), int(ctas), stream_ptr(stream),
-            *self._mc_ptrs(pb, gb))
-        check(rc, "dm_fused_sync_bucket")
+        self.lib.dm_fused_sync_bucket(
+            self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), self.ctx.rank, self.ctx.world_size, int(phase), begin, end,
+            early_begin, early_end, lr0, decay_rate, int(decay_steps), self.timeout_ms, self.shadow, int(ctas),
+            stream_ptr(stream), *self._mc_ptrs(pb, gb))
 
     def enqueue_bucket_v2(self, params: torch.Tensor, grads: torch.Tensor, g16, inbox, phase: int, fc1_begin: int,
                           fc1_end: int, lr0: float, decay_rate: float = 1.0, decay_steps: int = 1, ctas: int = 0,
@@ -252,29 +243,23 @@ class FusedBackend(Backend):
         on = self.use_nvls and self.ctx.world_size > 1
         mc_g16 = g16.multicast_ptr if on else 0
         mc_inbox = inbox.multicast_ptr if (on and inbox is not None) else 0
-        rc = self.lib.dm_bucket_sync(
+        self.lib.dm_bucket_sync(
             self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), g16.ptr_table(),
-            inbox.ptr_table() if inbox is not None else None, self.ctx.rank, self.ctx.world_size, int(phase),
-            ctypes.c_longlong(fc1_begin), ctypes.c_longlong(fc1_end), ctypes.c_longlong(params.numel()),
-            ctypes.c_double(lr0), ctypes.c_double(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
-            ctypes.c_void_p(0 if self.shadow is None else self.shadow.data_ptr()), int(ctas), stream_ptr(stream),
-            ctypes.c_void_p(mc_g16), ctypes.c_void_p(mc_inbox), int(self.late_ll), int(self.late_bf16))
-        check(rc, "dm_bucket_sync(phase %d)" % phase)
+            inbox.ptr_table() if inbox is not None else None, self.ctx.rank, self.ctx.world_size, int(phase), fc1_begin,
+            fc1_end, params.numel(), lr0, decay_rate, int(decay_steps), self.timeout_ms, self.shadow, int(ctas),
+            stream_ptr(stream), mc_g16, mc_inbox, int(self.late_ll), int(self.late_bf16))
 
     # ---- device-side interval mode (mode C, csrc/fused_interval.cu) ----------------------------------------------------------
     def interval_arm(self, interval_ms: float) -> None:
         """Start the interval clock on this replica (reference ``start_interval_updates``): first tick due in ``interval_ms``."""
         self.barrier()                       # replicas start their clocks together (each uses its own %globaltimer afterwards)
-        check(self.lib.dm_interval_arm(ctypes.c_void_p(self.ctrl.local_ptr), ctypes.c_double(interval_ms), stream_ptr()),
-              "dm_interval_arm")
+        self.lib.dm_interval_arm(self.ctrl.local_ptr, interval_ms, stream_ptr())
         torch.cuda.synchronize()
         self.barrier()
 
     def enqueue_interval_begin(self, params: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> None:
         """Start of an interval-mode iteration: adopt weights a committer has pushed (step counter, bf16 shadow)."""
-        check(self.lib.dm_interval_begin(ctypes.c_void_p(self.ctrl.local_ptr), ctypes.c_void_p(params.data_ptr()),
-                                         ctypes.c_void_p(0 if self.shadow is None else self.shadow.data_ptr()),
-                                         ctypes.c_longlong(params.numel()), stream_ptr(stream)), "dm_interval_begin")
+        self.lib.dm_interval_begin(self.ctrl.local_ptr, params, self.shadow, params.numel(), stream_ptr(stream))
 
     def enqueue_interval_end(self, params: torch.Tensor, grads: torch.Tensor, acc: torch.Tensor, lr0: float,
                              decay_rate: float = 1.0, decay_steps: int = 1,
@@ -283,10 +268,9 @@ class FusedBackend(Backend):
         tick (mean of whatever every replica has accumulated) -- never blocks on another replica's progress."""
         pb, gb, ab = self._by_ptr[params.data_ptr()], self._by_ptr[grads.data_ptr()], self._by_ptr[acc.data_ptr()]
         mc = pb.multicast_ptr if (self.use_nvls and pb.multicast_ptr) else 0
-        check(self.lib.dm_interval_end(self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), ab.ptr_table(), self.ctx.rank,
-                                       self.ctx.world_size, ctypes.c_longlong(params.numel()), ctypes.c_double(lr0),
-                                       ctypes.c_double(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
-                                       int(self.ctas), stream_ptr(stream), ctypes.c_void_p(mc)), "dm_interval_end")
+        self.lib.dm_interval_end(self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), ab.ptr_table(), self.ctx.rank,
+                                 self.ctx.world_size, params.numel(), lr0, decay_rate, int(decay_steps), self.timeout_ms,
+                                 int(self.ctas), stream_ptr(stream), mc)
 
     # ---- K > N gradients per update (count trigger, csrc/fused_interval.cu with COUNT) ---------------------------------------
     def kgtn_arm(self) -> None:
@@ -296,9 +280,7 @@ class FusedBackend(Backend):
     def enqueue_kgtn_begin(self, params: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> None:
         """Start of a K > N iteration: adopt weights a committer has pushed; gradients accumulated for the step after its
         contributors were frozen are counted as dropped."""
-        check(self.lib.dm_kgtn_begin(ctypes.c_void_p(self.ctrl.local_ptr), self.ctx.rank, ctypes.c_void_p(params.data_ptr()),
-                                     ctypes.c_void_p(0 if self.shadow is None else self.shadow.data_ptr()),
-                                     ctypes.c_longlong(params.numel()), stream_ptr(stream)), "dm_kgtn_begin")
+        self.lib.dm_kgtn_begin(self.ctrl.local_ptr, self.ctx.rank, params, self.shadow, params.numel(), stream_ptr(stream))
 
     def enqueue_kgtn_end(self, params: torch.Tensor, grads: torch.Tensor, acc: torch.Tensor, k: int, lr0: float,
                          decay_rate: float = 1.0, decay_steps: int = 1, stream: Optional[torch.cuda.Stream] = None) -> None:
@@ -306,11 +288,9 @@ class FusedBackend(Backend):
         weights are accumulated across the replicas, the first replica to see it commits their mean."""
         pb, gb, ab = self._by_ptr[params.data_ptr()], self._by_ptr[grads.data_ptr()], self._by_ptr[acc.data_ptr()]
         nv = self.use_nvls and bool(pb.multicast_ptr) and bool(ab.multicast_ptr)
-        check(self.lib.dm_kgtn_end(self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), ab.ptr_table(), self.ctx.rank,
-                                   self.ctx.world_size, int(k), ctypes.c_longlong(params.numel()), ctypes.c_double(lr0),
-                                   ctypes.c_double(decay_rate), int(decay_steps), ctypes.c_double(self.timeout_ms),
-                                   int(self.ctas), stream_ptr(stream), ctypes.c_void_p(pb.multicast_ptr if nv else 0),
-                                   ctypes.c_void_p(ab.multicast_ptr if nv else 0)), "dm_kgtn_end")
+        self.lib.dm_kgtn_end(self.ctrl.ptr_table(), pb.ptr_table(), gb.ptr_table(), ab.ptr_table(), self.ctx.rank,
+                             self.ctx.world_size, int(k), params.numel(), lr0, decay_rate, int(decay_steps), self.timeout_ms,
+                             int(self.ctas), stream_ptr(stream), pb.multicast_ptr if nv else 0, ab.multicast_ptr if nv else 0)
 
     @property
     def nvls_active(self) -> bool:
@@ -318,9 +298,7 @@ class FusedBackend(Backend):
 
     def enqueue_straggler_delay(self, prob: float, usec: float, seed: int = 12345,
                                 stream: Optional[torch.cuda.Stream] = None) -> None:
-        check(self.lib.dm_straggler_delay(ctypes.c_void_p(self.ctrl.local_ptr), ctypes.c_float(prob),
-                                          ctypes.c_uint(int(usec)), ctypes.c_uint(seed), stream_ptr(stream)),
-              "dm_straggler_delay")
+        self.lib.dm_straggler_delay(self.ctrl.local_ptr, prob, int(usec), seed, stream_ptr(stream))
 
     def arm_straggler(self, spec) -> None:
         """Sampled forms (``rank:exp|lognormal|profile:...``): upload the quantile table and allocate the sampler's state
@@ -345,9 +323,7 @@ class FusedBackend(Backend):
             return
         if getattr(self, "_strag_spec", None) is not spec:
             raise RuntimeError("enqueue_straggler: arm_straggler(spec) has not been called for this spec")
-        check(self.lib.dm_straggler_sample(ctypes.c_void_p(self._strag_state.data_ptr()),
-                                           ctypes.c_void_p(self._strag_table.data_ptr()), ctypes.c_uint(spec.seed_mix),
-                                           stream_ptr(stream)), "dm_straggler_sample")
+        self.lib.dm_straggler_sample(self._strag_state, self._strag_table, spec.seed_mix, stream_ptr(stream))
 
     def straggler_samples(self):
         """``(j, drawn_ns, spun_ns)`` of the sampled iterations still in the device ring (the last 1024), oldest first;
@@ -364,15 +340,15 @@ class FusedBackend(Backend):
         """Stream-ordered barrier over NVLink flags (csrc/fused_sync.cu): every replica's stream passes it within a flag hop of
         the last replica reaching it -- aligns the replicas far tighter than a host-side barrier can."""
         if self.ctx.world_size > 1:
-            check(self.lib.dm_device_barrier(self.ctrl.ptr_table(), self.ctx.rank, self.ctx.world_size,
-                                             ctypes.c_double(self.timeout_ms), stream_ptr(stream)), "dm_device_barrier")
+            self.lib.dm_device_barrier(self.ctrl.ptr_table(), self.ctx.rank, self.ctx.world_size,
+                                       self.timeout_ms, stream_ptr(stream))
 
     def enqueue_stamp_arrive(self, stream: Optional[torch.cuda.Stream] = None) -> None:
         """cdf telemetry: "my gradient is complete" on the compute chain, before it joins the exchange branch."""
-        check(self.lib.dm_stamp_arrive(ctypes.c_void_p(self.ctrl.local_ptr), stream_ptr(stream)), "dm_stamp_arrive")
+        self.lib.dm_stamp_arrive(self.ctrl.local_ptr, stream_ptr(stream))
 
     def enqueue_stamp_start(self, stream: Optional[torch.cuda.Stream] = None) -> None:
-        check(self.lib.dm_stamp_start(ctypes.c_void_p(self.ctrl.local_ptr), stream_ptr(stream)), "dm_stamp_start")
+        self.lib.dm_stamp_start(self.ctrl.local_ptr, stream_ptr(stream))
 
     def drop_connect_(self, grads: torch.Tensor, keep_prob: float, step: int) -> None:
         # Applied inside the fused kernel's load stage (per contributor); just arm it.

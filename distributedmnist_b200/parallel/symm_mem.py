@@ -27,7 +27,7 @@ from typing import Dict, List, Optional, Tuple
 import torch
 import torch.distributed as dist
 
-from ..ops.lib import check, load
+from ..ops.lib import load
 
 _TYPESTR = {torch.float32: "<f4", torch.uint8: "|u1", torch.int32: "<i4", torch.bfloat16: None, torch.int64: "<i8",
             torch.uint16: "<u2"}
@@ -49,22 +49,21 @@ class SymmetricBuffer:
         self.nbytes = (nbytes + 255) // 256 * 256
         self.rank, self.world_size, self.device = rank, world_size, device
         p = ctypes.c_void_p()
-        check(self.lib.dm_symm_alloc(ctypes.c_ulonglong(self.nbytes), ctypes.byref(p)), "dm_symm_alloc")
+        self.lib.dm_symm_alloc(self.nbytes, ctypes.byref(p))
         self.local_ptr = int(p.value)
         self.peer_ptrs: List[int] = [0] * world_size
         self.peer_ptrs[rank] = self.local_ptr
         self._opened: List[int] = []
         if world_size > 1:
             h = ctypes.create_string_buffer(64)
-            check(self.lib.dm_symm_ipc_handle(ctypes.c_void_p(self.local_ptr), h), "dm_symm_ipc_handle")
+            self.lib.dm_symm_ipc_handle(ctypes.c_void_p(self.local_ptr), h)
             handles: List[Optional[bytes]] = [None] * world_size
             dist.all_gather_object(handles, bytes(h.raw), group=group)
             for r, hb in enumerate(handles):
                 if r == rank:
                     continue
                 q = ctypes.c_void_p()
-                check(self.lib.dm_symm_ipc_open(ctypes.create_string_buffer(hb, 64), ctypes.byref(q)),
-                      "dm_symm_ipc_open(rank %d)" % r)
+                self.lib.dm_symm_ipc_open(ctypes.create_string_buffer(hb, 64), ctypes.byref(q))
                 self.peer_ptrs[r] = int(q.value)
                 self._opened.append(int(q.value))
         self.multicast_ptr = 0
@@ -199,7 +198,6 @@ class VmmBuffer:
     def __init__(self, nbytes: int, rank: int, world_size: int, device: torch.device, want_multicast: bool = True, group=None):
         self.lib = load()
         lib, dev = self.lib, device.index or 0
-        lib.dm_vmm_round_size.restype = ctypes.c_longlong
         self.rank, self.world_size, self.device = rank, world_size, device
         size = int(lib.dm_vmm_round_size(ctypes.c_ulonglong(max(nbytes, 256)), dev, world_size))
         if not _all_ok(size > 0, group):

@@ -2,7 +2,6 @@
 launched step against a second engine, validated snapshots next to an emulated peer (csrc/eval_snapshot.cu's test writer),
 a capture right after a restore, ``train()`` end to end with a checkpoint every step, and no host synchronisation per
 checkpoint."""
-import ctypes
 import os
 import re
 import subprocess
@@ -48,10 +47,8 @@ def _f(g, n):
 
 
 def _emulate(eng, g, mode, phases=7):
-    from distributedmnist_b200.ops.lib import check, stream_ptr
-    check(eng.lib.dm_snap_test_emulate(ctypes.c_void_p(eng.backend.ctrl.local_ptr), ctypes.c_void_p(eng.params.data_ptr()),
-                                       ctypes.c_longlong(eng.params.numel()), ctypes.c_uint(g), mode, 1, phases,
-                                       stream_ptr()), "snap_test_emulate")
+    from distributedmnist_b200.ops.lib import stream_ptr
+    eng.lib.dm_snap_test_emulate(eng.backend.ctrl.local_ptr, eng.params, eng.params.numel(), g, mode, 1, phases, stream_ptr())
 
 
 def test_lenet_live_capture_after_every_step_is_bit_exact():
@@ -107,7 +104,7 @@ def test_mlp2_live_capture_equals_the_arena_after_a_synchronise():
 def test_snapshot_capture_next_to_a_concurrent_paced_writer(mode):
     """One writer CTA on a second stream commits rounds into the arena while captures run on the current stream.  Every
     accepted capture equals f(g, .) of the step its record names, accepted steps never decrease; counts are printed."""
-    from distributedmnist_b200.ops.lib import check, stream_ptr
+    from distributedmnist_b200.ops.lib import stream_ptr
     eng, be = _engine(optimizer=False)
     eng._interval = mode == INTERVAL              # which commit-word layout select reads (attach_optimizer sets it in training)
     eng.arm_checkpoint(snapshot=True)
@@ -119,9 +116,7 @@ def test_snapshot_capture_next_to_a_concurrent_paced_writer(mode):
     report = {}
     for pace_us, rounds in ((0.0, 600), (400.0, 150)):
         flag = torch.zeros(4, dtype=torch.int32).pin_memory()
-        check(eng.lib.dm_snap_test_writer(ctypes.c_void_p(be.ctrl.local_ptr), ctypes.c_void_p(eng.params.data_ptr()),
-                                          ctypes.c_longlong(n), ctypes.c_uint(g), rounds, ctypes.c_double(pace_us), mode,
-                                          ctypes.c_void_p(flag.data_ptr()), stream_ptr(side)), "snap_test_writer")
+        eng.lib.dm_snap_test_writer(be.ctrl.local_ptr, eng.params, n, g, rounds, pace_us, mode, flag, stream_ptr(side))
         t0 = time.time()
         while int(flag[0]) == 0:
             assert time.time() - t0 < 30.0, "writer CTA never started"
@@ -149,7 +144,7 @@ def test_failed_captures_write_no_file_and_are_retried_at_the_next_step(tmp_path
     """A back-to-back writer: most captures fail.  The checkpointer writes no file for them and enqueues the retry at its
     next call; every file it writes holds f(g, .) of its step."""
     from distributedmnist_b200.checkpoint import Saver, get_checkpoint_state
-    from distributedmnist_b200.ops.lib import check, stream_ptr
+    from distributedmnist_b200.ops.lib import stream_ptr
     from distributedmnist_b200.train import _AsyncCheckpointer
     eng, be = _engine(optimizer=False)
     eng._interval = mode == INTERVAL
@@ -171,9 +166,7 @@ def test_failed_captures_write_no_file_and_are_retried_at_the_next_step(tmp_path
     ck.saver.save = lambda d, state, step: saved.append(step) or real_save(d, state, step)
     flag = torch.zeros(4, dtype=torch.int32).pin_memory()
     side = torch.cuda.Stream()
-    check(eng.lib.dm_snap_test_writer(ctypes.c_void_p(be.ctrl.local_ptr), ctypes.c_void_p(eng.params.data_ptr()),
-                                      ctypes.c_longlong(n), ctypes.c_uint(1), 3000, ctypes.c_double(0.0), mode,
-                                      ctypes.c_void_p(flag.data_ptr()), stream_ptr(side)), "snap_test_writer")
+    eng.lib.dm_snap_test_writer(be.ctrl.local_ptr, eng.params, n, 1, 3000, 0.0, mode, flag, stream_ptr(side))
     t0 = time.time()
     while int(flag[0]) == 0:
         assert time.time() - t0 < 30.0, "writer CTA never started"

@@ -1,7 +1,6 @@
 """Snapshot passes on the GPU (``CudaLeNetEngine.arm_eval(snapshot=True)``, csrc/eval_snapshot.cu): an exact copy of quiescent
 weights, deterministic interleavings with an emulated peer on one stream, a concurrent paced writer, and interval mode end to
 end on one replica."""
-import ctypes
 import os
 import re
 import subprocess
@@ -47,23 +46,20 @@ def _f(g, n):
 
 
 def _emulate(eng, g, mode, phases=7):
-    from distributedmnist_b200.ops.lib import check, stream_ptr
-    check(eng.lib.dm_snap_test_emulate(ctypes.c_void_p(eng.backend.ctrl.local_ptr), ctypes.c_void_p(eng.params.data_ptr()),
-                                       ctypes.c_longlong(eng.params.numel()), ctypes.c_uint(g), mode, 1, phases,
-                                       stream_ptr()), "snap_test_emulate")
+    from distributedmnist_b200.ops.lib import stream_ptr
+    eng.lib.dm_snap_test_emulate(eng.backend.ctrl.local_ptr, eng.params, eng.params.numel(), g, mode, 1, phases, stream_ptr())
 
 
 def _attempt(eng, a, part):
     """One part of snapshot attempt `a` of a 4-attempt pass, launched eagerly."""
-    from distributedmnist_b200.ops.lib import check, ptr, stream_ptr
-    lib, ctrl, st = eng.lib, ctypes.c_void_p(eng.backend.ctrl.local_ptr), ptr(eng._snap_state)
+    from distributedmnist_b200.ops.lib import stream_ptr
+    lib, ctrl, st = eng.lib, eng.backend.ctrl.local_ptr, eng._snap_state
     if part == "select":
-        check(lib.dm_snap_select(ctrl, st, a, int(eng._interval), ctypes.c_double(eng.SNAP_WATCHDOG_MS), stream_ptr()), part)
+        lib.dm_snap_select(ctrl, st, a, int(eng._interval), eng.SNAP_WATCHDOG_MS, stream_ptr())
     elif part == "copy":
-        check(lib.dm_snap_copy(st, ptr(eng.params), ptr(eng._snap), ptr(eng._snap16), ctypes.c_longlong(eng.params.numel()),
-                               *[ctypes.c_longlong(v) for v in eng._snap_bf_ranges], stream_ptr()), part)
+        lib.dm_snap_copy(st, eng.params, eng._snap, eng._snap16, eng.params.numel(), *eng._snap_bf_ranges, stream_ptr())
     else:
-        check(lib.dm_snap_validate(ctrl, st, a, eng.SNAP_ATTEMPTS, stream_ptr()), part)
+        lib.dm_snap_validate(ctrl, st, a, eng.SNAP_ATTEMPTS, stream_ptr())
 
 
 def _armed(mode, use_graph=False, n=2500):
@@ -74,7 +70,7 @@ def _armed(mode, use_graph=False, n=2500):
 
 
 def test_quiescent_snapshot_is_exact_and_scores_like_the_live_pass():
-    from distributedmnist_b200.ops.lib import check, ptr, stream_ptr
+    from distributedmnist_b200.ops.lib import stream_ptr
     eng, _ = _engine(use_graph=True)
     x, y = _valset(2500, 6)
     eng.arm_eval(x, y, snapshot=True)
@@ -85,7 +81,7 @@ def test_quiescent_snapshot_is_exact_and_scores_like_the_live_pass():
     snap, step = eng.eval_snapshot()
     assert step == 0 and torch.equal(_bits(snap), _bits(eng.params))
     ref16 = torch.empty_like(eng._snap16)
-    check(eng.lib.dm_f32_to_bf16(ptr(snap), ptr(ref16), ctypes.c_longlong(snap.numel()), stream_ptr()), "f32_to_bf16")
+    eng.lib.dm_f32_to_bf16(snap, ref16, snap.numel(), stream_ptr())
     rg = eng._snap_bf_ranges
     for b, e in zip(rg[0::2], rg[1::2]):
         assert torch.equal(eng._snap16[b:e].view(torch.int16), ref16[b:e].view(torch.int16))
@@ -170,7 +166,7 @@ def test_restore_with_an_empty_ring_scores_the_restored_step(mode):
 def test_concurrent_paced_writer(mode):
     """One writer CTA on a second stream commits rounds into the arena while snapshot passes run on the training stream.
     Every accepted snapshot equals f(g, .) of the step it reports; acceptance and retry counts are printed."""
-    from distributedmnist_b200.ops.lib import check, stream_ptr
+    from distributedmnist_b200.ops.lib import stream_ptr
     eng, be = _armed(mode, use_graph=True)
     n = eng.params.numel()
     _emulate(eng, 1, mode)
@@ -180,9 +176,7 @@ def test_concurrent_paced_writer(mode):
     report, before = {}, {}
     for pace_us, rounds in ((0.0, 600), (400.0, 150)):
         flag = torch.zeros(4, dtype=torch.int32).pin_memory()
-        check(eng.lib.dm_snap_test_writer(ctypes.c_void_p(be.ctrl.local_ptr), ctypes.c_void_p(eng.params.data_ptr()),
-                                          ctypes.c_longlong(n), ctypes.c_uint(g), rounds, ctypes.c_double(pace_us), mode,
-                                          ctypes.c_void_p(flag.data_ptr()), stream_ptr(side)), "snap_test_writer")
+        eng.lib.dm_snap_test_writer(be.ctrl.local_ptr, eng.params, n, g, rounds, pace_us, mode, flag, stream_ptr(side))
         t0 = time.time()
         while int(flag[0]) == 0:                                     # the writer is resident before any snapshot launches
             assert time.time() - t0 < 30.0, "writer CTA never started"

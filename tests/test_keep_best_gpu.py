@@ -3,7 +3,6 @@ against the host emulation and bit for bit on the lenet and mlp2 arena sizes; le
 checkpoint is bit-identical to the step-g checkpoint of a run cut at g and scores the same in the standalone evaluator,
 with unchanged weights, rows and step graph; the moving average; K > N and interval snapshot runs; a dropped snapshot pass
 that never becomes the best; and a run stopped by --target_accuracy."""
-import ctypes
 import json
 import os
 
@@ -84,7 +83,7 @@ def _lib():
 def _decide(correct, examples, loss_sum, step, n, best, status):
     """One eval_best_decide launch: (BestState tuple, decision word) as the device left them."""
     from distributedmnist_b200.best import BEST_CORRECT_WORD, BEST_EXAMPLES_WORD, BEST_STEP_WORD, BEST_VALID_WORD
-    from distributedmnist_b200.ops.lib import check, ptr, stream_ptr
+    from distributedmnist_b200.ops.lib import stream_ptr
     lib = _lib()
     ev = torch.zeros(int(lib.dm_eval_state_bytes()), dtype=torch.uint8)
     ev[0:8].view(torch.float64)[0] = loss_sum
@@ -96,8 +95,7 @@ def _decide(correct, examples, loss_sum, step, n, best, status):
     step_t = torch.tensor([step], dtype=torch.int32, device="cuda")
     st_t = None if status is None else torch.tensor([status], dtype=torch.int32, device="cuda")
     word = torch.full((1,), 7, dtype=torch.int32, device="cuda")
-    check(lib.dm_eval_best_decide(ptr(ev), ptr(step_t), ptr(st_t), ctypes.c_uint(n), ptr(w), ptr(word), stream_ptr()),
-          "eval_best_decide")
+    lib.dm_eval_best_decide(ev, step_t, st_t, n, w, word, stream_ptr())
     torch.cuda.synchronize()
     h = w.cpu()
     return ((int(h[BEST_STEP_WORD]), int(h[BEST_CORRECT_WORD]), int(h[BEST_EXAMPLES_WORD]),
@@ -122,7 +120,7 @@ def test_decide_matches_the_emulation(correct, examples, best_correct, status):
 
 def test_copy_is_bit_exact_and_skipped_on_a_zero_decision():
     from distributedmnist_b200.models import get_model
-    from distributedmnist_b200.ops.lib import check, ptr, stream_ptr
+    from distributedmnist_b200.ops.lib import stream_ptr
     lib = _lib()
     mlp2 = get_model("mlp2", 1024)[0].arena_numel
     sizes = [get_model("lenet")[0].arena_numel, mlp2, mlp2 + 3, 1, 7]    # odd lengths take the scalar tail
@@ -133,8 +131,7 @@ def test_copy_is_bit_exact_and_skipped_on_a_zero_decision():
         dst = torch.full((n,), -3.0, device="cuda")
         for decision in (0, 1):
             word = torch.tensor([decision], dtype=torch.int32, device="cuda")
-            check(lib.dm_eval_best_copy(ptr(word), ptr(src), ptr(dst), ctypes.c_longlong(n), stream_ptr()),
-                  "eval_best_copy")
+            lib.dm_eval_best_copy(word, src, dst, n, stream_ptr())
             torch.cuda.synchronize()
             want = src if decision else torch.full((n,), -3.0, device="cuda")
             assert torch.equal(dst.view(torch.int32), want.view(torch.int32)), (n, decision)
@@ -201,10 +198,8 @@ def test_snapshot_runs_best_file_scores_its_row(tmp_path, flags, capsys, extra):
 
 
 def _emulate(eng, g, mode, phases=7):
-    from distributedmnist_b200.ops.lib import check, stream_ptr
-    check(eng.lib.dm_snap_test_emulate(ctypes.c_void_p(eng.backend.ctrl.local_ptr), ctypes.c_void_p(eng.params.data_ptr()),
-                                       ctypes.c_longlong(eng.params.numel()), ctypes.c_uint(g), mode, 1, phases,
-                                       stream_ptr()), "snap_test_emulate")
+    from distributedmnist_b200.ops.lib import stream_ptr
+    eng.lib.dm_snap_test_emulate(eng.backend.ctrl.local_ptr, eng.params, eng.params.numel(), g, mode, 1, phases, stream_ptr())
 
 
 @pytest.mark.parametrize("mode", [K_OF_N, INTERVAL], ids=["k_of_n", "interval"])
@@ -214,7 +209,7 @@ def test_dropped_snapshot_pass_never_becomes_the_best(mode):
     copies W0 -- pushed as step 2 -- and is rejected because step 3 commits during the copy; the pass scores W0 (the
     highest count there is) with status -1 and must leave the best at step 1."""
     from distributedmnist_b200.engine_cuda import CudaLeNetEngine
-    from distributedmnist_b200.ops.lib import check, ptr, stream_ptr
+    from distributedmnist_b200.ops.lib import stream_ptr
     from distributedmnist_b200.ops.selfcheck import mnist_like
     from distributedmnist_b200.parallel.context import ReplicaContext
     from distributedmnist_b200.parallel.fused import FusedBackend
@@ -240,13 +235,11 @@ def test_dropped_snapshot_pass_never_becomes_the_best(mode):
     _emulate(eng, 2, mode, phases=1)
     eng.params.copy_(w0)
     _emulate(eng, 2, mode, phases=4)
-    lib, ctrl, st = eng.lib, ctypes.c_void_p(be.ctrl.local_ptr), ptr(eng._snap_state)
-    check(lib.dm_snap_select(ctrl, st, 0, int(eng._interval), ctypes.c_double(eng.SNAP_WATCHDOG_MS), stream_ptr()),
-          "snap_select")
-    check(lib.dm_snap_copy(st, ptr(eng.params), ptr(eng._snap), ptr(eng._snap16), ctypes.c_longlong(eng.params.numel()),
-                           *[ctypes.c_longlong(v) for v in eng._snap_bf_ranges], stream_ptr()), "snap_copy")
+    lib, ctrl, st = eng.lib, be.ctrl.local_ptr, eng._snap_state
+    lib.dm_snap_select(ctrl, st, 0, int(eng._interval), eng.SNAP_WATCHDOG_MS, stream_ptr())
+    lib.dm_snap_copy(st, eng.params, eng._snap, eng._snap16, eng.params.numel(), *eng._snap_bf_ranges, stream_ptr())
     _emulate(eng, 3, mode, phases=1)
-    check(lib.dm_snap_validate(ctrl, st, eng.SNAP_ATTEMPTS - 1, eng.SNAP_ATTEMPTS, stream_ptr()), "snap_validate")
+    lib.dm_snap_validate(ctrl, st, eng.SNAP_ATTEMPTS - 1, eng.SNAP_ATTEMPTS, stream_ptr())
     p, pb = eng._ev_views
     eng._launch_eval(publish=True, p=p, pb=pb)                   # the pass's chunks, then decide and copy
     torch.cuda.synchronize()

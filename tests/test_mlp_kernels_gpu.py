@@ -41,12 +41,13 @@ def test_relu_bwd_colsum(B, H):
     _run("check_relu_bwd_colsum", B=B, H=H, seed=B + H)
 
 
-def test_relu_bwd_colsum_refuses_odd_width():
+def test_relu_bwd_colsum_raises_on_odd_width():
     import torch
-    from distributedmnist_b200.ops.lib import load, ptr, stream_ptr
+    from distributedmnist_b200.ops.lib import KernelLibraryError, load, stream_ptr
     dh = torch.zeros(4, 4, dtype=torch.bfloat16, device="cuda")
     g = torch.zeros(4, device="cuda")
-    assert load().dm_relu_bwd_colsum(ptr(dh), ptr(None), ptr(None), ptr(g), 4, 3, stream_ptr()) == -1
+    with pytest.raises(KernelLibraryError, match=r"code -1\b"):
+        load().dm_relu_bwd_colsum(dh, None, None, g, 4, 3, stream_ptr())
 
 
 @pytest.mark.parametrize("B", [1, 3, 1001, 8191])

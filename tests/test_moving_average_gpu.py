@@ -2,7 +2,6 @@
 bit against the float32 emulation, graph-replayed lenet and mlp2 steps (training unperturbed, the shadow after every step
 equal to the emulation over the recorded weights), a lenet pass on the average, a device checkpoint carrying the average,
 ``train()`` with ``--eval_moving_average --target_accuracy``, and two replicas at K = N."""
-import ctypes
 import json
 import os
 
@@ -22,11 +21,9 @@ def _bits(a):
 
 
 def _launch(shadow, w, g, decay, bf16=None, ranges=(0, 0, 0, 0), step_out=None):
-    from distributedmnist_b200.ops.lib import check, load, ptr, stream_ptr
+    from distributedmnist_b200.ops.lib import load, stream_ptr
     epoch = torch.tensor([g], dtype=torch.int64, device="cuda").view(torch.int32)[:1]   # low word, little endian
-    check(load().dm_moving_average(ptr(shadow), ptr(w), ctypes.c_longlong(shadow.numel()), ptr(epoch),
-                                   ctypes.c_double(decay), ptr(step_out), ptr(bf16), *[ctypes.c_longlong(v) for v in ranges],
-                                   stream_ptr()), "moving_average")
+    load().dm_moving_average(shadow, w, shadow.numel(), epoch, decay, step_out, bf16, *ranges, stream_ptr())
     torch.cuda.synchronize()
 
 
@@ -67,16 +64,15 @@ def test_kernel_bit_exact_against_the_emulation(numel):
     assert torch.equal(bf.cpu()[r[0]:r[1]].view(torch.int16), torch.from_numpy(s[r[0]:r[1]]).to(torch.bfloat16).view(torch.int16))
 
 
-def test_kernel_refuses_bad_arguments():
-    from distributedmnist_b200.ops.lib import load, ptr, stream_ptr
+def test_kernel_raises_on_bad_arguments():
+    from distributedmnist_b200.ops.lib import KernelLibraryError, load, stream_ptr
     lib = load()
     t = torch.zeros(64, device="cuda")
     e = torch.zeros(1, dtype=torch.int32, device="cuda")
     b = torch.zeros(64, dtype=torch.bfloat16, device="cuda")
-    L = ctypes.c_longlong
     for decay, rg in ((1.0, (0, 0, 0, 0)), (0.0, (0, 0, 0, 0)), (0.5, (2, 8, 0, 0)), (0.5, (0, 68, 0, 0)), (0.5, (8, 4, 0, 0))):
-        assert lib.dm_moving_average(ptr(t), ptr(t), L(64), ptr(e), ctypes.c_double(decay), None, ptr(b), *map(L, rg),
-                                     stream_ptr()) == -1
+        with pytest.raises(KernelLibraryError, match=r"code -1\b"):
+            lib.dm_moving_average(t, t, 64, e, decay, None, b, *rg, stream_ptr())
 
 
 def _engine(model="lenet", B=256, seed=5, decay=None):

@@ -2,7 +2,6 @@
 with ``--max_steps=S`` (pipelined and non-pipelined loop), the device threshold at ``need - 1`` / ``need``, snapshot passes
 (a dropped pass never stops the run; K > N and interval end at min(max_steps, S)), the synchronise count per step, and the
 multi-replica runs."""
-import ctypes
 import json
 import os
 
@@ -129,10 +128,8 @@ def test_device_threshold_is_need_not_need_minus_one():
 
 
 def _emulate(eng, g, mode, phases=7):
-    from distributedmnist_b200.ops.lib import check, stream_ptr
-    check(eng.lib.dm_snap_test_emulate(ctypes.c_void_p(eng.backend.ctrl.local_ptr), ctypes.c_void_p(eng.params.data_ptr()),
-                                       ctypes.c_longlong(eng.params.numel()), ctypes.c_uint(g), mode, 1, phases,
-                                       stream_ptr()), "snap_test_emulate")
+    from distributedmnist_b200.ops.lib import stream_ptr
+    eng.lib.dm_snap_test_emulate(eng.backend.ctrl.local_ptr, eng.params, eng.params.numel(), g, mode, 1, phases, stream_ptr())
 
 
 @pytest.mark.parametrize("mode", [K_OF_N, INTERVAL], ids=["k_of_n", "interval"])

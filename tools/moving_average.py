@@ -72,10 +72,9 @@ def child_step_time(model, batch, hidden, decay, steps, warmup):
 
 
 def kernel_times(iters=200):
-    import ctypes
     import torch
     from distributedmnist_b200.models import get_model
-    from distributedmnist_b200.ops.lib import check, load, ptr, stream_ptr
+    from distributedmnist_b200.ops.lib import load, stream_ptr
     lib = load()
     out = []
     for model, hidden in (("lenet", 1024), ("mlp3", 4096)):
@@ -90,17 +89,14 @@ def kernel_times(iters=200):
             for name in ("conv2_weights", "fc1_weights"):
                 q = spec.param(name)
                 rg += [q.offset, q.offset + q.numel]
-        L = ctypes.c_longlong
-        variants = {"update": (ptr(w), None, [0, 0, 0, 0]), "update_bf16": (ptr(w), ptr(bf), rg),
-                    "bf16_only": (ctypes.c_void_p(0), ptr(bf), rg)}
+        variants = {"update": (w, None, [0, 0, 0, 0]), "update_bf16": (w, bf, rg), "bf16_only": (None, bf, rg)}
         row = dict(model=model, arena_floats=n)
         for name, (wp, bp, r) in variants.items():
             if model != "lenet" and name != "update":
                 continue
 
             def launch():
-                check(lib.dm_moving_average(ptr(s), wp, L(n), ptr(epoch), ctypes.c_double(0.999), None, bp,
-                                            *map(L, r), stream_ptr()), "moving_average")
+                lib.dm_moving_average(s, wp, n, epoch, 0.999, None, bp, *r, stream_ptr())
             for _ in range(10):
                 launch()
             t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
