@@ -10,11 +10,12 @@
 //                      stored into a page-locked host word that the host reads after the step's completion event.
 //
 // The stop words are one symmetric allocation (FusedBackend.allocate_buffer), 0 until a stop is set; only the chief writes
-// them, once.  Why every replica of a K = N run stops at the same S, and why margin = 2: DESIGN §4.4.
+// them, once (store_stop_once, stop_word.cuh: eval_patience, csrc/eval_patience.cu, may set the stop instead).  Why every replica of a K = N run stops at the same S, and why margin = 2: DESIGN §4.4.
 #include <stdint.h>
 
 #include "eval_state.cuh"
 #include "fused_sync.cuh"
+#include "stop_word.cuh"
 
 namespace dm {
 
@@ -36,12 +37,7 @@ __global__ void eval_target_kernel(const __grid_constant__ TargetArgs a) {
   if (a.status_ptr != nullptr && *a.status_ptr <= 0) return;
   const EvalState* st = a.st;
   if (st->examples != a.examples || st->correct < a.need) return;
-  if (*reinterpret_cast<volatile uint32_t*>(a.stop[a.rank]) != 0u) return;     // an earlier pass set the stop
-  const uint32_t s = *a.step_ptr + a.margin;
-  for (int r = 0; r < a.nranks; ++r) *reinterpret_cast<volatile uint32_t*>(a.stop[r]) = s;
-  // orders the stores before everything the chief's stream does after this kernel, in particular before its next step's
-  // exchange, which every peer has to observe before it can finish that step
-  __threadfence_system();
+  store_stop_once(a.stop, a.rank, a.nranks, *a.step_ptr + a.margin);
 }
 
 __global__ void stop_publish_kernel(const uint32_t* stop, volatile uint32_t* host) {

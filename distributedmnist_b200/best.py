@@ -16,14 +16,17 @@ BEST_DIR = "best"
 BEST_JSON = "worker%d_best.json"
 
 
+def counts(examples: int, n: int, status: Optional[int] = None) -> bool:
+    """True if a pass over ``examples`` rows may be compared with others at all: it scored the whole validation set of
+    ``n`` rows, and ``status`` -- None for a pass over the live arena or the moving average; for a snapshot pass its
+    SnapState.status -- says the snapshot was accepted (> 0).  The test eval_target and eval_patience apply too."""
+    return (status is None or status > 0) and examples == n
+
+
 def improves(correct: int, examples: int, n: int, best_correct: int, status: Optional[int] = None) -> bool:
-    """True if a pass with ``correct`` of ``examples`` rows becomes the new best over ``best_correct``: it scored the whole
-    validation set of ``n`` rows, and beats the best strictly (on ties the earlier pass stays).  ``status``: None for a
-    pass over the live arena or the moving average; for a snapshot pass its SnapState.status, which counts only when the
-    snapshot was accepted (> 0) -- the test eval_target applies too."""
-    if status is not None and status <= 0:
-        return False
-    return examples == n and correct > best_correct
+    """True if a pass with ``correct`` of ``examples`` rows becomes the new best over ``best_correct``: it counts (see
+    :func:`counts`) and beats the best strictly (on ties the earlier pass stays)."""
+    return counts(examples, n, status) and correct > best_correct
 
 
 def emulate_decide(correct: int, examples: int, loss_sum: float, step: int, n: int, best: Tuple,

@@ -32,7 +32,9 @@ from typing import Optional, Tuple
 import numpy as np
 import torch
 
+from . import early_stopping
 from .best import BEST_CORRECT_WORD, BEST_EXAMPLES_WORD, BEST_STEP_WORD, BEST_VALID_WORD
+from .early_stopping import PAT_BASELINE_WORD, PAT_BEST_STEP_WORD, PAT_BEST_WORD, PAT_SINCE_WORD, PAT_TRIGGER_WORD
 from .engine import ComputeEngine
 from .models import get_model
 from .models.lenet import dropout_seed_mix
@@ -1013,7 +1015,8 @@ class CudaLeNetEngine(_CudaEngine):
         self._ev_average = bool(moving_average)
         self._target = None
         self._best = None
-        self._launch_eval(publish=False)        # sets the kernels' function attributes outside a capture
+        self._patience = None
+        self._launch_eval(publish=False)       # sets the kernels' function attributes outside a capture
         torch.cuda.synchronize()
         if self._snapshot:
             self._ev_snap.reset()                 # statistics count real passes only
@@ -1077,6 +1080,10 @@ class CudaLeNetEngine(_CudaEngine):
             need, margin = self._target
             lib.dm_eval_target(self._ev_state, step_ptr, status_ptr, need, n, margin, self._stop.ptr_table(),
                                self.backend.ctx.rank, self.backend.ctx.world_size, sp)
+        if publish and self._patience is not None:
+            state, patience, delta_rows, margin = self._patience
+            lib.dm_eval_patience(self._ev_state, step_ptr, status_ptr, n, patience, delta_rows, margin, state,
+                                 self._stop.ptr_table(), self.backend.ctx.rank, self.backend.ctx.world_size, sp)
 
     def enqueue_eval(self) -> None:
         """Score the validation set with the current weights, on the current (training) stream, without a host
@@ -1245,6 +1252,36 @@ class CudaLeNetEngine(_CudaEngine):
         u = w.numpy().view(np.uint32)
         return (arena.clone(), int(u[BEST_STEP_WORD]), int(u[BEST_CORRECT_WORD]), int(u[BEST_EXAMPLES_WORD]),
                 float(w[:2].numpy().view(np.float64)[0]))
+
+    # ---- early stopping (csrc/eval_patience.cu) ---------------------------------------------------------------------------
+    # With a patience armed, every evaluation pass ends (after eval_best_* and eval_target) with eval_patience, which applies
+    # the rule of early_stopping.advance to the pass's record and PatienceState and, once the patience is exhausted, sets
+    # the stop step as eval_target does.  Nothing is read back until patience_state().
+    _patience = None               # (PatienceState words, patience, min_delta rows, margin), see arm_patience
+
+    def arm_patience(self, patience: int, min_delta_rows: int, margin: int) -> None:
+        """Chief, after :meth:`arm_eval` and :meth:`arm_stop`: stop the run at S = g + ``margin`` once ``patience``
+        counting passes in a row, the last of global step g, have not beaten the best count by more than
+        ``min_delta_rows``.  Re-captures the evaluation graph."""
+        if self._stop is None or getattr(self, "_ev_x", None) is None:
+            raise RuntimeError("arm_patience: arm_eval() and arm_stop() first")
+        n = int(self._ev_x.shape[0])
+        if int(patience) < 1 or not 0 <= int(min_delta_rows) < n or int(margin) < 1:
+            raise ValueError("arm_patience: patience %d, min_delta %d of %d rows, margin %d"
+                             % (patience, min_delta_rows, n, margin))
+        self._leave_native_runner()
+        words = torch.zeros(int(self.lib.dm_patience_state_bytes()) // 4, dtype=torch.int32, device=self.device)
+        self._patience = (words, int(patience), int(min_delta_rows), int(margin))
+        self._capture_eval()
+
+    def patience_state(self) -> Optional[early_stopping.State]:
+        """The PatienceState as the passes so far left it, or None when no patience is armed (synchronises the device)."""
+        if self._patience is None:
+            return None
+        torch.cuda.synchronize()
+        u = self._patience[0].cpu().numpy().view(np.uint32)
+        return early_stopping.State(int(u[PAT_BEST_WORD]), int(u[PAT_SINCE_WORD]), int(u[PAT_BEST_STEP_WORD]),
+                                    int(u[PAT_TRIGGER_WORD]), bool(u[PAT_BASELINE_WORD]))
 
 
 # dm_dense10_xent (csrc/mlp_simt.cu) stages the output-layer weights as [H][11] floats and refuses more than 220 KiB

@@ -277,6 +277,13 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_boolean("keep_best_checkpoint", False, "With --eval_every_steps: keep the weights of the best-scoring "
                                                     "in-training evaluation and save them at the end of the run as "
                                                     "train_dir/best/model.ckpt-<step> plus worker0_best.json")
+    F.DEFINE_integer("early_stopping_patience", 0, "With --eval_every_steps: stop the run once this many in-training "
+                                                   "evaluations in a row have not beaten the best so far (by more than "
+                                                   "--early_stopping_min_delta), at the scored step + 2; report in "
+                                                   "worker0_early_stopping.json; 0 = off, else P >= 1")
+    F.DEFINE_float("early_stopping_min_delta", 0.0, "With --early_stopping_patience: the accuracy an evaluation must beat "
+                                                    "the best by to reset the patience, rounded down to whole validation "
+                                                    "rows; 0 <= D < 1")
     return F
 
 

@@ -67,6 +67,9 @@ def _signatures() -> dict:
         "dm_eval_max_rows": (V, i, []),
         "dm_eval_stamp": (S, i, [P, P]),
         "dm_eval_head": (S, i, [P, ll, i, P, P, P, P, P, P, P, P, P, i, P, i, i, P]),
+        # eval_patience.cu
+        "dm_patience_state_bytes": (V, i, []),
+        "dm_eval_patience": (S, i, [P, P, P, u, u, u, u, P, PP, i, i, P]),
         # eval_snapshot.cu
         "dm_snap_state_bytes": (V, i, []),
         "dm_snap_select": (S, i, [P, P, i, i, d, P]),

@@ -31,9 +31,10 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
-from . import moving_average
+from . import best, early_stopping, moving_average
 from .best import BEST_DIR, BEST_JSON
 from .checkpoint import Saver
+from .early_stopping import EARLY_STOPPING_JSON
 from .engine import make_engine
 from .flags import FLAGS
 from .parallel.aggregators import (SyncReplicasOptimizer, TimeoutReplicasOptimizer,
@@ -328,6 +329,29 @@ def check_target_flags(flags, ctx: ReplicaContext) -> None:
                          % (flags.backend, "" if ctx.on_gpu else ", no GPU", ctx.world_size))
 
 
+def check_early_stopping_flags(flags, ctx: ReplicaContext) -> None:
+    """``--early_stopping_patience`` / ``--early_stopping_min_delta`` combinations that cannot work, rejected before any
+    device work starts.  Where the in-training evaluation itself is refused (check_eval_flags), so is early stopping."""
+    p = int(getattr(flags, "early_stopping_patience", 0) or 0)
+    d = float(getattr(flags, "early_stopping_min_delta", 0.0) or 0.0)
+    if p < 0:
+        raise ValueError("--early_stopping_patience must be >= 1 (0 = off), got %d" % p)
+    if not 0.0 <= d < 1.0:
+        raise ValueError("--early_stopping_min_delta must lie in [0, 1), got %r" % d)
+    if p == 0:
+        if d != 0.0:
+            raise ValueError("--early_stopping_min_delta needs --early_stopping_patience >= 1: without a patience there "
+                             "is nothing for it to change")
+        return
+    if getattr(flags, "eval_every_steps", 0) <= 0:
+        raise ValueError("--early_stopping_patience needs --eval_every_steps > 0: the patience counts in-training "
+                         "evaluations")
+    if not (ctx.on_gpu and flags.backend in ("auto", "fused")) and ctx.world_size > 1:
+        raise ValueError("--early_stopping_patience with the torch engine (--backend=%s%s) is implemented for one "
+                         "replica, not %d: only the chief evaluates and nothing tells the other replicas to stop"
+                         % (flags.backend, "" if ctx.on_gpu else ", no GPU", ctx.world_size))
+
+
 def check_best_flags(flags) -> None:
     """``--keep_best_checkpoint`` combinations that cannot work, rejected before any device work starts.  Where the
     in-training evaluation itself is refused (check_eval_flags), so is keeping its best weights."""
@@ -438,6 +462,35 @@ class _TimeToAccuracy:
         return out
 
 
+class _EarlyStopping:
+    """``--early_stopping_patience`` on the chief: :func:`early_stopping.advance` over the evaluation passes, in order.  On
+    the sm_90a path eval_patience has made the same decisions on the device, which set the stop; this replays them from
+    the pass records for the report.  With the torch engine this is where the stop is decided."""
+
+    def __init__(self, patience: int, min_delta: float, examples: int, weights: str):
+        self.patience, self.min_delta, self.examples, self.weights = patience, min_delta, examples, weights
+        self.delta_rows = early_stopping.min_delta_rows(min_delta, examples)
+        self.state = early_stopping.State()
+        self.counted = 0             # counting passes up to the one that exhausted the patience
+
+    def add(self, step: int, examples: int, correct: int, status: Optional[int] = None) -> bool:
+        """One completed pass (``status`` as best.counts takes it).  True if it exhausted the patience."""
+        if not early_stopping.exhausted(self.state, self.patience) and best.counts(examples, self.examples, status):
+            self.counted += 1
+        self.state, fired = early_stopping.advance(self.state, step, correct, examples, self.examples, self.patience,
+                                                   self.delta_rows, status)
+        return fired
+
+    def report(self) -> Dict:
+        s = self.state
+        fired = early_stopping.exhausted(s, self.patience)
+        return dict(patience=self.patience, min_delta=self.min_delta, min_delta_rows=self.delta_rows,
+                    examples=self.examples, triggered=fired, trigger_step=s.trigger_step if fired else None,
+                    stop_step=s.trigger_step + STOP_MARGIN if fired else None,
+                    best_step=s.best_step if s.baseline else None, best_correct=s.best if s.baseline else None,
+                    counted_passes=self.counted, weights=self.weights)
+
+
 def eval_due(global_step: int, last_mark: int, every: int) -> bool:
     """Snapshot passes (K < N, interval): the host learns the global step only after a step completes, and it may jump by
     more than one.  A pass is due once the newest consumed global step has crossed a multiple of ``every`` since
@@ -456,11 +509,14 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     is_chief = ctx.is_chief
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
     check_target_flags(flags, ctx)
+    check_early_stopping_flags(flags, ctx)
     check_best_flags(flags)
     check_moving_average_flags(flags, ctx, num_replicas_to_aggregate)
     check_device_data_flags(flags, ctx, dataset)
     device_data = bool(getattr(flags, "device_data", False))
     target = float(getattr(flags, "target_accuracy", 0.0) or 0.0)
+    patience = int(getattr(flags, "early_stopping_patience", 0) or 0)
+    stop_armed = bool(target or patience)      # something may set a stop step S before --max_steps
     ema_decay = float(getattr(flags, "moving_average_decay", 0.0) or 0.0) if is_chief else 0.0
     eval_average = bool(ema_decay and getattr(flags, "eval_moving_average", False))
 
@@ -550,15 +606,24 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     # every step's last kernel copies it to the host; torch engine (one replica): decided on the host after `evaluate`.
     max_steps = flags.max_steps
     tta = None
-    if target:
-        if fused_step:
-            engine.arm_stop()              # every replica (a symmetric allocation)
-        if is_chief:
-            n_val = dataset_test.num_examples
-            tta = _TimeToAccuracy(target, need_count(target, n_val), n_val, 1e-9 if device_eval else 1.0,
-                                  "device %globaltimer" if device_eval else "host")
-            if device_eval:
-                engine.arm_target(tta.need, STOP_MARGIN)
+    if stop_armed and fused_step:
+        engine.arm_stop()                  # every replica (a symmetric allocation), for a target or a patience
+    if target and is_chief:
+        n_val = dataset_test.num_examples
+        tta = _TimeToAccuracy(target, need_count(target, n_val), n_val, 1e-9 if device_eval else 1.0,
+                              "device %globaltimer" if device_eval else "host")
+        if device_eval:
+            engine.arm_target(tta.need, STOP_MARGIN)
+    eval_weights = "snapshot" if snapshot_eval else ("moving_average" if eval_average else "live")
+    # --early_stopping_patience: the run ends as --max_steps = min(--max_steps, S) would end it, S = g + STOP_MARGIN for the
+    # pass of global step g that exhausts the patience -- decided like the target (GPU path: eval_patience on the device,
+    # after eval_target, so whichever fires first sets S; torch engine: on the host after `evaluate`).
+    es = None
+    if patience and is_chief:
+        es = _EarlyStopping(patience, float(getattr(flags, "early_stopping_min_delta", 0.0) or 0.0),
+                            dataset_test.num_examples, eval_weights)
+        if device_eval:
+            engine.arm_patience(patience, es.delta_rows, STOP_MARGIN)
     # --keep_best_checkpoint: the chief keeps the weights of its best-scoring evaluation (GPU path: decided and copied on the
     # device inside the pass's graph; torch engine: after `evaluate`) and writes them once, after the final pass.  A best
     # file of an earlier run sets the count to beat.
@@ -661,14 +726,16 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     def collect_evals() -> None:
         """Device records completed so far (%globaltimer ns -> seconds, as push_device_times converts them)."""
         nonlocal test_acc_value
-        if tta is None:
+        if tta is None and es is None:
             recs = [(r, 0) for r in engine.eval_records()]
-        else:                      # dropped snapshot passes took training-stream time too
+        else:                      # dropped snapshot passes took training-stream time too, and count for neither rule
             recs = engine.eval_records_with_status()
             engine.eval_dropped += sum(1 for _r, status in recs if status < 0)
         for (gs, t0, t1, n_ex, correct, loss_sum), status in recs:
             if tta is not None:
                 tta.add(gs, t0, t1, n_ex, correct, status >= 0, time.time() - tta_wall0)
+            if es is not None:
+                es.add(gs, n_ex, correct, status if snapshot_eval else None)
             if status < 0:
                 continue
             eval_rows.append((gs, t0 * 1e-9, (t1 - t0) * 1e-9, n_ex, correct, loss_sum / max(n_ex, 1)))
@@ -710,6 +777,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         if keep_best:
             engine.note_eval(global_step, n_ex, n_ex, correct, loss * n_ex, moving_average=eval_average)
         if tta is not None and tta.add(global_step, t0, t1, n_ex, correct, True, t1 - tta_wall0):
+            max_steps = min(max_steps, global_step + STOP_MARGIN)
+        if es is not None and es.add(global_step, n_ex, correct):
             max_steps = min(max_steps, global_step + STOP_MARGIN)
 
     def save_evals() -> None:
@@ -758,7 +827,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 info = opt._account(backend.mirror_info(seq, check=True))
                 if device_eval:
                     collect_evals()            # passes enqueued before the step just waited for are complete
-                if target:
+                if stop_armed:
                     note_stop()
                 now = time.time()
                 finish_iteration(it, last_consume, info, (float(lbuf[0]), float(lbuf[1])))
@@ -801,7 +870,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 engine.train_step()
             t2 = time.perf_counter()
             info = opt._account(engine.step_info())   # device -> host read of the step's outcome (one packed copy)
-            if target:
+            if stop_armed:
                 note_stop()                           # (the read above waited for the whole step)
         else:
             engine.forward_backward(opt.local_step)
@@ -870,13 +939,29 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                         report["train_time_s"], tta.clock, report["wall_time_s"]))
         else:
             log.info("Time to accuracy: target %g not reached" % target)
+    if es is not None:
+        rep = results["early_stopping"] = es.report()
+        with open(os.path.join(flags.train_dir, EARLY_STOPPING_JSON % ctx.rank), "w") as f:
+            json.dump(rep, f, indent=1)
+            f.write("\n")
+        device_state = engine.patience_state() if device_eval else None
+        if device_state is not None and device_state != es.state:
+            log.warning("Early stopping: the device state %s differs from the replay of the evaluation records %s"
+                        % (device_state, es.state))
+        if rep["triggered"]:
+            log.info("Early stopping: patience %d exhausted by the evaluation of global step #%d, the best being that of "
+                     "global step #%d (%d of %d correct, min_delta %d rows); the run ends as --max_steps=%d would end it"
+                     % (patience, rep["trigger_step"], rep["best_step"], rep["best_correct"], rep["examples"],
+                        rep["min_delta_rows"], rep["stop_step"]))
+        else:
+            log.info("Early stopping: patience %d not exhausted after %d counted evaluation(s)"
+                     % (patience, rep["counted_passes"]))
     if keep_best:
-        kind = "snapshot" if snapshot_eval else ("moving_average" if eval_average else "live")
-        rep = results["best"] = save_best(engine, spec, flags.train_dir, ctx.rank, kind)
+        rep = results["best"] = save_best(engine, spec, flags.train_dir, ctx.rank, eval_weights)
         if rep is not None:
             log.info("Best weights: the evaluation of global step #%d (accuracy %f, %d of %d correct, mean loss %f, %s "
                      "weights) saved under %s" % (rep["global_step"], rep["accuracy"], rep["correct"], rep["examples"],
-                                                  rep["mean_loss"], kind, os.path.join(flags.train_dir, BEST_DIR)))
+                                                  rep["mean_loss"], eval_weights, os.path.join(flags.train_dir, BEST_DIR)))
         else:
             log.info("Best weights: no complete evaluation of this run scored more than %d correct; nothing written"
                      % best_seed)
