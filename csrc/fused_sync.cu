@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(SYNC_THREADS, 1) fused_sync_sgd_kernel(SyncPee
     const int end = min(begin + shard, a.numel4);
     own_begin = begin;
     own_end = end;
-    const float scale = cta_scale(a, epoch, (uint32_t)count);
+    const float scale = cta_scale(a, me, epoch, (uint32_t)count);
     const uint32_t drop_thresh = a.drop_keep > 0.f ? (uint32_t)(a.drop_keep * 16777216.f) : 0u;
     int contrib[SYNC_MAX_RANKS];
     int nc = 0;
@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(EARLY_THREADS) fused_sync_early_kernel(SyncPee
   const int shard = (n4 + a.nranks - 1) / a.nranks;
   const int begin = r.begin4 + a.rank * shard;
   const int end = min(begin + shard, r.end4);
-  const float scale = cta_scale(a, epoch, (uint32_t)a.nranks);
+  const float scale = cta_scale(a, me, epoch, (uint32_t)a.nranks);
   const float* wsrc = P.params[a.rank];
   const int stride = gridDim.x * EARLY_THREADS;
   if (a.mc_grads != nullptr && a.mc_params != nullptr) {
@@ -434,7 +434,7 @@ __global__ void __launch_bounds__(SYNC_THREADS, 1) fused_sync_late_kernel(SyncPe
   if (blockIdx.x == 0 && threadIdx.x == 0) me->t_phase[1] = globaltimer_ns();
 
   // ---- one-shot on the late bucket: every rank sums all contributions in rank order and updates its own copy -------------
-  const float scale = cta_scale(a, epoch, (uint32_t)a.nranks);
+  const float scale = cta_scale(a, me, epoch, (uint32_t)a.nranks);
   float* wdst = P.params[a.rank];
   const int stride = gridDim.x * SYNC_THREADS;
   // late bucket = [begin4, end4) minus the early range: walk a compacted index
@@ -695,6 +695,18 @@ int dm_fused_sync_bucket(void* const* ctrl, void* const* params, void* const* gr
 int dm_sync_set_host_mirror(void* ctrl, void* host_ptr) {
   using dm::SyncCtrl;
   DM_CUDA_OK(cudaMemcpy(reinterpret_cast<char*>(ctrl) + offsetof(SyncCtrl, host_mirror), &host_ptr, sizeof(void*),
+                        cudaMemcpyHostToDevice));
+  return 0;
+}
+
+// Point the control block's learning-rate cut table (SyncCtrl::lr_cuts: SYNC_MAX_CUTS u32 cut steps in device memory,
+// 0xFFFFFFFF = no cut) at `table`, with the factor 0 < `factor` < 1 each cut multiplies the rate by; null = no cuts.
+int dm_sync_set_lr_cuts(void* ctrl, const void* table, double factor) {
+  using dm::SyncCtrl;
+  if (ctrl == nullptr || (table != nullptr && !(factor > 0.0 && factor < 1.0))) return -1;
+  DM_CUDA_OK(cudaMemcpy(reinterpret_cast<char*>(ctrl) + offsetof(SyncCtrl, lr_cuts), &table, sizeof(void*),
+                        cudaMemcpyHostToDevice));
+  DM_CUDA_OK(cudaMemcpy(reinterpret_cast<char*>(ctrl) + offsetof(SyncCtrl, lr_factor), &factor, sizeof(double),
                         cudaMemcpyHostToDevice));
   return 0;
 }

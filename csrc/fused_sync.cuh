@@ -15,6 +15,7 @@ constexpr int SYNC_MAX_RANKS = 8;
 constexpr int SYNC_RING = 64;          // commit-word ring (steps)
 constexpr int SYNC_THREADS = 512;
 constexpr int TIMING_RING = 1024;      // per-rank arrival-timestamp ring (steps)
+constexpr int SYNC_MAX_CUTS = 32;      // learning-rate cuts per run (SyncCtrl::lr_cuts, lr_plateau.MAX_CUTS)
 
 // Control block, one per rank, in symmetric memory.  Words written remotely are spread over
 // separate 128-byte lines.
@@ -39,7 +40,12 @@ struct SyncCtrl {
   uint32_t error;                // watchdog: 1 = arrival timeout, 2 = done timeout
   uint32_t accepted_steps, dropped_steps;
   uint32_t last_mask, last_count, last_late;
-  uint32_t pad1[32];
+  uint32_t pad1[29];
+  // learning-rate cuts (--lr_plateau_patience, csrc/eval_plateau.cu): this replica's table of SYNC_MAX_CUTS cut steps
+  // (0xFFFFFFFF = no cut), written by the chief's eval_plateau over NVLink; null when no table is armed.  Set once by
+  // dm_sync_set_lr_cuts.  These words were padding: the size and every other offset of the block are unchanged.
+  const uint32_t* lr_cuts;
+  double lr_factor;              // F: the rate is multiplied by F^c, c = cuts in effect
   unsigned long long t_arrive[TIMING_RING];   // %globaltimer at arrival, per local step (cdf telemetry)
   unsigned long long t_start[TIMING_RING];    // %globaltimer stamped by the step's first kernel
   unsigned long long t_phase[8];              // last launch: kernel start, decided, reduced, pushed, landed, shadowed
@@ -73,6 +79,9 @@ struct SyncCtrl {
   uint32_t pad3[14];
   volatile uint32_t bar[SYNC_MAX_RANKS * 32];   // [p*32]: peer p entered device barrier number (value)
 };
+static_assert(SYNC_MAX_CUTS == 32, "cta_scale reads one cut-table entry per lane of a warp");
+static_assert(offsetof(SyncCtrl, lr_cuts) % 8 == 0 && offsetof(SyncCtrl, lr_factor) + 8 == offsetof(SyncCtrl, t_arrive),
+              "the cut-table words take the place of pad1's last words, with no change to the layout around them");
 
 struct SyncPeers {
   SyncCtrl* ctrl[SYNC_MAX_RANKS];
@@ -176,11 +185,25 @@ DMNIST_DEVICE void publish_status(SyncCtrl* me, uint32_t epoch_after, uint32_t a
 // and the division in double, rounded to fp32 once.  --use_fast_math leaves double precision alone (fp32 would turn the
 // power into lg2/ex2.approx and the division into div.approx); CUDA's double pow is within 2 ulp, far below fp32 rounding.
 // Thread 0 evaluates it and the CTA reads it after a barrier: every thread of the CTA must call this.
-DMNIST_DEVICE float cta_scale(const SyncArgs& a, uint32_t step, uint32_t count) {
+//
+// Learning-rate cuts (--lr_plateau_patience): when `ctrl` is non-null and holds a cut table, warp 0 counts the cuts in
+// effect at `step` -- c = entries <= step, one relaxed load per lane and a ballot -- and the rate becomes
+// lr0 * decay_rate^p * F^c / count, the product in that order in double, as schedule.LearningRateSchedule computes it.
+// With c = 0 the factor is 1.0 and the value is the one without a table.  The chief's stores into the table reach every
+// replica before any launch whose `step` they concern (DESIGN §4, learning-rate cuts).  ctrl = null (interval mode): no cuts.
+DMNIST_DEVICE float cta_scale(const SyncArgs& a, const SyncCtrl* ctrl, uint32_t step, uint32_t count) {
   __shared__ float s_scale;
-  if (threadIdx.x == 0) {
-    const double p = (double)(step / (uint32_t)max(a.decay_steps, 1));
-    s_scale = (float)(a.lr0 * pow(a.decay_rate, p) / (double)count);
+  if (threadIdx.x < 32) {
+    const uint32_t* cuts = ctrl != nullptr ? ctrl->lr_cuts : nullptr;
+    double f = 1.0;
+    if (cuts != nullptr) {
+      const int c = __popc(__ballot_sync(0xffffffffu, ld_relaxed_sys(cuts + threadIdx.x) <= step));
+      if (c > 0) f = pow(ctrl->lr_factor, (double)c);
+    }
+    if (threadIdx.x == 0) {
+      const double p = (double)(step / (uint32_t)max(a.decay_steps, 1));
+      s_scale = (float)(a.lr0 * pow(a.decay_rate, p) * f / (double)count);
+    }
   }
   __syncthreads();
   return s_scale;

@@ -32,9 +32,10 @@ from typing import Optional, Tuple
 import numpy as np
 import torch
 
-from . import early_stopping
+from . import early_stopping, lr_plateau
 from .best import BEST_CORRECT_WORD, BEST_EXAMPLES_WORD, BEST_STEP_WORD, BEST_VALID_WORD
 from .early_stopping import PAT_BASELINE_WORD, PAT_BEST_STEP_WORD, PAT_BEST_WORD, PAT_SINCE_WORD, PAT_TRIGGER_WORD
+from .lr_plateau import PL_BASELINE_WORD, PL_BEST_WORD, PL_CUTS_WORD, PL_SINCE_WORD, PL_TRIGGER_WORD
 from .engine import ComputeEngine
 from .models import get_model
 from .models.lenet import dropout_seed_mix
@@ -1016,6 +1017,7 @@ class CudaLeNetEngine(_CudaEngine):
         self._target = None
         self._best = None
         self._patience = None
+        self._plateau = None
         self._launch_eval(publish=False)       # sets the kernels' function attributes outside a capture
         torch.cuda.synchronize()
         if self._snapshot:
@@ -1084,6 +1086,10 @@ class CudaLeNetEngine(_CudaEngine):
             state, patience, delta_rows, margin = self._patience
             lib.dm_eval_patience(self._ev_state, step_ptr, status_ptr, n, patience, delta_rows, margin, state,
                                  self._stop.ptr_table(), self.backend.ctx.rank, self.backend.ctx.world_size, sp)
+        if publish and self._plateau is not None:
+            state, patience, delta_rows, margin = self._plateau
+            lib.dm_eval_plateau(self._ev_state, step_ptr, status_ptr, n, patience, delta_rows, margin, state,
+                                self._lr_table.ptr_table(), self.backend.ctx.world_size, sp)
 
     def enqueue_eval(self) -> None:
         """Score the validation set with the current weights, on the current (training) stream, without a host
@@ -1282,6 +1288,64 @@ class CudaLeNetEngine(_CudaEngine):
         u = self._patience[0].cpu().numpy().view(np.uint32)
         return early_stopping.State(int(u[PAT_BEST_WORD]), int(u[PAT_SINCE_WORD]), int(u[PAT_BEST_STEP_WORD]),
                                     int(u[PAT_TRIGGER_WORD]), bool(u[PAT_BASELINE_WORD]))
+
+    # ---- learning-rate cuts at a plateau (csrc/eval_plateau.cu) -----------------------------------------------------------
+    # Every replica owns a cut table (symmetric memory) that its control block points at: the aggregation kernels multiply
+    # the rate by F^c, c = the table's entries <= the step they update (cta_scale, csrc/fused_sync.cuh).  With a plateau
+    # armed, the chief's evaluation pass ends (after eval_patience) with eval_plateau, which applies the rule of
+    # lr_plateau.advance and stores each cut's step S into every replica's table.  The step graphs are not re-captured: the
+    # kernels read the table through the control block.  Nothing is read back until lr_plateau_state().
+    _lr_table = None               # symmetric u32[lr_plateau.MAX_CUTS] cut table, see arm_lr_cuts
+    _plateau = None                # (PlateauState words, patience, min_delta rows, margin), see arm_lr_plateau
+
+    def arm_lr_cuts(self, factor: float, cuts=()) -> None:
+        """Every replica (symmetric memory: collective, every rank calls it at the same point): allocate this replica's
+        cut table, store the steps ``cuts`` (those a restarted run keeps) in its first entries and point the aggregation
+        kernels at it, each cut multiplying the rate by ``factor``."""
+        cuts = [int(s) for s in cuts]
+        if not 0.0 < float(factor) < 1.0 or len(cuts) > lr_plateau.MAX_CUTS:
+            raise ValueError("arm_lr_cuts: factor %r, %d cuts" % (factor, len(cuts)))
+        self._lr_table = self.backend.allocate_buffer(4 * lr_plateau.MAX_CUTS)
+        words = np.full(lr_plateau.MAX_CUTS, lr_plateau.NO_CUT, dtype=np.uint32)
+        words[:len(cuts)] = cuts
+        self._lr_table.view(torch.int32, 0, lr_plateau.MAX_CUTS).copy_(torch.from_numpy(words.view(np.int32)))
+        torch.cuda.synchronize()
+        self.lib.dm_sync_set_lr_cuts(self.backend.ctrl.local_ptr, self._lr_table.local_ptr, float(factor))
+        if self.backend.ctx.world_size > 1:
+            self.backend.barrier()             # every table is in place before the chief can store a cut
+
+    def lr_cut_table(self):
+        """This replica's cut table as the device holds it: ``lr_plateau.MAX_CUTS`` steps, ``lr_plateau.NO_CUT`` where no
+        cut is stored (synchronises the device)."""
+        torch.cuda.synchronize()
+        return [int(x) for x in self._lr_table.view(torch.int32, 0, lr_plateau.MAX_CUTS).cpu().numpy().view(np.uint32)]
+
+    def arm_lr_plateau(self, patience: int, min_delta_rows: int, margin: int, restored: int = 0) -> None:
+        """Chief, after :meth:`arm_eval` and :meth:`arm_lr_cuts`: once ``patience`` counting passes in a row, the last of
+        global step g, have not beaten the best count by more than ``min_delta_rows``, cut the rate from S = g +
+        ``margin`` on every replica.  ``restored``: the cuts already in the tables (a restarted run's).  Re-captures the
+        evaluation graph."""
+        if self._lr_table is None or getattr(self, "_ev_x", None) is None:
+            raise RuntimeError("arm_lr_plateau: arm_eval() and arm_lr_cuts() first")
+        n = int(self._ev_x.shape[0])
+        if int(patience) < 1 or not 0 <= int(min_delta_rows) < n or int(margin) < 1 or \
+                not 0 <= int(restored) <= lr_plateau.MAX_CUTS:
+            raise ValueError("arm_lr_plateau: patience %d, min_delta %d of %d rows, margin %d, %d restored cuts"
+                             % (patience, min_delta_rows, n, margin, restored))
+        self._leave_native_runner()
+        words = torch.zeros(int(self.lib.dm_plateau_state_bytes()) // 4, dtype=torch.int32)
+        words[PL_CUTS_WORD] = int(restored)
+        self._plateau = (words.to(self.device), int(patience), int(min_delta_rows), int(margin))
+        self._capture_eval()
+
+    def lr_plateau_state(self) -> Optional[lr_plateau.State]:
+        """The PlateauState as the passes so far left it, or None when no plateau is armed (synchronises the device)."""
+        if self._plateau is None:
+            return None
+        torch.cuda.synchronize()
+        u = self._plateau[0].cpu().numpy().view(np.uint32)
+        return lr_plateau.State(int(u[PL_BEST_WORD]), int(u[PL_SINCE_WORD]), bool(u[PL_BASELINE_WORD]),
+                                int(u[PL_CUTS_WORD]), int(u[PL_TRIGGER_WORD]))
 
 
 # dm_dense10_xent (csrc/mlp_simt.cu) stages the output-layer weights as [H][11] floats and refuses more than 220 KiB

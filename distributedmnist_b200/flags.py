@@ -284,6 +284,16 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_float("early_stopping_min_delta", 0.0, "With --early_stopping_patience: the accuracy an evaluation must beat "
                                                     "the best by to reset the patience, rounded down to whole validation "
                                                     "rows; 0 <= D < 1")
+    F.DEFINE_integer("lr_plateau_patience", 0, "With --eval_every_steps: multiply the learning rate by "
+                                               "--lr_plateau_factor once this many in-training evaluations in a row "
+                                               "have not beaten the best so far (by more than --lr_plateau_min_delta), "
+                                               "from the scored step + 2; at most 32 cuts; report in "
+                                               "worker0_lr_plateau.json; 0 = off, else P >= 1")
+    F.DEFINE_float("lr_plateau_factor", 0.1, "With --lr_plateau_patience: the factor each cut multiplies the learning "
+                                             "rate by; 0 < F < 1")
+    F.DEFINE_float("lr_plateau_min_delta", 0.0, "With --lr_plateau_patience: the accuracy an evaluation must beat the "
+                                                "best by to reset the patience, rounded down to whole validation rows; "
+                                                "0 <= D < 1")
     return F
 
 

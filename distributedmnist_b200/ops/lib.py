@@ -70,6 +70,9 @@ def _signatures() -> dict:
         # eval_patience.cu
         "dm_patience_state_bytes": (V, i, []),
         "dm_eval_patience": (S, i, [P, P, P, u, u, u, u, P, PP, i, i, P]),
+        # eval_plateau.cu
+        "dm_plateau_state_bytes": (V, i, []),
+        "dm_eval_plateau": (S, i, [P, P, P, u, u, u, u, P, PP, i, P]),
         # eval_snapshot.cu
         "dm_snap_state_bytes": (V, i, []),
         "dm_snap_select": (S, i, [P, P, i, i, d, P]),
@@ -95,6 +98,7 @@ def _signatures() -> dict:
         "dm_fused_sync_sgd": (S, i, [PP, PP, PP, i, i, i, ll, d, d, i, f, u, d, P, i, P, P, P]),
         "dm_fused_sync_bucket": (S, i, [PP, PP, PP, i, i, i, ll, ll, ll, ll, d, d, i, d, P, i, P, P, P]),
         "dm_sync_set_host_mirror": (S, i, [P, P]),
+        "dm_sync_set_lr_cuts": (S, i, [P, P, d]),
         "dm_f32_to_bf16": (S, i, [P, P, ll, P]),
         "dm_straggler_delay": (S, i, [P, f, u, u, P]),
         "dm_straggler_state_bytes": (V, i, []),

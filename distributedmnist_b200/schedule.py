@@ -27,14 +27,21 @@ def exponential_decay(initial_learning_rate: float, global_step: int, decay_step
 
 
 class LearningRateSchedule:
-    """Callable ``step -> lr`` built from the reference's flags."""
+    """Callable ``step -> lr`` built from the reference's flags.
+
+    ``cuts`` (``--lr_plateau_patience``, lr_plateau.py): the global steps S_k from which a cut of the rate by ``factor``
+    takes effect.  With c(s) of them <= s the rate is ``lr0 * decay^p * factor^c(s)``, the product in that order in double
+    (``cta_scale`` in csrc/fused_sync.cuh computes the same); with no cut in effect it is the staircase decay alone.  The
+    training loop appends to ``cuts`` as the cuts are decided."""
 
     def __init__(self, initial_learning_rate: float, decay_steps: int, decay_rate: float,
-                 staircase: bool = True):
+                 staircase: bool = True, factor: float = 1.0, cuts=()):
         self.initial_learning_rate = float(initial_learning_rate)
         self.decay_steps = int(decay_steps)
         self.decay_rate = float(decay_rate)
         self.staircase = staircase
+        self.factor = float(factor)
+        self.cuts = [int(s) for s in cuts]
 
     @classmethod
     def from_flags(cls, flags, num_examples: int, num_replicas_to_aggregate: int) -> "LearningRateSchedule":
@@ -44,5 +51,7 @@ class LearningRateSchedule:
                    flags.learning_rate_decay_factor)
 
     def __call__(self, global_step: int) -> float:
-        return exponential_decay(self.initial_learning_rate, int(global_step), self.decay_steps,
-                                 self.decay_rate, self.staircase)
+        lr = exponential_decay(self.initial_learning_rate, int(global_step), self.decay_steps,
+                               self.decay_rate, self.staircase)
+        c = sum(1 for s in self.cuts if s <= int(global_step))
+        return lr * self.factor ** c if c else lr

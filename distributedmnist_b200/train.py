@@ -31,11 +31,12 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
-from . import best, early_stopping, moving_average
+from . import best, early_stopping, lr_plateau, moving_average
 from .best import BEST_DIR, BEST_JSON
 from .checkpoint import Saver
 from .early_stopping import EARLY_STOPPING_JSON
 from .engine import make_engine
+from .lr_plateau import LR_PLATEAU_JSON
 from .flags import FLAGS
 from .parallel.aggregators import (SyncReplicasOptimizer, TimeoutReplicasOptimizer,
                                    parse_straggler_spec)
@@ -352,6 +353,62 @@ def check_early_stopping_flags(flags, ctx: ReplicaContext) -> None:
                          % (flags.backend, "" if ctx.on_gpu else ", no GPU", ctx.world_size))
 
 
+def check_lr_plateau_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate: int) -> None:
+    """``--lr_plateau_patience`` / ``--lr_plateau_factor`` / ``--lr_plateau_min_delta`` combinations that cannot work,
+    rejected before any device work starts.  Where the in-training evaluation itself is refused (check_eval_flags), so
+    are learning-rate cuts."""
+    p = int(getattr(flags, "lr_plateau_patience", 0) or 0)
+    f = float(getattr(flags, "lr_plateau_factor", 0.1))
+    d = float(getattr(flags, "lr_plateau_min_delta", 0.0) or 0.0)
+    if p < 0:
+        raise ValueError("--lr_plateau_patience must be >= 1 (0 = off), got %d" % p)
+    if not 0.0 < f < 1.0:
+        raise ValueError("--lr_plateau_factor must lie in (0, 1), got %r" % f)
+    if not 0.0 <= d < 1.0:
+        raise ValueError("--lr_plateau_min_delta must lie in [0, 1), got %r" % d)
+    if p == 0:
+        if d != 0.0 or f != 0.1:
+            raise ValueError("--lr_plateau_factor and --lr_plateau_min_delta need --lr_plateau_patience >= 1: without a "
+                             "patience there is nothing for them to change")
+        return
+    if getattr(flags, "eval_every_steps", 0) <= 0:
+        raise ValueError("--lr_plateau_patience needs --eval_every_steps > 0: the patience counts in-training evaluations")
+    if not (ctx.on_gpu and flags.backend in ("auto", "fused")):
+        if ctx.world_size > 1:
+            raise ValueError("--lr_plateau_patience with the torch engine (--backend=%s%s) is implemented for one replica, "
+                             "not %d: only the chief evaluates and nothing tells the other replicas to cut their rate"
+                             % (flags.backend, "" if ctx.on_gpu else ", no GPU", ctx.world_size))
+        return
+    # every replica must apply a cut from the same global step S: the chief's table stores reach a peer before it finishes
+    # the chief's next step only when every step waits for all N replicas (DESIGN §4, learning-rate cuts)
+    why = ": its replicas are not in lock step, so no global step can be named from which every replica applies a cut " \
+          "(supported: K = N, or --worker_times_cdf_method without --interval_method)"
+    if flags.interval_method:
+        raise ValueError("--lr_plateau_patience cannot be combined with --interval_method" + why)
+    if not getattr(flags, "worker_times_cdf_method", False) and num_replicas_to_aggregate != ctx.world_size:
+        raise ValueError("--lr_plateau_patience needs --num_replicas_to_aggregate = number of replicas (%d), got %d (K %s N)"
+                         % (ctx.world_size, num_replicas_to_aggregate,
+                            "<" if num_replicas_to_aggregate < ctx.world_size else ">") + why)
+
+
+def restart_lr_cuts(train_dir: str, rank: int, restored_step: int, factor: float):
+    """The cuts an earlier run's ``worker<rank>_lr_plateau.json`` lists that a run restarted from the checkpoint of
+    ``restored_step`` keeps -- those with ``from_step <= restored_step`` -- as ``(kept, None)``, or ``([], reason)`` when
+    the restart must be refused: cuts are kept but the file's factor differs from ``factor``."""
+    try:
+        with open(os.path.join(train_dir, LR_PLATEAU_JSON % rank)) as f:
+            earlier = json.load(f)
+    except FileNotFoundError:
+        return [], None
+    kept = [dict(trigger_step=int(c["trigger_step"]), from_step=int(c["from_step"])) for c in earlier["cuts"]
+            if int(c["from_step"]) <= restored_step]
+    if kept and float(earlier["factor"]) != factor:
+        return [], ("--lr_plateau_factor=%r differs from the factor %r of the %d learning-rate cut(s) the restored "
+                    "checkpoint of global step #%d was trained with (%s)"
+                    % (factor, float(earlier["factor"]), len(kept), restored_step, LR_PLATEAU_JSON % rank))
+    return kept, None
+
+
 def check_best_flags(flags) -> None:
     """``--keep_best_checkpoint`` combinations that cannot work, rejected before any device work starts.  Where the
     in-training evaluation itself is refused (check_eval_flags), so is keeping its best weights."""
@@ -491,6 +548,57 @@ class _EarlyStopping:
                     counted_passes=self.counted, weights=self.weights)
 
 
+class _LrPlateau:
+    """``--lr_plateau_patience`` on the chief: :func:`lr_plateau.advance` over the evaluation passes, in order.  On the
+    sm_90a path eval_plateau has made the same decisions on the device and stored the cuts into every replica's table;
+    this replays them from the pass records for the log, the summary rate (``schedule``), the file and restarts.  With the
+    torch engine this is where the cuts are decided.  The file is rewritten as soon as a cut is known, before any
+    checkpoint of its ``from_step`` or later can be written."""
+
+    def __init__(self, patience: int, factor: float, min_delta: float, examples: int, weights: str, schedule,
+                 path: str, kept):
+        self.patience, self.factor, self.min_delta, self.examples, self.weights = patience, factor, min_delta, examples, weights
+        self.delta_rows = early_stopping.min_delta_rows(min_delta, examples)
+        self.schedule, self.path = schedule, path
+        self.cuts = list(kept)       # [{trigger_step, from_step}], the restored ones first
+        self.state = lr_plateau.State(cuts=len(self.cuts))
+        self.capped = False
+
+    def add(self, step: int, examples: int, correct: int, status: Optional[int] = None) -> None:
+        """One completed pass (``status`` as best.counts takes it)."""
+        cuts = self.state.cuts
+        self.state, fired = lr_plateau.advance(self.state, step, correct, examples, self.examples, self.patience,
+                                               self.delta_rows, status)
+        if not fired:
+            return
+        if self.state.cuts == cuts:
+            if not self.capped:
+                log.warning("Learning rate plateau: the evaluation of global step #%d exhausted the patience again, but "
+                            "%d cuts have been made, the most a run makes; this and every later trigger are ignored"
+                            % (step, lr_plateau.MAX_CUTS))
+                self.capped = True
+            return
+        s = step + STOP_MARGIN
+        self.cuts.append(dict(trigger_step=step, from_step=s))
+        self.schedule.cuts.append(s)
+        self.write()
+        log.info("Learning rate plateau: cut %d after the evaluation of global step #%d (%d of %d correct, best %d, "
+                 "patience %d, min_delta %d rows); from global step #%d the learning rate is %g"
+                 % (len(self.cuts), step, correct, examples, self.state.best, self.patience, self.delta_rows, s,
+                    self.schedule(s)))
+
+    def report(self) -> Dict:
+        return dict(patience=self.patience, factor=self.factor, min_delta=self.min_delta, min_delta_rows=self.delta_rows,
+                    examples=self.examples, weights=self.weights, cuts=list(self.cuts))
+
+    def write(self) -> None:
+        tmp = self.path + ".tmp"
+        with open(tmp, "w") as f:
+            json.dump(self.report(), f, indent=1)
+            f.write("\n")
+        os.replace(tmp, self.path)
+
+
 def eval_due(global_step: int, last_mark: int, every: int) -> bool:
     """Snapshot passes (K < N, interval): the host learns the global step only after a step completes, and it may jump by
     more than one.  A pass is due once the newest consumed global step has crossed a multiple of ``every`` since
@@ -510,6 +618,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
     check_target_flags(flags, ctx)
     check_early_stopping_flags(flags, ctx)
+    check_lr_plateau_flags(flags, ctx, num_replicas_to_aggregate)
     check_best_flags(flags)
     check_moving_average_flags(flags, ctx, num_replicas_to_aggregate)
     check_device_data_flags(flags, ctx, dataset)
@@ -517,6 +626,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     target = float(getattr(flags, "target_accuracy", 0.0) or 0.0)
     patience = int(getattr(flags, "early_stopping_patience", 0) or 0)
     stop_armed = bool(target or patience)      # something may set a stop step S before --max_steps
+    plateau = int(getattr(flags, "lr_plateau_patience", 0) or 0)
     ema_decay = float(getattr(flags, "moving_average_decay", 0.0) or 0.0) if is_chief else 0.0
     eval_average = bool(ema_decay and getattr(flags, "eval_moving_average", False))
 
@@ -624,6 +734,32 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                             dataset_test.num_examples, eval_weights)
         if device_eval:
             engine.arm_patience(patience, es.delta_rows, STOP_MARGIN)
+    # --lr_plateau_patience: from S = g + STOP_MARGIN on, for the pass of global step g that exhausts the patience, every
+    # update is made at the rate times --lr_plateau_factor once more (GPU path: eval_plateau stores S into every replica's
+    # cut table, which the aggregation kernels read; torch engine: decided on the host after `evaluate`, into the shared
+    # schedule).  A restarted run keeps the cuts of the restored checkpoint's past, from its file.
+    lp = None
+    if plateau:
+        factor = float(flags.lr_plateau_factor)
+        kept, refusal = restart_lr_cuts(flags.train_dir, ctx.rank, restored_step, factor) if is_chief else ([], None)
+        if num_workers > 1:
+            kept, refusal = backend.all_gather_object((kept, refusal))[0]
+        if refusal:
+            raise ValueError(refusal)
+        lr_schedule.factor = factor
+        lr_schedule.cuts = [c["from_step"] for c in kept]
+        if fused_step:
+            engine.arm_lr_cuts(factor, lr_schedule.cuts)          # every replica (a symmetric allocation)
+        if is_chief:
+            lp = _LrPlateau(plateau, factor, float(getattr(flags, "lr_plateau_min_delta", 0.0) or 0.0),
+                            dataset_test.num_examples, eval_weights, lr_schedule,
+                            os.path.join(flags.train_dir, LR_PLATEAU_JSON % ctx.rank), kept)
+            lp.write()
+            if kept:
+                log.info("Learning rate plateau: %d cut(s) up to the restored global step #%d kept; from there the "
+                         "learning rate is %g" % (len(kept), restored_step, lr_schedule(restored_step)))
+            if device_eval:
+                engine.arm_lr_plateau(plateau, lp.delta_rows, STOP_MARGIN, len(kept))
     # --keep_best_checkpoint: the chief keeps the weights of its best-scoring evaluation (GPU path: decided and copied on the
     # device inside the pass's graph; torch engine: after `evaluate`) and writes them once, after the final pass.  A best
     # file of an earlier run sets the count to beat.
@@ -726,7 +862,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     def collect_evals() -> None:
         """Device records completed so far (%globaltimer ns -> seconds, as push_device_times converts them)."""
         nonlocal test_acc_value
-        if tta is None and es is None:
+        if tta is None and es is None and lp is None:
             recs = [(r, 0) for r in engine.eval_records()]
         else:                      # dropped snapshot passes took training-stream time too, and count for neither rule
             recs = engine.eval_records_with_status()
@@ -736,6 +872,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 tta.add(gs, t0, t1, n_ex, correct, status >= 0, time.time() - tta_wall0)
             if es is not None:
                 es.add(gs, n_ex, correct, status if snapshot_eval else None)
+            if lp is not None:
+                lp.add(gs, n_ex, correct, status if snapshot_eval else None)
             if status < 0:
                 continue
             eval_rows.append((gs, t0 * 1e-9, (t1 - t0) * 1e-9, n_ex, correct, loss_sum / max(n_ex, 1)))
@@ -780,6 +918,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             max_steps = min(max_steps, global_step + STOP_MARGIN)
         if es is not None and es.add(global_step, n_ex, correct):
             max_steps = min(max_steps, global_step + STOP_MARGIN)
+        if lp is not None:
+            lp.add(global_step, n_ex, correct)
 
     def save_evals() -> None:
         np.save(os.path.join(flags.train_dir, "worker%d_eval.npy" % ctx.rank),
@@ -956,6 +1096,13 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         else:
             log.info("Early stopping: patience %d not exhausted after %d counted evaluation(s)"
                      % (patience, rep["counted_passes"]))
+    if lp is not None:
+        results["lr_plateau"] = lp.report()
+        lp.write()
+        device_state = engine.lr_plateau_state() if device_eval else None
+        if device_state is not None and device_state != lp.state:
+            log.warning("Learning rate plateau: the device state %s differs from the replay of the evaluation records %s"
+                        % (device_state, lp.state))
     if keep_best:
         rep = results["best"] = save_best(engine, spec, flags.train_dir, ctx.rank, eval_weights)
         if rep is not None:
