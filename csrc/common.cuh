@@ -61,6 +61,14 @@ DMNIST_DEVICE void red_add_f32x4(float* addr, float a, float b, float c, float d
   asm volatile("red.global.add.v4.f32 [%0], {%1, %2, %3, %4};" ::"l"(addr), "f"(a), "f"(b), "f"(c), "f"(d) : "memory");
 }
 
+// a * b + c with one rounding, subnormals kept: written in PTX because --use_fast_math turns fmaf into fma.rn.ftz, and
+// the L2 decay epilogues must equal an exact single-rounding emulation
+DMNIST_DEVICE float fma_rn(float a, float b, float c) {
+  float d;
+  asm("fma.rn.f32 %0, %1, %2, %3;" : "=f"(d) : "f"(a), "f"(b), "f"(c));
+  return d;
+}
+
 DMNIST_DEVICE uint64_t globaltimer_ns() {
   uint64_t t;
   asm volatile("mov.u64 %0, %%globaltimer;" : "=l"(t));

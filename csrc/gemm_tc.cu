@@ -30,7 +30,11 @@ enum GemmEpilogue : int { EPI_STORE_F32 = 0, EPI_ATOMIC_F32 = 1, EPI_STORE_BF16 
                           // tile is one pooled position x 64 channels; the epilogue scatters each value to the argmax
                           // pixel of its 2x2 window (dense bf16 [B,14,14,64], zeros elsewhere) and reduces the conv2
                           // bias gradient -- the separate unpool kernel and the [B,3136] intermediate disappear.
-                          EPI_UNPOOL2_BF16 = 4 };
+                          EPI_UNPOOL2_BF16 = 4,
+                          // fc weight gradient with L2 decay (--weight_decay): each element is fma(decay, W, acc) with one
+                          // rounding (then rounded to bf16 for the wire variant), W the fp32 weights in the output's layout;
+                          // each CTA also stores the sum of its tile's W^2, in double and a fixed order, into decay_part
+                          EPI_STORE_F32_DECAY = 5, EPI_STORE_BF16_DECAY = 6 };
 
 struct GemmParams {
   int M, N;        // logical output extent (predication)
@@ -41,6 +45,9 @@ struct GemmParams {
   const float* bias;        // EPI_BIAS_RELU_BF16: per-column bias (reference K2/K3 fused into the producer)
   const uint8_t* code;      // EPI_UNPOOL2_BF16: pooling codes [M][N] (bits 0-1 argmax position, bit 2 ReLU active)
   float* g_bias;            // EPI_UNPOOL2_BF16: conv2 bias gradient [64], the CTAs' sum is added to it (pre-zeroed)
+  const float* decay_w;     // EPI_*_DECAY: fp32 weights [M][ldo]
+  double* decay_part;       // EPI_*_DECAY: one W^2 partial per CTA, at blockIdx.y * gridDim.x + blockIdx.x
+  float decay;              // EPI_*_DECAY: lambda
 };
 
 template <int BN>
@@ -183,6 +190,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   named_bar_sync(1, GEMM_CONSUMERS);
 
   // ------------------------------ epilogue: thread = tile row, 32-column chunks ------------------------------
+  constexpr bool DECAY = EPI == EPI_STORE_F32_DECAY || EPI == EPI_STORE_BF16_DECAY;
+  double wsq = 0.0;                                  // DECAY: sum of this thread's W^2, chunk by chunk, column by column
   {
     const int lr = threadIdx.x & 127;                // tile row
     const int half = threadIdx.x >> 7;               // chunks half, half + 2, ...
@@ -209,8 +218,28 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         }
       }
       const int col0 = n0 + c * 32;
+      if (DECAY && row < p.M) {
+        // the W tile is read once: for the lambda * W term and for the W^2 partial
+        const float* wp = p.decay_w + (size_t)row * p.ldo + col0;
+        float w[32];
+        if (col0 + 32 <= p.N && (p.ldo & 3) == 0) {
+#pragma unroll
+          for (int j = 0; j < 32; j += 4) {
+            const float4 t = __ldg(reinterpret_cast<const float4*>(wp + j));
+            w[j] = t.x; w[j + 1] = t.y; w[j + 2] = t.z; w[j + 3] = t.w;
+          }
+        } else {
+#pragma unroll
+          for (int j = 0; j < 32; ++j) w[j] = col0 + j < p.N ? __ldg(wp + j) : 0.f;
+        }
+#pragma unroll
+        for (int j = 0; j < 32; ++j) {
+          v[j] = __float_as_uint(fma_rn(p.decay, w[j], __uint_as_float(v[j])));
+          wsq += (double)w[j] * (double)w[j];        // the product of two floats is exact in double
+        }
+      }
       if (row < p.M) {
-        if (EPI == EPI_STORE_F32) {
+        if (EPI == EPI_STORE_F32 || EPI == EPI_STORE_F32_DECAY) {
           float* o = reinterpret_cast<float*>(p.out) + (size_t)blockIdx.z * p.split_stride + (size_t)row * p.ldo + col0;
           if (col0 + 32 <= p.N && (p.ldo & 3) == 0) {
 #pragma unroll
@@ -328,6 +357,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       o[0] += sum.x; o[1] += sum.y; o[2] += sum.z; o[3] += sum.w;
     }
   }
+  if (DECAY) {
+    // the CTA's W^2 partial: a fixed butterfly per warp, then the eight warps in order
+    double* s_wsq = reinterpret_cast<double*>(smem + S::BPART_OFFSET);
+#pragma unroll
+    for (int o = 16; o > 0; o >>= 1) wsq += __shfl_xor_sync(0xffffffffu, wsq, o);
+    if (lane == 0) s_wsq[warp] = wsq;
+    named_bar_sync(1, GEMM_CONSUMERS);
+    if (threadIdx.x == 0) {
+      double s = 0.0;
+#pragma unroll
+      for (int w = 0; w < GEMM_CONSUMERS / 32; ++w) s += s_wsq[w];
+      p.decay_part[blockIdx.y * gridDim.x + blockIdx.x] = s;
+    }
+  }
 
 }
 
@@ -406,6 +449,31 @@ extern "C" int dm_gemm_bf16(const void* A, const void* B, void* out, int M, int 
     return -1;
   }
 #undef DM_DISPATCH
+}
+
+// fc weight gradient with L2 decay:  D[M,N] = A^T B + decay * W,  A [K rows][M cols] and B [K rows][N cols] bf16 (both
+// MN-major, K = batch), 128 x 128 tiles, no split-K.  W: fp32 [M][ldo], the layout of the output.  bf16_out: store bf16
+// (the bucketed aggregation's wire buffer) instead of fp32.  decay_part receives dm_gemm_decay_ctas(M, N) doubles, the
+// W^2 sum of each CTA's tile.
+extern "C" int dm_gemm_decay_ctas(int M, int N) {
+  return ((M + dm::GEMM_BM - 1) / dm::GEMM_BM) * ((N + 127) / 128);
+}
+
+extern "C" int dm_gemm_bf16_decay(const void* A, const void* B, void* out, int M, int N, int K, int lda, int ldb, int ldo,
+                                  int bf16_out, const void* w, float decay, void* decay_part, void* stream_) {
+  using namespace dm;
+  if (w == nullptr || decay_part == nullptr || M < 1 || N < 1 || K < 1) return -1;
+  if ((lda & 7) || (ldb & 7)) return -3;
+  CUtensorMap tmA, tmB;
+  int rc = make_tmap_2d_bf16(&tmA, A, (uint64_t)M, (uint64_t)K, (uint64_t)lda, 64, 64, 128);
+  if (rc) return 100 + rc;
+  rc = make_tmap_2d_bf16(&tmB, B, (uint64_t)N, (uint64_t)K, (uint64_t)ldb, 64, 64, 128);
+  if (rc) return 200 + rc;
+  GemmParams p{M, N, (K + GEMM_BK - 1) / GEMM_BK, ldo, out, 0, nullptr, nullptr, nullptr,
+               reinterpret_cast<const float*>(w), reinterpret_cast<double*>(decay_part), decay};
+  cudaStream_t stream = reinterpret_cast<cudaStream_t>(stream_);
+  if (bf16_out) return launch_gemm<128, true, true, EPI_STORE_BF16_DECAY>(tmA, tmB, p, 1, stream);
+  return launch_gemm<128, true, true, EPI_STORE_F32_DECAY>(tmA, tmB, p, 1, stream);
 }
 
 // fc1 dgrad fused with the maxpool2/ReLU2 backward and the conv2 bias gradient:

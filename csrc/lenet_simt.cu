@@ -171,13 +171,23 @@ __global__ void __launch_bounds__(F2_THREADS) fc2_fwd_bwd_kernel(Fc2Args a) {
 //   output o < 80       : g_w2[j0 + o / 10][o % 10] = sum_r h[r][j] * dl[r][c]
 //   output 80 .. 87     : g_b1[j0 + o - 80]         = sum_r dh[r][j]
 //   output 88 .. 97     : g_b2[o - 88]              = sum_r dl[r][c]        (CTA 0 only)
+// DECAY (--weight_decay): each output is fma(decay, v, sum) with one rounding, v = w2 / b1 / b2, and each CTA stores the
+// sum of the squares of the variables it owns, in double and a fixed order, into decay_part[blockIdx.x].
 constexpr int FW_J = 8;
 constexpr int FW_ROWS = 256;
+struct Fc2Decay {
+  const float* w2;           // [512][10]
+  const float* b2;           // [10]
+  const float* b1;           // [512]
+  float decay;
+  double* part;              // [512 / FW_J]
+};
+template <bool DECAY>
 __global__ void __launch_bounds__(256) fc2_wgrad_kernel(const float* __restrict__ h,            // [B,512]
                                                         const float* __restrict__ dl,           // [B,12]
                                                         const __nv_bfloat16* __restrict__ dh,   // [B,512]
                                                         float* __restrict__ g_w2, float* __restrict__ g_b2,
-                                                        float* __restrict__ g_b1, int B) {
+                                                        float* __restrict__ g_b1, int B, Fc2Decay dk) {
   __shared__ __align__(16) float s_h[FW_ROWS][FW_J];
   __shared__ __align__(16) float s_dh[FW_ROWS][FW_J];
   __shared__ __align__(16) float s_dl[FW_ROWS][DL_LD];
@@ -226,10 +236,50 @@ __global__ void __launch_bounds__(256) fc2_wgrad_kernel(const float* __restrict_
   __syncthreads();
   if (half == 0) {
     acc += s_red[o];
+    if (DECAY) {
+      float v = 0.f;                               // outputs this CTA does not store decay nothing
+      if (kind == 0) v = dk.w2[(j0 + oj) * NCLS + oc];
+      else if (kind == 1) v = dk.b1[j0 + oj];
+      else if (kind == 2 && blockIdx.x == 0) v = dk.b2[oc];
+      acc = fma_rn(dk.decay, v, acc);
+      s_red[o] = v;                                // (every thread has read s_red above; this is its own slot)
+    }
     if (kind == 0) g_w2[(size_t)(j0 + oj) * NCLS + oc] = acc;
     else if (kind == 1) g_b1[j0 + oj] = acc;
     else if (kind == 2 && blockIdx.x == 0) g_b2[oc] = acc;
   }
+  if (DECAY) {
+    __syncthreads();
+    if (t < 32) {
+      // lane l: outputs l, l + 32, l + 64, l + 96 in order, then a fixed butterfly
+      double s = 0.0;
+#pragma unroll
+      for (int i = 0; i < 4; ++i) {
+        const double v = s_red[t + 32 * i];
+        s += v * v;                                // the square of a float is exact in double
+      }
+#pragma unroll
+      for (int off = 16; off > 0; off >>= 1) s += __shfl_xor_sync(0xffffffffu, s, off);
+      if (t == 0) dk.part[blockIdx.x] = s;
+    }
+  }
+}
+
+template <bool DECAY>
+int launch_fc2_wgrad(const void* scratch_h, const void* scratch_dl, const void* dh, void* g_w2, void* g_b2, void* g_b1,
+                            int B, Fc2Decay dk, void* stream) {
+  // side-branch kernel: it has to share SMs with the tensor-core kernels (max-shared L1 split), see dm_fused_sync_bucket
+  static bool configured = false;
+  if (!configured) {
+    DM_CUDA_OK(cudaFuncSetAttribute(fc2_wgrad_kernel<DECAY>, cudaFuncAttributePreferredSharedMemoryCarveout,
+                                    cudaSharedmemCarveoutMaxShared));
+    configured = true;
+  }
+  return (int)launch_kernel(fc2_wgrad_kernel<DECAY>, dim3(HID / FW_J), dim3(256), 0,
+                                reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const float*>(scratch_h),
+                                reinterpret_cast<const float*>(scratch_dl), reinterpret_cast<const __nv_bfloat16*>(dh),
+                                reinterpret_cast<float*>(g_w2), reinterpret_cast<float*>(g_b2),
+                                reinterpret_cast<float*>(g_b1), B, dk);
 }
 
 }  // namespace dm
@@ -271,17 +321,19 @@ int dm_fc2_fwd_bwd(const void* h_part, long long part_stride, int splits, const 
 // Side-branch half: g_w2 [512][10], g_b2 [10], g_b1 [512] (plain stores).
 int dm_fc2_wgrad(const void* scratch_h, const void* scratch_dl, const void* dh, void* g_w2, void* g_b2, void* g_b1, int B,
                  void* stream) {
-  // side-branch kernel: it has to share SMs with the tensor-core kernels (max-shared L1 split), see dm_fused_sync_bucket
-  static bool configured = false;
-  if (!configured) {
-    DM_CUDA_OK(cudaFuncSetAttribute(dm::fc2_wgrad_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    configured = true;
-  }
-  return (int)dm::launch_kernel(dm::fc2_wgrad_kernel, dim3(dm::HID / dm::FW_J), dim3(256), 0,
-                                reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const float*>(scratch_h),
-                                reinterpret_cast<const float*>(scratch_dl), reinterpret_cast<const __nv_bfloat16*>(dh),
-                                reinterpret_cast<float*>(g_w2), reinterpret_cast<float*>(g_b2),
-                                reinterpret_cast<float*>(g_b1), B);
+  return dm::launch_fc2_wgrad<false>(scratch_h, scratch_dl, dh, g_w2, g_b2, g_b1, B, dm::Fc2Decay{}, stream);
+}
+
+// The same with L2 decay: g_w2 / g_b2 / g_b1 gain decay * w2 / b2 / b1 (one rounding each); decay_part receives
+// dm_fc2_wgrad_decay_ctas() doubles, the squares of the variables each CTA owns, summed.
+int dm_fc2_wgrad_decay_ctas() { return dm::HID / dm::FW_J; }
+
+int dm_fc2_wgrad_decay(const void* scratch_h, const void* scratch_dl, const void* dh, void* g_w2, void* g_b2, void* g_b1,
+                       int B, const void* w2, const void* b2, const void* b1, float decay, void* decay_part, void* stream) {
+  if (w2 == nullptr || b2 == nullptr || b1 == nullptr || decay_part == nullptr) return -1;
+  const dm::Fc2Decay dk{reinterpret_cast<const float*>(w2), reinterpret_cast<const float*>(b2),
+                        reinterpret_cast<const float*>(b1), decay, reinterpret_cast<double*>(decay_part)};
+  return dm::launch_fc2_wgrad<true>(scratch_h, scratch_dl, dh, g_w2, g_b2, g_b1, B, dk, stream);
 }
 
 }  // extern "C"

@@ -26,6 +26,7 @@ import torch
 
 from . import best
 from . import moving_average as ema
+from . import weight_decay
 from .models import ModelSpec, dropout_keep_mask, dropout_seed_mix, get_model, loss_and_accuracy
 from .models.lenet import FC1_OUT
 
@@ -107,10 +108,22 @@ class TorchEngine(ComputeEngine):
                 return self._fwd(views, images, train=train, keep_mask=mask, keep_prob=self.keep_prob).float()
         return self._fwd(views, images, train=train, keep_mask=mask, keep_prob=self.keep_prob)
 
+    # ---- L2 weight decay (see weight_decay.py) ----------------------------------------------------------------------------
+    _decay = 0.0
+
+    def arm_weight_decay(self, lam: float) -> None:
+        """From the next step on, differentiate CE + ``lam`` * R (R = sum of v^2 / 2 over the decayed variables); the loss
+        :meth:`loss_acc` reports includes the term."""
+        self._decay = float(lam)
+
     def forward_backward(self, step: int) -> None:
         p = self.params.detach().requires_grad_(True)
         logits = self._logits(p, self._images, True, step)
         loss, acc = loss_and_accuracy(logits, self._labels)
+        if self._decay:
+            views = self.spec.views(p)
+            reg = sum((views[q.name] * views[q.name]).sum() for q in weight_decay.decayed(self.spec)) * 0.5
+            loss = loss + self._decay * reg
         (g,) = torch.autograd.grad(loss, p)
         self.grads.copy_(g)
         self._loss, self._acc = loss.detach(), acc.detach()

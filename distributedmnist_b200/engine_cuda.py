@@ -32,7 +32,7 @@ from typing import Optional, Tuple
 import numpy as np
 import torch
 
-from . import early_stopping, lr_plateau
+from . import early_stopping, lr_plateau, weight_decay
 from .best import BEST_CORRECT_WORD, BEST_EXAMPLES_WORD, BEST_STEP_WORD, BEST_VALID_WORD
 from .early_stopping import PAT_BASELINE_WORD, PAT_BEST_STEP_WORD, PAT_BEST_WORD, PAT_SINCE_WORD, PAT_TRIGGER_WORD
 from .lr_plateau import PL_BASELINE_WORD, PL_BEST_WORD, PL_CUTS_WORD, PL_SINCE_WORD, PL_TRIGGER_WORD
@@ -405,6 +405,11 @@ class _CudaEngine(ComputeEngine):
         self._steps_launched = 0
         self.lib.dm_set_max_ctas(int(os.environ.get("DMNIST_MAX_CTAS", "0")))
 
+    def arm_weight_decay(self, lam: float) -> None:
+        """L2 weight decay (see weight_decay.py): implemented for lenet only (:class:`CudaLeNetEngine`)."""
+        if float(lam) != 0.0:
+            raise ValueError("--weight_decay on the GPU path is implemented for lenet, not --model=%s" % self.spec.name)
+
     def params_updated(self) -> None:
         """Parameters were written from the host (init / restore): refresh the bf16 shadow."""
         self.backend.refresh_shadow(self.params)
@@ -702,12 +707,53 @@ class CudaLeNetEngine(_CudaEngine):
     def _fc1_wgrad(self, dst: torch.Tensor, B: int) -> None:
         # dW1[3136,512] = a2^T (A MN-major) * dh (B MN-major), K = batch: fp32 into the gradient arena, or bf16 (half the
         # epilogue stores, half the NVLink bytes) into the bucketed aggregation's symmetric wire buffer
+        if self._decay:
+            # + lambda * W1 in the epilogue, from the fp32 weights the step's forward read (DESIGN §4, weight decay)
+            self.lib.dm_gemm_bf16_decay(self.a2, self.dh, dst, 3136, 512, B, 3136, 512, 512, int(dst.dtype == torch.bfloat16),
+                                        self.p["fc1_weights"], self._decay, self._decay_ws, stream_ptr())
+            return
         G.gemm_bf16_raw(self.a2, self.dh, dst, 3136, 512, B, 3136, 512, 512, True, True,
                         G.EPI_STORE_BF16 if dst.dtype == torch.bfloat16 else G.EPI_STORE_F32, bn=128)
 
     def _fc2_wgrad(self, B: int, sp) -> None:
         g = self.g
+        if self._decay:
+            p = self.p
+            self.lib.dm_fc2_wgrad_decay(self.h_act, self.dlogits, self.dh, g["fc2_weights"], g["fc2_biases"], g["fc1_biases"],
+                                        B, p["fc2_weights"], p["fc2_biases"], p["fc1_biases"], self._decay,
+                                        self._decay_ws_fc2, sp)
+            return
         self.lib.dm_fc2_wgrad(self.h_act, self.dlogits, self.dh, g["fc2_weights"], g["fc2_biases"], g["fc1_biases"], B, sp)
+
+    # ---- L2 weight decay (see weight_decay.py) ---------------------------------------------------------------------------
+    # The fc1 weight-gradient GEMM and fc2_wgrad add lambda * v to the four decayed variables' gradients in their epilogues
+    # and store the sums of v^2 they read, one double per CTA, into a workspace; weight_decay_loss adds those partials in a
+    # fixed order and (float)(lambda * R) to the step's loss word, on the loss read-back branch once both kernels are done.
+    _decay = 0.0                   # lambda; 0: off (the plain kernels, the step graph of an engine without the flag)
+
+    def arm_weight_decay(self, lam: float) -> None:
+        """Train on CE + ``lam`` * R from the next step on (0 <= lam < 1; 0 turns it off): allocates the workspace, selects
+        the decayed kernels and re-captures the step graphs.  The evaluation pass and :meth:`forward_logits` do not
+        change."""
+        lam = float(np.float32(lam))
+        if not 0.0 <= lam < 1.0:
+            raise ValueError("arm_weight_decay: lambda must lie in [0, 1), got %r" % lam)
+        assert {q.name for q in weight_decay.decayed(self.spec)} == {"fc1_weights", "fc1_biases", "fc2_weights",
+                                                                      "fc2_biases"}
+        self._leave_native_runner()
+        torch.cuda.synchronize()
+        if lam and getattr(self, "_decay_ws", None) is None:
+            n1 = int(self.lib.dm_gemm_decay_ctas(3136, 512))
+            self._decay_parts = n1 + int(self.lib.dm_fc2_wgrad_decay_ctas())
+            self._decay_ws = torch.zeros(self._decay_parts + 1, dtype=torch.float64, device=self.device)   # partials, R
+            self._decay_ws_fc2 = self._decay_ws[n1:]
+        self._decay = lam
+        self._graphs = [None, None]
+
+    def weight_decay_r(self) -> float:
+        """R of the step completed last, as the device summed it (synchronises the device)."""
+        torch.cuda.synchronize()
+        return float(self._decay_ws[self._decay_parts].item())
 
     def _fc1_dgrad(self, B: int, sp) -> None:
         # d(pool2 out)[B,3136] = dh[B,512] (K-major) * W1[3136,512] (rows = in, K = out contiguous), with maxpool2/ReLU2
@@ -748,17 +794,16 @@ class CudaLeNetEngine(_CudaEngine):
         # no extra call, only a wait on the step's completion event
         # (its own branch, joined only at the very end of the step: a memcpy node in front of the aggregation kernel
         # would cost that kernel its programmatic launch edge)
-        self._side[3].wait_event(fork1)
-        with torch.cuda.stream(self._side[3]):
-            self.h_loss_bufs[self._slot].copy_(self.d_loss_acc, non_blocking=True)
-            self._join_loss = torch.cuda.Event()
-            self._join_loss.record(self._side[3])
+        if not self._decay:
+            self._launch_loss_readback(fork1)
         sp = stream_ptr()
         self._fc1_dgrad(B, sp)
         # (the side branch is issued AFTER the chain's kernel: both become ready together and the first one dispatched takes
         #  the SMs -- the data-gradient GEMM must be that one)
         with torch.cuda.stream(self._side[0]):
             self._fc1_wgrad(self._g16_view if early_sync and self._bucket_v2 else self.g["fc1_weights"], B)
+            ev_w1 = torch.cuda.Event()
+            ev_w1.record(self._side[0])
             if not early_sync:
                 # fc2 weight/bias + fc1 bias gradients: only the aggregation kernel consumes them
                 self._fc2_wgrad(B, stream_ptr())
@@ -790,6 +835,9 @@ class CudaLeNetEngine(_CudaEngine):
                 self._fc2_wgrad(B, stream_ptr())
                 join3 = torch.cuda.Event()
                 join3.record(self._side[2])
+        if self._decay:
+            # the decay's loss term needs both weight-gradient kernels' partials (not the early bucket's exchange)
+            self._launch_loss_readback(fork1, ev_w1, join3 if early_sync else join1)
         # conv2 dgrad and wgrad each fill the machine (1 CTA/SM, ~200 KB smem): side by side they only slow the chain
         # down.  wgrad is forked AFTER dgrad instead and shares the SMs with conv1_wgrad.
         self._conv2_dgrad(B, sp)
@@ -810,7 +858,19 @@ class CudaLeNetEngine(_CudaEngine):
         main.wait_event(join1)
         if early_sync:
             main.wait_event(join3)
-        return 7     # (conv2_wgrad is two launches: the kernel and its reduction)
+        return 8 if self._decay else 7     # (conv2_wgrad is two launches: the kernel and its reduction)
+
+    def _launch_loss_readback(self, *after: torch.cuda.Event) -> None:
+        """The branch that copies (loss, accuracy) into the slot's page-locked host buffer, after the events ``after``;
+        with weight decay it first adds the loss term."""
+        for ev in after:
+            self._side[3].wait_event(ev)
+        with torch.cuda.stream(self._side[3]):
+            if self._decay:
+                self.lib.dm_weight_decay_loss(self._decay_ws, self._decay_parts, self._decay, self.d_loss_acc, stream_ptr())
+            self.h_loss_bufs[self._slot].copy_(self.d_loss_acc, non_blocking=True)
+            self._join_loss = torch.cuda.Event()
+            self._join_loss.record(self._side[3])
 
     def _zero_args(self, train: bool):
         """Regions conv1_fwd clears at the start of a training step (atomically accumulated gradients + loss)."""

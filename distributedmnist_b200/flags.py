@@ -294,6 +294,10 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_float("lr_plateau_min_delta", 0.0, "With --lr_plateau_patience: the accuracy an evaluation must beat the "
                                                 "best by to reset the patience, rounded down to whole validation rows; "
                                                 "0 <= D < 1")
+    F.DEFINE_float("weight_decay", 0.0, "L2 weight decay of the fully connected layers (the reference model's regulariser, "
+                                        "src/mnist.py:142-143): every replica differentiates CE + lambda * sum(v^2) / 2 over "
+                                        "lenet's fc1/fc2 weights and biases (every layer of mlp2 / mlp3), and the logged "
+                                        "training loss includes the term; 0 = off, else 0 < lambda < 1.  GPU path: lenet")
     return F
 
 

@@ -108,6 +108,8 @@ def _signatures() -> dict:
         "dm_stamp_start": (S, i, [P, P]),
         # gemm_tc.cu
         "dm_gemm_bf16": (S, i, [P, P, P, i, i, i, i, i, i, i, i, i, i, i, ll, P, P]),
+        "dm_gemm_decay_ctas": (V, i, [i, i]),
+        "dm_gemm_bf16_decay": (S, i, [P, P, P, i, i, i, i, i, i, i, P, f, P, P]),
         "dm_fc1_dgrad_unpool": (S, i, [P, P, P, P, P, i, P]),
         # host_utils.cu
         "dm_version": (V, i, []),
@@ -119,6 +121,8 @@ def _signatures() -> dict:
         # lenet_simt.cu, mlp_simt.cu, moving_average.cu
         "dm_fc2_fwd_bwd": (S, i, [P, ll, i, P, P, P, P, P, P, P, P, P, i, i, u, P, f, P]),
         "dm_fc2_wgrad": (S, i, [P, P, P, P, P, P, i, P]),
+        "dm_fc2_wgrad_decay_ctas": (V, i, []),
+        "dm_fc2_wgrad_decay": (S, i, [P, P, P, P, P, P, i, P, P, P, f, P, P]),
         "dm_dense10_xent": (S, i, [P, P, P, P, P, P, P, P, P, i, i, i, P]),
         "dm_relu_bwd_colsum": (S, i, [P, P, P, P, i, i, P]),
         "dm_moving_average": (S, i, [P, P, ll, P, d, P, P, ll, ll, ll, ll, P]),
@@ -149,6 +153,8 @@ def _signatures() -> dict:
         "dm_mc_create": (V, i, [ull, i, PULL, PI]),
         "dm_mc_add_device": (V, i, [ull, i]),
         "dm_mc_bind": (V, i, [ull, ull, ull]),
+        # weight_decay.cu
+        "dm_weight_decay_loss": (S, i, [P, i, f, P, P]),
     }
 
 

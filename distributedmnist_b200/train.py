@@ -31,7 +31,7 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
-from . import best, early_stopping, lr_plateau, moving_average
+from . import best, early_stopping, lr_plateau, moving_average, weight_decay
 from .best import BEST_DIR, BEST_JSON
 from .checkpoint import Saver
 from .early_stopping import EARLY_STOPPING_JSON
@@ -622,6 +622,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     check_best_flags(flags)
     check_moving_average_flags(flags, ctx, num_replicas_to_aggregate)
     check_device_data_flags(flags, ctx, dataset)
+    weight_decay.check_flags(flags, ctx)
     device_data = bool(getattr(flags, "device_data", False))
     target = float(getattr(flags, "target_accuracy", 0.0) or 0.0)
     patience = int(getattr(flags, "early_stopping_patience", 0) or 0)
@@ -652,6 +653,11 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     fused_step = hasattr(engine, "attach_optimizer")
     if fused_step:
         engine.attach_optimizer(opt)   # GPU path: compute + fused allreduce/SGD replay as one CUDA graph
+    decay = weight_decay.value(flags)
+    if decay:
+        engine.arm_weight_decay(decay)  # GPU path: after attach_optimizer, whose mode it checks
+        log.info("L2 weight decay %g of %s; the logged training loss includes it"
+                 % (decay, ", ".join(q.name for q in weight_decay.decayed(spec))))
 
     # Supervisor semantics: chief restores the newest checkpoint, everyone gets it.
     restored_step = 0
