@@ -252,6 +252,19 @@ def fc2_wgrad(h: torch.Tensor, dl: torch.Tensor, dh: torch.Tensor) -> Tuple[torc
     return h.t() @ dl, dl.sum(0), dh.to(F64).sum(0)
 
 
+def weight_decay_terms(spec, p, lam: float) -> Tuple[torch.Tensor, Dict[str, torch.Tensor]]:
+    """L2 weight decay (``weight_decay.py``) of the weights ``p`` (flat arena or ``spec.views`` dict): ``(R, terms)``,
+    R = sum of v^2 / 2 over the decayed variables and ``terms[name]`` = lambda * v, the decayed variable's gradient term,
+    both float64.  lambda is taken as the fp32 value the engines use (``weight_decay.value``)."""
+    from types import SimpleNamespace
+    from .. import weight_decay
+    lam = weight_decay.value(SimpleNamespace(weight_decay=lam))
+    views = spec.views(p) if isinstance(p, torch.Tensor) else p
+    qs = weight_decay.decayed(spec)
+    r = sum((views[q.name].to(F64) ** 2).sum() for q in qs) * 0.5
+    return r, {q.name: lam * views[q.name].to(F64) for q in qs}
+
+
 # ---------------------------------------------------------------------------------------------------------------------
 # MLP (csrc/mlp_simt.cu for the output layer and the bias gradients; hidden layers and weight gradients on the wgmma GEMM)
 # ---------------------------------------------------------------------------------------------------------------------

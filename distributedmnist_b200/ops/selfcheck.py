@@ -18,6 +18,7 @@ from ..models import dropout_keep_mask, dropout_seed_mix, get_model, lenet_forwa
 from ..models.lenet import dropout_threshold
 from ..parallel.context import ReplicaContext
 from ..parallel.fused import FusedBackend
+from . import aggrefs as A
 from . import gemm as G
 from . import refs as R
 from .lib import load, stream_ptr
@@ -118,6 +119,29 @@ def run_fc1_wgrad(a2, dh, bf16_out: bool = False):
     G.gemm_bf16_raw(a2, dh, out, 3136, 512, B, 3136, 512, 512, True, True,
                     G.EPI_STORE_BF16 if bf16_out else G.EPI_STORE_F32, bn=128)
     return out
+
+
+def run_fc1_wgrad_decay(a2, dh, w1, lam: float, bf16_out: bool = False, part=None):
+    """dW1 + lambda W1 (dm_gemm_bf16_decay) as the engine issues it: (output, W^2 partial of each CTA).  ``w1``: the fp32
+    weights, read through its data pointer as [3136][512] (a larger buffer holds rows the kernel must not read).  ``part``:
+    the partials' workspace (default: a fresh NaN-filled one)."""
+    lib, B = load(), a2.shape[0]
+    out = torch.full((3136, 512), 7.0, device="cuda").to(BF if bf16_out else torch.float32)
+    if part is None:
+        part = torch.full((int(lib.dm_gemm_decay_ctas(3136, 512)),), float("nan"), dtype=torch.float64, device="cuda")
+    lib.dm_gemm_bf16_decay(a2, dh, out, 3136, 512, B, 3136, 512, 512, int(bf16_out), w1, float(lam), part, stream_ptr())
+    return out, part
+
+
+def run_fc2_wgrad_decay(h, dl, dh, w2, b2, b1, lam: float, part=None):
+    """fc2_wgrad<true>: (g_w2, g_b2, g_b1, W^2 partial of each CTA); stale output contents must not matter."""
+    lib = load()
+    gw2, gb2, gb1 = torch.full((512, 10), 7.0, device="cuda"), torch.full((10,), 7.0, device="cuda"), \
+        torch.full((512,), 7.0, device="cuda")
+    if part is None:
+        part = torch.full((int(lib.dm_fc2_wgrad_decay_ctas()),), float("nan"), dtype=torch.float64, device="cuda")
+    lib.dm_fc2_wgrad_decay(h, dl, dh, gw2, gb2, gb1, h.shape[0], w2, b2, b1, float(lam), part, stream_ptr())
+    return gw2, gb2, gb1, part
 
 
 def run_fc1_dgrad_unpool(dh, w1, code2):
@@ -353,12 +377,14 @@ def _fc2_inputs(kind: str, g, B: int):
 
 
 def _fc2_results(tag: str, kind: str, o: Dict[str, torch.Tensor], ref: Dict[str, torch.Tensor], w2, B: int,
-                 train: bool) -> List[Result]:
+                 train: bool, decay_loss: Optional[float] = None) -> List[Result]:
     """fc2_fwd_bwd outputs.  logits and activations follow the data kind (exact on grid data, where the fc1 sum, bias,
     x2 dropout scale and fc2 products are all grid numbers).  Loss, d logits and d h go through exp/log (the kernel uses
     the fast __expf/__logf) and are compared by the continuous rule on both kinds.  The accuracy is exact, except for
     rows whose top two reference logits are closer than the logits' fp32 error.  A training step stores no logits: with
-    ``o["logits"]`` None they are judged through the loss and the accuracy alone."""
+    ``o["logits"]`` None they are judged through the loss and the accuracy alone.  ``decay_loss``: lambda R of an L2
+    weight decay, which weight_decay_loss has added to the loss word: the word must then be CE + lambda R within the CE
+    bound plus one fp32 ulp (the rounding of fp32(lambda R) and of the add)."""
     res: List[Result] = []
     la = o["la"].double()
     if kind == "grid":
@@ -366,7 +392,12 @@ def _fc2_results(tag: str, kind: str, o: Dict[str, torch.Tensor], ref: Dict[str,
         R.assert_exact_grid(ref["h"].abs() @ w2.abs().double() + 1, 1.0 / (2048 if train else 4096), tag + ".logits")
     if o.get("logits") is not None:
         res += R.compare(tag + ".logits", kind, o["logits"], ref["logits"])
-    res += R.cmp_fp32(tag + ".loss", la[0:1], ref["loss"].reshape(1))
+    if decay_loss is None:
+        res += R.cmp_fp32(tag + ".loss", la[0:1], ref["loss"].reshape(1))
+    else:
+        ce = float(ref["loss"])
+        want = ce + decay_loss
+        res.append((tag + ".loss(CE + lambda R)", abs(float(la[0]) - want), R.REL_FP32 * abs(ce) + 2.0 ** -23 * abs(want)))
     lg_slack = R.fp32_slack(ref["h"].abs() @ w2.abs().double(), 512).max(dim=1).values
     ok = ref["gap"] > 2 * lg_slack
     res.append((tag + ".acc", abs(float(la[1]) - float(ref["acc"])) * B - float((~ok).sum()), 0.5))
@@ -525,6 +556,236 @@ def fc1_wgrad_results(tag: str, kind: str, a2, dh, out) -> List[Result]:
     return R.compare(tag, kind, out, ref, R.fp32_slack(ra, a2.shape[0]))
 
 
+# ---------------------------------------------------------------------------------------------------------------------
+# L2 weight decay (--weight_decay): the decayed epilogues of fc1_wgrad / fc2_wgrad, their W^2 partials, weight_decay_loss
+# ---------------------------------------------------------------------------------------------------------------------
+DECAY_LAMS = (5e-4, 0.0123, 2.0 ** -4)
+DECAY_PART_REL = 1e-12         # sums of exact squares in double: another order moves them by ~n * 2^-53
+
+
+def _lam32(lam) -> float:
+    return float(np.float32(lam))
+
+
+def decayed_bound(abs_sum, n_terms: int, lam: float, v, ref):
+    """Elementwise error bound of a decayed fp32 output fma(lambda, v, acc) against the float64 ``ref`` = plain +
+    lambda v: the fp32 bound of a sum of ``n_terms`` terms whose magnitudes add up to ``abs_sum`` + lambda |v|, plus the
+    fma's one rounding."""
+    return R.fp32_slack(abs_sum.to(R.F64) + lam * v.to(R.F64).abs(), n_terms) + 2.0 ** -24 * ref.abs()
+
+
+def decayed_results(tag: str, kind: str, got, plain_ref, abs_sum, n_terms: int, lam: float, v) -> List[Result]:
+    """One decayed output ``got`` = fma(lambda, v, plain accumulator), stored fp32 or bf16.  ``plain_ref``: the float64
+    reference of the undecayed value, ``abs_sum`` its sum of |terms| over ``n_terms`` terms, ``v`` the fp32 variable.
+    Grid data (the accumulator is exact): bit for bit against the single-rounding emulation fma_f32(lambda, v, plain), then
+    RNE for bf16.  Continuous data: elementwise against plain + lambda v within :func:`decayed_bound`; a bf16 output must
+    lie within RNE of that interval."""
+    lam = _lam32(lam)
+    if kind == "grid":
+        want = A.fma_f32(np.float32(lam), A.f32(v), A.f32(plain_ref.to(torch.float32)))
+        if got.dtype == BF:
+            bad = got.detach().cpu().contiguous().view(torch.int16).numpy().view(np.uint16) != A.bf16_bits(want)
+        else:
+            bad = A.bits(got) != A.bits(want)
+        return [(tag + "[fma bits]", float(bad.sum()), 0.0)]
+    ref = plain_ref.to(R.F64) + lam * v.to(R.F64)
+    bound = decayed_bound(abs_sum, n_terms, lam, v, ref)
+    if got.dtype == BF:
+        return R.cmp_bf16_bound(tag, got, ref, bound)
+    return R.cmp_bound(tag, got, ref, bound)
+
+
+def decay_visible(tag: str, abs_sum, n_terms: int, lam: float, v, plain_ref) -> Result:
+    """Premise of a continuous-data decay check: somewhere lambda |v| exceeds twice :func:`decayed_bound`, so an output
+    without its decay term would fail the check."""
+    lam = _lam32(lam)
+    ref = plain_ref.to(R.F64) + lam * v.to(R.F64)
+    seen = bool((lam * v.to(R.F64).abs() > 2 * decayed_bound(abs_sum, n_terms, lam, v, ref)).any())
+    return (tag + ".decay_term_detectable", 0.0 if seen else 1.0, 0.0)
+
+
+def fc1_wgrad_decay_results(tag: str, kind: str, a2, dh, out, lam: float, w1) -> List[Result]:
+    """dW1 + lambda W1 (fp32 arena or bf16 wire) from a2 [B,3136], dh [B,512] and the fp32 weights w1 [3136,512]."""
+    ref = a2.double().t() @ dh.double()
+    ra = a2.double().abs().t() @ dh.double().abs()
+    return decayed_results(tag, kind, out, ref, ra, a2.shape[0], lam, w1)
+
+
+def fc2_wgrad_decay_results(tag: str, kind: str, h, dl, dh, gw2, gb2, gb1, lam: float, w2, b2, b1) -> List[Result]:
+    """fc2_wgrad<true>: g_w2 / g_b2 / g_b1 + lambda w2 / b2 / b1 from h_act, dlogits, dh and the fp32 variables."""
+    B = h.shape[0]
+    (rw2, rb2, rb1), (aw2, ab2, ab1) = R.fc2_wgrad(h, dl, dh), R.fc2_wgrad(h.abs(), dl.abs(), dh.abs())
+    return decayed_results(tag + ".g_w2", kind, gw2, rw2, aw2, B, lam, w2) + \
+        decayed_results(tag + ".g_b2", kind, gb2, rb2, ab2, B, lam, b2) + \
+        decayed_results(tag + ".g_b1", kind, gb1, rb1, ab1, B, lam, b1)
+
+
+def fc1_decay_partials(w1) -> torch.Tensor:
+    """float64 W^2 sums of dm_gemm_bf16_decay's CTAs for W1 [3136,512]: CTA (x = 128-row tile, y = 128-column tile) at
+    y * 25 + x.  The last row tile holds 64 rows."""
+    sq = torch.zeros(3200, 512, dtype=R.F64, device=w1.device)
+    sq[:3136] = w1.double() ** 2
+    return sq.reshape(25, 128, 4, 128).sum((1, 3)).t().reshape(-1)
+
+
+def fc2_decay_partials(w2, b2, b1) -> torch.Tensor:
+    """float64 sums of squares of fc2_wgrad<true>'s 64 CTAs: CTA c owns w2 rows and b1 entries 8c .. 8c + 7, CTA 0 also
+    b2."""
+    s = (w2.double() ** 2).reshape(64, 80).sum(1) + (b1.double() ** 2).reshape(64, 8).sum(1)
+    s[0] += (b2.double() ** 2).sum()
+    return s
+
+
+def decay_partials_results(tag: str, got, want) -> List[Result]:
+    """W^2 partials or R against their float64 sums, each within DECAY_PART_REL of its value (a zero one exactly)."""
+    return R.cmp_bound(tag, got.reshape(-1), want.reshape(-1), DECAY_PART_REL * want.reshape(-1).abs())
+
+
+def weight_decay_loss_emulated(part, n: int, lam: float, loss: float):
+    """csrc/weight_decay.cu on the host, in its order: lane l sums partials l, l + 32, ... in double, the xor butterfly
+    (16, 8, 4, 2, 1), R = 0.5 * lane 0's sum; the loss word becomes fp32(loss + fp32(double(lambda) * R)).  Returns
+    (R, new loss word) as numpy float64 / float32."""
+    part = np.asarray(part, dtype=np.float64)
+    lanes = [np.float64(0.0)] * 32
+    for lane in range(32):
+        s = np.float64(0.0)
+        for i in range(lane, n, 32):
+            s = s + part[i]
+        lanes[lane] = s
+    for off in (16, 8, 4, 2, 1):
+        lanes = [lanes[i] + lanes[i ^ off] for i in range(32)]
+    r = np.float64(0.5) * lanes[0]
+    term = np.float32(np.float64(np.float32(lam)) * r)
+    return r, np.float32(np.float32(loss) + term)
+
+
+def _fc1_decay_inputs(kind: str, g, B: int):
+    """(a2, dh, W1) on the data of :func:`check_fc1_wgrad`; W1 continuous, or on a k/64 grid."""
+    if kind == "rand":
+        return _bf(torch.rand(B, 3136, generator=g)), _bf(torch.randn(B, 512, generator=g) * 0.01), \
+            torch.randn(3136, 512, generator=g)
+    return _bf(R.grid(g, (B, 3136), 0, 2)), _bf(R.grid(g, (B, 512), -64, 64, 64)), R.grid(g, (3136, 512), -64, 64, 64)
+
+
+def check_fc1_wgrad_decay(B: int = 64, seed: int = 18, kinds: Sequence[str] = KINDS,
+                          lams: Sequence[float] = DECAY_LAMS) -> List[Result]:
+    """dW1 + lambda W1 with the fp32 and the bf16 epilogue, and each CTA's W^2 partial.  W1 lives in the first 3136 rows
+    of a buffer whose 64 rows after them hold 1024: the last row tile is half empty, and its missing rows must neither be
+    read into the partial nor stored."""
+    res: List[Result] = []
+    for kind in kinds:
+        g = _gen(seed)
+        a2, dh, w = _fc1_decay_inputs(kind, g, B)
+        wbuf = torch.full((3200, 512), 1024.0)
+        wbuf[:3136] = w
+        a2, dh, wbuf = _dev(a2, dh, wbuf)
+        w = wbuf[:3136]
+        ra = a2.double().abs().t() @ dh.double().abs()
+        if kind == "grid":
+            R.assert_exact_grid(ra, 1.0 / 64, "fc1_wgrad_decay")
+        want_part = fc1_decay_partials(w)
+        for lam in lams:
+            for bf in (False, True):
+                tag = "fc1_wgrad_decay.%s.%s.lam%g" % (kind, "bf16" if bf else "f32", lam)
+                out, part = run_fc1_wgrad_decay(a2, dh, wbuf, lam, bf)
+                res += fc1_wgrad_decay_results(tag, kind, a2, dh, out, lam, w)
+                res += decay_partials_results(tag + ".w2_partials", part, want_part)
+            if kind == "rand":
+                res.append(decay_visible("fc1_wgrad_decay.rand.lam%g" % lam, ra, B, lam, w, a2.double().t() @ dh.double()))
+    return res
+
+
+def _fc2_decay_inputs(kind: str, g, B: int):
+    """(h, dl, dh, w2, b2, b1): the grid data of :func:`check_fc2_wgrad` with the grid variables of :func:`_fc2_inputs`,
+    or continuous data."""
+    dl = torch.zeros(B, 12)
+    if kind == "rand":
+        h = torch.relu(torch.randn(B, 512, generator=g))
+        dl[:, :10] = torch.randn(B, 10, generator=g) * 0.01
+        dh = _bf(torch.randn(B, 512, generator=g) * 0.01)
+        w2, b2, b1 = (torch.randn(*s, generator=g) for s in ((512, 10), (10,), (512,)))
+        return h, dl, dh, w2, b2, b1
+    h = R.grid(g, (B, 512), 0, 16, 8) * (torch.rand(B, 512, generator=g) < 0.5)
+    dl[:, :10] = R.grid(g, (B, 10), -32, 32, 64)
+    dh = _bf(R.grid(g, (B, 512), -64, 64, 64))
+    b1, w2, b2, _ = _fc2_inputs("grid", g, B)
+    return h, dl, dh, w2, b2, b1
+
+
+def check_fc2_wgrad_decay(B: int = 64, seed: int = 17, kinds: Sequence[str] = KINDS,
+                          lams: Sequence[float] = DECAY_LAMS) -> List[Result]:
+    """fc2_wgrad<true>'s g_w2 / g_b2 / g_b1 and each CTA's sum of squares (b2 in CTA 0's only)."""
+    res: List[Result] = []
+    for kind in kinds:
+        h, dl, dh, w2, b2, b1 = _dev(*_fc2_decay_inputs(kind, _gen(seed), B))
+        aw2, ab2, ab1 = R.fc2_wgrad(h.abs(), dl.abs(), dh.abs())
+        if kind == "grid":
+            R.assert_exact_grid(aw2, 1.0 / 512, "fc2_wgrad_decay.g_w2")
+            R.assert_exact_grid(ab2, 1.0 / 64, "fc2_wgrad_decay.g_b2")
+            R.assert_exact_grid(ab1, 1.0 / 64, "fc2_wgrad_decay.g_b1")
+        want_part = fc2_decay_partials(w2, b2, b1)
+        for lam in lams:
+            tag = "fc2_wgrad_decay.%s.lam%g" % (kind, lam)
+            gw2, gb2, gb1, part = run_fc2_wgrad_decay(h, dl, dh, w2, b2, b1, lam)
+            res += fc2_wgrad_decay_results(tag, kind, h, dl, dh, gw2, gb2, gb1, lam, w2, b2, b1)
+            res += decay_partials_results(tag + ".w2_partials", part, want_part)
+            if kind == "rand":
+                rw2 = R.fc2_wgrad(h, dl, dh)[0]
+                res.append(decay_visible(tag, aw2, B, lam, w2, rw2))
+    return res
+
+
+def check_weight_decay_workspace(B: int = 129, seed: int = 19, lam: float = 0.0123) -> List[Result]:
+    """The engine's decay workspace (fc1 partials, fc2 partials, R) filled by two rounds of both weight-gradient kernels on
+    different weights, then weight_decay_loss: every partial and R must be the second round's, within DECAY_PART_REL of
+    float64, and the loss word must be the kernel's order emulated from the stored partials, bit for bit."""
+    lib = load()
+    n1, n2 = int(lib.dm_gemm_decay_ctas(3136, 512)), int(lib.dm_fc2_wgrad_decay_ctas())
+    ws = torch.full((n1 + n2 + 1,), float("nan"), dtype=torch.float64, device="cuda")
+    g = _gen(seed)
+    a2, dh, _ = _fc1_decay_inputs("rand", g, B)
+    h, dl, dh2, _, _, _ = _fc2_decay_inputs("rand", g, B)
+    a2, dh, h, dl, dh2 = _dev(a2, dh, h, dl, dh2)
+    for scale in (0.05, 0.2):
+        w1, w2, b2, b1 = _dev(*(torch.randn(*s, generator=g) * scale for s in ((3136, 512), (512, 10), (10,), (512,))))
+        run_fc1_wgrad_decay(a2, dh, w1, lam, part=ws[:n1])
+        run_fc2_wgrad_decay(h, dl, dh2, w2, b2, b1, lam, part=ws[n1:n1 + n2])
+    la = torch.tensor([2.5, 0.25], device="cuda")
+    lib.dm_weight_decay_loss(ws, n1 + n2, float(lam), la, stream_ptr())
+    torch.cuda.synchronize()
+    want = torch.cat([fc1_decay_partials(w1), fc2_decay_partials(w2, b2, b1)])
+    r, loss = weight_decay_loss_emulated(ws[:n1 + n2].cpu().numpy(), n1 + n2, lam, 2.5)
+    got = la.cpu().numpy()
+    return decay_partials_results("decay_ws.partials", ws[:n1 + n2], want) + \
+        decay_partials_results("decay_ws.R", ws[n1 + n2:], want.sum().reshape(1) / 2) + \
+        [("decay_ws.R_bits_vs_emulation", float(ws[n1 + n2].item() != r), 0.0),
+         ("decay_ws.loss_bits_vs_emulation", float(got[0].tobytes() != loss.tobytes()), 0.0),
+         ("decay_ws.acc_changed", float(got[1] != np.float32(0.25)), 0.0)]
+
+
+def check_weight_decay_loss(n: int, seed: int = 20, lams: Sequence[float] = DECAY_LAMS) -> List[Result]:
+    """weight_decay_loss alone on n partials spread over 40 binades (so that another summation order would round
+    differently): part[n] and the loss word bit for bit against :func:`weight_decay_loss_emulated`; the partials and the
+    accuracy word untouched."""
+    lib, res = load(), []
+    g = _gen(seed)
+    vals = torch.rand(n, generator=g, dtype=torch.float64) * torch.exp2(torch.randint(-20, 21, (n,), generator=g).double())
+    loss0, acc0 = np.float32(2.3025851), np.float32(0.375)
+    for lam in lams:
+        tag = "weight_decay_loss.n%d.lam%g" % (n, lam)
+        part = torch.cat([vals, torch.tensor([float("nan")], dtype=torch.float64)]).cuda()
+        la = torch.tensor([float(loss0), float(acc0)], dtype=torch.float32, device="cuda")
+        lib.dm_weight_decay_loss(part, n, float(lam), la, stream_ptr())
+        torch.cuda.synchronize()
+        r, loss = weight_decay_loss_emulated(vals.numpy(), n, lam, loss0)
+        got, p = la.cpu().numpy(), part.cpu().numpy()
+        res += [(tag + ".partials_changed", float((p[:n].view(np.uint64) != vals.numpy().view(np.uint64)).sum()), 0.0),
+                (tag + ".R_bits", float(p[n:].tobytes() != np.float64(r).tobytes()), 0.0),
+                (tag + ".loss_bits", float(got[0].tobytes() != loss.tobytes()), 0.0),
+                (tag + ".acc_changed", float(got[1].tobytes() != acc0.tobytes()), 0.0)]
+    return res
+
+
 def fc1_dgrad_results(tag: str, kind: str, dh, w1, code, dy, gb) -> List[Result]:
     """fc1_dgrad_unpool's dy2 [B,14,14,64] and conv2 bias gradient from dh, the bf16 weights w1 and the pool2 codes."""
     rdy, rgb = R.fc1_dgrad_unpool(dh, w1, code)
@@ -570,12 +831,20 @@ FP32_GRAD_TOLS = {"conv1_weights": 0.30, "conv1_biases": 0.15, "conv2_weights": 
                   "fc1_weights": 0.12, "fc1_biases": 0.12, "fc2_weights": 0.03, "fc2_biases": 0.03}
 
 
-def check_end_to_end(B: int = 64, seed: int = 5, images: str = "rand") -> List[Result]:
+def check_end_to_end(B: int = 64, seed: int = 5, images: str = "rand", lam: float = 0.0) -> List[Result]:
     """Whole forward+backward through the CUDA engine vs torch autograd on the bf16-emulating reference.
     ``images="mnist"``: an exact -0.5 background with strokes, so many pooling windows hold equal maxima and the
-    backward pass routes gradients through the first-max tie-break in both conv layers."""
+    backward pass routes gradients through the first-max tie-break in both conv layers.  ``lam``: L2 weight decay armed
+    on the engine; both references then differentiate CE + lambda R (``refs.weight_decay_terms``), and each decayed
+    variable's lambda v must be a larger share of its gradient than that variable's FP32_GRAD_TOLS, so a missing or
+    misplaced decay term fails."""
     eng, be = _engine(B, seed)
     spec, _ = get_model("lenet")
+    if lam:
+        eng.arm_weight_decay(lam)
+
+    def regularised(loss, flat):
+        return loss + _lam32(lam) * R.weight_decay_terms(spec, flat, lam)[0] if lam else loss
     g = torch.Generator(device="cpu").manual_seed(seed)
     x = (torch.rand(B, 28, 28, 1, generator=g) - 0.5) if images == "rand" else mnist_like(g, B)[..., None]
     y = torch.randint(0, 10, (B,), generator=g)
@@ -589,6 +858,7 @@ def check_end_to_end(B: int = 64, seed: int = 5, images: str = "rand") -> List[R
     logits = lenet_forward(spec.views(flat), x.cuda(), train=True, keep_mask=mask, emulate_bf16=True,
                            conv1_bf16=True)
     rloss, racc = loss_and_accuracy(logits, y.cuda())
+    rloss = regularised(rloss, flat)
     rloss.backward()
     out: List[Result] = [("e2e.loss", abs(loss - rloss.item()), 0.02 * max(1.0, abs(rloss.item()))),
                          ("e2e.acc", abs(acc - racc.item()), 2.0 / B + 1e-6)]
@@ -605,14 +875,20 @@ def check_end_to_end(B: int = 64, seed: int = 5, images: str = "rand") -> List[R
     try:
         logits32 = lenet_forward(spec.views(flat32), x.cuda(), train=True, keep_mask=mask, emulate_bf16=False, conv1_bf16=False)
         rloss32, _ = loss_and_accuracy(logits32, y.cuda())
+        rloss32 = regularised(rloss32, flat32)
         rloss32.backward()
     finally:
         torch.backends.cudnn.allow_tf32, torch.backends.cuda.matmul.allow_tf32 = tf32_conv, tf32_mm
     r32 = spec.views(flat32.grad)
+    terms = R.weight_decay_terms(spec, eng.params.detach(), lam)[1] if lam else {}
     for name in r32:
         num = (gv[name].double() - r32[name].double()).norm().item()
         den = r32[name].double().norm().item() + 1e-12
-        out.append(("e2e.grad_vs_fp32.%s(L2 rel)" % name, num / den, FP32_GRAD_TOLS.get(name, 0.3)))
+        tol = FP32_GRAD_TOLS.get(name, 0.3)
+        out.append(("e2e.grad_vs_fp32.%s(L2 rel)" % name, num / den, tol))
+        if name in terms:
+            share = terms[name].norm().item() / den
+            out.append(("e2e.decay_share_vs_tol.%s(tol/share)" % name, tol / share, 1.0))
     out.append(("e2e.loss_vs_fp32", abs(loss - rloss32.item()), 0.02 * max(1.0, abs(rloss32.item()))))
     # padding of the gradient arena must stay zero (the fused kernel reduces the whole arena)
     out.append(("e2e.grad.padding", eng.grads[~spec.valid_mask().cuda()].abs().max().item(), 1e-12))

@@ -20,6 +20,7 @@ from typing import Dict, List, Sequence
 
 import torch
 
+from ..lr_plateau import NO_CUT
 from ..models import dropout_keep_mask, dropout_seed_mix
 from . import aggrefs as A
 from . import refs as R
@@ -49,17 +50,27 @@ class StepRecorder:
         r.update(grads=e.grads.clone(), params=e.params.clone(), shadow=e.shadow.clone(), loss_acc=e.d_loss_acc.clone())
         if e._bucket_v2:
             r["g16"] = e._g16_view.clone()
+        if getattr(e, "_decay", 0.0):
+            r["decay_ws"] = e._decay_ws.clone()         # the W^2 partials of both weight-gradient kernels, then R
         self.records.append(r)
 
 
 def update_of(eng, sched, step0: int) -> dict:
     """How ``eng`` applies its gradients: ``mode`` "fused" (fused_sync_sgd), "bucket" (the bf16-wire bucketed kernels)
-    or "kgtn" (K > N: every k-th iteration commits), the schedule and the global step of the first step."""
+    or "kgtn" (K > N: every k-th iteration commits), the schedule and the global step of the first step.  ``drop``:
+    (seed, keep probability) of the drop-connect mask the fused kernel applies, None without it.  With a cut table armed
+    (``arm_lr_cuts``), ``sched`` must name the same cuts (raises ValueError otherwise): the step sizes are then those of
+    the schedule with the cuts (synchronises the device to read the table)."""
     be = eng.backend
     e0, e1 = eng._bucket_early
     mode = "kgtn" if eng._kgtn_k else ("bucket" if eng._bucket_v2 else "fused")
+    if getattr(eng, "_lr_table", None) is not None:
+        table = sorted(c for c in eng.lr_cut_table() if c != NO_CUT)
+        if table != sorted(getattr(sched, "cuts", ())):
+            raise ValueError("the engine's cut table holds %s, the schedule's cuts are %s" % (table, sched.cuts))
     return dict(mode=mode, sched=sched, step0=step0, k=max(eng._kgtn_k, 1), early=(e0, e1),
-                late_bf16=A.late_bucket_rounds_bf16(eng.spec.arena_numel, e1 - e0, be.late_ll, be.late_bf16))
+                late_bf16=A.late_bucket_rounds_bf16(eng.spec.arena_numel, e1 - e0, be.late_ll, be.late_bf16),
+                drop=(be.drop_seed, be.drop_keep) if be.drop_keep > 0.0 else None)
 
 
 def epoch_of(upd: dict, t: int) -> int:
@@ -73,9 +84,10 @@ def _shadow_bits(t: torch.Tensor):
 
 def update_results(tag: str, init: dict, records: Sequence[dict], upd: dict) -> List[Result]:
     """Each step's weights from the previous record (or ``init``) and the step's recorded gradients, bit for bit; with
-    K > N the weights stay put until the k-th iteration, which applies the accumulated k gradients."""
+    K > N the weights stay put until the k-th iteration, which applies the accumulated k gradients.  With drop-connect
+    the fused kernel masks the gradient with the mask of the step's global step."""
     res: List[Result] = []
-    mode, k = upd["mode"], upd["k"]
+    mode, k, drop = upd["mode"], upd["k"], upd.get("drop")
     res.append((tag + ".init.shadow_bits_differ", float((_shadow_bits(init["shadow"]) != A.bf16_bits(init["params"])).sum()), 0.0))
     w, acc = A.f32(init["params"]), []
     for t, r in enumerate(records):
@@ -88,7 +100,8 @@ def update_results(tag: str, init: dict, records: Sequence[dict], upd: dict) -> 
         elif mode == "bucket":
             want = A.bucket_step(w, [g], [A.f32(r["g16"].float()).reshape(-1)], upd["early"], scale, upd["late_bf16"])
         else:
-            want = A.fused_sync_step(w, [g], 1, scale)
+            want = A.fused_sync_step(w, [g], 1, scale,
+                                     drop=None if drop is None else (drop[0], epoch_of(upd, t), drop[1]))
         got = A.bits(r["params"])
         res.append(("%s.step%d.update_bits_differ" % (tag, t), float((got != A.bits(want)).sum()), 0.0))
         if mode != "kgtn":          # K > N refreshes the shadow when the next iteration adopts the commit
@@ -104,11 +117,20 @@ def _inputs(spec, init: dict, records: Sequence[dict], t: int, dev):
     return spec.views(p), spec.views(p.to(torch.bfloat16))
 
 
-def lenet_step_results(tag: str, spec, r: dict, p, pb, images, labels, mask, keep_prob: float) -> List[Result]:
+def lenet_step_results(tag: str, spec, r: dict, p, pb, images, labels, mask, keep_prob: float,
+                       lam: float = 0.0) -> List[Result]:
     """One LeNet training step from its record ``r``: every stage from the recorded inputs of that stage.  ``p`` / ``pb``:
-    the fp32 / bf16 weights the step read, ``images`` [B,28,28] / ``labels`` what it was fed, ``mask`` its dropout mask."""
+    the fp32 / bf16 weights the step read, ``images`` [B,28,28] / ``labels`` what it was fed, ``mask`` its dropout mask.
+
+    ``lam``: L2 weight decay armed.  The fc weight gradients are then checked elementwise against the plain reference +
+    lambda v, v from ``p`` (the wire buffer as RNE of that value), the recorded R against float64 R of ``p``, and the loss
+    word against CE + lambda R."""
     kind = "rand"
     B = labels.shape[0]
+    decay_loss = None
+    if lam:
+        r_ref = R.weight_decay_terms(spec, p, lam)[0]
+        decay_loss = S._lam32(lam) * float(r_ref)
     x = images.reshape(B, 28, 28)
     a2 = r["a2"]
     g = spec.views(r["grads"])
@@ -120,14 +142,23 @@ def lenet_step_results(tag: str, spec, r: dict, p, pb, images, labels, mask, kee
     hsum = a2.double() @ w1
     ref = R.fc2_fwd_bwd(hsum, p["fc1_biases"], p["fc2_weights"], p["fc2_biases"], labels, mask, keep_prob)
     o = dict(la=r["loss_acc"], h=r["h_act"], dl=r["dlogits"], dh=r["dh"])
-    res += S._fc2_results(tag + ".fc2_fwd_bwd", kind, o, ref, p["fc2_weights"], B, True)
+    res += S._fc2_results(tag + ".fc2_fwd_bwd", kind, o, ref, p["fc2_weights"], B, True, decay_loss=decay_loss)
     b1 = p["fc1_biases"].double()
     # the kernel's pre-activation: 7 fp32 GEMM partials of 448 products each, summed with the bias in fp32
     res += S.keep_pattern_results(tag + ".fc2_fwd_bwd.keep_pattern", r["h_act"], ref["h"], hsum + b1,
                                   R.fp32_slack(a2.double().abs() @ w1.abs() + b1.abs(), 3136 + 8))
-    res += S.fc2_wgrad_results(tag + ".fc2_wgrad", r["h_act"], r["dlogits"], r["dh"], g["fc2_weights"], g["fc2_biases"],
-                               g["fc1_biases"])
-    res += S.fc1_wgrad_results(tag + ".fc1_wgrad", kind, a2, r["dh"], r.get("g16", g["fc1_weights"]))
+    if lam:
+        ws = r["decay_ws"]
+        res += S.decay_partials_results(tag + ".decay_R", ws[-1:], r_ref.reshape(1).to(ws.device))
+        res += S.fc2_wgrad_decay_results(tag + ".fc2_wgrad", kind, r["h_act"], r["dlogits"], r["dh"], g["fc2_weights"],
+                                         g["fc2_biases"], g["fc1_biases"], lam, p["fc2_weights"], p["fc2_biases"],
+                                         p["fc1_biases"])
+        res += S.fc1_wgrad_decay_results(tag + ".fc1_wgrad", kind, a2, r["dh"], r.get("g16", g["fc1_weights"]), lam,
+                                         p["fc1_weights"])
+    else:
+        res += S.fc2_wgrad_results(tag + ".fc2_wgrad", r["h_act"], r["dlogits"], r["dh"], g["fc2_weights"],
+                                   g["fc2_biases"], g["fc1_biases"])
+        res += S.fc1_wgrad_results(tag + ".fc1_wgrad", kind, a2, r["dh"], r.get("g16", g["fc1_weights"]))
     res += S.fc1_dgrad_results(tag + ".fc1_dgrad_unpool", kind, r["dh"], pb["fc1_weights"], r["code2"], r["dy2"],
                                g["conv2_biases"])
     res += S.conv2_dgrad_results(tag + ".conv2_dgrad", kind, r["dy2"], pb["conv2_weights"], r["dx1"])
@@ -140,15 +171,17 @@ def lenet_step_results(tag: str, spec, r: dict, p, pb, images, labels, mask, kee
 
 
 def lenet_trajectory_results(tag: str, spec, init: dict, records: Sequence[dict], batches: Sequence, upd: dict,
-                             seed: int, rank: int, keep_prob: float) -> List[Result]:
-    """Every step of a LeNet run (``batches[t]`` = (images, labels) fed to step t) and every update."""
+                             seed: int, rank: int, keep_prob: float, lam: float = 0.0) -> List[Result]:
+    """Every step of a LeNet run (``batches[t]`` = (images, labels) fed to step t) and every update.  ``lam``: the L2
+    weight decay the run was armed with (see :func:`lenet_step_results`)."""
     res = update_results(tag, init, records, upd)
     for t, (r, (x, y)) in enumerate(zip(records, batches)):
         dev = r["a1"].device
         p, pb = _inputs(spec, init, records, t, dev)
         y = torch.as_tensor(y).to(dev)
         mask = dropout_keep_mask(dropout_seed_mix(seed, epoch_of(upd, t), rank), y.shape[0], 512, keep_prob, device=dev)
-        res += lenet_step_results("%s.step%d" % (tag, t), spec, r, p, pb, torch.as_tensor(x).to(dev), y, mask, keep_prob)
+        res += lenet_step_results("%s.step%d" % (tag, t), spec, r, p, pb, torch.as_tensor(x).to(dev), y, mask, keep_prob,
+                                  lam)
     return res
 
 

@@ -139,6 +139,47 @@ def test_grid_premise_is_enforced():
     assert R.assert_exact_grid(torch.tensor([2.0 ** 24 - 1]), 1.0, "fits") < 2 ** 24
 
 
+def _l2_loss(v):
+    """TF's ``tf.nn.l2_loss``: sum(v^2) / 2."""
+    return (v * v).sum() / 2
+
+
+# the reference model's regulariser (src/mnist.py, commented out there): l2_loss of these four, conv layers not decayed
+REFERENCE_REGULARISED = {"lenet": ("fc1_weights", "fc1_biases", "fc2_weights", "fc2_biases")}
+
+
+@pytest.mark.parametrize("model", ["lenet", "mlp2", "mlp3"])
+@pytest.mark.parametrize("lam", [5e-4, 0.0123, 2.0 ** -4])
+def test_weight_decay_terms_are_the_gradient_of_the_regulariser(model, lam):
+    """R and every decayed variable's gradient term against torch.autograd of lambda * sum l2_loss(v) in float64 (lambda
+    as its fp32 value), over the whole arena: a variable the helper leaves out, or one it decays that the objective does
+    not, fails here, as does sum v^2 in place of sum v^2 / 2."""
+    import numpy as np
+    from distributedmnist_b200.models import get_model
+    spec = get_model(model, 64)[0]
+    g = torch.Generator().manual_seed(3)
+    flat = (spec.init_flat(7).double() + 0.01 * torch.randn(spec.arena_numel, generator=g, dtype=torch.float64)) \
+        * spec.valid_mask()
+    names = REFERENCE_REGULARISED.get(model, tuple(q.name for q in spec.params))     # the MLPs: every layer is fc
+    x = flat.clone().requires_grad_(True)
+    v = spec.views(x)
+    lam32 = float(np.float32(lam))
+    obj = lam32 * sum(_l2_loss(v[n]) for n in names)
+    (grad,) = torch.autograd.grad(obj, x)
+    r, terms = R.weight_decay_terms(spec, flat, lam)
+    obj = float(obj.detach())
+    assert abs(float(r) * lam32 - obj) <= 1e-13 * obj
+    want = spec.views(grad)
+    assert set(terms) == set(names)
+    for q in spec.params:
+        if q.name in terms:
+            assert torch.allclose(terms[q.name], want[q.name], rtol=1e-15, atol=0), q.name
+        else:
+            assert not want[q.name].any(), q.name          # not decayed: the objective's gradient is zero there
+    if model == "lenet":
+        assert not any(n.startswith("conv") for n in terms)
+
+
 def test_first_max_tie_break():
     win = torch.tensor([[1.0, 3.0, 3.0, 2.0], [5.0, 5.0, 5.0, 5.0], [0.0, 0.0, 0.0, 1.0]], dtype=torch.float64)
     _, idx = R.first_max(win)

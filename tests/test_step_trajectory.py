@@ -1,8 +1,10 @@
 """The trajectory checker (ops/trajectory.py) on CPU-built records: small LeNet and MLP runs emulated from the float64
 references in the engine's storage formats pass unchanged, and each seeded ordering fault fails."""
+import numpy as np
 import pytest
 import torch
 
+from distributedmnist_b200 import weight_decay as W
 from distributedmnist_b200.models import dropout_keep_mask, dropout_seed_mix, get_model
 from distributedmnist_b200.ops import aggrefs as A
 from distributedmnist_b200.ops import refs as R
@@ -30,8 +32,9 @@ def _update(w, g):
     return lambda t: torch.from_numpy(A.fused_sync_step(A.f32(w), [A.f32(g)], 1, A.step_scale(SCHED, STEP0 + t, 1)))
 
 
-def _lenet_step(spec, params, x, y, mask, fault, prev):
-    """One LeNet step as the kernels store it.  ``fault``: "dgrad_post_update" runs fc1 dgrad on the updated shadow."""
+def _lenet_step(spec, params, x, y, mask, fault, prev, lam=0.0):
+    """One LeNet step as the kernels store it.  ``fault``: "dgrad_post_update" runs fc1 dgrad on the updated shadow.
+    ``lam``: L2 weight decay (see :func:`_decay`)."""
     B = x.shape[0]
     p, pb = spec.views(params), spec.views(params.to(BF))
     f1 = R.pool_fwd(R.conv5x5(x.to(BF)[..., None], p["conv1_weights"].to(BF)), p["conv1_biases"])
@@ -59,8 +62,32 @@ def _lenet_step(spec, params, x, y, mask, fault, prev):
     gw1, gbc1 = R.conv1_wgrad(x.to(BF), dx1, code1)
     g["conv1_weights"].copy_(gw1.reshape(5, 5, 1, 32)), g["conv1_biases"].copy_(gbc1)
     la = torch.tensor([float(ref["loss"]), float(ref["acc"])], dtype=torch.float32)
-    return dict(a1=a1, code1=code1, a2=a2, code2=code2, h_part=h_part, dh=dh, h_act=h_act, dlogits=dlogits, dy2=dy2,
-                dx1=dx1, grads=_ftz(grads), loss_acc=la)
+    r = dict(a1=a1, code1=code1, a2=a2, code2=code2, h_part=h_part, dh=dh, h_act=h_act, dlogits=dlogits, dy2=dy2,
+             dx1=dx1, grads=grads, loss_acc=la)
+    if lam:
+        _decay(spec, params, r, lam, fault, prev)
+    _ftz(grads)
+    return r
+
+
+def _decay(spec, params, r, lam, fault, prev):
+    """L2 weight decay as the kernels apply it: lambda v added to the four fc gradients, R of the weights the step read
+    into the workspace's last slot, fp32(lambda R) added to the loss word.  ``fault``: one of DECAY_FAULTS."""
+    lam = float(np.float32(lam))
+    p, g = spec.views(params), spec.views(r["grads"])
+    for name in W.LENET_DECAYED:
+        if fault == "decay_no_fc1_biases" and name == "fc1_biases":
+            continue
+        v = p[name]
+        if fault == "decay_post_update" and name == "fc1_weights":
+            v = spec.views(_update(params, _ftz(r["grads"].clone()))(prev["t"]))[name]   # after the early bucket's update
+        g[name].copy_(g[name].double() + (2 if fault == "decay_twice" else 1) * lam * v.double())
+    if fault == "decay_conv2_biases":
+        g["conv2_biases"].copy_(g["conv2_biases"].double() + lam * p["conv2_biases"].double())
+    rr = R.weight_decay_terms(spec, prev["params"] if fault == "decay_R_previous_step" else params, lam)[0]
+    r["decay_ws"] = torch.tensor([float(rr)], dtype=torch.float64)
+    if fault != "loss_without_decay":
+        r["loss_acc"][0] = r["loss_acc"][0] + np.float32(lam * float(rr))
 
 
 def _mlp_step(spec, params, x, y, fault, prev):
@@ -95,15 +122,16 @@ def _mlp_step(spec, params, x, y, fault, prev):
     return dict(x16=x16, h=hs, dh=dhs, dl_pad=dl_pad, grads=_ftz(grads), loss_acc=la)
 
 
-def _run(model, fault=None, steps=4, B=8):
-    """(spec, init, records, batches fed, update) of an emulated run with at most one seeded fault."""
+def _run(model, fault=None, steps=4, B=8, lam=0.0):
+    """(spec, init, records, batches fed, update) of an emulated run with at most one seeded fault; ``lam``: L2 weight
+    decay (LeNet)."""
     spec = get_model(model, 64)[0]
     gen = torch.Generator().manual_seed(11)
     shape = (B, 28, 28) if model == "lenet" else (B, 784)
     batches = [(torch.rand(*shape, generator=gen) - 0.5, torch.randint(0, 10, (B,), generator=gen)) for _ in range(steps)]
     params = spec.init_flat(SEED)
     init = dict(params=params.clone(), shadow=params.to(BF))
-    records, prev = [], dict(t=0, grads=None)
+    records, prev = [], dict(t=0, grads=None, params=params.clone())
     for t in range(steps):
         x, y = batches[t]
         if fault == "batch_t_plus_2" and t == 1:
@@ -114,7 +142,7 @@ def _run(model, fault=None, steps=4, B=8):
         if model == "lenet":
             e = STEP0 + t - (1 if fault == "mask_previous_epoch" and t > 0 else 0)
             mask = dropout_keep_mask(dropout_seed_mix(SEED, e, RANK), B, 512, KEEP)
-            r = _lenet_step(spec, params, x, y, mask, fault, prev)
+            r = _lenet_step(spec, params, x, y, mask, fault, prev, lam)
         else:
             r = _mlp_step(spec, params, x, y, fault, prev)
         g = prev["grads"] if fault == "stale_gradient" and t > 0 else r["grads"]
@@ -122,14 +150,15 @@ def _run(model, fault=None, steps=4, B=8):
         r.update(params=params.clone(), shadow=params.to(BF))
         records.append(r)
         prev["grads"] = r["grads"]
+        prev["params"] = (init["params"] if t == 0 else records[t - 1]["params"]).clone()   # what step t read
     upd = dict(mode="fused", sched=SCHED, step0=STEP0, k=1, early=(spec.param("fc1_weights").offset,) * 2, late_bf16=False)
     return spec, init, records, batches, upd
 
 
-def _results(model, fault=None):
-    spec, init, records, batches, upd = _run(model, fault)
+def _results(model, fault=None, lam=0.0):
+    spec, init, records, batches, upd = _run(model, fault, lam=lam)
     if model == "lenet":
-        return T.lenet_trajectory_results("lenet", spec, init, records, batches, upd, SEED, RANK, KEEP)
+        return T.lenet_trajectory_results("lenet", spec, init, records, batches, upd, SEED, RANK, KEEP, lam)
     return T.mlp_trajectory_results("mlp3", spec, init, records, batches, upd)
 
 
@@ -172,3 +201,53 @@ def test_kgtn_update_commits_every_k_th_iteration():
     assert [T.epoch_of(upd, t) for t in range(4)] == [STEP0, STEP0, STEP0 + 1, STEP0 + 1]
     recs[1] = dict(recs[1], params=w)                  # the commit not applied
     assert T.failures(T.update_results("kgtn", init, recs, upd))
+
+
+# ---- L2 weight decay ----------------------------------------------------------------------------------------------------
+# 2^-6: with the step size above, one update moves the weights by a visible fraction of lambda W
+DECAY_LAM = 2.0 ** -6
+
+
+@pytest.mark.parametrize("lam", [5e-4, DECAY_LAM])
+def test_emulated_decayed_trajectory_passes(lam):
+    res = _results("lenet", lam=lam)
+    assert not T.failures(res), T.failures(res)
+    worst = T.worst_by_stage("lenet", res)
+    for stage in ("decay_R[err/bound]", "fc2_wgrad.g_b1[err/bound]", "fc1_wgrad[err/bound]", "fc2_fwd_bwd.loss(CE + lambda R)"):
+        assert stage in worst, (stage, sorted(worst))
+    assert all(0 <= v <= 1 for v in worst.values()), worst
+
+
+@pytest.mark.parametrize("fault,stage", [
+    ("decay_no_fc1_biases", "fc2_wgrad.g_b1"),
+    ("decay_conv2_biases", "fc1_dgrad_unpool.g_bias"),
+    ("decay_twice", "fc1_wgrad"),
+    ("decay_post_update", "fc1_wgrad"),
+    ("decay_R_previous_step", "decay_R"),
+    ("loss_without_decay", "fc2_fwd_bwd.loss"),
+])
+def test_seeded_decay_fault_fails(fault, stage):
+    bad = T.failures(_results("lenet", fault, lam=DECAY_LAM))
+    assert any(stage in n for n, _, _ in bad), (fault, bad[:10])
+
+
+def test_decayed_update_with_drop_connect_and_cuts():
+    """The update check with drop-connect (the fused kernel's mask of the step's global step, over the decayed gradient)
+    and a schedule with cuts inside the run; the same records fail without the mask or without the cuts."""
+    spec = get_model("lenet", 64)[0]
+    gen = torch.Generator().manual_seed(4)
+    w = spec.init_flat(SEED)
+    init = dict(params=w.clone(), shadow=w.to(BF))
+    sched = LearningRateSchedule(4.0, 1, 0.999, factor=0.5, cuts=[STEP0 + 1, STEP0 + 3])
+    seed, keep = 0x2545F491, 0.8
+    recs, cur = [], w
+    for t in range(4):
+        g = torch.randn(spec.arena_numel, generator=gen) * 1e-2 * spec.valid_mask()
+        g = g + DECAY_LAM * cur * spec.valid_mask()
+        cur = torch.from_numpy(A.fused_sync_step(A.f32(cur), [A.f32(g)], 1, A.step_scale(sched, STEP0 + t, 1),
+                                                 drop=(seed, STEP0 + t, keep)))
+        recs.append(dict(grads=g, params=cur, shadow=cur.to(BF)))
+    upd = dict(mode="fused", sched=sched, step0=STEP0, k=1, early=(0, 0), late_bf16=False, drop=(seed, keep))
+    assert not T.failures(T.update_results("drop", init, recs, upd))
+    assert T.failures(T.update_results("drop", init, recs, dict(upd, drop=None)))
+    assert T.failures(T.update_results("drop", init, recs, dict(upd, sched=SCHED)))

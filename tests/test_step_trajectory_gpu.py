@@ -4,7 +4,12 @@ another, so the fork/join edges of the step graphs, the carrying of weights, sha
 the clearing of atomically accumulated gradients and both slot graphs are all exercised as training runs them.
 
 Every run starts at global step 3001 with a schedule whose rate changes every step, and has at least 6 steps unless
-stated otherwise: the first two capture the two slot graphs, the rest replay them pipelined."""
+stated otherwise: the first two capture the two slot graphs, the rest replay them pipelined.
+
+The L2 weight decay (``--weight_decay``) runs are checked the same way, with the fc gradients against the plain reference
++ lambda v of the weights the step read, R against float64 and the loss word against CE + lambda R.  Interval mode is not
+among them: its commits follow a wall-clock deadline, which the update check has no model of, so it is covered by a
+smoke run (tests/test_weight_decay_gpu.py) only.  Runs with more than one replica need more than one GPU."""
 import json
 import os
 
@@ -29,21 +34,23 @@ def _backend():
     return FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
 
 
-def _start(eng, be, k=1):
+def _start(eng, be, k=1, lam=0.0, drop=None, sched=None):
     from distributedmnist_b200.ops.trajectory import StepRecorder
     from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
-    eng.attach_optimizer(SyncReplicasOptimizer(be, _sched(), k, 1))
+    eng.attach_optimizer(SyncReplicasOptimizer(be, sched or _sched(), k, 1, drop_connect_probability=drop))
+    if lam:
+        eng.arm_weight_decay(lam)
     be.set_global_step(STEP0)
     if k > 1:
         be.kgtn_arm()
     return StepRecorder(eng)
 
 
-def _lenet(B, keep_prob=0.5, k=1):
+def _lenet(B, keep_prob=0.5, k=1, lam=0.0, drop=None, sched=None):
     from distributedmnist_b200.engine_cuda import CudaLeNetEngine
     be = _backend()
     eng = CudaLeNetEngine(B, be, seed=SEED, rank=0, keep_prob=keep_prob, use_graph=True)
-    return eng, be, _start(eng, be, k)
+    return eng, be, _start(eng, be, k, lam, drop, sched)
 
 
 def _mlp(model, B, hidden, k=1):
@@ -92,16 +99,20 @@ def _feed(eng, rec, batches, how="numpy", sleep_after=None):
     return keep
 
 
-def _check(tag, eng, be, rec, batches):
+def _check(tag, eng, be, rec, batches, lam=0.0, sched=None):
+    """``lam``: the L2 weight decay the engine was armed with; ``sched``: the schedule it was attached with (default
+    :func:`_sched`)."""
     from distributedmnist_b200.ops import trajectory as T
     be.check_error()
-    upd = T.update_of(eng, _sched(), STEP0)
-    assert upd["mode"] == ("kgtn" if eng._kgtn_k else ("bucket" if os.environ.get("DMNIST_BUCKET", "2") == "2" else "fused"))
+    upd = T.update_of(eng, sched or _sched(), STEP0)
+    bucket = os.environ.get("DMNIST_BUCKET", "2") == "2" and be.drop_keep <= 0.0     # drop-connect: the single kernel
+    assert upd["mode"] == ("kgtn" if eng._kgtn_k else ("bucket" if bucket else "fused"))
+    assert getattr(eng, "_decay", 0.0) == float(np.float32(lam)) and (("decay_ws" in rec.records[0]) == bool(lam))
     if not eng._kgtn_k:
         assert be.device_epoch == STEP0 + len(batches)
     if hasattr(eng, "h_part"):
         res = T.lenet_trajectory_results(tag, eng.spec, rec.init, rec.records, batches, upd, eng.seed, eng.rank,
-                                         eng.keep_prob)
+                                         eng.keep_prob, lam)
     else:
         res = T.mlp_trajectory_results(tag, eng.spec, rec.init, rec.records, batches, upd)
     worst = T.worst_by_stage(tag, res)
@@ -195,3 +206,79 @@ def test_mlp2_k2_trajectory():
     batches = _batches(eng, 6)
     _feed(eng, rec, batches)
     _check("mlp2.B128.H1024.k2", eng, be, rec, batches)
+
+
+# ---- L2 weight decay ----------------------------------------------------------------------------------------------------
+LAM = 5e-4
+LAM_LARGE = 0.25               # a decay read from the wrong weights differs from the right one far beyond the bound
+
+
+@pytest.mark.parametrize("B,lam", [(37, LAM), (129, LAM), (256, LAM), (1024, LAM), (256, LAM_LARGE)])
+def test_lenet_decayed_bucketed_trajectory(B, lam, monkeypatch):
+    """fc1's decayed gradient leaves the GEMM as bf16 on the wire; the early bucket then updates fc1 on the same branch,
+    after the decayed epilogue read it."""
+    monkeypatch.setenv("DMNIST_BUCKET", "2")
+    eng, be, rec = _lenet(B, lam=lam)
+    batches = _batches(eng, 6, seed=B)
+    _feed(eng, rec, batches)
+    _check("lenet.B%d.bucket2.decay%g" % (B, lam), eng, be, rec, batches, lam)
+
+
+def test_lenet_decayed_single_kernel_trajectory(monkeypatch):
+    monkeypatch.setenv("DMNIST_BUCKET", "0")
+    eng, be, rec = _lenet(128, lam=LAM)
+    batches = _batches(eng, 6)
+    _feed(eng, rec, batches)
+    _check("lenet.B128.bucket0.decay", eng, be, rec, batches, LAM)
+
+
+def test_lenet_decayed_keep_08_trajectory(monkeypatch):
+    monkeypatch.setenv("DMNIST_BUCKET", "2")
+    eng, be, rec = _lenet(128, keep_prob=0.8, lam=LAM)
+    batches = _batches(eng, 6)
+    _feed(eng, rec, batches)
+    _check("lenet.B128.keep0.8.decay", eng, be, rec, batches, LAM)
+
+
+@pytest.mark.parametrize("how", ["packed", "step_indices"])
+def test_lenet_decayed_native_runner_feeds(how, monkeypatch):
+    monkeypatch.setenv("DMNIST_BUCKET", "2")
+    eng, be, rec = _lenet(256, lam=LAM)
+    batches = _batches(eng, 7)
+    _feed(eng, rec, batches, how)
+    assert eng._runner is not None
+    _check("lenet.B256.%s.decay" % how, eng, be, rec, batches, LAM)
+
+
+@pytest.mark.parametrize("lam", [LAM, LAM_LARGE])
+def test_lenet_decayed_k4_trajectory(lam):
+    """K = 4 on one replica, 2 commits: every iteration is decayed at the weights of the commit it adopted (DESIGN §4,
+    which weights the decay term reads), which the previous record holds."""
+    eng, be, rec = _lenet(128, k=4, lam=lam)
+    batches = _batches(eng, 8)
+    _feed(eng, rec, batches)
+    _check("lenet.B128.k4.decay%g" % lam, eng, be, rec, batches, lam)
+
+
+def test_lenet_decayed_drop_connect_trajectory():
+    """--drop_connect runs the single fused kernel, which masks each gradient element, its lambda v included."""
+    eng, be, rec = _lenet(128, lam=LAM, drop=0.8)
+    assert be.drop_keep == pytest.approx(0.8) and not eng._bucket_v2
+    batches = _batches(eng, 6)
+    _feed(eng, rec, batches)
+    _check("lenet.B128.drop0.8.decay", eng, be, rec, batches, LAM)
+
+
+@pytest.mark.parametrize("bucket", ["2", "0"])
+def test_lenet_decayed_trajectory_with_lr_cuts(bucket, monkeypatch):
+    """A cut table with entries before, inside and at the end of the run: the step sizes are those of the schedule with
+    the cuts, and the decay is unaffected."""
+    from distributedmnist_b200.schedule import LearningRateSchedule
+    monkeypatch.setenv("DMNIST_BUCKET", bucket)
+    cuts = [2990, STEP0 + 2, STEP0 + 4, STEP0 + 4]
+    sched = LearningRateSchedule(0.05, 1, 0.999, factor=0.5, cuts=cuts)
+    eng, be, rec = _lenet(128, lam=LAM, sched=sched)
+    eng.arm_lr_cuts(0.5, cuts)
+    batches = _batches(eng, 6)
+    _feed(eng, rec, batches)
+    _check("lenet.B128.bucket%s.cuts.decay" % bucket, eng, be, rec, batches, LAM, sched)
