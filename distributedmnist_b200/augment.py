@@ -1,0 +1,137 @@
+"""Random affine augmentation of the training images (``--augment_max_shift``, ``--augment_max_rotation``,
+``--augment_max_scale``): small shifts, rotations and zooms, as Keras's ``ImageDataGenerator`` and torchvision's
+``RandomAffine`` provide them.  Training batches only: no evaluation is ever augmented, and labels are unchanged.
+
+The transform, defined here once (csrc/augment.cu computes the same one in fp32 on the device):
+
+* Row ``b`` of replica ``r`` at augmentation iteration ``i`` draws four uniforms ``u_k = (h_k >> 8) * 2^-24`` with
+  ``h_k = hash_mix(hash_mix(seed_mix(seed, r), i), 4 b + k)``, ``hash_mix`` the murmur3 finaliser the dropout mask uses
+  (models/lenet.py), keyed by a mixing constant of its own so the draws are independent of dropout's.  A row's draws do
+  not depend on the batch size.
+* ``theta = R pi/180 (2 u0 - 1)``, ``s = 1 + S (2 u1 - 1)``, ``tx = T (2 u2 - 1)``, ``ty = T (2 u3 - 1)``.
+* Output pixel ``(x, y)`` samples the source bilinearly at the inverse map around the centre ``c = 13.5``:
+  ``sx = c + a dx + b dy``, ``sy = c - b dx + a dy`` with ``a = cos(theta) / s``, ``b = sin(theta) / s``,
+  ``dx = x - c - tx``, ``dy = y - c - ty``.  A tap outside ``[0, 27]^2`` reads the background ``BACKGROUND = -0.5``, the
+  value of a zero pixel after data.py's ``(x - 127.5) / 255`` scaling.
+
+``i`` counts the replica's training iterations, starting at the restored global step, so two iterations never share
+draws and a restarted run does not replay those of its first steps.  Nothing enters the checkpoint.
+
+The numpy hash here is exact (integer arithmetic); :func:`warp` is the float64 warp.  The torch engine applies
+:func:`augment_batch`; the tests compare the kernel's draws and pixels against both.
+"""
+from __future__ import annotations
+
+import math
+from typing import NamedTuple, Optional
+
+import numpy as np
+
+_M32 = 0xFFFFFFFF
+CENTRE = 13.5
+BACKGROUND = -0.5
+MAX_SHIFT = 8.0                 # pixels
+MAX_ROTATION = 180.0            # degrees
+
+
+class Ranges(NamedTuple):
+    max_shift: float            # T, pixels
+    max_rotation: float         # R, degrees
+    max_scale: float            # S
+
+
+def seed_mix(seed: int, rank: int) -> int:
+    """The per-replica key of the draws (constants distinct from models/lenet.py's ``dropout_seed_mix``)."""
+    return (seed * 0x2C1B3C6D + rank * 0x297A2D39 + 0x5BD1E995) & _M32
+
+
+def hash_mix(key, idx):
+    """csrc/common.cuh ``hash_mix`` on uint64 arrays (or ints) holding u32 values."""
+    x = (np.asarray(idx, dtype=np.uint64) * np.uint64(0x9E3779B1) + np.uint64(key)) & np.uint64(_M32)
+    x ^= x >> np.uint64(16)
+    x = (x * np.uint64(0x85EBCA6B)) & np.uint64(_M32)
+    x ^= x >> np.uint64(13)
+    x = (x * np.uint64(0xC2B2AE35)) & np.uint64(_M32)
+    x ^= x >> np.uint64(16)
+    return x
+
+
+def uniforms(mix: int, iteration: int, rows: int) -> np.ndarray:
+    """float64 ``[rows, 4]``: the draws ``u0..u3`` of rows ``0..rows-1`` at ``iteration`` (each a multiple of 2^-24 in
+    [0, 1), exact in fp32)."""
+    key = int(hash_mix(mix, int(iteration) & _M32))
+    idx = (np.arange(rows, dtype=np.uint64)[:, None] * np.uint64(4) + np.arange(4, dtype=np.uint64)[None, :]) \
+        & np.uint64(_M32)
+    return (hash_mix(key, idx) >> np.uint64(8)).astype(np.float64) * 2.0 ** -24
+
+
+def coefficients(u: np.ndarray, ranges: Ranges):
+    """``(a, b, tx, ty)``, float64 ``[rows]`` each, of the draws ``u`` ``[rows, 4]``."""
+    T, R, S = (float(v) for v in (ranges.max_shift, ranges.max_rotation, ranges.max_scale))
+    theta = R * math.pi / 180.0 * (2.0 * u[:, 0] - 1.0)
+    s = 1.0 + S * (2.0 * u[:, 1] - 1.0)
+    return np.cos(theta) / s, np.sin(theta) / s, T * (2.0 * u[:, 2] - 1.0), T * (2.0 * u[:, 3] - 1.0)
+
+
+def affine(theta, scale, tx, ty):
+    """``(a, b, tx, ty)`` of a rotation by ``theta`` (radians) and a zoom ``scale``, as float64 arrays."""
+    theta, scale = np.asarray(theta, dtype=np.float64), np.asarray(scale, dtype=np.float64)
+    return np.cos(theta) / scale, np.sin(theta) / scale, np.asarray(tx, np.float64), np.asarray(ty, np.float64)
+
+
+def warp(images: np.ndarray, a, b, tx, ty) -> np.ndarray:
+    """The float64 warp of ``images`` (``[rows, 28, 28]`` or ``[rows, 784]``, row-major y, x) with per-row coefficients;
+    returns float64 ``[rows, 28, 28]``."""
+    img = np.asarray(images, dtype=np.float64).reshape(-1, 28, 28)
+    n = img.shape[0]
+    a, b, tx, ty = (np.broadcast_to(np.asarray(v, dtype=np.float64), (n,))[:, None, None] for v in (a, b, tx, ty))
+    y, x = np.meshgrid(np.arange(28, dtype=np.float64), np.arange(28, dtype=np.float64), indexing="ij")
+    dx, dy = x[None] - CENTRE - tx, y[None] - CENTRE - ty
+    sx = CENTRE + a * dx + b * dy
+    sy = CENTRE - b * dx + a * dy
+    x0, y0 = np.floor(sx), np.floor(sy)
+    fx, fy = sx - x0, sy - y0
+    pad = np.pad(img, ((0, 0), (1, 1), (1, 1)), constant_values=BACKGROUND)     # index 0 and 29: background
+
+    def tap(yy, xx):
+        inside = (yy >= 0) & (yy <= 27) & (xx >= 0) & (xx <= 27)
+        yi = np.where(inside, yy, -1).astype(np.int64) + 1
+        xi = np.where(inside, xx, -1).astype(np.int64) + 1
+        return pad[np.arange(n)[:, None, None], yi, xi]
+
+    v00, v01, v10, v11 = tap(y0, x0), tap(y0, x0 + 1), tap(y0 + 1, x0), tap(y0 + 1, x0 + 1)
+    return (1.0 - fy) * ((1.0 - fx) * v00 + fx * v01) + fy * ((1.0 - fx) * v10 + fx * v11)
+
+
+def augment_batch(images: np.ndarray, mix: int, iteration: int, ranges: Ranges) -> np.ndarray:
+    """The augmented batch (float64 warp from the float64 coefficients, rounded to fp32), in the shape of ``images``."""
+    img = np.asarray(images)
+    u = uniforms(mix, iteration, img.shape[0])
+    return warp(img, *coefficients(u, ranges)).astype(np.float32).reshape(img.shape)
+
+
+def check_ranges(ranges: Ranges) -> None:
+    """Raises ValueError unless every range is finite and within bounds."""
+    for name, v, hi, closed in (("--augment_max_shift", ranges.max_shift, MAX_SHIFT, True),
+                                ("--augment_max_rotation", ranges.max_rotation, MAX_ROTATION, True),
+                                ("--augment_max_scale", ranges.max_scale, 1.0, False)):
+        v = float(v)
+        if not math.isfinite(v) or v < 0.0 or (v > hi if closed else v >= hi):
+            raise ValueError("%s must be finite and lie in [0, %g%s (0 = off), got %r" % (name, hi, "]" if closed else ")", v))
+
+
+def from_flags(flags) -> Optional[Ranges]:
+    """The three ranges, or None when augmentation is off (all 0).  Raises ValueError on a value out of range."""
+    r = Ranges(*(float(getattr(flags, "augment_" + k, 0.0) or 0.0) for k in ("max_shift", "max_rotation", "max_scale")))
+    check_ranges(r)
+    return r if any(r) else None
+
+
+def check_flags(flags) -> None:
+    """The augmentation flags, checked before any device work starts."""
+    from_flags(flags)
+
+
+def describe(r: Ranges) -> str:
+    return "shift up to %g px, rotation up to %g degrees, zoom in [%g, %g]" % (r.max_shift, r.max_rotation,
+                                                                             1.0 - r.max_scale, 1.0 + r.max_scale)

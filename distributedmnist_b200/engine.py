@@ -24,7 +24,7 @@ from typing import Callable, Optional, Tuple
 import numpy as np
 import torch
 
-from . import best
+from . import augment, best
 from . import moving_average as ema
 from . import weight_decay
 from .models import ModelSpec, dropout_keep_mask, dropout_seed_mix, get_model, loss_and_accuracy
@@ -116,9 +116,35 @@ class TorchEngine(ComputeEngine):
         :meth:`loss_acc` reports includes the term."""
         self._decay = float(lam)
 
+    # ---- random affine augmentation (see augment.py) ----------------------------------------------------------------------
+    _aug = None                    # (augment.Ranges, seed mix)
+    _aug_images: Optional[torch.Tensor] = None
+
+    def arm_augment(self, max_shift: float, max_rotation: float, max_scale: float, start_iteration: int = 0) -> None:
+        """Augment every training batch from the next :meth:`forward_backward` on, its first draws those of iteration
+        ``start_iteration``; all three ranges 0 turns it off.  The same transform and draws as the sm_90a kernel, by the
+        float64 warp rounded to fp32."""
+        r = augment.Ranges(float(max_shift), float(max_rotation), float(max_scale))
+        augment.check_ranges(r)
+        self._aug = (r, augment.seed_mix(self.seed, self.rank)) if any(r) else None
+        self._aug_iteration = int(start_iteration) & 0xFFFFFFFF
+
+    def augment_iteration(self) -> int:
+        return self._aug_iteration
+
+    def augmented_batch(self) -> Optional[torch.Tensor]:
+        """The images the last augmented step read (None when augmentation is off)."""
+        return None if self._aug is None else self._aug_images
+
     def forward_backward(self, step: int) -> None:
+        images = self._images
+        if self._aug is not None:
+            r, mix = self._aug
+            out = augment.augment_batch(images.detach().cpu().numpy(), mix, self._aug_iteration, r)
+            images = self._aug_images = torch.from_numpy(out).to(self.device)
+            self._aug_iteration = (self._aug_iteration + 1) & 0xFFFFFFFF
         p = self.params.detach().requires_grad_(True)
-        logits = self._logits(p, self._images, True, step)
+        logits = self._logits(p, images, True, step)
         loss, acc = loss_and_accuracy(logits, self._labels)
         if self._decay:
             views = self.spec.views(p)

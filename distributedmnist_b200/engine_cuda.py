@@ -32,7 +32,7 @@ from typing import Optional, Tuple
 import numpy as np
 import torch
 
-from . import early_stopping, lr_plateau, weight_decay
+from . import augment, early_stopping, lr_plateau, weight_decay
 from .best import BEST_CORRECT_WORD, BEST_EXAMPLES_WORD, BEST_STEP_WORD, BEST_VALID_WORD
 from .early_stopping import PAT_BASELINE_WORD, PAT_BEST_STEP_WORD, PAT_BEST_WORD, PAT_SINCE_WORD, PAT_TRIGGER_WORD
 from .lr_plateau import PL_BASELINE_WORD, PL_BEST_WORD, PL_CUTS_WORD, PL_SINCE_WORD, PL_TRIGGER_WORD
@@ -133,6 +133,7 @@ class _CudaEngine(ComputeEngine):
         self.device = dev = backend.ctx.device
         self.spec = spec
         self.batch_size = B = batch_size
+        self.seed = seed
         self.use_graph = use_graph
         self.params = backend.allocate(spec.arena_numel)
         self.params.copy_(spec.init_flat(seed).to(dev))
@@ -410,6 +411,52 @@ class _CudaEngine(ComputeEngine):
         if float(lam) != 0.0:
             raise ValueError("--weight_decay on the GPU path is implemented for lenet, not --model=%s" % self.spec.name)
 
+    # ---- random affine augmentation (see augment.py, csrc/augment.cu) ---------------------------------------------------
+    # With augmentation armed, every training step starts (after the cdf start stamp) with augment_affine, which warps the
+    # input slot's images into _aug_images; every reader of the step's training images reads that buffer instead.  The
+    # step graphs replay one after another on the training stream, so one buffer serves both slots.  The iteration word
+    # _aug_counter[0] is advanced by the kernel itself; _aug_counter[1] is its ticket.  Evaluation never augments.
+    _aug = None                    # (augment.Ranges, seed mix), see arm_augment
+
+    def arm_augment(self, max_shift: float, max_rotation: float, max_scale: float, start_iteration: int = 0) -> None:
+        """Augment every training step from the next one on, its first draws those of iteration ``start_iteration`` (a
+        restarted run: the restored global step).  All three ranges 0 turns augmentation off.  Re-captures the step
+        graphs."""
+        r = augment.Ranges(float(max_shift), float(max_rotation), float(max_scale))
+        augment.check_ranges(r)
+        self._leave_native_runner()
+        torch.cuda.synchronize()
+        if any(r):
+            if getattr(self, "_aug_images", None) is None:
+                self._aug_images = torch.zeros(self.batch_size, 784, dtype=torch.float32, device=self.device)
+                self._aug_counter = torch.zeros(2, dtype=torch.int32, device=self.device)
+            words = np.array([int(start_iteration) & 0xFFFFFFFF, 0], dtype=np.uint32).view(np.int32)
+            self._aug_counter.copy_(torch.from_numpy(words))
+            self._aug = (r, augment.seed_mix(self.seed, self.backend.ctx.rank))
+        else:
+            self._aug = None
+        self._graphs = [None, None]
+        torch.cuda.synchronize()
+
+    def _launch_augment(self, slot: int) -> torch.Tensor:
+        """augment_affine on the current stream: slot ``slot``'s images -> the augmented buffer, in the slot's shape."""
+        r, mix = self._aug
+        self.lib.dm_augment_affine(self.images[slot], self._aug_images, self.batch_size, self._aug_counter, mix,
+                                   r.max_shift, r.max_rotation, r.max_scale, None, stream_ptr())
+        return self._aug_images.view(self.images[slot].shape)
+
+    def augment_iteration(self) -> int:
+        """The iteration whose draws the next augmented step uses (synchronises the device)."""
+        torch.cuda.synchronize()
+        return int(self._aug_counter[0].item()) & 0xFFFFFFFF
+
+    def augmented_batch(self) -> Optional[torch.Tensor]:
+        """Copy of the images the last augmented step read, ``[B, 784]`` (None when augmentation is off)."""
+        if self._aug is None:
+            return None
+        torch.cuda.synchronize()
+        return self._aug_images.clone()
+
     def params_updated(self) -> None:
         """Parameters were written from the host (init / restore): refresh the bf16 shadow."""
         self.backend.refresh_shadow(self.params)
@@ -441,8 +488,11 @@ class _CudaEngine(ComputeEngine):
         if self.use_graph:
             key = s
             if self._graphs[key] is None or self._graphs[key][1] != with_sync:
+                counter = self._aug_counter.clone() if self._aug is not None else None
                 self._launch_step(s, False)           # warm-up (gradients only): sets func attributes outside capture
                 torch.cuda.synchronize()
+                if counter is not None:
+                    self._aug_counter.copy_(counter)  # the warm-up is not an iteration: it must not consume draws
                 gr = torch.cuda.CUDAGraph()
                 cap = torch.cuda.Stream(device=self.device, priority=self._main_priority)
                 with _capture(gr, cap):
@@ -949,12 +999,16 @@ class CudaLeNetEngine(_CudaEngine):
                 self.backend.enqueue_straggler(self._straggler)
                 self._delay_in_chain = True
                 n += 1
+        images = self.images[slot]
+        if self._aug is not None:
+            images = self._launch_augment(slot)     # conv1_fwd and conv1_wgrad read the augmented batch
+            n += 1
         if interval:
             self._enqueue_iteration_begin()
             n += 2
         n += self._launch_zero()
-        n += self._launch_forward(self.images[slot], self.labels[slot], self.batch_size, True)
-        n += self._launch_backward(self.images[slot], self.batch_size, early_sync=bucketed)
+        n += self._launch_forward(images, self.labels[slot], self.batch_size, True)
+        n += self._launch_backward(images, self.batch_size, early_sync=bucketed)
         if bucketed:
             oa = self._opt_args
             e0, e1 = self._bucket_early
@@ -1536,13 +1590,17 @@ class CudaMlpEngine(_CudaEngine):
     def _launch_step(self, slot: int, with_sync: bool) -> None:
         B = self.batch_size
         n = 0
+        images = self.images[slot]
+        if self._aug is not None:
+            images = self._launch_augment(slot)     # dm_f32_to_bf16 reads the augmented batch
+            n += 1
         interval = with_sync and getattr(self, "_interval", False)
         if interval:
             self._enqueue_iteration_begin()
             n += 2
         bucketed = with_sync and self._bucket_v2 and not interval
         n += self._launch_zero()
-        n += self._forward(self.images[slot], self.labels[slot], B, True)
+        n += self._forward(images, self.labels[slot], B, True)
         n += self._backward(B, early_sync=bucketed)
         if bucketed:
             if self._straggler is not None:

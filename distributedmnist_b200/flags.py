@@ -298,6 +298,13 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
                                         "src/mnist.py:142-143): every replica differentiates CE + lambda * sum(v^2) / 2 over "
                                         "lenet's fc1/fc2 weights and biases (every layer of mlp2 / mlp3), and the logged "
                                         "training loss includes the term; 0 = off, else 0 < lambda < 1.  GPU path: lenet")
+    F.DEFINE_float("augment_max_shift", 0.0, "Random affine augmentation of the training images: translate each image by "
+                                             "tx, ty ~ U[-T, T] pixels; 0 <= T <= 8 (0 = no shift).  Augmentation is on "
+                                             "when any --augment_max_* is non-zero; evaluation is never augmented")
+    F.DEFINE_float("augment_max_rotation", 0.0, "Random affine augmentation: rotate each training image by theta ~ U[-R, R] "
+                                                "degrees about its centre; 0 <= R <= 180 (0 = no rotation)")
+    F.DEFINE_float("augment_max_scale", 0.0, "Random affine augmentation: zoom each training image by s ~ U[1-S, 1+S]; "
+                                             "0 <= S < 1 (0 = no zoom)")
     return F
 
 

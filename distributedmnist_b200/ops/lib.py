@@ -50,6 +50,8 @@ def _signatures() -> dict:
     f, d, s = ctypes.c_float, ctypes.c_double, ctypes.c_char_p
     S, V = STATUS, VALUE
     return {
+        # augment.cu
+        "dm_augment_affine": (S, i, [P, P, i, P, u, d, d, d, P, P]),
         # batch_gather.cu
         "dm_gather_batch": (S, i, [P, P, P, i, P, P]),
         # conv1_tc.cu, conv2_tc.cu

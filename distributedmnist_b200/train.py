@@ -31,7 +31,7 @@ from typing import Dict, Optional
 import numpy as np
 import torch
 
-from . import best, early_stopping, lr_plateau, moving_average, weight_decay
+from . import augment, best, early_stopping, lr_plateau, moving_average, weight_decay
 from .best import BEST_DIR, BEST_JSON
 from .checkpoint import Saver
 from .early_stopping import EARLY_STOPPING_JSON
@@ -623,6 +623,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     check_moving_average_flags(flags, ctx, num_replicas_to_aggregate)
     check_device_data_flags(flags, ctx, dataset)
     weight_decay.check_flags(flags, ctx)
+    aug_ranges = augment.from_flags(flags)
     device_data = bool(getattr(flags, "device_data", False))
     target = float(getattr(flags, "target_accuracy", 0.0) or 0.0)
     patience = int(getattr(flags, "early_stopping_patience", 0) or 0)
@@ -683,6 +684,12 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             backend.set_global_step(restored_step)
     if hasattr(engine, "params_updated"):
         engine.params_updated()
+    if aug_ranges is not None:
+        # every replica, after attach_optimizer: each training iteration draws from its own counter, which starts at the
+        # restored global step so that a restarted run does not replay the draws of its first steps
+        engine.arm_augment(*aug_ranges, start_iteration=restored_step)
+        log.info("Random affine augmentation of the training images: %s, draws from iteration %d; evaluation is not "
+                 "augmented" % (augment.describe(aug_ranges), restored_step))
     if ema_decay:
         # the chief's average starts from the restored averages, else from the (initial or restored) weights; from here on
         # every global step ends with its update (GPU path: a node at the end of the chief's step graph)
