@@ -14,8 +14,10 @@ The transform, defined here once (csrc/augment.cu computes the same one in fp32 
   ``dx = x - c - tx``, ``dy = y - c - ty``.  A tap outside ``[0, 27]^2`` reads the background ``BACKGROUND = -0.5``, the
   value of a zero pixel after data.py's ``(x - 127.5) / 255`` scaling.
 
-``i`` counts the replica's training iterations, starting at the restored global step, so two iterations never share
-draws and a restarted run does not replay those of its first steps.  Nothing enters the checkpoint.
+``i`` counts the replica's training iterations, so two iterations of one run never share draws.  A restarted run starts
+it past the iterations that went into the restored global step (:func:`start_iteration`), so a one-replica run does
+not replay the draws of the steps it restored; a multi-replica K > N run or an interval run can repeat some (see
+there).  Nothing enters the checkpoint.
 
 The numpy hash here is exact (integer arithmetic); :func:`warp` is the float64 warp.  The torch engine applies
 :func:`augment_batch`; the tests compare the kernel's draws and pixels against both.
@@ -32,6 +34,7 @@ CENTRE = 13.5
 BACKGROUND = -0.5
 MAX_SHIFT = 8.0                 # pixels
 MAX_ROTATION = 180.0            # degrees
+RANK_MIX = 0x297A2D39           # seed_mix(seed, r + 1) = seed_mix(seed, r) + RANK_MIX (mod 2^32)
 
 
 class Ranges(NamedTuple):
@@ -42,7 +45,7 @@ class Ranges(NamedTuple):
 
 def seed_mix(seed: int, rank: int) -> int:
     """The per-replica key of the draws (constants distinct from models/lenet.py's ``dropout_seed_mix``)."""
-    return (seed * 0x2C1B3C6D + rank * 0x297A2D39 + 0x5BD1E995) & _M32
+    return (seed * 0x2C1B3C6D + rank * RANK_MIX + 0x5BD1E995) & _M32
 
 
 def hash_mix(key, idx):
@@ -79,16 +82,17 @@ def affine(theta, scale, tx, ty):
     return np.cos(theta) / scale, np.sin(theta) / scale, np.asarray(tx, np.float64), np.asarray(ty, np.float64)
 
 
-def warp(images: np.ndarray, a, b, tx, ty) -> np.ndarray:
+def warp(images: np.ndarray, a, b, tx, ty, centre: float = CENTRE) -> np.ndarray:
     """The float64 warp of ``images`` (``[rows, 28, 28]`` or ``[rows, 784]``, row-major y, x) with per-row coefficients;
-    returns float64 ``[rows, 28, 28]``."""
+    returns float64 ``[rows, 28, 28]``.  ``centre``: the transform's is ``CENTRE`` (the tests warp about others to show
+    that their bounds tell the two apart)."""
     img = np.asarray(images, dtype=np.float64).reshape(-1, 28, 28)
     n = img.shape[0]
     a, b, tx, ty = (np.broadcast_to(np.asarray(v, dtype=np.float64), (n,))[:, None, None] for v in (a, b, tx, ty))
     y, x = np.meshgrid(np.arange(28, dtype=np.float64), np.arange(28, dtype=np.float64), indexing="ij")
-    dx, dy = x[None] - CENTRE - tx, y[None] - CENTRE - ty
-    sx = CENTRE + a * dx + b * dy
-    sy = CENTRE - b * dx + a * dy
+    dx, dy = x[None] - centre - tx, y[None] - centre - ty
+    sx = centre + a * dx + b * dy
+    sy = centre - b * dx + a * dy
     x0, y0 = np.floor(sx), np.floor(sy)
     fx, fy = sx - x0, sy - y0
     pad = np.pad(img, ((0, 0), (1, 1), (1, 1)), constant_values=BACKGROUND)     # index 0 and 29: background
@@ -108,6 +112,26 @@ def augment_batch(images: np.ndarray, mix: int, iteration: int, ranges: Ranges) 
     img = np.asarray(images)
     u = uniforms(mix, iteration, img.shape[0])
     return warp(img, *coefficients(u, ranges)).astype(np.float32).reshape(img.shape)
+
+
+def start_iteration(restored_step: int, count_triggered: bool, k: int, n: int) -> int:
+    """The first iteration a run restored at global step ``restored_step`` draws from (u32).
+
+    A synchronous run with K <= N gradients per update (``count_triggered``: mode A; ``k``, ``n``: K and the number of
+    replicas) computes at most one iteration per replica per global step, so its replicas used iterations below the
+    restored step.  With K > N each step commits once K gradients computed on its weights are accumulated, and the start
+    is ``k * restored_step``.  On one replica that is exact: every step takes exactly K iterations.
+
+    With K > N on more than one replica it is not a bound.  A replica counts at most K iterations of a step (the close
+    that brings its own count to K sees the sum reach K, so the step commits).  But once another replica has committed
+    the step, this one keeps computing iterations on the step's weights until the committer's pushes have landed
+    (``iv_adopt`` waits for the ``done`` flag), and the gate drops each of them; each still advances the counter.  How
+    many such stale iterations run depends on timing, not on the global step, so a restarted multi-replica K > N run can
+    repeat some draws of the run it restored.
+
+    Interval and cdf runs start at the restored step.  An interval replica's iteration count follows a wall-clock
+    deadline and is not a function of the global step either, so a restarted interval run can repeat draws too."""
+    return (int(restored_step) * (int(k) if count_triggered and k > n else 1)) & _M32
 
 
 def check_ranges(ranges: Ranges) -> None:

@@ -420,8 +420,8 @@ class _CudaEngine(ComputeEngine):
 
     def arm_augment(self, max_shift: float, max_rotation: float, max_scale: float, start_iteration: int = 0) -> None:
         """Augment every training step from the next one on, its first draws those of iteration ``start_iteration`` (a
-        restarted run: the restored global step).  All three ranges 0 turns augmentation off.  Re-captures the step
-        graphs."""
+        restarted run: ``augment.start_iteration`` of the restored global step).  All three ranges 0 turns augmentation
+        off.  Re-captures the step graphs."""
         r = augment.Ranges(float(max_shift), float(max_rotation), float(max_scale))
         augment.check_ranges(r)
         self._leave_native_runner()

@@ -786,6 +786,81 @@ def check_weight_decay_loss(n: int, seed: int = 20, lams: Sequence[float] = DECA
     return res
 
 
+# ---- random affine augmentation (augment.py, csrc/augment.cu) ---------------------------------------------------------
+AUG_U = 2.0 ** -24
+AUG_PREMISE_ROWS = 256         # rows the premise checks of augment_results warp (a large batch's would only cost time)
+
+
+def augment_pixel_bound(coef, coef_ulps: int = 0) -> np.ndarray:
+    """Per-pixel bound on |augment_affine - float64 warp of the fp32 coefficients ``coef``| ([B, 4]: a, b, tx, ty),
+    float64 [B, 784].
+
+    The kernel computes dx = fl(xc - tx) (xc = x - 13.5 exact), t = fma(b, dy, 13.5), sx = fma(a, dx, t) and likewise sy,
+    each with one rounding, so with u = 2^-24: |dx_f - dx| <= u |dx|, and
+        |sx_f - sx| <= |a| u |dx| + |b| u |dy| + u |t| + u |sx|   (to first order in u; the factor 1.001 covers the rest)
+    and the same for sy with (a, -b).  Clamping sx, sy to [-2, 29] is 1-Lipschitz and changes nothing where a tap could
+    be inside the image.  Bilinear interpolation with the background -0.5 is continuous in (sx, sy) and, for pixel values
+    in [-0.5, 0.5], Lipschitz with constant <= 1 per axis (each slope is a difference of two such values), also across
+    cell boundaries, so the sample point's error costs at most |sx_f - sx| + |sy_f - sy|.  The blend top = fma(fx, v01 -
+    v00, v00), bot likewise, out = fma(fy, bot - top, top) with fx, fy exact adds at most 3u (|v| <= 0.5: each difference
+    is rounded to within u/2, each fma to within u/4, and the errors of top and bot enter out with weights summing to 1);
+    4u is used.  The float64 reference itself is exact to ~1e-15.
+
+    ``coef_ulps``: the kernel's coefficients may each differ from ``coef`` by that many fp32 ulps (<= 2^-23 |c| each):
+    its double ``sincos`` and numpy's may round to different fp32 neighbours near a tie.  Since sx = c + a dx + b dy with
+    dx = x - c - tx, a change of e |a|, e |b|, e |tx|, e |ty| moves sx by at most e (|a| (|dx| + |tx|) + |b| (|dy| + |ty|))
+    and sy by e (|b| (|dx| + |tx|) + |a| (|dy| + |ty|)), which the same Lipschitz argument adds to the bound."""
+    a, b, tx, ty = (np.asarray(coef, dtype=np.float64)[:, k][:, None] for k in range(4))
+    y, x = np.divmod(np.arange(784, dtype=np.float64), 28)
+    dx, dy = x[None] - 13.5 - tx, y[None] - 13.5 - ty
+    tsx, tsy = b * dy + 13.5, -b * dx + 13.5
+    sx, sy = a * dx + tsx, a * dy + tsy
+    bsx = AUG_U * (np.abs(a * dx) + np.abs(b * dy) + np.abs(tsx) + np.abs(sx))
+    bsy = AUG_U * (np.abs(a * dy) + np.abs(b * dx) + np.abs(tsy) + np.abs(sy))
+    if coef_ulps:
+        e = coef_ulps * 2.0 ** -23
+        ax, by = np.abs(dx) + np.abs(tx), np.abs(dy) + np.abs(ty)
+        bsx = bsx + e * (np.abs(a) * ax + np.abs(b) * by)
+        bsy = bsy + e * (np.abs(b) * ax + np.abs(a) * by)
+    return 1.001 * (bsx + bsy) + 4 * AUG_U + 1e-12
+
+
+def augment_coefficients(mix: int, iteration: int, B: int, ranges) -> np.ndarray:
+    """[B, 4] (a, b, tx, ty) of rows 0..B-1 at ``iteration``: the float64 coefficients rounded to fp32, as float64."""
+    from .. import augment as AU
+    c = np.stack(AU.coefficients(AU.uniforms(mix, iteration, B), ranges), axis=1)
+    return c.astype(np.float32).astype(np.float64)
+
+
+def augment_results(tag: str, fed, got, mix: int, iteration: int, ranges) -> List[Result]:
+    """One augmented step's buffer ``got`` [B, 784] against ``augment.warp`` of the batch it was ``fed`` (fp32, [B, 784]
+    or [B, 28, 28], values in [-0.5, 0.5]) with the draws of ``iteration`` under ``mix``, the coefficients rounded to fp32,
+    within :func:`augment_pixel_bound` widened by one ulp of each coefficient.
+
+    Premise: the warps of iterations ``iteration`` +- 1, of the next rank's mix and about the centre 14.0 each differ from
+    the reference by more than the bound on some pixel of the first ``AUG_PREMISE_ROWS`` rows, so a step that drew from a
+    neighbouring iteration, used another replica's key or shifted the centre by half a pixel fails the check."""
+    from .. import augment as AU
+    x = (fed.detach().cpu().numpy() if torch.is_tensor(fed) else np.asarray(fed)).astype(np.float64)
+    B = x.shape[0]
+    x = x.reshape(B, 784)
+    c = augment_coefficients(mix, iteration, B, ranges)
+    want = AU.warp(x, *c.T).reshape(B, 784)
+    bound = augment_pixel_bound(c, coef_ulps=1)
+    g = got.detach().reshape(B, 784)
+    res = R.cmp_bound(tag, g, torch.from_numpy(want).to(g.device), torch.from_numpy(bound).to(g.device))
+    n = min(B, AUG_PREMISE_ROWS)
+    xs = x[:n]
+    alts = (("iteration_minus_1", AU.warp(xs, *augment_coefficients(mix, iteration - 1, n, ranges).T)),
+            ("iteration_plus_1", AU.warp(xs, *augment_coefficients(mix, iteration + 1, n, ranges).T)),
+            ("next_rank", AU.warp(xs, *augment_coefficients((mix + AU.RANK_MIX) & 0xFFFFFFFF, iteration, n, ranges).T)),
+            ("centre_14", AU.warp(xs, *c[:n].T, centre=14.0)))
+    for name, alt in alts:
+        seen = bool((np.abs(alt.reshape(n, 784) - want[:n]) > bound[:n]).any())
+        res.append(("%s.premise.%s_detectable" % (tag, name), 0.0 if seen else 1.0, 0.0))
+    return res
+
+
 def fc1_dgrad_results(tag: str, kind: str, dh, w1, code, dy, gb) -> List[Result]:
     """fc1_dgrad_unpool's dy2 [B,14,14,64] and conv2 bias gradient from dh, the bf16 weights w1 and the pool2 codes."""
     rdy, rgb = R.fc1_dgrad_unpool(dh, w1, code)

@@ -7,7 +7,10 @@ bounds the kernel checks use (``ops/selfcheck.py``):
 
 * each stage from its recorded inputs, on the weights the previous step committed (the initial arena for the first);
   the bf16 shadow a step reads is RNE of those weights, the dropout mask the one of the epoch word the step read;
-* the update bit for bit against ``ops/aggrefs.py``, and the recorded shadow as RNE of the recorded weights.
+* the update bit for bit against ``ops/aggrefs.py``, and the recorded shadow as RNE of the recorded weights;
+* with random affine augmentation armed, the recorded augmented buffer against the float64 warp of the fed batch with
+  the draws of the step's own iteration, the iteration counter after every step, and every reader of the images
+  (conv1 forward and wgrad, the MLP's x16) against that step's recorded buffer.
 
 The input slots are not recorded: the copy stream may refill a slot as soon as the step that read it is done.  The caller
 passes what it fed each step, so a step that computed on another batch fails its stage checks.
@@ -39,6 +42,8 @@ class StepRecorder:
     def __init__(self, eng):
         self.eng = eng
         self.init = dict(params=eng.params.clone(), shadow=eng.shadow.clone())
+        if getattr(eng, "_aug", None) is not None:
+            self.init["aug_counter"] = eng._aug_counter.clone()
         self.records: List[Dict[str, object]] = []
 
     def record(self) -> None:
@@ -52,15 +57,20 @@ class StepRecorder:
             r["g16"] = e._g16_view.clone()
         if getattr(e, "_decay", 0.0):
             r["decay_ws"] = e._decay_ws.clone()         # the W^2 partials of both weight-gradient kernels, then R
+        if getattr(e, "_aug", None) is not None:        # the next step's augment_affine overwrites both
+            r["aug_images"] = e._aug_images.clone()
+            r["aug_counter"] = e._aug_counter.clone()
         self.records.append(r)
 
 
-def update_of(eng, sched, step0: int) -> dict:
+def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
     """How ``eng`` applies its gradients: ``mode`` "fused" (fused_sync_sgd), "bucket" (the bf16-wire bucketed kernels)
     or "kgtn" (K > N: every k-th iteration commits), the schedule and the global step of the first step.  ``drop``:
     (seed, keep probability) of the drop-connect mask the fused kernel applies, None without it.  With a cut table armed
     (``arm_lr_cuts``), ``sched`` must name the same cuts (raises ValueError otherwise): the step sizes are then those of
-    the schedule with the cuts (synchronises the device to read the table)."""
+    the schedule with the cuts (synchronises the device to read the table).  ``aug``: (ranges, seed mix) of the armed
+    augmentation, None without it; ``aug_start`` the iteration the run's first step draws from (see
+    :func:`augment_stage_results`)."""
     be = eng.backend
     e0, e1 = eng._bucket_early
     mode = "kgtn" if eng._kgtn_k else ("bucket" if eng._bucket_v2 else "fused")
@@ -70,12 +80,45 @@ def update_of(eng, sched, step0: int) -> dict:
             raise ValueError("the engine's cut table holds %s, the schedule's cuts are %s" % (table, sched.cuts))
     return dict(mode=mode, sched=sched, step0=step0, k=max(eng._kgtn_k, 1), early=(e0, e1),
                 late_bf16=A.late_bucket_rounds_bf16(eng.spec.arena_numel, e1 - e0, be.late_ll, be.late_bf16),
-                drop=(be.drop_seed, be.drop_keep) if be.drop_keep > 0.0 else None)
+                drop=(be.drop_seed, be.drop_keep) if be.drop_keep > 0.0 else None,
+                aug=getattr(eng, "_aug", None), aug_start=int(aug_start))
 
 
 def epoch_of(upd: dict, t: int) -> int:
     """The epoch word step t reads: the global step, which with K > N stays put over the k iterations of a commit."""
     return upd["step0"] + t // upd["k"]
+
+
+def augment_iteration_of(upd: dict, t: int) -> int:
+    """The iteration whose draws step t uses: one per step in every mode, K > N included (the counter advances once per
+    iteration, unlike the epoch word), modulo 2^32."""
+    return (upd["aug_start"] + t) & 0xFFFFFFFF
+
+
+def _words(t: torch.Tensor) -> List[int]:
+    return [int(v) for v in t.detach().cpu().numpy().view("<u4")]
+
+
+def augment_stage_results(tag: str, init: dict, records: Sequence[dict], batches: Sequence, upd: dict) -> List[Result]:
+    """With augmentation armed (``upd["aug"]``): each step's recorded buffer against the warp of the batch it was fed
+    (:func:`selfcheck.augment_results`) with the draws of :func:`augment_iteration_of`, and the counter words: the
+    iteration before the first step, and after step t the next one with the ticket back at 0."""
+    if upd.get("aug") is None:
+        return []
+    ranges, mix = upd["aug"]
+    start = augment_iteration_of(upd, 0)
+    res: List[Result] = [(tag + ".init.aug_counter_differs", float(_words(init["aug_counter"]) != [start, 0]), 0.0)]
+    for t, (r, (x, _y)) in enumerate(zip(records, batches)):
+        it = augment_iteration_of(upd, t)
+        res += S.augment_results("%s.step%d.augment" % (tag, t), x, r["aug_images"], mix, it, ranges)
+        res.append(("%s.step%d.aug_counter_differs" % (tag, t),
+                    float(_words(r["aug_counter"]) != [(it + 1) & 0xFFFFFFFF, 0]), 0.0))
+    return res
+
+
+def _images_read(upd: dict, r: dict, fed):
+    """The images a step's image readers must have read: its recorded augmented buffer, or the batch it was fed."""
+    return r["aug_images"] if upd.get("aug") is not None else fed
 
 
 def _shadow_bits(t: torch.Tensor):
@@ -173,23 +216,25 @@ def lenet_step_results(tag: str, spec, r: dict, p, pb, images, labels, mask, kee
 def lenet_trajectory_results(tag: str, spec, init: dict, records: Sequence[dict], batches: Sequence, upd: dict,
                              seed: int, rank: int, keep_prob: float, lam: float = 0.0) -> List[Result]:
     """Every step of a LeNet run (``batches[t]`` = (images, labels) fed to step t) and every update.  ``lam``: the L2
-    weight decay the run was armed with (see :func:`lenet_step_results`)."""
-    res = update_results(tag, init, records, upd)
+    weight decay the run was armed with (see :func:`lenet_step_results`).  With augmentation armed, the augment stage is
+    checked against the fed batch and conv1 forward and conv1 wgrad against the step's recorded augmented images."""
+    res = update_results(tag, init, records, upd) + augment_stage_results(tag, init, records, batches, upd)
     for t, (r, (x, y)) in enumerate(zip(records, batches)):
         dev = r["a1"].device
         p, pb = _inputs(spec, init, records, t, dev)
         y = torch.as_tensor(y).to(dev)
         mask = dropout_keep_mask(dropout_seed_mix(seed, epoch_of(upd, t), rank), y.shape[0], 512, keep_prob, device=dev)
-        res += lenet_step_results("%s.step%d" % (tag, t), spec, r, p, pb, torch.as_tensor(x).to(dev), y, mask, keep_prob,
-                                  lam)
+        res += lenet_step_results("%s.step%d" % (tag, t), spec, r, p, pb, torch.as_tensor(_images_read(upd, r, x)).to(dev),
+                                  y, mask, keep_prob, lam)
     return res
 
 
 def mlp_trajectory_results(tag: str, spec, init: dict, records: Sequence[dict], batches: Sequence,
                            upd: dict) -> List[Result]:
     """Every step of an MLP run through :func:`selfcheck._mlp_step_results`, and every update.  With the bucketed
-    aggregation the early layer's weight gradient is the bf16 wire buffer."""
-    res = update_results(tag, init, records, upd)
+    aggregation the early layer's weight gradient is the bf16 wire buffer.  With augmentation armed, the augment stage is
+    checked against the fed batch and x16 against the step's recorded augmented images."""
+    res = update_results(tag, init, records, upd) + augment_stage_results(tag, init, records, batches, upd)
     n_layers = len(spec.params) // 2
     early = next(q.name for q in spec.params if q.offset == upd["early"][0])
     for t, (r, (x, y)) in enumerate(zip(records, batches)):
@@ -201,7 +246,8 @@ def mlp_trajectory_results(tag: str, spec, init: dict, records: Sequence[dict], 
         B = r["x16"].shape[0]
         rec = SimpleNamespace(p=p, pb=pb, g=g, n_layers=n_layers, batch_size=B, x16=r["x16"], h=r["h"], dh=r["dh"],
                               dl_pad=r["dl_pad"], d_loss_acc=r["loss_acc"], grads=r["grads"], spec=spec)
-        res += S._mlp_step_results("%s.step%d" % (tag, t), "rand", rec, torch.as_tensor(x).to(dev).reshape(B, 784),
+        res += S._mlp_step_results("%s.step%d" % (tag, t), "rand", rec,
+                                   torch.as_tensor(_images_read(upd, r, x)).to(dev).reshape(B, 784),
                                    torch.as_tensor(y).to(dev))
     return res
 

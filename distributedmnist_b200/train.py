@@ -685,11 +685,14 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     if hasattr(engine, "params_updated"):
         engine.params_updated()
     if aug_ranges is not None:
-        # every replica, after attach_optimizer: each training iteration draws from its own counter, which starts at the
-        # restored global step so that a restarted run does not replay the draws of its first steps
-        engine.arm_augment(*aug_ranges, start_iteration=restored_step)
+        # every replica, after attach_optimizer: each training iteration draws from its own counter, which starts past the
+        # iterations that went into the restored global step, so that a restarted one-replica run does not replay their
+        # draws (multi-replica K > N and interval runs can: see augment.start_iteration)
+        aug_start = augment.start_iteration(restored_step, isinstance(opt, SyncReplicasOptimizer),
+                                            num_replicas_to_aggregate, num_workers)
+        engine.arm_augment(*aug_ranges, start_iteration=aug_start)
         log.info("Random affine augmentation of the training images: %s, draws from iteration %d; evaluation is not "
-                 "augmented" % (augment.describe(aug_ranges), restored_step))
+                 "augmented" % (augment.describe(aug_ranges), aug_start))
     if ema_decay:
         # the chief's average starts from the restored averages, else from the (initial or restored) weights; from here on
         # every global step ends with its update (GPU path: a node at the end of the chief's step graph)

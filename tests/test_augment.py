@@ -108,6 +108,24 @@ def test_draws_do_not_depend_on_the_batch_size():
     assert np.array_equal(AU.uniforms(mix, 2 ** 32 + 4, 4), AU.uniforms(mix, 4, 4))   # the iteration is a u32
 
 
+def test_rank_mix_steps_to_the_next_rank():
+    for seed, rank in ((66478, 0), (7, 3), (2 ** 31 + 5, 6)):
+        assert (AU.seed_mix(seed, rank) + AU.RANK_MIX) & 0xFFFFFFFF == AU.seed_mix(seed, rank + 1)
+
+
+def test_restart_start_iteration():
+    """Past the iterations that went into the restored step: g with K <= N, K g with K > N (count-triggered runs only),
+    g for interval / cdf runs; a u32."""
+    assert AU.start_iteration(0, True, 4, 1) == 0
+    assert AU.start_iteration(13, True, 1, 1) == 13
+    assert AU.start_iteration(13, True, 6, 8) == 13                   # K < N: one iteration per global step
+    assert AU.start_iteration(13, True, 8, 8) == 13
+    assert AU.start_iteration(13, True, 4, 1) == 52
+    assert AU.start_iteration(13, True, 16, 8) == 208
+    assert AU.start_iteration(13, False, 16, 8) == 13                 # interval: not a function of the global step
+    assert AU.start_iteration(2 ** 31, True, 4, 1) == 0
+
+
 # ---- the warp ----------------------------------------------------------------------------------------------------------
 def test_zero_ranges_are_the_identity():
     img = _images(16).astype(np.float32)

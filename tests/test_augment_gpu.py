@@ -15,7 +15,6 @@ from distributedmnist_b200 import augment as AU
 
 pytestmark = pytest.mark.gpu
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-U = 2.0 ** -24
 
 
 def _lib():
@@ -61,26 +60,10 @@ def test_draws_equal_the_numpy_emulation(B):
 
 
 def _pixel_bound(p):
-    """Per-pixel bound on |kernel - float64 warp of the kernel's own fp32 coefficients|, [B, 784].
-
-    The kernel computes dx = fl(xc - tx) (xc = x - 13.5 exact), t = fma(b, dy, 13.5), sx = fma(a, dx, t) and likewise sy,
-    each with one rounding, so with u = 2^-24: |dx_f - dx| <= u |dx|, and
-        |sx_f - sx| <= |a| u |dx| + |b| u |dy| + u |t| + u |sx|   (to first order in u; the factor 1.001 covers the rest)
-    and the same for sy with (a, -b).  Clamping sx, sy to [-2, 29] is 1-Lipschitz and changes nothing where a tap could
-    be inside the image.  Bilinear interpolation with the background -0.5 is continuous in (sx, sy) and, for pixel values
-    in [-0.5, 0.5], Lipschitz with constant <= 1 per axis (each slope is a difference of two such values), also across
-    cell boundaries, so the sample point's error costs at most |sx_f - sx| + |sy_f - sy|.  The blend top = fma(fx, v01 -
-    v00, v00), bot likewise, out = fma(fy, bot - top, top) with fx, fy exact adds at most 3u (|v| <= 0.5: each difference
-    is rounded to within u/2, each fma to within u/4, and the errors of top and bot enter out with weights summing to 1);
-    4u is used.  The float64 reference itself is exact to ~1e-15."""
-    a, b, tx, ty = (p[:, k].astype(np.float64)[:, None] for k in range(4, 8))
-    y, x = np.divmod(np.arange(784, dtype=np.float64), 28)
-    dx, dy = x[None] - 13.5 - tx, y[None] - 13.5 - ty
-    tsx, tsy = b * dy + 13.5, -b * dx + 13.5
-    sx, sy = a * dx + tsx, a * dy + tsy
-    bsx = U * (np.abs(a * dx) + np.abs(b * dy) + np.abs(tsx) + np.abs(sx))
-    bsy = U * (np.abs(a * dy) + np.abs(b * dx) + np.abs(tsy) + np.abs(sy))
-    return 1.001 * (bsx + bsy) + 4 * U + 1e-12
+    """Per-pixel bound on |kernel - float64 warp of the kernel's own fp32 coefficients| (params_out columns 4..7),
+    [B, 784]: see ``selfcheck.augment_pixel_bound``."""
+    from distributedmnist_b200.ops.selfcheck import augment_pixel_bound
+    return augment_pixel_bound(p[:, 4:8])
 
 
 @pytest.mark.parametrize("r", [AU.Ranges(8.0, 180.0, 0.9), AU.Ranges(30.0, 10.0, 0.5), AU.Ranges(2.0, 15.0, 0.1),
@@ -103,6 +86,30 @@ def test_pixels_are_the_float64_warp_within_the_bound(r):
     if r.max_shift == 30.0:                         # shifts that move the whole image off: background everywhere
         full = np.all(got == AU.BACKGROUND, axis=1)
         assert full.sum() > 50 and np.array_equal(full, np.all(want == AU.BACKGROUND, axis=1))
+
+
+def _grid_edge_batches():
+    """The batch sizes where the grid logic changes: one row; around 4 CTAs per SM (grid = min(4 SMs, B)); 32 rows in
+    every CTA of 4 per SM and one row more, where the grid grows to ceil(B / 32); and 40000 rows."""
+    sms = int(_lib().dm_num_sms())
+    return [1, 4 * sms - 1, 4 * sms, 4 * sms + 1, 128 * sms, 128 * sms + 1, 40000]
+
+
+def test_grid_edges_draws_pixels_rows_and_counter():
+    """At each grid edge: the draws bit for bit, the pixels within the bound, every row of the NaN-filled output written,
+    and the counter advanced once with the ticket back at 0."""
+    r = AU.Ranges(8.0, 180.0, 0.5)
+    mix = AU.seed_mix(11, 1)
+    for B in _grid_edge_batches():
+        src = _images(B, 1000 + B)
+        it = 2 ** 32 - 1 if B % 2 else 4321
+        got, p, ctr = _launch(src.cuda(), mix, it, r)
+        assert np.array_equal(p[:, :4], AU.uniforms(mix, it, B).astype(np.float32)), B
+        assert not np.isnan(got).any(), (B, np.flatnonzero(np.isnan(got).any(axis=1))[:10])
+        want = AU.warp(src.numpy(), *(p[:, k].astype(np.float64) for k in range(4, 8))).reshape(B, 784)
+        err, bound = np.abs(got.astype(np.float64) - want), _pixel_bound(p)
+        assert np.all(err <= bound), (B, float((err / bound).max()))
+        assert ctr.tolist() == [(it + 1) & 0xFFFFFFFF, 0], (B, ctr)
 
 
 def test_argument_checks():
@@ -284,7 +291,8 @@ def test_evaluation_is_never_augmented():
     assert ev == eng.evaluate(vx, vy)
 
 
-def test_restart_draws_from_the_restored_step(tmp_path):
+def _train_twice(tmp_path, *extra):
+    """A 12-step lenet run with augmentation and its restart to 20 steps: (first log, restart log, restored step)."""
     train_dir = str(tmp_path / "train")
     env = dict(os.environ, CUDA_VISIBLE_DEVICES="0")
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
@@ -294,12 +302,24 @@ def test_restart_draws_from_the_restored_step(tmp_path):
         tr = subprocess.run([sys.executable, os.path.join(ROOT, "src", "mnist_distributed_train.py"), "--job_name=worker",
                              "--task_id=0", "--worker_hosts=localhost:1234", "--batch_size=128", "--max_steps=%d" % steps,
                              "--augment_max_shift=2", "--augment_max_rotation=10", "--save_interval_secs=1000",
-                             "--train_dir=" + train_dir], env=env, capture_output=True, text=True, timeout=600)
+                             "--train_dir=" + train_dir] + list(extra), env=env, capture_output=True, text=True,
+                            timeout=600)
         logs.append(tr.stdout + tr.stderr)
         assert tr.returncode == 0, logs[-1][-3000:]
     assert "draws from iteration 0;" in logs[0]
     m = re.search(r"Restored model from \S+ at step=(\d+)", logs[1])
     assert m and int(m.group(1)) > 0, logs[1][-2000:]
-    assert "draws from iteration %s;" % m.group(1) in logs[1]
     losses = [float(x) for x in re.findall(r"loss = ([0-9.]+),", logs[1])]
     assert losses and np.all(np.isfinite(losses))
+    return logs[0], logs[1], int(m.group(1))
+
+
+def test_restart_draws_from_the_restored_step(tmp_path):
+    _first, restart, g = _train_twice(tmp_path)
+    assert "draws from iteration %d;" % g in restart
+
+
+def test_restart_with_k4_draws_past_the_restored_iterations(tmp_path):
+    """K = 4 on one replica: the global step g the restart restores took iterations 0 .. 4g - 1, so it draws from 4g."""
+    _first, restart, g = _train_twice(tmp_path, "--num_replicas_to_aggregate=4")
+    assert "draws from iteration %d;" % (4 * g) in restart

@@ -121,6 +121,41 @@ def test_train_one_replica_k4(tmp_path, clean_flags):
         LearningRateSchedule.from_flags(FLAGS, ds.train.num_examples, 4).decay_steps
 
 
+def test_restarted_k4_run_draws_past_the_iterations_it_restored(tmp_path, clean_flags, caplog, monkeypatch):
+    """Random affine augmentation with K = 4 on one replica: a run restored at global step g used the draws of iterations
+    0 .. 4g - 1 (4 per step), so the restarted run draws from 4g on and no iteration's draws are used twice."""
+    from distributedmnist_b200.engine import TorchEngine
+    seen = []
+    fb = TorchEngine.forward_backward
+
+    def record_step(self, step):
+        fb(self, step)
+        seen[-1].append(self.augment_iteration() - 1)          # the iteration whose draws this step used
+
+    monkeypatch.setattr(TorchEngine, "forward_backward", record_step)
+    finals = []
+    for steps in (12, 20):
+        seen.append([])
+        caplog.clear()
+        FLAGS.reset()
+        FLAGS.parse(["--train_dir=%s" % (tmp_path / "train"), "--batch_size=32", "--max_steps=%d" % steps, "--model=mlp2",
+                     "--mlp_hidden=32", "--save_results_period=5", "--save_interval_secs=1000",
+                     "--initial_learning_rate=0.05", "--num_replicas_to_aggregate=4", "--augment_max_shift=2",
+                     "--augment_max_rotation=15", "--augment_max_scale=0.1"])
+        ctx = init_context(FLAGS, want_gpu=False)
+        ds = mnist_data.load_mnist(FLAGS.data_dir, worker_id=0, n_workers=1, seed=FLAGS.seed, synthetic=True,
+                                   synthetic_sizes=(256, 64))
+        res = train(ctx, ds.train, ds.validation, FLAGS)
+        finals.append(res["final_step"])
+        assert res["accepted"] == len(seen[-1])
+        start = 4 * finals[0] if steps == 20 else 0
+        assert any("draws from iteration %d;" % start in r.getMessage() for r in caplog.records), \
+            [r.getMessage() for r in caplog.records if "draws from" in r.getMessage()]
+    first, second = seen
+    assert finals == [13, 21] and first == list(range(52)) and second == list(range(52, 84))
+    assert not set(first) & set(second)
+
+
 GPU = SimpleNamespace(on_gpu=True, world_size=2)
 
 

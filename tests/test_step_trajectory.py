@@ -4,6 +4,7 @@ import numpy as np
 import pytest
 import torch
 
+from distributedmnist_b200 import augment as AU
 from distributedmnist_b200 import weight_decay as W
 from distributedmnist_b200.models import dropout_keep_mask, dropout_seed_mix, get_model
 from distributedmnist_b200.ops import aggrefs as A
@@ -16,6 +17,12 @@ SEED, RANK, KEEP = 5, 0, 0.5
 # a large step size, so that one step's update moves the bf16 shadow and the activations visibly
 SCHED = LearningRateSchedule(4.0, 1, 0.999)
 STEP0 = 3001
+# augmentation: draws from an iteration that is not STEP0 and wraps through 0 inside the run
+AUG_RANGES = AU.Ranges(3.0, 20.0, 0.15)
+AUG_START = 2 ** 32 - 3
+AUG_MIX = AU.seed_mix(SEED, RANK)
+AUG_FAULTS = ("aug_iteration_plus_1", "aug_keyed_by_epoch", "aug_other_rank", "conv1_reads_unaugmented",
+              "conv1_wgrad_reads_next_warp", "x16_from_fed", "counter_not_advanced")
 
 
 def _bf(x):
@@ -32,9 +39,9 @@ def _update(w, g):
     return lambda t: torch.from_numpy(A.fused_sync_step(A.f32(w), [A.f32(g)], 1, A.step_scale(SCHED, STEP0 + t, 1)))
 
 
-def _lenet_step(spec, params, x, y, mask, fault, prev, lam=0.0):
+def _lenet_step(spec, params, x, y, mask, fault, prev, lam=0.0, x_wgrad=None):
     """One LeNet step as the kernels store it.  ``fault``: "dgrad_post_update" runs fc1 dgrad on the updated shadow.
-    ``lam``: L2 weight decay (see :func:`_decay`)."""
+    ``lam``: L2 weight decay (see :func:`_decay`).  ``x_wgrad``: the images conv1 wgrad reads, if not ``x``."""
     B = x.shape[0]
     p, pb = spec.views(params), spec.views(params.to(BF))
     f1 = R.pool_fwd(R.conv5x5(x.to(BF)[..., None], p["conv1_weights"].to(BF)), p["conv1_biases"])
@@ -59,7 +66,7 @@ def _lenet_step(spec, params, x, y, mask, fault, prev, lam=0.0):
     g["conv2_biases"].copy_(gbc2)
     dx1 = _bf(R.conv5x5_dgrad(dy2, pb["conv2_weights"]))
     g["conv2_weights"].copy_(R.conv5x5_wgrad(a1, dy2))
-    gw1, gbc1 = R.conv1_wgrad(x.to(BF), dx1, code1)
+    gw1, gbc1 = R.conv1_wgrad((x if x_wgrad is None else x_wgrad).to(BF), dx1, code1)
     g["conv1_weights"].copy_(gw1.reshape(5, 5, 1, 32)), g["conv1_biases"].copy_(gbc1)
     la = torch.tensor([float(ref["loss"]), float(ref["acc"])], dtype=torch.float32)
     r = dict(a1=a1, code1=code1, a2=a2, code2=code2, h_part=h_part, dh=dh, h_act=h_act, dlogits=dlogits, dy2=dy2,
@@ -122,15 +129,44 @@ def _mlp_step(spec, params, x, y, fault, prev):
     return dict(x16=x16, h=hs, dh=dhs, dl_pad=dl_pad, grads=_ftz(grads), loss_acc=la)
 
 
-def _run(model, fault=None, steps=4, B=8, lam=0.0):
+def _counter(it):
+    """The augmentation counter words [iteration, ticket] as the engine stores them (int32)."""
+    return torch.from_numpy(np.array([it & 0xFFFFFFFF, 0], dtype=np.uint32).view(np.int32))
+
+
+def _augment(x, t, steps, batches, fault):
+    """The images augment_affine writes for step t, and those conv1 forward, conv1 wgrad and mlp x16 read: all the
+    same buffer unless ``fault`` (one of AUG_FAULTS) says otherwise."""
+    it, mix = AUG_START + t, AUG_MIX
+    if fault == "aug_iteration_plus_1":              # as if the graph capture's warm-up had consumed an iteration
+        it += 1
+    if fault == "aug_keyed_by_epoch":
+        it = STEP0 + t
+    if fault == "aug_other_rank":
+        mix = AU.seed_mix(SEED, RANK + 1)
+    xa = torch.from_numpy(AU.augment_batch(x.numpy(), mix, it, AUG_RANGES))
+    read = dict(fwd=xa, wgrad=xa, x16=xa)
+    if fault == "conv1_reads_unaugmented":
+        read["fwd"] = x
+    if fault == "conv1_wgrad_reads_next_warp" and t + 1 < steps:
+        read["wgrad"] = torch.from_numpy(AU.augment_batch(batches[t + 1][0].numpy(), mix, it + 1, AUG_RANGES))
+    if fault == "x16_from_fed":
+        read["x16"] = x
+    return xa, read
+
+
+def _run(model, fault=None, steps=4, B=8, lam=0.0, aug=False):
     """(spec, init, records, batches fed, update) of an emulated run with at most one seeded fault; ``lam``: L2 weight
-    decay (LeNet)."""
+    decay (LeNet); ``aug``: random affine augmentation from iteration AUG_START (on with any of AUG_FAULTS)."""
+    aug = aug or fault in AUG_FAULTS
     spec = get_model(model, 64)[0]
     gen = torch.Generator().manual_seed(11)
     shape = (B, 28, 28) if model == "lenet" else (B, 784)
     batches = [(torch.rand(*shape, generator=gen) - 0.5, torch.randint(0, 10, (B,), generator=gen)) for _ in range(steps)]
     params = spec.init_flat(SEED)
     init = dict(params=params.clone(), shadow=params.to(BF))
+    if aug:
+        init["aug_counter"] = _counter(AUG_START)
     records, prev = [], dict(t=0, grads=None, params=params.clone())
     for t in range(steps):
         x, y = batches[t]
@@ -138,25 +174,29 @@ def _run(model, fault=None, steps=4, B=8, lam=0.0):
             x, y = batches[t + 2]
         if fault == "slot1_reads_slot0" and t % 2 == 1:
             x, y = batches[t - 1]
+        xa, read = _augment(x, t, steps, batches, fault) if aug else (None, dict(fwd=x, wgrad=x, x16=x))
         prev["t"] = t
         if model == "lenet":
             e = STEP0 + t - (1 if fault == "mask_previous_epoch" and t > 0 else 0)
             mask = dropout_keep_mask(dropout_seed_mix(SEED, e, RANK), B, 512, KEEP)
-            r = _lenet_step(spec, params, x, y, mask, fault, prev, lam)
+            r = _lenet_step(spec, params, read["fwd"], y, mask, fault, prev, lam, x_wgrad=read["wgrad"])
         else:
-            r = _mlp_step(spec, params, x, y, fault, prev)
+            r = _mlp_step(spec, params, read["x16"], y, fault, prev)
         g = prev["grads"] if fault == "stale_gradient" and t > 0 else r["grads"]
         params = _update(params, g)(t)
         r.update(params=params.clone(), shadow=params.to(BF))
+        if aug:
+            r.update(aug_images=xa.reshape(B, 784), aug_counter=_counter(AUG_START + t + (fault != "counter_not_advanced")))
         records.append(r)
         prev["grads"] = r["grads"]
         prev["params"] = (init["params"] if t == 0 else records[t - 1]["params"]).clone()   # what step t read
-    upd = dict(mode="fused", sched=SCHED, step0=STEP0, k=1, early=(spec.param("fc1_weights").offset,) * 2, late_bf16=False)
+    upd = dict(mode="fused", sched=SCHED, step0=STEP0, k=1, early=(spec.param("fc1_weights").offset,) * 2, late_bf16=False,
+               aug=(AUG_RANGES, AUG_MIX) if aug else None, aug_start=AUG_START if aug else 0)
     return spec, init, records, batches, upd
 
 
-def _results(model, fault=None, lam=0.0):
-    spec, init, records, batches, upd = _run(model, fault, lam=lam)
+def _results(model, fault=None, lam=0.0, aug=False):
+    spec, init, records, batches, upd = _run(model, fault, lam=lam, aug=aug)
     if model == "lenet":
         return T.lenet_trajectory_results("lenet", spec, init, records, batches, upd, SEED, RANK, KEEP, lam)
     return T.mlp_trajectory_results("mlp3", spec, init, records, batches, upd)
@@ -251,3 +291,37 @@ def test_decayed_update_with_drop_connect_and_cuts():
     assert not T.failures(T.update_results("drop", init, recs, upd))
     assert T.failures(T.update_results("drop", init, recs, dict(upd, drop=None)))
     assert T.failures(T.update_results("drop", init, recs, dict(upd, sched=SCHED)))
+
+
+# ---- random affine augmentation ---------------------------------------------------------------------------------------
+@pytest.mark.parametrize("model", ["lenet", "mlp3"])
+def test_emulated_augmented_trajectory_passes(model):
+    """Augmented from iteration 2^32 - 3, so the counter wraps through 0 within the 4 steps: the augment stage, the
+    counter words and every stage that reads the images (conv1 forward and wgrad, mlp3's x16) against the recorded
+    augmented buffer pass, and each premise holds."""
+    res = _results(model, aug=True)
+    assert not T.failures(res), T.failures(res)
+    worst = T.worst_by_stage(model, res)
+    for stage in ("augment[err/bound]", "aug_counter_differs", "init.aug_counter_differs",
+                  "augment.premise.iteration_plus_1_detectable", "augment.premise.centre_14_detectable"):
+        assert stage in worst, (stage, sorted(worst))
+    assert all(0 <= v <= 1 for v in worst.values()), worst
+    assert sum(1 for n, _, _ in res if ".step3.augment" in n) == 5
+
+
+@pytest.mark.parametrize("model,fault,stage", [
+    ("lenet", "aug_iteration_plus_1", "step0.augment[err/bound]"),
+    ("lenet", "aug_keyed_by_epoch", "step0.augment[err/bound]"),
+    ("lenet", "aug_other_rank", "step0.augment[err/bound]"),
+    ("mlp3", "aug_iteration_plus_1", "step0.augment[err/bound]"),
+    ("lenet", "conv1_reads_unaugmented", "step0.conv1_fwd"),
+    ("lenet", "conv1_wgrad_reads_next_warp", "step0.conv1_wgrad"),
+    ("mlp3", "x16_from_fed", "step0.x16"),
+    ("lenet", "counter_not_advanced", "step0.aug_counter_differs"),
+])
+def test_seeded_augment_fault_fails(model, fault, stage):
+    """Each fault fails at its own stage, and only the stages it touches fail."""
+    bad = T.failures(_results(model, fault))
+    assert any(stage in n for n, _, _ in bad), (fault, bad[:10])
+    family = stage.split(".")[1].split("[")[0]
+    assert all(family in n for n, _, _ in bad), (fault, bad[:10])
