@@ -3,22 +3,24 @@
 //
 // K = 25 taps is too thin to be FLOP-relevant, but SIMT kernels sit on the fp32 FMA-pipe floor, so the thin
 // GEMMs move to wgmma anyway.  With C_in = 1 no TMA box can express the im2col operand (a K
-// step would be 2 bytes), so the operand is built in shared memory by software -- 36 input values per pooled
-// pixel -- in the 64-byte-swizzled layout TMA would write.
+// step would be 2 bytes), so the operands are built in shared memory by software, in the swizzled layouts TMA would
+// write.
 //
-// Tile = 128 consecutive POOLED pixels (flat index over batch x 14 x 14).  For each of the four positions p of the
-// 2x2 pooling window there is one im2col tile  A_p[128 pooled pixels][32 taps]  (taps 0-24 = the 5x5 window of conv
-// pixel (2ph + p/2, 2pw + p%2), tap 25 = 1.0, taps 26-31 = 0).  Read row-wise (ldmatrix) it is the forward A
-// (rows = M = pixels, K = taps); read transposed (ldmatrix.trans) it is the weight-gradient A (M = taps,
-// K = pixels): same bytes.
-//
-//   forward  D_p[pixel, co] = A_p * W[tap, co]   four m64n32 accumulators per warpgroup; every thread holds the
-//            same (pixel, channel) positions of all four, so the 2x2 max-pool is an in-thread max, fused with
-//            bias, ReLU and the argmax code.
-//   wgrad    D[tap, co] += A_p^T * G_p[pixel, co]   where G_p keeps a pooled gradient only where the forward pass
-//            selected position p and ReLU was active (pool/ReLU backward fused into the operand build); tap 25
-//            accumulates the bias gradient.  Accumulators stay in registers for the CTA's whole pixel range; the
-//            CTAs' partial sums are added up in a fixed order, so the gradient is the same to the bit in every run.
+//   forward  Tile = 128 consecutive POOLED pixels (flat index over batch x 14 x 14).  For each of the four positions p
+//            of the 2x2 pooling window there is one im2col tile  A_p[128 pooled pixels][32 taps]  (taps 0-24 = the 5x5
+//            window of conv pixel (2ph + p/2, 2pw + p%2), tap 25 = 1.0, taps 26-31 = 0; 64-byte swizzle), read
+//            row-wise with ldmatrix.  D_p[pixel, co] = A_p * W[tap, co]: four m64n32 accumulators per warpgroup; every
+//            thread holds the same (pixel, channel) positions of all four, so the 2x2 max-pool is an in-thread max,
+//            fused with bias, ReLU and the argmax code.
+//   wgrad    One row per pooled pixel P = (b, ph, pw): its 6x6 input patch X_P (input rows 2ph-2 .. 2ph+3, columns
+//            2pw-2 .. 2pw+3), element j = 6 r + c, then a 1.0 at j = 36 (0 for padding pixels past the batch), then
+//            zeros up to 64 bf16 = 128 B (128-byte swizzle).  The 5x5 window of position p = (dy, dx) lies inside the
+//            patch: tap (kh, kw) of position p is X_P[(dy + kh) 6 + dx + kw].  E[j, (p, co)] = sum_P X_P[j] G_P[p, co]
+//            with the patch tile read MN-major as A (M = j) and N = 128 = (p, co), where G_P keeps a pooled gradient
+//            only where the forward pass selected position p and ReLU was active (pool/ReLU backward fused into the
+//            operand build).  Each CTA folds E to dW[kh, kw, co] = sum_p E[(dy + kh) 6 + dx + kw, 32 p + co] and
+//            db[co] = sum_p E[36, 32 p + co] (p in order 0..3), and the CTAs' partial sums are added up in a fixed
+//            order, so the gradient is the same to the bit in every run.
 #include "common.cuh"
 #include "host_utils.h"
 
@@ -26,7 +28,8 @@ namespace dm {
 
 constexpr int C1T_FW_THREADS = 256;       // two warpgroups: operand builders, then MMA + epilogue
 constexpr int C1T_TILE = 128;             // pooled pixels per tile
-constexpr int C1T_AP_BYTES = 128 * 64;    // one A_p (or G_p) tile: 128 rows x 32 bf16
+constexpr int C1T_AP_BYTES = 128 * 64;    // one A_p tile: 128 rows x 32 bf16
+constexpr int C1T_ROW_BYTES = 128;        // one patch row of the weight gradient: 64 bf16
 
 struct ZeroRanges3 {
   float* ptr[3];
@@ -35,6 +38,8 @@ struct ZeroRanges3 {
 
 // 16-byte chunk `c` of 64-byte row `r` inside a 64B-swizzled tile (address bits [4,5] ^= bits [7,8])
 DMNIST_DEVICE uint32_t swz64(uint32_t r, uint32_t c) { return r * 64u + ((c ^ ((r >> 1) & 3u)) << 4); }
+// 16-byte chunk `c` of 128-byte row `r` inside a 128B-swizzled, 1024-aligned tile (address bits [4,7) ^= bits [7,10))
+DMNIST_DEVICE uint32_t swz128(uint32_t r, uint32_t c) { return r * 128u + ((c ^ (r & 7u)) << 4); }
 
 DMNIST_DEVICE void sts128(uint8_t* p, uint32_t a, uint32_t b, uint32_t c, uint32_t d) {
   *reinterpret_cast<uint4*>(p) = make_uint4(a, b, c, d);
@@ -76,7 +81,7 @@ DMNIST_DEVICE void load_patch_half(PatchRegs& pr, int h, long long P, long long 
   }
 }
 
-DMNIST_DEVICE void store_im2col_half(uint8_t* a_tiles, int m, int h, const PatchRegs& pr, int tile_bytes = C1T_AP_BYTES) {
+DMNIST_DEVICE void store_im2col_half(uint8_t* a_tiles, int m, int h, const PatchRegs& pr) {
 #pragma unroll
   for (int px = 0; px < 2; ++px) {
     uint32_t w[16];                                   // 32 taps as bf16 pairs
@@ -87,7 +92,7 @@ DMNIST_DEVICE void store_im2col_half(uint8_t* a_tiles, int m, int h, const Patch
       const float v1 = t1 < 25 ? pr.v[t1 / 5][px + t1 % 5] : (t1 == 25 ? pr.one : 0.f);
       w[j] = pack_bf16x2(v0, v1);
     }
-    uint8_t* tile = a_tiles + (2 * h + px) * tile_bytes;
+    uint8_t* tile = a_tiles + (2 * h + px) * C1T_AP_BYTES;
 #pragma unroll
     for (int c = 0; c < 4; ++c) sts128(tile + swz64(m, c), w[4 * c], w[4 * c + 1], w[4 * c + 2], w[4 * c + 3]);
   }
@@ -213,37 +218,87 @@ conv1_fwd_tc_kernel(const float* __restrict__ images,   // [B,28,28] fp32
   }
 }
 
+// Two threads build a patch row: half h = 0 writes chunks 0-3 (j 0..31), half h = 1 chunks 4-7 (j 32..35, the 1.0 and
+// zeros).  Loading and packing are separate steps, so the loads of the next tile are in flight while the current tile
+// is multiplied.
+template <int H>
+DMNIST_DEVICE void load_patch_row_half_t(float (&v)[32], long long P, long long total, const float* __restrict__ images) {
+  if (P < total) {
+    const int b = (int)(P / 196), pos = (int)(P - (long long)b * 196);
+    const int ph = pos / 14, pw = pos - ph * 14;
+    const float* img = images + (size_t)b * 784;
+#pragma unroll
+    for (int u = 0; u < 16; ++u) {
+      const int j = 32 * H + 2 * u;
+      if (j < 36) {
+        const int y = 2 * ph - 2 + j / 6, x = 2 * pw - 2 + j % 6;   // x even: the pair (x, x+1) is inside or outside as a whole
+        float2 t = make_float2(0.f, 0.f);
+        if (y >= 0 && y < 28 && x >= 0 && x < 28) t = __ldg(reinterpret_cast<const float2*>(img + y * 28 + x));
+        v[2 * u] = t.x;
+        v[2 * u + 1] = t.y;
+      } else {
+        v[2 * u] = j == 36 ? 1.f : 0.f;
+        v[2 * u + 1] = 0.f;
+      }
+    }
+  } else {
+#pragma unroll
+    for (int u = 0; u < 32; ++u) v[u] = 0.f;
+  }
+}
+
+DMNIST_DEVICE void load_patch_row_half(float (&v)[32], int h, long long P, long long total, const float* __restrict__ images) {
+  if (h == 0) load_patch_row_half_t<0>(v, P, total, images);
+  else load_patch_row_half_t<1>(v, P, total, images);
+}
+
+DMNIST_DEVICE void store_patch_row_half(uint8_t* tile, int m, int h, const float (&v)[32]) {
+#pragma unroll
+  for (int c = 0; c < 4; ++c)
+    sts128(tile + swz128(m, 4 * h + c), pack_bf16x2(v[8 * c], v[8 * c + 1]), pack_bf16x2(v[8 * c + 2], v[8 * c + 3]),
+           pack_bf16x2(v[8 * c + 4], v[8 * c + 5]), pack_bf16x2(v[8 * c + 6], v[8 * c + 7]));
+}
+
 // ------------------------------------------------------------------------------------------------------
-// weight gradient (+ bias gradient as tap 25), fused with the maxpool1 / ReLU1 backward
+// weight gradient (+ bias gradient from the 1.0 at j = 36), fused with the maxpool1 / ReLU1 backward
 // ------------------------------------------------------------------------------------------------------
-// TILE = 64 or 128 pooled pixels per tile; 2 * TILE threads (two builders per pooled pixel: window rows h = 0, 1) =
-// TILE / 64 warpgroups, warpgroup g reducing over pixels 64 g .. 64 g + 63 of every tile.  M = 64 rows of taps of
-// which 32 are real: warps 2 and 3 of a warpgroup feed zero operands.  The 64-pixel tile needs half the shared
-// memory (2 x 32 KB), so a CTA fits next to conv2_wgrad's and the two weight-gradient kernels can overlap.
-// Per-warpgroup partial sums of the weight gradient (rows = taps, 25 = bias; rows 26-31 unused), reduced in slot order
-// by the last CTA (see arrive_last_cta).
-constexpr int C1WG_SLOT = 32 * 32;
+// One warpgroup per CTA over a contiguous range of 64-pixel tiles.  Thread (m, h) builds half h of pixel m's patch row
+// and G half h: the masked gradient of positions 2h, 2h+1 (128 B).  A three-stage ring with one barrier per stage and
+// one commit group per tile, waited with wait_group 1: the builders fill the next stage while the tensor core works on
+// this one.  The stage written at tile i was last read by tile i - 3's MMAs, which every warp has waited for before the
+// barrier of tile i - 1.
+constexpr int C1WG_THREADS = 128;
+constexpr int C1WG_TILE = 64;
+constexpr int C1WG_STAGES = 3;
+constexpr int C1WG_SLOT = 26 * 32;        // taps 0-24, then the bias
 constexpr int C1WG_MAX_SLOTS = 512;
-// One launch of this kernel in flight per device: the workspace and ticket are static (see arrive_last_cta).
-__device__ float g_c1wg_part[C1WG_MAX_SLOTS * C1WG_SLOT];
+constexpr int C1WG_MAX_GROUPS = 32;       // >= ceil(sqrt(C1WG_MAX_SLOTS))
+// Two-level reduction of the per-CTA slots: the last CTA of each group of `group` consecutive CTAs adds its group's
+// slots in slot order into a group slot, the last group to finish adds the group slots in order into g_w / g_b.  One
+// launch of this kernel in flight per device: the workspaces and tickets are static (see arrive_last_cta).
+static_assert(C1WG_MAX_GROUPS * C1WG_MAX_GROUPS >= C1WG_MAX_SLOTS, "too few group slots");
+__device__ __align__(16) float g_c1wg_part[C1WG_MAX_SLOTS * C1WG_SLOT];
+__device__ __align__(16) float g_c1wg_group[C1WG_MAX_GROUPS * C1WG_SLOT];
+__device__ unsigned int g_c1wg_group_ticket[C1WG_MAX_GROUPS];
 __device__ unsigned int g_c1wg_ticket;
 
-template <int TILE>
 struct C1WgSmem {
-  static constexpr int TILE_BYTES = TILE * 64;                   // TILE pooled pixels x 32 bf16
-  static constexpr int STAGE_BYTES = 8 * TILE_BYTES;            // A_0..A_3 then G_0..G_3
-  static constexpr int TOTAL = 2 * STAGE_BYTES + 1024;
+  static constexpr int PATCH_BYTES = C1WG_TILE * C1T_ROW_BYTES;  // [64 pixels][64 j] bf16
+  static constexpr int G_BYTES = 2 * C1WG_TILE * 128;            // two [64 pixels][64 (p, co)] bf16 halves
+  static constexpr int STAGE_BYTES = PATCH_BYTES + G_BYTES;
+  static constexpr int E_LD = 136;                               // fold scratch: E rows 0..36, fp32, over the ring
+  static constexpr int TOTAL = C1WG_STAGES * STAGE_BYTES + 1024;
+  static_assert(37 * E_LD * 4 <= C1WG_STAGES * STAGE_BYTES, "fold scratch exceeds the ring");
 };
 
-template <int TILE>
-__global__ void __launch_bounds__(2 * TILE, 1)
+__global__ void __launch_bounds__(C1WG_THREADS, 1)
 conv1_wgrad_tc_kernel(const float* __restrict__ images,          // [B,28,28]
                       const __nv_bfloat16* __restrict__ dpool,   // [B,14,14,32] gradient w.r.t. the pooled activations
                       const uint8_t* __restrict__ code,          // [B,14,14,32]
                       float* __restrict__ g_w,                   // [25][32], the CTAs' sum is added to it (pre-zeroed)
                       float* __restrict__ g_b,                   // [32]
-                      long long total, int num_tiles) {
-  using S = C1WgSmem<TILE>;
+                      long long total, int num_tiles, int group) {
+  using S = C1WgSmem;
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -253,47 +308,37 @@ conv1_wgrad_tc_kernel(const float* __restrict__ images,          // [B,28,28]
   const int nt = t_end - t_begin;
   pdl_wait();
 
-  const int h = threadIdx.x / TILE, m = threadIdx.x % TILE;     // builder role
-  const int wg = warp >> 2, wq = warp & 3;                       // MMA role: warpgroup, warp inside it
-  // A_p^T via ldmatrix.trans: x4 tile i covers taps + 8 (i & 1) and pixels + 8 (i >> 1)
-  const int a_chunk = 2 * wq + ((lane >> 3) & 1);
-  const int a_row = 64 * wg + 8 * (lane >> 4) + (lane & 7);
-  struct TileRegs {
-    PatchRegs patch;
-    uint4 gq[4];      // pooled gradient, 32 channels bf16
-    uint4 cq[2];      // pooling codes, 32 channels
-  };
-  auto load_tile = [&](TileRegs& tr, int i) {
-    const long long P = (long long)(t_begin + i) * TILE + m;
-    load_patch_half(tr.patch, h, P, total, images);
+  const int h = threadIdx.x / C1WG_TILE, m = threadIdx.x % C1WG_TILE;     // builder role
+  float v[32];
+  uint4 gq[4];      // pooled gradient, 32 channels bf16
+  uint4 cq[2];      // pooling codes, 32 channels
+  auto load_tile = [&](int i) {
+    const long long P = (long long)(t_begin + i) * C1WG_TILE + m;
+    load_patch_row_half(v, h, P, total, images);
     if (P < total) {
       const uint4* gp = reinterpret_cast<const uint4*>(dpool + (size_t)P * 32);
       const uint4* cp = reinterpret_cast<const uint4*>(code + (size_t)P * 32);
 #pragma unroll
-      for (int j = 0; j < 4; ++j) tr.gq[j] = gp[j];
-      tr.cq[0] = __ldg(cp);
-      tr.cq[1] = __ldg(cp + 1);
+      for (int j = 0; j < 4; ++j) gq[j] = gp[j];
+      cq[0] = __ldg(cp);
+      cq[1] = __ldg(cp + 1);
     } else {
 #pragma unroll
-      for (int j = 0; j < 4; ++j) tr.gq[j] = make_uint4(0, 0, 0, 0);
-      tr.cq[0] = tr.cq[1] = make_uint4(0, 0, 0, 0);
+      for (int j = 0; j < 4; ++j) gq[j] = make_uint4(0, 0, 0, 0);
+      cq[0] = cq[1] = make_uint4(0, 0, 0, 0);
     }
   };
-  float acc[16];
+  float acc[64];
 #pragma unroll
-  for (int j = 0; j < 16; ++j) acc[j] = 0.f;
-  TileRegs cur, nxt;
-  if (nt > 0) load_tile(cur, 0);
+  for (int j = 0; j < 64; ++j) acc[j] = 0.f;
+  if (nt > 0) load_tile(0);
   for (int i = 0; i < nt; ++i) {
-    const int s = i & 1;
-    uint8_t* stage = smem + s * S::STAGE_BYTES;
-    if (i + 1 < nt) load_tile(nxt, i + 1);        // next tile's global loads are in flight while this one is packed
-    store_im2col_half(stage, m, h, cur.patch, S::TILE_BYTES);
-    const uint4* gq = cur.gq;
-    const uint4* cq = cur.cq;
+    uint8_t* stage = smem + (i % C1WG_STAGES) * S::STAGE_BYTES;
+    store_patch_row_half(stage, m, h, v);
     const uint32_t g32[16] = {gq[0].x, gq[0].y, gq[0].z, gq[0].w, gq[1].x, gq[1].y, gq[1].z, gq[1].w,
                               gq[2].x, gq[2].y, gq[2].z, gq[2].w, gq[3].x, gq[3].y, gq[3].z, gq[3].w};
     const uint32_t cw[8] = {cq[0].x, cq[0].y, cq[0].z, cq[0].w, cq[1].x, cq[1].y, cq[1].z, cq[1].w};
+    uint8_t* g_half = stage + S::PATCH_BYTES + h * (C1WG_TILE * 128);
 #pragma unroll
     for (int px = 0; px < 2; ++px) {
       const uint32_t p = 2u * (uint32_t)h + (uint32_t)px;
@@ -305,60 +350,65 @@ conv1_wgrad_tc_kernel(const float* __restrict__ images,          // [B,28,28]
         o[2 * w8] = g32[2 * w8] & prmt(hit, 0u, 0x9988u);
         o[2 * w8 + 1] = g32[2 * w8 + 1] & prmt(hit, 0u, 0xbbaau);
       }
-      uint8_t* tile = stage + (4 + p) * S::TILE_BYTES;
 #pragma unroll
-      for (int c = 0; c < 4; ++c) sts128(tile + swz64(m, c), o[4 * c], o[4 * c + 1], o[4 * c + 2], o[4 * c + 3]);
+      for (int c = 0; c < 4; ++c) sts128(g_half + swz128(m, 4 * px + c), o[4 * c], o[4 * c + 1], o[4 * c + 2], o[4 * c + 3]);
     }
-    fence_proxy_async_smem();                     // G_p is read by wgmma (async proxy)
-    __syncthreads();     // stage s complete; every thread is past its reads of stage s ^ 1 (written next iteration)
+    if (i + 1 < nt) load_tile(i + 1);             // in flight during the MMAs
+    fence_proxy_async_smem();                     // the operands are read by wgmma (async proxy)
+    __syncthreads();
 
-    fence_regs(acc);
+    // A = patch rows read MN-major (M = j, one 128 B chunk), B = G MN-major (N = 128: two chunks 8 KB apart); both
+    // with pixel k-rows of 128 B, 8-row groups 1024 B apart: a K step of 16 pixels is 2048 B
+    const uint64_t da = make_smem_desc(smem_u32(stage), 8192, 1024, SWZ_128B);
+    const uint64_t db = make_smem_desc(smem_u32(stage + S::PATCH_BYTES), 8192, 1024, SWZ_128B);
+    wgmma_fence();
+#pragma unroll
+    for (int ks = 0; ks < 4; ++ks) wgmma_m64n128_ss<1, 1>(acc, desc_advance(da, 2048 * ks), desc_advance(db, 2048 * ks), 1);
+    wgmma_commit();
+    wgmma_wait<1>();
+  }
+  wgmma_wait<0>();
+  fence_regs(acc);
+  __syncthreads();                                // every warp's MMAs are done with the ring: the fold scratch reuses it
+
+  // E rows 0..36 -> shared memory, then fold the four positions into this CTA's slot
+  float* E = reinterpret_cast<float*>(smem);
+#pragma unroll
+  for (int half = 0; half < 2; ++half) {
+    const int r = 16 * warp + (lane >> 2) + 8 * half;
+    if (r < 37) {
+#pragma unroll
+      for (int j = 0; j < 16; ++j)
+        *reinterpret_cast<float2*>(E + r * S::E_LD + 8 * j + 2 * (lane & 3)) = make_float2(acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
+    }
+  }
+  __syncthreads();
+  float* part = g_c1wg_part + (size_t)blockIdx.x * C1WG_SLOT;
+  for (int e = threadIdx.x; e < C1WG_SLOT; e += C1WG_THREADS) {
+    const int tap = e >> 5, co = e & 31;
+    float s = 0.f;
 #pragma unroll
     for (int p = 0; p < 4; ++p) {
-      // G_p as B (MN-major, 64B swizzle): k-row = pooled pixel (64 B = 32 co), 8-row groups 512 B apart
-      const uint32_t g_base = smem_u32(stage + (4 + p) * S::TILE_BYTES) + 64 * 64 * wg;
-      uint32_t a[4][4];
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks) {
-        if (wq < 2) {
-          ldsm_x4_trans(smem_u32(stage + p * S::TILE_BYTES + swz64(a_row + 16 * ks, a_chunk)), a[ks]);
-        } else {
-          a[ks][0] = a[ks][1] = a[ks][2] = a[ks][3] = 0u;
-        }
-      }
-      wgmma_fence();
-#pragma unroll
-      for (int ks = 0; ks < 4; ++ks)
-        wgmma_m64n32_rs<1>(acc, a[ks], make_smem_desc(g_base + 1024 * ks, 8192, 512, SWZ_64B), 1);
+      const int j = tap < 25 ? ((p >> 1) + tap / 5) * 6 + (p & 1) + tap % 5 : 36;
+      s += E[j * S::E_LD + 32 * p + co];
     }
-    wgmma_commit();
-    wgmma_wait<0>();
-    fence_regs(acc);
-    cur = nxt;
+    part[e] = s;
   }
-  constexpr int NWG = TILE / 64;
-  if (wq < 2) {
-    // accumulator rows = taps (25 = bias) -> this warpgroup's slot
-    float* part = g_c1wg_part + (size_t)(blockIdx.x * NWG + wg) * C1WG_SLOT;
-#pragma unroll
-    for (int half = 0; half < 2; ++half) {
-      const int tap = 16 * wq + (lane >> 2) + 8 * half;
-#pragma unroll
-      for (int j = 0; j < 4; ++j)
-        *reinterpret_cast<float2*>(part + tap * 32 + 8 * j + 2 * (lane & 3)) =
-            make_float2(acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
-    }
-  }
+
   __shared__ unsigned int s_last;
-  if (arrive_last_cta(&g_c1wg_ticket, gridDim.x, 1, 2 * TILE, &s_last)) {
-    const int nslots = gridDim.x * NWG;
-    for (int e4 = threadIdx.x; e4 < 26 * 32 / 4; e4 += 2 * TILE) {
-      const float4 sum = ordered_sum4(reinterpret_cast<const float4*>(g_c1wg_part) + e4, nslots, C1WG_SLOT / 4);
-      const int row = e4 >> 3, col = (e4 & 7) * 4;
-      float4* o = reinterpret_cast<float4*>((row < 25 ? g_w + row * 32 : g_b) + col);
-      const float4 cur = *o;
-      *o = make_float4(cur.x + sum.x, cur.y + sum.y, cur.z + sum.z, cur.w + sum.w);
-    }
+  const int grp = blockIdx.x / group, g0 = grp * group;
+  const int gn = min(group, (int)gridDim.x - g0), ngroups = ((int)gridDim.x + group - 1) / group;
+  if (!arrive_last_cta(&g_c1wg_group_ticket[grp], gn, 1, C1WG_THREADS, &s_last)) return;
+  float4* gslot = reinterpret_cast<float4*>(g_c1wg_group + (size_t)grp * C1WG_SLOT);
+  for (int e4 = threadIdx.x; e4 < C1WG_SLOT / 4; e4 += C1WG_THREADS)
+    gslot[e4] = ordered_sum4(reinterpret_cast<const float4*>(g_c1wg_part + (size_t)g0 * C1WG_SLOT) + e4, gn, C1WG_SLOT / 4);
+  if (!arrive_last_cta(&g_c1wg_ticket, ngroups, 1, C1WG_THREADS, &s_last)) return;
+  for (int e4 = threadIdx.x; e4 < C1WG_SLOT / 4; e4 += C1WG_THREADS) {
+    const float4 sum = ordered_sum4(reinterpret_cast<const float4*>(g_c1wg_group) + e4, ngroups, C1WG_SLOT / 4);
+    const int row = e4 >> 3, col = (e4 & 7) * 4;
+    float4* o = reinterpret_cast<float4*>((row < 25 ? g_w + row * 32 : g_b) + col);
+    const float4 cur = *o;
+    *o = make_float4(cur.x + sum.x, cur.y + sum.y, cur.z + sum.z, cur.w + sum.w);
   }
 }
 
@@ -390,28 +440,23 @@ int dm_conv1_fwd_tc(const void* images, const void* w, const void* bias, void* o
 
 }  // extern "C"
 
-template <int TILE>
-static int launch_conv1_wgrad(const void* images, const void* dpool, const void* code, void* g_w, void* g_b, int B,
-                              void* stream) {
+// g_w [25][32] and g_b [32] must be zeroed by the caller (the gradient is added to them).
+extern "C" int dm_conv1_wgrad_tc(const void* images, const void* dpool, const void* code, void* g_w, void* g_b, int B, void* stream) {
   using namespace dm;
-  auto kern = conv1_wgrad_tc_kernel<TILE>;
   static bool configured = false;
   if (!configured) {
-    DM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributeMaxDynamicSharedMemorySize, C1WgSmem<TILE>::TOTAL));
-    DM_CUDA_OK(cudaFuncSetAttribute(kern, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    DM_CUDA_OK(cudaFuncSetAttribute(conv1_wgrad_tc_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, C1WgSmem::TOTAL));
+    DM_CUDA_OK(cudaFuncSetAttribute(conv1_wgrad_tc_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }
   const long long total = (long long)B * 196;
-  const int tiles = (int)((total + TILE - 1) / TILE);
+  const int tiles = (int)((total + C1WG_TILE - 1) / C1WG_TILE);
   int grid = tiles < max_ctas() ? tiles : max_ctas();
-  if (grid * (TILE / 64) > C1WG_MAX_SLOTS) grid = C1WG_MAX_SLOTS / (TILE / 64);
-  return (int)launch_kernel(kern, dim3(grid), dim3(2 * TILE), C1WgSmem<TILE>::TOTAL,
+  if (grid > C1WG_MAX_SLOTS) grid = C1WG_MAX_SLOTS;
+  int group = 1;                                  // ceil(sqrt(grid)) CTAs per group, so at most as many groups
+  while (group * group < grid) ++group;
+  return (int)launch_kernel(conv1_wgrad_tc_kernel, dim3(grid), dim3(C1WG_THREADS), C1WgSmem::TOTAL,
                             reinterpret_cast<cudaStream_t>(stream), reinterpret_cast<const float*>(images),
                             reinterpret_cast<const __nv_bfloat16*>(dpool), reinterpret_cast<const uint8_t*>(code),
-                            reinterpret_cast<float*>(g_w), reinterpret_cast<float*>(g_b), total, tiles);
-}
-
-// g_w [25][32] and g_b [32] must be zeroed by the caller (the gradient is added to them).
-extern "C" int dm_conv1_wgrad_tc(const void* images, const void* dpool, const void* code, void* g_w, void* g_b, int B, void* stream) {
-  return launch_conv1_wgrad<64>(images, dpool, code, g_w, g_b, B, stream);
+                            reinterpret_cast<float*>(g_w), reinterpret_cast<float*>(g_b), total, tiles, group);
 }

@@ -13,7 +13,7 @@ import sys
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 LIB = os.path.join(ROOT, "distributedmnist_b200", "lib", "libdmnist_b200.so")
 HOT = [("conv2_fwd", r"conv2_fwd_kernel"), ("conv2_dgrad", r"conv2_dgrad_kernel"), ("conv2_wgrad", r"conv2_wgrad_kernel"),
-       ("conv1_fwd_tc", r"conv1_fwd_tc_kernel"), ("conv1_wgrad_tc64", r"conv1_wgrad_tc_kernelILi64E"),
+       ("conv1_fwd_tc", r"conv1_fwd_tc_kernel"), ("conv1_wgrad_tc", r"conv1_wgrad_tc_kernel"),
        ("gemm_fc1_fwd", r"gemm_tc_kernelILi64ELb0ELb1ELi0E"), ("gemm_fc1_dgrad_unpool", r"gemm_tc_kernelILi64ELb0ELb0ELi4E"),
        ("gemm_fc1_wgrad_bf16", r"gemm_tc_kernelILi128ELb1ELb1ELi2E"), ("bucket_early_n8", r"bucket_early_kernelILi8E"),
        ("bucket_late_ll", r"bucket_late_ll_kernel"), ("fused_sync_sgd_kofn", r"fused_sync_sgd_kernelILb1E"),
