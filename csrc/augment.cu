@@ -18,21 +18,10 @@
 //
 // CTA = AUG_THREADS threads over rows blockIdx.x, blockIdx.x + gridDim.x, ... (at most AUG_MAX_ROWS): thread t first
 // computes the coefficients of the CTA's row t, then the CTA stages each row in shared memory and writes its 784 pixels.
-#include <math.h>
-
-#include "common.cuh"
+#include "augment.cuh"
 #include "host_utils.h"
 
 namespace dm {
-
-constexpr int AUG_THREADS = 256;
-constexpr int AUG_MAX_ROWS = 32;          // rows per CTA; the grid grows past 4 CTAs per SM beyond that
-constexpr int AUG_PIX = 784;
-constexpr int AUG_PARAMS = 8;             // params_out per row: u0..u3, a, b, tx, ty
-
-struct AugRange {
-  double max_shift, max_rotation, max_scale;   // T (pixels), R (degrees), S
-};
 
 __global__ void __launch_bounds__(AUG_THREADS) augment_affine_kernel(const float* __restrict__ src,
                                                                      float* __restrict__ dst, int batch,
@@ -47,23 +36,7 @@ __global__ void __launch_bounds__(AUG_THREADS) augment_affine_kernel(const float
   if (t < nrows) {
     const uint32_t it = __ldcg(counter);    // read before this CTA arrives on the ticket
     const int b = (int)blockIdx.x + t * (int)gridDim.x;
-    const uint32_t key = hash_mix(seed_mix, it);
-    float u[4];
-#pragma unroll
-    for (int k = 0; k < 4; ++k) u[k] = (float)(hash_mix(key, 4u * (uint32_t)b + (uint32_t)k) >> 8) * 0x1p-24f;
-    const double theta = rg.max_rotation * M_PI / 180.0 * (2.0 * (double)u[0] - 1.0);
-    const double s = 1.0 + rg.max_scale * (2.0 * (double)u[1] - 1.0);
-    double sn, cs;
-    sincos(theta, &sn, &cs);
-    const float4 c = make_float4(__double2float_rn(cs / s), __double2float_rn(sn / s),
-                                 __double2float_rn(rg.max_shift * (2.0 * (double)u[2] - 1.0)),
-                                 __double2float_rn(rg.max_shift * (2.0 * (double)u[3] - 1.0)));
-    s_coef[t] = c;
-    if (params_out != nullptr) {
-      float* p = params_out + (size_t)b * AUG_PARAMS;
-      p[0] = u[0]; p[1] = u[1]; p[2] = u[2]; p[3] = u[3];
-      p[4] = c.x; p[5] = c.y; p[6] = c.z; p[7] = c.w;
-    }
+    s_coef[t] = affine_row_coefficients(hash_mix(seed_mix, it), b, rg, params_out);
   }
   for (int r = 0; r < nrows; ++r) {
     const size_t row = (size_t)((int)blockIdx.x + r * (int)gridDim.x) * AUG_PIX;
@@ -111,9 +84,7 @@ int dm_augment_affine(const void* src, void* dst, int batch, void* counter, unsi
   if (!(isfinite(max_shift) && isfinite(max_rotation) && isfinite(max_scale)) || max_shift < 0.0 || max_rotation < 0.0 ||
       max_scale < 0.0 || max_scale >= 1.0)
     return -1;
-  int grid = 4 * num_sms();
-  if (grid > batch) grid = batch;
-  if (grid < (batch + AUG_MAX_ROWS - 1) / AUG_MAX_ROWS) grid = (batch + AUG_MAX_ROWS - 1) / AUG_MAX_ROWS;
+  const int grid = augment_grid(batch, num_sms());
   const AugRange rg{max_shift, max_rotation, max_scale};
   return (int)launch_kernel(augment_affine_kernel, dim3(grid), dim3(AUG_THREADS), 0, reinterpret_cast<cudaStream_t>(stream),
                             reinterpret_cast<const float*>(src), reinterpret_cast<float*>(dst), batch,

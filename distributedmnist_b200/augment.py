@@ -14,6 +14,19 @@ The transform, defined here once (csrc/augment.cu computes the same one in fp32 
   ``dx = x - c - tx``, ``dy = y - c - ty``.  A tap outside ``[0, 27]^2`` reads the background ``BACKGROUND = -0.5``, the
   value of a zero pixel after data.py's ``(x - 127.5) / 255`` scaling.
 
+Elastic distortion (``--augment_elastic_alpha``, ``--augment_elastic_sigma``; Simard, Steinkraus and Platt, "Best
+practices for convolutional neural networks applied to visual document analysis", 2003), csrc/augment_elastic.cu:
+
+* Row ``b`` of replica ``r`` at iteration ``i`` draws ``2 x 784`` uniforms ``v = 2 u - 1``, ``u = (h >> 8) * 2^-24``
+  with ``h = hash_mix(hash_mix(E, i), 1568 b + 784 d + p)``, ``E = seed_mix(seed, r) + ELASTIC_MIX (mod 2^32)``, ``d``
+  0 for the x component and 1 for y, ``p = 28 y + x``.  The batch is limited to ``MAX_ELASTIC_BATCH`` rows so that the
+  index fits in u32.  The affine draws above do not change.
+* Each component is smoothed by the normalised Gaussian of width ``sigma`` (:func:`gaussian_weights`, radius
+  ``R = floor(4 sigma + 0.5)``, taps outside the image read 0: ``scipy.ndimage.gaussian_filter(v, sigma,
+  mode="constant", cval=0, truncate=4)``) and scaled by ``alpha``: the displacement ``(ex, ey)`` in pixels.
+* Output pixel ``(x, y)`` is first displaced to ``(x + ex, y + ey)``, which the affine inverse map above then takes
+  in place of ``(x, y)``; the bilinear sample and the background are those above.
+
 ``i`` counts the replica's training iterations, so two iterations of one run never share draws.  A restarted run starts
 it past the iterations that went into the restored global step (:func:`start_iteration`), so a one-replica run does
 not replay the draws of the steps it restored; a multi-replica K > N run or an interval run can repeat some (see
@@ -35,6 +48,19 @@ BACKGROUND = -0.5
 MAX_SHIFT = 8.0                 # pixels
 MAX_ROTATION = 180.0            # degrees
 RANK_MIX = 0x297A2D39           # seed_mix(seed, r + 1) = seed_mix(seed, r) + RANK_MIX (mod 2^32)
+# the elastic key's offset from the affine key; not k * RANK_MIX (mod 2^32) for |k| < 1024, so no replica's elastic key
+# is any replica's affine key in a run of up to 1024 replicas
+ELASTIC_MIX = 0x6A09E667
+ELASTIC_DRAWS = 2 * 784         # draws per row: the x then the y component, pixel-major
+MAX_ELASTIC_BATCH = 2 ** 32 // ELASTIC_DRAWS    # rows whose every draw index 1568 b + 784 d + p fits in u32
+MAX_ALPHA = 64.0                # pixels
+MIN_SIGMA, MAX_SIGMA = 0.5, 8.0     # the radius floor(4 sigma + 0.5) is then at most 32
+DEFAULT_SIGMA = 4.0             # Simard et al.'s width
+
+
+class Elastic(NamedTuple):
+    alpha: float                # scale of the smoothed field, pixels
+    sigma: float                # width of the Gaussian, pixels
 
 
 class Ranges(NamedTuple):
@@ -82,15 +108,50 @@ def affine(theta, scale, tx, ty):
     return np.cos(theta) / scale, np.sin(theta) / scale, np.asarray(tx, np.float64), np.asarray(ty, np.float64)
 
 
-def warp(images: np.ndarray, a, b, tx, ty, centre: float = CENTRE) -> np.ndarray:
+def gaussian_weights(sigma: float) -> np.ndarray:
+    """float64 ``[R + 1]``: the normalised Gaussian's taps ``w_0 .. w_R`` (``w_-k = w_k``), ``R = floor(4 sigma + 0.5)``,
+    ``w_k = exp(-k^2 / 2 sigma^2) / sum_{|j| <= R} exp(-j^2 / 2 sigma^2)`` (scipy.ndimage's ``truncate=4`` kernel)."""
+    sigma = float(sigma)
+    radius = int(4.0 * sigma + 0.5)
+    w = np.exp(-0.5 / (sigma * sigma) * np.arange(-radius, radius + 1, dtype=np.float64) ** 2)
+    return (w / w.sum())[radius:]
+
+
+def elastic_uniforms(mix: int, iteration: int, rows: int) -> np.ndarray:
+    """float64 ``[rows, 2, 784]``: the elastic draws ``v = 2 u - 1`` of rows ``0..rows-1`` at ``iteration`` under the
+    replica's affine key ``mix`` (component 0: x, 1: y; each exact in fp32)."""
+    if rows > MAX_ELASTIC_BATCH:
+        raise ValueError("elastic distortion draws %d values per row: at most %d rows, got %d"
+                         % (ELASTIC_DRAWS, MAX_ELASTIC_BATCH, rows))
+    key = int(hash_mix((int(mix) + ELASTIC_MIX) & _M32, int(iteration) & _M32))
+    idx = np.arange(rows * ELASTIC_DRAWS, dtype=np.uint64).reshape(rows, 2, 784)
+    return (hash_mix(key, idx) >> np.uint64(8)).astype(np.float64) * 2.0 ** -23 - 1.0
+
+
+def elastic_field(mix: int, iteration: int, rows: int, elastic: Elastic) -> np.ndarray:
+    """float64 ``[rows, 2, 28, 28]``: the displacement ``(ex, ey)`` in pixels of rows ``0..rows-1`` at ``iteration``,
+    ``alpha G V G^T`` with ``G`` the banded 28 x 28 matrix of :func:`gaussian_weights` (taps outside the image read 0)."""
+    w = gaussian_weights(elastic.sigma)
+    k = np.abs(np.arange(28)[:, None] - np.arange(28)[None, :])
+    g = np.where(k < len(w), w[np.minimum(k, len(w) - 1)], 0.0)
+    v = elastic_uniforms(mix, iteration, rows).reshape(rows, 2, 28, 28)
+    return float(elastic.alpha) * (g @ v @ g.T)
+
+
+def warp(images: np.ndarray, a, b, tx, ty, centre: float = CENTRE, field=None) -> np.ndarray:
     """The float64 warp of ``images`` (``[rows, 28, 28]`` or ``[rows, 784]``, row-major y, x) with per-row coefficients;
     returns float64 ``[rows, 28, 28]``.  ``centre``: the transform's is ``CENTRE`` (the tests warp about others to show
-    that their bounds tell the two apart)."""
+    that their bounds tell the two apart).  ``field``: None, or the elastic displacement ``[rows, 2, 28, 28]`` (or
+    ``[rows, 2, 784]``) that moves each output pixel before the affine map."""
     img = np.asarray(images, dtype=np.float64).reshape(-1, 28, 28)
     n = img.shape[0]
     a, b, tx, ty = (np.broadcast_to(np.asarray(v, dtype=np.float64), (n,))[:, None, None] for v in (a, b, tx, ty))
     y, x = np.meshgrid(np.arange(28, dtype=np.float64), np.arange(28, dtype=np.float64), indexing="ij")
-    dx, dy = x[None] - centre - tx, y[None] - centre - ty
+    if field is None:
+        dx, dy = x[None] - centre - tx, y[None] - centre - ty
+    else:
+        f = np.asarray(field, dtype=np.float64).reshape(n, 2, 28, 28)
+        dx, dy = (x[None] + f[:, 0]) - centre - tx, (y[None] + f[:, 1]) - centre - ty
     sx = centre + a * dx + b * dy
     sy = centre - b * dx + a * dy
     x0, y0 = np.floor(sx), np.floor(sy)
@@ -107,11 +168,15 @@ def warp(images: np.ndarray, a, b, tx, ty, centre: float = CENTRE) -> np.ndarray
     return (1.0 - fy) * ((1.0 - fx) * v00 + fx * v01) + fy * ((1.0 - fx) * v10 + fx * v11)
 
 
-def augment_batch(images: np.ndarray, mix: int, iteration: int, ranges: Ranges) -> np.ndarray:
-    """The augmented batch (float64 warp from the float64 coefficients, rounded to fp32), in the shape of ``images``."""
+def augment_batch(images: np.ndarray, mix: int, iteration: int, ranges: Ranges,
+                  elastic: Optional[Elastic] = None) -> np.ndarray:
+    """The augmented batch (float64 warp from the float64 coefficients and, with ``elastic``, the float64 field, rounded
+    to fp32), in the shape of ``images``."""
     img = np.asarray(images)
-    u = uniforms(mix, iteration, img.shape[0])
-    return warp(img, *coefficients(u, ranges)).astype(np.float32).reshape(img.shape)
+    n = img.shape[0]
+    u = uniforms(mix, iteration, n)
+    field = None if elastic is None else elastic_field(mix, iteration, n, elastic)
+    return warp(img, *coefficients(u, ranges), field=field).astype(np.float32).reshape(img.shape)
 
 
 def start_iteration(restored_step: int, count_triggered: bool, k: int, n: int) -> int:
@@ -151,11 +216,38 @@ def from_flags(flags) -> Optional[Ranges]:
     return r if any(r) else None
 
 
+def check_elastic(elastic: Elastic) -> None:
+    """Raises ValueError unless alpha and sigma are finite and within bounds."""
+    a, s = float(elastic.alpha), float(elastic.sigma)
+    if not math.isfinite(a) or not 0.0 <= a <= MAX_ALPHA:
+        raise ValueError("--augment_elastic_alpha must be finite and lie in [0, %g] (0 = off), got %r" % (MAX_ALPHA, a))
+    if not math.isfinite(s) or not MIN_SIGMA <= s <= MAX_SIGMA:
+        raise ValueError("--augment_elastic_sigma must be finite and lie in [%g, %g], got %r" % (MIN_SIGMA, MAX_SIGMA, s))
+
+
+def elastic_from_flags(flags) -> Optional[Elastic]:
+    """``Elastic(alpha, sigma)``, or None when elastic distortion is off (alpha 0).  Raises ValueError on a value out of
+    range, and on a sigma other than the default without an alpha: it would change nothing."""
+    e = Elastic(float(getattr(flags, "augment_elastic_alpha", 0.0) or 0.0),
+                float(getattr(flags, "augment_elastic_sigma", DEFAULT_SIGMA)))
+    check_elastic(e)
+    if e.alpha == 0.0:
+        if e.sigma != DEFAULT_SIGMA:
+            raise ValueError("--augment_elastic_sigma needs --augment_elastic_alpha > 0: without an alpha there is no "
+                             "field for it to smooth")
+        return None
+    return e
+
+
 def check_flags(flags) -> None:
     """The augmentation flags, checked before any device work starts."""
     from_flags(flags)
+    elastic_from_flags(flags)
 
 
-def describe(r: Ranges) -> str:
-    return "shift up to %g px, rotation up to %g degrees, zoom in [%g, %g]" % (r.max_shift, r.max_rotation,
-                                                                             1.0 - r.max_scale, 1.0 + r.max_scale)
+def describe(r: Ranges, elastic: Optional[Elastic] = None) -> str:
+    s = "shift up to %g px, rotation up to %g degrees, zoom in [%g, %g]" % (r.max_shift, r.max_rotation,
+                                                                          1.0 - r.max_scale, 1.0 + r.max_scale)
+    if elastic is not None:
+        s += ", elastic distortion alpha %g px, sigma %g px" % (elastic.alpha, elastic.sigma)
+    return s

@@ -116,17 +116,25 @@ class TorchEngine(ComputeEngine):
         :meth:`loss_acc` reports includes the term."""
         self._decay = float(lam)
 
-    # ---- random affine augmentation (see augment.py) ----------------------------------------------------------------------
+    # ---- random affine augmentation and elastic distortion (see augment.py) ---------------------------------------------
     _aug = None                    # (augment.Ranges, seed mix)
+    _aug_elastic = None            # augment.Elastic while elastic distortion is armed
     _aug_images: Optional[torch.Tensor] = None
 
-    def arm_augment(self, max_shift: float, max_rotation: float, max_scale: float, start_iteration: int = 0) -> None:
+    def arm_augment(self, max_shift: float, max_rotation: float, max_scale: float, start_iteration: int = 0,
+                    elastic: Optional[augment.Elastic] = None) -> None:
         """Augment every training batch from the next :meth:`forward_backward` on, its first draws those of iteration
-        ``start_iteration``; all three ranges 0 turns it off.  The same transform and draws as the sm_90a kernel, by the
+        ``start_iteration``; all three ranges 0 and no ``elastic`` (or alpha 0) turns it off.  ``elastic``: the elastic
+        distortion composed in front of the affine map.  The same transform and draws as the sm_90a kernels, by the
         float64 warp rounded to fp32."""
         r = augment.Ranges(float(max_shift), float(max_rotation), float(max_scale))
         augment.check_ranges(r)
-        self._aug = (r, augment.seed_mix(self.seed, self.rank)) if any(r) else None
+        if elastic is not None:
+            elastic = augment.Elastic(float(elastic.alpha), float(elastic.sigma))
+            augment.check_elastic(elastic)
+        self._aug_elastic = elastic if elastic is not None and elastic.alpha != 0.0 else None
+        on = any(r) or self._aug_elastic is not None
+        self._aug = (r, augment.seed_mix(self.seed, self.rank)) if on else None
         self._aug_iteration = int(start_iteration) & 0xFFFFFFFF
 
     def augment_iteration(self) -> int:
@@ -140,7 +148,7 @@ class TorchEngine(ComputeEngine):
         images = self._images
         if self._aug is not None:
             r, mix = self._aug
-            out = augment.augment_batch(images.detach().cpu().numpy(), mix, self._aug_iteration, r)
+            out = augment.augment_batch(images.detach().cpu().numpy(), mix, self._aug_iteration, r, self._aug_elastic)
             images = self._aug_images = torch.from_numpy(out).to(self.device)
             self._aug_iteration = (self._aug_iteration + 1) & 0xFFFFFFFF
         p = self.params.detach().requires_grad_(True)

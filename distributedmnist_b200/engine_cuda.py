@@ -25,6 +25,7 @@ calls cuDNN, cuBLAS or NCCL.
 from __future__ import annotations
 
 import contextlib
+import ctypes
 import gc
 import os
 from typing import Optional, Tuple
@@ -416,17 +417,31 @@ class _CudaEngine(ComputeEngine):
     # input slot's images into _aug_images; every reader of the step's training images reads that buffer instead.  The
     # step graphs replay one after another on the training stream, so one buffer serves both slots.  The iteration word
     # _aug_counter[0] is advanced by the kernel itself; _aug_counter[1] is its ticket.  Evaluation never augments.
+    # With elastic distortion armed, augment_elastic (csrc/augment_elastic.cu) takes augment_affine's place: the same
+    # node, buffer and counter, the elastic field composed in front of the affine map.
     _aug = None                    # (augment.Ranges, seed mix), see arm_augment
+    _aug_elastic = None            # augment.Elastic while elastic distortion is armed
+    _aug_taps = None               # its Gaussian taps w_0 .. w_R as a ctypes double array, and R
 
-    def arm_augment(self, max_shift: float, max_rotation: float, max_scale: float, start_iteration: int = 0) -> None:
+    def arm_augment(self, max_shift: float, max_rotation: float, max_scale: float, start_iteration: int = 0,
+                    elastic: Optional[augment.Elastic] = None) -> None:
         """Augment every training step from the next one on, its first draws those of iteration ``start_iteration`` (a
-        restarted run: ``augment.start_iteration`` of the restored global step).  All three ranges 0 turns augmentation
-        off.  Re-captures the step graphs."""
+        restarted run: ``augment.start_iteration`` of the restored global step).  ``elastic``: elastic distortion
+        composed in front of the affine map (None or alpha 0: none).  All three ranges 0 and no elastic distortion turns
+        augmentation off.  Re-captures the step graphs."""
         r = augment.Ranges(float(max_shift), float(max_rotation), float(max_scale))
         augment.check_ranges(r)
+        if elastic is not None:
+            elastic = augment.Elastic(float(elastic.alpha), float(elastic.sigma))
+            augment.check_elastic(elastic)
+            if elastic.alpha == 0.0:
+                elastic = None
+            elif self.batch_size > augment.MAX_ELASTIC_BATCH:
+                raise ValueError("elastic distortion takes at most %d rows per batch, got %d"
+                                 % (augment.MAX_ELASTIC_BATCH, self.batch_size))
         self._leave_native_runner()
         torch.cuda.synchronize()
-        if any(r):
+        if any(r) or elastic is not None:
             if getattr(self, "_aug_images", None) is None:
                 self._aug_images = torch.zeros(self.batch_size, 784, dtype=torch.float32, device=self.device)
                 self._aug_counter = torch.zeros(2, dtype=torch.int32, device=self.device)
@@ -435,14 +450,25 @@ class _CudaEngine(ComputeEngine):
             self._aug = (r, augment.seed_mix(self.seed, self.backend.ctx.rank))
         else:
             self._aug = None
+        self._aug_elastic = elastic
+        if elastic is not None:
+            w = augment.gaussian_weights(elastic.sigma)
+            self._aug_taps = ((ctypes.c_double * len(w))(*w), len(w) - 1)
         self._graphs = [None, None]
         torch.cuda.synchronize()
 
     def _launch_augment(self, slot: int) -> torch.Tensor:
-        """augment_affine on the current stream: slot ``slot``'s images -> the augmented buffer, in the slot's shape."""
+        """augment_affine, or augment_elastic with elastic distortion armed, on the current stream: slot ``slot``'s
+        images -> the augmented buffer, in the slot's shape."""
         r, mix = self._aug
-        self.lib.dm_augment_affine(self.images[slot], self._aug_images, self.batch_size, self._aug_counter, mix,
-                                   r.max_shift, r.max_rotation, r.max_scale, None, stream_ptr())
+        if self._aug_elastic is None:
+            self.lib.dm_augment_affine(self.images[slot], self._aug_images, self.batch_size, self._aug_counter, mix,
+                                       r.max_shift, r.max_rotation, r.max_scale, None, stream_ptr())
+        else:
+            w, radius = self._aug_taps
+            self.lib.dm_augment_elastic(self.images[slot], self._aug_images, self.batch_size, self._aug_counter, mix,
+                                        r.max_shift, r.max_rotation, r.max_scale, self._aug_elastic.alpha, w, radius,
+                                        None, None, stream_ptr())
         return self._aug_images.view(self.images[slot].shape)
 
     def augment_iteration(self) -> int:

@@ -305,6 +305,13 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
                                                 "degrees about its centre; 0 <= R <= 180 (0 = no rotation)")
     F.DEFINE_float("augment_max_scale", 0.0, "Random affine augmentation: zoom each training image by s ~ U[1-S, 1+S]; "
                                              "0 <= S < 1 (0 = no zoom)")
+    F.DEFINE_float("augment_elastic_alpha", 0.0, "Elastic distortion of the training images (Simard et al. 2003): "
+                                                 "displace each pixel by alpha pixels times uniform noise in [-1, 1] "
+                                                 "smoothed by a Gaussian of width --augment_elastic_sigma, before the "
+                                                 "affine warp; 0 <= alpha <= 64 (0 = off).  Augmentation is on when "
+                                                 "alpha or any --augment_max_* is non-zero")
+    F.DEFINE_float("augment_elastic_sigma", 4.0, "With --augment_elastic_alpha: the width in pixels of the Gaussian that "
+                                                 "smooths the displacement field; 0.5 <= sigma <= 8")
     return F
 
 

@@ -52,6 +52,8 @@ def _signatures() -> dict:
     return {
         # augment.cu
         "dm_augment_affine": (S, i, [P, P, i, P, u, d, d, d, P, P]),
+        # augment_elastic.cu
+        "dm_augment_elastic": (S, i, [P, P, i, P, u, d, d, d, d, P, i, P, P, P]),
         # batch_gather.cu
         "dm_gather_batch": (S, i, [P, P, P, i, P, P]),
         # conv1_tc.cu, conv2_tc.cu

@@ -791,7 +791,7 @@ AUG_U = 2.0 ** -24
 AUG_PREMISE_ROWS = 256         # rows the premise checks of augment_results warp (a large batch's would only cost time)
 
 
-def augment_pixel_bound(coef, coef_ulps: int = 0) -> np.ndarray:
+def augment_pixel_bound(coef, coef_ulps: int = 0, field=None, field_err=None) -> np.ndarray:
     """Per-pixel bound on |augment_affine - float64 warp of the fp32 coefficients ``coef``| ([B, 4]: a, b, tx, ty),
     float64 [B, 784].
 
@@ -809,14 +809,29 @@ def augment_pixel_bound(coef, coef_ulps: int = 0) -> np.ndarray:
     ``coef_ulps``: the kernel's coefficients may each differ from ``coef`` by that many fp32 ulps (<= 2^-23 |c| each):
     its double ``sincos`` and numpy's may round to different fp32 neighbours near a tie.  Since sx = c + a dx + b dy with
     dx = x - c - tx, a change of e |a|, e |b|, e |tx|, e |ty| moves sx by at most e (|a| (|dx| + |tx|) + |b| (|dy| + |ty|))
-    and sy by e (|b| (|dx| + |tx|) + |a| (|dy| + |ty|)), which the same Lipschitz argument adds to the bound."""
+    and sy by e (|b| (|dx| + |tx|) + |a| (|dy| + |ty|)), which the same Lipschitz argument adds to the bound.
+
+    ``field``: the elastic displacement [B, 2, 784] (augment_elastic; fp32 values) the bound is taken around.  That
+    kernel computes dx = fl(fl(xc + ex) - tx), two roundings: |dx_f - dx| <= u (|xc + ex| + |dx|), which enters sx with
+    weight |a| and sy with |b| (dy likewise with |b|, |a|).  ``field_err``: [B, 2, 784] bound on |kernel field - field|;
+    a change of the displacement by (fx, fy) moves sx by |a| fx + |b| fy and sy by |b| fx + |a| fy."""
     a, b, tx, ty = (np.asarray(coef, dtype=np.float64)[:, k][:, None] for k in range(4))
     y, x = np.divmod(np.arange(784, dtype=np.float64), 28)
     dx, dy = x[None] - 13.5 - tx, y[None] - 13.5 - ty
+    if field is not None:
+        f = np.asarray(field, dtype=np.float64).reshape(-1, 2, 784)
+        dx, dy = (x[None] - 13.5 + f[:, 0]) - tx, (y[None] - 13.5 + f[:, 1]) - ty
     tsx, tsy = b * dy + 13.5, -b * dx + 13.5
     sx, sy = a * dx + tsx, a * dy + tsy
     bsx = AUG_U * (np.abs(a * dx) + np.abs(b * dy) + np.abs(tsx) + np.abs(sx))
     bsy = AUG_U * (np.abs(a * dy) + np.abs(b * dx) + np.abs(tsy) + np.abs(sy))
+    if field is not None:
+        rx, ry = AUG_U * np.abs(x[None] - 13.5 + f[:, 0]), AUG_U * np.abs(y[None] - 13.5 + f[:, 1])
+        if field_err is not None:
+            fe = np.asarray(field_err, dtype=np.float64).reshape(-1, 2, 784)
+            rx, ry = rx + fe[:, 0], ry + fe[:, 1]
+        bsx = bsx + np.abs(a) * rx + np.abs(b) * ry
+        bsy = bsy + np.abs(b) * rx + np.abs(a) * ry
     if coef_ulps:
         e = coef_ulps * 2.0 ** -23
         ax, by = np.abs(dx) + np.abs(tx), np.abs(dy) + np.abs(ty)
@@ -832,14 +847,18 @@ def augment_coefficients(mix: int, iteration: int, B: int, ranges) -> np.ndarray
     return c.astype(np.float32).astype(np.float64)
 
 
-def augment_results(tag: str, fed, got, mix: int, iteration: int, ranges) -> List[Result]:
+def augment_results(tag: str, fed, got, mix: int, iteration: int, ranges, elastic=None) -> List[Result]:
     """One augmented step's buffer ``got`` [B, 784] against ``augment.warp`` of the batch it was ``fed`` (fp32, [B, 784]
     or [B, 28, 28], values in [-0.5, 0.5]) with the draws of ``iteration`` under ``mix``, the coefficients rounded to fp32,
     within :func:`augment_pixel_bound` widened by one ulp of each coefficient.
 
     Premise: the warps of iterations ``iteration`` +- 1, of the next rank's mix and about the centre 14.0 each differ from
     the reference by more than the bound on some pixel of the first ``AUG_PREMISE_ROWS`` rows, so a step that drew from a
-    neighbouring iteration, used another replica's key or shifted the centre by half a pixel fails the check."""
+    neighbouring iteration, used another replica's key or shifted the centre by half a pixel fails the check.
+
+    ``elastic``: the ``augment.Elastic`` the step was armed with; see :func:`elastic_augment_results`."""
+    if elastic is not None:
+        return elastic_augment_results(tag, fed, got, mix, iteration, ranges, elastic)
     from .. import augment as AU
     x = (fed.detach().cpu().numpy() if torch.is_tensor(fed) else np.asarray(fed)).astype(np.float64)
     B = x.shape[0]
@@ -855,6 +874,57 @@ def augment_results(tag: str, fed, got, mix: int, iteration: int, ranges) -> Lis
             ("iteration_plus_1", AU.warp(xs, *augment_coefficients(mix, iteration + 1, n, ranges).T)),
             ("next_rank", AU.warp(xs, *augment_coefficients((mix + AU.RANK_MIX) & 0xFFFFFFFF, iteration, n, ranges).T)),
             ("centre_14", AU.warp(xs, *c[:n].T, centre=14.0)))
+    for name, alt in alts:
+        seen = bool((np.abs(alt.reshape(n, 784) - want[:n]) > bound[:n]).any())
+        res.append(("%s.premise.%s_detectable" % (tag, name), 0.0 if seen else 1.0, 0.0))
+    return res
+
+
+def elastic_field_f32(mix: int, iteration: int, B: int, elastic) -> np.ndarray:
+    """[B, 2, 784] float64 ``augment.elastic_field`` rounded to fp32: the field augment_elastic computes, each component
+    within :func:`elastic_field_err` of it."""
+    from .. import augment as AU
+    return AU.elastic_field(mix, iteration, B, elastic).reshape(B, 2, 784).astype(np.float32).astype(np.float64)
+
+
+def elastic_field_err(field, elastic) -> np.ndarray:
+    """Bound on |augment_elastic's field - ``field``| per component: one fp32 ulp (<= 2^-23 |e|), and alpha 2^-44 for
+    the double passes of the kernel and of the float64 reference where the field nearly cancels (csrc/augment_elastic.cu
+    derives < alpha 2^-45 for each)."""
+    return 2.0 ** -23 * np.abs(field) + float(elastic.alpha) * 2.0 ** -44
+
+
+def elastic_augment_results(tag: str, fed, got, mix: int, iteration: int, ranges, elastic) -> List[Result]:
+    """An elastic step's buffer ``got`` [B, 784] against ``augment.warp`` of the batch it was ``fed`` with the
+    coefficients and the field of ``iteration`` under ``mix``, each rounded to fp32, within :func:`augment_pixel_bound`
+    widened by one ulp of each coefficient and of each field component (:func:`elastic_field_err`).
+
+    Premise: the warps of iterations ``iteration`` +- 1, of the next rank's mix, with the field's x and y components
+    swapped, without the field, and with sigma 1.25 times as wide each differ from the reference by more than the bound
+    on some pixel of the first ``AUG_PREMISE_ROWS`` rows."""
+    from .. import augment as AU
+    x = (fed.detach().cpu().numpy() if torch.is_tensor(fed) else np.asarray(fed)).astype(np.float64)
+    B = x.shape[0]
+    x = x.reshape(B, 784)
+    c = augment_coefficients(mix, iteration, B, ranges)
+    f = elastic_field_f32(mix, iteration, B, elastic)
+    want = AU.warp(x, *c.T, field=f).reshape(B, 784)
+    bound = augment_pixel_bound(c, coef_ulps=1, field=f, field_err=elastic_field_err(f, elastic))
+    g = got.detach().reshape(B, 784)
+    res = R.cmp_bound(tag, g, torch.from_numpy(want).to(g.device), torch.from_numpy(bound).to(g.device))
+    n = min(B, AUG_PREMISE_ROWS)
+    xs, cn, fn = x[:n], c[:n].T, f[:n]
+    nxt = (mix + AU.RANK_MIX) & 0xFFFFFFFF
+    wide = AU.Elastic(elastic.alpha, 1.25 * elastic.sigma)
+    alts = (("iteration_minus_1", AU.warp(xs, *augment_coefficients(mix, iteration - 1, n, ranges).T,
+                                          field=elastic_field_f32(mix, iteration - 1, n, elastic))),
+            ("iteration_plus_1", AU.warp(xs, *augment_coefficients(mix, iteration + 1, n, ranges).T,
+                                         field=elastic_field_f32(mix, iteration + 1, n, elastic))),
+            ("next_rank", AU.warp(xs, *augment_coefficients(nxt, iteration, n, ranges).T,
+                                  field=elastic_field_f32(nxt, iteration, n, elastic))),
+            ("swapped_components", AU.warp(xs, *cn, field=fn[:, ::-1])),
+            ("no_field", AU.warp(xs, *cn)),
+            ("sigma_1.25", AU.warp(xs, *cn, field=elastic_field_f32(mix, iteration, n, wide))))
     for name, alt in alts:
         seen = bool((np.abs(alt.reshape(n, 784) - want[:n]) > bound[:n]).any())
         res.append(("%s.premise.%s_detectable" % (tag, name), 0.0 if seen else 1.0, 0.0))

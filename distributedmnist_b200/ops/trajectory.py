@@ -8,8 +8,8 @@ bounds the kernel checks use (``ops/selfcheck.py``):
 * each stage from its recorded inputs, on the weights the previous step committed (the initial arena for the first);
   the bf16 shadow a step reads is RNE of those weights, the dropout mask the one of the epoch word the step read;
 * the update bit for bit against ``ops/aggrefs.py``, and the recorded shadow as RNE of the recorded weights;
-* with random affine augmentation armed, the recorded augmented buffer against the float64 warp of the fed batch with
-  the draws of the step's own iteration, the iteration counter after every step, and every reader of the images
+* with random affine augmentation (and elastic distortion) armed, the recorded augmented buffer against the float64 warp
+  of the fed batch with the draws of the step's own iteration, the iteration counter after every step, and every reader of the images
   (conv1 forward and wgrad, the MLP's x16) against that step's recorded buffer.
 
 The input slots are not recorded: the copy stream may refill a slot as soon as the step that read it is done.  The caller
@@ -57,7 +57,7 @@ class StepRecorder:
             r["g16"] = e._g16_view.clone()
         if getattr(e, "_decay", 0.0):
             r["decay_ws"] = e._decay_ws.clone()         # the W^2 partials of both weight-gradient kernels, then R
-        if getattr(e, "_aug", None) is not None:        # the next step's augment_affine overwrites both
+        if getattr(e, "_aug", None) is not None:        # the next step's augmentation node overwrites both
             r["aug_images"] = e._aug_images.clone()
             r["aug_counter"] = e._aug_counter.clone()
         self.records.append(r)
@@ -70,7 +70,7 @@ def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
     (``arm_lr_cuts``), ``sched`` must name the same cuts (raises ValueError otherwise): the step sizes are then those of
     the schedule with the cuts (synchronises the device to read the table).  ``aug``: (ranges, seed mix) of the armed
     augmentation, None without it; ``aug_start`` the iteration the run's first step draws from (see
-    :func:`augment_stage_results`)."""
+    :func:`augment_stage_results`); ``elastic`` the armed ``augment.Elastic``, None without elastic distortion."""
     be = eng.backend
     e0, e1 = eng._bucket_early
     mode = "kgtn" if eng._kgtn_k else ("bucket" if eng._bucket_v2 else "fused")
@@ -81,7 +81,7 @@ def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
     return dict(mode=mode, sched=sched, step0=step0, k=max(eng._kgtn_k, 1), early=(e0, e1),
                 late_bf16=A.late_bucket_rounds_bf16(eng.spec.arena_numel, e1 - e0, be.late_ll, be.late_bf16),
                 drop=(be.drop_seed, be.drop_keep) if be.drop_keep > 0.0 else None,
-                aug=getattr(eng, "_aug", None), aug_start=int(aug_start))
+                aug=getattr(eng, "_aug", None), aug_start=int(aug_start), elastic=getattr(eng, "_aug_elastic", None))
 
 
 def epoch_of(upd: dict, t: int) -> int:
@@ -101,7 +101,8 @@ def _words(t: torch.Tensor) -> List[int]:
 
 def augment_stage_results(tag: str, init: dict, records: Sequence[dict], batches: Sequence, upd: dict) -> List[Result]:
     """With augmentation armed (``upd["aug"]``): each step's recorded buffer against the warp of the batch it was fed
-    (:func:`selfcheck.augment_results`) with the draws of :func:`augment_iteration_of`, and the counter words: the
+    (:func:`selfcheck.augment_results`; with ``upd["elastic"]`` the elastic warp) with the draws of
+    :func:`augment_iteration_of`, and the counter words: the
     iteration before the first step, and after step t the next one with the ticket back at 0."""
     if upd.get("aug") is None:
         return []
@@ -110,7 +111,7 @@ def augment_stage_results(tag: str, init: dict, records: Sequence[dict], batches
     res: List[Result] = [(tag + ".init.aug_counter_differs", float(_words(init["aug_counter"]) != [start, 0]), 0.0)]
     for t, (r, (x, _y)) in enumerate(zip(records, batches)):
         it = augment_iteration_of(upd, t)
-        res += S.augment_results("%s.step%d.augment" % (tag, t), x, r["aug_images"], mix, it, ranges)
+        res += S.augment_results("%s.step%d.augment" % (tag, t), x, r["aug_images"], mix, it, ranges, upd.get("elastic"))
         res.append(("%s.step%d.aug_counter_differs" % (tag, t),
                     float(_words(r["aug_counter"]) != [(it + 1) & 0xFFFFFFFF, 0]), 0.0))
     return res

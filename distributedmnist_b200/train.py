@@ -624,6 +624,9 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     check_device_data_flags(flags, ctx, dataset)
     weight_decay.check_flags(flags, ctx)
     aug_ranges = augment.from_flags(flags)
+    aug_elastic = augment.elastic_from_flags(flags)
+    if aug_elastic is not None and aug_ranges is None:
+        aug_ranges = augment.Ranges(0.0, 0.0, 0.0)          # elastic distortion alone
     device_data = bool(getattr(flags, "device_data", False))
     target = float(getattr(flags, "target_accuracy", 0.0) or 0.0)
     patience = int(getattr(flags, "early_stopping_patience", 0) or 0)
@@ -690,9 +693,14 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         # draws (multi-replica K > N and interval runs can: see augment.start_iteration)
         aug_start = augment.start_iteration(restored_step, isinstance(opt, SyncReplicasOptimizer),
                                             num_replicas_to_aggregate, num_workers)
-        engine.arm_augment(*aug_ranges, start_iteration=aug_start)
-        log.info("Random affine augmentation of the training images: %s, draws from iteration %d; evaluation is not "
-                 "augmented" % (augment.describe(aug_ranges), aug_start))
+        if aug_elastic is None:
+            engine.arm_augment(*aug_ranges, start_iteration=aug_start)
+            log.info("Random affine augmentation of the training images: %s, draws from iteration %d; evaluation is "
+                     "not augmented" % (augment.describe(aug_ranges), aug_start))
+        else:
+            engine.arm_augment(*aug_ranges, start_iteration=aug_start, elastic=aug_elastic)
+            log.info("Random affine augmentation and elastic distortion of the training images: %s, draws from "
+                     "iteration %d; evaluation is not augmented" % (augment.describe(aug_ranges, aug_elastic), aug_start))
     if ema_decay:
         # the chief's average starts from the restored averages, else from the (initial or restored) weights; from here on
         # every global step ends with its update (GPU path: a node at the end of the chief's step graph)
