@@ -1616,6 +1616,10 @@ class CudaMlpEngine(_CudaEngine):
     def _launch_step(self, slot: int, with_sync: bool) -> None:
         B = self.batch_size
         n = 0
+        if self._stamp:
+            # cdf telemetry: the start of the step's compute (read_timing); the aggregation kernel stamps its arrival
+            self.backend.enqueue_stamp_start()
+            n += 1
         images = self.images[slot]
         if self._aug is not None:
             images = self._launch_augment(slot)     # dm_f32_to_bf16 reads the augmented batch

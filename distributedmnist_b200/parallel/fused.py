@@ -77,6 +77,7 @@ class FusedBackend(Backend):
         self.shadow: Optional[torch.Tensor] = None     # bf16 copy of the parameter arena
         self.drop_keep = 0.0
         self.drop_seed = 0
+        self.interval_ns: Optional[int] = None     # the interval clock's period, once armed (interval_arm)
 
     # ---- memory ---------------------------------------------------------------------------
     def allocate(self, numel: int) -> torch.Tensor:
@@ -253,6 +254,7 @@ class FusedBackend(Backend):
     def interval_arm(self, interval_ms: float) -> None:
         """Start the interval clock on this replica (reference ``start_interval_updates``): first tick due in ``interval_ms``."""
         self.barrier()                       # replicas start their clocks together (each uses its own %globaltimer afterwards)
+        self.interval_ns = int(float(interval_ms) * 1e6)      # what the device holds: the kernel truncates the same way
         self.lib.dm_interval_arm(self.ctrl.local_ptr, interval_ms, stream_ptr())
         torch.cuda.synchronize()
         self.barrier()

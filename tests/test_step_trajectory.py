@@ -39,11 +39,12 @@ def _update(w, g):
     return lambda t: torch.from_numpy(A.fused_sync_step(A.f32(w), [A.f32(g)], 1, A.step_scale(SCHED, STEP0 + t, 1)))
 
 
-def _lenet_step(spec, params, x, y, mask, fault, prev, lam=0.0, x_wgrad=None):
+def _lenet_step(spec, params, x, y, mask, fault, prev, lam=0.0, x_wgrad=None, shadow=None):
     """One LeNet step as the kernels store it.  ``fault``: "dgrad_post_update" runs fc1 dgrad on the updated shadow.
-    ``lam``: L2 weight decay (see :func:`_decay`).  ``x_wgrad``: the images conv1 wgrad reads, if not ``x``."""
+    ``lam``: L2 weight decay (see :func:`_decay`).  ``x_wgrad``: the images conv1 wgrad reads, if not ``x``.  ``shadow``:
+    the fp32 weights the bf16 shadow was made from, if not ``params``."""
     B = x.shape[0]
-    p, pb = spec.views(params), spec.views(params.to(BF))
+    p, pb = spec.views(params), spec.views((params if shadow is None else shadow).to(BF))
     f1 = R.pool_fwd(R.conv5x5(x.to(BF)[..., None], p["conv1_weights"].to(BF)), p["conv1_biases"])
     a1, code1 = _bf(f1["out"]), f1["code"]
     f2 = R.pool_fwd(R.conv5x5(a1, pb["conv2_weights"]), p["conv2_biases"])
@@ -97,12 +98,12 @@ def _decay(spec, params, r, lam, fault, prev):
         r["loss_acc"][0] = r["loss_acc"][0] + np.float32(lam * float(rr))
 
 
-def _mlp_step(spec, params, x, y, fault, prev):
+def _mlp_step(spec, params, x, y, fault, prev, shadow=None):
     """One MLP step as the kernels store it.  ``fault``: "bias_not_cleared" adds the previous step's atomically
-    accumulated output-layer bias gradient."""
+    accumulated output-layer bias gradient.  ``shadow``: as for :func:`_lenet_step`."""
     L = len(spec.params) // 2
     B = x.shape[0]
-    p, pb = spec.views(params), spec.views(params.to(BF))
+    p, pb = spec.views(params), spec.views((params if shadow is None else shadow).to(BF))
     x16 = _bf(x.reshape(B, 784))
     hs, src = [], x16
     for i in range(1, L):
@@ -226,8 +227,10 @@ def test_seeded_fault_fails(model, fault, stage):
     assert any(stage in n for n, _, _ in bad), (fault, bad[:10])
 
 
-def test_kgtn_update_commits_every_k_th_iteration():
-    """K > N: the weights stay put for k - 1 iterations, then take the accumulated k gradients at the commit's step size."""
+def test_kgtn_update_commits_every_k_th_iteration_and_the_next_adoption_refreshes_the_shadow():
+    """K > N: the weights stay put for k - 1 iterations, then take the accumulated k gradients at the commit's step size.
+    The commit leaves the bf16 shadow alone; the next iteration's adoption refreshes it, so after iteration t it is RNE
+    of the weights recorded after iteration t - 1."""
     spec = get_model("mlp2", 64)[0]
     gen = torch.Generator().manual_seed(3)
     w = spec.init_flat(SEED)
@@ -236,9 +239,13 @@ def test_kgtn_update_commits_every_k_th_iteration():
     c1 = torch.from_numpy(A.sgd(A.f32(w), A.interval_accumulate([A.f32(g) for g in gs[:2]]), A.step_scale(SCHED, STEP0, 2)))
     c2 = torch.from_numpy(A.sgd(A.f32(c1), A.interval_accumulate([A.f32(g) for g in gs[2:]]), A.step_scale(SCHED, STEP0 + 1, 2)))
     upd = dict(mode="kgtn", sched=SCHED, step0=STEP0, k=2, early=(0, 0), late_bf16=False)
-    recs = [dict(grads=g, params=p, shadow=p.to(BF)) for g, p in zip(gs, (w, c1, c1, c2))]
+    # the shadow is refreshed by the adoption at the start of the iteration after a commit
+    recs = [dict(grads=g, params=p, shadow=s.to(BF)) for g, p, s in zip(gs, (w, c1, c1, c2), (w, w, c1, c1))]
     assert not T.failures(T.update_results("kgtn", init, recs, upd))
     assert [T.epoch_of(upd, t) for t in range(4)] == [STEP0, STEP0, STEP0 + 1, STEP0 + 1]
+    bad = dict(recs[2], shadow=w.to(BF))               # the adoption did not refresh the shadow
+    assert [n for n, _, _ in T.failures(T.update_results("kgtn", init, recs[:2] + [bad] + recs[3:], upd))] == \
+        ["kgtn.step2.shadow_bits_differ"]
     recs[1] = dict(recs[1], params=w)                  # the commit not applied
     assert T.failures(T.update_results("kgtn", init, recs, upd))
 
@@ -325,3 +332,193 @@ def test_seeded_augment_fault_fails(model, fault, stage):
     assert any(stage in n for n, _, _ in bad), (fault, bad[:10])
     family = stage.split(".")[1].split("[")[0]
     assert all(family in n for n, _, _ in bad), (fault, bad[:10])
+
+
+# ---- interval mode ------------------------------------------------------------------------------------------------------
+# The control block of one replica in host memory, laid out by an offset table of its own (the checker reads the words
+# through the offsets it is given), and an emulated clock in nanoseconds.  Every step takes 10 ns: the adoption (and
+# t_start) at its start, the gate (t_arrive) at +6, the close at +8.  The host paces the ticks: before the last step of
+# each tick it waits until the deadline has passed, so that step's close commits the tick.
+CTRL_OFF = dict(epoch=0, error=4, accepted_steps=8, dropped_steps=12, last_count=16, iv_ticks_committed=20, iv_state=24,
+                iv_deadline=32, t_start=40, t_arrive=40 + 8 * T.TIMING_RING)
+CTRL_BYTES = 40 + 16 * T.TIMING_RING
+TICKS = (1, 3, 2, 4)
+INTERVAL_NS = 10_000
+IV_FAULTS = ("divisor_1", "divisor_t_minus_1", "accumulator_overwritten", "adoption_late", "k_eq_n_updates",
+             "mask_step0_plus_t", "shadow_not_refreshed", "commit_before_deadline", "deadline_rearmed_without_adoption",
+             "count_word_off", "epoch_without_commit")
+
+
+class _Ctrl:
+    """The words of the control block the interval kernels write, at CTRL_OFF."""
+
+    def __init__(self):
+        self.b = np.zeros(CTRL_BYTES, dtype=np.uint8)
+
+    def _view(self, f):
+        n = 8 if f in T.CTRL_U64 else 4
+        return self.b[CTRL_OFF[f]:CTRL_OFF[f] + n].view("<u%d" % n)
+
+    def __getitem__(self, f):
+        return int(self._view(f)[0])
+
+    def __setitem__(self, f, v):
+        self._view(f)[0] = v
+
+    def stamp(self, ring, ns):
+        """t_start / t_arrive of the current epoch word."""
+        o = CTRL_OFF[ring] + 8 * (self["epoch"] % T.TIMING_RING)
+        self.b[o:o + 8].view("<u8")[0] = ns
+
+    def snapshot(self):
+        return torch.from_numpy(self.b.copy())
+
+
+def _run_interval(model, fault=None):
+    """(spec, init, records, batches fed, update) of an emulated one-replica interval run with ticks of TICKS gradients
+    and at most one seeded fault (one of IV_FAULTS)."""
+    spec = get_model(model, 64)[0]
+    steps, B = sum(TICKS), 8
+    last_of_tick = set(np.cumsum(TICKS) - 1)
+    gen = torch.Generator().manual_seed(12)
+    shape = (B, 28, 28) if model == "lenet" else (B, 784)
+    batches = [(torch.rand(*shape, generator=gen) - 0.5, torch.randint(0, 10, (B,), generator=gen)) for _ in range(steps)]
+    params = spec.init_flat(SEED)
+    c, now = _Ctrl(), 10 ** 9
+    c["epoch"] = STEP0                                   # set_global_step, then the clock is armed
+    c["iv_state"], c["iv_deadline"] = (STEP0 + 1) << 32, now + INTERVAL_NS
+    init = dict(params=params.clone(), shadow=params.to(BF), ctrl=c.snapshot())
+    records, gs, shadow, committed, before = [], [], params.clone(), None, None
+    for t in range(steps):
+        x, y = batches[t]
+        if t in last_of_tick and fault != "commit_before_deadline":
+            now = max(now, c["iv_deadline"] + 100)       # the host slept past the deadline
+        # iv_adopt + iv_shadow
+        if committed is not None:
+            c["epoch"] = c["epoch"] + 1
+            c["iv_deadline"], c["last_count"], c["iv_state"] = now + INTERVAL_NS, committed, (c["epoch"] + 1) << 32
+            if fault != "shadow_not_refreshed":
+                shadow = params.clone()
+        if fault == "epoch_without_commit" and t == 2:
+            c["epoch"] = c["epoch"] + 1
+        if fault == "deadline_rearmed_without_adoption" and t == 2:
+            c["iv_deadline"] = now + INTERVAL_NS
+        c.stamp("t_start", now)
+        w_fp32, w_bf16 = params, shadow
+        if fault == "adoption_late" and committed is not None:
+            w_fp32 = w_bf16 = before                     # computes on the weights from before the commit it should adopt
+        committed = None
+        if model == "lenet":
+            e = STEP0 + t if fault == "mask_step0_plus_t" else c["epoch"]
+            mask = dropout_keep_mask(dropout_seed_mix(SEED, e, RANK), B, 512, KEEP)
+            r = _lenet_step(spec, w_fp32, x, y, mask, None, dict(t=t), shadow=w_bf16)
+        else:
+            r = _mlp_step(spec, w_fp32, x, y, None, dict(t=t), shadow=w_bf16)
+        # iv_gate, iv_accumulate, iv_close (+ commit), iv_apply
+        c.stamp("t_arrive", now + 6)
+        gs.append(r["grads"])
+        c["iv_state"] = c["iv_state"] + 1 + (fault == "count_word_off" and t == 1)
+        c["accepted_steps"] = c["accepted_steps"] + 1
+        if t in last_of_tick:
+            n = len(gs)
+            div = {"divisor_1": 1, "divisor_t_minus_1": max(n - 1, 1)}.get(fault, n)
+            acc = A.f32(gs[-1]) if fault == "accumulator_overwritten" else A.interval_accumulate([A.f32(g) for g in gs])
+            before = params
+            params = torch.from_numpy(A.fused_sync_step(A.f32(params), [acc], 1, A.step_scale(SCHED, c["epoch"], div)))
+            c["iv_ticks_committed"] = c["iv_ticks_committed"] + 1
+            committed, gs = n, []
+        elif fault == "k_eq_n_updates":
+            params = torch.from_numpy(A.fused_sync_step(A.f32(params), [A.f32(r["grads"])], 1,
+                                                        A.step_scale(SCHED, c["epoch"], 1)))
+        now += 10
+        r.update(params=params.clone(), shadow=shadow.to(BF), ctrl=c.snapshot())
+        records.append(r)
+    upd = dict(mode="interval", sched=SCHED, step0=STEP0, k=1, early=(spec.param("fc1_weights").offset,) * 2,
+               late_bf16=False, aug=None, aug_start=0, interval_ns=INTERVAL_NS, ctrl_off=CTRL_OFF)
+    return spec, init, records, batches, upd
+
+
+def _interval_results(model, fault=None, mode="interval"):
+    spec, init, records, batches, upd = _run_interval(model, fault)
+    upd["mode"] = mode
+    if model == "lenet":
+        return T.lenet_trajectory_results("lenet", spec, init, records, batches, upd, SEED, RANK, KEEP)
+    return T.mlp_trajectory_results("mlp3", spec, init, records, batches, upd)
+
+
+@pytest.mark.parametrize("model", ["lenet", "mlp3"])
+def test_emulated_interval_trajectory_passes(model):
+    """Ticks of 1, 3, 2 and 4 gradients: every stage on the weights and epoch word of the commit the step adopted, the
+    weights unchanged by steps that did not commit, each commit bit for bit, and the control block's words and stamps."""
+    spec, init, records, batches, upd = _run_interval(model)
+    tr = T.interval_trace(upd, init, records)
+    assert tr["commit"] == [t in set(np.cumsum(TICKS) - 1) for t in range(sum(TICKS))]
+    assert [n for n, cm in zip(tr["count"], tr["commit"]) if cm] == list(TICKS)
+    assert tr["epoch"] == [STEP0, STEP0 + 1, STEP0 + 1, STEP0 + 1, STEP0 + 2, STEP0 + 2] + [STEP0 + 3] * 4
+    res = _interval_results(model)
+    assert not T.failures(res), T.failures(res)
+    worst = T.worst_by_stage(model, res)
+    for stage in ("update_bits_differ", "shadow_bits_differ", "init.clock_armed_before_global_step", "count_differs",
+                  "epoch_differs", "last_count_differs", "stamps_out_of_order", "open_tick_past_deadline",
+                  "commit_before_deadline", "deadline_moved_without_commit", "deadline_not_rearmed_at_adoption"):
+        assert stage in worst, (stage, sorted(worst))
+    assert all(0 <= v <= 1 for v in worst.values()), worst
+
+
+def test_emulated_interval_trajectory_fails_under_the_k_eq_n_model():
+    """The premise of the GPU runs' check: the K = N model (an update and a new epoch word every step) tells an
+    interval run apart."""
+    bad = T.failures(_interval_results("lenet", mode="fused"))
+    assert any("step1.update_bits_differ" in n for n, _, _ in bad), bad[:10]
+
+
+@pytest.mark.parametrize("model,fault,stage", [
+    ("lenet", "divisor_1", "step3.update_bits_differ"),
+    ("mlp3", "divisor_t_minus_1", "step3.update_bits_differ"),
+    ("lenet", "accumulator_overwritten", "step3.update_bits_differ"),
+    ("mlp3", "accumulator_overwritten", "step3.update_bits_differ"),
+    ("lenet", "adoption_late", "step1.conv1_fwd"),
+    ("mlp3", "adoption_late", "step1.h1"),
+    ("lenet", "k_eq_n_updates", "step1.update_bits_differ"),
+    ("mlp3", "k_eq_n_updates", "step1.update_bits_differ"),
+    ("lenet", "mask_step0_plus_t", "step2.fc2_fwd_bwd"),
+    ("lenet", "shadow_not_refreshed", "step1.shadow_bits_differ"),
+    ("mlp3", "shadow_not_refreshed", "step1.shadow_bits_differ"),
+    ("lenet", "commit_before_deadline", "step0.commit_before_deadline"),
+    ("lenet", "deadline_rearmed_without_adoption", "step2.deadline_moved_without_commit"),
+    ("lenet", "count_word_off", "step1.count_differs"),
+    ("lenet", "epoch_without_commit", "step2.epoch_differs"),
+])
+def test_seeded_interval_fault_fails(model, fault, stage):
+    bad = T.failures(_interval_results(model, fault))
+    assert any(stage in n for n, _, _ in bad), (fault, bad[:10])
+
+
+def test_interval_clock_armed_before_the_global_step_fails():
+    """The clock armed at epoch 0 and the global step set afterwards: the step half of iv_state is 1, not STEP0 + 1."""
+    spec, init, records, batches, upd = _run_interval("mlp3")
+    c = _Ctrl()
+    c.b[:] = init["ctrl"].numpy()
+    c["iv_state"] = 1 << 32
+    bad = T.failures(T.control_results("mlp3", dict(init, ctrl=c.snapshot()), records, upd))
+    assert [n for n, _, _ in bad] == ["mlp3.init.clock_armed_before_global_step"]
+
+
+def test_stamps_of_a_k_eq_n_run():
+    """cdf mode: the stamps of step t sit at its global step; a step whose start was never stamped fails."""
+    spec, init, records, batches, upd = _run("mlp3")
+    c = _Ctrl()
+    init = dict(init, ctrl=c.snapshot())
+    for t, r in enumerate(records):
+        c["epoch"] = STEP0 + t
+        c.stamp("t_start", 100 * t + 1)
+        c.stamp("t_arrive", 100 * t + 50)
+        c["epoch"] = STEP0 + t + 1
+        r["ctrl"] = c.snapshot()
+    upd = dict(upd, ctrl_off=CTRL_OFF)
+    res = T.control_results("mlp3", init, records, upd)
+    assert len(res) == len(records) and not T.failures(res), res
+    c.b[CTRL_OFF["t_start"]:CTRL_OFF["t_arrive"]] = 0        # t_start never stamped
+    records[-1]["ctrl"] = c.snapshot()
+    bad = T.failures(T.control_results("mlp3", init, records, upd))
+    assert [n for n, _, _ in bad] == ["mlp3.step3.stamps_out_of_order"]

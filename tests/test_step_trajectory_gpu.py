@@ -10,11 +10,21 @@ Every run starts at global step 3001 with a schedule whose rate changes every st
 stated otherwise: the first two capture the two slot graphs, the rest replay them pipelined.
 
 The L2 weight decay (``--weight_decay``) runs are checked the same way, with the fc gradients against the plain reference
-+ lambda v of the weights the step read, R against float64 and the loss word against CE + lambda R.  Interval mode is not
-among them: its commits follow a wall-clock deadline, which the update check has no model of, so it is covered by a
-smoke run (tests/test_weight_decay_gpu.py) only.  Runs with more than one replica need more than one GPU."""
++ lambda v of the weights the step read, R against float64 and the loss word against CE + lambda R.
+
+Interval mode (``--interval_method``) runs the non-bucketed backward between the adoption of pushed weights and the
+gate / accumulate / close / apply kernels, and commits a tick when its close finds the wall-clock deadline passed.  The
+recorder clones the replica's control block after every step, so the checker reads which steps committed and with how
+many gradients, judges every update bit for bit against those ticks and every stage on the weights and epoch word of the
+commit the step adopted, and checks the decisions against the device's own %globaltimer stamps (trajectory.control_results).
+The runs tick every step (a 1 us interval) or are paced by the host (ticks of 3, 4 and 2 gradients), with dropout keep
+0.8, weight decay, augmentation with elastic distortion, the native runner, eager launches and the MLPs.  cdf mode
+(``--worker_times_cdf_method``) computes what K = N computes, with the start and arrival stamp nodes (and a straggler's
+delay) in the step graph; its runs are checked as K = N runs, and each step's stamps as its own.  Runs with more than one
+replica need more than one GPU."""
 import json
 import os
+import time
 
 import numpy as np
 import pytest
@@ -37,33 +47,43 @@ def _backend():
     return FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
 
 
-def _start(eng, be, k=1, lam=0.0, drop=None, sched=None, aug=None):
-    """``aug``: (ranges, first iteration) of the random affine augmentation to arm, None for none."""
+def _start(eng, be, k=1, lam=0.0, drop=None, sched=None, aug=None, mode=None, interval_ms=None, straggler=None):
+    """``aug``: (ranges, first iteration[, elastic distortion]) of the random affine augmentation to arm, None for none.
+    ``mode``: "interval" or "cdf" (TimeoutReplicasOptimizer, ``interval_ms``, ``straggler`` as parse_straggler_spec
+    returns it), None for SyncReplicasOptimizer."""
     from distributedmnist_b200.ops.trajectory import StepRecorder
-    from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
-    eng.attach_optimizer(SyncReplicasOptimizer(be, sched or _sched(), k, 1, drop_connect_probability=drop))
+    from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer, TimeoutReplicasOptimizer
+    if mode is None:
+        opt = SyncReplicasOptimizer(be, sched or _sched(), k, 1, drop_connect_probability=drop)
+    else:
+        opt = TimeoutReplicasOptimizer(be, sched or _sched(), 1, mode=mode, interval_ms=interval_ms or 1000,
+                                       straggler=straggler, seed=SEED)
+    eng.attach_optimizer(opt)
     if lam:
         eng.arm_weight_decay(lam)
     if aug is not None:
-        eng.arm_augment(*aug[0], start_iteration=aug[1])
+        eng.arm_augment(*aug[0], start_iteration=aug[1], elastic=aug[2] if len(aug) > 2 else None)
     be.set_global_step(STEP0)
     if k > 1:
         be.kgtn_arm()
+    if mode == "interval":
+        be.interval_arm(interval_ms)    # after set_global_step, as train.py arms it: the clock's step half is STEP0 + 1
     return StepRecorder(eng)
 
 
-def _lenet(B, keep_prob=0.5, k=1, lam=0.0, drop=None, sched=None, aug=None, use_graph=True):
+def _lenet(B, keep_prob=0.5, k=1, lam=0.0, drop=None, sched=None, aug=None, use_graph=True, mode=None, interval_ms=None,
+           straggler=None):
     from distributedmnist_b200.engine_cuda import CudaLeNetEngine
     be = _backend()
     eng = CudaLeNetEngine(B, be, seed=SEED, rank=0, keep_prob=keep_prob, use_graph=use_graph)
-    return eng, be, _start(eng, be, k, lam, drop, sched, aug)
+    return eng, be, _start(eng, be, k, lam, drop, sched, aug, mode, interval_ms, straggler)
 
 
-def _mlp(model, B, hidden, k=1, aug=None):
+def _mlp(model, B, hidden, k=1, aug=None, mode=None, interval_ms=None, straggler=None):
     from distributedmnist_b200.engine_cuda import CudaMlpEngine
     be = _backend()
     eng = CudaMlpEngine(model, B, be, hidden=hidden, seed=SEED, use_graph=True)
-    return eng, be, _start(eng, be, k, aug=aug)
+    return eng, be, _start(eng, be, k, aug=aug, mode=mode, interval_ms=interval_ms, straggler=straggler)
 
 
 def _batches(eng, n, seed=9):
@@ -121,10 +141,12 @@ def _check(tag, eng, be, rec, batches, lam=0.0, sched=None, aug=None):
         assert upd["aug"] is None and "aug_images" not in rec.records[0]
     else:
         assert upd["aug"] == (aug[0], AU.seed_mix(SEED, 0)) and "aug_images" in rec.records[0]
-    bucket = os.environ.get("DMNIST_BUCKET", "2") == "2" and be.drop_keep <= 0.0     # drop-connect: the single kernel
-    assert upd["mode"] == ("kgtn" if eng._kgtn_k else ("bucket" if bucket else "fused"))
+    # drop-connect: the single kernel; interval mode: its own kernels
+    bucket = os.environ.get("DMNIST_BUCKET", "2") == "2" and be.drop_keep <= 0.0 and not eng._interval
+    assert upd["mode"] == ("kgtn" if eng._kgtn_k else "interval" if eng._interval else "bucket" if bucket else "fused")
     assert getattr(eng, "_decay", 0.0) == float(np.float32(lam)) and (("decay_ws" in rec.records[0]) == bool(lam))
-    if not eng._kgtn_k:
+    assert ("ctrl" in rec.records[0]) == (eng._interval or eng._stamp)
+    if not eng._interval:
         assert be.device_epoch == STEP0 + len(batches)
     if hasattr(eng, "h_part"):
         res = T.lenet_trajectory_results(tag, eng.spec, rec.init, rec.records, batches, upd, eng.seed, eng.rank,
@@ -477,3 +499,165 @@ def test_lenet_augmented_unrecorded_run_matches_the_checked_one(how, use_graph, 
         del keep
     for name, a, b in zip(("params", "grads", "aug_images", "aug_counter"), *ends):
         assert torch.equal(a, b), name
+
+
+# ---- interval mode ------------------------------------------------------------------------------------------------------
+# One replica: every tick's commit is its own (the mask is rank 0, the divisor its count).  Paced runs: the host enqueues
+# the first T - 1 steps of a tick back to back, waits for them, sleeps past the deadline and enqueues the T-th, whose close
+# commits the tick; the next step adopts it and re-arms the deadline.  The checker follows what the device recorded, so a
+# host stall that let a tick commit early changes the ticks, not the verdict; each paced run still asserts that a tick of
+# at least 3 gradients committed.
+PACE_MS = 1000.0
+PACED_TICKS = (3, 4, 2)
+
+
+def _pace(be, ticks=PACED_TICKS, interval_ms=PACE_MS):
+    """``(after, early)``: the ``after`` callback of :func:`_feed` that paces ``ticks``, and the list of the ticks' last
+    steps before which the tick had already committed (a host stall past the deadline)."""
+    last = set(np.cumsum(ticks) - 1)
+    early = []
+    base = be._read_u32("iv_ticks_committed")
+
+    def after(t):
+        if t + 1 in last:
+            torch.cuda.synchronize()
+            if be._read_u32("iv_ticks_committed") - base != sum(1 for s in last if s <= t):
+                early.append(t + 1)
+            time.sleep(interval_ms * 1e-3 + 0.05)
+    return after, early
+
+
+def _ticks(eng, rec):
+    """Gradients of each committed tick, as the control blocks recorded them."""
+    from distributedmnist_b200.ops import trajectory as T
+    tr = T.interval_trace(T.update_of(eng, _sched(), STEP0), rec.init, rec.records)
+    return [n for n, c in zip(tr["count"], tr["commit"]) if c], tr
+
+
+def _paced(tag, eng, be, rec, how="numpy", lam=0.0, aug=None):
+    after, early = _pace(be)
+    batches = _batches(eng, sum(PACED_TICKS))
+    _feed(eng, rec, batches, how, after=after)
+    if how != "numpy":
+        assert eng._runner is not None
+    worst = _check(tag, eng, be, rec, batches, lam, aug=aug)
+    sizes, _tr = _ticks(eng, rec)
+    print("TICKS %s committed %s, paced %s, committed before their last step: %s" % (tag, sizes, PACED_TICKS, early))
+    assert any(n >= 3 for n in sizes), sizes
+    if not early:
+        assert sizes == list(PACED_TICKS), sizes
+    return batches, worst
+
+
+def test_lenet_interval_every_step_commits():
+    """A 1 us interval: every close comes after the deadline, so every step commits a tick of its own gradient."""
+    eng, be, rec = _lenet(128, mode="interval", interval_ms=0.001)
+    assert eng._interval and not eng._kgtn_k and not eng._bucketed
+    batches = _batches(eng, 6)
+    _feed(eng, rec, batches)
+    _check("lenet.B128.interval1us", eng, be, rec, batches)
+    sizes, tr = _ticks(eng, rec)
+    assert tr["commit"] == [True] * 6 and sizes == [1] * 6, tr
+    assert be.device_epoch == STEP0 + 5               # the last commit is adopted by the next step
+
+
+def test_lenet_interval_paced_trajectory():
+    """Ticks of 3, 4 and 2 gradients.  Premise: judged as K = N steps (an update and a new epoch word every step) the
+    same records fail."""
+    from distributedmnist_b200.ops import trajectory as T
+    eng, be, rec = _lenet(128, mode="interval", interval_ms=PACE_MS)
+    batches, _ = _paced("lenet.B128.interval", eng, be, rec)
+    upd = dict(T.update_of(eng, _sched(), STEP0), mode="fused")
+    bad = T.failures(T.lenet_trajectory_results("kn", eng.spec, rec.init, rec.records, batches, upd, eng.seed, eng.rank,
+                                                eng.keep_prob))
+    stages = sorted({n.split(".", 2)[2] for n, _, _ in bad})
+    print("K = N model on the interval records: %d checks fail, stages %s" % (len(bad), stages[:12]))
+    assert any(n.endswith("update_bits_differ") for n, _, _ in bad) and any("fc2_fwd_bwd" in n for n, _, _ in bad)
+
+
+def test_lenet_interval_keep_08_trajectory():
+    eng, be, rec = _lenet(128, keep_prob=0.8, mode="interval", interval_ms=PACE_MS)
+    _paced("lenet.B128.keep0.8.interval", eng, be, rec)
+
+
+@pytest.mark.parametrize("lam", [LAM, LAM_LARGE])
+def test_lenet_interval_decayed_trajectory(lam):
+    """Every iteration of a tick is decayed at the weights it adopted, which the previous record holds."""
+    eng, be, rec = _lenet(128, lam=lam, mode="interval", interval_ms=PACE_MS)
+    _paced("lenet.B128.interval.decay%g" % lam, eng, be, rec, lam=lam)
+
+
+def test_lenet_interval_elastic_trajectory():
+    """The augmentation counter advances once per iteration (the first step's plus t), the epoch word once per commit."""
+    from distributedmnist_b200 import augment as AU
+    aug = _aug() + (AU.Elastic(34.0, 4.0),)
+    eng, be, rec = _lenet(128, aug=aug, mode="interval", interval_ms=PACE_MS)
+    assert eng._aug_elastic is not None
+    _paced("lenet.B128.interval.elastic", eng, be, rec, aug=aug)
+
+
+@pytest.mark.parametrize("how", ["packed", "step_indices"])
+def test_lenet_interval_native_runner_feeds(how):
+    eng, be, rec = _lenet(128, mode="interval", interval_ms=PACE_MS)
+    _paced("lenet.B128.interval.%s" % how, eng, be, rec, how)
+
+
+def test_lenet_interval_eager_trajectory():
+    eng, be, rec = _lenet(128, use_graph=False, mode="interval", interval_ms=PACE_MS)
+    _paced("lenet.B128.interval.eager", eng, be, rec)
+
+
+@pytest.mark.parametrize("model", ["mlp2", "mlp3"])
+def test_mlp_interval_trajectory(model):
+    eng, be, rec = _mlp(model, 128, 1024, mode="interval", interval_ms=PACE_MS)
+    _paced("%s.B128.H1024.interval" % model, eng, be, rec)
+
+
+# ---- cdf mode -------------------------------------------------------------------------------------------------------------
+# The updates are those of K = N; the step graph adds the start and arrival stamps and, with a straggler, the delay inside
+# the stamped span.  Every step's stamps must be its own (trajectory.control_results) and span its delay.
+def _straggler(form):
+    from distributedmnist_b200.parallel.aggregators import parse_straggler_spec
+    return None if form is None else parse_straggler_spec(form, 30000)
+
+
+def _check_cdf(tag, eng, be, rec, batches, form):
+    from distributedmnist_b200.ops import trajectory as T
+    assert eng._stamp and not eng._interval
+    _check(tag, eng, be, rec, batches)
+    spans = np.array([(w["t_arrive"] - w["t_start"]) for w in
+                      (T.ctrl_words(r["ctrl"], be._off, STEP0 + t) for t, r in enumerate(rec.records))], dtype=np.int64)
+    if form is None:
+        return
+    if form.split(":")[1] == "exp":
+        j, _drawn, spun = be.straggler_samples()
+        assert np.array_equal(j, np.arange(len(batches))), j
+        delay = spun.astype(np.int64)
+    else:
+        delay = np.full(len(batches), int(float(form.split(":")[2]) * 1000), dtype=np.int64)
+    print("CDF %s compute span - delay (us): %s" % (tag, ((spans - delay) / 1e3).round(1).tolist()))
+    assert (spans >= delay).all(), (spans, delay)
+
+
+@pytest.mark.parametrize("form", [None, "0:1.0:50", "0:exp:20"], ids=["none", "fixed", "sampled"])
+@pytest.mark.parametrize("bucket", ["2", "0"])
+def test_lenet_cdf_trajectory(bucket, form, monkeypatch):
+    """Bucketed, the delay sits in the compute chain after the start stamp (_delay_in_chain), and the arrival stamp
+    waits for the small fc gradients' branch; with the single kernel both come after the backward pass."""
+    monkeypatch.setenv("DMNIST_BUCKET", bucket)
+    eng, be, rec = _lenet(256, mode="cdf", straggler=_straggler(form))
+    batches = _batches(eng, 6)
+    _feed(eng, rec, batches)
+    assert eng._bucketed == (bucket == "2") and eng._delay_in_chain == (bucket == "2" and form is not None)
+    _check_cdf("lenet.B256.bucket%s.cdf.%s" % (bucket, form or "none"), eng, be, rec, batches, form)
+
+
+@pytest.mark.parametrize("form", [None, "0:exp:20"], ids=["none", "sampled"])
+def test_mlp2_cdf_trajectory(form, monkeypatch):
+    """The MLP step graph's start stamp: without it read_timing hands the cdf telemetry t_start = 0, a compute time of
+    the whole %globaltimer value."""
+    monkeypatch.setenv("DMNIST_BUCKET", "2")
+    eng, be, rec = _mlp("mlp2", 128, 1024, mode="cdf", straggler=_straggler(form))
+    batches = _batches(eng, 6)
+    _feed(eng, rec, batches)
+    _check_cdf("mlp2.B128.H1024.cdf.%s" % (form or "none"), eng, be, rec, batches, form)
