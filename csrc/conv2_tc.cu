@@ -2,10 +2,12 @@
 // reference op K5 (tf.nn.conv2d #2, src/mnist.py:119-122) = 82 % of the model FLOPs, fused with
 // K2/K3/K4 (bias, ReLU, 2x2 max-pool, src/mnist.py:123-127) in the forward epilogue.
 //
-// No im2col buffer exists anywhere: activations stay NHWC bf16 and a tile's whole receptive field is
-// one 4-D TMA box (channels, 12 pixels of a row, 20 rows, 1 image); the SAME padding halo and the
-// 14 -> 16 row/column round-up are TMA out-of-bounds zero fill.  In fwd and dgrad an M tile is 128 pixels
-// (16 rows x 8 columns, 112 or 84 of them real) of one image; two tiles cover an image.
+// No im2col buffer exists anywhere: activations stay NHWC bf16.  In fwd and dgrad an M tile is 128 real pixels of the
+// batch: 32 consecutive pooled pixels x 4 window positions (fwd) or 128 consecutive pixels (dgrad), so a tile may span
+// two images.  Seen as one stack of B * 14 image rows, its receptive field is at most 16 (fwd) or 14 (dgrad) consecutive
+// full-width rows, staged by ONE TMA box (channels, 14 pixels, rows, 1) of fixed size per tile: 14 / 24.5 KB per stage.
+// Taps whose source pixel lies outside the output pixel's own image (the SAME padding halo, or the neighbouring image in
+// the stack) read a 1 KB zero block instead; a per-lane 25-bit mask, computed once per tile, picks them.
 //
 //   fwd    D[pixel, co]  += X[pixel + tap, ci] (A: registers)  * W[tap][ci][co] (B: MN-major smem, 128B swizzle)
 //   dgrad  D[pixel, ci]  += dY[pixel - tap, co] (A: registers) * W[tap][ci][co] (B: K-major smem,  128B swizzle)
@@ -32,36 +34,78 @@ constexpr int W_BYTES = 800 * 64 * 2;   // 102400
 // (64 B: 16-byte chunk bits [4,5] ^= address bits [7,8]; 128 B: bits [4,6] ^= bits [7,9]); patches start on a
 // 1024-byte boundary.  Swizzling the full address (rather than adding a per-pixel swizzled offset to the base) leaves
 // no loop-invariant per-tap offsets for the compiler to keep live across tiles; that keeps the pipelined tap loops at
-// about 100 registers, so the fc1 update kernel's small CTAs still fit next to conv2_dgrad's in each SM sub-partition.
+// about 80 registers, so the fc1 update kernel's small CTAs still fit next to conv2_dgrad's in each SM sub-partition.
 template <int ROW_BYTES>
 DMNIST_DEVICE uint32_t patch_addr(uint32_t base, int pixel, int chunk) {
   const uint32_t a = base + pixel * ROW_BYTES + chunk * 16;
   return a ^ ((a >> 3) & (ROW_BYTES == 64 ? 0x30 : 0x70));
 }
 
+// Taps (bit kh * 5 + kw) whose source pixel (h + DIR * (kh - 2), w + DIR * (kw - 2)) lies inside the 14 x 14 image; the
+// other taps read SAME padding.  Each coordinate's valid range of kh / kw is contiguous.
+template <int DIR>
+DMNIST_DEVICE uint32_t inside_taps(int h, int w) {
+  const int rlo = max(0, DIR > 0 ? 2 - h : h - 11), rhi = min(4, DIR > 0 ? 15 - h : h + 2);
+  const int clo = max(0, DIR > 0 ? 2 - w : w - 11), chi = min(4, DIR > 0 ? 15 - w : w + 2);
+  const uint32_t rows = (1u << (5 * rhi + 5)) - (1u << (5 * rlo));   // every kw of kh in [rlo, rhi]
+  const uint32_t cols = ((2u << chi) - (1u << clo)) * 0x108421u;      // kw in [clo, chi], repeated for each kh
+  return rows & cols;
+}
+
+// ldmatrix row address of one tap: the staged pixel `pix`, or, for a tap that reads padding, pixel pix mod 8 of the
+// zero block, so the eight rows of a matrix keep the distinct banks they would have had.
+template <int ROW_BYTES>
+DMNIST_DEVICE uint32_t tap_addr(uint32_t patch, uint32_t zero, uint32_t inside, int tap, int pix, int chunk) {
+  const bool in = (inside >> tap) & 1;
+  return patch_addr<ROW_BYTES>(in ? patch : zero, in ? pix : (pix & 7), chunk);
+}
+
+// First row of a tile's receptive field in the batch seen as one stack of B * 14 image rows: two rows above the tile's
+// first pixel row, clipped at the top of its image.
+DMNIST_DEVICE int first_staged_row(int stack_row) { return stack_row - min(stack_row % 14, 2); }
+
 // ------------------------------------------------------------------------------------------------------
 // forward
 // ------------------------------------------------------------------------------------------------------
+constexpr int FW_POOLED = 32;                  // pooled pixels per tile: 128 conv pixels = 32 x 4 window positions
+constexpr int FW_ROWS = 16;                    // staged image rows per tile, the most any tile start needs
 constexpr int FW_STAGES = 4;
-constexpr int FW_A_BYTES = 20 * 12 * 32 * 2;   // ONE patch per tile: 20 rows x 12 pixels x 32 ch = 15 KB, all 25 taps inside
+constexpr int FW_A_BYTES = FW_ROWS * 14 * 32 * 2;   // 14 KB: 16 rows x 14 pixels x 32 ch
 constexpr int FW_ACC_LD = 64 + 4;              // fp32 accumulator staging row (padded)
+constexpr int ZERO_BYTES = 1024;               // 8 zero pixels of up to 128 B, read by the taps that fall in the padding
 struct FwSmem {
   static constexpr int A_OFF = W_BYTES;
-  static constexpr int ACC_OFF = A_OFF + FW_STAGES * FW_A_BYTES;
+  static constexpr int ZERO_OFF = A_OFF + FW_STAGES * FW_A_BYTES;
+  static constexpr int ACC_OFF = ZERO_OFF + ZERO_BYTES;
   static constexpr int BIAS_OFF = ACC_OFF + 128 * FW_ACC_LD * 4;   // 64 floats
   static constexpr int BAR_OFF = BIAS_OFF + 256;
   static constexpr int TOTAL = BAR_OFF + 256 + 1024;
 };
+static_assert(FW_A_BYTES % 1024 == 0 && FwSmem::ZERO_OFF % 1024 == 0, "patches and the zero block must stay 1024-aligned");
+
+// M row r of a forward tile holds window position p = r & 3 of pooled pixel fw_pooled(r).  Each group of 8 rows (one
+// ldmatrix matrix) pairs two pooled pixels 7 apart, i.e. one pooled row apart: 28 staged pixels, so the group's eight conv
+// pixels (+0, +1, +14, +15 and +28, +29, +42, +43) are distinct mod 8 and the gather has no bank conflicts.  Pixels 0-27
+// pair as (l, l + 7) within each half; 28-31 pair as (28, 30), (29, 31), conflict-free unless a pooled row ends between.
+DMNIST_DEVICE int fw_pooled(int r) {
+  const int g = r >> 3, slot = (r >> 2) & 1;
+  return g < 14 ? 14 * (g / 7) + 7 * slot + g % 7 : 28 + 2 * slot + (g - 14);
+}
+DMNIST_DEVICE int fw_row(int l, int p) {
+  const int g = l < 28 ? 7 * (l / 14) + l % 7 : 14 + (l & 1);
+  const int slot = l < 28 ? (l % 14) / 7 : (l >> 1) & 1;
+  return 8 * g + 4 * slot + p;
+}
 
 // The pool epilogue stages the 128 x 64 accumulator tile in shared memory; thread = (pooled pixel, 8 channels) then
 // reads the four window positions of its channels and stores 16 B of activations and 8 B of pooling codes.
 __global__ void __launch_bounds__(CV_THREADS, 1)
-conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,32], box (32,12,20,1), 64B swizzle
+conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 as [B*14 rows][14][32], box (32,14,16,1), 64B swizzle
                  const __grid_constant__ CUtensorMap tmW,   // W [800][64], box (64,200), 128B swizzle
                  const float* __restrict__ bias,            // [64]
                  __nv_bfloat16* __restrict__ out,           // pooled [B,7,7,64]
                  uint8_t* __restrict__ code,                // [B,7,7,64]
-                 int num_tiles) {
+                 int num_tiles, int pooled) {               // pooled = B * 49
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + FwSmem::BAR_OFF);
@@ -79,6 +123,7 @@ conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,
     fence_mbar_init();
   }
   if (threadIdx.x < 64) s_bias[threadIdx.x] = __ldg(bias + threadIdx.x);
+  if (threadIdx.x < ZERO_BYTES / 16) reinterpret_cast<uint4*>(smem + FwSmem::ZERO_OFF)[threadIdx.x] = make_uint4(0, 0, 0, 0);
   __syncthreads();
   pdl_wait();
   // (no early launch_dependents: resident-but-blocked CTAs of the next kernel steal SM resources from this one)
@@ -89,21 +134,23 @@ conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,
       for (int i = 0; i < 4; ++i) tma_load_2d(smem + i * 25600, &tmW, w_full, 0, 200 * i);
       int it = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-        // tile = 16 rows x 8 columns of one image (columns w0 .. w0+7); its receptive field is the 20 x 12 patch
-        // starting at (-2, w0-2).  One TMA box; halo, rows 14-15 and columns 14-15 are OOB zero fill.
-        const int img = t >> 1, w0 = (t & 1) * 8;
+        // tile = pooled pixels [32t, 32t + 32); its receptive field lies in the 16 stack rows from row0 (rows past the
+        // batch are OOB zero fill, and rows the tile does not reach are staged but never read)
+        const int q0 = t * FW_POOLED;
+        const int row0 = first_staged_row((q0 / 49) * 14 + 2 * ((q0 % 49) / 7));
         const int s = it % FW_STAGES;
         mbar_wait(&a_empty[s], ((it / FW_STAGES) & 1) ^ 1);
         mbar_expect_tx(&a_full[s], FW_A_BYTES);
-        tma_load_4d(smem + FwSmem::A_OFF + s * FW_A_BYTES, &tmX, &a_full[s], 0, w0 - 2, -2, img);
+        tma_load_4d(smem + FwSmem::A_OFF + s * FW_A_BYTES, &tmX, &a_full[s], 0, 0, row0, 0);
       }
     }
     return;
   }
 
-  // ldmatrix rows of this lane: tile row r = h * 8 + w (tiles 0/1 of x4: rows +0 / +8, tiles 2/3: channel chunk + 1)
+  // ldmatrix rows of this lane: tile row r (tiles 0/1 of x4: rows +0 / +8, tiles 2/3: channel chunk + 1)
   const int r = 16 * warp + (lane & 7) + ((lane >> 3) & 1) * 8;
-  const int hr = r >> 3, wr = r & 7, kc = lane >> 4;
+  const int lr = fw_pooled(r), pr = r & 3, kc = lane >> 4;
+  const uint32_t zero = smem_u32(smem + FwSmem::ZERO_OFF);
   // W (MN-major, 128B swizzle): k-row = tap * 32 + ci (128 B = 64 co), 8-row groups 1024 B apart; a tap is 4096 B,
   // a K step of 16 ci 2048 B
   const uint64_t db0 = make_smem_desc(smem_u32(smem), 8192, 1024, SWZ_128B);
@@ -113,15 +160,23 @@ conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,
   for (int j = 0; j < 32; ++j) acc[j] = 0.f;
   int it = 0;
   for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-    const int img = t >> 1, w0 = (t & 1) * 8;
+    const int q0 = t * FW_POOLED;
+    const int row0 = first_staged_row((q0 / 49) * 14 + 2 * ((q0 % 49) / 7));
+    // this lane's conv pixel (h, w) of image img; rows of pooled pixels past the batch recompute the last one and are
+    // never stored
+    const int q = min(q0 + lr, pooled - 1);
+    const int img = q / 49, ph = (q % 49) / 7, pw = q % 7;
+    const int h = 2 * ph + (pr >> 1), w = 2 * pw + (pr & 1);
+    const int pix = (img * 14 + h - row0) * 14 + w;
+    const uint32_t inside = inside_taps<1>(h, w);
     const int s = it % FW_STAGES;
     mbar_wait(&a_full[s], (it / FW_STAGES) & 1);
     const uint32_t patch = smem_u32(smem + FwSmem::A_OFF + s * FW_A_BYTES);
-    // A fragments (two 16-channel K steps) of one tap; output pixel (h, w) reads patch pixel (h + kh, w + kw)
+    // A fragments (two 16-channel K steps) of one tap; output pixel (h, w) reads pixel (h + kh - 2, w + kw - 2)
     auto load_tap = [&](int tap, uint32_t (&a)[2][4]) {
-      const int pix = (hr + tap / 5) * 12 + wr + tap % 5;
-      ldsm_x4(patch_addr<64>(patch, pix, kc), a[0]);
-      ldsm_x4(patch_addr<64>(patch, pix, 2 + kc), a[1]);
+      const int p = pix + (tap / 5 - 2) * 14 + tap % 5 - 2;
+      ldsm_x4(tap_addr<64>(patch, zero, inside, tap, p, kc), a[0]);
+      ldsm_x4(tap_addr<64>(patch, zero, inside, tap, p, 2 + kc), a[1]);
     };
     // Two-deep register ring, one commit group per tap: tap + 1 is gathered while tap's wgmmas run.  A buffer is
     // overwritten only after the wgmmas that read it (tap - 1's group) have completed; every wgmma must be able to
@@ -157,15 +212,13 @@ conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,
     }
     named_bar_sync(1, CV_CONSUMERS);
     {
-      // 32 pooled pixels (8 x 4) x 8 groups of 8 channels
-      const int pooled = threadIdx.x >> 3, cg = threadIdx.x & 7;
-      const int ph = pooled >> 2, pwl = pooled & 3;
-      const int pw = (w0 >> 1) + pwl;
-      if (ph < 7 && pw < 7) {
+      // 32 pooled pixels x 8 groups of 8 channels
+      const int l = threadIdx.x >> 3, cg = threadIdx.x & 7;
+      if (q0 + l < pooled) {
         float val[4][8];
 #pragma unroll
         for (int p = 0; p < 4; ++p) {                // window position p = dy * 2 + dx
-          const float* src = s_acc + ((2 * ph + (p >> 1)) * 8 + 2 * pwl + (p & 1)) * FW_ACC_LD + cg * 8;
+          const float* src = s_acc + fw_row(l, p) * FW_ACC_LD + cg * 8;
           const float4 lo = *reinterpret_cast<const float4*>(src), hi = *reinterpret_cast<const float4*>(src + 4);
           val[p][0] = lo.x; val[p][1] = lo.y; val[p][2] = lo.z; val[p][3] = lo.w;
           val[p][4] = hi.x; val[p][5] = hi.y; val[p][6] = hi.z; val[p][7] = hi.w;
@@ -186,7 +239,7 @@ conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,
           if (jj & 1) pk[jj >> 1] = pack_bf16x2(__uint_as_float(pk[jj >> 1]), o);
           else pk[jj >> 1] = __float_as_uint(o);
         }
-        const size_t off = (((size_t)img * 7 + ph) * 7 + pw) * 64 + cg * 8;
+        const size_t off = (size_t)(q0 + l) * 64 + cg * 8;
         *reinterpret_cast<uint4*>(out + off) = make_uint4(pk[0], pk[1], pk[2], pk[3]);
         *reinterpret_cast<uint2*>(code + off) = make_uint2(cd[0], cd[1]);
       }
@@ -197,19 +250,24 @@ conv2_fwd_kernel(const __grid_constant__ CUtensorMap tmX,   // a1 NHWC [B,14,14,
 // ------------------------------------------------------------------------------------------------------
 // dgrad
 // ------------------------------------------------------------------------------------------------------
+constexpr int DG_ROWS = 14;                    // staged image rows per tile, the most any tile start needs
 constexpr int DG_STAGES = 3;
-constexpr int DG_A_BYTES = 20 * 12 * 64 * 2;   // ONE patch per tile: 20 rows x 12 pixels x 64 ch = 30 KB
+constexpr int DG_A_BYTES = DG_ROWS * 14 * 64 * 2;   // 24.5 KB: 14 rows x 14 pixels x 64 ch
+constexpr int DG_A_SLOT = 25 * 1024;                // keeps every patch 1024-aligned (128B swizzle)
+static_assert(DG_A_BYTES <= DG_A_SLOT, "a patch runs into the next stage");
 struct DgSmem {
   static constexpr int A_OFF = W_BYTES;
-  static constexpr int BAR_OFF = A_OFF + DG_STAGES * DG_A_BYTES;
+  static constexpr int ZERO_OFF = A_OFF + DG_STAGES * DG_A_SLOT;
+  static constexpr int BAR_OFF = ZERO_OFF + ZERO_BYTES;
   static constexpr int TOTAL = BAR_OFF + 512 + 1024;
 };
 
 __global__ void __launch_bounds__(CV_THREADS, 1)
-conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,14,64], box (64,12,20,1), 128B swizzle
+conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY as [B*14 rows][14][64], box (64,14,14,1), 128B swizzle
                    const __grid_constant__ CUtensorMap tmW,
                    __nv_bfloat16* __restrict__ dx,            // [B,14,14,32]
-                   int num_tiles, unsigned long long* __restrict__ dbg) {   // dbg: optional timeline of CTA 0
+                   int num_tiles, int pixels,                 // pixels = B * 196
+                   unsigned long long* __restrict__ dbg) {    // dbg: optional timeline of CTA 0
   extern __shared__ uint8_t smem_raw[];
   uint8_t* smem = reinterpret_cast<uint8_t*>((reinterpret_cast<uintptr_t>(smem_raw) + 1023) & ~uintptr_t(1023));
   uint64_t* a_full = reinterpret_cast<uint64_t*>(smem + DgSmem::BAR_OFF);
@@ -224,6 +282,7 @@ conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,1
     mbar_init(w_full, 1);
     fence_mbar_init();
   }
+  if (threadIdx.x < ZERO_BYTES / 16) reinterpret_cast<uint4*>(smem + DgSmem::ZERO_OFF)[threadIdx.x] = make_uint4(0, 0, 0, 0);
   const bool dbg_on = dbg != nullptr && blockIdx.x == 0;
   if (dbg_on && threadIdx.x == 0) dbg[0] = globaltimer_ns();
   __syncthreads();
@@ -237,19 +296,18 @@ conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,1
       for (int i = 0; i < 4; ++i) tma_load_2d(smem + i * 25600, &tmW, w_full, 0, 200 * i);
       int it = 0;
       for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-        const int img = t >> 1, w0 = (t & 1) * 8;
         const int s = it % DG_STAGES;
         mbar_wait(&a_empty[s], ((it / DG_STAGES) & 1) ^ 1);
         if (dbg_on && it < 20) dbg[8 + it] = globaltimer_ns();          // producer: slot free, issuing load `it`
         mbar_expect_tx(&a_full[s], DG_A_BYTES);
-        // dX[y,x] += dY[y + 2 - kh, x + 2 - kw] * W[kh,kw]: same 20 x 12 patch at (-2, w0-2); tap (kh,kw)
-        // starts (4-kh) rows and (4-kw) pixels into it
-        tma_load_4d(smem + DgSmem::A_OFF + s * DG_A_BYTES, &tmDY, &a_full[s], 0, w0 - 2, -2, img);
+        // tile = pixels [128t, 128t + 128); dX[y,x] += dY[y + 2 - kh, x + 2 - kw] * W[kh,kw] reaches two rows either side
+        tma_load_4d(smem + DgSmem::A_OFF + s * DG_A_SLOT, &tmDY, &a_full[s], 0, 0, first_staged_row(t * 128 / 14), 0);
       }
     }
   } else {
     const int r = 16 * warp + (lane & 7) + ((lane >> 3) & 1) * 8;
-    const int hr = r >> 3, wr = r & 7, kc = lane >> 4;
+    const int kc = lane >> 4;
+    const uint32_t zero = smem_u32(smem + DgSmem::ZERO_OFF);
     // W[tap] as B: 32 ci rows x 64 co, K-major (128 B rows, 8-row groups 1024 B apart); a K step of 16 co = 32 B
     const uint64_t db0 = make_smem_desc(smem_u32(smem), 16, 1024, SWZ_128B);
     mbar_wait(w_full, 0);
@@ -259,16 +317,21 @@ conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,1
     for (int j = 0; j < 16; ++j) acc[j] = 0.f;
     int it = 0;
     for (int t = blockIdx.x; t < num_tiles; t += gridDim.x, ++it) {
-      const int img = t >> 1, w0 = (t & 1) * 8;
+      const int g0 = t * 128;
+      // this lane's pixel: M row r of the tile; rows past the batch recompute the last pixel and are never stored
+      const int g = min(g0 + r, pixels - 1);
+      const int row = g / 14, w = g % 14;
+      const int pix = g - first_staged_row(g0 / 14) * 14;
+      const uint32_t inside = inside_taps<-1>(row % 14, w);
       const int s = it % DG_STAGES;
       mbar_wait(&a_full[s], (it / DG_STAGES) & 1);
       if (dbg_on && threadIdx.x == 0 && it < 20) dbg[32 + it] = globaltimer_ns();   // MMA: data of load `it` landed
-      const uint32_t patch = smem_u32(smem + DgSmem::A_OFF + s * DG_A_BYTES);
-      // A fragments (four 16-channel K steps) of one tap; tap (kh, kw) reads patch pixel (h + 4 - kh, w + 4 - kw)
+      const uint32_t patch = smem_u32(smem + DgSmem::A_OFF + s * DG_A_SLOT);
+      // A fragments (four 16-channel K steps) of one tap; tap (kh, kw) reads pixel (h + 2 - kh, w + 2 - kw)
       auto load_tap = [&](int tap, uint32_t (&a)[4][4]) {
-        const int pix = (hr + 4 - tap / 5) * 12 + wr + 4 - tap % 5;
+        const int p = pix + (2 - tap / 5) * 14 + 2 - tap % 5;
 #pragma unroll
-        for (int k = 0; k < 4; ++k) ldsm_x4(patch_addr<128>(patch, pix, 2 * k + kc), a[k]);
+        for (int k = 0; k < 4; ++k) ldsm_x4(tap_addr<128>(patch, zero, inside, tap, p, 2 * k + kc), a[k]);
       };
       // Same two-deep register ring as the forward tap loop.
       uint32_t a[2][4][4];
@@ -294,10 +357,9 @@ conv2_dgrad_kernel(const __grid_constant__ CUtensorMap tmDY,  // dY NHWC [B,14,1
       const int r0 = 16 * warp + (lane >> 2);
 #pragma unroll
       for (int half = 0; half < 2; ++half) {
-        const int rr = r0 + 8 * half;
-        const int h = rr >> 3, w = w0 + (rr & 7);
-        if (h < 14 && w < 14) {
-          __nv_bfloat16* o = dx + (((size_t)img * 14 + h) * 14 + w) * 32 + 2 * (lane & 3);
+        const int gg = g0 + r0 + 8 * half;
+        if (gg < pixels) {
+          __nv_bfloat16* o = dx + (size_t)gg * 32 + 2 * (lane & 3);
 #pragma unroll
           for (int j = 0; j < 4; ++j)
             *reinterpret_cast<uint32_t*>(o + 8 * j) = pack_bf16x2(acc[4 * j + 2 * half], acc[4 * j + 2 * half + 1]);
@@ -474,7 +536,7 @@ extern "C" {
 int dm_conv2_fwd(const void* a1, const void* w_bf16, const void* bias, void* out, void* code, int B, void* stream) {
   using namespace dm;
   CUtensorMap tmX, tmW;
-  if (make_tmap_nhwc_bf16(&tmX, a1, 32, 14, 14, B, 32, 12, 20, 64)) return 101;
+  if (make_tmap_nhwc_bf16(&tmX, a1, 32, 14, 14 * B, 1, 32, 14, FW_ROWS, 64)) return 101;
   if (make_tmap_2d_bf16(&tmW, w_bf16, 64, 800, 64, 64, 200, 128)) return 102;
   static bool configured = false;
   if (!configured) {
@@ -482,18 +544,18 @@ int dm_conv2_fwd(const void* a1, const void* w_bf16, const void* bias, void* out
     DM_CUDA_OK(cudaFuncSetAttribute(conv2_fwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }
-  const int tiles = 2 * B;
+  const int tiles = (B * 49 + FW_POOLED - 1) / FW_POOLED;
   const int grid = tiles < num_sms() ? tiles : num_sms();
   return (int)launch_kernel(conv2_fwd_kernel, dim3(grid), dim3(CV_THREADS), FwSmem::TOTAL,
                             reinterpret_cast<cudaStream_t>(stream), tmX, tmW, reinterpret_cast<const float*>(bias),
-                            reinterpret_cast<__nv_bfloat16*>(out), reinterpret_cast<uint8_t*>(code), tiles);
+                            reinterpret_cast<__nv_bfloat16*>(out), reinterpret_cast<uint8_t*>(code), tiles, B * 49);
 }
 
 // dy: [B,14,14,64] bf16 -> dx: [B,14,14,32] bf16
 int dm_conv2_dgrad(const void* dy, const void* w_bf16, void* dx, int B, void* stream) {
   using namespace dm;
   CUtensorMap tmDY, tmW;
-  if (make_tmap_nhwc_bf16(&tmDY, dy, 64, 14, 14, B, 64, 12, 20, 128)) return 101;
+  if (make_tmap_nhwc_bf16(&tmDY, dy, 64, 14, 14 * B, 1, 64, 14, DG_ROWS, 128)) return 101;
   if (make_tmap_2d_bf16(&tmW, w_bf16, 64, 800, 64, 64, 200, 128)) return 102;
   static bool configured = false;
   if (!configured) {
@@ -501,11 +563,11 @@ int dm_conv2_dgrad(const void* dy, const void* w_bf16, void* dx, int B, void* st
     DM_CUDA_OK(cudaFuncSetAttribute(conv2_dgrad_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }
-  const int tiles = 2 * B;
+  const int tiles = (B * 196 + 127) / 128;
   const int grid = tiles < max_ctas() ? tiles : max_ctas();
   return (int)launch_kernel(conv2_dgrad_kernel, dim3(grid), dim3(CV_THREADS), DgSmem::TOTAL,
                             reinterpret_cast<cudaStream_t>(stream), tmDY, tmW, reinterpret_cast<__nv_bfloat16*>(dx), tiles,
-                            static_cast<unsigned long long*>(nullptr));
+                            B * 196, static_cast<unsigned long long*>(nullptr));
 }
 
 // g_w ([25][32][64] fp32) must be zeroed by the caller; the gradient is added to it.  Two launches: the weight-gradient

@@ -63,16 +63,39 @@ def run_conv1_wgrad(x, dpool, code, tc: bool = True):
     return gw, gb
 
 
-def run_conv2_fwd(a1, w, b):
+def _output(shape, dtype, guard: int = 0) -> torch.Tensor:
+    """A zeroed output buffer; with ``guard`` > 0 the head of an allocation ``guard`` elements longer, all of it poison:
+    NaN, or 0xFF for pooling codes (a code is an argmax position 0-3 plus the ReLU flag 4).  ``unwritten_results``
+    then finds every element the kernel left alone and every element it wrote past the end."""
+    if not guard:
+        return torch.zeros(shape, dtype=dtype, device="cuda")
+    n = int(np.prod(shape))
+    fill = 0xFF if dtype == torch.uint8 else float("nan")
+    return torch.full((n + guard,), fill, dtype=dtype, device="cuda")[:n].view(shape)
+
+
+def unwritten_results(tag: str, t: torch.Tensor, guard: int) -> List[Result]:
+    """Poison left inside ``t`` (elements never written) and guard elements past its end that are no longer poison
+    (writes out of bounds); both must be 0.  ``t`` comes from ``_output(..., guard)``."""
+    full = torch.as_strided(t, (t.numel() + guard,), (1,), t.storage_offset())
+    poison = full == 0xFF if t.dtype == torch.uint8 else torch.isnan(full)
+    n = t.numel()
+    return [(tag + ".unwritten", float(poison[:n].sum()), 0.0),
+            (tag + ".written_past_end", float((~poison[n:]).sum()), 0.0)]
+
+
+def run_conv2_fwd(a1, w, b, guard: int = 0):
+    """``guard``: see ``_output``."""
     B = a1.shape[0]
-    out = torch.zeros(B, 7, 7, 64, dtype=BF, device="cuda")
-    code = torch.zeros(B, 7, 7, 64, dtype=torch.uint8, device="cuda")
+    out = _output((B, 7, 7, 64), BF, guard)
+    code = _output((B, 7, 7, 64), torch.uint8, guard)
     load().dm_conv2_fwd(a1, w, b, out, code, B, stream_ptr())
     return out, code
 
 
-def run_conv2_dgrad(dy, w):
-    dx = torch.zeros(dy.shape[0], 14, 14, 32, dtype=BF, device="cuda")
+def run_conv2_dgrad(dy, w, guard: int = 0):
+    """``guard``: see ``_output``."""
+    dx = _output((dy.shape[0], 14, 14, 32), BF, guard)
     load().dm_conv2_dgrad(dy, w, dx, dy.shape[0], stream_ptr())
     return dx
 
@@ -313,13 +336,17 @@ def conv2_fwd_results(tag: str, kind: str, a1, w, b, out, code) -> List[Result]:
     return _pool_results(tag, kind, out, code, z, za, b, 800)
 
 
-def check_conv2_fwd(B: int = 8, seed: int = 1, kinds: Sequence[str] = KINDS) -> List[Result]:
+def check_conv2_fwd(B: int = 8, seed: int = 1, kinds: Sequence[str] = KINDS, guard: int = 0) -> List[Result]:
+    """``guard`` > 0: the outputs start out as poison with a poisoned guard tail (``_output``), and the check also counts
+    elements left unwritten or written past the end."""
     res: List[Result] = []
     for kind in kinds:
         tag = "conv2_fwd.%s" % kind
         a1, w, b = _dev(*_conv2_data(kind, _gen(seed), B))
-        out, code = run_conv2_fwd(a1, w, b)
+        out, code = run_conv2_fwd(a1, w, b, guard)
         res += conv2_fwd_results(tag, kind, a1, w, b, out, code)
+        if guard:
+            res += unwritten_results(tag + ".out", out, guard) + unwritten_results(tag + ".code", code, guard)
     return res
 
 
@@ -330,7 +357,8 @@ def conv2_dgrad_results(tag: str, kind: str, dy, w, dx) -> List[Result]:
     return R.compare(tag, kind, dx, ref, R.fp32_slack(ra, 1600))
 
 
-def check_conv2_dgrad(B: int = 8, seed: int = 2, kinds: Sequence[str] = KINDS) -> List[Result]:
+def check_conv2_dgrad(B: int = 8, seed: int = 2, kinds: Sequence[str] = KINDS, guard: int = 0) -> List[Result]:
+    """``guard``: as in ``check_conv2_fwd``."""
     res: List[Result] = []
     for kind in kinds:
         tag = "conv2_dgrad.%s" % kind
@@ -340,7 +368,10 @@ def check_conv2_dgrad(B: int = 8, seed: int = 2, kinds: Sequence[str] = KINDS) -
         else:
             dy, w = _bf(R.grid(g, (B, 14, 14, 64), -4, 4)), _bf(R.grid(g, (5, 5, 32, 64), -8, 8, 64))
         dy, w = _dev(dy, w)
-        res += conv2_dgrad_results(tag, kind, dy, w, run_conv2_dgrad(dy, w))
+        dx = run_conv2_dgrad(dy, w, guard)
+        res += conv2_dgrad_results(tag, kind, dy, w, dx)
+        if guard:
+            res += unwritten_results(tag + ".dx", dx, guard)
     return res
 
 
