@@ -294,6 +294,12 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
         const int pos = col0 >> 6, ch0 = col0 & 63;
         const int ph = pos / 7, pw = pos - ph * 7;
         float gs[32];                                   // masked gradient (bias-gradient contribution)
+        // The tile's 128 rows x 4 pixels x 64 channels are staged in the (idle) ring, 512 B per row, and then stored a
+        // row per warp instruction: 4 whole 128-byte lines (a lane per row would write 16 B into each of 32 lines per
+        // instruction, and the stores would take most of the kernel's time).
+        // 16-byte chunk j = 8 q4 + 4 half + k of row r sits at j ^ (r & 7): staging and reading are conflict-free.
+        uint4* s_dy = reinterpret_cast<uint4*>(smem);
+        named_bar_sync(1, GEMM_CONSUMERS);              // every thread has read its accumulator row from the ring
         if (row < p.M) {
           // code byte = argmax position (bits 0-1) | ReLU active (bit 2).  Byte-parallel: for window position q4,
           // x = (codes & 7) ^ (4 | q4) is zero exactly in the matching bytes; x + 0x7f sets bit 7 of the others
@@ -304,11 +310,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
           for (int j = 0; j < 16; ++j) pk[j] = pack_bf16x2(__uint_as_float(v[2 * j]), __uint_as_float(v[2 * j + 1]));
 #pragma unroll
           for (int j = 0; j < 32; ++j) gs[j] = ((cw[j >> 2] >> ((j & 3) * 8)) & 4u) ? __uint_as_float(v[j]) : 0.f;
-          __nv_bfloat16* dy = reinterpret_cast<__nv_bfloat16*>(p.out);
 #pragma unroll
           for (int q4 = 0; q4 < 4; ++q4) {              // the four pixels of the 2x2 window: 64 B each
-            const int y = 2 * ph + (q4 >> 1), x = 2 * pw + (q4 & 1);
-            uint4* dst = reinterpret_cast<uint4*>(dy + (((size_t)row * 14 + y) * 14 + x) * 64 + ch0);
             uint32_t o[16];
 #pragma unroll
             for (int w8 = 0; w8 < 8; ++w8) {            // code word w8 <-> channels 4*w8 .. 4*w8+3 <-> pk[2*w8], pk[2*w8+1]
@@ -318,11 +321,22 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
               o[2 * w8 + 1] = pk[2 * w8 + 1] & prmt(hit, 0u, 0xbbaau);  // bytes {2,2,3,3}
             }
 #pragma unroll
-            for (int k = 0; k < 4; ++k) dst[k] = make_uint4(o[4 * k], o[4 * k + 1], o[4 * k + 2], o[4 * k + 3]);
+            for (int k = 0; k < 4; ++k)
+              s_dy[lr * 32 + ((8 * q4 + 4 * half + k) ^ (lr & 7))] = make_uint4(o[4 * k], o[4 * k + 1], o[4 * k + 2], o[4 * k + 3]);
           }
         } else {
 #pragma unroll
           for (int j = 0; j < 32; ++j) gs[j] = 0.f;
+        }
+        named_bar_sync(1, GEMM_CONSUMERS);
+        {
+          __nv_bfloat16* dy = reinterpret_cast<__nv_bfloat16*>(p.out);
+          const int q4 = lane >> 3, cc = lane & 7;      // pixel of the window, 16-byte chunk of its 64 channels
+          const int y = 2 * ph + (q4 >> 1), x = 2 * pw + (q4 & 1);
+#pragma unroll 4
+          for (int r = warp; r < GEMM_BM; r += GEMM_CONSUMERS / 32)
+            if (m0 + r < p.M)
+              *reinterpret_cast<uint4*>(dy + (((size_t)(m0 + r) * 14 + y) * 14 + x) * 64 + 8 * cc) = s_dy[r * 32 + (lane ^ (r & 7))];
         }
         // column sums over the warp's 32 rows: butterfly transpose-reduce (31 shuffles), lane l ends with channel ch0 + l
 #pragma unroll
@@ -350,11 +364,35 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
       g_unpool_bias_part[cta * 64 + threadIdx.x] =
           s_bpart[threadIdx.x] + s_bpart[64 + threadIdx.x] + s_bpart[128 + threadIdx.x] + s_bpart[192 + threadIdx.x];
     volatile unsigned int* s_flag = reinterpret_cast<volatile unsigned int*>(smem + S::BPART_OFFSET + 1024);
-    if (arrive_last_cta(&g_unpool_ticket, gridDim.x * gridDim.y, 1, GEMM_CONSUMERS, s_flag) && threadIdx.x < 16) {
-      const float4 sum = ordered_sum4(reinterpret_cast<const float4*>(g_unpool_bias_part) + threadIdx.x,
-                                      gridDim.x * gridDim.y, 16);
-      float* o = p.g_bias + 4 * threadIdx.x;
-      o[0] += sum.x; o[1] += sum.y; o[2] += sum.z; o[3] += sum.w;
+    const int nslots = gridDim.x * gridDim.y;
+    if (arrive_last_cta(&g_unpool_ticket, nslots, 1, GEMM_CONSUMERS, s_flag)) {
+      // channel c = the CTAs' values added in CTA order (thread c < 64).  All consumer threads first copy a chunk of
+      // slots into the idle ring, 4 loads in flight each, so this tail of the launch waits for one L2 round trip per
+      // 64 slots.
+      constexpr int CHUNK = S::BAR_OFFSET / 256;     // slots of 64 floats
+      float4* s_slots = reinterpret_cast<float4*>(smem);
+      const float4* src = reinterpret_cast<const float4*>(g_unpool_bias_part);
+      float sum = 0.f;
+      for (int k0 = 0; k0 < nslots; k0 += CHUNK) {
+        const int n4 = min(CHUNK, nslots - k0) * 16;
+        for (int i0 = threadIdx.x; i0 < n4; i0 += 4 * GEMM_CONSUMERS) {
+          float4 v[4];
+#pragma unroll
+          for (int u = 0; u < 4; ++u)
+            if (i0 + u * GEMM_CONSUMERS < n4) v[u] = __ldcg(src + (size_t)k0 * 16 + i0 + u * GEMM_CONSUMERS);
+#pragma unroll
+          for (int u = 0; u < 4; ++u)
+            if (i0 + u * GEMM_CONSUMERS < n4) s_slots[i0 + u * GEMM_CONSUMERS] = v[u];
+        }
+        named_bar_sync(1, GEMM_CONSUMERS);
+        if (threadIdx.x < 64) {
+          const float* sp = reinterpret_cast<const float*>(s_slots) + threadIdx.x;
+#pragma unroll 8
+          for (int k = 0; k < n4 / 16; ++k) sum += sp[k * 64];
+        }
+        named_bar_sync(1, GEMM_CONSUMERS);
+      }
+      if (threadIdx.x < 64) p.g_bias[threadIdx.x] += sum;
     }
   }
   if (DECAY) {
