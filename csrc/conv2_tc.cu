@@ -387,6 +387,8 @@ constexpr int WG_A_SLOT = 21 * 1024;                 // keeps the dY tile 1024-a
 constexpr int WG_B_BYTES = 16 * WG_KSTEPS * 64 * 2;  // 26624: the dY tile
 constexpr int WG_STAGE_BYTES = WG_A_SLOT + WG_B_BYTES;
 constexpr int WG_GROUPS = 7;
+constexpr int WG_FOLD = 64;                          // images per wgmma accumulator stretch (even: a loop step is 2 images)
+static_assert(WG_FOLD % 2 == 0, "the image loop folds at the start of a step");
 static_assert(WG_A_BYTES <= WG_A_SLOT, "the patch runs into the dY tile");
 struct WgSmem {
   static constexpr int BAR_OFF = WG_STAGES * WG_STAGE_BYTES;
@@ -448,9 +450,12 @@ conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,18
   // patch pixel of this chunk's tap window for image pixel 0; group 6 chunks 1-3 are padding
   const int tap_px = group < 5 ? q * 18 + group : (group == 5 ? 4 * 18 + q : 4 * 18 + 4);
   const bool real_chunk = group < 6 || q == 0;
-  float acc[32];
+  // The wgmma accumulator holds at most WG_FOLD images: the tensor cores do not round their fp32 accumulation to nearest,
+  // and the error of one accumulator grows with the K steps it collects (a single split of 4133 images came to a
+  // normwise 9.1e-4 of the float64 gradient on an H100).  Each full stretch is then added to `folded` in fp32.
+  float acc[32], folded[32];
 #pragma unroll
-  for (int j = 0; j < 32; ++j) acc[j] = 0.f;
+  for (int j = 0; j < 32; ++j) acc[j] = folded[j] = 0.f;
   fence_regs(acc);
   // One commit group per K step and a two-deep register ring running across image boundaries, as in the forward tap
   // loop: step k + 1's A fragment is gathered while step k's wgmma runs, and only the wait_group 1 after step k + 1
@@ -463,6 +468,16 @@ conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,18
   int s = 0, s_prev = 0;
   uint32_t phase = 0;
   for (int i0 = 0; i0 < ni; i0 += 2) {
+    if (i0 != 0 && i0 % WG_FOLD == 0) {
+      wgmma_wait<0>();
+      fence_regs(acc);
+#pragma unroll
+      for (int j = 0; j < 32; ++j) {
+        folded[j] += acc[j];
+        acc[j] = 0.f;
+      }
+      fence_regs(acc);
+    }
 #pragma unroll
     for (int k = 0; k < 2 * WG_KSTEPS; ++k) {
       const int ks = k % WG_KSTEPS;
@@ -496,6 +511,10 @@ conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,18
   }
   wgmma_wait<0>();
   fence_regs(acc);
+  if (ni > WG_FOLD) {                              // a split of at most WG_FOLD images stores its accumulator as it is
+#pragma unroll
+    for (int j = 0; j < 32; ++j) acc[j] += folded[j];
+  }
 
   const int ci0 = 16 * (warp & 1) + (lane >> 2);
   float* part = g_c2wg_part + (size_t)blockIdx.x * WG_PART_FLOATS;

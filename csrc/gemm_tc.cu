@@ -72,6 +72,8 @@ constexpr int UNPOOL_MAX_CTAS = 4096;                  // batch <= 4096 / 49 row
 __device__ float g_unpool_bias_part[UNPOOL_MAX_CTAS * 64];
 __device__ unsigned int g_unpool_ticket;
 
+int fc1_dgrad_unpool_max_batch() { return UNPOOL_MAX_CTAS / (3136 / 64) * GEMM_BM; }
+
 template <int BN, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
 gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ CUtensorMap tmB, GemmParams p) {

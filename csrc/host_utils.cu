@@ -106,6 +106,15 @@ extern "C" int dm_get_max_ctas() { return dm::g_max_ctas; }
 
 extern "C" int dm_num_sms() { return dm::num_sms(); }
 
+// The largest batch every kernel of the LeNet training step and evaluation accepts (DESIGN.md §3, "Batch limit"):
+// fc1_dgrad_unpool's 4096 bias-gradient slots at 49 per 128-row tile (10 624 rows) and fc2_fwd_bwd's 65 536 per-row
+// loss slots.  Every other LeNet kernel loops over the batch or caps its grid, and the evaluation runs in chunks of
+// at most dm_eval_max_rows() rows whatever the batch.
+extern "C" int dm_lenet_max_batch() {
+  const int a = dm::fc1_dgrad_unpool_max_batch(), b = dm::fc2_fwd_bwd_max_batch();
+  return a < b ? a : b;
+}
+
 extern "C" int dm_set_pdl(int on) {
   dm::g_pdl = on ? 1 : 0;
   return dm::g_pdl;

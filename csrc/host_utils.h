@@ -62,6 +62,10 @@ int make_tmap_2d_bf16(CUtensorMap* out, const void* base, uint64_t inner, uint64
 int make_tmap_nhwc_bf16(CUtensorMap* out, const void* base, int C, int W, int H, int N, uint32_t box_c,
                         uint32_t box_w, uint32_t box_h, int swizzle_bytes);
 
+// The largest batch a LeNet kernel with a workspace sized at compile time accepts; dm_lenet_max_batch is their minimum.
+int fc1_dgrad_unpool_max_batch();   // gemm_tc.cu
+int fc2_fwd_bwd_max_batch();        // lenet_simt.cu
+
 // Rows `idx[0..batch)` of a device-resident training set (fp32 images [N, 784], int64 labels [N]) -> an input slot in
 // pack_batch's layout (csrc/batch_gather.cu).
 cudaError_t launch_gather_batch(const int32_t* idx, const float* images, const int64_t* labels, int batch, void* slot,

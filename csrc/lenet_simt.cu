@@ -55,6 +55,8 @@ constexpr int F2_MAX_ROWS = 1 << 16;                      // batch limit of dm_f
 __device__ float g_f2_row_terms[F2_MAX_ROWS * 2];
 __device__ unsigned int g_f2_ticket;
 
+int fc2_fwd_bwd_max_batch() { return F2_MAX_ROWS; }
+
 __global__ void __launch_bounds__(F2_THREADS) fc2_fwd_bwd_kernel(Fc2Args a) {
   __shared__ float s_part[F2_THREADS / 32][DL_LD];
   const int t = threadIdx.x, warp = t >> 5, lane = t & 31;

@@ -726,11 +726,23 @@ class _CudaEngine(ComputeEngine):
         return tot_loss / n, tot_hit / n
 
 
+def check_lenet_batch(batch_size: int) -> None:
+    """Refuse a batch the LeNet kernels cannot run, before anything is allocated or launched.  The limit is
+    ``dm_lenet_max_batch()``: fc1_dgrad_unpool keeps one conv2 bias-gradient slot per CTA in a workspace of 4096 slots,
+    49 CTAs per 128-row tile (DESIGN.md §3, "Batch limit")."""
+    limit = int(load().dm_lenet_max_batch())
+    if not 1 <= batch_size <= limit:
+        raise ValueError("--batch_size=%d is outside what the LeNet kernels on the GPU path can run: use 1 <= --batch_size "
+                         "<= %d (fc1_dgrad_unpool keeps one conv2 bias-gradient slot per CTA, 4096 slots for 49 CTAs per "
+                         "128 rows)" % (batch_size, limit))
+
+
 class CudaLeNetEngine(_CudaEngine):
     _main_priority = -1           # see _side
 
     def __init__(self, batch_size: int, backend: FusedBackend, seed: int = 66478, rank: int = 0,
                  keep_prob: float = 0.5, use_graph: bool = True):
+        check_lenet_batch(batch_size)
         super().__init__(get_model("lenet")[0], batch_size, backend, seed, use_graph, (28, 28))
         B, dev = batch_size, self.device
         self.seed, self.rank, self.keep_prob = seed, rank, keep_prob

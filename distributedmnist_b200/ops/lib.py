@@ -120,6 +120,7 @@ def _signatures() -> dict:
         "dm_set_max_ctas": (V, i, [i]),
         "dm_get_max_ctas": (V, i, []),
         "dm_num_sms": (V, i, []),
+        "dm_lenet_max_batch": (V, i, []),
         "dm_set_pdl": (V, i, [i]),
         "dm_device_cc": (V, i, [i]),
         # lenet_simt.cu, mlp_simt.cu, moving_average.cu

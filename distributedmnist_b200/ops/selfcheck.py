@@ -41,6 +41,54 @@ def _dev(*ts):
 
 
 # ---------------------------------------------------------------------------------------------------------------------
+# references of large batches, a chunk of rows at a time
+# ---------------------------------------------------------------------------------------------------------------------
+REF_ROWS = 1024        # batch rows per float64 reference evaluation: a conv1 activation of 1024 rows is 206 MB in float64
+
+
+def row_slices(B: int) -> List[slice]:
+    return [slice(r, min(B, r + REF_ROWS)) for r in range(0, B, REF_ROWS)]
+
+
+def merge_row_chunks(parts: Sequence[List[Result]], rows: Sequence[int]) -> List[Result]:
+    """The results of the same comparisons on row chunks of the same outputs, as if made on the whole outputs: counts add
+    up, ``[inexact]`` fractions are weighted by rows (each row holds as many elements), ``[err/bound]`` ratios take the
+    maximum.  A normwise ``[rel]`` error does not split into chunks and is refused."""
+    if len(parts) == 1:
+        return list(parts[0])
+    merged: List[Result] = []
+    for i, (name, _, tol) in enumerate(parts[0]):
+        assert all(p[i][0] == name and p[i][2] == tol for p in parts), name
+        vals = [p[i][1] for p in parts]
+        if name.endswith("[inexact]"):
+            v = sum(x * n for x, n in zip(vals, rows)) / sum(rows)
+        elif name.endswith("[err/bound]"):
+            v = max(vals)
+        elif name.endswith("[rel]"):
+            raise ValueError("%s: a normwise error does not split into row chunks" % name)
+        else:
+            v = sum(vals)
+        merged.append((name, float(v), tol))
+    return merged
+
+
+def by_rows(fn, B: int, *rows: torch.Tensor) -> List[Result]:
+    """``fn`` on chunks of REF_ROWS batch rows of each tensor in ``rows``, its results merged (:func:`merge_row_chunks`)."""
+    slices = row_slices(B)
+    return merge_row_chunks([fn(*(t[s] for t in rows)) for s in slices], [s.stop - s.start for s in slices])
+
+
+def sum_by_rows(fn, B: int, *rows: torch.Tensor):
+    """The float64 sum over chunks of REF_ROWS batch rows of ``fn``'s results (a tensor or a tuple of tensors): a weight
+    gradient reference over the whole batch without the whole batch's float64 activations."""
+    total = None
+    for s in row_slices(B):
+        r = fn(*(t[s] for t in rows))
+        total = r if total is None else (tuple(a + b for a, b in zip(total, r)) if isinstance(r, tuple) else total + r)
+    return total
+
+
+# ---------------------------------------------------------------------------------------------------------------------
 # launchers: one kernel, fresh outputs
 # ---------------------------------------------------------------------------------------------------------------------
 def run_conv1_fwd(x, w, b):
@@ -167,9 +215,13 @@ def run_fc2_wgrad_decay(h, dl, dh, w2, b2, b1, lam: float, part=None):
     return gw2, gb2, gb1, part
 
 
-def run_fc1_dgrad_unpool(dh, w1, code2):
+def run_fc1_dgrad_unpool(dh, w1, code2, guard: int = 0):
+    """``guard``: see ``_output`` (without it dy2 starts out as 7, which every element must overwrite)."""
     B = dh.shape[0]
-    dy = torch.full((B, 14, 14, 64), 7.0, dtype=BF, device="cuda")      # every element must be overwritten
+    if guard:
+        dy = _output((B, 14, 14, 64), BF, guard)
+    else:
+        dy = torch.full((B, 14, 14, 64), 7.0, dtype=BF, device="cuda")
     gb = torch.zeros(64, device="cuda")
     load().dm_fc1_dgrad_unpool(dh, w1, code2, dy, gb, B, stream_ptr())
     return dy, gb
@@ -276,12 +328,16 @@ def _pool_results(tag: str, kind: str, out, code, z, za, bias, n_terms: int) -> 
 
 def conv1_fwd_results(tag: str, kind: str, x, w, b, out, code) -> List[Result]:
     """conv1_fwd's pooled output and codes from images x [B,28,28] fp32, weights w [5,5,1,32] fp32, bias b."""
-    x, w = x.to(BF), w.to(BF)       # the kernel rounds its operands to bf16 (grid values are bf16 numbers already)
-    z = R.conv5x5(x[..., None], w)
-    za = R.conv5x5(x.abs()[..., None], w.abs())
-    if kind != "rand":
-        R.assert_exact_grid(za + b.abs().double().max(), 1.0 / 512, tag)
-    return _pool_results(tag, kind, out, code, z, za, b, 25)
+    w = w.to(BF)                    # the kernel rounds its operands to bf16 (grid values are bf16 numbers already)
+
+    def rows(x, out, code):
+        x = x.to(BF)
+        z = R.conv5x5(x[..., None], w)
+        za = R.conv5x5(x.abs()[..., None], w.abs())
+        if kind != "rand":
+            R.assert_exact_grid(za + b.abs().double().max(), 1.0 / 512, tag)
+        return _pool_results(tag, kind, out, code, z, za, b, 25)
+    return by_rows(rows, x.shape[0], x, out, code)
 
 
 def check_conv1_fwd(B: int = 8, seed: int = 0, kinds: Sequence[str] = KINDS) -> List[Result]:
@@ -320,9 +376,9 @@ def check_conv1_wgrad(B: int = 8, seed: int = 7, kinds: Sequence[str] = KINDS, s
 def conv1_wgrad_results(tag: str, kind: str, x, dp, code, gw, gb) -> List[Result]:
     """conv1 weight [25,32] / bias gradients from images x [B,28,28] fp32, d pool1 output dp and pool1 codes."""
     xr = x.to(BF)                       # the kernel rounds the images to bf16
-    rw, rb = R.conv1_wgrad(xr, dp, code)
+    rw, rb = sum_by_rows(R.conv1_wgrad, x.shape[0], xr, dp, code)
     if kind == "grid":
-        aw, ab = R.conv1_wgrad(xr.abs(), dp.abs(), code)
+        aw, ab = sum_by_rows(lambda x, d, c: R.conv1_wgrad(x.abs(), d.abs(), c), x.shape[0], xr, dp, code)
         R.assert_exact_grid(aw, 1.0 / 8, tag + ".g_w")
         R.assert_exact_grid(ab, 1.0, tag + ".g_b")
     return R.compare(tag + ".g_w", kind, gw, rw) + R.compare(tag + ".g_b", kind, gb, rb)
@@ -330,10 +386,12 @@ def conv1_wgrad_results(tag: str, kind: str, x, dp, code, gw, gb) -> List[Result
 
 def conv2_fwd_results(tag: str, kind: str, a1, w, b, out, code) -> List[Result]:
     """conv2_fwd's pooled output and codes [B,7,7,64] from a1 and the bf16 weights w."""
-    z, za = R.conv5x5(a1, w), R.conv5x5(a1.abs(), w.abs())
-    if kind != "rand":
-        R.assert_exact_grid(za + b.abs().double().max(), 1.0 / 64, tag)
-    return _pool_results(tag, kind, out, code, z, za, b, 800)
+    def rows(a1, out, code):
+        z, za = R.conv5x5(a1, w), R.conv5x5(a1.abs(), w.abs())
+        if kind != "rand":
+            R.assert_exact_grid(za + b.abs().double().max(), 1.0 / 64, tag)
+        return _pool_results(tag, kind, out, code, z, za, b, 800)
+    return by_rows(rows, a1.shape[0], a1, out, code)
 
 
 def check_conv2_fwd(B: int = 8, seed: int = 1, kinds: Sequence[str] = KINDS, guard: int = 0) -> List[Result]:
@@ -351,10 +409,12 @@ def check_conv2_fwd(B: int = 8, seed: int = 1, kinds: Sequence[str] = KINDS, gua
 
 
 def conv2_dgrad_results(tag: str, kind: str, dy, w, dx) -> List[Result]:
-    ref, ra = R.conv5x5_dgrad(dy, w), R.conv5x5_dgrad(dy.abs(), w.abs())
-    if kind == "grid":
-        R.assert_exact_grid(ra, 1.0 / 64, tag)
-    return R.compare(tag, kind, dx, ref, R.fp32_slack(ra, 1600))
+    def rows(dy, dx):
+        ref, ra = R.conv5x5_dgrad(dy, w), R.conv5x5_dgrad(dy.abs(), w.abs())
+        if kind == "grid":
+            R.assert_exact_grid(ra, 1.0 / 64, tag)
+        return R.compare(tag, kind, dx, ref, R.fp32_slack(ra, 1600))
+    return by_rows(rows, dy.shape[0], dy, dx)
 
 
 def check_conv2_dgrad(B: int = 8, seed: int = 2, kinds: Sequence[str] = KINDS, guard: int = 0) -> List[Result]:
@@ -376,9 +436,10 @@ def check_conv2_dgrad(B: int = 8, seed: int = 2, kinds: Sequence[str] = KINDS, g
 
 
 def conv2_wgrad_results(tag: str, kind: str, a1, dy, gw) -> List[Result]:
-    ref = R.conv5x5_wgrad(a1, dy)
+    B = a1.shape[0]
+    ref = sum_by_rows(R.conv5x5_wgrad, B, a1, dy)
     if kind == "grid":
-        R.assert_exact_grid(R.conv5x5_wgrad(a1.abs(), dy.abs()), 1.0, tag)
+        R.assert_exact_grid(sum_by_rows(lambda a, d: R.conv5x5_wgrad(a.abs(), d.abs()), B, a1, dy), 1.0, tag)
     return R.compare(tag, kind, gw, ref)
 
 
@@ -964,17 +1025,26 @@ def elastic_augment_results(tag: str, fed, got, mix: int, iteration: int, ranges
 
 def fc1_dgrad_results(tag: str, kind: str, dh, w1, code, dy, gb) -> List[Result]:
     """fc1_dgrad_unpool's dy2 [B,14,14,64] and conv2 bias gradient from dh, the bf16 weights w1 and the pool2 codes."""
-    rdy, rgb = R.fc1_dgrad_unpool(dh, w1, code)
-    ady, _ = R.fc1_dgrad_unpool(dh.abs(), w1.abs(), code)
+    slices = row_slices(dh.shape[0])
+    parts, rgb, agb = [], 0.0, 0.0
+    for s in slices:
+        rdy, g = R.fc1_dgrad_unpool(dh[s], w1, code[s])
+        ady, _ = R.fc1_dgrad_unpool(dh[s].abs(), w1.abs(), code[s])
+        if kind == "grid":
+            R.assert_exact_grid(ady, 1.0 / 64, tag + ".dy")
+        parts.append(R.compare(tag + ".dy", kind, dy[s], rdy, R.fp32_slack(ady, 512)))
+        rgb, agb = rgb + g, agb + rdy.abs().sum((0, 1, 2))
     if kind == "grid":
-        R.assert_exact_grid(ady, 1.0 / 64, tag + ".dy")
         # the bias gradient adds the exact fp32 values: its partial sums are bounded by the sum of their magnitudes
-        R.assert_exact_grid(rdy.abs().sum((0, 1, 2)), 1.0 / 64, tag + ".g_bias")
-    return R.compare(tag + ".dy", kind, dy, rdy, R.fp32_slack(ady, 512)) + R.compare(tag + ".g_bias", kind, gb, rgb)
+        R.assert_exact_grid(agb, 1.0 / 64, tag + ".g_bias")
+    return merge_row_chunks(parts, [s.stop - s.start for s in slices]) + R.compare(tag + ".g_bias", kind, gb, rgb)
 
 
-def check_fc1_dgrad_unpool(B: int = 200, seed: int = 6, kinds: Sequence[str] = KINDS, stale_B: int = 0) -> List[Result]:
-    """fc1 dgrad GEMM with the maxpool2/ReLU2 backward + conv2 bias gradient fused into its epilogue."""
+def check_fc1_dgrad_unpool(B: int = 200, seed: int = 6, kinds: Sequence[str] = KINDS, stale_B: int = 0,
+                           guard: int = 0) -> List[Result]:
+    """fc1 dgrad GEMM with the maxpool2/ReLU2 backward + conv2 bias gradient fused into its epilogue.  ``guard``: as in
+    ``check_conv2_fwd``, for dy2.  The grid weights are k/64 with |k| <= 8, or <= 4 above 8192 rows: the bias gradient
+    sums about 25 B values of dy2 per channel, and its exact partial sums must stay below 2^24 units of 1/64."""
     res: List[Result] = []
     for kind in kinds:
         tag = "fc1_dgrad_unpool.%s" % kind
@@ -982,12 +1052,15 @@ def check_fc1_dgrad_unpool(B: int = 200, seed: int = 6, kinds: Sequence[str] = K
         if kind == "rand":
             dh, w1 = _bf(torch.randn(B, 512, generator=g) * 0.1), _bf(torch.randn(3136, 512, generator=g) * 0.05)
         else:
-            dh, w1 = _bf(R.grid(g, (B, 512), -1, 1)), _bf(R.grid(g, (3136, 512), -8, 8, 64))
+            wk = 8 if B <= 8192 else 4
+            dh, w1 = _bf(R.grid(g, (B, 512), -1, 1)), _bf(R.grid(g, (3136, 512), -wk, wk, 64))
         dh, w1, code = _dev(dh, w1, _codes(g, (B, 3136)))
         if stale_B:
             prime_workspace("fc1_dgrad_unpool", stale_B)
-        dy, gb = run_fc1_dgrad_unpool(dh, w1, code)
+        dy, gb = run_fc1_dgrad_unpool(dh, w1, code, guard)
         res += fc1_dgrad_results(tag, kind, dh, w1, code, dy, gb)
+        if guard:
+            res += unwritten_results(tag + ".dy", dy, guard)
     return res
 
 

@@ -285,6 +285,13 @@ def check_device_data_flags(flags, ctx: ReplicaContext, dataset) -> None:
                          "(--backend=%s%s) feeds its batches from the host" % (flags.backend, "" if ctx.on_gpu else ", no GPU"))
 
 
+def check_batch_flags(flags, ctx: ReplicaContext) -> None:
+    """A ``--batch_size`` the GPU path's LeNet kernels cannot run, rejected before any device work starts."""
+    if ctx.on_gpu and flags.backend in ("auto", "fused") and flags.model == "lenet":
+        from .engine_cuda import check_lenet_batch
+        check_lenet_batch(flags.batch_size)
+
+
 def check_eval_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate: int, dataset_test) -> None:
     """``--eval_every_steps`` combinations that cannot work, rejected before any device work starts."""
     if getattr(flags, "eval_every_steps", 0) < 0:
@@ -615,6 +622,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         num_replicas_to_aggregate = flags.num_replicas_to_aggregate
     assert num_workers > 0
     is_chief = ctx.is_chief
+    check_batch_flags(flags, ctx)
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
     check_target_flags(flags, ctx)
     check_early_stopping_flags(flags, ctx)

@@ -120,6 +120,52 @@ def test_seeded_weight_gradient_fault_fails(fault, kind):
     assert not _passes(res), "fault %s passed on %s data: %s" % (fault, kind, res)
 
 
+def _bump(t, idx, ulps):
+    """``t`` with the elements at ``idx`` moved by ``ulps`` bf16 ulps"""
+    t = t.clone()
+    t.view(torch.int16)[idx] += ulps
+    return t
+
+
+@pytest.mark.parametrize("kind", ["grid", "rand"])
+def test_references_in_row_chunks_give_the_whole_batch_results(kind, monkeypatch):
+    """Large batches evaluate the float64 references S.REF_ROWS rows at a time.  On 7 rows in chunks of 3, 3 and 1,
+    with outputs wrong in a few elements of several chunks, every result equals the one on the whole batch."""
+    n, bf = 7, torch.bfloat16
+    g = S._gen(11)
+    a1, w, b = S._conv2_data(kind, g, n)
+    p2 = R.pool_fwd(R.conv5x5(a1, w), b)
+    out2 = _bump(p2["out"].float().to(bf), ([0, 4, 6], 3, 2, 5), 2)
+    code2 = p2["code"].clone()
+    code2[[1, 5], 0, 0, 0] ^= 4
+    dy = S._bf(R.grid(g, (n, 14, 14, 64), -4, 4)) if kind == "grid" else S._bf(torch.randn(n, 14, 14, 64, generator=g) * 0.1)
+    dx = _bump(R.conv5x5_dgrad(dy, w).float().to(bf), ([2, 3, 6], 1, 1, 1), 3)
+    gw2 = R.conv5x5_wgrad(a1, dy).float()
+    dh, w1 = S._bf(R.grid(g, (n, 512), -1, 1)), S._bf(R.grid(g, (3136, 512), -8, 8, 64))
+    c2 = S._codes(g, (n, 3136))
+    rdy, rgb = R.fc1_dgrad_unpool(dh, w1, c2)
+    dy2 = _bump(rdy.float().to(bf), ([0, 6], 5, 5, 7), 2)
+    x, w_1, b_1 = S._conv1_data(kind, g, n)
+    p1 = R.pool_fwd(R.conv5x5(x.to(bf)[..., None], w_1.to(bf)), b_1)
+    out1 = _bump(p1["out"].float().to(bf), ([3, 6], 7, 7, 0), 2)
+    dp, c1 = S._bf(R.grid(g, (n, 14, 14, 32), -4, 4)), S._codes(g, (n, 14, 14, 32))
+    gw1, gb1 = (t.float() for t in R.conv1_wgrad(x.to(bf), dp, c1))
+
+    def results():
+        return (S.conv2_fwd_results("c2f", kind, a1, w, b, out2, code2) + S.conv2_dgrad_results("c2d", kind, dy, w, dx)
+                + S.conv2_wgrad_results("c2w", kind, a1, dy, gw2 + (gw2 == gw2.max()))
+                + S.fc1_dgrad_results("f1d", "grid", dh, w1, c2, dy2, rgb.float())
+                + S.conv1_fwd_results("c1f", kind, x, w_1, b_1, out1, p1["code"])
+                + S.conv1_wgrad_results("c1w", "grid", x, dp, c1, gw1, gb1 + 1))
+    whole = results()
+    monkeypatch.setattr(S, "REF_ROWS", 3)
+    chunked = results()
+    assert [r[0] for r in chunked] == [r[0] for r in whole]
+    for (name, e, t), (_, e2, t2) in zip(whole, chunked):
+        assert e2 == pytest.approx(e, rel=1e-9, abs=1e-15) and t2 == t, name
+    assert sum(e > t for (_, e, t) in whole) >= 7, whole
+
+
 def test_bf16_rule_one_ulp_and_exact_fraction():
     ref = torch.linspace(-3, 3, 1000, dtype=torch.float64)
     good = R.rne_bf16(ref).to(torch.bfloat16)
