@@ -175,7 +175,7 @@ __global__ void __launch_bounds__(EARLY2_THREADS) bucket_early_kernel(SyncPeers 
   }
 
   // ---- SGD on my fp32 master copy of fc1 from the (identical everywhere) bf16 gradient sum; fresh bf16 shadow ---------------
-  const float scale = cta_scale(a, me, epoch, (uint32_t)NR);
+  const float scale = cta_scale(a, me, true, epoch, (uint32_t)NR);
   float* w = P.params[a.rank] + 4 * (size_t)r.fc1_b4;
   __nv_bfloat16* sh = a.shadow != nullptr ? a.shadow + 4 * (size_t)r.fc1_b4 : nullptr;
   constexpr int A = 2;
@@ -270,7 +270,7 @@ __global__ void __launch_bounds__(LATE2_THREADS, 1) bucket_late_kernel(SyncPeers
   }
 
   // ---- sum the N contributions in rank order, SGD on my copy, bf16 shadow --------------------------------------------------
-  const float scale = cta_scale(a, me, epoch, (uint32_t)NR);
+  const float scale = cta_scale(a, me, true, epoch, (uint32_t)NR);
   float* wdst = P.params[a.rank];
   const float* inbox = r.inbox[a.rank];
   for (int j = tid; j < n_late4; j += stride) {
@@ -381,7 +381,7 @@ __global__ void __launch_bounds__(LATE2_THREADS) bucket_late_ll_kernel(SyncPeers
   }
 
   // ---- receive: poll my inbox until the other replicas' lines of this step are there; rank-ordered sum; SGD; shadow -------
-  const float scale = cta_scale(a, me, epoch, (uint32_t)NR);
+  const float scale = cta_scale(a, me, true, epoch, (uint32_t)NR);
   float* wdst = P.params[a.rank];
   const uint4* inbox = reinterpret_cast<const uint4*>(r.inbox[a.rank]);
   for (int j = tid; j < n_late4; j += stride) {

@@ -203,7 +203,7 @@ __global__ void __launch_bounds__(IV_THREADS, 1) iv_apply_kernel(SyncPeers P, Sy
   const uint32_t e = me->epoch;
   if (me->iv_commit_go != e + 1) return;
   const uint32_t mask = me->iv_commit_mask, total = me->iv_commit_total;
-  const float scale = cta_scale(a, nullptr, e, max(total, 1u));
+  const float scale = cta_scale(a, me, false, e, max(total, 1u));
   int contrib[SYNC_MAX_RANKS];
   int nc = 0;
   for (int q = 0; q < a.nranks; ++q)

@@ -158,7 +158,7 @@ __global__ void __launch_bounds__(SYNC_THREADS, 1) fused_sync_sgd_kernel(SyncPee
     const int end = min(begin + shard, a.numel4);
     own_begin = begin;
     own_end = end;
-    const float scale = cta_scale(a, me, epoch, (uint32_t)count);
+    const float scale = cta_scale(a, me, true, epoch, (uint32_t)count);
     const uint32_t drop_thresh = a.drop_keep > 0.f ? (uint32_t)(a.drop_keep * 16777216.f) : 0u;
     int contrib[SYNC_MAX_RANKS];
     int nc = 0;
@@ -338,7 +338,7 @@ __global__ void __launch_bounds__(EARLY_THREADS) fused_sync_early_kernel(SyncPee
   const int shard = (n4 + a.nranks - 1) / a.nranks;
   const int begin = r.begin4 + a.rank * shard;
   const int end = min(begin + shard, r.end4);
-  const float scale = cta_scale(a, me, epoch, (uint32_t)a.nranks);
+  const float scale = cta_scale(a, me, true, epoch, (uint32_t)a.nranks);
   const float* wsrc = P.params[a.rank];
   const int stride = gridDim.x * EARLY_THREADS;
   if (a.mc_grads != nullptr && a.mc_params != nullptr) {
@@ -434,7 +434,7 @@ __global__ void __launch_bounds__(SYNC_THREADS, 1) fused_sync_late_kernel(SyncPe
   if (blockIdx.x == 0 && threadIdx.x == 0) me->t_phase[1] = globaltimer_ns();
 
   // ---- one-shot on the late bucket: every rank sums all contributions in rank order and updates its own copy -------------
-  const float scale = cta_scale(a, me, epoch, (uint32_t)a.nranks);
+  const float scale = cta_scale(a, me, true, epoch, (uint32_t)a.nranks);
   float* wdst = P.params[a.rank];
   const int stride = gridDim.x * SYNC_THREADS;
   // late bucket = [begin4, end4) minus the early range: walk a compacted index
@@ -707,6 +707,27 @@ int dm_sync_set_lr_cuts(void* ctrl, const void* table, double factor) {
   DM_CUDA_OK(cudaMemcpy(reinterpret_cast<char*>(ctrl) + offsetof(SyncCtrl, lr_cuts), &table, sizeof(void*),
                         cudaMemcpyHostToDevice));
   DM_CUDA_OK(cudaMemcpy(reinterpret_cast<char*>(ctrl) + offsetof(SyncCtrl, lr_factor), &factor, sizeof(double),
+                        cudaMemcpyHostToDevice));
+  return 0;
+}
+
+// Arm the control block's learning-rate schedule (SyncCtrl::lr_warmup_steps .. lr_cosine_alpha, see cta_scale): linear
+// warmup over the first `warmup_steps` global steps from the factor 0 <= `warmup_start` < 1, and cosine decay over
+// `cosine_steps` steps down to the floor 0 <= `alpha` < 1 in place of the staircase decay.  0 steps: that part is off;
+// both 0: the schedule is disarmed.  Step counts are below 2^32 - 1.
+int dm_sync_set_lr_schedule(void* ctrl, unsigned int warmup_steps, double warmup_start, unsigned int cosine_steps,
+                            double alpha) {
+  using dm::SyncCtrl;
+  if (ctrl == nullptr || warmup_steps == 0xFFFFFFFFu || cosine_steps == 0xFFFFFFFFu ||
+      !(warmup_start >= 0.0 && warmup_start < 1.0) || !(alpha >= 0.0 && alpha < 1.0))
+    return -1;
+  DM_CUDA_OK(cudaMemcpy(reinterpret_cast<char*>(ctrl) + offsetof(SyncCtrl, lr_warmup_steps), &warmup_steps, sizeof(uint32_t),
+                        cudaMemcpyHostToDevice));
+  DM_CUDA_OK(cudaMemcpy(reinterpret_cast<char*>(ctrl) + offsetof(SyncCtrl, lr_cosine_steps), &cosine_steps, sizeof(uint32_t),
+                        cudaMemcpyHostToDevice));
+  DM_CUDA_OK(cudaMemcpy(reinterpret_cast<char*>(ctrl) + offsetof(SyncCtrl, lr_warmup_start), &warmup_start, sizeof(double),
+                        cudaMemcpyHostToDevice));
+  DM_CUDA_OK(cudaMemcpy(reinterpret_cast<char*>(ctrl) + offsetof(SyncCtrl, lr_cosine_alpha), &alpha, sizeof(double),
                         cudaMemcpyHostToDevice));
   return 0;
 }

@@ -40,7 +40,14 @@ struct SyncCtrl {
   uint32_t error;                // watchdog: 1 = arrival timeout, 2 = done timeout
   uint32_t accepted_steps, dropped_steps;
   uint32_t last_mask, last_count, last_late;
-  uint32_t pad1[29];
+  uint32_t pad1[23];
+  // learning-rate schedule (--lr_warmup_steps, --lr_cosine_decay_steps): linear warmup over the first W global steps from
+  // the factor f0, and TF's cosine_decay over T steps with the floor alpha in place of the staircase decay; W = T = 0: off.
+  // Set once by dm_sync_set_lr_schedule, read by cta_scale.  These words were padding, like the cut table's below.
+  uint32_t lr_warmup_steps;      // W
+  uint32_t lr_cosine_steps;      // T
+  double lr_warmup_start;        // f0
+  double lr_cosine_alpha;        // alpha
   // learning-rate cuts (--lr_plateau_patience, csrc/eval_plateau.cu): this replica's table of SYNC_MAX_CUTS cut steps
   // (0xFFFFFFFF = no cut), written by the chief's eval_plateau over NVLink; null when no table is armed.  Set once by
   // dm_sync_set_lr_cuts.  These words were padding: the size and every other offset of the block are unchanged.
@@ -82,6 +89,11 @@ struct SyncCtrl {
 static_assert(SYNC_MAX_CUTS == 32, "cta_scale reads one cut-table entry per lane of a warp");
 static_assert(offsetof(SyncCtrl, lr_cuts) % 8 == 0 && offsetof(SyncCtrl, lr_factor) + 8 == offsetof(SyncCtrl, t_arrive),
               "the cut-table words take the place of pad1's last words, with no change to the layout around them");
+static_assert(sizeof(SyncCtrl) == 23520 && offsetof(SyncCtrl, pad1) == 3540 && offsetof(SyncCtrl, lr_warmup_steps) == 3632 &&
+                  offsetof(SyncCtrl, lr_cuts) == 3656 && offsetof(SyncCtrl, t_arrive) == 3672 &&
+                  offsetof(SyncCtrl, bar) == 22496,
+              "the schedule words take the place of pad1's last words before the cut table: the size of the block and "
+              "every other offset are unchanged");
 
 struct SyncPeers {
   SyncCtrl* ctrl[SYNC_MAX_RANKS];
@@ -186,23 +198,43 @@ DMNIST_DEVICE void publish_status(SyncCtrl* me, uint32_t epoch_after, uint32_t a
 // power into lg2/ex2.approx and the division into div.approx); CUDA's double pow is within 2 ulp, far below fp32 rounding.
 // Thread 0 evaluates it and the CTA reads it after a barrier: every thread of the CTA must call this.
 //
-// Learning-rate cuts (--lr_plateau_patience): when `ctrl` is non-null and holds a cut table, warp 0 counts the cuts in
+// Learning-rate cuts (--lr_plateau_patience): when `cuts` is set and `ctrl` holds a cut table, warp 0 counts the cuts in
 // effect at `step` -- c = entries <= step, one relaxed load per lane and a ballot -- and the rate becomes
 // lr0 * decay_rate^p * F^c / count, the product in that order in double, as schedule.LearningRateSchedule computes it.
 // With c = 0 the factor is 1.0 and the value is the one without a table.  The chief's stores into the table reach every
-// replica before any launch whose `step` they concern (DESIGN §4, learning-rate cuts).  ctrl = null (interval mode): no cuts.
-DMNIST_DEVICE float cta_scale(const SyncArgs& a, const SyncCtrl* ctrl, uint32_t step, uint32_t count) {
+// replica before any launch whose `step` they concern (DESIGN §4, learning-rate cuts).  Interval mode passes cuts = false.
+//
+// Learning-rate schedule (--lr_warmup_steps, --lr_cosine_decay_steps): when `ctrl` has one armed, the rate is
+// lr0 * D * Wf * F^c / count, left to right, with D = (1 - alpha) * (v * v) + alpha, v = sin(pi * (T - min(s, T)) / (2T))
+// in place of decay_rate^p when T > 0, and Wf = f0 + ((1 - f0) * s) / W for s < W.  Every operation of D and Wf is an
+// explicitly rounded one: nvcc would contract (1 - alpha) * c + alpha into an FMA the host cannot reproduce.  CUDA's
+// double sin is within 2 ulp.  With nothing armed the expression is the one above, unchanged.
+DMNIST_DEVICE float cta_scale(const SyncArgs& a, const SyncCtrl* ctrl, bool cuts, uint32_t step, uint32_t count) {
   __shared__ float s_scale;
   if (threadIdx.x < 32) {
-    const uint32_t* cuts = ctrl != nullptr ? ctrl->lr_cuts : nullptr;
+    const uint32_t* table = cuts && ctrl != nullptr ? ctrl->lr_cuts : nullptr;
     double f = 1.0;
-    if (cuts != nullptr) {
-      const int c = __popc(__ballot_sync(0xffffffffu, ld_relaxed_sys(cuts + threadIdx.x) <= step));
+    if (table != nullptr) {
+      const int c = __popc(__ballot_sync(0xffffffffu, ld_relaxed_sys(table + threadIdx.x) <= step));
       if (c > 0) f = pow(ctrl->lr_factor, (double)c);
     }
     if (threadIdx.x == 0) {
-      const double p = (double)(step / (uint32_t)max(a.decay_steps, 1));
-      s_scale = (float)(a.lr0 * pow(a.decay_rate, p) * f / (double)count);
+      const uint32_t W = ctrl != nullptr ? ctrl->lr_warmup_steps : 0u, T = ctrl != nullptr ? ctrl->lr_cosine_steps : 0u;
+      double d;
+      if (T > 0) {
+        const double q = __ddiv_rn((double)(T - min(step, T)), __dmul_rn(2.0, (double)T));
+        const double v = sin(__dmul_rn(3.141592653589793, q));
+        const double al = ctrl->lr_cosine_alpha;
+        d = __dadd_rn(__dmul_rn(__dadd_rn(1.0, -al), __dmul_rn(v, v)), al);
+      } else {
+        d = pow(a.decay_rate, (double)(step / (uint32_t)max(a.decay_steps, 1)));
+      }
+      double lr = a.lr0 * d;
+      if (step < W) {
+        const double f0 = ctrl->lr_warmup_start;
+        lr = __dmul_rn(lr, __dadd_rn(f0, __ddiv_rn(__dmul_rn(__dadd_rn(1.0, -f0), (double)step), (double)W)));
+      }
+      s_scale = (float)(lr * f / (double)count);
     }
   }
   __syncthreads();

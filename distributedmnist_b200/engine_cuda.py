@@ -365,6 +365,10 @@ class _CudaEngine(ComputeEngine):
                              "the number of replicas (%d)" % (int(k), n))
         self._opt_args = dict(k=int(k), lr0=float(sched.initial_learning_rate), decay_rate=float(sched.decay_rate),
                               decay_steps=int(sched.decay_steps))
+        # warmup / cosine decay: evaluated by the aggregation kernels at the step they update, from this replica's own
+        # control block (every replica arms its own; nothing to agree on beyond the step)
+        self.backend.set_lr_schedule(getattr(sched, "warmup_steps", 0), getattr(sched, "warmup_start", 1.0 / 3),
+                                     getattr(sched, "cosine_steps", 0), getattr(sched, "cosine_alpha", 0.0))
         if getattr(opt, "drop_connect_probability", None) is not None:
             self.backend.drop_connect_(self.grads, opt.drop_connect_probability, 0)
         self._straggler = getattr(opt, "_straggler", None)

@@ -294,6 +294,20 @@ def define_engine_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_float("lr_plateau_min_delta", 0.0, "With --lr_plateau_patience: the accuracy an evaluation must beat the "
                                                 "best by to reset the patience, rounded down to whole validation rows; "
                                                 "0 <= D < 1")
+    F.DEFINE_integer("lr_warmup_steps", 0, "Linear learning-rate warmup (Goyal et al. 2017): the update of global step s < W "
+                                           "is made at the rate times f0 + (1 - f0) * s / W, f0 = "
+                                           "--lr_warmup_start_factor; counts global steps (interval mode: ticks; K > N: "
+                                           "committed steps) from 0, on top of the decay; 0 = off, else W < 2^32 - 1")
+    F.DEFINE_float("lr_warmup_start_factor", 1.0 / 3, "With --lr_warmup_steps: the factor f0 of the rate at global step 0 "
+                                                      "(torch's LinearLR start_factor); 0 <= f0 < 1")
+    F.DEFINE_integer("lr_cosine_decay_steps", 0, "Replace the staircase decay by TF's cosine_decay over T global steps: "
+                                                 "the rate is lr0 * ((1 - alpha) * (1 + cos(pi * min(s, T) / T)) / 2 + "
+                                                 "alpha), from step 0 (a warmup multiplies its first steps); from step T on "
+                                                 "it is lr0 * alpha, so alpha = 0 stops the weights there.  Not with "
+                                                 "--learning_rate_decay_factor or --num_epochs_per_decay; 0 = off, else "
+                                                 "T < 2^32 - 1")
+    F.DEFINE_float("lr_cosine_alpha", 0.0, "With --lr_cosine_decay_steps: the floor alpha of the cosine decay as a fraction "
+                                           "of the initial learning rate (TF's alpha); 0 <= alpha < 1")
     F.DEFINE_float("weight_decay", 0.0, "L2 weight decay of the fully connected layers (the reference model's regulariser, "
                                         "src/mnist.py:142-143): every replica differentiates CE + lambda * sum(v^2) / 2 over "
                                         "lenet's fc1/fc2 weights and biases (every layer of mlp2 / mlp3), and the logged "

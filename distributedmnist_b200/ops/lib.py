@@ -103,6 +103,7 @@ def _signatures() -> dict:
         "dm_fused_sync_bucket": (S, i, [PP, PP, PP, i, i, i, ll, ll, ll, ll, d, d, i, d, P, i, P, P, P]),
         "dm_sync_set_host_mirror": (S, i, [P, P]),
         "dm_sync_set_lr_cuts": (S, i, [P, P, d]),
+        "dm_sync_set_lr_schedule": (S, i, [P, u, d, u, d]),
         "dm_f32_to_bf16": (S, i, [P, P, ll, P]),
         "dm_straggler_delay": (S, i, [P, f, u, u, P]),
         "dm_straggler_state_bytes": (V, i, []),

@@ -78,6 +78,7 @@ class FusedBackend(Backend):
         self.drop_keep = 0.0
         self.drop_seed = 0
         self.interval_ns: Optional[int] = None     # the interval clock's period, once armed (interval_arm)
+        self.lr_schedule_armed = False             # the control block evaluates a warmup / cosine (set_lr_schedule)
 
     # ---- memory ---------------------------------------------------------------------------
     def allocate(self, numel: int) -> torch.Tensor:
@@ -124,6 +125,19 @@ class FusedBackend(Backend):
         self._write_u32("decider_claim", step)
         torch.cuda.synchronize()
         self.barrier()
+
+    def set_lr_schedule(self, warmup_steps: int, warmup_start: float, cosine_steps: int, alpha: float) -> None:
+        """Arm this replica's control block with the learning-rate schedule's warmup and cosine decay (``cta_scale`` in
+        csrc/fused_sync.cuh): every aggregation kernel then evaluates them at the step it updates.  Not collective: each
+        replica arms its own block.  ``warmup_steps = cosine_steps = 0`` disarms it."""
+        self.lib.dm_sync_set_lr_schedule(self.ctrl.local_ptr, int(warmup_steps), float(warmup_start), int(cosine_steps),
+                                         float(alpha))
+        self.lr_schedule_armed = int(warmup_steps) > 0 or int(cosine_steps) > 0
+
+    def _refuse_host_rate(self, what: str) -> None:
+        if self.lr_schedule_armed:
+            raise RuntimeError("FusedBackend.%s passes a learning rate the host evaluated, but the control block has a "
+                               "learning-rate schedule armed that the kernel would apply on top of it" % what)
 
     def read_status(self) -> Dict[str, int]:
         """epoch / error / accepted / dropped / last_mask / last_count / last_late with ONE device->host copy (synchronises
@@ -366,6 +380,7 @@ class FusedBackend(Backend):
                         stale=bool(late))
 
     def sync_step(self, params, grads, lr, local_step, k, delay_s: float = 0.0) -> StepInfo:
+        self._refuse_host_rate("sync_step")
         if delay_s > 0:
             self.enqueue_straggler_delay(1.0, delay_s * 1e6)
         self.enqueue(params, grads, k, lr0=float(lr))
@@ -374,6 +389,7 @@ class FusedBackend(Backend):
     def interval_tick(self, params, acc, count, lr, tick) -> StepInfo:
         """Mode C tick: every rank joins; ranks with an empty accumulator contribute zeros and the
         divisor is the total number of accumulated gradients (mean of whatever arrived)."""
+        self._refuse_host_rate("interval_tick")
         counts = self.all_gather_object(int(count))
         total = sum(counts)
         mask = sum(1 << i for i, c in enumerate(counts) if c > 0)

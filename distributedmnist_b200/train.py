@@ -398,6 +398,50 @@ def check_lr_plateau_flags(flags, ctx: ReplicaContext, num_replicas_to_aggregate
                             "<" if num_replicas_to_aggregate < ctx.world_size else ">") + why)
 
 
+def check_lr_schedule_flags(flags) -> None:
+    """``--lr_warmup_steps`` / ``--lr_warmup_start_factor`` / ``--lr_cosine_decay_steps`` / ``--lr_cosine_alpha``
+    values and combinations that cannot work, rejected before any device work starts.  The schedule itself works in every
+    aggregation mode: it is a function of the global step alone."""
+    w = int(getattr(flags, "lr_warmup_steps", 0) or 0)
+    f0 = float(getattr(flags, "lr_warmup_start_factor", 1.0 / 3))
+    t = int(getattr(flags, "lr_cosine_decay_steps", 0) or 0)
+    alpha = float(getattr(flags, "lr_cosine_alpha", 0.0))
+    limit = 2 ** 32 - 1
+    if not 0 <= w < limit:
+        raise ValueError("--lr_warmup_steps must lie in [0, 2^32 - 1) (0 = off), got %d" % w)
+    if not 0 <= t < limit:
+        raise ValueError("--lr_cosine_decay_steps must lie in [0, 2^32 - 1) (0 = off), got %d" % t)
+    if not 0.0 <= f0 < 1.0:           # also refuses nan and inf
+        raise ValueError("--lr_warmup_start_factor must lie in [0, 1), got %r" % f0)
+    if not 0.0 <= alpha < 1.0:
+        raise ValueError("--lr_cosine_alpha must lie in [0, 1), got %r" % alpha)
+    if w == 0 and f0 != 1.0 / 3:
+        raise ValueError("--lr_warmup_start_factor needs --lr_warmup_steps >= 1: without a warmup there is nothing for "
+                         "it to change")
+    if t == 0 and alpha != 0.0:
+        raise ValueError("--lr_cosine_alpha needs --lr_cosine_decay_steps >= 1: without a cosine decay there is nothing "
+                         "for it to change")
+    if t > 0:
+        present = getattr(flags, "is_present", lambda name: False)
+        given = [n for n in ("learning_rate_decay_factor", "num_epochs_per_decay") if present(n)]
+        if given:
+            raise ValueError("--lr_cosine_decay_steps replaces the staircase decay, so %s would do nothing"
+                             % " and ".join("--" + n for n in given))
+
+
+def describe_lr_schedule(sched: LearningRateSchedule) -> str:
+    """The start-up log's account of the schedule (without the plateau cuts, which are logged as they are made)."""
+    if sched.cosine_steps:
+        text = "%g with cosine decay over %d global steps to %g" % (
+            sched.initial_learning_rate, sched.cosine_steps, sched.initial_learning_rate * sched.cosine_alpha)
+    else:
+        text = "%g decayed by %g every %d global steps" % (sched.initial_learning_rate, sched.decay_rate,
+                                                           sched.decay_steps)
+    if sched.warmup_steps:
+        text += ", linear warmup from %g of it over global steps 0 to %d" % (sched.warmup_start, sched.warmup_steps - 1)
+    return text
+
+
 def restart_lr_cuts(train_dir: str, rank: int, restored_step: int, factor: float):
     """The cuts an earlier run's ``worker<rank>_lr_plateau.json`` lists that a run restarted from the checkpoint of
     ``restored_step`` keeps -- those with ``from_step <= restored_step`` -- as ``(kept, None)``, or ``([], reason)`` when
@@ -627,6 +671,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     check_target_flags(flags, ctx)
     check_early_stopping_flags(flags, ctx)
     check_lr_plateau_flags(flags, ctx, num_replicas_to_aggregate)
+    check_lr_schedule_flags(flags)
     check_best_flags(flags)
     check_moving_average_flags(flags, ctx, num_replicas_to_aggregate)
     check_device_data_flags(flags, ctx, dataset)
@@ -723,6 +768,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                      "restored weights")
         log.info("Moving average of the weights: decay %g; the in-training evaluation scores the %s weights"
                  % (ema_decay, "averaged" if eval_average else "live"))
+    log.info("Learning rate schedule: %s; the update of global step #%d is made at %g"
+             % (describe_lr_schedule(lr_schedule), restored_step, lr_schedule(restored_step)))
     log.info("%s Supervisor" % datetime.now())
 
     # --eval_every_steps: the chief scores the validation set after every E-th global step and after the last one.  GPU path:
@@ -837,7 +884,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     time_acc_list = []
     step = restored_step
     loss_value = train_acc_value = float("nan")
-    results = {"steps": [], "losses": [], "accepted": 0, "dropped": 0}
+    results = {"steps": [], "losses": [], "accepted": 0, "dropped": 0, "lr_schedule": lr_schedule.describe()}
     # cdf telemetry (reference timeout_manager.py:55-61): compute time = gradient done - token dequeued, the barrier wait
     # NOT included.  interval wins when both flags are set (as in the reference) and its replicas are not in lock step, so
     # the collective flush of the cdf tables must not run then.
