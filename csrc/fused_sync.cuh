@@ -83,7 +83,10 @@ struct SyncCtrl {
   uint32_t* host_mirror;                   // 4 slots x 8 words in mapped pinned host memory, or null
   uint32_t decider_claim;                  // step+1 of the newest launch whose arrival/commit decision a CTA has claimed
   uint32_t bar_seq;                        // device barriers completed so far (dm_device_barrier)
-  uint32_t pad3[14];
+  // ---- asynchronous SGD (csrc/fused_async.cu): these words were padding ------------------------------------------------------
+  uint32_t as_pull;                        // r: the chief's update counter when this iteration pulled its weights
+  uint32_t as_ticket;                      // s: the global step this iteration's update produces
+  uint32_t pad3[12];
   volatile uint32_t bar[SYNC_MAX_RANKS * 32];   // [p*32]: peer p entered device barrier number (value)
 };
 static_assert(SYNC_MAX_CUTS == 32, "cta_scale reads one cut-table entry per lane of a warp");
@@ -94,6 +97,8 @@ static_assert(sizeof(SyncCtrl) == 23520 && offsetof(SyncCtrl, pad1) == 3540 && o
                   offsetof(SyncCtrl, bar) == 22496,
               "the schedule words take the place of pad1's last words before the cut table: the size of the block and "
               "every other offset are unchanged");
+static_assert(offsetof(SyncCtrl, as_ticket) + 4 == offsetof(SyncCtrl, pad3) && offsetof(SyncCtrl, pad3) + 48 == offsetof(SyncCtrl, bar),
+              "the asynchronous-SGD words take the place of pad3's first words, with no change to the layout around them");
 
 struct SyncPeers {
   SyncCtrl* ctrl[SYNC_MAX_RANKS];

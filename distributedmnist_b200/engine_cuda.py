@@ -123,6 +123,8 @@ class _CudaEngine(ComputeEngine):
     runner, the optimizer binding and the graph-replayed step.  A subclass builds its kernel sequence in ``_launch_step``,
     clears its gradients in ``_launch_zero`` and names its early bucket (``_bucket_early``, ``_g16_shape``)."""
     _kgtn_k = 0                  # K > N: gradients per update (count trigger); 0 = the K <= N / interval paths
+    _async = False               # asynchronous SGD (csrc/fused_async.cu), see attach_optimizer
+    _master = None               # asynchronous SGD: this replica's master copy of the weights (symmetric memory)
     _table = None                # device-resident training set (images, labels), see arm_train_data
     _runner = None               # native step runner (csrc/step_runner.cu), see _make_runner
     _stamp = False               # cdf telemetry stamps in the step
@@ -385,6 +387,16 @@ class _CudaEngine(ComputeEngine):
             self._acc = self.backend.allocate(self.spec.arena_numel)
         if self._kgtn_k:
             self.backend.kgtn_arm()          # nothing else arms it (e.g. bench.py); train.py re-arms after a restore
+        # asynchronous SGD (csrc/fused_async.cu): every iteration pulls this replica's master copy into the working arena
+        # and adds its own update to every replica's master copy; the working arena stays private between iterations
+        self._async = getattr(opt, "mode", "") == "async"
+        if self._async:
+            if getattr(opt, "drop_connect_probability", None) is not None:
+                raise ValueError("--drop_connect cannot be combined with --async_method")
+            if self._master is None:
+                self._master = self.backend.allocate(self.spec.arena_numel)
+                self._as_stats = torch.zeros(int(self.lib.dm_async_stats_bytes()), dtype=torch.uint8, device=self.device)
+            self.async_arm()                 # train.py re-arms after a restore
         # Bucketed aggregation (csrc/fused_sync.cu): full participation on 2/4/8 replicas.  fc1's weight gradient (96.5 % of
         # the bytes) is exchanged by small co-resident CTAs NEXT TO conv2 dgrad/wgrad + conv1 wgrad; the rest goes one-shot.
         #   DMNIST_BUCKET=2 (default): csrc/fused_bucket.cu -- fc1's gradient leaves the GEMM epilogue as bf16, is reduced in
@@ -392,7 +404,7 @@ class _CudaEngine(ComputeEngine):
         #     pass; the small bucket is pushed into every replica's inbox.  Also used on ONE replica (no exchange, the fc1
         #     update still leaves the critical path).   =1: round-1 fp32 two-shot / one-shot kernels.   =0: single kernel.
         mode = os.environ.get("DMNIST_BUCKET", "2")
-        can = int(k) == n and self.backend.drop_keep <= 0.0 and getattr(opt, "mode", "") != "interval"
+        can = int(k) == n and self.backend.drop_keep <= 0.0 and getattr(opt, "mode", "") not in ("interval", "async")
         self._bucket_v2 = can and mode == "2" and n in (1, 2, 4, 8)
         self._bucketed = can and ((mode == "1" and n in (2, 4, 8)) or self._bucket_v2)
         if self._bucket_v2 and self._g16 is None:
@@ -496,20 +508,49 @@ class _CudaEngine(ComputeEngine):
         raise NotImplementedError
 
     def _enqueue_iteration_begin(self) -> None:
-        """Interval mode / K > N: adopt pushed weights (+ shadow refresh) at the start of an iteration."""
-        if self._kgtn_k:
+        """Interval mode / K > N: adopt pushed weights (+ shadow refresh) at the start of an iteration.  Asynchronous SGD:
+        read the update counter, pull the master copy (+ shadow)."""
+        if self._async:
+            self.backend.enqueue_async_begin(self._master, self.params)
+        elif self._kgtn_k:
             self.backend.enqueue_kgtn_begin(self.params)
         else:
             self.backend.enqueue_interval_begin(self.params)
 
     def _enqueue_iteration_end(self) -> None:
-        """Interval mode / K > N: gate, accumulate, close (+ commit attempt), apply."""
+        """Interval mode / K > N: gate, accumulate, close (+ commit attempt), apply.  Asynchronous SGD: ticket, apply."""
         oa = self._opt_args
-        if self._kgtn_k:
+        if self._async:
+            self.backend.enqueue_async_end(self._master, self.grads, self._as_stats, oa["lr0"], oa["decay_rate"],
+                                           oa["decay_steps"])
+        elif self._kgtn_k:
             self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"], oa["decay_rate"],
                                           oa["decay_steps"])
         else:
             self.backend.enqueue_interval_end(self.params, self.grads, self._acc, oa["lr0"], oa["decay_rate"], oa["decay_steps"])
+
+    # ---- asynchronous SGD (csrc/fused_async.cu) ------------------------------------------------------------------------------
+    def async_arm(self) -> None:
+        """Every master copy := the working arena (the initial or restored weights), staleness statistics zeroed; the
+        first pull reads them.  Collective."""
+        self._leave_native_runner()
+        self.backend.async_arm(self._master, self.params, self._as_stats)
+
+    def async_finish(self) -> int:
+        """End of an asynchronous run, after the last step was enqueued: every replica's last update has been applied, the
+        device barrier (every replica's updates are in every master copy after it), then one more pull into the working
+        arena.  Returns the global step of the pulled weights: the total number of updates.  Collective."""
+        self._leave_native_runner()
+        torch.cuda.synchronize()
+        self.backend.device_barrier()
+        self.backend.enqueue_async_begin(self._master, self.params)
+        torch.cuda.synchronize()
+        self.backend.check_error()
+        return self.backend.device_epoch
+
+    def async_staleness(self) -> dict:
+        """This replica's staleness statistics (see FusedBackend.async_stats); synchronises the device."""
+        return self.backend.async_stats(self._as_stats)
 
     def _run(self, with_sync: bool) -> None:
         s = self._slot
@@ -682,6 +723,8 @@ class _CudaEngine(ComputeEngine):
         if getattr(self, "_interval", False) or self._opt_args["k"] != self.backend.ctx.world_size:
             raise ValueError("the moving average is kept for K = N and cdf mode only: with K < N, K > N or interval "
                              "aggregation peers write the chief's arena at any time")
+        if self._async:
+            raise ValueError("the moving average is kept for K = N and cdf mode only, not for asynchronous SGD")
         self._leave_native_runner()
         torch.cuda.synchronize()
         off = self.backend._off["epoch"]
@@ -982,7 +1025,8 @@ class CudaLeNetEngine(_CudaEngine):
         names = ["memsets", "conv1_fwd", "conv2_fwd", "fc1_fwd", "fc2_fwd_bwd", "fc1_wgrad", "fc2_wgrad", "fc1_dgrad", "unpool2",
                  "conv2_wgrad", "conv2_dgrad", "conv1_wgrad"]
         # K > N: adopt + shadow refresh, and gate + accumulate + close + apply, in place of the fused sync kernel
-        names = (["kgtn_begin"] + names + ["kgtn_end"]) if self._kgtn_k else names + ["fused_sync_sgd"]
+        names = (["kgtn_begin"] + names + ["kgtn_end"]) if self._kgtn_k else \
+            (["async_begin"] + names + ["async_end"]) if self._async else names + ["fused_sync_sgd"]
         tot = {n: 0.0 for n in names}
         B, s = self.batch_size, self._slot
         img, lbl = self.images[s], self.labels[s]
@@ -991,6 +1035,8 @@ class CudaLeNetEngine(_CudaEngine):
         def seq():
             if self._kgtn_k:
                 yield "kgtn_begin", lambda: self.backend.enqueue_kgtn_begin(self.params)
+            elif self._async:
+                yield "async_begin", lambda: self._enqueue_iteration_begin()
             yield "memsets", lambda: self._launch_zero()
             # forward / backward are issued kernel by kernel so an event can sit between any two
             yield "conv1_fwd", lambda: self._conv1_fwd(img, B, True, sp)
@@ -1003,7 +1049,9 @@ class CudaLeNetEngine(_CudaEngine):
             yield "conv2_wgrad", lambda: self._conv2_wgrad(B, sp)
             yield "conv2_dgrad", lambda: self._conv2_dgrad(B, sp)
             yield "conv1_wgrad", lambda: self._conv1_wgrad(img, B, sp)
-            if self._kgtn_k:
+            if self._async:
+                yield "async_end", lambda: self._enqueue_iteration_end()
+            elif self._kgtn_k:
                 oa = self._opt_args
                 yield "kgtn_end", lambda: self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"],
                                                                         oa["decay_rate"], oa["decay_steps"])
@@ -1030,7 +1078,7 @@ class CudaLeNetEngine(_CudaEngine):
 
     def _launch_step(self, slot: int, with_sync: bool) -> None:
         n = 0
-        interval = with_sync and getattr(self, "_interval", False)
+        interval = with_sync and (getattr(self, "_interval", False) or self._async)     # free-running iteration
         bucketed = with_sync and self._bucketed and not interval
         self._delay_in_chain = False
         if self._stamp:
@@ -1067,7 +1115,7 @@ class CudaLeNetEngine(_CudaEngine):
                 n += 1
             if interval:
                 self._enqueue_iteration_end()
-                n += 4
+                n += 2 if self._async else 4
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1
@@ -1640,7 +1688,7 @@ class CudaMlpEngine(_CudaEngine):
         if self._aug is not None:
             images = self._launch_augment(slot)     # dm_f32_to_bf16 reads the augmented batch
             n += 1
-        interval = with_sync and getattr(self, "_interval", False)
+        interval = with_sync and (getattr(self, "_interval", False) or self._async)     # free-running iteration
         if interval:
             self._enqueue_iteration_begin()
             n += 2
@@ -1663,7 +1711,7 @@ class CudaMlpEngine(_CudaEngine):
                 n += 1
             if interval:
                 self._enqueue_iteration_end()
-                n += 4
+                n += 2 if self._async else 4
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1

@@ -196,6 +196,9 @@ def define_reference_flags(F: FlagValues = FLAGS) -> FlagValues:
     # reference: src/distributed_train.py:36-39
     F.DEFINE_boolean("worker_times_cdf_method", False, "Track worker times cdf (full-barrier mode with timing capture)")
     F.DEFINE_boolean("interval_method", False, "Use the fixed wall-clock interval aggregation method")
+    F.DEFINE_boolean("async_method", False, "Asynchronous SGD: every replica applies its own gradient to the shared "
+                                            "weights at once, without waiting for or averaging with any other; reports "
+                                            "the staleness of its updates (workerN_staleness.json)")
     F.DEFINE_boolean("should_summarize", False, "Whether the chief should write summaries")
     F.DEFINE_boolean("timeline_logging", False, "Dump a chrome-trace timeline json per step")
     # reference: src/distributed_train.py:40-48

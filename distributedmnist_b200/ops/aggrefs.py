@@ -184,3 +184,26 @@ def interval_accumulate(grads_in_order: Sequence) -> np.ndarray:
         acc = f32(g) + acc
         assert_no_subnormal("accumulate", acc)
     return acc
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# asynchronous SGD (csrc/fused_async.cu)
+# ---------------------------------------------------------------------------------------------------------------------
+def ftz(x) -> np.ndarray:
+    """Subnormal fp32 values flushed to a zero of their sign, as the kernels' FTZ arithmetic flushes operands and results."""
+    x = f32(x)
+    return np.where(np.abs(x) < np.float32(FLT_MIN), np.copysign(np.float32(0), x), x).astype(np.float32)
+
+
+def async_update(g, scale) -> np.ndarray:
+    """The update as_apply_kernel adds to every master copy: ``-fl(scale * g)``, one fp32 product (``__fmul_rn``, FTZ)."""
+    return -ftz(np.float32(scale) * ftz(g))
+
+
+def async_apply(w, xs: Sequence) -> np.ndarray:
+    """A master copy after the updates ``xs`` (each from :func:`async_update`) landed in that order: one fp32 add per
+    update, with the FTZ of the in-memory reduction (``REDG.E.ADD.F32x4.FTZ.RN``)."""
+    w = ftz(w)
+    for x in xs:
+        w = ftz(w + f32(x))
+    return w

@@ -89,6 +89,10 @@ def _signatures() -> dict:
         "dm_tta_stamp": (S, i, [P, P]),
         "dm_eval_target": (S, i, [P, P, P, u, u, u, PP, i, i, P]),
         "dm_stop_publish": (S, i, [P, P, P]),
+        # fused_async.cu
+        "dm_async_stats_bytes": (V, i, []),
+        "dm_async_begin": (S, i, [PP, i, P, P, P, ll, i, P]),
+        "dm_async_end": (S, i, [PP, PP, P, P, i, i, ll, d, d, i, i, P, P]),
         # fused_bucket.cu, fused_interval.cu
         "dm_bucket_sync": (S, i, [PP, PP, PP, PP, PP, i, i, i, ll, ll, ll, d, d, i, d, P, i, P, P, P, i, i]),
         "dm_interval_arm": (S, i, [P, d, P]),

@@ -55,7 +55,10 @@ class StepRecorder:
 
     def __init__(self, eng):
         self.eng = eng
-        self.init = dict(params=eng.params.clone(), shadow=eng.shadow.clone())
+        # asynchronous SGD: ``params`` is the master copy, which the update changes (with one replica the next step pulls
+        # it as it is); the working arena is recorded as ``pulled``
+        self._async = getattr(eng, "_async", False)
+        self.init = dict(params=(eng._master if self._async else eng.params).clone(), shadow=eng.shadow.clone())
         if getattr(eng, "_aug", None) is not None:
             self.init["aug_counter"] = eng._aug_counter.clone()
         self._ctrl = getattr(eng, "_interval", False) or getattr(eng, "_stamp", False)
@@ -69,7 +72,10 @@ class StepRecorder:
         for name in (LENET_BUFFERS if hasattr(e, "h_part") else MLP_BUFFERS):
             v = getattr(e, name)
             r[name] = [t.clone() for t in v] if isinstance(v, list) else v.clone()
-        r.update(grads=e.grads.clone(), params=e.params.clone(), shadow=e.shadow.clone(), loss_acc=e.d_loss_acc.clone())
+        r.update(grads=e.grads.clone(), params=(e._master if self._async else e.params).clone(), shadow=e.shadow.clone(),
+                 loss_acc=e.d_loss_acc.clone())
+        if self._async:
+            r["pulled"] = e.params.clone()
         if e._bucket_v2:
             r["g16"] = e._g16_view.clone()
         if getattr(e, "_decay", 0.0):
@@ -99,8 +105,8 @@ def ctrl_words(raw, off: Dict[str, int], stamp_step: Optional[int] = None) -> Di
 
 def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
     """How ``eng`` applies its gradients: ``mode`` "fused" (fused_sync_sgd), "bucket" (the bf16-wire bucketed kernels),
-    "kgtn" (K > N: every k-th iteration commits) or "interval" (a tick commits when its deadline has passed; ``interval_ns``
-    the armed period), the schedule and the global step of the first step.  ``drop``:
+    "kgtn" (K > N: every k-th iteration commits), "interval" (a tick commits when its deadline has passed; ``interval_ns``
+    the armed period) or "async" (asynchronous SGD on one replica: every step pulls the master copy and adds its update), the schedule and the global step of the first step.  ``drop``:
     (seed, keep probability) of the drop-connect mask the fused kernel applies, None without it.  With a cut table armed
     (``arm_lr_cuts``), ``sched`` must name the same cuts (raises ValueError otherwise): the step sizes are then those of
     the schedule with the cuts (synchronises the device to read the table).  ``aug``: (ranges, seed mix) of the armed
@@ -109,7 +115,9 @@ def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
     ``ctrl_off``: the control block's byte offsets, for the recorded blocks (see :func:`ctrl_words`)."""
     be = eng.backend
     e0, e1 = eng._bucket_early
-    if eng._kgtn_k:
+    if getattr(eng, "_async", False):
+        mode = "async"
+    elif eng._kgtn_k:
         mode = "kgtn"
     elif getattr(eng, "_interval", False):
         mode = "interval"
@@ -219,6 +227,9 @@ def update_results(tag: str, init: dict, records: Sequence[dict], upd: dict) -> 
                 T = max(iv["count"][t], 1)          # a count of 0 fails its own check (control_results)
                 want = A.fused_sync_step(w, [A.interval_accumulate(acc)], 1, A.step_scale(upd["sched"], epochs[t], T))
                 acc = []
+        elif mode == "async":
+            want = A.async_apply(w, [A.async_update(g, scale)])
+            res.append(("%s.step%d.pull_bits_differ" % (tag, t), float((A.bits(r["pulled"]) != A.bits(w)).sum()), 0.0))
         elif mode == "bucket":
             want = A.bucket_step(w, [g], [A.f32(r["g16"].float()).reshape(-1)], upd["early"], scale, upd["late_bf16"])
         else:
@@ -226,7 +237,7 @@ def update_results(tag: str, init: dict, records: Sequence[dict], upd: dict) -> 
                                      drop=None if drop is None else (drop[0], epochs[t], drop[1]))
         got = A.bits(r["params"])
         res.append(("%s.step%d.update_bits_differ" % (tag, t), float((got != A.bits(want)).sum()), 0.0))
-        adopted = (init if t == 0 else records[t - 1])["params"] if mode in ("kgtn", "interval") else r["params"]
+        adopted = (init if t == 0 else records[t - 1])["params"] if mode in ("kgtn", "interval", "async") else r["params"]
         res.append(("%s.step%d.shadow_bits_differ" % (tag, t),
                     float((_shadow_bits(r["shadow"]) != A.bf16_bits(adopted)).sum()), 0.0))
         w = A.f32(r["params"])

@@ -24,7 +24,7 @@ import dataclasses
 import random
 import time
 from dataclasses import dataclass, field
-from typing import Callable, Dict, List, Optional
+from typing import Callable, Dict, List, Optional, Sequence
 
 import numpy as np
 import torch
@@ -213,6 +213,52 @@ class SyncReplicasOptimizer(_AggregatorBase):
         info = self.backend.sync_step(params, grads, lr, self.local_step, self.replicas_to_aggregate,
                                       delay_s=self._delay_s())
         return self._account(info)
+
+
+STALENESS_BUCKETS = 64         # staleness histogram: bucket b counts tau = b, the last one tau >= 63
+
+
+def staleness_report(hist: Sequence[int], tau_sum: int, tau_max: int) -> Dict:
+    """Updates applied, the histogram, mean, max and p50 / p99 of the staleness tau = s - r of one replica's updates.  The
+    percentiles are read from the histogram: a value of 63 means >= 63."""
+    hist = [int(h) for h in hist]
+    assert len(hist) == STALENESS_BUCKETS
+    n = sum(hist)
+
+    def pct(q: float) -> int:
+        need, run = max(1, int(np.ceil(q * n))), 0
+        for b, h in enumerate(hist):
+            run += h
+            if run >= need:
+                return b
+        return 0
+    return dict(updates=n, hist=hist, mean=(float(tau_sum) / n if n else 0.0), max=int(tau_max),
+                p50=pct(0.5) if n else 0, p99=pct(0.99) if n else 0)
+
+
+class AsyncSGDOptimizer(_AggregatorBase):
+    """Asynchronous SGD (TF's asynchronous parameter-server training): every replica applies its own gradient as soon as it
+    has it, at the learning rate of the global step its update produces, and nothing is averaged, dropped or waited for.
+    The GPU path runs it on the device (csrc/fused_async.cu, see ``FusedBackend.enqueue_async_begin``); here, for the torch
+    engine, it is implemented for one replica only, where it is plain SGD and every update has staleness 0."""
+    mode = "async"
+
+    def __init__(self, backend: Backend, lr_schedule, total_num_replicas: int, straggler=None, seed: int = 0):
+        super().__init__(backend, lr_schedule, total_num_replicas, straggler, seed)
+        self.staleness_hist = [0] * STALENESS_BUCKETS
+        self.tau_sum = self.tau_max = 0
+
+    def apply_gradients(self, params: torch.Tensor, grads: torch.Tensor) -> StepInfo:
+        if self.backend.ctx.world_size != 1:
+            raise ValueError("--async_method with the torch engine is implemented for one replica, not %d"
+                             % self.backend.ctx.world_size)
+        info = self.backend.sync_step(params, grads, self.lr_schedule(self.local_step), self.local_step, 1,
+                                      delay_s=self._delay_s())
+        self.staleness_hist[0] += 1          # one replica: the update is made on the weights it was computed from
+        return self._account(info)
+
+    def staleness(self) -> Dict:
+        return staleness_report(self.staleness_hist, self.tau_sum, self.tau_max)
 
 
 class TimeoutReplicasOptimizer(_AggregatorBase):

@@ -308,6 +308,48 @@ class FusedBackend(Backend):
                              self.ctx.world_size, int(k), params.numel(), lr0, decay_rate, int(decay_steps), self.timeout_ms,
                              int(self.ctas), stream_ptr(stream), pb.multicast_ptr if nv else 0, ab.multicast_ptr if nv else 0)
 
+    # ---- asynchronous SGD (csrc/fused_async.cu) ------------------------------------------------------------------------------
+    def async_arm(self, master: torch.Tensor, params: torch.Tensor, stats: torch.Tensor) -> None:
+        """Start asynchronous SGD from the current weights and global step: the master copy ``master`` (an :meth:`allocate`
+        arena) := ``params``, the staleness statistics ``stats`` (``dm_async_stats_bytes()`` bytes of device memory) zeroed.
+        The chief's update counter is the ``global_step`` word that :meth:`set_global_step` sets.  Collective: every rank
+        calls it, and no replica's first update can land before every copy holds the starting weights."""
+        torch.cuda.synchronize()
+        self.barrier()
+        master.copy_(params)
+        stats.zero_()
+        torch.cuda.synchronize()
+        self.barrier()
+
+    def enqueue_async_begin(self, master: torch.Tensor, params: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Start of an asynchronous iteration: read the update counter r, pull my master copy into ``params`` and the bf16
+        shadow."""
+        self.lib.dm_async_begin(self.ctrl.ptr_table(), self.ctx.rank, master, params, self.shadow, params.numel(),
+                                int(self.ctas), stream_ptr(stream))
+
+    def enqueue_async_end(self, master: torch.Tensor, grads: torch.Tensor, stats: torch.Tensor, lr0: float,
+                          decay_rate: float = 1.0, decay_steps: int = 1, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """End of an asynchronous iteration: take the ticket s of the update, add ``-fl(lr(s) * grads)`` to every replica's
+        master copy (in-switch under the NVLS policy, else one reduction per copy).  Never waits for another replica."""
+        mb = self._by_ptr[master.data_ptr()]
+        mc = mb.multicast_ptr if (self.use_nvls and mb.multicast_ptr) else 0
+        self.lib.dm_async_end(self.ctrl.ptr_table(), mb.ptr_table(), grads, stats, self.ctx.rank, self.ctx.world_size,
+                              master.numel(), lr0, decay_rate, int(decay_steps), int(self.ctas), stream_ptr(stream), mc)
+
+    @staticmethod
+    def async_stats(stats: torch.Tensor) -> Dict:
+        """Decode the staleness statistics (synchronises the device): ``updates``, ``hist`` (64 buckets, the last one
+        counting tau >= 63), ``tau_sum``, ``tau_max`` and ``pairs``, the (r, s) of the last min(updates, 1024) updates, oldest
+        first."""
+        torch.cuda.synchronize()
+        raw = stats.cpu().numpy()
+        hist = raw[:256].view("<u4").astype(np.int64)
+        updates = int(raw[268:272].view("<u4")[0])
+        ring = raw[272:].view("<u4").reshape(-1, 2).astype(np.int64)
+        j = np.arange(max(0, updates - len(ring)), updates)
+        return dict(updates=updates, hist=hist.tolist(), tau_sum=int(raw[256:264].view("<u8")[0]),
+                    tau_max=int(raw[264:268].view("<u4")[0]), pairs=ring[j % len(ring)])
+
     @property
     def nvls_active(self) -> bool:
         return self.use_nvls and bool(self._buffers) and all(b.multicast_ptr for b in self._buffers[:2])

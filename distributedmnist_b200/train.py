@@ -38,8 +38,8 @@ from .early_stopping import EARLY_STOPPING_JSON
 from .engine import make_engine
 from .lr_plateau import LR_PLATEAU_JSON
 from .flags import FLAGS
-from .parallel.aggregators import (SyncReplicasOptimizer, TimeoutReplicasOptimizer,
-                                   parse_straggler_spec)
+from .parallel.aggregators import (AsyncSGDOptimizer, SyncReplicasOptimizer, TimeoutReplicasOptimizer,
+                                   parse_straggler_spec, staleness_report)
 from .parallel.backends import make_backend
 from .parallel.context import ReplicaContext
 from .parallel.timeout_manager import launch_manager
@@ -49,6 +49,8 @@ from .utils.summary import SummaryWriter
 from .utils.timeline import Timeline, cupti_device_spans, timeline_path
 
 log = get_logger()
+
+STALENESS_JSON = "worker%d_staleness.json"
 
 LOG_FORMAT = ("Worker %d: %s: step %d, loss = %f, train_acc = %f, test_acc = %f"
               "(%.1f examples/sec; %.3f  sec/batch)")
@@ -272,6 +274,35 @@ class _IndexFeed:
 
     def close(self) -> None:
         pass                       # no helper thread to stop (same interface as _BatchPacker)
+
+
+def check_async_flags(flags, ctx: ReplicaContext) -> None:
+    """``--async_method`` combinations that cannot work, rejected before any device work starts."""
+    if not getattr(flags, "async_method", False):
+        return
+    if flags.interval_method:
+        raise ValueError("--async_method cannot be combined with --interval_method: both are aggregation modes, and "
+                         "asynchronous SGD applies every gradient on its own instead of a tick's mean")
+    if getattr(flags, "worker_times_cdf_method", False):
+        raise ValueError("--async_method cannot be combined with --worker_times_cdf_method: the cdf mode waits for all "
+                         "replicas behind a full barrier, and asynchronous SGD never waits")
+    k = flags.num_replicas_to_aggregate
+    if k != -1 and k != ctx.world_size:
+        raise ValueError("--async_method applies every gradient on its own, so --num_replicas_to_aggregate must be left "
+                         "unset or equal the number of replicas (%d), got %d" % (ctx.world_size, k))
+    if flags.drop_connect:
+        raise ValueError("--async_method cannot be combined with --drop_connect: the gradient mask is implemented in the "
+                         "synchronous aggregation kernels only")
+    if int(getattr(flags, "lr_plateau_patience", 0) or 0):
+        raise ValueError("--async_method cannot be combined with --lr_plateau_patience: its replicas are not in lock "
+                         "step, so no global step can be named from which every replica applies a cut")
+    if float(getattr(flags, "moving_average_decay", 0.0) or 0.0):
+        raise ValueError("--async_method cannot be combined with --moving_average_decay: the chief's average follows its "
+                         "own arena once per global step, and asynchronous updates land in it at any time")
+    if not (ctx.on_gpu and flags.backend in ("auto", "fused")) and ctx.world_size > 1:
+        raise ValueError("--async_method with the torch engine (--backend=%s%s) is implemented for one replica, not %d: "
+                         "the replicas would need shared weights that every one of them updates"
+                         % (flags.backend, "" if ctx.on_gpu else ", no GPU", ctx.world_size))
 
 
 def check_device_data_flags(flags, ctx: ReplicaContext, dataset) -> None:
@@ -666,6 +697,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         num_replicas_to_aggregate = flags.num_replicas_to_aggregate
     assert num_workers > 0
     is_chief = ctx.is_chief
+    check_async_flags(flags, ctx)
     check_batch_flags(flags, ctx)
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
     check_target_flags(flags, ctx)
@@ -694,7 +726,10 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     lr_schedule = LearningRateSchedule.from_flags(flags, dataset.num_examples, num_replicas_to_aggregate)
     straggler = parse_straggler_spec(flags.inject_straggler, flags.sync_timeout_ms)
 
-    if flags.interval_method or flags.worker_times_cdf_method:
+    async_mode = bool(getattr(flags, "async_method", False))
+    if async_mode:
+        opt = AsyncSGDOptimizer(backend, lr_schedule, total_num_replicas=num_workers, straggler=straggler, seed=flags.seed)
+    elif flags.interval_method or flags.worker_times_cdf_method:
         # reference :179-183 -- interval wins when both are set, as there.
         mode = "interval" if flags.interval_method else "cdf"
         opt = TimeoutReplicasOptimizer(backend, lr_schedule, total_num_replicas=num_workers, mode=mode,
@@ -781,7 +816,10 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         or bool(flags.worker_times_cdf_method and not flags.interval_method)
     # K < N / interval: peers push into the chief's arena at any time -> score a validated snapshot (--eval_snapshot);
     # the host cannot name the step a pass scores in advance, so passes follow the consumed global step (eval_due)
-    snapshot_eval = device_eval and bool(getattr(flags, "eval_snapshot", False)) and not exact
+    snapshot_eval = device_eval and bool(getattr(flags, "eval_snapshot", False)) and not exact and not async_mode
+    # asynchronous SGD: the working arena is private to its replica between iterations, so the pass scores it live, labelled
+    # with the global step r it was pulled at; like snapshot passes, passes follow the consumed global step
+    follow_eval = snapshot_eval or (device_eval and async_mode)
     if device_eval:
         if eval_average:
             engine.arm_eval(dataset_test.images, dataset_test.labels, snapshot=snapshot_eval, moving_average=True)
@@ -861,7 +899,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         # when no peer writes it between steps (the same `exact` test as the evaluation pass), else a validated snapshot
         device_ckpt = fused_step and hasattr(engine, "arm_checkpoint")
         if device_ckpt:
-            engine.arm_checkpoint(snapshot=not exact)
+            engine.arm_checkpoint(snapshot=not (exact or async_mode))
         ckpt = _AsyncCheckpointer(flags.train_dir, spec, flags.save_interval_secs, engine=engine if device_ckpt else None,
                                   timeout_s=flags.sync_timeout_ms * 1e-3,
                                   average=engine._ema if ema_decay and not device_ckpt else None)
@@ -880,6 +918,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             opt.start_interval_updates()   # CPU plumbing path: shared absolute host-clock deadlines
     elif getattr(engine, "_kgtn_k", 0):
         backend.kgtn_arm()                 # K > N on the device: a restore moved the step counter, accumulate from there
+    elif async_mode and fused_step:
+        engine.async_arm()                 # every master copy holds the (restored) weights before the first pull
 
     time_acc_list = []
     step = restored_step
@@ -970,7 +1010,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         nonlocal test_acc_value, last_eval_step, eval_mark, max_steps
         if device_eval:
             collect_evals()        # the step read-back above waited for the pass enqueued after the previous step
-        if snapshot_eval:
+        if follow_eval:
             if global_step <= max_steps and eval_due(global_step, eval_mark, eval_every):
                 eval_mark = global_step
                 engine.enqueue_eval()          # the final pass follows the loop
@@ -1036,7 +1076,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             # input DMA (+ gather) + step graph: one native call
             token = (cur_iteration, engine.step_indices(packer.next()) if device_data else engine.step_packed(packer.next()))
             launched += 1
-            if device_eval and not snapshot_eval and \
+            if device_eval and not follow_eval and \
                     ((restored_step + launched) % eval_every == 0 or restored_step + launched > max_steps):
                 engine.enqueue_eval()          # K == N: restored_step + launched is the global step of the weights it scores
             prev, pending = pending, token
@@ -1051,7 +1091,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
                 now = time.time()
                 finish_iteration(it, last_consume, info, (float(lbuf[0]), float(lbuf[1])))
                 last_consume = now
-                if snapshot_eval and not stop and eval_due(step, eval_mark, eval_every):
+                if follow_eval and not stop and eval_due(step, eval_mark, eval_every):
                     eval_mark = step
                     engine.enqueue_eval()      # after the step just launched: scores the newest committed weights then
                 if device_times and it > 10 and (it % 50 == 0 or it == 500):
@@ -1133,7 +1173,11 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         pending = None
     if packer is not None:
         packer.close()
-    if snapshot_eval:
+    if async_mode and fused_step:
+        # every replica's last update applied, the device barrier, one more pull: the chief's arena, the final pass and
+        # the final checkpoint hold every update of the run, and their global step is the number of updates
+        step = engine.async_finish()
+    if follow_eval:
         engine.enqueue_eval()          # once after the last step
     if device_eval:
         torch.cuda.synchronize()       # the pass after the final step
@@ -1218,6 +1262,17 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         torch.cuda.synchronize()
         st = backend.read_status()
         opt.accepted_steps, opt.dropped_steps = st["accepted_steps"], st["dropped_steps"]
+    if async_mode:
+        st = engine.async_staleness() if fused_step else None
+        rep = staleness_report(st["hist"], st["tau_sum"], st["tau_max"]) if st is not None else opt.staleness()
+        opt.accepted_steps, opt.dropped_steps = rep["updates"], 0
+        results["staleness"] = rep
+        with open(os.path.join(flags.train_dir, STALENESS_JSON % ctx.rank), "w") as f:
+            json.dump(rep, f, indent=1)
+            f.write("\n")
+        log.info("Staleness: worker %d applied %d update(s); staleness of its updates (global steps between pull and "
+                 "update) mean %.3f, p50 %d, p99 %d, max %d; final global step %d"
+                 % (ctx.rank, rep["updates"], rep["mean"], rep["p50"], rep["p99"], rep["max"], step))
     results.update(final_step=step, accepted=opt.accepted_steps, dropped=opt.dropped_steps,
                    params=engine.params, elapsed=time.time() - begin_time,
                    timeout_server=timeout_server, engine=engine, optimizer=opt)
