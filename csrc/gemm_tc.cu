@@ -191,6 +191,20 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
   }
   named_bar_sync(1, GEMM_CONSUMERS);
 
+  if (EPI == EPI_STORE_F32 && n0 + BN <= p.N && (p.ldo & 3) == 0) {
+    // plain fp32 store of a full-width tile (the fc1 forward's split partials): whole rows from the staging tile, BN / 4
+    // consecutive lanes per row, so a warp instruction writes whole 128-byte lines instead of 16 bytes into each of 32
+    float* o = reinterpret_cast<float*>(p.out) + (size_t)blockIdx.z * p.split_stride + n0;
+    constexpr int F4_PER_ROW = BN / 4;
+#pragma unroll 4
+    for (int i = threadIdx.x; i < GEMM_BM * F4_PER_ROW; i += GEMM_CONSUMERS) {
+      const int lr = i / F4_PER_ROW, j = i % F4_PER_ROW;
+      if (m0 + lr < p.M)
+        *reinterpret_cast<float4*>(o + (size_t)(m0 + lr) * p.ldo + 4 * j) = *reinterpret_cast<const float4*>(stage + lr * S::ACC_LD + 4 * j);
+    }
+    return;
+  }
+
   // ------------------------------ epilogue: thread = tile row, 32-column chunks ------------------------------
   constexpr bool DECAY = EPI == EPI_STORE_F32_DECAY || EPI == EPI_STORE_BF16_DECAY;
   double wsq = 0.0;                                  // DECAY: sum of this thread's W^2, chunk by chunk, column by column

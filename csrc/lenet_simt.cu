@@ -52,7 +52,7 @@ struct Fc2Args {
 // not depend on the order in which the rows' CTAs finish.
 constexpr int F2_MAX_ROWS = 1 << 16;                      // batch limit of dm_fc2_fwd_bwd
 // One launch of this kernel in flight per device: the workspace and ticket are static (see arrive_last_cta).
-__device__ float g_f2_row_terms[F2_MAX_ROWS * 2];
+__device__ __align__(8) float g_f2_row_terms[F2_MAX_ROWS * 2];
 __device__ unsigned int g_f2_ticket;
 
 int fc2_fwd_bwd_max_batch() { return F2_MAX_ROWS; }
@@ -138,10 +138,17 @@ __global__ void __launch_bounds__(F2_THREADS) fc2_fwd_bwd_kernel(Fc2Args a) {
   {
     __shared__ unsigned int s_last;
     if (arrive_last_cta(&g_f2_ticket, gridDim.x, 1, F2_THREADS, &s_last) && warp == 0) {
+      // lane l adds rows l, l + 32, ... in row order; 16 rows' loads in flight per round (one L2 round trip at B <= 512)
+      const float2* terms = reinterpret_cast<const float2*>(g_f2_row_terms);
+      const int rows = (int)gridDim.x;
       float l = 0.f, h = 0.f;
-      for (int r = lane; r < (int)gridDim.x; r += 32) {
-        l += __ldcg(g_f2_row_terms + 2 * r);
-        h += __ldcg(g_f2_row_terms + 2 * r + 1);
+      for (int r0 = lane; r0 < rows; r0 += 32 * 16) {
+        float2 v[16];
+#pragma unroll
+        for (int u = 0; u < 16; ++u) v[u] = r0 + 32 * u < rows ? __ldcg(terms + r0 + 32 * u) : make_float2(0.f, 0.f);
+#pragma unroll
+        for (int u = 0; u < 16; ++u)
+          if (r0 + 32 * u < rows) { l += v[u].x; h += v[u].y; }
       }
 #pragma unroll
       for (int o = 16; o > 0; o >>= 1) {
@@ -149,8 +156,9 @@ __global__ void __launch_bounds__(F2_THREADS) fc2_fwd_bwd_kernel(Fc2Args a) {
         h += __shfl_xor_sync(0xffffffffu, h, o);
       }
       if (lane == 0) {
-        a.loss_acc[0] += l;
-        a.loss_acc[1] += h;
+        // fire-and-forget: the launch's last CTA does not wait for a load of the words (same rounding as +=)
+        atomicAdd(a.loss_acc, l);
+        atomicAdd(a.loss_acc + 1, h);
       }
     }
   }
