@@ -125,6 +125,7 @@ class _CudaEngine(ComputeEngine):
     _kgtn_k = 0                  # K > N: gradients per update (count trigger); 0 = the K <= N / interval paths
     _async = False               # asynchronous SGD (csrc/fused_async.cu), see attach_optimizer
     _master = None               # asynchronous SGD: this replica's master copy of the weights (symmetric memory)
+    _local = 0                   # local SGD (csrc/fused_local.cu): H, the averaging period; 0 = off
     _table = None                # device-resident training set (images, labels), see arm_train_data
     _runner = None               # native step runner (csrc/step_runner.cu), see _make_runner
     _stamp = False               # cdf telemetry stamps in the step
@@ -397,6 +398,16 @@ class _CudaEngine(ComputeEngine):
                 self._master = self.backend.allocate(self.spec.arena_numel)
                 self._as_stats = torch.zeros(int(self.lib.dm_async_stats_bytes()), dtype=torch.uint8, device=self.device)
             self.async_arm()                 # train.py re-arms after a restore
+        # local SGD (csrc/fused_local.cu): every iteration updates this replica's own arena; every H-th global step the
+        # arenas are averaged between two device barriers.  Whether a step averages is decided on the device from the epoch
+        # word, so the two slot graphs serve every step; a restore moves that word, and with it the next averaging step
+        self._local = int(getattr(opt, "period", 0)) if getattr(opt, "mode", "") == "local" else 0
+        if self._local:
+            if getattr(opt, "drop_connect_probability", None) is not None:
+                raise ValueError("--drop_connect cannot be combined with --local_sgd_steps")
+            if getattr(self, "_ls_stats", None) is None:
+                self._ls_stats = torch.zeros(int(self.lib.dm_local_stats_bytes()), dtype=torch.uint8, device=self.device)
+            self._ls_stats.zero_()
         # Bucketed aggregation (csrc/fused_sync.cu): full participation on 2/4/8 replicas.  fc1's weight gradient (96.5 % of
         # the bytes) is exchanged by small co-resident CTAs NEXT TO conv2 dgrad/wgrad + conv1 wgrad; the rest goes one-shot.
         #   DMNIST_BUCKET=2 (default): csrc/fused_bucket.cu -- fc1's gradient leaves the GEMM epilogue as bf16, is reduced in
@@ -404,7 +415,7 @@ class _CudaEngine(ComputeEngine):
         #     pass; the small bucket is pushed into every replica's inbox.  Also used on ONE replica (no exchange, the fc1
         #     update still leaves the critical path).   =1: round-1 fp32 two-shot / one-shot kernels.   =0: single kernel.
         mode = os.environ.get("DMNIST_BUCKET", "2")
-        can = int(k) == n and self.backend.drop_keep <= 0.0 and getattr(opt, "mode", "") not in ("interval", "async")
+        can = int(k) == n and self.backend.drop_keep <= 0.0 and getattr(opt, "mode", "") not in ("interval", "async", "local")
         self._bucket_v2 = can and mode == "2" and n in (1, 2, 4, 8)
         self._bucketed = can and ((mode == "1" and n in (2, 4, 8)) or self._bucket_v2)
         if self._bucket_v2 and self._g16 is None:
@@ -518,9 +529,14 @@ class _CudaEngine(ComputeEngine):
             self.backend.enqueue_interval_begin(self.params)
 
     def _enqueue_iteration_end(self) -> None:
-        """Interval mode / K > N: gate, accumulate, close (+ commit attempt), apply.  Asynchronous SGD: ticket, apply."""
+        """Interval mode / K > N: gate, accumulate, close (+ commit attempt), apply.  Asynchronous SGD: ticket, apply.
+        Local SGD: the local update, then the averaging round, which only an averaging step runs."""
         oa = self._opt_args
-        if self._async:
+        if self._local:
+            self.backend.enqueue_local_step(self.params, self.grads, self._local, oa["lr0"], oa["decay_rate"],
+                                            oa["decay_steps"])
+            self.backend.enqueue_local_average(self.params, self._ls_stats, self._local)
+        elif self._async:
             self.backend.enqueue_async_end(self._master, self.grads, self._as_stats, oa["lr0"], oa["decay_rate"],
                                            oa["decay_steps"])
         elif self._kgtn_k:
@@ -551,6 +567,24 @@ class _CudaEngine(ComputeEngine):
     def async_staleness(self) -> dict:
         """This replica's staleness statistics (see FusedBackend.async_stats); synchronises the device."""
         return self.backend.async_stats(self._as_stats)
+
+    # ---- local SGD (csrc/fused_local.cu) ---------------------------------------------------------------------------------
+    def local_finish(self) -> int:
+        """End of a local-SGD run, after the last step was enqueued: if that step was not an averaging step, one more
+        average (without a step), so the weights every replica ends with are the mean.  Returns the global step.
+        Collective: every replica ends on the same step, so all of them average here or none does."""
+        self._leave_native_runner()
+        torch.cuda.synchronize()
+        step = self.backend.device_epoch
+        if step % self._local:
+            self.backend.enqueue_local_average(self.params, self._ls_stats, 1, close=False)
+            torch.cuda.synchronize()
+        self.backend.check_error()
+        return step
+
+    def local_stats(self) -> dict:
+        """This replica's averaging statistics (see FusedBackend.local_stats); synchronises the device."""
+        return self.backend.local_stats(self._ls_stats)
 
     def _run(self, with_sync: bool) -> None:
         s = self._slot
@@ -725,6 +759,8 @@ class _CudaEngine(ComputeEngine):
                              "aggregation peers write the chief's arena at any time")
         if self._async:
             raise ValueError("the moving average is kept for K = N and cdf mode only, not for asynchronous SGD")
+        if self._local:
+            raise ValueError("the moving average is kept for K = N and cdf mode only, not for local SGD")
         self._leave_native_runner()
         torch.cuda.synchronize()
         off = self.backend._off["epoch"]
@@ -1026,7 +1062,8 @@ class CudaLeNetEngine(_CudaEngine):
                  "conv2_wgrad", "conv2_dgrad", "conv1_wgrad"]
         # K > N: adopt + shadow refresh, and gate + accumulate + close + apply, in place of the fused sync kernel
         names = (["kgtn_begin"] + names + ["kgtn_end"]) if self._kgtn_k else \
-            (["async_begin"] + names + ["async_end"]) if self._async else names + ["fused_sync_sgd"]
+            (["async_begin"] + names + ["async_end"]) if self._async else \
+            names + ["local_end"] if self._local else names + ["fused_sync_sgd"]
         tot = {n: 0.0 for n in names}
         B, s = self.batch_size, self._slot
         img, lbl = self.images[s], self.labels[s]
@@ -1051,6 +1088,8 @@ class CudaLeNetEngine(_CudaEngine):
             yield "conv1_wgrad", lambda: self._conv1_wgrad(img, B, sp)
             if self._async:
                 yield "async_end", lambda: self._enqueue_iteration_end()
+            elif self._local:
+                yield "local_end", lambda: self._enqueue_iteration_end()
             elif self._kgtn_k:
                 oa = self._opt_args
                 yield "kgtn_end", lambda: self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"],
@@ -1078,7 +1117,7 @@ class CudaLeNetEngine(_CudaEngine):
 
     def _launch_step(self, slot: int, with_sync: bool) -> None:
         n = 0
-        interval = with_sync and (getattr(self, "_interval", False) or self._async)     # free-running iteration
+        interval = with_sync and (getattr(self, "_interval", False) or self._async or bool(self._local))   # own iteration end
         bucketed = with_sync and self._bucketed and not interval
         self._delay_in_chain = False
         if self._stamp:
@@ -1093,7 +1132,7 @@ class CudaLeNetEngine(_CudaEngine):
         if self._aug is not None:
             images = self._launch_augment(slot)     # conv1_fwd and conv1_wgrad read the augmented batch
             n += 1
-        if interval:
+        if interval and not self._local:
             self._enqueue_iteration_begin()
             n += 2
         n += self._launch_zero()
@@ -1115,7 +1154,7 @@ class CudaLeNetEngine(_CudaEngine):
                 n += 1
             if interval:
                 self._enqueue_iteration_end()
-                n += 2 if self._async else 4
+                n += 5 if self._local else 2 if self._async else 4     # local SGD: the update, the round's four
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1
@@ -1688,8 +1727,8 @@ class CudaMlpEngine(_CudaEngine):
         if self._aug is not None:
             images = self._launch_augment(slot)     # dm_f32_to_bf16 reads the augmented batch
             n += 1
-        interval = with_sync and (getattr(self, "_interval", False) or self._async)     # free-running iteration
-        if interval:
+        interval = with_sync and (getattr(self, "_interval", False) or self._async or bool(self._local))   # own iteration end
+        if interval and not self._local:
             self._enqueue_iteration_begin()
             n += 2
         bucketed = with_sync and self._bucket_v2 and not interval
@@ -1711,7 +1750,7 @@ class CudaMlpEngine(_CudaEngine):
                 n += 1
             if interval:
                 self._enqueue_iteration_end()
-                n += 2 if self._async else 4
+                n += 5 if self._local else 2 if self._async else 4     # local SGD: the update, the round's four
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1

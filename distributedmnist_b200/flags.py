@@ -199,6 +199,10 @@ def define_reference_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_boolean("async_method", False, "Asynchronous SGD: every replica applies its own gradient to the shared "
                                             "weights at once, without waiting for or averaging with any other; reports "
                                             "the staleness of its updates (workerN_staleness.json)")
+    F.DEFINE_integer("local_sgd_steps", 0, "Local SGD (periodic model averaging): every replica applies its own "
+                                           "gradients to its own weights, and every H-th global step the replicas' "
+                                           "weights are replaced by their mean (H = this value; 0 = off); reports the "
+                                           "averaging rounds and their barrier waits (workerN_local_sgd.json)")
     F.DEFINE_boolean("should_summarize", False, "Whether the chief should write summaries")
     F.DEFINE_boolean("timeline_logging", False, "Dump a chrome-trace timeline json per step")
     # reference: src/distributed_train.py:40-48

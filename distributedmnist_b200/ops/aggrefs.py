@@ -207,3 +207,17 @@ def async_apply(w, xs: Sequence) -> np.ndarray:
     for x in xs:
         w = ftz(w + f32(x))
     return w
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# local SGD (csrc/fused_local.cu)
+# ---------------------------------------------------------------------------------------------------------------------
+def local_average(ws: Sequence) -> np.ndarray:
+    """ls_average_kernel's peer-load path: ``fl(S / N)``, S the fp32 sum of the N copies ``ws`` from +0.0 in rank order,
+    the division correctly rounded (``__fdiv_rn``), every operand and result flushed to zero as the FTZ kernels do."""
+    s = None
+    for w in ws:
+        w = ftz(w)
+        s = np.zeros_like(w) if s is None else s
+        s = ftz(s + w)
+    return ftz(s / np.float32(len(ws)))

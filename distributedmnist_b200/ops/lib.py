@@ -93,6 +93,11 @@ def _signatures() -> dict:
         "dm_async_stats_bytes": (V, i, []),
         "dm_async_begin": (S, i, [PP, i, P, P, P, ll, i, P]),
         "dm_async_end": (S, i, [PP, PP, P, P, i, i, ll, d, d, i, i, P, P]),
+        # fused_local.cu
+        "dm_local_stats_bytes": (V, i, []),
+        "dm_local_apply": (S, i, [PP, i, P, P, P, ll, u, d, d, i, i, P, P]),
+        "dm_local_average": (S, i, [PP, PP, P, P, i, i, ll, u, i, d, i, P, P]),
+        "dm_local_average_shard": (S, i, [P, PP, i, i, ll, u, i, P, P]),
         # fused_bucket.cu, fused_interval.cu
         "dm_bucket_sync": (S, i, [PP, PP, PP, PP, PP, i, i, i, ll, ll, ll, d, d, i, d, P, i, P, P, P, i, i]),
         "dm_interval_arm": (S, i, [P, d, P]),

@@ -106,7 +106,9 @@ def ctrl_words(raw, off: Dict[str, int], stamp_step: Optional[int] = None) -> Di
 def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
     """How ``eng`` applies its gradients: ``mode`` "fused" (fused_sync_sgd), "bucket" (the bf16-wire bucketed kernels),
     "kgtn" (K > N: every k-th iteration commits), "interval" (a tick commits when its deadline has passed; ``interval_ns``
-    the armed period) or "async" (asynchronous SGD on one replica: every step pulls the master copy and adds its update), the schedule and the global step of the first step.  ``drop``:
+    the armed period), "async" (asynchronous SGD on one replica: every step pulls the master copy and adds its update) or
+    "local" (local SGD on one replica: every step applies its own update, every ``period``-th global step is averaged),
+    the schedule and the global step of the first step.  ``drop``:
     (seed, keep probability) of the drop-connect mask the fused kernel applies, None without it.  With a cut table armed
     (``arm_lr_cuts``), ``sched`` must name the same cuts (raises ValueError otherwise): the step sizes are then those of
     the schedule with the cuts (synchronises the device to read the table).  ``aug``: (ranges, seed mix) of the armed
@@ -117,6 +119,8 @@ def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
     e0, e1 = eng._bucket_early
     if getattr(eng, "_async", False):
         mode = "async"
+    elif getattr(eng, "_local", 0):
+        mode = "local"
     elif eng._kgtn_k:
         mode = "kgtn"
     elif getattr(eng, "_interval", False):
@@ -131,7 +135,8 @@ def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
                 late_bf16=A.late_bucket_rounds_bf16(eng.spec.arena_numel, e1 - e0, be.late_ll, be.late_bf16),
                 drop=(be.drop_seed, be.drop_keep) if be.drop_keep > 0.0 else None,
                 aug=getattr(eng, "_aug", None), aug_start=int(aug_start), elastic=getattr(eng, "_aug_elastic", None),
-                interval_ns=be.interval_ns if mode == "interval" else None, ctrl_off=dict(be._off))
+                interval_ns=be.interval_ns if mode == "interval" else None, ctrl_off=dict(be._off),
+                period=getattr(eng, "_local", 0))
 
 
 def epoch_of(upd: dict, t: int) -> int:
@@ -230,6 +235,10 @@ def update_results(tag: str, init: dict, records: Sequence[dict], upd: dict) -> 
         elif mode == "async":
             want = A.async_apply(w, [A.async_update(g, scale)])
             res.append(("%s.step%d.pull_bits_differ" % (tag, t), float((A.bits(r["pulled"]) != A.bits(w)).sum()), 0.0))
+        elif mode == "local":
+            want = A.sgd(w, g, scale)
+            if (epochs[t] + 1) % upd["period"] == 0:
+                want = A.local_average([want])
         elif mode == "bucket":
             want = A.bucket_step(w, [g], [A.f32(r["g16"].float()).reshape(-1)], upd["early"], scale, upd["late_bf16"])
         else:

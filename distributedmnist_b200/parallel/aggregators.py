@@ -261,6 +261,56 @@ class AsyncSGDOptimizer(_AggregatorBase):
         return staleness_report(self.staleness_hist, self.tau_sum, self.tau_max)
 
 
+def local_sgd_report(period: int, rounds: int, wait_total_ns: int, wait_max_ns: int) -> Dict:
+    """H, the averaging rounds one replica took part in, and the time it spent in their barriers."""
+    return dict(period=int(period), rounds=int(rounds), wait_total_s=int(wait_total_ns) * 1e-9,
+                wait_max_s=int(wait_max_ns) * 1e-9, wait_mean_s=int(wait_total_ns) * 1e-9 / rounds if rounds else 0.0)
+
+
+class LocalSGDOptimizer(_AggregatorBase):
+    """Local SGD (periodic model averaging): every replica applies its own gradient to its own weights, at the learning
+    rate of the global step, and after every ``period``-th global step every replica's weights become the mean of all
+    replicas' weights.  The GPU path runs it on the device (csrc/fused_local.cu, see ``FusedBackend.enqueue_local_step``);
+    here, for the torch engine, the average is an ``all_reduce`` of the weights over the process group, divided by N."""
+    mode = "local"
+
+    def __init__(self, backend: Backend, lr_schedule, total_num_replicas: int, period: int, straggler=None, seed: int = 0):
+        super().__init__(backend, lr_schedule, total_num_replicas, straggler, seed)
+        if int(period) < 1:
+            raise ValueError("local SGD needs an averaging period of at least 1 step, got %d" % period)
+        self.period = int(period)
+        self.rounds = 0
+        self.wait_total_ns = self.wait_max_ns = 0
+        self.before_average: Optional[torch.Tensor] = None    # this replica's weights before the newest average
+
+    def apply_gradients(self, params: torch.Tensor, grads: torch.Tensor) -> StepInfo:
+        delay = self._delay_s()
+        if delay > 0:
+            time.sleep(delay)
+        params.add_(grads, alpha=-float(self.lr_schedule(self.local_step)))
+        step = self.local_step + 1
+        if step % self.period == 0:
+            self.average(params)
+        return self._account(StepInfo(step, True, 1 << self.backend.ctx.rank, 1))
+
+    def average(self, params: torch.Tensor) -> None:
+        """Every replica's ``params`` := the mean of all of them (collective).  The time spent in the collective is this
+        path's barrier wait."""
+        n = self.backend.ctx.world_size
+        self.before_average = params.detach().clone()
+        if n > 1:
+            t0 = time.perf_counter_ns()
+            torch.distributed.all_reduce(params, op=torch.distributed.ReduceOp.SUM)
+            params.div_(n)
+            ns = time.perf_counter_ns() - t0
+            self.wait_total_ns += ns
+            self.wait_max_ns = max(self.wait_max_ns, ns)
+        self.rounds += 1
+
+    def report(self) -> Dict:
+        return local_sgd_report(self.period, self.rounds, self.wait_total_ns, self.wait_max_ns)
+
+
 class TimeoutReplicasOptimizer(_AggregatorBase):
     """Modes B ("cdf": full barrier + per-iteration timing) and C ("interval")."""
 

@@ -350,6 +350,39 @@ class FusedBackend(Backend):
         return dict(updates=updates, hist=hist.tolist(), tau_sum=int(raw[256:264].view("<u8")[0]),
                     tau_max=int(raw[264:268].view("<u4")[0]), pairs=ring[j % len(ring)])
 
+    # ---- local SGD (csrc/fused_local.cu) ---------------------------------------------------------------------------------
+    def _local_mc(self, params: torch.Tensor) -> int:
+        pb = self._by_ptr[params.data_ptr()]
+        return pb.multicast_ptr if (self.use_nvls and pb.multicast_ptr and self.ctx.world_size > 1) else 0
+
+    def enqueue_local_step(self, params: torch.Tensor, grads: torch.Tensor, period: int, lr0: float,
+                           decay_rate: float = 1.0, decay_steps: int = 1, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """The local update of one iteration: ``params -= fp32(lr(s)) * grads`` and the bf16 shadow, s = this replica's
+        global step, with the armed schedule.  Never waits for another replica."""
+        self.lib.dm_local_apply(self.ctrl.ptr_table(), self.ctx.rank, params, grads, self.shadow, params.numel(),
+                                int(period), lr0, decay_rate, int(decay_steps), int(self.ctas), stream_ptr(stream),
+                                self._local_mc(params))
+
+    def enqueue_local_average(self, params: torch.Tensor, stats: torch.Tensor, period: int, close: bool = True,
+                              stream: Optional[torch.cuda.Stream] = None) -> None:
+        """After :meth:`enqueue_local_step` (``close``): the step is closed, and when its global step is a multiple of
+        ``period`` every replica's arena and shadow become the mean of all arenas, between two device barriers.  The
+        NVLS policy picks the in-switch reduction, else the rank-ordered peer loads.  ``close=False, period=1``: one
+        unconditional average that closes no step (the end of a run).  ``stats``: ``dm_local_stats_bytes()`` bytes."""
+        pb = self._by_ptr[params.data_ptr()]
+        self.lib.dm_local_average(self.ctrl.ptr_table(), pb.ptr_table(), self.shadow, stats, self.ctx.rank,
+                                  self.ctx.world_size, params.numel(), int(period), int(bool(close)), self.timeout_ms,
+                                  int(self.ctas), stream_ptr(stream), self._local_mc(params))
+
+    @staticmethod
+    def local_stats(stats: torch.Tensor) -> Dict:
+        """Decode the averaging statistics (synchronises the device): ``rounds``, ``wait_total_ns``, ``wait_max_ns`` (the
+        %globaltimer time of a round's two barriers, summed and at most)."""
+        torch.cuda.synchronize()
+        raw = stats.cpu().numpy()
+        return dict(rounds=int(raw[0:4].view("<u4")[0]), wait_total_ns=int(raw[8:16].view("<u8")[0]),
+                    wait_max_ns=int(raw[16:24].view("<u8")[0]))
+
     @property
     def nvls_active(self) -> bool:
         return self.use_nvls and bool(self._buffers) and all(b.multicast_ptr for b in self._buffers[:2])

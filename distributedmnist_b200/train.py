@@ -38,8 +38,8 @@ from .early_stopping import EARLY_STOPPING_JSON
 from .engine import make_engine
 from .lr_plateau import LR_PLATEAU_JSON
 from .flags import FLAGS
-from .parallel.aggregators import (AsyncSGDOptimizer, SyncReplicasOptimizer, TimeoutReplicasOptimizer,
-                                   parse_straggler_spec, staleness_report)
+from .parallel.aggregators import (AsyncSGDOptimizer, LocalSGDOptimizer, SyncReplicasOptimizer, TimeoutReplicasOptimizer,
+                                   local_sgd_report, parse_straggler_spec, staleness_report)
 from .parallel.backends import make_backend
 from .parallel.context import ReplicaContext
 from .parallel.timeout_manager import launch_manager
@@ -51,6 +51,7 @@ from .utils.timeline import Timeline, cupti_device_spans, timeline_path
 log = get_logger()
 
 STALENESS_JSON = "worker%d_staleness.json"
+LOCAL_SGD_JSON = "worker%d_local_sgd.json"
 
 LOG_FORMAT = ("Worker %d: %s: step %d, loss = %f, train_acc = %f, test_acc = %f"
               "(%.1f examples/sec; %.3f  sec/batch)")
@@ -89,10 +90,12 @@ class _AsyncCheckpointer:
             self._thread = threading.Thread(target=self._write_loop, daemon=True)
             self._thread.start()
 
-    def maybe_save(self, params: torch.Tensor, global_step: int) -> None:
+    def maybe_save(self, params: torch.Tensor, global_step: int, capture: bool = True) -> None:
+        """``capture=False``: the weights after the step are not to be saved (local SGD between two averages); a capture
+        in flight is still collected, and a due one waits for a call that allows it."""
         if self.engine is not None:
             self._collect(self.engine.checkpoint_poll() if self._pending else None)
-            if self._pending or not (self._retry or time.time() >= self._next):
+            if self._pending or not capture or not (self._retry or time.time() >= self._next):
                 return
             with self._lock:
                 buf = next((b for b, free in enumerate(self._free) if free), None)
@@ -101,7 +104,7 @@ class _AsyncCheckpointer:
             self._next = time.time() + self.interval_s
             self._enqueue(buf)
             return
-        if time.time() >= self._next:
+        if capture and time.time() >= self._next:
             self._next = time.time() + self.interval_s
             self.save(params, global_step, blocking=False)
 
@@ -303,6 +306,51 @@ def check_async_flags(flags, ctx: ReplicaContext) -> None:
         raise ValueError("--async_method with the torch engine (--backend=%s%s) is implemented for one replica, not %d: "
                          "the replicas would need shared weights that every one of them updates"
                          % (flags.backend, "" if ctx.on_gpu else ", no GPU", ctx.world_size))
+
+
+def check_local_sgd_flags(flags, ctx: ReplicaContext) -> None:
+    """``--local_sgd_steps`` combinations that cannot work, rejected before any device work starts."""
+    h = getattr(flags, "local_sgd_steps", 0)
+    if isinstance(h, bool) or not isinstance(h, int):
+        raise ValueError("--local_sgd_steps must be an integer, got %r" % (h,))
+    if h == 0:
+        return
+    if not 1 <= h < 2 ** 31:
+        raise ValueError("--local_sgd_steps is the number of local steps between two averages: 1 <= H < 2^31, or 0 for "
+                         "off; got %d" % h)
+    if flags.interval_method:
+        raise ValueError("--local_sgd_steps cannot be combined with --interval_method: both are aggregation modes, and "
+                         "local SGD averages weights every H steps instead of a tick's gradients")
+    if getattr(flags, "worker_times_cdf_method", False):
+        raise ValueError("--local_sgd_steps cannot be combined with --worker_times_cdf_method: the cdf mode times a full "
+                         "barrier on every step, and local SGD has one only every H steps")
+    if getattr(flags, "async_method", False):
+        raise ValueError("--local_sgd_steps cannot be combined with --async_method: asynchronous SGD shares one set of "
+                         "weights, and local SGD keeps one per replica")
+    k = flags.num_replicas_to_aggregate
+    if k != -1 and k != ctx.world_size:
+        raise ValueError("--local_sgd_steps averages every replica's weights, so --num_replicas_to_aggregate must be left "
+                         "unset or equal the number of replicas (%d), got %d" % (ctx.world_size, k))
+    if flags.drop_connect:
+        raise ValueError("--local_sgd_steps cannot be combined with --drop_connect: the gradient mask is implemented in "
+                         "the synchronous aggregation kernels only")
+    if float(getattr(flags, "moving_average_decay", 0.0) or 0.0):
+        raise ValueError("--local_sgd_steps cannot be combined with --moving_average_decay: between two averages the "
+                         "chief's weights are its own, not the model's")
+    if int(getattr(flags, "lr_plateau_patience", 0) or 0):
+        raise ValueError("--local_sgd_steps cannot be combined with --lr_plateau_patience: a cut must take effect on "
+                         "the same global step on every replica, and the plateau rule does not place it on an "
+                         "averaging step")
+    every = int(getattr(flags, "eval_every_steps", 0) or 0)
+    if every % h:
+        raise ValueError("--eval_every_steps (%d) must be a multiple of --local_sgd_steps (%d): the in-training "
+                         "evaluation scores the averaged model, which exists only after an averaging step" % (every, h))
+
+
+def stop_margin(flags) -> int:
+    """S - g: the stop step S of an evaluation pass of global step g that stops the run.  STOP_MARGIN steps, or
+    STOP_MARGIN averaging periods with local SGD (DESIGN §4.4)."""
+    return STOP_MARGIN * max(1, int(getattr(flags, "local_sgd_steps", 0) or 0))
 
 
 def check_device_data_flags(flags, ctx: ReplicaContext, dataset) -> None:
@@ -606,8 +654,9 @@ class _EarlyStopping:
     the sm_90a path eval_patience has made the same decisions on the device, which set the stop; this replays them from
     the pass records for the report.  With the torch engine this is where the stop is decided."""
 
-    def __init__(self, patience: int, min_delta: float, examples: int, weights: str):
+    def __init__(self, patience: int, min_delta: float, examples: int, weights: str, margin: int = None):
         self.patience, self.min_delta, self.examples, self.weights = patience, min_delta, examples, weights
+        self.margin = STOP_MARGIN if margin is None else int(margin)
         self.delta_rows = early_stopping.min_delta_rows(min_delta, examples)
         self.state = early_stopping.State()
         self.counted = 0             # counting passes up to the one that exhausted the patience
@@ -625,7 +674,7 @@ class _EarlyStopping:
         fired = early_stopping.exhausted(s, self.patience)
         return dict(patience=self.patience, min_delta=self.min_delta, min_delta_rows=self.delta_rows,
                     examples=self.examples, triggered=fired, trigger_step=s.trigger_step if fired else None,
-                    stop_step=s.trigger_step + STOP_MARGIN if fired else None,
+                    stop_step=s.trigger_step + self.margin if fired else None,
                     best_step=s.best_step if s.baseline else None, best_correct=s.best if s.baseline else None,
                     counted_passes=self.counted, weights=self.weights)
 
@@ -698,6 +747,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     assert num_workers > 0
     is_chief = ctx.is_chief
     check_async_flags(flags, ctx)
+    check_local_sgd_flags(flags, ctx)
     check_batch_flags(flags, ctx)
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
     check_target_flags(flags, ctx)
@@ -727,8 +777,13 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     straggler = parse_straggler_spec(flags.inject_straggler, flags.sync_timeout_ms)
 
     async_mode = bool(getattr(flags, "async_method", False))
+    local_h = int(getattr(flags, "local_sgd_steps", 0) or 0)
+    margin = stop_margin(flags)
     if async_mode:
         opt = AsyncSGDOptimizer(backend, lr_schedule, total_num_replicas=num_workers, straggler=straggler, seed=flags.seed)
+    elif local_h:
+        opt = LocalSGDOptimizer(backend, lr_schedule, total_num_replicas=num_workers, period=local_h, straggler=straggler,
+                                seed=flags.seed)
     elif flags.interval_method or flags.worker_times_cdf_method:
         # reference :179-183 -- interval wins when both are set, as there.
         mode = "interval" if flags.interval_method else "cdf"
@@ -812,8 +867,10 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     # host memory once the following step has been consumed; torch engine: engine.evaluate, synchronously.
     eval_every = int(getattr(flags, "eval_every_steps", 0) or 0) if is_chief else 0
     device_eval = bool(eval_every and fused_step)
+    # local SGD is in lock step too: every replica makes one iteration per global step, and no peer writes the chief's
+    # arena outside the averaging rounds the chief takes part in
     exact = isinstance(opt, SyncReplicasOptimizer) and num_replicas_to_aggregate == num_workers \
-        or bool(flags.worker_times_cdf_method and not flags.interval_method)
+        or bool(flags.worker_times_cdf_method and not flags.interval_method) or bool(local_h)
     # K < N / interval: peers push into the chief's arena at any time -> score a validated snapshot (--eval_snapshot);
     # the host cannot name the step a pass scores in advance, so passes follow the consumed global step (eval_due)
     snapshot_eval = device_eval and bool(getattr(flags, "eval_snapshot", False)) and not exact and not async_mode
@@ -840,7 +897,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         tta = _TimeToAccuracy(target, need_count(target, n_val), n_val, 1e-9 if device_eval else 1.0,
                               "device %globaltimer" if device_eval else "host")
         if device_eval:
-            engine.arm_target(tta.need, STOP_MARGIN)
+            engine.arm_target(tta.need, margin)
     eval_weights = "snapshot" if snapshot_eval else ("moving_average" if eval_average else "live")
     # --early_stopping_patience: the run ends as --max_steps = min(--max_steps, S) would end it, S = g + STOP_MARGIN for the
     # pass of global step g that exhausts the patience -- decided like the target (GPU path: eval_patience on the device,
@@ -848,9 +905,9 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     es = None
     if patience and is_chief:
         es = _EarlyStopping(patience, float(getattr(flags, "early_stopping_min_delta", 0.0) or 0.0),
-                            dataset_test.num_examples, eval_weights)
+                            dataset_test.num_examples, eval_weights, margin)
         if device_eval:
-            engine.arm_patience(patience, es.delta_rows, STOP_MARGIN)
+            engine.arm_patience(patience, es.delta_rows, margin)
     # --lr_plateau_patience: from S = g + STOP_MARGIN on, for the pass of global step g that exhausts the patience, every
     # update is made at the rate times --lr_plateau_factor once more (GPU path: eval_plateau stores S into every replica's
     # cut table, which the aggregation kernels read; torch engine: decided on the host after `evaluate`, into the shared
@@ -970,7 +1027,10 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             if eval_every:
                 save_evals()
         if is_chief:
-            ckpt.maybe_save(engine.params, step)
+            # local SGD: only the weights after an averaging step are the model; the capture follows the newest launched
+            # step (one past `step` in the pipelined loop)
+            ckpt.maybe_save(engine.params, step, capture=not local_h or (restored_step + launched if pipelined else step)
+                            % local_h == 0)
             if summary is not None and next_summary_time < time.time():
                 log.info("Running Summary operation on the chief.")
                 summary.add_scalars({"loss": loss_value, "train_acc": train_acc_value,
@@ -1017,6 +1077,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             return
         if global_step == last_eval_step or not (global_step % eval_every == 0 or global_step > max_steps):
             return
+        if local_h and global_step > max_steps and not local_done:
+            return                 # the final pass follows the run's final average
         last_eval_step = global_step
         if device_eval:
             engine.enqueue_eval()
@@ -1034,9 +1096,9 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         if keep_best:
             engine.note_eval(global_step, n_ex, n_ex, correct, loss * n_ex, moving_average=eval_average)
         if tta is not None and tta.add(global_step, t0, t1, n_ex, correct, True, t1 - tta_wall0):
-            max_steps = min(max_steps, global_step + STOP_MARGIN)
+            max_steps = min(max_steps, global_step + margin)
         if es is not None and es.add(global_step, n_ex, correct):
-            max_steps = min(max_steps, global_step + STOP_MARGIN)
+            max_steps = min(max_steps, global_step + margin)
         if lp is not None:
             lp.add(global_step, n_ex, correct)
 
@@ -1056,6 +1118,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             timeout_client.broadcast_worker_finished_computing_gradients(it, ta * 1e-9)
         cdf_pushed = upto + 1
 
+    local_done = False
     last_consume = time.time()
     tta_wall0 = time.time()        # --target_accuracy: the run's first step starts now (host clock) ...
     if tta is not None and device_eval:
@@ -1077,7 +1140,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             token = (cur_iteration, engine.step_indices(packer.next()) if device_data else engine.step_packed(packer.next()))
             launched += 1
             if device_eval and not follow_eval and \
-                    ((restored_step + launched) % eval_every == 0 or restored_step + launched > max_steps):
+                    ((restored_step + launched) % eval_every == 0 or restored_step + launched > max_steps) and \
+                    not (local_h and restored_step + launched > max_steps):
                 engine.enqueue_eval()          # K == N: restored_step + launched is the global step of the weights it scores
             prev, pending = pending, token
             if prev is not None:
@@ -1177,6 +1241,21 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         # every replica's last update applied, the device barrier, one more pull: the chief's arena, the final pass and
         # the final checkpoint hold every update of the run, and their global step is the number of updates
         step = engine.async_finish()
+    local_done = True              # local SGD: eval_after_step may score the step past --max_steps from here on
+    if local_h:
+        # the last step was not an averaging step: one more average, so the final pass, the final checkpoint and the
+        # returned weights are the model every replica holds (collective: every replica ends on the same step)
+        if fused_step:
+            step = engine.local_finish()
+        elif step % local_h:
+            opt.average(engine.params)
+            if hasattr(engine, "params_updated"):
+                engine.params_updated()
+        if eval_every:
+            if device_eval:
+                engine.enqueue_eval()
+            else:
+                eval_after_step(step)
     if follow_eval:
         engine.enqueue_eval()          # once after the last step
     if device_eval:
@@ -1273,6 +1352,17 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         log.info("Staleness: worker %d applied %d update(s); staleness of its updates (global steps between pull and "
                  "update) mean %.3f, p50 %d, p99 %d, max %d; final global step %d"
                  % (ctx.rank, rep["updates"], rep["mean"], rep["p50"], rep["p99"], rep["max"], step))
+    if local_h:
+        st = engine.local_stats() if fused_step else None
+        rep = local_sgd_report(local_h, st["rounds"], st["wait_total_ns"], st["wait_max_ns"]) if st is not None \
+            else opt.report()
+        results["local_sgd"] = rep
+        with open(os.path.join(flags.train_dir, LOCAL_SGD_JSON % ctx.rank), "w") as f:
+            json.dump(rep, f, indent=1)
+            f.write("\n")
+        log.info("Local SGD: worker %d averaged every %d step(s); %d averaging round(s), %.6f s in their barriers "
+                 "(mean %.6f s, max %.6f s); final global step %d"
+                 % (ctx.rank, local_h, rep["rounds"], rep["wait_total_s"], rep["wait_mean_s"], rep["wait_max_s"], step))
     results.update(final_step=step, accepted=opt.accepted_steps, dropped=opt.dropped_steps,
                    params=engine.params, elapsed=time.time() - begin_time,
                    timeout_server=timeout_server, engine=engine, optimizer=opt)
