@@ -16,6 +16,16 @@
 // is private to its replica between iterations, so the live evaluation pass and the live checkpoint capture read one
 // pulled state.  Visibility of my own update before my next pull, the end of a run and the bound on extra updates:
 // DESIGN.md §4, "Asynchronous SGD".
+//
+// Stale synchronous parallel (--ssp_staleness=s) adds two 1-warp kernels around that iteration:
+//
+//   ssp_wait     (1 warp)   before as_pull_step: wait until every peer p that has not retired has clock c_p >= c - s,
+//                           c = my clock (updates I have applied); statistics
+//   ssp_publish  (1 warp)   after as_apply: c := c + 1, released into line `rank` of every replica's clock board; the
+//                           same kernel with 0xFFFFFFFF retires me once my last iteration is enqueued
+//
+// These are the only async kernels that poll a word another replica writes.  The wait rule, the ordering argument and
+// the bounds it gives: DESIGN.md §4, "Stale synchronous parallel".
 #include "fused_sync.cuh"
 
 namespace dm {
@@ -121,6 +131,78 @@ __global__ void __launch_bounds__(AS_THREADS) as_apply_kernel(AsyncPeers P, Sync
   if (threadIdx.x == 0) fence_acq_rel_sys();
 }
 
+// ---- stale synchronous parallel ---------------------------------------------------------------------------------------
+constexpr int SSP_LOG = 1024;                  // ring of the last (c, min peer clock) pairs
+constexpr uint32_t SSP_RETIRED = 0xFFFFFFFFu;  // the clock of a replica that has enqueued its last iteration
+
+// Bound statistics and the clock of one replica, in plain device memory owned by its engine (nobody else writes it).
+struct SSPStats {
+  uint32_t clock;                  // c: updates this replica has applied and published since the bound was armed
+  uint32_t waits;                  // iterations whose wait found some peer too far behind
+  uint32_t lead_max;               // largest c - (min clock of the non-retired peers) at a pull
+  uint32_t pad;
+  unsigned long long wait_total_ns;
+  unsigned long long wait_max_ns;
+  uint32_t pairs[2 * SSP_LOG];     // (c, min non-retired peer clock or 0xFFFFFFFF) of iteration c at [2 * (c % SSP_LOG)]
+};
+static_assert(sizeof(SSPStats) == 32 + 8 * SSP_LOG, "distributedmnist_b200/parallel/fused.py decodes this layout");
+
+// The clock boards: every replica owns one symmetric board of SYNC_MAX_RANKS 128-byte lines, as SyncCtrl::bar is laid
+// out; line p holds peer p's clock.
+struct SSPBoards {
+  uint32_t* board[SYNC_MAX_RANKS];
+};
+
+// Lane p polls peer p's clock in my board with relaxed loads; spin_until ends the wait with one acquire load of it.  The
+// predicate c_p + s >= c in 64 bits is c_p >= c - s without a wrap at small c, and always true for a retired peer.  Once
+// the warp has synchronised, lane 0's system-scope fence makes every lane's acquire cumulative, and the kernel boundary
+// carries it to as_pull_step and as_pull: the pull reads every update each peer applied before it released the clock it
+// was seen with (DESIGN.md §4).
+__global__ void ssp_wait_kernel(const uint32_t* board, SyncCtrl* me, SSPStats* st, int rank, int nranks, uint32_t s,
+                                unsigned long long timeout_ns) {
+  pdl_wait();
+  const int lane = threadIdx.x;
+  const uint32_t c = st->clock;
+  const volatile uint32_t* line = board + 32 * lane;
+  const bool peer = lane < nranks && lane != rank;
+  const auto ready = [&] { return (unsigned long long)ld_relaxed_sys(line) + s >= (unsigned long long)c; };
+  const unsigned long long t0 = globaltimer_ns();
+  const bool behind = peer && !ready();
+  bool ok = true;
+  uint32_t seen = SSP_RETIRED;
+  if (peer) {
+    ok = spin_until(ready, timeout_ns, line);
+    seen = ld_relaxed_sys(line);             // >= the value that satisfied the wait: a clock only grows
+  }
+  const bool waited = __any_sync(0xffffffffu, behind);
+  const bool all_ok = __all_sync(0xffffffffu, ok);
+  const uint32_t lo = __reduce_min_sync(0xffffffffu, seen);
+  if (lane == 0) {
+    fence_acq_rel_sys();
+    if (!all_ok) me->error = 3;
+    if (waited) {
+      const unsigned long long ns = globaltimer_ns() - t0;
+      st->waits += 1;
+      st->wait_total_ns += ns;
+      st->wait_max_ns = max(st->wait_max_ns, ns);
+    }
+    if (lo != SSP_RETIRED && c > lo) st->lead_max = max(st->lead_max, c - lo);
+    st->pairs[2 * (c % SSP_LOG)] = c;
+    st->pairs[2 * (c % SSP_LOG) + 1] = lo;
+  }
+}
+
+// c := c + 1 (or the retired value), stored with release semantics into line `rank` of every board.  It follows as_apply
+// on the stream, whose CTAs each ended with a system-scope fence (after fence.proxy.alias on the NVLS path): the release
+// is ordered after my update has been added to every master copy.
+__global__ void ssp_publish_kernel(SSPBoards B, SSPStats* st, int rank, int nranks, int retire) {
+  pdl_wait();
+  const uint32_t c = retire ? SSP_RETIRED : st->clock + 1u;
+  __syncwarp();
+  if (threadIdx.x < nranks) st_release_sys(B.board[threadIdx.x] + 32 * rank, c);
+  if (threadIdx.x == 0 && !retire) st->clock = c;
+}
+
 }  // namespace dm
 
 extern "C" {
@@ -165,6 +247,34 @@ int dm_async_end(void* const* ctrl, void* const* master, const void* grads, void
   if (e != cudaSuccess) return (int)e;
   return (int)launch_kernel(as_apply_kernel, dim3(ctas), dim3(AS_THREADS), 0, st, P, a, (const SyncCtrl*)me,
                             reinterpret_cast<const float*>(grads), reinterpret_cast<float*>(mc_master));
+}
+
+int dm_ssp_stats_bytes() { return (int)sizeof(dm::SSPStats); }
+
+// Stale synchronous parallel, before dm_async_begin: wait until every peer of `nranks` that has not retired has a clock
+// of at least c - `s` in my clock board `board` (c: my clock in `stats`).  On a timeout of `timeout_ms` the error word of
+// my control block `ctrl` becomes 3.
+int dm_ssp_wait(const void* board, void* ctrl, void* stats, int rank, int nranks, unsigned int s, double timeout_ms,
+                void* stream_) {
+  using namespace dm;
+  if (nranks < 1 || nranks > SYNC_MAX_RANKS || rank < 0 || rank >= nranks || s > 0x7fffffffu || board == nullptr ||
+      ctrl == nullptr || stats == nullptr)
+    return -1;
+  return (int)launch_kernel(ssp_wait_kernel, dim3(1), dim3(32), 0, reinterpret_cast<cudaStream_t>(stream_),
+                            reinterpret_cast<const uint32_t*>(board), reinterpret_cast<SyncCtrl*>(ctrl),
+                            reinterpret_cast<SSPStats*>(stats), rank, nranks, s,
+                            (unsigned long long)(timeout_ms * 1e6));
+}
+
+// After dm_async_end: advance my clock in `stats` and publish it into every board of the table `boards`; `retire` != 0
+// publishes the retired value 0xFFFFFFFF instead and leaves the clock alone.
+int dm_ssp_publish(void* const* boards, void* stats, int rank, int nranks, int retire, void* stream_) {
+  using namespace dm;
+  if (nranks < 1 || nranks > SYNC_MAX_RANKS || rank < 0 || rank >= nranks || stats == nullptr) return -1;
+  SSPBoards B;
+  for (int i = 0; i < SYNC_MAX_RANKS; ++i) B.board[i] = reinterpret_cast<uint32_t*>(boards[i < nranks ? i : rank]);
+  return (int)launch_kernel(ssp_publish_kernel, dim3(1), dim3(32), 0, reinterpret_cast<cudaStream_t>(stream_), B,
+                            reinterpret_cast<SSPStats*>(stats), rank, nranks, retire);
 }
 
 }  // extern "C"

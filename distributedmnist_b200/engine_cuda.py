@@ -125,6 +125,8 @@ class _CudaEngine(ComputeEngine):
     _kgtn_k = 0                  # K > N: gradients per update (count trigger); 0 = the K <= N / interval paths
     _async = False               # asynchronous SGD (csrc/fused_async.cu), see attach_optimizer
     _master = None               # asynchronous SGD: this replica's master copy of the weights (symmetric memory)
+    _ssp = -1                    # asynchronous SGD: the staleness bound s (--ssp_staleness); -1 = unbounded
+    _ssp_stats = None            # its statistics and clock (FusedBackend.ssp_arm)
     _local = 0                   # local SGD (csrc/fused_local.cu): H, the averaging period; 0 = off
     _table = None                # device-resident training set (images, labels), see arm_train_data
     _runner = None               # native step runner (csrc/step_runner.cu), see _make_runner
@@ -397,6 +399,11 @@ class _CudaEngine(ComputeEngine):
             if self._master is None:
                 self._master = self.backend.allocate(self.spec.arena_numel)
                 self._as_stats = torch.zeros(int(self.lib.dm_async_stats_bytes()), dtype=torch.uint8, device=self.device)
+        # stale synchronous parallel: a wait before the pull and a clock publication after the apply
+        self._ssp = int(getattr(opt, "ssp_staleness", -1)) if self._async else -1
+        if self._async:
+            if self._ssp >= 0 and self._ssp_stats is None:
+                self._ssp_stats = self.backend.ssp_arm()
             self.async_arm()                 # train.py re-arms after a restore
         # local SGD (csrc/fused_local.cu): every iteration updates this replica's own arena; every H-th global step the
         # arenas are averaged between two device barriers.  Whether a step averages is decided on the device from the epoch
@@ -520,8 +527,10 @@ class _CudaEngine(ComputeEngine):
 
     def _enqueue_iteration_begin(self) -> None:
         """Interval mode / K > N: adopt pushed weights (+ shadow refresh) at the start of an iteration.  Asynchronous SGD:
-        read the update counter, pull the master copy (+ shadow)."""
+        read the update counter, pull the master copy (+ shadow), after the staleness bound's wait when one is armed."""
         if self._async:
+            if self._ssp >= 0:
+                self.backend.enqueue_ssp_wait(self._ssp_stats, self._ssp)
             self.backend.enqueue_async_begin(self._master, self.params)
         elif self._kgtn_k:
             self.backend.enqueue_kgtn_begin(self.params)
@@ -539,6 +548,8 @@ class _CudaEngine(ComputeEngine):
         elif self._async:
             self.backend.enqueue_async_end(self._master, self.grads, self._as_stats, oa["lr0"], oa["decay_rate"],
                                            oa["decay_steps"])
+            if self._ssp >= 0:
+                self.backend.enqueue_ssp_publish(self._ssp_stats)
         elif self._kgtn_k:
             self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"], oa["decay_rate"],
                                           oa["decay_steps"])
@@ -548,15 +559,20 @@ class _CudaEngine(ComputeEngine):
     # ---- asynchronous SGD (csrc/fused_async.cu) ------------------------------------------------------------------------------
     def async_arm(self) -> None:
         """Every master copy := the working arena (the initial or restored weights), staleness statistics zeroed; the
-        first pull reads them.  Collective."""
+        first pull reads them.  With the staleness bound armed, every clock board and the bound's statistics, with this
+        replica's clock, are zeroed too.  Collective."""
         self._leave_native_runner()
-        self.backend.async_arm(self._master, self.params, self._as_stats)
+        self.backend.async_arm(self._master, self.params, self._as_stats, self._ssp_stats if self._ssp >= 0 else None)
 
     def async_finish(self) -> int:
-        """End of an asynchronous run, after the last step was enqueued: every replica's last update has been applied, the
-        device barrier (every replica's updates are in every master copy after it), then one more pull into the working
-        arena.  Returns the global step of the pulled weights: the total number of updates.  Collective."""
+        """End of an asynchronous run, after the last step was enqueued: with the staleness bound armed, this replica
+        retires (no peer waits for its clock again); every replica's last update has been applied, the device barrier
+        (every replica's updates are in every master copy after it), then one more pull into the working arena.  Returns
+        the global step of the pulled weights: the total number of updates.  Collective."""
         self._leave_native_runner()
+        if self._ssp >= 0:
+            # before anything waits for a peer: a peer still in its last iterations may be waiting for this clock
+            self.backend.enqueue_ssp_retire(self._ssp_stats)
         torch.cuda.synchronize()
         self.backend.device_barrier()
         self.backend.enqueue_async_begin(self._master, self.params)
@@ -567,6 +583,10 @@ class _CudaEngine(ComputeEngine):
     def async_staleness(self) -> dict:
         """This replica's staleness statistics (see FusedBackend.async_stats); synchronises the device."""
         return self.backend.async_stats(self._as_stats)
+
+    def ssp_stats(self) -> dict:
+        """This replica's staleness-bound statistics (see FusedBackend.ssp_stats); synchronises the device."""
+        return self.backend.ssp_stats(self._ssp_stats)
 
     # ---- local SGD (csrc/fused_local.cu) ---------------------------------------------------------------------------------
     def local_finish(self) -> int:
@@ -1134,7 +1154,7 @@ class CudaLeNetEngine(_CudaEngine):
             n += 1
         if interval and not self._local:
             self._enqueue_iteration_begin()
-            n += 2
+            n += 3 if self._ssp >= 0 else 2       # the staleness bound's wait before the pull
         n += self._launch_zero()
         n += self._launch_forward(images, self.labels[slot], self.batch_size, True)
         n += self._launch_backward(images, self.batch_size, early_sync=bucketed)
@@ -1154,7 +1174,7 @@ class CudaLeNetEngine(_CudaEngine):
                 n += 1
             if interval:
                 self._enqueue_iteration_end()
-                n += 5 if self._local else 2 if self._async else 4     # local SGD: the update, the round's four
+                n += 5 if self._local else (2 + (self._ssp >= 0)) if self._async else 4     # local SGD: the update, the round's four
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1
@@ -1730,7 +1750,7 @@ class CudaMlpEngine(_CudaEngine):
         interval = with_sync and (getattr(self, "_interval", False) or self._async or bool(self._local))   # own iteration end
         if interval and not self._local:
             self._enqueue_iteration_begin()
-            n += 2
+            n += 3 if self._ssp >= 0 else 2       # the staleness bound's wait before the pull
         bucketed = with_sync and self._bucket_v2 and not interval
         n += self._launch_zero()
         n += self._forward(images, self.labels[slot], B, True)
@@ -1750,7 +1770,7 @@ class CudaMlpEngine(_CudaEngine):
                 n += 1
             if interval:
                 self._enqueue_iteration_end()
-                n += 5 if self._local else 2 if self._async else 4     # local SGD: the update, the round's four
+                n += 5 if self._local else (2 + (self._ssp >= 0)) if self._async else 4     # local SGD: the update, the round's four
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1

@@ -199,6 +199,10 @@ def define_reference_flags(F: FlagValues = FLAGS) -> FlagValues:
     F.DEFINE_boolean("async_method", False, "Asynchronous SGD: every replica applies its own gradient to the shared "
                                             "weights at once, without waiting for or averaging with any other; reports "
                                             "the staleness of its updates (workerN_staleness.json)")
+    F.DEFINE_integer("ssp_staleness", -1, "Stale synchronous parallel, with --async_method: no replica starts an "
+                                          "iteration more than s of its own updates ahead of the slowest replica that "
+                                          "is still running (s = this value, 0 <= s < 2^31; -1 = off, plain "
+                                          "asynchronous SGD); reports its waits (workerN_ssp.json)")
     F.DEFINE_integer("local_sgd_steps", 0, "Local SGD (periodic model averaging): every replica applies its own "
                                            "gradients to its own weights, and every H-th global step the replicas' "
                                            "weights are replaced by their mean (H = this value; 0 = off); reports the "

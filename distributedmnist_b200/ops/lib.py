@@ -93,6 +93,9 @@ def _signatures() -> dict:
         "dm_async_stats_bytes": (V, i, []),
         "dm_async_begin": (S, i, [PP, i, P, P, P, ll, i, P]),
         "dm_async_end": (S, i, [PP, PP, P, P, i, i, ll, d, d, i, i, P, P]),
+        "dm_ssp_stats_bytes": (V, i, []),
+        "dm_ssp_wait": (S, i, [P, P, P, i, i, u, d, P]),
+        "dm_ssp_publish": (S, i, [PP, P, i, i, i, P]),
         # fused_local.cu
         "dm_local_stats_bytes": (V, i, []),
         "dm_local_apply": (S, i, [PP, i, P, P, P, ll, u, d, d, i, i, P, P]),

@@ -240,13 +240,19 @@ class AsyncSGDOptimizer(_AggregatorBase):
     """Asynchronous SGD (TF's asynchronous parameter-server training): every replica applies its own gradient as soon as it
     has it, at the learning rate of the global step its update produces, and nothing is averaged, dropped or waited for.
     The GPU path runs it on the device (csrc/fused_async.cu, see ``FusedBackend.enqueue_async_begin``); here, for the torch
-    engine, it is implemented for one replica only, where it is plain SGD and every update has staleness 0."""
+    engine, it is implemented for one replica only, where it is plain SGD and every update has staleness 0.
+
+    ``ssp_staleness`` = s >= 0 bounds it (stale synchronous parallel, ``--ssp_staleness``): no replica starts its
+    iteration c before every peer that has not retired has applied c - s updates.  -1: unbounded.  One replica never
+    waits, so here it changes nothing."""
     mode = "async"
 
-    def __init__(self, backend: Backend, lr_schedule, total_num_replicas: int, straggler=None, seed: int = 0):
+    def __init__(self, backend: Backend, lr_schedule, total_num_replicas: int, straggler=None, seed: int = 0,
+                 ssp_staleness: int = -1):
         super().__init__(backend, lr_schedule, total_num_replicas, straggler, seed)
         self.staleness_hist = [0] * STALENESS_BUCKETS
         self.tau_sum = self.tau_max = 0
+        self.ssp_staleness = int(ssp_staleness)
 
     def apply_gradients(self, params: torch.Tensor, grads: torch.Tensor) -> StepInfo:
         if self.backend.ctx.world_size != 1:
@@ -259,6 +265,13 @@ class AsyncSGDOptimizer(_AggregatorBase):
 
     def staleness(self) -> Dict:
         return staleness_report(self.staleness_hist, self.tau_sum, self.tau_max)
+
+
+def ssp_report(s: int, waits: int, wait_total_ns: int, wait_max_ns: int, lead_max: int, updates: int) -> Dict:
+    """The staleness bound s of one replica, the iterations that waited for a peer, the time spent waiting, the largest
+    clock lead over the slowest non-retired peer seen at a pull, and the updates the replica applied."""
+    return dict(s=int(s), waits=int(waits), wait_total_ns=int(wait_total_ns), wait_max_ns=int(wait_max_ns),
+                lead_max=int(lead_max), updates=int(updates))
 
 
 def local_sgd_report(period: int, rounds: int, wait_total_ns: int, wait_max_ns: int) -> Dict:

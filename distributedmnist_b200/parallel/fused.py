@@ -29,6 +29,8 @@ from .backends import Backend, StepInfo
 from .context import ReplicaContext
 from .symm_mem import SymmetricBuffer, allocate_symmetric
 
+SSP_LINES = 8                  # clock-board lines, one per possible replica (SYNC_MAX_RANKS in csrc/fused_sync.cuh)
+
 
 class FusedBackend(Backend):
     name = "fused"
@@ -79,6 +81,7 @@ class FusedBackend(Backend):
         self.drop_seed = 0
         self.interval_ns: Optional[int] = None     # the interval clock's period, once armed (interval_arm)
         self.lr_schedule_armed = False             # the control block evaluates a warmup / cosine (set_lr_schedule)
+        self._ssp_board: Optional[SymmetricBuffer] = None   # stale synchronous parallel: this replica's clock board
 
     # ---- memory ---------------------------------------------------------------------------
     def allocate(self, numel: int) -> torch.Tensor:
@@ -171,7 +174,7 @@ class FusedBackend(Backend):
                 import sys
                 self.debug_dump(sys.stderr)
             raise RuntimeError("fused sync watchdog fired on rank %d: %s timeout (DMNIST_DEBUG_SYNC=1 / --debug_sync dumps "
-                               "the control block)" % (self.ctx.rank, {1: "arrival", 2: "push-complete"}.get(e, str(e))))
+                               "the control block)" % (self.ctx.rank, {1: "arrival", 2: "push-complete", 3: "staleness-bound"}.get(e, str(e))))
 
     def debug_dump(self, out=None) -> str:
         """The accumulator / token-queue state of the reference's debug Print ops (…modified.py:230-234,383-387), here: every
@@ -309,15 +312,21 @@ class FusedBackend(Backend):
                              int(self.ctas), stream_ptr(stream), pb.multicast_ptr if nv else 0, ab.multicast_ptr if nv else 0)
 
     # ---- asynchronous SGD (csrc/fused_async.cu) ------------------------------------------------------------------------------
-    def async_arm(self, master: torch.Tensor, params: torch.Tensor, stats: torch.Tensor) -> None:
+    def async_arm(self, master: torch.Tensor, params: torch.Tensor, stats: torch.Tensor,
+                  ssp_stats: Optional[torch.Tensor] = None) -> None:
         """Start asynchronous SGD from the current weights and global step: the master copy ``master`` (an :meth:`allocate`
         arena) := ``params``, the staleness statistics ``stats`` (``dm_async_stats_bytes()`` bytes of device memory) zeroed.
         The chief's update counter is the ``global_step`` word that :meth:`set_global_step` sets.  Collective: every rank
-        calls it, and no replica's first update can land before every copy holds the starting weights."""
+        calls it, and no replica's first update can land before every copy holds the starting weights.  ``ssp_stats``
+        (from :meth:`ssp_arm`): the staleness bound is armed too -- the clock board and the bound's statistics, with the
+        clock, are zeroed, and no replica's first wait can read a clock of an earlier run."""
         torch.cuda.synchronize()
         self.barrier()
         master.copy_(params)
         stats.zero_()
+        if ssp_stats is not None:
+            self._ssp_board.view(torch.int32, 0, 32 * SSP_LINES).zero_()
+            ssp_stats.zero_()
         torch.cuda.synchronize()
         self.barrier()
 
@@ -349,6 +358,46 @@ class FusedBackend(Backend):
         j = np.arange(max(0, updates - len(ring)), updates)
         return dict(updates=updates, hist=hist.tolist(), tau_sum=int(raw[256:264].view("<u8")[0]),
                     tau_max=int(raw[264:268].view("<u4")[0]), pairs=ring[j % len(ring)])
+
+    # ---- stale synchronous parallel (csrc/fused_async.cu) ----------------------------------------------------------------
+    def ssp_arm(self) -> torch.Tensor:
+        """Prepare the staleness bound: this replica's clock board (one 128-byte line per peer, symmetric, allocated on
+        first use -- collective, like :meth:`allocate`) and a new statistics block (``dm_ssp_stats_bytes()`` bytes of
+        device memory, which also holds the clock), returned.  :meth:`async_arm` with ``ssp_stats`` zeroes both."""
+        if self._ssp_board is None:
+            self._ssp_board = self.allocate_buffer(128 * SSP_LINES)
+        return torch.zeros(int(self.lib.dm_ssp_stats_bytes()), dtype=torch.uint8, device=self.ctx.device)
+
+    def enqueue_ssp_wait(self, stats: torch.Tensor, s: int, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Before :meth:`enqueue_async_begin`: wait until every peer that has not retired has applied at least c - ``s``
+        updates, c = this replica's clock.  A wait longer than the watchdog sets the error word (3)."""
+        self.lib.dm_ssp_wait(self._ssp_board.local_ptr, self.ctrl.local_ptr, stats, self.ctx.rank, self.ctx.world_size,
+                             int(s), self.timeout_ms, stream_ptr(stream))
+
+    def enqueue_ssp_publish(self, stats: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """After :meth:`enqueue_async_end`: this replica's clock + 1, released into every replica's board."""
+        self.lib.dm_ssp_publish(self._ssp_board.ptr_table(), stats, self.ctx.rank, self.ctx.world_size, 0,
+                                stream_ptr(stream))
+
+    def enqueue_ssp_retire(self, stats: torch.Tensor, stream: Optional[torch.cuda.Stream] = None) -> None:
+        """Once this replica's last iteration is enqueued: publish the retired clock, so no peer waits for it again."""
+        self.lib.dm_ssp_publish(self._ssp_board.ptr_table(), stats, self.ctx.rank, self.ctx.world_size, 1,
+                                stream_ptr(stream))
+
+    @staticmethod
+    def ssp_stats(stats: torch.Tensor) -> Dict:
+        """Decode the bound's statistics (synchronises the device): ``clock`` (updates applied), ``waits``,
+        ``wait_total_ns``, ``wait_max_ns``, ``lead_max`` and ``pairs``, the (c, min clock of the non-retired peers --
+        0xFFFFFFFF: none) of the last min(clock + 1, 1024) pulls, oldest first."""
+        torch.cuda.synchronize()
+        raw = stats.cpu().numpy()
+        w = raw[:16].view("<u4")
+        ring = raw[32:].view("<u4").reshape(-1, 2).astype(np.int64)
+        clock = int(w[0])
+        j = np.arange(max(0, clock + 1 - len(ring)), clock + 1)
+        pairs = ring[j % len(ring)]
+        return dict(clock=clock, waits=int(w[1]), lead_max=int(w[2]), wait_total_ns=int(raw[16:24].view("<u8")[0]),
+                    wait_max_ns=int(raw[24:32].view("<u8")[0]), pairs=pairs[pairs[:, 0] == j])
 
     # ---- local SGD (csrc/fused_local.cu) ---------------------------------------------------------------------------------
     def _local_mc(self, params: torch.Tensor) -> int:

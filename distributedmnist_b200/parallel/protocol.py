@@ -564,21 +564,39 @@ class BucketV2Model:
             waiting[r] = w
 
 
-def explore_schedules(make_model, max_runs: int = 200000) -> int:
+class _Visited(Exception):
+    """explore_schedules(dedup=True): the run reached a choice point whose state an earlier run has expanded."""
+
+
+def explore_schedules(make_model, max_runs: int = 200000, dedup: bool = False) -> int:
     """Run ``make_model().run`` under EVERY schedule (depth-first over the scheduler's choice points, replaying prefixes).
-    Returns the number of complete schedules; raises the first ``ProtocolHazard``."""
-    stack, runs = [[]], 0
+    Returns the number of complete schedules; raises the first ``ProtocolHazard``.
+
+    ``dedup``: the model's ``state()`` names everything its future depends on, so a choice point whose (state, runnable
+    actors) an earlier run has already expanded is not expanded again and its run ends there.  Every reachable state and
+    every transition is still visited -- what a model's per-step and end-of-run checks need -- without enumerating the
+    exponentially many orders that lead to the same state.  The return value then counts runs, not schedules."""
+    stack, runs, seen = [[]], 0, set()
     while stack:
         prefix = stack.pop()
         trace = []
+        model = make_model()
 
-        def choose(runnable, prefix=prefix, trace=trace):
+        def choose(runnable, prefix=prefix, trace=trace, model=model):
             i = len(trace)
+            if dedup and i >= len(prefix):
+                key = (model.state(), tuple(runnable))
+                if key in seen:
+                    raise _Visited()
+                seen.add(key)
             c = prefix[i] if i < len(prefix) else 0
             trace.append((c, len(runnable)))
             return runnable[c]
 
-        make_model().run(choose)
+        try:
+            model.run(choose)
+        except _Visited:
+            pass
         runs += 1
         if runs > max_runs:
             raise RuntimeError("more than %d schedules" % max_runs)
@@ -1160,6 +1178,133 @@ class TargetStopModel:
         if self.evals != want:
             raise ProtocolHazard("the chief enqueued passes after steps %s, a run with --max_steps=%d after %s"
                                  % (self.evals, s, want))
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Stale synchronous parallel -- word-level model of ssp_wait / as_pull_step / as_pull / as_ticket / as_apply / ssp_publish
+# (csrc/fused_async.cu) and of the training loop's stop rule with retirement
+# ----------------------------------------------------------------------------------------------------------------------
+SSP_RETIRED = 0xFFFFFFFF
+
+
+class SSPModel:
+    """N replicas running asynchronous SGD under the staleness bound s, as generators for :func:`explore_schedules`.
+
+    Memory: ``counts[d][p]`` is the number of replica p's updates that have landed in replica d's master copy (with
+    integer updates this is what the copy's slot p holds), ``board[d][p]`` peer p's clock in replica d's clock board,
+    ``counter`` the chief's update counter.  One iteration of replica q with clock c is two atomic steps:
+
+    * the wait (blocked until every peer's clock in q's board is >= c - s, or retired), the read of r and the pull of
+      q's master copy -- as one step, the earliest the pull can happen: a copy's counts and the counter only grow, so a
+      later read could only see more;
+    * the ticket, the apply to every copy and the publication of c + 1 into every board -- as one step, the latest the
+      ticket and the apply can happen before the release, which the kernels' fences order after them.
+
+    The host's stop rule: the pipelined loop has launched iteration i + 1 when it reads iteration i's ticket t, and stops
+    launching once t + 1 > ``max_steps``; replica q also stops after ``iters[q]`` iterations (a replica that stops early).
+    A stopped replica publishes the retired clock into every board.
+
+    Checked at every step (``ProtocolHazard`` otherwise), B1-B4 of DESIGN.md §4:
+    B1 q's pull holds its own c updates, at least c - s of each peer it saw running, and every update of each peer it
+    saw retired; B2 c - (smallest running peer clock seen) <= s; B3 tau = ticket - r <= (N - 1)(2s + 1); B4 no state
+    in which every unfinished replica is blocked.  At the end: every copy holds every update, the tickets are 0 .. T - 1,
+    and two replicas that both stopped by the stop rule differ by at most s + 3 updates.
+
+    Mutants, each of which must fail: ``publish_before_apply`` (the clock is released before the update lands),
+    ``retire=False`` and ``slack=1`` (the wait admits c - s - 1)."""
+
+    def __init__(self, n: int, s: int, iters, max_steps: int = 1 << 30, publish_before_apply: bool = False,
+                 retire: bool = True, slack: int = 0):
+        self.n, self.s, self.iters, self.max_steps = n, s, list(iters), max_steps
+        self.publish_before_apply, self.retire, self.slack = publish_before_apply, retire, slack
+        self.counts = [[0] * n for _ in range(n)]
+        self.board = [[0] * n for _ in range(n)]
+        self.counter = 0
+        self.clock = [0] * n           # updates q has applied and published
+        self.r = [-1] * n              # r of q's current iteration, -1 between iterations
+        self.stop_at = list(self.iters)   # iterations q runs: lowered by the stop rule
+        self.by_rule = [False] * n     # q stopped by the stop rule (not by its own iteration count)
+        self.tickets: List[int] = []
+        self.done = [False] * n
+        self.pc = [0] * n              # where q's generator stands: 0 wait, 1 pulled, 2 published (mutant), 3 applied
+
+    def state(self):
+        return (tuple(map(tuple, self.counts)), tuple(map(tuple, self.board)), self.counter, tuple(self.clock),
+                tuple(self.r), tuple(self.stop_at), tuple(self.by_rule), tuple(self.done), tuple(self.pc))
+
+    def replica(self, q: int):
+        n, s = self.n, self.s
+        peers = [p for p in range(n) if p != q]
+        c = 0
+        while c < self.stop_at[q]:
+            self.pc[q] = 0
+            yield (lambda c=c: all(self.board[q][p] + s + self.slack >= c for p in peers))
+            seen = [self.board[q][p] for p in range(n)]
+            pulled = list(self.counts[q])
+            self.r[q] = self.counter
+            if pulled[q] != c:
+                raise ProtocolHazard("B1: replica %d pulled %d of its own updates in iteration %d" % (q, pulled[q], c))
+            for p in peers:
+                if seen[p] == SSP_RETIRED and pulled[p] != self.stop_at[p]:
+                    raise ProtocolHazard("B1: replica %d saw %d retired but pulled %d of its %d updates"
+                                         % (q, p, pulled[p], self.stop_at[p]))
+                if seen[p] != SSP_RETIRED and pulled[p] < c - s:
+                    raise ProtocolHazard("B1: replica %d pulled %d of replica %d's updates in iteration %d, s = %d"
+                                         % (q, pulled[p], p, c, s))
+            running = [seen[p] for p in peers if seen[p] != SSP_RETIRED]
+            if running and c - min(running) > s:
+                raise ProtocolHazard("B2: replica %d started iteration %d with peer clocks %s, s = %d" % (q, c, seen, s))
+            self.pc[q] = 1
+            yield None
+            t = self.counter
+            self.counter += 1
+            self.tickets.append(t)
+            if t - self.r[q] > (n - 1) * (2 * s + 1):
+                raise ProtocolHazard("B3: replica %d pulled at r = %d and took ticket %d" % (q, self.r[q], t))
+            self.r[q] = -1
+            if self.publish_before_apply:
+                for d in range(n):
+                    self.board[d][q] = c + 1
+                self.pc[q] = 2
+                yield None
+            for d in range(n):
+                self.counts[d][q] += 1
+            for d in range(n):
+                self.board[d][q] = c + 1
+            self.clock[q] = c + 1
+            # the host read this iteration's ticket with the next one launched: stop after that one
+            if t + 1 > self.max_steps and c + 2 < self.stop_at[q]:
+                self.stop_at[q] = c + 2
+                self.by_rule[q] = True
+            c += 1
+            self.pc[q] = 3
+            yield None
+        if self.retire:
+            for d in range(n):
+                self.board[d][q] = SSP_RETIRED
+        self.done[q] = True
+
+    def run(self, choose) -> None:
+        gens = {q: self.replica(q) for q in range(self.n)}
+        waiting = {}
+        for q in list(gens):
+            BucketV2Model._advance(q, gens, waiting)
+        while gens:
+            runnable = [q for q in sorted(gens) if q not in waiting or waiting[q]()]
+            if not runnable:
+                raise ProtocolHazard("B4: deadlock, replicas %s wait forever (clocks %s, boards %s)"
+                                     % (sorted(gens), self.clock, self.board))
+            q = choose(runnable)
+            waiting.pop(q, None)
+            BucketV2Model._advance(q, gens, waiting)
+        for d in range(self.n):
+            if self.counts[d] != self.clock:
+                raise ProtocolHazard("replica %d's copy holds %s updates, the replicas applied %s" % (d, self.counts[d], self.clock))
+        if sorted(self.tickets) != list(range(sum(self.clock))):
+            raise ProtocolHazard("tickets %s are not a permutation" % sorted(self.tickets))
+        ruled = [self.clock[q] for q in range(self.n) if self.by_rule[q]]
+        if ruled and max(ruled) - min(ruled) > self.s + 3:
+            raise ProtocolHazard("replicas stopped by the stop rule applied %s updates, s = %d" % (self.clock, self.s))
 
 
 def run_random(make_model, seeds) -> int:

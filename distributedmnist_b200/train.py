@@ -39,7 +39,7 @@ from .engine import make_engine
 from .lr_plateau import LR_PLATEAU_JSON
 from .flags import FLAGS
 from .parallel.aggregators import (AsyncSGDOptimizer, LocalSGDOptimizer, SyncReplicasOptimizer, TimeoutReplicasOptimizer,
-                                   local_sgd_report, parse_straggler_spec, staleness_report)
+                                   local_sgd_report, parse_straggler_spec, ssp_report, staleness_report)
 from .parallel.backends import make_backend
 from .parallel.context import ReplicaContext
 from .parallel.timeout_manager import launch_manager
@@ -51,6 +51,7 @@ from .utils.timeline import Timeline, cupti_device_spans, timeline_path
 log = get_logger()
 
 STALENESS_JSON = "worker%d_staleness.json"
+SSP_JSON = "worker%d_ssp.json"
 LOCAL_SGD_JSON = "worker%d_local_sgd.json"
 
 LOG_FORMAT = ("Worker %d: %s: step %d, loss = %f, train_acc = %f, test_acc = %f"
@@ -280,8 +281,17 @@ class _IndexFeed:
 
 
 def check_async_flags(flags, ctx: ReplicaContext) -> None:
-    """``--async_method`` combinations that cannot work, rejected before any device work starts."""
+    """``--async_method`` (and ``--ssp_staleness``) combinations that cannot work, rejected before any device work
+    starts."""
+    s = getattr(flags, "ssp_staleness", -1)
+    if isinstance(s, bool) or not isinstance(s, int):
+        raise ValueError("--ssp_staleness must be an integer, got %r" % (s,))
+    if not -1 <= s < 2 ** 31:
+        raise ValueError("--ssp_staleness is the number of its own updates a replica may run ahead of the slowest one: "
+                         "0 <= s < 2^31, or -1 for off; got %d" % s)
     if not getattr(flags, "async_method", False):
+        if s != -1:
+            raise ValueError("--ssp_staleness bounds asynchronous SGD and needs --async_method")
         return
     if flags.interval_method:
         raise ValueError("--async_method cannot be combined with --interval_method: both are aggregation modes, and "
@@ -780,7 +790,8 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     local_h = int(getattr(flags, "local_sgd_steps", 0) or 0)
     margin = stop_margin(flags)
     if async_mode:
-        opt = AsyncSGDOptimizer(backend, lr_schedule, total_num_replicas=num_workers, straggler=straggler, seed=flags.seed)
+        opt = AsyncSGDOptimizer(backend, lr_schedule, total_num_replicas=num_workers, straggler=straggler, seed=flags.seed,
+                                ssp_staleness=int(getattr(flags, "ssp_staleness", -1)))
     elif local_h:
         opt = LocalSGDOptimizer(backend, lr_schedule, total_num_replicas=num_workers, period=local_h, straggler=straggler,
                                 seed=flags.seed)
@@ -1352,6 +1363,19 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         log.info("Staleness: worker %d applied %d update(s); staleness of its updates (global steps between pull and "
                  "update) mean %.3f, p50 %d, p99 %d, max %d; final global step %d"
                  % (ctx.rank, rep["updates"], rep["mean"], rep["p50"], rep["p99"], rep["max"], step))
+        ssp = int(getattr(flags, "ssp_staleness", -1))
+        if ssp >= 0:
+            # the torch engine runs one replica, which never waits
+            b = engine.ssp_stats() if fused_step else dict(waits=0, wait_total_ns=0, wait_max_ns=0, lead_max=0)
+            rep = ssp_report(ssp, b["waits"], b["wait_total_ns"], b["wait_max_ns"], b["lead_max"], rep["updates"])
+            results["ssp"] = rep
+            with open(os.path.join(flags.train_dir, SSP_JSON % ctx.rank), "w") as f:
+                json.dump(rep, f, indent=1)
+                f.write("\n")
+            log.info("Stale synchronous: worker %d ran at most %d update(s) ahead of the slowest running replica; %d of "
+                     "its %d update(s) waited, %.6f s in total, longest %.6f s; largest lead seen %d; final global step %d"
+                     % (ctx.rank, ssp, rep["waits"], rep["updates"], rep["wait_total_ns"] * 1e-9,
+                        rep["wait_max_ns"] * 1e-9, rep["lead_max"], step))
     if local_h:
         st = engine.local_stats() if fused_step else None
         rep = local_sgd_report(local_h, st["rounds"], st["wait_total_ns"], st["wait_max_ns"]) if st is not None \
