@@ -528,6 +528,9 @@ int dm_bucket_sync(void* const* ctrl, void* const* params, void* const* grads, v
   // large late bucket (the MLPs: megabytes) is bandwidth-bound and goes as plain data + release flags
   if (late_ll && (long long)n_late4 * 16 <= (1ll << 20)) {        // no in-kernel barrier: any grid size is safe
     if (grid > 296) grid = 296;
+    // ... across GPUs.  Every thread polls peers' lines, so replicas that share one GPU need their grids co-resident:
+    // `ctas` >= 1 caps the grid (the loops stride by the grid), 0 keeps the one-round grid above.
+    if (ctas >= 1 && grid > ctas) grid = ctas;
     if (late_bf16) return (int)launch_kernel(bucket_late_ll_kernel<true>, dim3(grid), dim3(LATE2_THREADS), 0, stream, P, a, r);
     return (int)launch_kernel(bucket_late_ll_kernel<false>, dim3(grid), dim3(LATE2_THREADS), 0, stream, P, a, r);
   }
