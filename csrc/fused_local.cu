@@ -34,29 +34,12 @@ struct LocalPeers {
 
 DMNIST_DEVICE bool averaging_step(const SyncCtrl* me, uint32_t period) { return me->epoch % period == 0u; }
 
-// The barrier of both rounds' sides, on the existing device-barrier words (bar[], bar_seq), so that it and
-// dm_device_barrier keep one sequence: every replica runs the same steps, hence the same barriers in the same order.
-// Lane p releases my arrival into peer p's block and polls peer p's arrival in mine with relaxed loads; spin_until ends
-// every wait with one acquire load of the flag it polled.  Reading the peers' weights after the barrier needs that
-// acquire: the polls alone order nothing.  Once the warp has synchronised, lane 0 adds one system-scope fence, so every
-// lane's acquire is cumulative through it, and the kernel boundary carries it to every later kernel of the stream:
-// after this kernel, everything each peer wrote before its release is visible here.  Returns the nanoseconds spent.
+// The barrier of both rounds' sides: peer_barrier (fused_sync.cuh) over every rank, on the device barrier's words, so
+// that it and dm_device_barrier keep one sequence: every replica runs the same steps, hence the same barriers in the same
+// order.  Returns the nanoseconds spent.
 DMNIST_DEVICE unsigned long long ls_barrier(const LocalPeers& P, SyncCtrl* me, int rank, int nranks,
                                             unsigned long long timeout_ns) {
-  const unsigned long long t0 = globaltimer_ns();
-  const uint32_t seq = me->bar_seq + 1;
-  if (threadIdx.x < nranks) {
-    st_release_sys(&P.ctrl[threadIdx.x]->bar[rank * 32], seq);
-    if (!spin_until([&] { return ld_relaxed_sys(&me->bar[threadIdx.x * 32]) >= seq; }, timeout_ns,
-                    &me->bar[threadIdx.x * 32]))
-      me->error = 1;
-  }
-  __syncwarp();
-  if (threadIdx.x == 0) {
-    fence_acq_rel_sys();
-    me->bar_seq = seq;
-  }
-  return globaltimer_ns() - t0;
+  return peer_barrier(P, me, rank, (1u << nranks) - 1u, timeout_ns);
 }
 
 __global__ void __launch_bounds__(LS_THREADS) ls_apply_kernel(SyncArgs a, SyncCtrl* me, const float* __restrict__ grads,

@@ -267,4 +267,35 @@ DMNIST_DEVICE bool spin_until(Pred pred, unsigned long long timeout_ns, const vo
   return ok;
 }
 
+// Device barrier over the ranks of `set` (bit p: rank p; mine may be among them), on the device barrier's words (bar[],
+// bar_seq), so that every barrier a replica takes part in, whoever its partners, advances one sequence: local SGD's
+// rounds (every rank), gossip SGD's steps (the ring neighbours) and dm_device_barrier.  `P.ctrl` is the table of every
+// replica's control block.  Called by one full warp.  Lane p releases my arrival into peer p's block and polls peer p's
+// arrival in mine with relaxed loads; spin_until ends every wait with one acquire load of the flag it polled.  Reading a
+// peer's data after the barrier needs that acquire: the polls alone order nothing.  Once the warp has synchronised, lane
+// 0 adds one system-scope fence, so every lane's acquire is cumulative through it, and the kernel boundary carries it to
+// every later kernel of the stream: after this kernel, everything each peer of `set` wrote before its release is
+// visible here.  A wait past `timeout_ns` sets the error word to 1.  Returns the nanoseconds spent; `waited` (may be
+// null) becomes true when some peer had not yet arrived at the first poll.
+template <class Peers>
+DMNIST_DEVICE unsigned long long peer_barrier(const Peers& P, SyncCtrl* me, int rank, uint32_t set,
+                                              unsigned long long timeout_ns, bool* waited = nullptr) {
+  const unsigned long long t0 = globaltimer_ns();
+  const uint32_t seq = me->bar_seq + 1;
+  bool late = false;
+  if (threadIdx.x < SYNC_MAX_RANKS && ((set >> threadIdx.x) & 1u)) {
+    st_release_sys(&P.ctrl[threadIdx.x]->bar[rank * 32], seq);
+    const volatile uint32_t* flag = &me->bar[threadIdx.x * 32];
+    if (waited != nullptr) late = ld_relaxed_sys(flag) < seq;
+    if (!spin_until([&] { return ld_relaxed_sys(flag) >= seq; }, timeout_ns, flag)) me->error = 1;
+  }
+  if (waited != nullptr) *waited = __any_sync(0xffffffffu, late);
+  __syncwarp();
+  if (threadIdx.x == 0) {
+    fence_acq_rel_sys();
+    me->bar_seq = seq;
+  }
+  return globaltimer_ns() - t0;
+}
+
 }  // namespace dm

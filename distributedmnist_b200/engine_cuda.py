@@ -128,6 +128,8 @@ class _CudaEngine(ComputeEngine):
     _ssp = -1                    # asynchronous SGD: the staleness bound s (--ssp_staleness); -1 = unbounded
     _ssp_stats = None            # its statistics and clock (FusedBackend.ssp_arm)
     _local = 0                   # local SGD (csrc/fused_local.cu): H, the averaging period; 0 = off
+    _gossip = False              # gossip SGD (csrc/fused_gossip.cu), see attach_optimizer
+    _gs_stats = None             # its statistics (FusedBackend.gossip_arm)
     _table = None                # device-resident training set (images, labels), see arm_train_data
     _runner = None               # native step runner (csrc/step_runner.cu), see _make_runner
     _stamp = False               # cdf telemetry stamps in the step
@@ -415,6 +417,17 @@ class _CudaEngine(ComputeEngine):
             if getattr(self, "_ls_stats", None) is None:
                 self._ls_stats = torch.zeros(int(self.lib.dm_local_stats_bytes()), dtype=torch.uint8, device=self.device)
             self._ls_stats.zero_()
+        # gossip SGD (csrc/fused_gossip.cu): every iteration writes its half step into this replica's send buffer, takes the
+        # barrier with its two ring neighbours and mixes the neighbourhood's half steps into its own arena; the run ends with
+        # one local-SGD average of every arena (gossip_finish)
+        self._gossip = getattr(opt, "mode", "") == "gossip"
+        if self._gossip:
+            if getattr(opt, "drop_connect_probability", None) is not None:
+                raise ValueError("--drop_connect cannot be combined with --gossip_method")
+            if self._gs_stats is None:
+                self._gs_stats = self.backend.gossip_arm(self.spec.arena_numel)
+                self._ls_stats = torch.zeros(int(self.lib.dm_local_stats_bytes()), dtype=torch.uint8, device=self.device)
+            self._gs_stats.zero_()
         # Bucketed aggregation (csrc/fused_sync.cu): full participation on 2/4/8 replicas.  fc1's weight gradient (96.5 % of
         # the bytes) is exchanged by small co-resident CTAs NEXT TO conv2 dgrad/wgrad + conv1 wgrad; the rest goes one-shot.
         #   DMNIST_BUCKET=2 (default): csrc/fused_bucket.cu -- fc1's gradient leaves the GEMM epilogue as bf16, is reduced in
@@ -422,7 +435,8 @@ class _CudaEngine(ComputeEngine):
         #     pass; the small bucket is pushed into every replica's inbox.  Also used on ONE replica (no exchange, the fc1
         #     update still leaves the critical path).   =1: round-1 fp32 two-shot / one-shot kernels.   =0: single kernel.
         mode = os.environ.get("DMNIST_BUCKET", "2")
-        can = int(k) == n and self.backend.drop_keep <= 0.0 and getattr(opt, "mode", "") not in ("interval", "async", "local")
+        can = int(k) == n and self.backend.drop_keep <= 0.0 and \
+            getattr(opt, "mode", "") not in ("interval", "async", "local", "gossip")
         self._bucket_v2 = can and mode == "2" and n in (1, 2, 4, 8)
         self._bucketed = can and ((mode == "1" and n in (2, 4, 8)) or self._bucket_v2)
         if self._bucket_v2 and self._g16 is None:
@@ -539,9 +553,13 @@ class _CudaEngine(ComputeEngine):
 
     def _enqueue_iteration_end(self) -> None:
         """Interval mode / K > N: gate, accumulate, close (+ commit attempt), apply.  Asynchronous SGD: ticket, apply.
-        Local SGD: the local update, then the averaging round, which only an averaging step runs."""
+        Local SGD: the local update, then the averaging round, which only an averaging step runs.  Gossip SGD: the half
+        step, the neighbours' barrier, the mix."""
         oa = self._opt_args
-        if self._local:
+        if self._gossip:
+            self.backend.enqueue_gossip_step(self.params, self.grads, self._gs_stats, oa["lr0"], oa["decay_rate"],
+                                             oa["decay_steps"])
+        elif self._local:
             self.backend.enqueue_local_step(self.params, self.grads, self._local, oa["lr0"], oa["decay_rate"],
                                             oa["decay_steps"])
             self.backend.enqueue_local_average(self.params, self._ls_stats, self._local)
@@ -605,6 +623,22 @@ class _CudaEngine(ComputeEngine):
     def local_stats(self) -> dict:
         """This replica's averaging statistics (see FusedBackend.local_stats); synchronises the device."""
         return self.backend.local_stats(self._ls_stats)
+
+    # ---- gossip SGD (csrc/fused_gossip.cu) -------------------------------------------------------------------------------
+    def gossip_finish(self) -> int:
+        """End of a gossip run, after the last step was enqueued: one average of every replica's arena (the local-SGD
+        round, unconditional, closing no step), so the weights every replica ends with are the consensus mean.  Returns the
+        global step.  Collective: every replica ends on the same iteration."""
+        self._leave_native_runner()
+        torch.cuda.synchronize()
+        self.backend.enqueue_local_average(self.params, self._ls_stats, 1, close=False)
+        torch.cuda.synchronize()
+        self.backend.check_error()
+        return self.backend.device_epoch
+
+    def gossip_stats(self) -> dict:
+        """This replica's gossip statistics (see FusedBackend.gossip_stats); synchronises the device."""
+        return self.backend.gossip_stats(self._gs_stats)
 
     def _run(self, with_sync: bool) -> None:
         s = self._slot
@@ -781,6 +815,8 @@ class _CudaEngine(ComputeEngine):
             raise ValueError("the moving average is kept for K = N and cdf mode only, not for asynchronous SGD")
         if self._local:
             raise ValueError("the moving average is kept for K = N and cdf mode only, not for local SGD")
+        if self._gossip:
+            raise ValueError("the moving average is kept for K = N and cdf mode only, not for gossip SGD")
         self._leave_native_runner()
         torch.cuda.synchronize()
         off = self.backend._off["epoch"]
@@ -1083,7 +1119,7 @@ class CudaLeNetEngine(_CudaEngine):
         # K > N: adopt + shadow refresh, and gate + accumulate + close + apply, in place of the fused sync kernel
         names = (["kgtn_begin"] + names + ["kgtn_end"]) if self._kgtn_k else \
             (["async_begin"] + names + ["async_end"]) if self._async else \
-            names + ["local_end"] if self._local else names + ["fused_sync_sgd"]
+            names + ["local_end"] if self._local else names + ["gossip_end"] if self._gossip else names + ["fused_sync_sgd"]
         tot = {n: 0.0 for n in names}
         B, s = self.batch_size, self._slot
         img, lbl = self.images[s], self.labels[s]
@@ -1110,6 +1146,8 @@ class CudaLeNetEngine(_CudaEngine):
                 yield "async_end", lambda: self._enqueue_iteration_end()
             elif self._local:
                 yield "local_end", lambda: self._enqueue_iteration_end()
+            elif self._gossip:
+                yield "gossip_end", lambda: self._enqueue_iteration_end()
             elif self._kgtn_k:
                 oa = self._opt_args
                 yield "kgtn_end", lambda: self.backend.enqueue_kgtn_end(self.params, self.grads, self._acc, self._kgtn_k, oa["lr0"],
@@ -1137,7 +1175,8 @@ class CudaLeNetEngine(_CudaEngine):
 
     def _launch_step(self, slot: int, with_sync: bool) -> None:
         n = 0
-        interval = with_sync and (getattr(self, "_interval", False) or self._async or bool(self._local))   # own iteration end
+        own = bool(self._local) or self._gossip          # local / gossip SGD: an iteration end without an iteration begin
+        interval = with_sync and (getattr(self, "_interval", False) or self._async or own)   # own iteration end
         bucketed = with_sync and self._bucketed and not interval
         self._delay_in_chain = False
         if self._stamp:
@@ -1152,7 +1191,7 @@ class CudaLeNetEngine(_CudaEngine):
         if self._aug is not None:
             images = self._launch_augment(slot)     # conv1_fwd and conv1_wgrad read the augmented batch
             n += 1
-        if interval and not self._local:
+        if interval and not own:
             self._enqueue_iteration_begin()
             n += 3 if self._ssp >= 0 else 2       # the staleness bound's wait before the pull
         n += self._launch_zero()
@@ -1174,7 +1213,8 @@ class CudaLeNetEngine(_CudaEngine):
                 n += 1
             if interval:
                 self._enqueue_iteration_end()
-                n += 5 if self._local else (2 + (self._ssp >= 0)) if self._async else 4     # local SGD: the update, the round's four
+                # local SGD: the update, the round's four; gossip SGD: the half step, the barrier, the mix
+                n += 5 if self._local else 3 if self._gossip else (2 + (self._ssp >= 0)) if self._async else 4
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1
@@ -1747,8 +1787,9 @@ class CudaMlpEngine(_CudaEngine):
         if self._aug is not None:
             images = self._launch_augment(slot)     # dm_f32_to_bf16 reads the augmented batch
             n += 1
-        interval = with_sync and (getattr(self, "_interval", False) or self._async or bool(self._local))   # own iteration end
-        if interval and not self._local:
+        own = bool(self._local) or self._gossip          # local / gossip SGD: an iteration end without an iteration begin
+        interval = with_sync and (getattr(self, "_interval", False) or self._async or own)   # own iteration end
+        if interval and not own:
             self._enqueue_iteration_begin()
             n += 3 if self._ssp >= 0 else 2       # the staleness bound's wait before the pull
         bucketed = with_sync and self._bucket_v2 and not interval
@@ -1770,7 +1811,8 @@ class CudaMlpEngine(_CudaEngine):
                 n += 1
             if interval:
                 self._enqueue_iteration_end()
-                n += 5 if self._local else (2 + (self._ssp >= 0)) if self._async else 4     # local SGD: the update, the round's four
+                # local SGD: the update, the round's four; gossip SGD: the half step, the barrier, the mix
+                n += 5 if self._local else 3 if self._gossip else (2 + (self._ssp >= 0)) if self._async else 4
             else:
                 self.backend.enqueue(self.params, self.grads, **self._opt_args)
                 n += 1

@@ -207,6 +207,10 @@ def define_reference_flags(F: FlagValues = FLAGS) -> FlagValues:
                                            "gradients to its own weights, and every H-th global step the replicas' "
                                            "weights are replaced by their mean (H = this value; 0 = off); reports the "
                                            "averaging rounds and their barrier waits (workerN_local_sgd.json)")
+    F.DEFINE_boolean("gossip_method", False, "Gossip (decentralized) SGD on a ring: every step each replica averages its "
+                                             "half step w - lr * g with those of its two ring neighbours, waiting for "
+                                             "those two only; the run ends with one average of every replica; reports "
+                                             "the barrier waits (workerN_gossip.json)")
     F.DEFINE_boolean("should_summarize", False, "Whether the chief should write summaries")
     F.DEFINE_boolean("timeline_logging", False, "Dump a chrome-trace timeline json per step")
     # reference: src/distributed_train.py:40-48

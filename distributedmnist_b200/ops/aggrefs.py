@@ -221,3 +221,22 @@ def local_average(ws: Sequence) -> np.ndarray:
         s = np.zeros_like(w) if s is None else s
         s = ftz(s + w)
     return ftz(s / np.float32(len(ws)))
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# gossip SGD (csrc/fused_gossip.cu)
+# ---------------------------------------------------------------------------------------------------------------------
+def ring_neighbours(i: int, n: int) -> list:
+    """N(i) = {i - 1, i, i + 1} mod n in increasing rank order: every rank for n <= 3."""
+    return sorted({(i - 1) % n, i % n, (i + 1) % n})
+
+
+def gossip_mix(hs: Sequence, i: int) -> np.ndarray:
+    """gs_mix_kernel of replica ``i``: ``fl(S / m)``, S the fp32 sum of the half steps ``hs[q]`` over q in N(i) from +0.0
+    in increasing rank order, m = |N(i)|, the division correctly rounded (``__fdiv_rn``), every operand and result
+    flushed to zero as the FTZ kernels do.  For len(hs) <= 3 this is :func:`local_average` of every copy."""
+    nb = ring_neighbours(i, len(hs))
+    s = np.zeros_like(f32(hs[nb[0]]))
+    for q in nb:
+        s = ftz(s + ftz(f32(hs[q])))
+    return ftz(s / np.float32(len(nb)))

@@ -96,6 +96,10 @@ def _signatures() -> dict:
         "dm_ssp_stats_bytes": (V, i, []),
         "dm_ssp_wait": (S, i, [P, P, P, i, i, u, d, P]),
         "dm_ssp_publish": (S, i, [PP, P, i, i, i, P]),
+        # fused_gossip.cu
+        "dm_gossip_stats_bytes": (V, i, []),
+        "dm_gossip_apply": (S, i, [PP, i, P, P, P, ll, d, d, i, i, P]),
+        "dm_gossip_exchange": (S, i, [PP, PP, P, P, P, i, i, ll, d, i, P]),
         # fused_local.cu
         "dm_local_stats_bytes": (V, i, []),
         "dm_local_apply": (S, i, [PP, i, P, P, P, ll, u, d, d, i, i, P, P]),

@@ -106,9 +106,9 @@ def ctrl_words(raw, off: Dict[str, int], stamp_step: Optional[int] = None) -> Di
 def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
     """How ``eng`` applies its gradients: ``mode`` "fused" (fused_sync_sgd), "bucket" (the bf16-wire bucketed kernels),
     "kgtn" (K > N: every k-th iteration commits), "interval" (a tick commits when its deadline has passed; ``interval_ns``
-    the armed period), "async" (asynchronous SGD on one replica: every step pulls the master copy and adds its update) or
-    "local" (local SGD on one replica: every step applies its own update, every ``period``-th global step is averaged),
-    the schedule and the global step of the first step.  ``drop``:
+    the armed period), "async" (asynchronous SGD on one replica: every step pulls the master copy and adds its update),
+    "local" (local SGD on one replica: every step applies its own update, every ``period``-th global step is averaged) or
+    "gossip" (gossip SGD on one replica: every step mixes its own half step, a neighbourhood of one), the schedule and the global step of the first step.  ``drop``:
     (seed, keep probability) of the drop-connect mask the fused kernel applies, None without it.  With a cut table armed
     (``arm_lr_cuts``), ``sched`` must name the same cuts (raises ValueError otherwise): the step sizes are then those of
     the schedule with the cuts (synchronises the device to read the table).  ``aug``: (ranges, seed mix) of the armed
@@ -121,6 +121,8 @@ def update_of(eng, sched, step0: int, aug_start: int = 0) -> dict:
         mode = "async"
     elif getattr(eng, "_local", 0):
         mode = "local"
+    elif getattr(eng, "_gossip", False):
+        mode = "gossip"
     elif eng._kgtn_k:
         mode = "kgtn"
     elif getattr(eng, "_interval", False):
@@ -239,6 +241,8 @@ def update_results(tag: str, init: dict, records: Sequence[dict], upd: dict) -> 
             want = A.sgd(w, g, scale)
             if (epochs[t] + 1) % upd["period"] == 0:
                 want = A.local_average([want])
+        elif mode == "gossip":
+            want = A.gossip_mix([A.sgd(w, g, scale)], 0)
         elif mode == "bucket":
             want = A.bucket_step(w, [g], [A.f32(r["g16"].float()).reshape(-1)], upd["early"], scale, upd["late_bf16"])
         else:

@@ -29,6 +29,7 @@ from typing import Callable, Dict, List, Optional, Sequence
 import numpy as np
 import torch
 
+from ..ops.aggrefs import ring_neighbours
 from .backends import Backend, StepInfo
 from .straggler import delay_limit_ns, parametric_table, profile_table, sample_ns, seed_mix
 
@@ -322,6 +323,73 @@ class LocalSGDOptimizer(_AggregatorBase):
 
     def report(self) -> Dict:
         return local_sgd_report(self.period, self.rounds, self.wait_total_ns, self.wait_max_ns)
+
+
+def gossip_report(replicas: int, iterations: int, waits: int, wait_total_ns: int, wait_max_ns: int) -> Dict:
+    """The ring of one replica (N replicas, m = min(N, 3) in each neighbourhood), the iterations it made, the barriers in
+    which it found a neighbour not yet arrived, and the time it spent in its barriers."""
+    return dict(replicas=int(replicas), neighbourhood=min(int(replicas), 3), iterations=int(iterations),
+                waits=int(waits), wait_total_s=int(wait_total_ns) * 1e-9, wait_max_s=int(wait_max_ns) * 1e-9,
+                wait_mean_s=int(wait_total_ns) * 1e-9 / iterations if iterations else 0.0)
+
+
+class GossipSGDOptimizer(_AggregatorBase):
+    """Gossip (decentralized) SGD on a ring, adapt-then-combine: every step each replica forms the half step
+    ``h = w - lr(s) * g`` on its own weights and replaces its weights with the mean of the half steps of its
+    neighbourhood {i - 1, i, i + 1} mod N (every replica for N <= 3).  The GPU path runs it on the device
+    (csrc/fused_gossip.cu, see ``FusedBackend.enqueue_gossip_step``), where a replica waits for its two neighbours only;
+    here, for the torch engine, the mix is an ``all_gather`` of the half steps followed by the same rank-order fp32 sum
+    and division, so gloo runs are a real multi-replica reference."""
+    mode = "gossip"
+
+    def __init__(self, backend: Backend, lr_schedule, total_num_replicas: int, straggler=None, seed: int = 0):
+        super().__init__(backend, lr_schedule, total_num_replicas, straggler, seed)
+        self.iterations = self.waits = 0
+        self.wait_total_ns = self.wait_max_ns = 0
+        self.half_step: Optional[torch.Tensor] = None     # this replica's newest half step
+
+    def apply_gradients(self, params: torch.Tensor, grads: torch.Tensor) -> StepInfo:
+        delay = self._delay_s()
+        if delay > 0:
+            time.sleep(delay)
+        self.half_step = params.add(grads, alpha=-float(self.lr_schedule(self.local_step)))
+        self.mix(params, self.half_step)
+        return self._account(StepInfo(self.local_step + 1, True, 1 << self.backend.ctx.rank, 1))
+
+    def mix(self, params: torch.Tensor, h: torch.Tensor) -> None:
+        """``params`` := the mean of the neighbourhood's half steps (collective).  The time spent in the collective is
+        this path's barrier wait."""
+        n, rank = self.backend.ctx.world_size, self.backend.ctx.rank
+        hs = [h]
+        if n > 1:
+            t0 = time.perf_counter_ns()
+            hs = [torch.empty_like(h) for _ in range(n)]
+            torch.distributed.all_gather(hs, h.contiguous())
+            ns = time.perf_counter_ns() - t0
+            self.wait_total_ns += ns
+            self.wait_max_ns = max(self.wait_max_ns, ns)
+        nb = ring_neighbours(rank, n)
+        s = torch.zeros_like(h)
+        for q in nb:
+            s.add_(hs[q])
+        params.copy_(s.div_(len(nb)))
+        self.iterations += 1
+
+    def average(self, params: torch.Tensor) -> None:
+        """The end of a run: every replica's ``params`` := the mean of all of them, summed in rank order from +0.0 as
+        the device's final local-SGD round sums them (collective)."""
+        n = self.backend.ctx.world_size
+        if n > 1:
+            ws = [torch.empty_like(params) for _ in range(n)]
+            torch.distributed.all_gather(ws, params.detach().contiguous())
+            s = torch.zeros_like(params)
+            for w in ws:
+                s.add_(w)
+            params.copy_(s.div_(n))
+
+    def report(self) -> Dict:
+        return gossip_report(self.backend.ctx.world_size, self.iterations, self.waits, self.wait_total_ns,
+                             self.wait_max_ns)
 
 
 class TimeoutReplicasOptimizer(_AggregatorBase):

@@ -82,6 +82,7 @@ class FusedBackend(Backend):
         self.interval_ns: Optional[int] = None     # the interval clock's period, once armed (interval_arm)
         self.lr_schedule_armed = False             # the control block evaluates a warmup / cosine (set_lr_schedule)
         self._ssp_board: Optional[SymmetricBuffer] = None   # stale synchronous parallel: this replica's clock board
+        self._gossip_send: Optional[SymmetricBuffer] = None  # gossip SGD: this replica's two send buffers
 
     # ---- memory ---------------------------------------------------------------------------
     def allocate(self, numel: int) -> torch.Tensor:
@@ -431,6 +432,38 @@ class FusedBackend(Backend):
         raw = stats.cpu().numpy()
         return dict(rounds=int(raw[0:4].view("<u4")[0]), wait_total_ns=int(raw[8:16].view("<u8")[0]),
                     wait_max_ns=int(raw[16:24].view("<u8")[0]))
+
+    # ---- gossip SGD (csrc/fused_gossip.cu) ---------------------------------------------------------------------------------
+    def gossip_arm(self, numel: int) -> torch.Tensor:
+        """This replica's two send buffers of ``numel`` fp32 each (one symmetric allocation, on first use -- collective,
+        like :meth:`allocate`) and a new, zeroed statistics block (``dm_gossip_stats_bytes()`` bytes), returned."""
+        if self._gossip_send is None:
+            self._gossip_send = self.allocate_buffer(2 * 4 * int(numel))
+        return torch.zeros(int(self.lib.dm_gossip_stats_bytes()), dtype=torch.uint8, device=self.ctx.device)
+
+    def enqueue_gossip_step(self, params: torch.Tensor, grads: torch.Tensor, stats: torch.Tensor, lr0: float,
+                            decay_rate: float = 1.0, decay_steps: int = 1,
+                            stream: Optional[torch.cuda.Stream] = None) -> None:
+        """One gossip iteration after the gradient (after :meth:`gossip_arm`): the half step ``params - fp32(lr(s)) *
+        grads`` into this replica's send buffer s % 2, s = its global step, with the armed schedule; the step is closed
+        and the barrier with the two ring neighbours taken; then ``params`` and the shadow := the mean of the half steps
+        of the neighbourhood, summed in rank order over the peer path."""
+        self.lib.dm_gossip_apply(self.ctrl.ptr_table(), self.ctx.rank, params, grads, self._gossip_send.local_ptr,
+                                 params.numel(), lr0, decay_rate, int(decay_steps), int(self.ctas), stream_ptr(stream))
+        self.lib.dm_gossip_exchange(self.ctrl.ptr_table(), self._gossip_send.ptr_table(), params, self.shadow, stats,
+                                    self.ctx.rank, self.ctx.world_size, params.numel(), self.timeout_ms, int(self.ctas),
+                                    stream_ptr(stream))
+
+    @staticmethod
+    def gossip_stats(stats: torch.Tensor) -> Dict:
+        """Decode the gossip statistics (synchronises the device): ``iterations``, ``waits`` (barriers at whose first
+        poll a neighbour had not arrived), ``wait_total_ns``, ``wait_max_ns`` (%globaltimer time in the barriers) and
+        ``t_pass``, the ring of the %globaltimer stamps at which the barrier of iteration s was passed, at s % 1024."""
+        torch.cuda.synchronize()
+        raw = stats.cpu().numpy()
+        return dict(iterations=int(raw[0:4].view("<u4")[0]), waits=int(raw[4:8].view("<u4")[0]),
+                    wait_total_ns=int(raw[8:16].view("<u8")[0]), wait_max_ns=int(raw[16:24].view("<u8")[0]),
+                    t_pass=raw[32:].view("<u8").copy())
 
     @property
     def nvls_active(self) -> bool:

@@ -1315,3 +1315,155 @@ def run_random(make_model, seeds) -> int:
         rng = random.Random(seed)
         make_model().run(lambda runnable: runnable[rng.randrange(len(runnable))])
     return len(seeds)
+
+
+# ----------------------------------------------------------------------------------------------------------------------
+# Gossip SGD -- word-level model of gs_apply / gs_barrier / gs_mix (csrc/fused_gossip.cu), stop_publish and the pipelined
+# host loop's stop rule
+# ----------------------------------------------------------------------------------------------------------------------
+class GossipModel:
+    """N replicas of gossip SGD on a ring, each a host loop and a device stream, as generators for
+    :func:`explore_schedules` (actors 0..N-1 the hosts, N..2N-1 the devices).
+
+    Memory: ``send[i][p]`` the iteration whose half step replica i's send buffer p holds, ``bar[i][p]`` (sequence, knows)
+    the barrier word peer p released into i's block, ``stop`` the stop step once the chief's pass set it.  ``knows[i]``:
+    replica i is ordered after the chief's stop stores (the stores themselves, or an acquire of a release that is); only
+    then is stop_publish sure to read S, and a replica that is not reads 0 -- the worst case for the stop rule, since an
+    early read only stops a host sooner.  Iteration s of device i is five atomic steps: the apply (send[i][s % 2] := s),
+    the release of s + 1 into both neighbours' blocks, the wait for both neighbours' s + 1 (the acquire), the mix (reads
+    send[q][s % 2] for q in N(i)), and stop_publish + completion; after it the chief runs the pass the host enqueued
+    after step s + 1, which sets S = s + 1 + ``margin`` once s + 1 >= ``reach``.  Host i: launch step j (the chief enqueues
+    a pass after it when j % ``every`` == 0 or j > max), wait for step j - 1, lower max to the stop word read, stop
+    launching once j > max.
+
+    Checked (``ProtocolHazard`` otherwise), G1-G4 of DESIGN.md §4: G1 every mix reads exactly the neighbourhood's half
+    steps of its own iteration; G2 at every moment two replicas at ring distance d have passed barrier counts that differ
+    by at most d; G3 no deadlock, and every replica ends on the same iteration; G4 every replica launches exactly the steps
+    of a ``--max_steps=S`` run, S = min(max_steps, stop step).  Mutants, each of which must fail: ``parities=1`` (one send
+    buffer), ``skip=True`` (the barrier does not wait for the right neighbour), ``parity_offset=1`` (the mix reads
+    send[q][(s + 1) % 2]), and a ``margin`` below :func:`train.stop_margin`'s."""
+
+    def __init__(self, n: int, max_steps: int, every: int = 1, reach: int = 1 << 30, margin: int = 2, parities: int = 2,
+                 skip: bool = False, parity_offset: int = 0, hosts: bool = True):
+        self.n, self.max_steps, self.every, self.reach, self.margin = n, max_steps, every, reach, margin
+        self.hosts = hosts
+        self.parities, self.skip, self.parity_offset = parities, skip, parity_offset
+        self.nb = [sorted({(i - 1) % n, i, (i + 1) % n}) for i in range(n)]
+        self.send = [[-1] * parities for _ in range(n)]
+        self.bar = [[(0, False)] * n for _ in range(n)]
+        self.knows = [False] * n
+        self.passed = [0] * n
+        self.launched = [0] * n
+        self.completed = [0] * n
+        self.host_word = [0] * n
+        self.host_max = [max_steps] * n
+        self.host_done = [False] * n
+        self.stop = 0
+        self.evals: List[int] = []
+        self.pc = [0] * (2 * n)
+        if not hosts:                  # every step launched up front: the devices alone, without the stop rule
+            self.launched = [max_steps + 1] * n
+            self.host_done = [True] * n
+            self.evals = [j for j in range(1, max_steps + 2) if j % every == 0 or j > max_steps]
+
+    def state(self):
+        return (tuple(map(tuple, self.send)), tuple(map(tuple, self.bar)), tuple(self.knows), tuple(self.passed),
+                tuple(self.launched), tuple(self.completed), tuple(self.host_word), tuple(self.host_max),
+                tuple(self.host_done), self.stop, tuple(self.evals), tuple(self.pc))
+
+    def dist(self, a: int, b: int) -> int:
+        d = abs(a - b)
+        return min(d, self.n - d)
+
+    def host(self, r: int):
+        j = 0
+        while True:
+            j += 1
+            self.launched[r] = j
+            if r == 0 and (j % self.every == 0 or j > self.host_max[r]):
+                self.evals.append(j)
+            self.pc[r] += 1
+            yield None
+            if j > 1:
+                self.pc[r] += 1
+                yield (lambda w=j - 1: self.completed[r] >= w)
+                if self.host_word[r]:
+                    self.host_max[r] = min(self.host_max[r], self.host_word[r])
+            if j > self.host_max[r]:
+                break
+            self.pc[r] += 1
+            yield None
+        self.pc[r] += 1
+        yield (lambda: self.completed[r] >= j)
+        self.host_done[r] = True
+
+    def _wait_set(self, i: int) -> List[int]:
+        right = (i + 1) % self.n
+        return [p for p in self.nb[i] if not (self.skip and p == right and p != i)]
+
+    def device(self, i: int):
+        a, s = self.n + i, 0
+        while True:
+            self.pc[a] += 1
+            yield (lambda: self.launched[i] > s or self.host_done[i])
+            if self.launched[i] <= s:
+                return
+            self.send[i][s % self.parities] = s                          # gs_apply (ends with its system fence)
+            self.pc[a] += 1
+            yield None
+            for p in self.nb[i]:                                         # gs_barrier: the releases
+                self.bar[p][i] = (s + 1, self.knows[i])
+            self.pc[a] += 1
+            yield None
+            self.pc[a] += 1
+            yield (lambda: all(self.bar[i][p][0] >= s + 1 for p in self._wait_set(i)))
+            self.knows[i] = self.knows[i] or any(self.bar[i][p][1] for p in self._wait_set(i))   # the acquire
+            self.passed[i] = s + 1
+            for q in range(self.n):
+                if self.passed[q] - self.passed[i] > self.dist(q, i) or self.passed[i] - self.passed[q] > self.dist(q, i):
+                    raise ProtocolHazard("G2: replicas %d and %d at ring distance %d have passed %d and %d barriers"
+                                         % (i, q, self.dist(q, i), self.passed[i], self.passed[q]))
+            self.pc[a] += 1
+            yield None
+            par = (s + self.parity_offset) % self.parities                # gs_mix
+            for q in self.nb[i]:
+                if self.send[q][par] != s:
+                    raise ProtocolHazard("G1: replica %d's mix of iteration %d read replica %d's half step of iteration %d"
+                                         % (i, s, q, self.send[q][par]))
+            self.pc[a] += 1
+            yield None
+            self.host_word[i] = self.stop if self.knows[i] else 0        # stop_publish, the step's last node
+            self.completed[i] = s + 1
+            s += 1
+            if i == 0:
+                # the pass after step s (if any) is known once step s + 1 is launched or the host has finished
+                self.pc[a] += 1
+                yield (lambda: self.launched[0] > s or self.host_done[0])
+                if s in self.evals and s >= self.reach and not self.stop:
+                    self.stop = s + self.margin                           # eval_target's stores and fence
+                    self.knows[0] = True
+
+    def run(self, choose) -> None:
+        n = self.n
+        gens = {a: (self.host(a) if a < n else self.device(a - n)) for a in range(0 if self.hosts else n, 2 * n)}
+        waiting = {}
+        for a in list(gens):
+            BucketV2Model._advance(a, gens, waiting)
+        while gens:
+            runnable = [a for a in sorted(gens) if a not in waiting or waiting[a]()]
+            if not runnable:
+                raise ProtocolHazard("G3: deadlock, %s wait forever (launched %s, passed %s)"
+                                     % (sorted(gens), self.launched, self.passed))
+            a = choose(runnable)
+            waiting.pop(a, None)
+            BucketV2Model._advance(a, gens, waiting)
+        first = next((j for j in range(1, self.max_steps + 2) if j >= self.reach and
+                      (j % self.every == 0 or j > self.max_steps)), None)
+        s = min(self.max_steps, first + self.margin) if first is not None else self.max_steps
+        if self.launched != [s + 1] * n or self.completed != [s + 1] * n:
+            raise ProtocolHazard("G3/G4: replicas launched %s and completed %s steps, a run with --max_steps=%d launches "
+                                 "%d" % (self.launched, self.completed, s, s + 1))
+        want = [j for j in range(1, s + 2) if j % self.every == 0 or j > s]
+        if self.evals != want:
+            raise ProtocolHazard("G4: the chief enqueued passes after steps %s, a run with --max_steps=%d after %s"
+                                 % (self.evals, s, want))

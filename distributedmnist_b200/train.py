@@ -38,8 +38,9 @@ from .early_stopping import EARLY_STOPPING_JSON
 from .engine import make_engine
 from .lr_plateau import LR_PLATEAU_JSON
 from .flags import FLAGS
-from .parallel.aggregators import (AsyncSGDOptimizer, LocalSGDOptimizer, SyncReplicasOptimizer, TimeoutReplicasOptimizer,
-                                   local_sgd_report, parse_straggler_spec, ssp_report, staleness_report)
+from .parallel.aggregators import (AsyncSGDOptimizer, GossipSGDOptimizer, LocalSGDOptimizer, SyncReplicasOptimizer,
+                                   TimeoutReplicasOptimizer, gossip_report, local_sgd_report, parse_straggler_spec,
+                                   ssp_report, staleness_report)
 from .parallel.backends import make_backend
 from .parallel.context import ReplicaContext
 from .parallel.timeout_manager import launch_manager
@@ -53,6 +54,7 @@ log = get_logger()
 STALENESS_JSON = "worker%d_staleness.json"
 SSP_JSON = "worker%d_ssp.json"
 LOCAL_SGD_JSON = "worker%d_local_sgd.json"
+GOSSIP_JSON = "worker%d_gossip.json"
 
 LOG_FORMAT = ("Worker %d: %s: step %d, loss = %f, train_acc = %f, test_acc = %f"
               "(%.1f examples/sec; %.3f  sec/batch)")
@@ -357,9 +359,43 @@ def check_local_sgd_flags(flags, ctx: ReplicaContext) -> None:
                          "evaluation scores the averaged model, which exists only after an averaging step" % (every, h))
 
 
-def stop_margin(flags) -> int:
-    """S - g: the stop step S of an evaluation pass of global step g that stops the run.  STOP_MARGIN steps, or
-    STOP_MARGIN averaging periods with local SGD (DESIGN §4.4)."""
+def check_gossip_flags(flags, ctx: ReplicaContext) -> None:
+    """``--gossip_method`` combinations that cannot work, rejected before any device work starts."""
+    if not getattr(flags, "gossip_method", False):
+        return
+    if flags.interval_method:
+        raise ValueError("--gossip_method cannot be combined with --interval_method: both are aggregation modes, and "
+                         "gossip SGD mixes every replica's weights with its neighbours' instead of a tick's gradients")
+    if getattr(flags, "worker_times_cdf_method", False):
+        raise ValueError("--gossip_method cannot be combined with --worker_times_cdf_method: the cdf mode times a full "
+                         "barrier on every step, and gossip SGD waits for the ring neighbours only")
+    if getattr(flags, "async_method", False):
+        raise ValueError("--gossip_method cannot be combined with --async_method (or --ssp_staleness): asynchronous SGD "
+                         "shares one set of weights, and gossip SGD keeps one per replica")
+    if int(getattr(flags, "local_sgd_steps", 0) or 0):
+        raise ValueError("--gossip_method cannot be combined with --local_sgd_steps: gossip with local steps between "
+                         "exchanges is not implemented")
+    k = flags.num_replicas_to_aggregate
+    if k != -1 and k != ctx.world_size:
+        raise ValueError("--gossip_method applies every replica's own gradient, so --num_replicas_to_aggregate must be "
+                         "left unset or equal the number of replicas (%d), got %d" % (ctx.world_size, k))
+    if flags.drop_connect:
+        raise ValueError("--gossip_method cannot be combined with --drop_connect: the gradient mask is implemented in "
+                         "the synchronous aggregation kernels only")
+    if float(getattr(flags, "moving_average_decay", 0.0) or 0.0):
+        raise ValueError("--gossip_method cannot be combined with --moving_average_decay: the replicas are not in lock "
+                         "step, and the chief's weights are its own, not the model's")
+    if int(getattr(flags, "lr_plateau_patience", 0) or 0):
+        raise ValueError("--gossip_method cannot be combined with --lr_plateau_patience: a cut must take effect on the "
+                         "same global step on every replica, and gossip replicas are not in lock step")
+
+
+def stop_margin(flags, replicas: int = 1) -> int:
+    """S - g: the stop step S of an evaluation pass of global step g that stops the run.  STOP_MARGIN steps,
+    STOP_MARGIN averaging periods with local SGD, or max(STOP_MARGIN, floor(N / 2)) steps with gossip SGD on a ring of N
+    ``replicas`` (DESIGN §4.4)."""
+    if getattr(flags, "gossip_method", False):
+        return max(STOP_MARGIN, int(replicas) // 2)
     return STOP_MARGIN * max(1, int(getattr(flags, "local_sgd_steps", 0) or 0))
 
 
@@ -758,6 +794,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     is_chief = ctx.is_chief
     check_async_flags(flags, ctx)
     check_local_sgd_flags(flags, ctx)
+    check_gossip_flags(flags, ctx)
     check_batch_flags(flags, ctx)
     check_eval_flags(flags, ctx, num_replicas_to_aggregate, dataset_test)
     check_target_flags(flags, ctx)
@@ -788,13 +825,16 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
 
     async_mode = bool(getattr(flags, "async_method", False))
     local_h = int(getattr(flags, "local_sgd_steps", 0) or 0)
-    margin = stop_margin(flags)
+    gossip = bool(getattr(flags, "gossip_method", False))
+    margin = stop_margin(flags, num_workers)
     if async_mode:
         opt = AsyncSGDOptimizer(backend, lr_schedule, total_num_replicas=num_workers, straggler=straggler, seed=flags.seed,
                                 ssp_staleness=int(getattr(flags, "ssp_staleness", -1)))
     elif local_h:
         opt = LocalSGDOptimizer(backend, lr_schedule, total_num_replicas=num_workers, period=local_h, straggler=straggler,
                                 seed=flags.seed)
+    elif gossip:
+        opt = GossipSGDOptimizer(backend, lr_schedule, total_num_replicas=num_workers, straggler=straggler, seed=flags.seed)
     elif flags.interval_method or flags.worker_times_cdf_method:
         # reference :179-183 -- interval wins when both are set, as there.
         mode = "interval" if flags.interval_method else "cdf"
@@ -879,9 +919,10 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
     eval_every = int(getattr(flags, "eval_every_steps", 0) or 0) if is_chief else 0
     device_eval = bool(eval_every and fused_step)
     # local SGD is in lock step too: every replica makes one iteration per global step, and no peer writes the chief's
-    # arena outside the averaging rounds the chief takes part in
+    # arena outside the averaging rounds the chief takes part in.  Gossip SGD: no peer ever writes the chief's arena, and
+    # its epoch word counts the chief's own iterations
     exact = isinstance(opt, SyncReplicasOptimizer) and num_replicas_to_aggregate == num_workers \
-        or bool(flags.worker_times_cdf_method and not flags.interval_method) or bool(local_h)
+        or bool(flags.worker_times_cdf_method and not flags.interval_method) or bool(local_h) or gossip
     # K < N / interval: peers push into the chief's arena at any time -> score a validated snapshot (--eval_snapshot);
     # the host cannot name the step a pass scores in advance, so passes follow the consumed global step (eval_due)
     snapshot_eval = device_eval and bool(getattr(flags, "eval_snapshot", False)) and not exact and not async_mode
@@ -1088,7 +1129,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             return
         if global_step == last_eval_step or not (global_step % eval_every == 0 or global_step > max_steps):
             return
-        if local_h and global_step > max_steps and not local_done:
+        if (local_h or gossip) and global_step > max_steps and not local_done:
             return                 # the final pass follows the run's final average
         last_eval_step = global_step
         if device_eval:
@@ -1152,7 +1193,7 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
             launched += 1
             if device_eval and not follow_eval and \
                     ((restored_step + launched) % eval_every == 0 or restored_step + launched > max_steps) and \
-                    not (local_h and restored_step + launched > max_steps):
+                    not ((local_h or gossip) and restored_step + launched > max_steps):
                 engine.enqueue_eval()          # K == N: restored_step + launched is the global step of the weights it scores
             prev, pending = pending, token
             if prev is not None:
@@ -1252,7 +1293,21 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         # every replica's last update applied, the device barrier, one more pull: the chief's arena, the final pass and
         # the final checkpoint hold every update of the run, and their global step is the number of updates
         step = engine.async_finish()
-    local_done = True              # local SGD: eval_after_step may score the step past --max_steps from here on
+    local_done = True              # local / gossip SGD: eval_after_step may score the step past --max_steps from here on
+    if gossip:
+        # one average of every replica's weights, so the final pass, the final checkpoint and the returned weights are
+        # the consensus mean (collective: every replica ends on the same iteration)
+        if fused_step:
+            step = engine.gossip_finish()
+        else:
+            opt.average(engine.params)
+            if hasattr(engine, "params_updated"):
+                engine.params_updated()
+        if eval_every:
+            if device_eval:
+                engine.enqueue_eval()
+            else:
+                eval_after_step(step)
     if local_h:
         # the last step was not an averaging step: one more average, so the final pass, the final checkpoint and the
         # returned weights are the model every replica holds (collective: every replica ends on the same step)
@@ -1387,6 +1442,18 @@ def train(ctx: ReplicaContext, dataset, dataset_test=None, flags=FLAGS) -> Dict:
         log.info("Local SGD: worker %d averaged every %d step(s); %d averaging round(s), %.6f s in their barriers "
                  "(mean %.6f s, max %.6f s); final global step %d"
                  % (ctx.rank, local_h, rep["rounds"], rep["wait_total_s"], rep["wait_mean_s"], rep["wait_max_s"], step))
+    if gossip:
+        st = engine.gossip_stats() if fused_step else None
+        rep = gossip_report(num_workers, st["iterations"], st["waits"], st["wait_total_ns"], st["wait_max_ns"]) \
+            if st is not None else opt.report()
+        results["gossip"] = rep
+        with open(os.path.join(flags.train_dir, GOSSIP_JSON % ctx.rank), "w") as f:
+            json.dump(rep, f, indent=1)
+            f.write("\n")
+        log.info("Gossip SGD: worker %d mixed with %d replica(s) of a ring of %d; %d iteration(s), %d of whose barriers "
+                 "waited for a neighbour, %.6f s in them (mean %.6f s, max %.6f s); final global step %d"
+                 % (ctx.rank, rep["neighbourhood"], rep["replicas"], rep["iterations"], rep["waits"],
+                    rep["wait_total_s"], rep["wait_mean_s"], rep["wait_max_s"], step))
     results.update(final_step=step, accepted=opt.accepted_steps, dropped=opt.dropped_steps,
                    params=engine.params, elapsed=time.time() - begin_time,
                    timeout_server=timeout_server, engine=engine, optimizer=opt)
