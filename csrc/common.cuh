@@ -272,6 +272,37 @@ DMNIST_DEVICE float4 ordered_sum4(const float4* p, int n, size_t stride) {
   return s;
 }
 
+// out[4q .. 4q + 3] += columns 4q .. 4q + 3 of sum_{k < n} slots[k][0..63], each column added in slot order from zero.
+// The NT threads of the CTA copy 4 NT slots' float4 at a time into s_buf, all loads in flight together (one L2 round
+// trip per 4 NT slots), and thread 0 adds them.
+template <int NT>
+DMNIST_DEVICE void add_ordered_slot_sum64(const float* slots, int n, int q, float* out, float4 (&s_buf)[4 * NT]) {
+  float4 s = make_float4(0.f, 0.f, 0.f, 0.f);
+  const float4* src = reinterpret_cast<const float4*>(slots) + q;
+  for (int k0 = 0; k0 < n; k0 += 4 * NT) {
+    float4 v[4];
+#pragma unroll
+    for (int u = 0; u < 4; ++u) {
+      const int k = k0 + u * NT + (int)threadIdx.x;
+      if (k < n) v[u] = __ldcg(src + (size_t)k * 16);
+    }
+#pragma unroll
+    for (int u = 0; u < 4; ++u)
+      if (k0 + u * NT + (int)threadIdx.x < n) s_buf[u * NT + threadIdx.x] = v[u];
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      const int m = min(4 * NT, n - k0);
+      for (int k = 0; k < m; ++k) { s.x += s_buf[k].x; s.y += s_buf[k].y; s.z += s_buf[k].z; s.w += s_buf[k].w; }
+    }
+    __syncthreads();
+  }
+  if (threadIdx.x == 0) {
+    float4* o = reinterpret_cast<float4*>(out) + q;
+    const float4 cur = *o;
+    *o = make_float4(cur.x + s.x, cur.y + s.y, cur.z + s.z, cur.w + s.w);
+  }
+}
+
 // ---------------------------------------------------------------------------------
 // wgmma shared-memory matrix descriptors
 // ---------------------------------------------------------------------------------

@@ -529,13 +529,24 @@ conv2_wgrad_kernel(const __grid_constant__ CUtensorMap tmX,    // a1, box (32,18
 // g_w += the sum of the partials over the image slices, in slice order.  Thread = 4 output channels of one (tap, ci):
 // 25 x 32 x 16 = 12800 threads, so the 4 MB of partials are read by the whole machine at once.  Chained to
 // conv2_wgrad_kernel by programmatic dependent launch: its launch overlaps the weight-gradient kernel's last CTAs.
+// With bias_part, 16 more CTAs add the conv2 bias gradient: g_bias += the sum of dm_fc1_dgrad_unpool_slots' n_bias
+// slots in slot order, CTA q channels 4q .. 4q + 3.  In the training step that sum then sits on this side branch, not
+// at the end of the data-gradient GEMM.
 constexpr int WGR_THREADS = 64;
 constexpr int WGR_ITEMS = 25 * 32 * 64 / 4;
+constexpr int WGR_CTAS = WGR_ITEMS / WGR_THREADS;
+constexpr int WGR_BIAS_CTAS = 16;
+static_assert(WGR_ITEMS % WGR_THREADS == 0, "every thread of the weight CTAs owns an item");
 __global__ void __launch_bounds__(WGR_THREADS)
-conv2_wgrad_reduce_kernel(float* __restrict__ g_w, int splits) {
+conv2_wgrad_reduce_kernel(float* __restrict__ g_w, int splits, const float* __restrict__ bias_part, int n_bias,
+                          float* __restrict__ g_bias) {
+  __shared__ float4 s_buf[4 * WGR_THREADS];
   pdl_wait();
+  if (blockIdx.x >= WGR_CTAS) {
+    add_ordered_slot_sum64<WGR_THREADS>(bias_part, n_bias, blockIdx.x - WGR_CTAS, g_bias, s_buf);
+    return;
+  }
   const int e4 = blockIdx.x * WGR_THREADS + threadIdx.x;
-  if (e4 >= WGR_ITEMS) return;
   const int tap = e4 >> 9, row4 = e4 & 511;        // row4 = ci * 16 + co / 4
   const int kh = tap / 5, kw = tap % 5;
   const int group = kh < 4 ? kw : (kw < 4 ? 5 : 6);
@@ -545,6 +556,29 @@ conv2_wgrad_reduce_kernel(float* __restrict__ g_w, int splits) {
   float4* o = reinterpret_cast<float4*>(g_w) + e4;
   const float4 cur = *o;
   *o = make_float4(cur.x + sum.x, cur.y + sum.y, cur.z + sum.z, cur.w + sum.w);
+}
+
+int launch_conv2_wgrad(const void* a1, const void* dy, void* g_w, const void* bias_part, int n_bias, void* g_bias,
+                       int B, void* stream) {
+  CUtensorMap tmX, tmDY;
+  if (make_tmap_nhwc_bf16(&tmX, a1, 32, 14, 14, B, 32, 18, 18, 64)) return 101;
+  // dY viewed as [B][196 pixels][64 co]: the 208-pixel box ends in zero fill rather than in the next image
+  if (make_tmap_nhwc_bf16(&tmDY, dy, 64, 196, B, 1, 64, 16 * WG_KSTEPS, 1, 128)) return 102;
+  int splits = max_ctas() / WG_GROUPS;
+  if (splits * WG_GROUPS > WG_MAX_PARTS) splits = WG_MAX_PARTS / WG_GROUPS;
+  if (splits > B) splits = B;
+  static bool configured = false;
+  if (!configured) {
+    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem::TOTAL));
+    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    configured = true;
+  }
+  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
+  DM_CUDA_OK(launch_kernel(conv2_wgrad_kernel, dim3(WG_GROUPS * splits), dim3(CV_THREADS), WgSmem::TOTAL, st, tmX, tmDY,
+                           B, splits));
+  return (int)launch_kernel(conv2_wgrad_reduce_kernel, dim3(WGR_CTAS + (bias_part ? WGR_BIAS_CTAS : 0)), dim3(WGR_THREADS),
+                            0, st, reinterpret_cast<float*>(g_w), splits, reinterpret_cast<const float*>(bias_part),
+                            n_bias, reinterpret_cast<float*>(g_bias));
 }
 
 }  // namespace dm
@@ -592,25 +626,15 @@ int dm_conv2_dgrad(const void* dy, const void* w_bf16, void* dx, int B, void* st
 // g_w ([25][32][64] fp32) must be zeroed by the caller; the gradient is added to it.  Two launches: the weight-gradient
 // kernel and the reduction of its partial sums.
 int dm_conv2_wgrad(const void* a1, const void* dy, void* g_w, int B, void* stream) {
-  using namespace dm;
-  CUtensorMap tmX, tmDY;
-  if (make_tmap_nhwc_bf16(&tmX, a1, 32, 14, 14, B, 32, 18, 18, 64)) return 101;
-  // dY viewed as [B][196 pixels][64 co]: the 208-pixel box ends in zero fill rather than in the next image
-  if (make_tmap_nhwc_bf16(&tmDY, dy, 64, 196, B, 1, 64, 16 * WG_KSTEPS, 1, 128)) return 102;
-  int splits = max_ctas() / WG_GROUPS;
-  if (splits * WG_GROUPS > WG_MAX_PARTS) splits = WG_MAX_PARTS / WG_GROUPS;
-  if (splits > B) splits = B;
-  static bool configured = false;
-  if (!configured) {
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, WgSmem::TOTAL));
-    DM_CUDA_OK(cudaFuncSetAttribute(conv2_wgrad_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
-    configured = true;
-  }
-  const cudaStream_t st = reinterpret_cast<cudaStream_t>(stream);
-  DM_CUDA_OK(launch_kernel(conv2_wgrad_kernel, dim3(WG_GROUPS * splits), dim3(CV_THREADS), WgSmem::TOTAL, st, tmX, tmDY,
-                           B, splits));
-  return (int)launch_kernel(conv2_wgrad_reduce_kernel, dim3(WGR_ITEMS / WGR_THREADS), dim3(WGR_THREADS), 0, st,
-                            reinterpret_cast<float*>(g_w), splits);
+  return dm::launch_conv2_wgrad(a1, dy, g_w, nullptr, 0, nullptr, B, stream);
+}
+
+// The same, and g_bias ([64] fp32, pre-zeroed) += the sum of the n_bias conv2 bias-gradient slots that
+// dm_fc1_dgrad_unpool_slots stored into bias_part, in slot order: what dm_fc1_dgrad_unpool adds, to the bit.
+int dm_conv2_wgrad_bias(const void* a1, const void* dy, void* g_w, const void* bias_part, int n_bias, void* g_bias, int B,
+                        void* stream) {
+  if (bias_part == nullptr || g_bias == nullptr || n_bias < 1) return -1;
+  return dm::launch_conv2_wgrad(a1, dy, g_w, bias_part, n_bias, g_bias, B, stream);
 }
 
 }  // extern "C"

@@ -44,7 +44,7 @@ struct GemmParams {
   long long split_stride;   // EPI_STORE_F32 with split-K: split z writes its partial tile at out + z*split_stride
   const float* bias;        // EPI_BIAS_RELU_BF16: per-column bias (reference K2/K3 fused into the producer)
   const uint8_t* code;      // EPI_UNPOOL2_BF16: pooling codes [M][N] (bits 0-1 argmax position, bit 2 ReLU active)
-  float* g_bias;            // EPI_UNPOOL2_BF16: conv2 bias gradient [64], the CTAs' sum is added to it (pre-zeroed)
+  float* bias_part;         // EPI_UNPOOL2_BF16: [CTAs][64] conv2 bias-gradient partials, one slot per CTA
   const float* decay_w;     // EPI_*_DECAY: fp32 weights [M][ldo]
   double* decay_part;       // EPI_*_DECAY: one W^2 partial per CTA, at blockIdx.y * gridDim.x + blockIdx.x
   float decay;              // EPI_*_DECAY: lambda
@@ -57,7 +57,7 @@ struct GemmSmem {
   static constexpr int STAGE_BYTES = A_BYTES + B_BYTES;
   static constexpr int STAGES = GEMM_STAGES;
   static constexpr int BAR_OFFSET = STAGES * STAGE_BYTES;
-  static constexpr int BPART_OFFSET = BAR_OFFSET + 128;   // EPI_UNPOOL2_BF16: [4 row quarters][64] bias partials + flag
+  static constexpr int BPART_OFFSET = BAR_OFFSET + 128;   // EPI_UNPOOL2_BF16: [4 row quarters][64] bias partials
   static constexpr int TOTAL = BAR_OFFSET + 2048 + 1024;  // barriers, bias partials + alignment slack
   // epilogue staging (reuses the ring): rows padded by 4 floats so that 32 threads reading 16 B of 32 different rows
   // hit distinct banks
@@ -65,14 +65,23 @@ struct GemmSmem {
   static_assert(GEMM_BM * ACC_LD * 4 <= BAR_OFFSET, "accumulator staging must fit in the operand ring");
 };
 
-// EPI_UNPOOL2_BF16: per-CTA conv2 bias-gradient partials, added up in CTA order by the last CTA (arrive_last_cta), so the
-// result does not depend on the order in which the CTAs finish.
+// EPI_UNPOOL2_BF16: each CTA stores its conv2 bias-gradient partials to its own slot, and a later kernel adds the slots up
+// in CTA order (add_ordered_slot_sum64), so the result does not depend on the order in which the CTAs finish, and nothing
+// waits for the sum before the data gradient is out.
 constexpr int UNPOOL_MAX_CTAS = 4096;                  // batch <= 4096 / 49 row tiles x 128 = 10 624 rows
-// One launch of this kernel in flight per device: the workspace and ticket are static (see arrive_last_cta).
+// The slots of dm_fc1_dgrad_unpool, which sums them right after the GEMM: one launch pair in flight per device.
 __device__ float g_unpool_bias_part[UNPOOL_MAX_CTAS * 64];
-__device__ unsigned int g_unpool_ticket;
 
 int fc1_dgrad_unpool_max_batch() { return UNPOOL_MAX_CTAS / (3136 / 64) * GEMM_BM; }
+
+int unpool_bias_slots(int B) { return (B + GEMM_BM - 1) / GEMM_BM * (3136 / 64); }
+
+// g_bias += the slots' sum in slot order: 16 CTAs, CTA q adds channels 4q .. 4q + 3
+__global__ void __launch_bounds__(64) unpool_bias_sum_kernel(const float* slots, int n, float* g_bias) {
+  __shared__ float4 s_buf[4 * 64];
+  pdl_wait();
+  add_ordered_slot_sum64<64>(slots, n, blockIdx.x, g_bias, s_buf);
+}
 
 template <int BN, bool A_MN, bool B_MN, int EPI>
 __global__ void __launch_bounds__(GEMM_THREADS, 1)
@@ -377,39 +386,8 @@ gemm_tc_kernel(const __grid_constant__ CUtensorMap tmA, const __grid_constant__ 
     named_bar_sync(1, GEMM_CONSUMERS);
     const int cta = blockIdx.y * gridDim.x + blockIdx.x;
     if (threadIdx.x < 64)
-      g_unpool_bias_part[cta * 64 + threadIdx.x] =
+      p.bias_part[cta * 64 + threadIdx.x] =
           s_bpart[threadIdx.x] + s_bpart[64 + threadIdx.x] + s_bpart[128 + threadIdx.x] + s_bpart[192 + threadIdx.x];
-    volatile unsigned int* s_flag = reinterpret_cast<volatile unsigned int*>(smem + S::BPART_OFFSET + 1024);
-    const int nslots = gridDim.x * gridDim.y;
-    if (arrive_last_cta(&g_unpool_ticket, nslots, 1, GEMM_CONSUMERS, s_flag)) {
-      // channel c = the CTAs' values added in CTA order (thread c < 64).  All consumer threads first copy a chunk of
-      // slots into the idle ring, 4 loads in flight each, so this tail of the launch waits for one L2 round trip per
-      // 64 slots.
-      constexpr int CHUNK = S::BAR_OFFSET / 256;     // slots of 64 floats
-      float4* s_slots = reinterpret_cast<float4*>(smem);
-      const float4* src = reinterpret_cast<const float4*>(g_unpool_bias_part);
-      float sum = 0.f;
-      for (int k0 = 0; k0 < nslots; k0 += CHUNK) {
-        const int n4 = min(CHUNK, nslots - k0) * 16;
-        for (int i0 = threadIdx.x; i0 < n4; i0 += 4 * GEMM_CONSUMERS) {
-          float4 v[4];
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (i0 + u * GEMM_CONSUMERS < n4) v[u] = __ldcg(src + (size_t)k0 * 16 + i0 + u * GEMM_CONSUMERS);
-#pragma unroll
-          for (int u = 0; u < 4; ++u)
-            if (i0 + u * GEMM_CONSUMERS < n4) s_slots[i0 + u * GEMM_CONSUMERS] = v[u];
-        }
-        named_bar_sync(1, GEMM_CONSUMERS);
-        if (threadIdx.x < 64) {
-          const float* sp = reinterpret_cast<const float*>(s_slots) + threadIdx.x;
-#pragma unroll 8
-          for (int k = 0; k < n4 / 16; ++k) sum += sp[k * 64];
-        }
-        named_bar_sync(1, GEMM_CONSUMERS);
-      }
-      if (threadIdx.x < 64) p.g_bias[threadIdx.x] += sum;
-    }
   }
   if (DECAY) {
     // the CTA's W^2 partial: a fixed butterfly per warp, then the eight warps in order
@@ -530,20 +508,38 @@ extern "C" int dm_gemm_bf16_decay(const void* A, const void* B, void* out, int M
   return launch_gemm<128, true, true, EPI_STORE_F32_DECAY>(tmA, tmB, p, 1, stream);
 }
 
-// fc1 dgrad fused with the maxpool2/ReLU2 backward and the conv2 bias gradient:
+// fc1 dgrad fused with the maxpool2/ReLU2 backward, and the conv2 bias gradient's per-CTA partials:
 //   dxfc[b, j] = sum_k dh[b, k] * W1[j, k]   (A = dh [B,512] K-major, B = W1 [3136,512] rows = j, K contiguous)
 //   dy2[b, 2ph+dy, 2pw+dx, c] = dxfc[b, (ph*7+pw)*64 + c] where code says (dy,dx) is the argmax and ReLU was active
-//   g_bias2[c] += sum of the scattered values (summed in a fixed order: bit-reproducible).          dy2: [B,14,14,64] bf16, fully written (zeros included).
-extern "C" int dm_fc1_dgrad_unpool(const void* dh, const void* w1_bf16, const void* code2, void* dy2, void* g_bias2, int B,
-                                   void* stream_) {
+//   bias_part[cta][c] = the CTA's sum of the scattered values of channel c.      dy2: [B,14,14,64] bf16, fully written (zeros included).
+// bias_part holds dm_unpool_bias_slots(B) slots of 64 floats.
+extern "C" int dm_fc1_dgrad_unpool_slots(const void* dh, const void* w1_bf16, const void* code2, void* dy2, void* bias_part,
+                                         int B, void* stream_) {
   using namespace dm;
   CUtensorMap tmA, tmB;
   int rc = make_tmap_2d_bf16(&tmA, dh, 512, (uint64_t)B, 512, 64, 128, 128);
   if (rc) return 100 + rc;
   rc = make_tmap_2d_bf16(&tmB, w1_bf16, 512, 3136, 512, 64, 64, 128);
   if (rc) return 200 + rc;
-  if (((B + GEMM_BM - 1) / GEMM_BM) * (3136 / 64) > UNPOOL_MAX_CTAS) return -6;
+  if (bias_part == nullptr) return -1;
   GemmParams p{B, 3136, 512 / GEMM_BK, 0, dy2, 0, nullptr, reinterpret_cast<const uint8_t*>(code2),
-               reinterpret_cast<float*>(g_bias2)};
+               reinterpret_cast<float*>(bias_part)};
   return launch_gemm<64, false, false, EPI_UNPOOL2_BF16>(tmA, tmB, p, 1, reinterpret_cast<cudaStream_t>(stream_));
+}
+
+extern "C" int dm_unpool_bias_slots(int B) { return dm::unpool_bias_slots(B); }
+
+// The same, with g_bias2[c] += the slots' sum in CTA order (pre-zeroed; bit-reproducible): the GEMM into a static
+// workspace, then unpool_bias_sum.  Returns -6 without launching for a batch above the workspace's 10 624 rows.
+extern "C" int dm_fc1_dgrad_unpool(const void* dh, const void* w1_bf16, const void* code2, void* dy2, void* g_bias2, int B,
+                                   void* stream_) {
+  using namespace dm;
+  const int n = unpool_bias_slots(B);
+  if (n > UNPOOL_MAX_CTAS) return -6;
+  float* slots = nullptr;
+  DM_CUDA_OK(cudaGetSymbolAddress(reinterpret_cast<void**>(&slots), g_unpool_bias_part));
+  const int rc = dm_fc1_dgrad_unpool_slots(dh, w1_bf16, code2, dy2, slots, B, stream_);
+  if (rc) return rc;
+  return (int)launch_kernel(unpool_bias_sum_kernel, dim3(16), dim3(64), 0, reinterpret_cast<cudaStream_t>(stream_),
+                            static_cast<const float*>(slots), n, reinterpret_cast<float*>(g_bias2));
 }

@@ -39,6 +39,7 @@ struct Fc2Args {
   float* h_out;              // [B,512] out: post ReLU/dropout activations (fc2_wgrad operand)  (train)
   float* dl_out;             // [B,12]  out: d loss / d logits, columns 10-11 zero              (train)
   float* loss_acc;           // [2]: sum of per-row loss / B, number of correct / B  (pre-zeroed)
+  float2* row_terms;         // [B] per-row (loss, hit) terms; null: g_f2_row_terms, added up by the launch's last CTA
   float* logits_out;         // optional [B,10]
   int B;
   int train;
@@ -48,14 +49,46 @@ struct Fc2Args {
   float inv_batch;           // 1 / (rows that make up the mean)
 };
 
-// Per-row (loss, hit) terms, added up in row order by the last CTA (arrive_last_cta): the reported loss and accuracy do
-// not depend on the order in which the rows' CTAs finish.
+// Per-row (loss, hit) terms, added up in row order by fc2_loss_sum: the reported loss and accuracy do not depend on the
+// order in which the rows' CTAs finish.  dm_fc2_fwd_bwd stores them into a static workspace and its last CTA
+// (arrive_last_cta) adds them; dm_fc2_fwd_bwd_rows stores them into the caller's buffer and exits, and
+// dm_fc2_loss_sum adds them later, where nothing on the training step's data-gradient chain waits for the sum.
 constexpr int F2_MAX_ROWS = 1 << 16;                      // batch limit of dm_fc2_fwd_bwd
-// One launch of this kernel in flight per device: the workspace and ticket are static (see arrive_last_cta).
-__device__ __align__(8) float g_f2_row_terms[F2_MAX_ROWS * 2];
+// One launch of dm_fc2_fwd_bwd in flight per device: the workspace and ticket are static (see arrive_last_cta).
+__device__ float2 g_f2_row_terms[F2_MAX_ROWS];
 __device__ unsigned int g_f2_ticket;
 
 int fc2_fwd_bwd_max_batch() { return F2_MAX_ROWS; }
+
+// One warp: lane l adds rows l, l + 32, ... in row order (16 rows' loads in flight per round: one L2 round trip at
+// B <= 512), then a fixed butterfly; lane 0 adds the two sums onto the pre-zeroed loss words.
+DMNIST_DEVICE void fc2_loss_sum(const float2* terms, int rows, float* loss_acc) {
+  const int lane = threadIdx.x & 31;
+  float l = 0.f, h = 0.f;
+  for (int r0 = lane; r0 < rows; r0 += 32 * 16) {
+    float2 v[16];
+#pragma unroll
+    for (int u = 0; u < 16; ++u) v[u] = r0 + 32 * u < rows ? __ldcg(terms + r0 + 32 * u) : make_float2(0.f, 0.f);
+#pragma unroll
+    for (int u = 0; u < 16; ++u)
+      if (r0 + 32 * u < rows) { l += v[u].x; h += v[u].y; }
+  }
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) {
+    l += __shfl_xor_sync(0xffffffffu, l, o);
+    h += __shfl_xor_sync(0xffffffffu, h, o);
+  }
+  if (lane == 0) {
+    // fire-and-forget: the warp does not wait for a load of the words (same rounding as +=)
+    atomicAdd(loss_acc, l);
+    atomicAdd(loss_acc + 1, h);
+  }
+}
+
+__global__ void __launch_bounds__(32) fc2_loss_sum_kernel(const float2* terms, int rows, float* loss_acc) {
+  pdl_wait();
+  fc2_loss_sum(terms, rows, loss_acc);
+}
 
 __global__ void __launch_bounds__(F2_THREADS) fc2_fwd_bwd_kernel(Fc2Args a) {
   __shared__ float s_part[F2_THREADS / 32][DL_LD];
@@ -128,39 +161,16 @@ __global__ void __launch_bounds__(F2_THREADS) fc2_fwd_bwd_kernel(Fc2Args a) {
     // first index attaining the maximum (ties: lowest class, like the reference's in_top_k / argmax)
     const unsigned hit = __ballot_sync(0xffffffffu, lane < NCLS && logit == m);
     const float l_label = __shfl_sync(0xffffffffu, logit, label);
-    if (lane == 0) {
-      g_f2_row_terms[2 * row] = (__logf(ssum) - (l_label - m)) * a.inv_batch;
-      g_f2_row_terms[2 * row + 1] = ((__ffs(hit) - 1) == label ? 1.f : 0.f) * a.inv_batch;
-    }
+    if (lane == 0)
+      (a.row_terms ? a.row_terms : g_f2_row_terms)[row] =
+          make_float2((__logf(ssum) - (l_label - m)) * a.inv_batch, ((__ffs(hit) - 1) == label ? 1.f : 0.f) * a.inv_batch);
     if (a.logits_out && lane < NCLS) a.logits_out[(size_t)row * NCLS + lane] = logit;
     if (a.train && lane < DL_LD) a.dl_out[(size_t)row * DL_LD + lane] = dl_mine;
   }
-  {
+  if (!a.row_terms) {
     __shared__ unsigned int s_last;
-    if (arrive_last_cta(&g_f2_ticket, gridDim.x, 1, F2_THREADS, &s_last) && warp == 0) {
-      // lane l adds rows l, l + 32, ... in row order; 16 rows' loads in flight per round (one L2 round trip at B <= 512)
-      const float2* terms = reinterpret_cast<const float2*>(g_f2_row_terms);
-      const int rows = (int)gridDim.x;
-      float l = 0.f, h = 0.f;
-      for (int r0 = lane; r0 < rows; r0 += 32 * 16) {
-        float2 v[16];
-#pragma unroll
-        for (int u = 0; u < 16; ++u) v[u] = r0 + 32 * u < rows ? __ldcg(terms + r0 + 32 * u) : make_float2(0.f, 0.f);
-#pragma unroll
-        for (int u = 0; u < 16; ++u)
-          if (r0 + 32 * u < rows) { l += v[u].x; h += v[u].y; }
-      }
-#pragma unroll
-      for (int o = 16; o > 0; o >>= 1) {
-        l += __shfl_xor_sync(0xffffffffu, l, o);
-        h += __shfl_xor_sync(0xffffffffu, h, o);
-      }
-      if (lane == 0) {
-        // fire-and-forget: the launch's last CTA does not wait for a load of the words (same rounding as +=)
-        atomicAdd(a.loss_acc, l);
-        atomicAdd(a.loss_acc + 1, h);
-      }
-    }
+    if (arrive_last_cta(&g_f2_ticket, gridDim.x, 1, F2_THREADS, &s_last) && warp == 0)
+      fc2_loss_sum(g_f2_row_terms, (int)gridDim.x, a.loss_acc);
   }
   if (!a.train) return;
   float d[4] = {0.f, 0.f, 0.f, 0.f};
@@ -292,17 +302,13 @@ int launch_fc2_wgrad(const void* scratch_h, const void* scratch_dl, const void* 
                                 reinterpret_cast<float*>(g_b1), B, dk);
 }
 
-}  // namespace dm
-
-extern "C" {
-
-// Critical-path half: logits / loss / accuracy and (train) dh, h_out, dl_out.  scratch_h [B,512] fp32 and
-// scratch_dl [B,12] fp32 are only touched when train != 0.
-int dm_fc2_fwd_bwd(const void* h_part, long long part_stride, int splits, const void* b1, const void* w2, const void* b2,
-                   const void* labels, void* dh, void* scratch_h, void* scratch_dl, void* loss_acc, void* logits_out,
-                   int B, int train, unsigned int seed_mix, const void* step_ptr, float keep_prob, void* stream) {
-  if (splits < 1 || splits > dm::F2_MAX_SPLITS || B < 1 || B > dm::F2_MAX_ROWS) return -1;
-  dm::Fc2Args a;
+// row_terms == nullptr: the per-row terms go to g_f2_row_terms and the launch's last CTA adds them onto loss_acc
+int launch_fc2_fwd_bwd(const void* h_part, long long part_stride, int splits, const void* b1, const void* w2,
+                       const void* b2, const void* labels, void* dh, void* scratch_h, void* scratch_dl, void* loss_acc,
+                       void* row_terms, void* logits_out, int B, int train, unsigned int seed_mix, const void* step_ptr,
+                       float keep_prob, void* stream) {
+  if (splits < 1 || splits > F2_MAX_SPLITS || B < 1 || B > F2_MAX_ROWS) return -1;
+  Fc2Args a;
   a.h_part = reinterpret_cast<const float*>(h_part);
   a.part_stride = part_stride;
   a.splits = splits;
@@ -314,6 +320,7 @@ int dm_fc2_fwd_bwd(const void* h_part, long long part_stride, int splits, const 
   a.h_out = reinterpret_cast<float*>(scratch_h);
   a.dl_out = reinterpret_cast<float*>(scratch_dl);
   a.loss_acc = reinterpret_cast<float*>(loss_acc);
+  a.row_terms = reinterpret_cast<float2*>(row_terms);
   a.logits_out = reinterpret_cast<float*>(logits_out);
   a.B = B; a.train = train; a.seed_mix = seed_mix;
   a.step_ptr = reinterpret_cast<const uint32_t*>(step_ptr);
@@ -321,11 +328,42 @@ int dm_fc2_fwd_bwd(const void* h_part, long long part_stride, int splits, const 
   a.inv_batch = 1.f / (float)B;
   static bool configured = false;
   if (!configured) {
-    DM_CUDA_OK(cudaFuncSetAttribute(dm::fc2_fwd_bwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
+    DM_CUDA_OK(cudaFuncSetAttribute(fc2_fwd_bwd_kernel, cudaFuncAttributePreferredSharedMemoryCarveout, cudaSharedmemCarveoutMaxShared));
     configured = true;
   }
-  return (int)dm::launch_kernel(dm::fc2_fwd_bwd_kernel, dim3(B), dim3(dm::F2_THREADS), 0,
-                                reinterpret_cast<cudaStream_t>(stream), a);
+  return (int)launch_kernel(fc2_fwd_bwd_kernel, dim3(B), dim3(F2_THREADS), 0, reinterpret_cast<cudaStream_t>(stream), a);
+}
+
+}  // namespace dm
+
+extern "C" {
+
+// Critical-path half: logits / loss / accuracy and (train) dh, h_out, dl_out.  scratch_h [B,512] fp32 and
+// scratch_dl [B,12] fp32 are only touched when train != 0.
+int dm_fc2_fwd_bwd(const void* h_part, long long part_stride, int splits, const void* b1, const void* w2, const void* b2,
+                   const void* labels, void* dh, void* scratch_h, void* scratch_dl, void* loss_acc, void* logits_out,
+                   int B, int train, unsigned int seed_mix, const void* step_ptr, float keep_prob, void* stream) {
+  return dm::launch_fc2_fwd_bwd(h_part, part_stride, splits, b1, w2, b2, labels, dh, scratch_h, scratch_dl, loss_acc,
+                                nullptr, logits_out, B, train, seed_mix, step_ptr, keep_prob, stream);
+}
+
+// The same, except that the per-row (loss, hit) terms go to row_terms ([B] float pairs) and loss_acc is not touched:
+// dm_fc2_loss_sum(row_terms, B, loss_acc) then adds them as dm_fc2_fwd_bwd would have, to the bit.  The training step
+// runs the sum on a side branch, so nothing on its data-gradient chain waits for it.
+int dm_fc2_fwd_bwd_rows(const void* h_part, long long part_stride, int splits, const void* b1, const void* w2,
+                        const void* b2, const void* labels, void* dh, void* scratch_h, void* scratch_dl, void* row_terms,
+                        void* logits_out, int B, int train, unsigned int seed_mix, const void* step_ptr, float keep_prob,
+                        void* stream) {
+  if (row_terms == nullptr) return -1;
+  return dm::launch_fc2_fwd_bwd(h_part, part_stride, splits, b1, w2, b2, labels, dh, scratch_h, scratch_dl, nullptr,
+                                row_terms, logits_out, B, train, seed_mix, step_ptr, keep_prob, stream);
+}
+
+// loss_acc[0] += the rows' loss terms, loss_acc[1] += their hit terms, each in row order (one warp).
+int dm_fc2_loss_sum(const void* row_terms, int B, void* loss_acc, void* stream) {
+  if (row_terms == nullptr || loss_acc == nullptr || B < 1) return -1;
+  return (int)dm::launch_kernel(dm::fc2_loss_sum_kernel, dim3(1), dim3(32), 0, reinterpret_cast<cudaStream_t>(stream),
+                                reinterpret_cast<const float2*>(row_terms), B, reinterpret_cast<float*>(loss_acc));
 }
 
 // Side-branch half: g_w2 [512][10], g_b2 [10], g_b1 [512] (plain stores).

@@ -8,12 +8,13 @@ Step = (reference src/distributed_train.py:332 ``sess.run(apply_gradients_op)``)
     conv2_fwd        wgmma implicit GEMM + bias/ReLU/pool csrc/conv2_tc.cu
     fc1_fwd          wgmma GEMM, split-K into fp32        csrc/gemm_tc.cu
     fc2_fwd_bwd      bias+ReLU+dropout, fc2, softmax-CE,
-                     accuracy, dlogits, d(fc1)              csrc/lenet_simt.cu
+                     accuracy, dlogits, d(fc1), per-row loss terms   csrc/lenet_simt.cu
+    fc2_loss_sum     the row terms summed in fixed order -> loss words   (loss read-back branch)
     fc2_wgrad        fc2 weight/bias + fc1 bias gradients   (side branch)
     fc1_wgrad        wgmma GEMM (MN-major x MN-major) -> gradient arena
-    fc1_dgrad        wgmma GEMM, maxpool2/ReLU2 backward + conv2 bias grad in the epilogue
+    fc1_dgrad        wgmma GEMM, maxpool2/ReLU2 backward + per-CTA conv2 bias-gradient slots in the epilogue
     conv2_wgrad      wgmma, K = whole images, per-CTA partials -> workspace
-    conv2_wgrad_reduce  the partials summed in fixed order -> gradient arena
+    conv2_wgrad_reduce  the partials and the conv2 bias slots summed in fixed order -> gradient arena
     conv2_dgrad      wgmma
     conv1_wgrad      wgmma, maxpool1/ReLU1 backward fused into the operand build
     fused_sync_sgd   arrival -> mask -> NVLink reduce -> 1/count -> SGD -> push -> bf16 shadow
@@ -897,6 +898,13 @@ class CudaLeNetEngine(_CudaEngine):
         self.dlogits = torch.zeros(B, 12, dtype=f32, device=dev)     # d loss / d logits, 48-byte rows
         self.dy2 = torch.zeros(B, 14, 14, 64, dtype=bf, device=dev)
         self.dx1 = torch.zeros(B, 14, 14, 32, dtype=bf, device=dev)
+        # Workspaces of the step's two reproducible sums that run off the data-gradient chain: fc2_fwd_bwd's per-row
+        # (loss, hit) terms, added by fc2_loss_sum on the loss read-back branch, and fc1_dgrad's per-CTA conv2
+        # bias-gradient slots, added by conv2_wgrad's reduction.  They belong to the engine, so no other launch of those
+        # kernels (an evaluation pass, another engine in the process) can write them between the store and the sum.
+        self._row_terms = torch.zeros(B, 2, dtype=f32, device=dev)
+        self._bias2_slots = int(self.lib.dm_unpool_bias_slots(B))
+        self._bias2_part = torch.zeros(self._bias2_slots, 64, dtype=f32, device=dev)
         # the data-gradient chain is the critical path: it is captured on a high-priority stream (_main_priority), the
         # weight-gradient side branches on low-priority ones, so the block scheduler serves the chain first whenever both
         # have CTAs pending
@@ -925,11 +933,18 @@ class CudaLeNetEngine(_CudaEngine):
         G.gemm_bf16_raw(self.a2, self.pb["fc1_weights"], self.h_part, B, 512, 3136, 3136, 512, 512, False, True,
                         G.EPI_STORE_F32, splits=self.fc1_splits, bn=64, split_stride=self.h_part.stride(0))
 
-    def _fc2_fwd_bwd(self, labels: torch.Tensor, B: int, train: bool, sp, logits_out: Optional[torch.Tensor] = None) -> None:
+    def _fc2_fwd_bwd(self, labels: torch.Tensor, B: int, train: bool, sp, logits_out: Optional[torch.Tensor] = None,
+                     rows: bool = False) -> None:
+        """``rows``: the training step's form -- the per-row loss terms go to ``_row_terms`` and :meth:`_fc2_loss_sum`
+        adds them into the loss words; otherwise the kernel's last CTA adds them."""
         p = self.p
-        self.lib.dm_fc2_fwd_bwd(self.h_part, self.h_part.stride(0), self.fc1_splits, p["fc1_biases"], p["fc2_weights"],
-                                p["fc2_biases"], labels, self.dh, self.h_act, self.dlogits, self.d_loss_acc, logits_out, B,
-                                int(train), self._seed_mix0, self._epoch_ptr if train else None, self.keep_prob, sp)
+        fn, acc = (self.lib.dm_fc2_fwd_bwd_rows, self._row_terms) if rows else (self.lib.dm_fc2_fwd_bwd, self.d_loss_acc)
+        fn(self.h_part, self.h_part.stride(0), self.fc1_splits, p["fc1_biases"], p["fc2_weights"], p["fc2_biases"], labels,
+           self.dh, self.h_act, self.dlogits, acc, logits_out, B, int(train), self._seed_mix0,
+           self._epoch_ptr if train else None, self.keep_prob, sp)
+
+    def _fc2_loss_sum(self, B: int, sp) -> None:
+        self.lib.dm_fc2_loss_sum(self._row_terms, B, self.d_loss_acc, sp)
 
     def _fc1_wgrad(self, dst: torch.Tensor, B: int) -> None:
         # dW1[3136,512] = a2^T (A MN-major) * dh (B MN-major), K = batch: fp32 into the gradient arena, or bf16 (half the
@@ -984,11 +999,13 @@ class CudaLeNetEngine(_CudaEngine):
 
     def _fc1_dgrad(self, B: int, sp) -> None:
         # d(pool2 out)[B,3136] = dh[B,512] (K-major) * W1[3136,512] (rows = in, K = out contiguous), with maxpool2/ReLU2
-        # backward and the conv2 bias gradient in the GEMM epilogue (no [B,3136] intermediate)
-        self.lib.dm_fc1_dgrad_unpool(self.dh, self.pb["fc1_weights"], self.code2, self.dy2, self.g["conv2_biases"], B, sp)
+        # backward and the conv2 bias gradient's per-CTA slots in the GEMM epilogue (no [B,3136] intermediate)
+        self.lib.dm_fc1_dgrad_unpool_slots(self.dh, self.pb["fc1_weights"], self.code2, self.dy2, self._bias2_part, B, sp)
 
     def _conv2_wgrad(self, B: int, sp) -> None:
-        self.lib.dm_conv2_wgrad(self.a1, self.dy2, self.g["conv2_weights"], B, sp)
+        # conv2 weight gradient, and the conv2 bias gradient: fc1_dgrad's slots added in slot order by the reduction
+        self.lib.dm_conv2_wgrad_bias(self.a1, self.dy2, self.g["conv2_weights"], self._bias2_part, self._bias2_slots,
+                                     self.g["conv2_biases"], B, sp)
 
     def _conv2_dgrad(self, B: int, sp) -> None:
         self.lib.dm_conv2_dgrad(self.dy2, self.pb["conv2_weights"], self.dx1, B, sp)
@@ -999,12 +1016,13 @@ class CudaLeNetEngine(_CudaEngine):
 
     # ---- kernel sequence ------------------------------------------------------------------------------
     def _launch_forward(self, images: torch.Tensor, labels: torch.Tensor, B: int, train: bool,
-                        logits_out: Optional[torch.Tensor] = None) -> int:
+                        logits_out: Optional[torch.Tensor] = None, step: bool = False) -> int:
+        """``step``: the training step's forward, whose loss words the backward's read-back branch adds up."""
         sp = stream_ptr()
         self._conv1_fwd(images, B, train, sp)
         self._conv2_fwd(B, sp)
         self._fc1_fwd(B)
-        self._fc2_fwd_bwd(labels, B, train, sp, logits_out)
+        self._fc2_fwd_bwd(labels, B, train, sp, logits_out, rows=step)
         return 4
 
     def _launch_backward(self, images: torch.Tensor, B: int, early_sync: bool = False) -> int:
@@ -1016,17 +1034,19 @@ class CudaLeNetEngine(_CudaEngine):
         fork1 = torch.cuda.Event()
         fork1.record(main)
         self._side[0].wait_event(fork1)
-        # (loss, accuracy) are final after fc2_fwd_bwd: their copy into the slot's page-locked host buffer is a branch of
-        # the step (a memcpy node of the graph) that runs under the backward pass -- reading the result costs the host
-        # no extra call, only a wait on the step's completion event
-        # (its own branch, joined only at the very end of the step: a memcpy node in front of the aggregation kernel
-        # would cost that kernel its programmatic launch edge)
-        if not self._decay:
-            self._launch_loss_readback(fork1)
         sp = stream_ptr()
         self._fc1_dgrad(B, sp)
-        # (the side branch is issued AFTER the chain's kernel: both become ready together and the first one dispatched takes
-        #  the SMs -- the data-gradient GEMM must be that one)
+        # (the side branches are issued AFTER the chain's kernel: they become ready together and the first one dispatched
+        #  takes the SMs -- the data-gradient GEMM must be that one)
+        if early_sync:
+            # the small fc gradients (fc2 weights/biases, fc1 biases) belong to the late bucket: their own branch.  Issued
+            # before fc1_wgrad: its small CTAs then run beside fc1_dgrad's instead of queueing behind fc1_wgrad's and
+            # running beside conv2_dgrad, which they slowed down (BASELINE.md, "Loss and conv2 bias sums off the chain")
+            self._side[2].wait_event(fork1)
+            with torch.cuda.stream(self._side[2]):
+                self._fc2_wgrad(B, stream_ptr())
+                join3 = torch.cuda.Event()
+                join3.record(self._side[2])
         with torch.cuda.stream(self._side[0]):
             self._fc1_wgrad(self._g16_view if early_sync and self._bucket_v2 else self.g["fc1_weights"], B)
             ev_w1 = torch.cuda.Event()
@@ -1056,15 +1076,15 @@ class CudaLeNetEngine(_CudaEngine):
                                                 oa["decay_steps"], ctas=self._early_ctas, stream=self._side[0])
                 join1 = torch.cuda.Event()
                 join1.record(self._side[0])
-            # the small fc gradients (fc2 weights/biases, fc1 biases) belong to the late bucket: their own branch
-            self._side[2].wait_event(fork1)
-            with torch.cuda.stream(self._side[2]):
-                self._fc2_wgrad(B, stream_ptr())
-                join3 = torch.cuda.Event()
-                join3.record(self._side[2])
-        if self._decay:
-            # the decay's loss term needs both weight-gradient kernels' partials (not the early bucket's exchange)
-            self._launch_loss_readback(fork1, ev_w1, join3 if early_sync else join1)
+        # (loss, accuracy) are added up from fc2_fwd_bwd's row terms and copied into the slot's page-locked host buffer on
+        # a branch of the step (a kernel and a memcpy node of the graph) that runs under the backward pass -- nothing on
+        # the data-gradient chain waits for the sum, and reading the result costs the host no extra call, only a wait on
+        # the step's completion event.  Its own branch, joined only at the very end of the step: a memcpy node in front of
+        # the aggregation kernel would cost that kernel its programmatic launch edge.  It is captured after fc1_dgrad:
+        # captured before it, the sum kernel took the forward's stream in the replayed graph, the data-gradient chain
+        # moved to another one, and the step was about 1 us slower (BASELINE.md, "Loss and conv2 bias sums off the chain").
+        # With decay, the loss term needs both weight-gradient kernels' partials (not the early bucket's exchange).
+        self._launch_loss_readback(fork1, *((ev_w1, join3 if early_sync else join1) if self._decay else ()))
         # conv2 dgrad and wgrad each fill the machine (1 CTA/SM, ~200 KB smem): side by side they only slow the chain
         # down.  wgrad is forked AFTER dgrad instead and shares the SMs with conv1_wgrad.
         self._conv2_dgrad(B, sp)
@@ -1085,14 +1105,16 @@ class CudaLeNetEngine(_CudaEngine):
         main.wait_event(join1)
         if early_sync:
             main.wait_event(join3)
-        return 8 if self._decay else 7     # (conv2_wgrad is two launches: the kernel and its reduction)
+        # (conv2_wgrad is two launches: the kernel and its reduction; the read-back branch's loss sum is one more)
+        return 9 if self._decay else 8
 
     def _launch_loss_readback(self, *after: torch.cuda.Event) -> None:
-        """The branch that copies (loss, accuracy) into the slot's page-locked host buffer, after the events ``after``;
-        with weight decay it first adds the loss term."""
+        """The branch that adds up the loss words and copies (loss, accuracy) into the slot's page-locked host buffer,
+        after the events ``after``; with weight decay it then adds the decay's loss term."""
         for ev in after:
             self._side[3].wait_event(ev)
         with torch.cuda.stream(self._side[3]):
+            self._fc2_loss_sum(self.batch_size, stream_ptr())
             if self._decay:
                 self.lib.dm_weight_decay_loss(self._decay_ws, self._decay_parts, self._decay, self.d_loss_acc, stream_ptr())
             self.h_loss_bufs[self._slot].copy_(self.d_loss_acc, non_blocking=True)
@@ -1114,8 +1136,8 @@ class CudaLeNetEngine(_CudaEngine):
         """Average device time of every kernel of the step, measured in place with CUDA events between
         eager launches (caches warm, as in the replayed graph; includes the launch gap).  ``unpool2`` is part of
         fc1_dgrad's epilogue and stays at 0."""
-        names = ["memsets", "conv1_fwd", "conv2_fwd", "fc1_fwd", "fc2_fwd_bwd", "fc1_wgrad", "fc2_wgrad", "fc1_dgrad", "unpool2",
-                 "conv2_wgrad", "conv2_dgrad", "conv1_wgrad"]
+        names = ["memsets", "conv1_fwd", "conv2_fwd", "fc1_fwd", "fc2_fwd_bwd", "fc2_loss_sum", "fc1_wgrad", "fc2_wgrad",
+                 "fc1_dgrad", "unpool2", "conv2_wgrad", "conv2_dgrad", "conv1_wgrad"]
         # K > N: adopt + shadow refresh, and gate + accumulate + close + apply, in place of the fused sync kernel
         names = (["kgtn_begin"] + names + ["kgtn_end"]) if self._kgtn_k else \
             (["async_begin"] + names + ["async_end"]) if self._async else \
@@ -1135,7 +1157,8 @@ class CudaLeNetEngine(_CudaEngine):
             yield "conv1_fwd", lambda: self._conv1_fwd(img, B, True, sp)
             yield "conv2_fwd", lambda: self._conv2_fwd(B, sp)
             yield "fc1_fwd", lambda: self._fc1_fwd(B)
-            yield "fc2_fwd_bwd", lambda: self._fc2_fwd_bwd(lbl, B, True, sp)
+            yield "fc2_fwd_bwd", lambda: self._fc2_fwd_bwd(lbl, B, True, sp, rows=True)
+            yield "fc2_loss_sum", lambda: self._fc2_loss_sum(B, sp)
             yield "fc1_wgrad", lambda: self._fc1_wgrad(self.g["fc1_weights"], B)
             yield "fc2_wgrad", lambda: self._fc2_wgrad(B, sp)
             yield "fc1_dgrad", lambda: self._fc1_dgrad(B, sp)
@@ -1195,7 +1218,7 @@ class CudaLeNetEngine(_CudaEngine):
             self._enqueue_iteration_begin()
             n += 3 if self._ssp >= 0 else 2       # the staleness bound's wait before the pull
         n += self._launch_zero()
-        n += self._launch_forward(images, self.labels[slot], self.batch_size, True)
+        n += self._launch_forward(images, self.labels[slot], self.batch_size, True, step=True)
         n += self._launch_backward(images, self.batch_size, early_sync=bucketed)
         if bucketed:
             oa = self._opt_args

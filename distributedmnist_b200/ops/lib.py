@@ -62,6 +62,7 @@ def _signatures() -> dict:
         "dm_conv2_fwd": (S, i, [P, P, P, P, P, i, P]),
         "dm_conv2_dgrad": (S, i, [P, P, P, i, P]),
         "dm_conv2_wgrad": (S, i, [P, P, P, i, P]),
+        "dm_conv2_wgrad_bias": (S, i, [P, P, P, P, i, P, i, P]),
         # eval_best.cu
         "dm_best_state_bytes": (V, i, []),
         "dm_eval_best_decide": (S, i, [P, P, P, u, P, P, P]),
@@ -131,6 +132,8 @@ def _signatures() -> dict:
         "dm_gemm_bf16": (S, i, [P, P, P, i, i, i, i, i, i, i, i, i, i, i, ll, P, P]),
         "dm_gemm_decay_ctas": (V, i, [i, i]),
         "dm_gemm_bf16_decay": (S, i, [P, P, P, i, i, i, i, i, i, i, P, f, P, P]),
+        "dm_fc1_dgrad_unpool_slots": (S, i, [P, P, P, P, P, i, P]),
+        "dm_unpool_bias_slots": (V, i, [i]),
         "dm_fc1_dgrad_unpool": (S, i, [P, P, P, P, P, i, P]),
         # host_utils.cu
         "dm_version": (V, i, []),
@@ -142,6 +145,8 @@ def _signatures() -> dict:
         "dm_device_cc": (V, i, [i]),
         # lenet_simt.cu, mlp_simt.cu, moving_average.cu
         "dm_fc2_fwd_bwd": (S, i, [P, ll, i, P, P, P, P, P, P, P, P, P, i, i, u, P, f, P]),
+        "dm_fc2_fwd_bwd_rows": (S, i, [P, ll, i, P, P, P, P, P, P, P, P, P, i, i, u, P, f, P]),
+        "dm_fc2_loss_sum": (S, i, [P, i, P, P]),
         "dm_fc2_wgrad": (S, i, [P, P, P, P, P, P, i, P]),
         "dm_fc2_wgrad_decay_ctas": (V, i, []),
         "dm_fc2_wgrad_decay": (S, i, [P, P, P, P, P, P, i, P, P, P, f, P, P]),
