@@ -18,28 +18,14 @@ accepted, the other three exit at once).
     python tools/ckpt_overhead.py [--steps 2000] [--rounds 3] [--batch 256] [--out results/ckpt_overhead.json]
 """
 import argparse
-import json
-import os
-import subprocess
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-from distributedmnist_b200.data import make_synthetic_mnist  # noqa: E402
-from distributedmnist_b200.engine_cuda import CudaLeNetEngine  # noqa: E402
-from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer  # noqa: E402
-from distributedmnist_b200.parallel.context import ReplicaContext  # noqa: E402
-from distributedmnist_b200.parallel.fused import FusedBackend  # noqa: E402
-from distributedmnist_b200.schedule import LearningRateSchedule  # noqa: E402
-
-
-def gpu_info():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                       capture_output=True, text=True)
-    name, power, clock = [v.strip() for v in r.stdout.strip().split(",")] if r.returncode == 0 else ("?", "?", "?")
-    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
+import gpu_timing
+import numpy as np
+import torch
+from distributedmnist_b200.data import make_synthetic_mnist
+from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
+from distributedmnist_b200.schedule import LearningRateSchedule
 
 
 class _Capture:
@@ -120,11 +106,9 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("ckpt_overhead.py measures on a GPU; none found")
-    torch.cuda.set_device(0)
     B = a.batch
-    be = FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
-    eng = CudaLeNetEngine(B, be, use_graph=True)
-    eng.attach_optimizer(SyncReplicasOptimizer(be, LearningRateSchedule(0.05, 10 ** 6, 1.0), 1, 1))
+    eng = gpu_timing.one_replica_engine(
+        "lenet", B, 0, lambda be: SyncReplicasOptimizer(be, LearningRateSchedule(0.05, 10 ** 6, 1.0), 1, 1))
     eng.arm_checkpoint(snapshot=False)
     trx, try_, _tex, _tey = make_synthetic_mnist(B * 16, 16, seed=5)
     bufs = [eng.pack_batch(trx[i * B:(i + 1) * B], try_[i * B:(i + 1) * B]) for i in range(16)]
@@ -146,23 +130,18 @@ def main():
     snap, done = capture_alone(eng, bufs, done, snapshot=True)
     snap["stats"] = eng.checkpoint_stats()
     eng._leave_native_runner()
-    be.check_error()
+    eng.backend.check_error()
     base = float(np.mean(t_step[(0, "capture")]))
 
     def name(c):
         return "off" if c[0] == 0 else "E=%d_%s" % c
-    res = dict(gpu_info(), batch=B, steps_per_window=a.steps, rounds=a.rounds, arena_bytes=4 * eng.spec.arena_numel,
+    res = dict(gpu_timing.card(), batch=B, steps_per_window=a.steps, rounds=a.rounds, arena_bytes=4 * eng.spec.arena_numel,
                captures_landed=landed,
                step_us={name(c): {"mean": float(np.mean(v)) * 1e6, "min": float(np.min(v)) * 1e6,
                                   "max": float(np.max(v)) * 1e6} for c, v in t_step.items()},
                overhead={name(c): float(np.mean(v)) / base - 1.0 for c, v in t_step.items() if c[0]},
                capture_live=live, capture_snapshot=snap)
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+    gpu_timing.emit(res, a.out)
 
 
 if __name__ == "__main__":

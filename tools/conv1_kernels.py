@@ -8,23 +8,13 @@ SM clock are read in the same call and printed with the numbers.  Prints one JSO
 """
 import argparse
 import json
-import os
-import subprocess
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import torch  # noqa: E402
-
-from distributedmnist_b200.ops.lib import load, stream_ptr  # noqa: E402
+import gpu_timing
+import torch
+from distributedmnist_b200.ops.lib import load, stream_ptr
 
 BF = torch.bfloat16
-
-
-def gpu_info() -> dict:
-    q = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"],
-                       capture_output=True, text=True).stdout.strip().splitlines()
-    name, power, clock = [f.strip() for f in q[0].split(",")] if q else ("?", "?", "?")
-    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
 
 
 def inputs(B: int, seed: int):
@@ -39,19 +29,6 @@ def inputs(B: int, seed: int):
     return [t.cuda() for t in (x, w, b, dpool, code, a1, dy)]
 
 
-def per_launch_us(fn, n: int, warmup: int) -> float:
-    for _ in range(warmup):
-        fn()
-    torch.cuda.synchronize()
-    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    e0.record()
-    for _ in range(n):
-        fn()
-    e1.record()
-    torch.cuda.synchronize()
-    return e0.elapsed_time(e1) * 1e3 / n
-
-
 def main() -> None:
     ap = argparse.ArgumentParser(description=__doc__, formatter_class=argparse.RawDescriptionHelpFormatter)
     ap.add_argument("--launches", type=int, default=2000)
@@ -62,8 +39,7 @@ def main() -> None:
     if not torch.cuda.is_available():
         sys.exit("conv1_kernels.py needs a CUDA device")
     lib = load()
-    info = gpu_info()
-    res = dict(info)
+    res = gpu_timing.card()
     n, wu = args.launches, args.warmup
 
     def fwd(B):
@@ -72,8 +48,8 @@ def main() -> None:
         code = torch.empty(B, 14, 14, 32, dtype=torch.uint8, device="cuda")
         return lambda: lib.dm_conv1_fwd_tc(x, w, b, out, code, B, None, 0, None, 0, None, 0, stream_ptr())
 
-    res["conv1_fwd_us_B%d" % args.batch] = per_launch_us(fwd(args.batch), n, wu)
-    res["conv1_fwd_us_B%d" % args.eval_batch] = per_launch_us(fwd(args.eval_batch), n, wu)
+    res["conv1_fwd_us_B%d" % args.batch] = gpu_timing.timed_launches(fwd(args.batch), n, wu)
+    res["conv1_fwd_us_B%d" % args.eval_batch] = gpu_timing.timed_launches(fwd(args.eval_batch), n, wu)
 
     B = args.batch
     x, _, _, dpool, code, a1, dy = inputs(B, 2)
@@ -98,9 +74,9 @@ def main() -> None:
         join.record(side)
         main_s.wait_event(join)
 
-    res["conv1_wgrad_us_B%d" % B] = per_launch_us(c1, n, wu)
-    res["conv2_wgrad_reduce_us_B%d" % B] = per_launch_us(c2, n, wu)
-    res["conv2_wgrad_reduce_plus_conv1_wgrad_beside_us_B%d" % B] = per_launch_us(both, n, wu)
+    res["conv1_wgrad_us_B%d" % B] = gpu_timing.timed_launches(c1, n, wu)
+    res["conv2_wgrad_reduce_us_B%d" % B] = gpu_timing.timed_launches(c2, n, wu)
+    res["conv2_wgrad_reduce_plus_conv1_wgrad_beside_us_B%d" % B] = gpu_timing.timed_launches(both, n, wu)
     res["launches"] = n
     print(json.dumps({k: (round(v, 2) if isinstance(v, float) else v) for k, v in res.items()}), flush=True)
 

@@ -7,14 +7,11 @@ SM clock are read in the same call and printed with the numbers.  Prints one JSO
 """
 import argparse
 import json
-import os
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import torch  # noqa: E402
-
-from distributedmnist_b200.ops.lib import load, stream_ptr  # noqa: E402
-from tools.conv1_kernels import gpu_info, per_launch_us  # noqa: E402
+import gpu_timing
+import torch
+from distributedmnist_b200.ops.lib import load, stream_ptr
 
 BF = torch.bfloat16
 
@@ -28,7 +25,7 @@ def main() -> None:
     if not torch.cuda.is_available():
         sys.exit("conv2_kernels.py needs a CUDA device")
     lib = load()
-    res = dict(gpu_info())
+    res = gpu_timing.card()
     for B in [int(b) for b in args.batches.split(",")]:
         g = torch.Generator(device="cpu").manual_seed(B)
         a1 = torch.rand(B, 14, 14, 32, generator=g).to(BF).cuda()
@@ -38,9 +35,9 @@ def main() -> None:
         out = torch.empty(B, 7, 7, 64, dtype=BF, device="cuda")
         code = torch.empty(B, 7, 7, 64, dtype=torch.uint8, device="cuda")
         dx = torch.empty(B, 14, 14, 32, dtype=BF, device="cuda")
-        res["conv2_fwd_us_B%d" % B] = per_launch_us(
+        res["conv2_fwd_us_B%d" % B] = gpu_timing.timed_launches(
             lambda: lib.dm_conv2_fwd(a1, w, b, out, code, B, stream_ptr()), args.launches, args.warmup)
-        res["conv2_dgrad_us_B%d" % B] = per_launch_us(
+        res["conv2_dgrad_us_B%d" % B] = gpu_timing.timed_launches(
             lambda: lib.dm_conv2_dgrad(dy, w, dx, B, stream_ptr()), args.launches, args.warmup)
     res["launches"] = args.launches
     print(json.dumps({k: (round(v, 2) if isinstance(v, float) else v) for k, v in res.items()}), flush=True)

@@ -14,55 +14,26 @@ Prints one JSON line.
 """
 import argparse
 import ctypes
-import json
 import os
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import gpu_timing
+import torch
+from distributedmnist_b200 import augment
+from distributedmnist_b200.ops.lib import load, stream_ptr
+from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
+from distributedmnist_b200.schedule import LearningRateSchedule
 
 RANGES = (2.0, 15.0, 0.1)                  # shift px, rotation degrees, zoom
 ALPHA, SIGMA = 34.0, 4.0
 CONFIGS = ("off", "affine", "elastic")
 
 
-def gpu_info():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                       capture_output=True, text=True)
-    name, power, clock = [v.strip() for v in r.stdout.strip().split(",")] if r.returncode == 0 else ("?", "?", "?")
-    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
-
-
 def _engine(model, B, hidden, config):
-    import torch
-    from distributedmnist_b200 import augment
-    from distributedmnist_b200.engine_cuda import CudaLeNetEngine, CudaMlpEngine
-    from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
-    from distributedmnist_b200.parallel.context import ReplicaContext
-    from distributedmnist_b200.parallel.fused import FusedBackend
-    from distributedmnist_b200.schedule import LearningRateSchedule
-    be = FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
-    eng = CudaLeNetEngine(B, be, use_graph=True) if model == "lenet" else \
-        CudaMlpEngine(model, B, be, hidden=hidden, use_graph=True)
-    eng.attach_optimizer(SyncReplicasOptimizer(be, LearningRateSchedule(0.01, 10 ** 6, 1.0), 1, 1))
+    eng = gpu_timing.one_replica_engine(
+        model, B, hidden, lambda be: SyncReplicasOptimizer(be, LearningRateSchedule(0.01, 10 ** 6, 1.0), 1, 1))
     if config != "off":
         eng.arm_augment(*RANGES, elastic=augment.Elastic(ALPHA, SIGMA) if config == "elastic" else None)
-    g = torch.Generator().manual_seed(1)
-    packed = [eng.pack_batch(torch.rand(B, 784, generator=g) - 0.5, torch.randint(0, 10, (B,), generator=g),
-                             pin=False).cuda() for _ in range(2)]
-    return eng, packed
-
-
-def _window(eng, packed, steps):
-    import torch
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0.record()
-    for i in range(steps):
-        eng.step_packed(packed[i & 1])
-    t1.record()
-    torch.cuda.synchronize()
-    return t0.elapsed_time(t1) * 1e3 / steps
+    return eng, gpu_timing.packed_batches(eng, 2, 1, on_device=True)
 
 
 def _median(v):
@@ -71,12 +42,7 @@ def _median(v):
 
 def step_times(model, B, hidden, rounds, steps, warmup):
     engines = {k: _engine(model, B, hidden, k) for k in CONFIGS}
-    for eng, packed in engines.values():
-        _window(eng, packed, warmup)
-    us = {k: [] for k in CONFIGS}
-    for _ in range(rounds):
-        for k, (eng, packed) in engines.items():
-            us[k].append(_window(eng, packed, steps))
+    us = gpu_timing.alternate(engines, steps, warmup, rounds)
     out = dict(model=model, batch=B, hidden=hidden if model != "lenet" else None)
     for k, (eng, _p) in engines.items():
         eng.backend.check_error()
@@ -90,9 +56,6 @@ def step_times(model, B, hidden, rounds, steps, warmup):
 
 
 def kernel_time(B, iters):
-    import torch
-    from distributedmnist_b200 import augment
-    from distributedmnist_b200.ops.lib import load, stream_ptr
     lib = load()
     src = torch.rand(B, 784, device="cuda") - 0.5
     dst = torch.empty_like(src)
@@ -110,16 +73,7 @@ def kernel_time(B, iters):
 
     out = dict(batch=B)
     for name, launch in (("elastic", elastic), ("affine", affine)):
-        for _ in range(50):
-            launch()
-        torch.cuda.synchronize()
-        t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-        t0.record()
-        for _ in range(iters):
-            launch()
-        t1.record()
-        torch.cuda.synchronize()
-        out[name + "_us"] = t0.elapsed_time(t1) * 1e3 / iters
+        out[name + "_us"] = gpu_timing.timed_launches(launch, iters, 50)
     # taps inside the image per output, summed over the 28 positions of a line: both passes, both components
     taps_per_line = sum(min(R, 27 - p) + min(R, p) + 1 for p in range(28))
     out["dfma_per_launch"] = B * 2 * 2 * 28 * taps_per_line
@@ -138,19 +92,13 @@ def main():
     args = ap.parse_args()
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         os.environ.pop(k, None)
-    import torch
     torch.cuda.set_device(0)
     out = dict(tool="elastic", ranges=dict(zip(("max_shift", "max_rotation", "max_scale"), RANGES)),
-               elastic=dict(alpha=ALPHA, sigma=SIGMA), **gpu_info())
+               elastic=dict(alpha=ALPHA, sigma=SIGMA), **gpu_timing.card())
     out["kernel"] = [kernel_time(B, args.iters) for B in (256, 8192)]
     out["step_time"] = [step_times("lenet", 256, 0, args.rounds, args.steps, args.warmup),
                         step_times("mlp3", 8192, 4096, args.rounds, args.mlp_steps, args.warmup // 10)]
-    line = json.dumps(out)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
-    print(line)
+    gpu_timing.emit(out, args.out)
 
 
 if __name__ == "__main__":

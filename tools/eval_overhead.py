@@ -16,28 +16,14 @@ with and without it, and the snapshot attempts alone (one accepted attempt and t
 between steps, quiescent weights.
 """
 import argparse
-import json
-import os
-import subprocess
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-from distributedmnist_b200.data import make_synthetic_mnist  # noqa: E402
-from distributedmnist_b200.engine_cuda import CudaLeNetEngine  # noqa: E402
-from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer  # noqa: E402
-from distributedmnist_b200.parallel.context import ReplicaContext  # noqa: E402
-from distributedmnist_b200.parallel.fused import FusedBackend  # noqa: E402
-from distributedmnist_b200.schedule import LearningRateSchedule  # noqa: E402
-
-
-def gpu_info():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                       capture_output=True, text=True)
-    name, power, clock = [v.strip() for v in r.stdout.strip().split(",")] if r.returncode == 0 else ("?", "?", "?")
-    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
+import gpu_timing
+import numpy as np
+import torch
+from distributedmnist_b200.data import make_synthetic_mnist
+from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
+from distributedmnist_b200.schedule import LearningRateSchedule
 
 
 def window(eng, bufs, steps, every, first):
@@ -100,11 +86,9 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("eval_overhead.py measures on a GPU; none found")
-    torch.cuda.set_device(0)
     B = a.batch
-    be = FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
-    eng = CudaLeNetEngine(B, be, use_graph=True)
-    eng.attach_optimizer(SyncReplicasOptimizer(be, LearningRateSchedule(0.05, 10 ** 6, 1.0), 1, 1))
+    eng = gpu_timing.one_replica_engine(
+        "lenet", B, 0, lambda be: SyncReplicasOptimizer(be, LearningRateSchedule(0.05, 10 ** 6, 1.0), 1, 1))
     trx, try_, tex, tey = make_synthetic_mnist(B * 16, 10000, seed=5)
     eng.arm_eval(tex, tey)
     bufs = [eng.pack_batch(trx[i * B:(i + 1) * B], try_[i * B:(i + 1) * B]) for i in range(16)]
@@ -136,10 +120,10 @@ def main():
         torch.cuda.synchronize()
         ev_times.append(e0.elapsed_time(e1) * 1e-3)
     eng._leave_native_runner()
-    be.check_error()
+    eng.backend.check_error()
     base = float(np.mean(t_step[0]))
     t_eval = float(np.median(stamps)) if stamps else float("nan")
-    res = dict(gpu_info(), batch=B, steps_per_window=a.steps, rounds=a.rounds, eval_examples=10000,
+    res = dict(gpu_timing.card(), batch=B, steps_per_window=a.steps, rounds=a.rounds, eval_examples=10000,
                step_us={("off" if e == 0 else "E=%d" % e): {"mean": float(np.mean(v)) * 1e6, "min": float(np.min(v)) * 1e6,
                                                           "max": float(np.max(v)) * 1e6} for e, v in t_step.items()},
                eval_pass_us={"globaltimer_median": t_eval * 1e6, "globaltimer_min": float(np.min(stamps)) * 1e6,
@@ -152,13 +136,8 @@ def main():
                                        "measured_max": float(np.max(t_step[e])) / float(np.min(t_step[0])) - 1.0}
     if a.snapshot:
         res["snapshot"] = snapshot_cost(eng, tex, tey, bufs, done)
-        be.check_error()
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+        eng.backend.check_error()
+    gpu_timing.emit(res, a.out)
 
 
 if __name__ == "__main__":

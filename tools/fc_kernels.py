@@ -10,13 +10,10 @@ with the numbers.  Prints one JSON line.
 """
 import argparse
 import json
-import os
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import torch  # noqa: E402
-
-from tools.conv1_kernels import gpu_info  # noqa: E402
+import gpu_timing
+import torch
 
 
 def graph_us(fn, iters: int, reps: int = 5) -> float:
@@ -71,7 +68,7 @@ def main() -> None:
         sys.exit("fc_kernels.py needs a CUDA device")
     from distributedmnist_b200.ops.lib import stream_ptr
     torch.cuda.set_device(0)
-    res = dict(gpu_info())
+    res = gpu_timing.card()
     for B in [int(b) for b in args.batches.split(",")]:
         eng, be = engine(B)
         lbl = eng.labels[eng._slot]

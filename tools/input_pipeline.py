@@ -29,25 +29,16 @@ import sys
 import tempfile
 import time
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
+import gpu_timing
+import numpy as np
+import torch
+from distributedmnist_b200.data import DataSet, make_synthetic_mnist
+from distributedmnist_b200.flags import FLAGS
+from distributedmnist_b200.parallel.context import init_context
+from distributedmnist_b200.train import train
 
-from distributedmnist_b200.data import DataSet, make_synthetic_mnist  # noqa: E402
-from distributedmnist_b200.flags import FLAGS  # noqa: E402
-from distributedmnist_b200.parallel.context import init_context  # noqa: E402
-from distributedmnist_b200.train import train  # noqa: E402
-
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 B = 256
 _STEP_LINE = re.compile(r"Worker 0: .*: step ([0-9]+), loss = ")
-
-
-def gpu_info():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                       capture_output=True, text=True)
-    name, power, clock = [v.strip() for v in r.stdout.strip().split(",")] if r.returncode == 0 else ("?", "?", "?")
-    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
 
 
 class _Stamps(logging.Handler):
@@ -87,8 +78,8 @@ def run(ctx, table, device_data: bool, steps: int, window_from: int):
 
 
 def bench_rate(steps: int):
-    r = subprocess.run([sys.executable, os.path.join(ROOT, "bench.py"), "--gpus", "1", "--steps", str(steps), "--warmup", "200"],
-                       capture_output=True, text=True, cwd=tempfile.gettempdir())
+    r = subprocess.run([sys.executable, os.path.join(gpu_timing.ROOT, "bench.py"), "--gpus", "1", "--steps", str(steps),
+                        "--warmup", "200"], capture_output=True, text=True, cwd=tempfile.gettempdir())
     line = [ln for ln in r.stdout.splitlines() if ln.startswith("{")]
     if r.returncode != 0 or not line:
         raise RuntimeError("bench.py failed:\n" + (r.stdout + r.stderr)[-3000:])
@@ -148,7 +139,7 @@ def main():
         sys.exit(1)
     for k in ("RANK", "WORLD_SIZE", "LOCAL_RANK"):
         os.environ.pop(k, None)
-    info = gpu_info()
+    info = gpu_timing.card()
     ctx = init_context(FLAGS)
     tr_x, tr_y, _, _ = make_synthetic_mnist(60000, 10, seed=1234)
     table = (tr_x, tr_y)
@@ -168,10 +159,7 @@ def main():
         os.makedirs(args.trace, exist_ok=True)
         out["trace"] = {name: trace(ctx, table, name == "device_data", os.path.join(args.trace, "trace_%s.json" % name))
                         for name in ("host", "device_data")}
-    os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-    with open(args.out, "w") as f:
-        json.dump(out, f, indent=1)
-    print(json.dumps(out))
+    gpu_timing.emit(out, args.out)
 
 
 if __name__ == "__main__":

@@ -12,24 +12,15 @@ pass in turn so that the three share the same conditions:
     python tools/keep_best.py [--passes 60] [--batch 256] [--out results/keep_best.json]
 """
 import argparse
-import json
-import os
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-from distributedmnist_b200.best import BEST_CORRECT_WORD, BEST_VALID_WORD  # noqa: E402
-from distributedmnist_b200.data import make_synthetic_mnist  # noqa: E402
-from distributedmnist_b200.engine_cuda import CudaLeNetEngine  # noqa: E402
-from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer  # noqa: E402
-from distributedmnist_b200.parallel.context import ReplicaContext  # noqa: E402
-from distributedmnist_b200.parallel.fused import FusedBackend  # noqa: E402
-from distributedmnist_b200.schedule import LearningRateSchedule  # noqa: E402
-
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from eval_overhead import gpu_info  # noqa: E402
+import gpu_timing
+import numpy as np
+import torch
+from distributedmnist_b200.best import BEST_CORRECT_WORD, BEST_VALID_WORD
+from distributedmnist_b200.data import make_synthetic_mnist
+from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
+from distributedmnist_b200.schedule import LearningRateSchedule
 
 
 def main():
@@ -40,11 +31,9 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("keep_best.py measures on a GPU; none found")
-    torch.cuda.set_device(0)
     B = a.batch
-    be = FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
-    eng = CudaLeNetEngine(B, be, use_graph=True)
-    eng.attach_optimizer(SyncReplicasOptimizer(be, LearningRateSchedule(0.05, 10 ** 6, 1.0), 1, 1))
+    eng = gpu_timing.one_replica_engine(
+        "lenet", B, 0, lambda be: SyncReplicasOptimizer(be, LearningRateSchedule(0.05, 10 ** 6, 1.0), 1, 1))
     n = 10000
     trx, try_, tex, tey = make_synthetic_mnist(B * 16, n, seed=5)
     bufs = [eng.pack_batch(trx[i * B:(i + 1) * B], try_[i * B:(i + 1) * B]) for i in range(16)]
@@ -77,20 +66,15 @@ def main():
                 copies[name] += int(state[BEST_VALID_WORD].item())
         eng.eval_records()
     eng._leave_native_runner()
-    be.check_error()
+    eng.backend.check_error()
     assert copies["improve"] == a.passes and copies["no_improve"] == 0, copies
     med = {k: float(np.median(v)) for k, v in times.items()}
-    res = dict(gpu_info(), batch=B, eval_examples=n, passes_per_config=a.passes, arena_bytes=4 * eng.spec.arena_numel,
+    res = dict(gpu_timing.card(), batch=B, eval_examples=n, passes_per_config=a.passes, arena_bytes=4 * eng.spec.arena_numel,
                pass_us={k: {"median": med[k] * 1e6, "min": float(np.min(v)) * 1e6, "max": float(np.max(v)) * 1e6}
                         for k, v in times.items()},
                added_us={k: (med[k] - med["off"]) * 1e6 for k in ("no_improve", "improve")},
                added_share={k: med[k] / med["off"] - 1.0 for k in ("no_improve", "improve")})
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+    gpu_timing.emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -13,24 +13,15 @@ conditions:
     python tools/lr_plateau.py [--passes 200] [--blocks 40] [--block-steps 50] [--batch 256] [--out results/lr_plateau.json]
 """
 import argparse
-import json
-import os
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-from distributedmnist_b200.data import make_synthetic_mnist  # noqa: E402
-from distributedmnist_b200.engine_cuda import CudaLeNetEngine  # noqa: E402
-from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer  # noqa: E402
-from distributedmnist_b200.parallel.context import ReplicaContext  # noqa: E402
-from distributedmnist_b200.parallel.fused import FusedBackend  # noqa: E402
-from distributedmnist_b200.schedule import LearningRateSchedule  # noqa: E402
-from distributedmnist_b200.train import STOP_MARGIN  # noqa: E402
-
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from eval_overhead import gpu_info  # noqa: E402
+import gpu_timing
+import numpy as np
+import torch
+from distributedmnist_b200.data import make_synthetic_mnist
+from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
+from distributedmnist_b200.schedule import LearningRateSchedule
+from distributedmnist_b200.train import STOP_MARGIN
 
 
 def _stats(v):
@@ -47,11 +38,10 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("lr_plateau.py measures on a GPU; none found")
-    torch.cuda.set_device(0)
     B = a.batch
-    be = FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
-    eng = CudaLeNetEngine(B, be, use_graph=True)
-    eng.attach_optimizer(SyncReplicasOptimizer(be, LearningRateSchedule(0.05, 10 ** 6, 1.0), 1, 1))
+    eng = gpu_timing.one_replica_engine(
+        "lenet", B, 0, lambda be: SyncReplicasOptimizer(be, LearningRateSchedule(0.05, 10 ** 6, 1.0), 1, 1))
+    be = eng.backend
     n = 10000
     trx, try_, tex, tey = make_synthetic_mnist(B * 16, n, seed=5)
     bufs = [eng.pack_batch(trx[i * B:(i + 1) * B], try_[i * B:(i + 1) * B]) for i in range(16)]
@@ -106,18 +96,13 @@ def main():
 
     mp = {k: float(np.median(v)) for k, v in pass_s.items()}
     ms = {k: float(np.median(v)) for k, v in step_s.items()}
-    res = dict(gpu_info(), batch=B, eval_examples=n, passes_per_config=a.passes, step_blocks_per_config=a.blocks,
+    res = dict(gpu_timing.card(), batch=B, eval_examples=n, passes_per_config=a.passes, step_blocks_per_config=a.blocks,
                steps_per_block=a.block_steps,
                pass_us={k: _stats(v) for k, v in pass_s.items()},
                pass_added_us=(mp["armed"] - mp["off"]) * 1e6,
                step_us={k: _stats(v) for k, v in step_s.items()},
                step_added_us=(ms["armed"] - ms["off"]) * 1e6, step_added_share=ms["armed"] / ms["off"] - 1.0)
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+    gpu_timing.emit(res, a.out)
 
 
 if __name__ == "__main__":

@@ -14,23 +14,14 @@ The step graph is the same in all three; only the control block's schedule words
     python tools/lr_schedule.py [--blocks 40] [--block-steps 50] [--batch 256] [--out results/lr_schedule.json]
 """
 import argparse
-import json
-import os
 import sys
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-import numpy as np  # noqa: E402
-import torch  # noqa: E402
-
-from distributedmnist_b200.data import make_synthetic_mnist  # noqa: E402
-from distributedmnist_b200.engine_cuda import CudaLeNetEngine  # noqa: E402
-from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer  # noqa: E402
-from distributedmnist_b200.parallel.context import ReplicaContext  # noqa: E402
-from distributedmnist_b200.parallel.fused import FusedBackend  # noqa: E402
-from distributedmnist_b200.schedule import LearningRateSchedule  # noqa: E402
-
-sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
-from eval_overhead import gpu_info  # noqa: E402
+import gpu_timing
+import numpy as np
+import torch
+from distributedmnist_b200.data import make_synthetic_mnist
+from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
+from distributedmnist_b200.schedule import LearningRateSchedule
 
 LONG = 2 ** 31                     # steps: longer than any run of this tool
 CONFIGS = {"off": (0, 1.0 / 3, 0, 0.0), "warmup": (LONG, 0.1, 0, 0.0), "cosine": (LONG, 0.1, LONG, 0.01)}
@@ -49,11 +40,10 @@ def main():
     a = ap.parse_args()
     if not torch.cuda.is_available():
         sys.exit("lr_schedule.py measures on a GPU; none found")
-    torch.cuda.set_device(0)
     B = a.batch
-    be = FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
-    eng = CudaLeNetEngine(B, be, use_graph=True)
-    eng.attach_optimizer(SyncReplicasOptimizer(be, LearningRateSchedule(0.01, 10 ** 6, 1.0), 1, 1))
+    eng = gpu_timing.one_replica_engine(
+        "lenet", B, 0, lambda be: SyncReplicasOptimizer(be, LearningRateSchedule(0.01, 10 ** 6, 1.0), 1, 1))
+    be = eng.backend
     trx, try_, _tex, _tey = make_synthetic_mnist(B * 16, 100, seed=5)
     bufs = [eng.pack_batch(trx[i * B:(i + 1) * B], try_[i * B:(i + 1) * B]) for i in range(16)]
     names = list(CONFIGS)
@@ -78,17 +68,12 @@ def main():
     be.set_lr_schedule(*CONFIGS["off"])
 
     ms = {k: float(np.median(v)) for k, v in step_s.items()}
-    res = dict(gpu_info(), batch=B, step_blocks_per_config=a.blocks, steps_per_block=a.block_steps,
+    res = dict(gpu_timing.card(), batch=B, step_blocks_per_config=a.blocks, steps_per_block=a.block_steps,
                step_us={k: _stats(v) for k, v in step_s.items()},
                images_per_s={k: B / v for k, v in ms.items()},
                step_added_us={k: (ms[k] - ms["off"]) * 1e6 for k in names if k != "off"},
                step_added_share={k: ms[k] / ms["off"] - 1.0 for k in names if k != "off"})
-    line = json.dumps(res)
-    print(line)
-    if a.out:
-        os.makedirs(os.path.dirname(os.path.abspath(a.out)), exist_ok=True)
-        with open(a.out, "w") as f:
-            f.write(line + "\n")
+    gpu_timing.emit(res, a.out)
 
 
 if __name__ == "__main__":

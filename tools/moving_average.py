@@ -15,64 +15,31 @@
 import argparse
 import json
 import os
-import subprocess
-import sys
 import tempfile
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import gpu_timing
+import torch
+from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
+from distributedmnist_b200.schedule import LearningRateSchedule
 
 STEP_CONFIGS = [("lenet", 256, 1024), ("mlp3", 8192, 4096)]
 
 
-def gpu_info():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                       capture_output=True, text=True)
-    name, power, clock = [v.strip() for v in r.stdout.strip().split(",")] if r.returncode == 0 else ("?", "?", "?")
-    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
-
-
-def _engine(model, batch, hidden, decay):
-    import torch
-    from distributedmnist_b200.engine_cuda import CudaLeNetEngine, CudaMlpEngine
-    from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
-    from distributedmnist_b200.parallel.context import ReplicaContext
-    from distributedmnist_b200.parallel.fused import FusedBackend
-    from distributedmnist_b200.schedule import LearningRateSchedule
-    torch.cuda.set_device(0)
-    be = FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
-    eng = CudaLeNetEngine(batch, be, use_graph=True) if model == "lenet" else \
-        CudaMlpEngine(model, batch, be, hidden=hidden, use_graph=True)
-    eng.attach_optimizer(SyncReplicasOptimizer(be, LearningRateSchedule(0.01, 10 ** 6, 1.0), 1, 1))
+def child_step_time(model, batch, hidden, decay, steps, warmup):
+    eng = gpu_timing.one_replica_engine(
+        model, batch, hidden, lambda be: SyncReplicasOptimizer(be, LearningRateSchedule(0.01, 10 ** 6, 1.0), 1, 1))
     if decay:
         eng.arm_moving_average(decay)
-    return eng, be
-
-
-def child_step_time(model, batch, hidden, decay, steps, warmup):
-    import torch
-    eng, be = _engine(model, batch, hidden, decay)
-    g = torch.Generator().manual_seed(1)
-    packed = [eng.pack_batch(torch.rand(batch, 784, generator=g) - 0.5, torch.randint(0, 10, (batch,), generator=g),
-                             pin=False).cuda() for _ in range(2)]
-    for i in range(warmup):
-        eng.step_packed(packed[i & 1])
-    torch.cuda.synchronize()
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0.record()
-    for i in range(steps):
-        eng.step_packed(packed[i & 1])
-    t1.record()
-    torch.cuda.synchronize()
-    be.check_error()
-    us = t0.elapsed_time(t1) * 1e3 / steps
+    packed = gpu_timing.packed_batches(eng, 2, 1, on_device=True)
+    gpu_timing.timed_steps(eng, packed, warmup)
+    us = gpu_timing.timed_steps(eng, packed, steps)
+    eng.backend.check_error()
     eng._leave_native_runner()
     return dict(model=model, batch=batch, hidden=hidden if model != "lenet" else None, average=bool(decay),
                 arena_floats=eng.spec.arena_numel, launches_per_step=eng.launches_per_step, us_per_step=us)
 
 
 def kernel_times(iters=200):
-    import torch
     from distributedmnist_b200.models import get_model
     from distributedmnist_b200.ops.lib import load, stream_ptr
     lib = load()
@@ -151,16 +118,9 @@ def main():
         model, batch, hidden, decay = args.child.split(":")
         print(json.dumps(child_step_time(model, int(batch), int(hidden), float(decay), args.steps, args.warmup)))
         return
-    steps = []
-    for _ in range(args.rounds):
-        for model, batch, hidden in STEP_CONFIGS:
-            for decay in (0.0, args.decay):
-                r = subprocess.run([sys.executable, os.path.abspath(__file__), "--steps=%d" % args.steps,
-                                    "--warmup=%d" % args.warmup, "--child=%s:%d:%d:%r" % (model, batch, hidden, decay)],
-                                   capture_output=True, text=True)
-                if r.returncode != 0:
-                    raise RuntimeError(r.stdout[-2000:] + r.stderr[-4000:])
-                steps.append(json.loads(r.stdout.strip().splitlines()[-1]))
+    steps = [gpu_timing.child_json([__file__, "--steps=%d" % args.steps, "--warmup=%d" % args.warmup,
+                                    "--child=%s:%d:%d:%r" % (model, batch, hidden, decay)])
+             for _ in range(args.rounds) for model, batch, hidden in STEP_CONFIGS for decay in (0.0, args.decay)]
     from distributedmnist_b200 import data as mnist_data
     from distributedmnist_b200.flags import FLAGS
     kern = kernel_times()
@@ -172,13 +132,8 @@ def main():
             tta.append(tta_run(ds, args, average))
     out = dict(tool="moving_average", decay=args.decay, step_time=steps, kernel=kern,
                time_to_accuracy=dict(data="synthetic MNIST-shaped (not MNIST)", target=args.target, batch_size=128,
-                                     eval_every_steps=args.eval_every, runs=tta), **gpu_info())
-    line = json.dumps(out)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
-    print(line)
+                                     eval_every_steps=args.eval_every, runs=tta), **gpu_timing.card())
+    gpu_timing.emit(out, args.out)
 
 
 if __name__ == "__main__":

@@ -11,25 +11,14 @@ prototypes, shifted, scaled and noised), so the numbers are not MNIST numbers.
                                      [--out results/time_to_accuracy.json]
 """
 import argparse
-import json
 import os
-import subprocess
-import sys
 import tempfile
 
-sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-
-from distributedmnist_b200 import data as mnist_data  # noqa: E402
-from distributedmnist_b200.flags import FLAGS  # noqa: E402
-from distributedmnist_b200.parallel.context import init_context  # noqa: E402
-from distributedmnist_b200.train import train  # noqa: E402
-
-
-def gpu_info():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                       capture_output=True, text=True)
-    name, power, clock = [v.strip() for v in r.stdout.strip().split(",")] if r.returncode == 0 else ("?", "?", "?")
-    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
+import gpu_timing
+from distributedmnist_b200 import data as mnist_data
+from distributedmnist_b200.flags import FLAGS
+from distributedmnist_b200.parallel.context import init_context
+from distributedmnist_b200.train import train
 
 
 def run(ds, args, k: int) -> dict:
@@ -69,13 +58,8 @@ def main():
             runs.append(run(ds, args, k))
     out = dict(tool="time_to_accuracy", data="synthetic MNIST-shaped (not MNIST)", target=args.target,
                batch_size=args.batch_size, eval_every_steps=args.eval_every, max_steps=args.max_steps,
-               validation_examples=ds.validation.num_examples, runs=runs, **gpu_info())
-    line = json.dumps(out)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
-    print(line)
+               validation_examples=ds.validation.num_examples, runs=runs, **gpu_timing.card())
+    gpu_timing.emit(out, args.out)
 
 
 if __name__ == "__main__":

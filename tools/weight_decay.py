@@ -14,57 +14,31 @@
 import argparse
 import json
 import os
-import subprocess
-import sys
 
-ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
-sys.path.insert(0, ROOT)
+import gpu_timing
+import torch
+from distributedmnist_b200.ops import gemm as G
+from distributedmnist_b200.ops.lib import load, stream_ptr
+from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
+from distributedmnist_b200.schedule import LearningRateSchedule
 
 B = 256
 
 
-def gpu_info():
-    r = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader", "-i", "0"],
-                       capture_output=True, text=True)
-    name, power, clock = [v.strip() for v in r.stdout.strip().split(",")] if r.returncode == 0 else ("?", "?", "?")
-    return {"gpu": name, "power_limit": power, "max_sm_clock": clock}
-
-
 def child_step_time(lam, steps, warmup):
-    import torch
-    from distributedmnist_b200.engine_cuda import CudaLeNetEngine
-    from distributedmnist_b200.parallel.aggregators import SyncReplicasOptimizer
-    from distributedmnist_b200.parallel.context import ReplicaContext
-    from distributedmnist_b200.parallel.fused import FusedBackend
-    from distributedmnist_b200.schedule import LearningRateSchedule
-    torch.cuda.set_device(0)
-    be = FusedBackend(ReplicaContext(0, 1, 0, torch.device("cuda", 0), "none"))
-    eng = CudaLeNetEngine(B, be, use_graph=True)
-    eng.attach_optimizer(SyncReplicasOptimizer(be, LearningRateSchedule(0.01, 10 ** 6, 1.0), 1, 1))
+    eng = gpu_timing.one_replica_engine(
+        "lenet", B, 0, lambda be: SyncReplicasOptimizer(be, LearningRateSchedule(0.01, 10 ** 6, 1.0), 1, 1))
     if lam:
         eng.arm_weight_decay(lam)
-    g = torch.Generator().manual_seed(1)
-    packed = [eng.pack_batch(torch.rand(B, 784, generator=g) - 0.5, torch.randint(0, 10, (B,), generator=g),
-                             pin=False).cuda() for _ in range(2)]
-    for i in range(warmup):
-        eng.step_packed(packed[i & 1])
-    torch.cuda.synchronize()
-    t0, t1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
-    t0.record()
-    for i in range(steps):
-        eng.step_packed(packed[i & 1])
-    t1.record()
-    torch.cuda.synchronize()
-    be.check_error()
-    us = t0.elapsed_time(t1) * 1e3 / steps
+    packed = gpu_timing.packed_batches(eng, 2, 1, on_device=True)
+    gpu_timing.timed_steps(eng, packed, warmup)
+    us = gpu_timing.timed_steps(eng, packed, steps)
+    eng.backend.check_error()
     eng._leave_native_runner()
     return dict(lam=lam, launches_per_step=eng.launches_per_step, us_per_step=us)
 
 
 def kernel_times(lam, iters, blocks=5):
-    import torch
-    from distributedmnist_b200.ops import gemm as G
-    from distributedmnist_b200.ops.lib import load, stream_ptr
     lib = load()
     g = torch.Generator().manual_seed(2)
     a2 = torch.rand(B, 3136, generator=g).to(torch.bfloat16).cuda()
@@ -118,22 +92,11 @@ def main():
     if args.child is not None:
         print(json.dumps(child_step_time(float(args.child), args.steps, args.warmup)))
         return
-    steps = []
-    for _ in range(args.rounds):
-        for lam in (0.0, args.lam):
-            r = subprocess.run([sys.executable, os.path.abspath(__file__), "--steps=%d" % args.steps,
-                                "--warmup=%d" % args.warmup, "--child=%r" % lam], capture_output=True, text=True)
-            if r.returncode != 0:
-                raise RuntimeError(r.stdout[-2000:] + r.stderr[-4000:])
-            steps.append(json.loads(r.stdout.strip().splitlines()[-1]))
+    steps = [gpu_timing.child_json([__file__, "--steps=%d" % args.steps, "--warmup=%d" % args.warmup, "--child=%r" % lam])
+             for _ in range(args.rounds) for lam in (0.0, args.lam)]
     out = dict(tool="weight_decay", model="lenet", batch=B, lam=args.lam, step_time=steps,
-               kernel=kernel_times(args.lam, args.iters), **gpu_info())
-    line = json.dumps(out)
-    if args.out:
-        os.makedirs(os.path.dirname(os.path.abspath(args.out)), exist_ok=True)
-        with open(args.out, "w") as f:
-            f.write(line + "\n")
-    print(line)
+               kernel=kernel_times(args.lam, args.iters), **gpu_timing.card())
+    gpu_timing.emit(out, args.out)
 
 
 if __name__ == "__main__":
